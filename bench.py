@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- env transitions/sec of the B200-native SlateRecEnv hot path (BASELINE.json metric).
+"""bench.py -- env transitions/sec of the H100-native SlateRecEnv hot path (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            # our arm (torchrun for N > 1)
     python bench.py --impl reference --steps K --warmup W    # the reference's CPU path (oracle port)
@@ -24,14 +24,21 @@ JSON keys beyond the base contract:
   env_only  the same rollout without the learner pass.
   e2e       the reference-facing call with HOST buffers: README.md:14-21 loop, numpy actions in,
             numpy obs/mask/reward out, every copy inside the timed region.
-  roofline  the dominant kernel: the tcgen05 AUGRU recurrence (k_augru_pair2 / k_augru_pp, one profile slot), timed
-            live with CUDA events on the launching stream during the `value` loop; FLOPs = rows x 2 seq x 64 steps x
-            2*(256*512 + 256*256) (DESIGN.md section 4) against the measured sustained bf16 GEMM peak.
+  roofline  the dominant kernel: the wgmma AUGRU recurrence (k_augru_tc, one profile slot), timed live with CUDA
+            events on the launching stream during the `value` loop; FLOPs = rows x 2 seq x 64 steps x
+            2*(256*512 + 256*256) (DESIGN.md section 4) against the bf16 peak (MEASURED_PEAKS.json, else the H100 SXM
+            data sheet's dense 989 TFLOP/s).
   hbm_8d    SURVEY.md section 8(d)'s own HBM figure: transitions/s x algorithmic bytes per transition
             (176 768 B Slate-9, 170 565 B Seq-27) / (N x measured HBM peak), for `value` and `env_only`.
   cpu_baseline  the oracle port (oracle/env_np.py + dien_np.py, run by oracle/cpu_arm.py) on ALL host threads of this box:
             one single-threaded worker process per host thread, the batch's rows spread over them (<= 128 each),
             episodes started together; the same arm is `--impl reference`.
+
+--dump-outputs DIR writes what the timed `value` path computed in its last step, as DIR/<name>.npy (float32 / float64):
+on a fixed, seeded sample of at most 512 env rows, the rollout buffers of that iteration (reward, value, logp, action,
+obs, logits, action mask [T, rows, ...]), what the episode's last env.step returned (final obs, mask, done) and the
+policy parameters after its learner pass; with --conti the last env step's reward, done, obs and mask.  At most 64 MB.  The inputs are seeded, so two builds run with the
+same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -75,11 +82,12 @@ def load_peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d.get("hbm_gbs"), "bf16_tflops": d.get("bf16_tflops"),
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained"), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 -- not reached, an upper bound
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "data-sheet"}
 
 
 class ClockSampler(object):
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -219,7 +227,7 @@ def workload_config(args, seq):
                                 ":117-131 at j = 8), so %d simulator row-forwards per env row and episode instead of %d "
                                 "(R4_NO_PAY_OBS_REUSE=1 launches the duplicate pass)" % ((2 * T + 1 - T // 9), 2 * T + 1),
             "l2": "per-step working set (AUGRU input-projection cache ~0.21 MB/row, 0.87 GB at batch 4096) "
-                  "exceeds the 126 MB L2; no explicit flush"}
+                  "exceeds the 50 MB L2; no explicit flush"}
 
 
 def emit(line):
@@ -232,6 +240,42 @@ _REAL_STDOUT = 1
 if __name__ == "__main__":                      # not when imported (tests, the CPU arm's worker processes)
     _REAL_STDOUT = os.dup(1)
     os.dup2(2, 1)
+
+
+DUMP_ROWS = 512          # env rows that --dump-outputs keeps: a fixed, seeded sample, so the dump stays small at any batch
+DUMP_SEED = 20240901
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, trainer, last, B):
+    """What the timed path computed in its last step, on a seeded sample of env rows -> out_dir/<name>.npy (float32, or
+    float64 for f64 / integer data).  Refuses to write more than DUMP_MAX_BYTES."""
+    import torch
+    rows = np.sort(np.random.default_rng(DUMP_SEED).permutation(B)[:min(B, DUMP_ROWS)])
+    if trainer is not None:
+        buf = trainer.buf
+        sel = torch.as_tensor(rows, device=buf.obs.device)
+        final_obs, final_done = trainer.final_step
+        arrays = {"reward": buf.reward[:, sel], "value": buf.value[:, sel], "logp": buf.logp[:, sel], "action": buf.action[:, sel],
+                  "obs": buf.obs[:, sel], "logits": buf.logits[:, sel], "mask": buf.mask[:, sel],
+                  "final_obs": final_obs["obs"][sel], "final_mask": final_obs["action_mask"][sel],
+                  "final_done": torch.as_tensor(final_done, device=buf.obs.device)[sel],
+                  "policy_params": trainer.policy.flat.detach()}
+    else:
+        sel = torch.as_tensor(rows, device=last["obs"].device)
+        arrays = {"reward": last["reward"][sel], "done": torch.as_tensor(last["done"], device=sel.device)[sel],
+                  "obs": last["obs"][sel], "mask": last["mask"][sel]}
+    arrays["rows"] = rows
+    out = {}
+    for name, a in arrays.items():
+        a = a.detach().cpu().numpy() if hasattr(a, "detach") else np.asarray(a)
+        out[name] = a.astype(np.float64 if a.dtype in (np.float64, np.int64, np.int32) else np.float32)
+    total = sum(a.nbytes for a in out.values())
+    if total > DUMP_MAX_BYTES:
+        raise SystemExit("bench: --dump-outputs would write %d bytes (limit %d)" % (total, DUMP_MAX_BYTES))
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def main():
@@ -250,6 +294,8 @@ def main():
     ap.add_argument("--cpu-sample-rows", type=int, default=128, help="CPU arm: at most this many env rows per worker process")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--kernels", action="store_true", help="also print a per-kernel time breakdown (stderr)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path computed in its last step to DIR/<name>.npy (see the module doc)")
     args = ap.parse_args()
     world_env = int(os.environ.get("WORLD_SIZE", "1"))
     if world_env > 1:
@@ -298,6 +344,7 @@ def main():
     env.seed(rank)
     eng = env.sim.engine
     trainer, learner_launches = None, (lambda: 0)
+    last = {}                                                           # --conti: the last env step's outputs
     if args.conti:
         gen = torch.Generator(device=dev).manual_seed(1234 + rank)
 
@@ -307,6 +354,7 @@ def main():
                 a = env.offline_action                                  # logged items' embeddings, f64 [B, 32] on the device
                 a = a + 0.3 * torch.randn(a.shape, generator=gen, device=dev, dtype=a.dtype)
                 obs, reward, done, info = env.step(a)
+            last.update(obs=obs["obs"], mask=obs["action_mask"], reward=reward, done=done)
             return reward
 
         episode_device = episode_env_only = rollout_conti
@@ -344,6 +392,8 @@ def main():
         clocks.start()
     ms = timed(episode_device, args.steps)
     clk = clocks.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, trainer, last, B)
     prof = eng.profile_read()
     eng.profile(0)
     gpu_launches = eng.launch_count() + learner_launches() - launches0   # env kernels + policy/learner kernels
@@ -397,17 +447,11 @@ def main():
         au = au[0]
         achieved = au["work"] / (au["ms"] / 1e3) / 1e12
         peak = peaks["bf16_tflops_sustained"]
-        traffic, traffic_src = None, None
-        tp = os.path.join(ROOT, "profiles", "augru_traffic.json")
-        if os.path.exists(tp):
-            tj = json.load(open(tp))
-            traffic, traffic_src = tj.get("dram_bytes_per_launch"), tj.get("source")
-        roofline = {"kernel": "AUGRU recurrence, tcgen05.mma.cta_group::2 kind::f16, bf16 hi/lo split x3, fp32 TMEM accumulators: k_augru_pair2 "
-                              "(one recurrence per CTA pair) / k_augru_pp (two per pair), chosen per launch by r4_augru_kernel_for",
+        roofline = {"kernel": "AUGRU recurrence k_augru_tc: wgmma m64n64k16 bf16, hi/lo split x3, fp32 register accumulators, "
+                              "one warpgroup per 64 rows, weights streamed by bulk copy",
                     "bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
-                    "frac": achieved / peak, "traffic": traffic,
-                    "traffic_source": traffic_src or "profiles/augru_traffic.json (ncu --set full capture of an observation-pass launch, committed; not re-measured in this run)",
-                    "peak_source": "%s bf16 GEMM, sustained (kernel timed inside a long step)" % peaks["source"],
+                    "frac": achieved / peak, "traffic": None, "traffic_source": "not measured",
+                    "peak_source": "%s bf16 peak" % peaks["source"],
                     "launches": au["launches"], "avg_launch_ms": au["ms"] / au["launches"],
                     "share_of_step": au["ms"] / ms}
     bpt = BYTES_PER_TRANSITION.get(T, 176768)
@@ -418,16 +462,10 @@ def main():
         if gk:
             gk = gk[0]
             gbs = gk["work"] / (gk["ms"] / 1e3) / 1e9
-            traffic, traffic_src = None, None
-            tp = os.path.join(ROOT, "profiles", "dnn_gather_traffic.json")
-            if os.path.exists(tp):
-                tj = json.load(open(tp))
-                traffic, traffic_src = tj.get("dram_bytes_per_launch"), tj.get("source")
             roofline = {"kernel": "k_cat_pool: Embedding gather + GlobalAveragePooling1D of the dnn simulator, 21 x 512 B rows per "
                                   "feature row staged by cp.async.bulk (1-D TMA) into shared memory, 128-bit reduction reads",
-                        "bound": "hbm", "achieved": gbs, "peak": hbm, "unit": "GB/s", "frac": gbs / hbm, "traffic": traffic,
-                        "traffic_source": traffic_src or "profiles/dnn_gather_traffic.json (ncu capture; the 51 MB table is L2-resident, "
-                                                          "so DRAM traffic is far below the algorithmic bytes)",
+                        "bound": "hbm", "achieved": gbs, "peak": hbm, "unit": "GB/s", "frac": gbs / hbm, "traffic": None,
+                        "traffic_source": "not measured",
                         "algorithmic_bytes_per_row": 21 * 4 + 21 * 512, "launches": gk["launches"],
                         "avg_launch_ms": gk["ms"] / gk["launches"], "share_of_step": gk["ms"] / ms,
                         "peak_source": "%s HBM copy bandwidth" % peaks["source"]}

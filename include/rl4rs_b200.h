@@ -1,5 +1,5 @@
 /*
- * rl4rs_b200.h -- C-ABI of the B200-native RL4RS hot path (librl4rs_b200.so).
+ * rl4rs_b200.h -- C-ABI of the H100-native RL4RS hot path (librl4rs_b200.so).
  *
  * The reference has no FFI: its "operator API" for this path is the Python protocol
  * RecEnvBase / RecSimBase / RecState (rl4rs/env/base.py:26-57,111-175,178-273).  Each entry
@@ -162,11 +162,10 @@ int r4_profile(r4_env* env, int mode);
 int r4_profile_read(r4_env* env, int slot, const char** name, double* ms, int64_t* launches, double* work);
 /* ABI version of the build */
 int r4_abi_version(void);
-/* Which AUGRU kernel an observation / reward pass of `ctas` = 2 x ceil(rows / 128) tile-sequences runs on a device
- * with `sms` multiprocessors: 2 = k_augru_pair2 (one recurrence per 2-CTA cluster, tcgen05.mma.cta_group::2),
- * 3 = k_augru_pp (both sequences of a tile per cluster); 0 for bad arguments.  Pure host arithmetic, exposed so the
- * choice is testable and so a caller can predict the rounding regime of a launch (the two kernels agree to the parity
- * tolerance, not bit for bit).  No reference counterpart. */
+/* Wave-count rule between two AUGRU kernel shapes (2 = one recurrence per CTA pair, 3 = two per pair) for `ctas` =
+ * 2 x ceil(rows / 128) tile-sequences on a device with `sms` multiprocessors; 0 for bad arguments.  Pure host arithmetic.
+ * This build has ONE AUGRU kernel (k_augru_tc, wgmma): the rule and the "augru_*" / "scores_impl" options below are kept
+ * for ABI compatibility and do not change which kernel runs.  No reference counterpart. */
 int r4_augru_kernel_for(int ctas, int sms);
 /* Process-wide kernel-choice overrides for parity tests and A/B timing (no reference counterpart):
  *   "augru_kernel"     0 = by r4_augru_kernel_for (default), 2 = always the pair kernel, 3 = always the ping-pong pair kernel

@@ -1,4 +1,4 @@
-"""rl4rs_b200 -- B200-native batched SlateRecEnv / SeqSlateRecEnv (the RL4RS hot path).
+"""rl4rs_b200 -- H100-native batched SlateRecEnv / SeqSlateRecEnv (the RL4RS hot path).
 
 Importing the package does not need a GPU; constructing an env does (no CPU fallback).
 Env ids are registered like rl4rs/__init__.py:10-18.

@@ -1,6 +1,6 @@
 """ctypes binding of librl4rs_b200.so (include/rl4rs_b200.h).  Thin: no compute here.
 
-The library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_100a).  There is NO CPU
+The library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_90a).  There is NO CPU
 fallback: if the shared object is missing or cannot be loaded the import of any env class fails
 with the reason; if it loads but no CUDA device is present, creating an env fails.
 """

@@ -1,19 +1,10 @@
-// r4_augru_tc.cuh -- common ground of the tcgen05 recurrence kernels (AUGRU pair / ping-pong kernels, GRU-1, attention
-// scores, GEMM): constants of the AUGRU problem, the PTX wrappers (mbarrier, bulk copy, tcgen05.mma / ld / st / commit,
-// descriptors), the bf16 hi/lo split, the quad-layout input loads and the parameter structs of the AUGRU kernels.
+// r4_augru_tc.cuh -- common ground of the tensor-core kernels (GRU-1 / AUGRU recurrences, attention scores, GEMM):
+// constants of the AUGRU problem, the PTX wrappers (wgmma, mbarrier, bulk copy), the bf16 hi/lo split, the quad-layout
+// input loads and the parameter structs of the AUGRU kernel (r4_recur.cuh).
 //
-// The AUGRU recurrence (deepctr VecAttGRUCell, nets/utils.py:123-124), per step, with h the 256-wide state:
-//     u = sigmoid(Xu_t + h Wu)      r = sigmoid(Xr_t + h Wr)      c = tanh(Xc_t + (r*h) Wc)
-//     u' = (1 - score_t) u ;  h <- u' h + (1 - u') c
-// fp32 parity on a bf16 tensor pipe: every fp32 operand x is split x = hi + lo (both bf16, lo =
-// bf16(x - hi)) and each product is issued as hi*hi + lo*hi + hi*lo (3 MMAs, fp32 accumulate):
-// relative error ~2^-16 per term, measured 1e-5..3e-5 of rms on the 64-step recurrence against
-// f64 (tools/split_sim.py) -- inside the 1e-4 parity bound.  The state h itself stays fp32 in the
-// epilogue threads' registers; only the MMA operand copies are rounded.
-//
-// The kernels: r4_augru_pair2.cuh (one recurrence per CTA pair) and r4_augru_pp.cuh (two per pair).  The round-1 kernel
-// that lived here (k_augru_tc: one CTA per 128-row tile-sequence, 36.7 k cycles per step against 15.5 k / 14.3 k) lost
-// every regime to them and was deleted at the end of round 2.
+// fp32 parity on a bf16 tensor pipe: every fp32 operand x is split x = hi + lo (both bf16, lo = bf16(x - hi)) and each
+// product is issued as hi*hi + lo*hi + hi*lo (3 MMAs, fp32 accumulate): relative error ~2^-16 per term, inside the 1e-4
+// parity bound on the 64-step recurrence.  The state h itself stays fp32 in registers; only the MMA operand copies are rounded.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -23,34 +14,41 @@
 
 namespace r4tc {
 
-constexpr int TM = 128;                 // rows per CTA tile (UMMA_M)
+constexpr int TM = 128;                 // rows per lane-major input tile
 constexpr int HID = 256;                // AUGRU hidden = GEMM N and K
 constexpr int STEPS = 64;
 constexpr int KB = 32;                  // K elements per B stage
 constexpr int NKB = HID / KB;           // 8 K blocks per matrix
-constexpr int STAGE_BYTES = HID * KB * 2;            // 16384
-constexpr int A_BYTES = TM * HID * 2;                // 65536 per split
 constexpr int LBO = 128;                             // K-adjacent core matrices
-constexpr int A_SBO = (HID / 8) * 128;               // 4096: 8-row groups of the A operand
-constexpr int B_SBO = (KB / 8) * 128;                // 512:  8-row groups inside a B stage
-constexpr int W_IMAGE_BYTES = 3 * NKB * 2 * STAGE_BYTES;   // 786432 per sequence: r, u, c x 8 K blocks x (hi, lo)
+constexpr int B_SBO = (KB / 8) * 128;                // 512:  8-row groups inside a 32-deep weight block
 constexpr int XT_COLS = 3 * HID;                     // transposed input halves: [r | u | c] rows of 128 lanes
-constexpr int NTHREADS = 384;               // 8 epilogue warps + one control warpgroup (MMA, TMA, 2 idle)
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
+// Shared-memory matrix descriptor of a wgmma operand in the SWIZZLE_NONE K-major layout: 8-row x 16-byte core matrices,
+// `lbo` = byte distance of K-adjacent core matrices, `sbo` = byte distance of 8-row groups (layout type 0 in bits 62-63).
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
   return (uint64_t)((saddr >> 4) & 0x3fff) | ((uint64_t)((lbo >> 4) & 0x3fff) << 16) |
-         ((uint64_t)((sbo >> 4) & 0x3fff) << 32) | ((uint64_t)1 << 46);   // version 1, SWIZZLE_NONE
+         ((uint64_t)((sbo >> 4) & 0x3fff) << 32);
 }
-__device__ __forceinline__ constexpr uint32_t make_idesc(int m, int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+// D[64 x N] (+)= A[64 x 16] . B[16 x N]^T, bf16 in, fp32 accumulators in the registers of the issuing warpgroup.  Register
+// i of a thread (warp w of the warpgroup, lane l) holds row 16 w + l / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (l % 4) + i % 2.
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+               : "l"(da), "l"(db), "r"(1) : "memory");
 }
-__device__ __forceinline__ void mma_bf16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-               :: "r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(acc) : "memory");
+__device__ __forceinline__ void wgmma_m64n16k16_rs(float (&d)[8], const uint32_t (&a)[4], uint64_t db) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, 0;\n\t}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(1) : "memory");
 }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
+
 __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(smem_u32(bar)), "r"(count) : "memory");
 }
@@ -70,28 +68,18 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                :: "r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// generic-proxy shared-memory stores -> visible to the async proxy (wgmma operand reads, bulk copies)
 __device__ __forceinline__ void proxy_fence() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t* u = reinterpret_cast<uint32_t*>(v);
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-               : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]),
-                 "=r"(u[8]), "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15])
-               : "r"(taddr) : "memory");
+__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
+  asm volatile("bar.sync %0, %1;" :: "r"(id), "r"(nthreads) : "memory");
 }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float* v) {
-  const uint32_t* u = reinterpret_cast<const uint32_t*>(v);
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-               :: "r"(taddr), "r"(u[0]), "r"(u[1]), "r"(u[2]), "r"(u[3]), "r"(u[4]), "r"(u[5]), "r"(u[6]), "r"(u[7]),
-                  "r"(u[8]), "r"(u[9]), "r"(u[10]), "r"(u[11]), "r"(u[12]), "r"(u[13]), "r"(u[14]), "r"(u[15]) : "memory");
+// two fp32 -> bf16 pair words (low half = first value): hi = bf16(x), lo = bf16(x - hi)
+__device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
+  const __nv_bfloat162 h = __floats2bfloat162_rn(x0, x1);
+  const __nv_bfloat162 l = __floats2bfloat162_rn(x0 - __bfloat162float(h.x), x1 - __bfloat162float(h.y));
+  hi = *reinterpret_cast<const uint32_t*>(&h);
+  lo = *reinterpret_cast<const uint32_t*>(&l);
 }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // MUFU-based gate functions: ex2.approx (rel. error 2^-22) + rcp.approx (1 ulp); saturate correctly
 // (ex2 -> +inf gives rcp -> 0).  No slow-path calls (the IEEE __frcp_rn costs a CALL per element).
@@ -139,7 +127,7 @@ __device__ __forceinline__ void load_x16(float* dst, const float* ts, int colbas
 
 struct AugruTcSeq {
   const float* XT;        // transposed input halves [n_tiles_cached, 64, 768 / 4, 128, 4]  (tile, step, column quad, lane, column % 4)
-  const uint8_t* Wimg;    // pre-tiled bf16 hi/lo weight image of the pair kernels (r4_augru_pair.cuh: build_pair_image)
+  const uint8_t* Wimg;    // pre-tiled bf16 hi/lo weight stream (r4_recur.cuh: build_recur_image)
   const float* scoresT;   // [n_row_tiles, 64, 128]
   float* out;             // final state, row stride out_ld
   int shared;             // 1: every row reads cached sequence 0
@@ -147,7 +135,6 @@ struct AugruTcSeq {
 struct AugruTcParams {
   AugruTcSeq s[2];
   int R, row0, div, out_ld;
-  long long* dbg;         // optional: per-step phase timestamps of CTA 0 (development probe), else null
 };
 
 // host-side bf16 rounding (round to nearest even) shared by the weight-image builders

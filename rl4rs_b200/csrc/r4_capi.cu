@@ -3,12 +3,9 @@
 #include "../../include/rl4rs_b200.h"
 #include "r4_kernels.cuh"
 #include "r4_augru_tc.cuh"
-#include "r4_augru_pair.cuh"
-#include "r4_augru_pair2.cuh"
-#include "r4_augru_pp.cuh"
 #include "r4_gemm_tc.cuh"
 #include "r4_scores_tc.cuh"
-#include "r4_gru_tc.cuh"
+#include "r4_recur.cuh"
 #include "r4_ppo.cuh"
 #include "r4_comm.cuh"
 
@@ -19,6 +16,12 @@
 #include <map>
 #include <string>
 #include <vector>
+
+// SMs of the current device (132 on an H100 SXM)
+static int sm_count() {
+  static const int n = [] { int d = 0, v = 132; cudaGetDevice(&d); cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, d); return v; }();
+  return n;
+}
 
 using namespace r4;
 
@@ -43,9 +46,7 @@ struct PerSeq {
   float *au_wx = nullptr, *au_bx = nullptr, *au_wgh = nullptr, *au_wch = nullptr;
   float *wqd = nullptr, *wp = nullptr, *ab1 = nullptr, *aw2 = nullptr, *ab2 = nullptr, *akv = nullptr;
   uint8_t *gru_wx_img = nullptr, *au_wx_img = nullptr, *wp_img = nullptr, *gru_img = nullptr;   // pre-tiled bf16 hi/lo images of the input projections
-  uint8_t* au_pair_img = nullptr;   // the same weights tiled per CTA rank for the 2-CTA kernel (r4_augru_pair.cuh)
-  CUtensorMap au_pair_tmap;    // au_pair_img as a 2-D tensor of 1 KB rows (r4_augru_pair2.cuh: tensor-map TMA ring)
-  bool au_pair_tmap_ok = false;
+  uint8_t* au_img = nullptr;   // the same weights as the recurrence kernel's weight stream (r4_recur.cuh)
   float abk = 0.f;
 };
 
@@ -123,7 +124,7 @@ int fail(r4_env* e, int code, const std::string& msg) {
 enum { SL_ACT = 0, SL_ASSEMBLE, SL_SEQIDS, SL_GEMM_XIN, SL_GRU1, SL_GEMM_XK, SL_SCORES, SL_AUGRU, SL_CAT,
        SL_GEMM_DENSE, SL_GEMM_HEAD, SL_RHEAD, SL_REWARD, SL_XT, SL_MISC, SL_COUNT };
 const char* const SLOT_NAMES[SL_COUNT] = {"k_act", "k_assemble", "k_seq_ids", "k_gemm_tc[gru1 input proj + E_s gather]",
-    "k_gru_tc[GRU-1 tcgen05]", "k_gemm_tc[augru/att input proj]", "k_scores_tc", "k_augru[AUGRU tcgen05: pair2 / pp]", "k_cat_attn | k_cat_pool",
+    "k_gru_tc[GRU-1 wgmma]", "k_gemm_tc[augru/att input proj]", "k_scores_tc", "k_augru_tc[AUGRU wgmma]", "k_cat_attn | k_cat_pool",
     "k_gemm_tc[dense tower]", "k_gemm_tc[head 3456x256]", "k_reward_head", "k_reward", "k_transpose_x", "k_query"};
 
 // Brackets one launch with CUDA events on the launching stream when profiling is on.
@@ -202,7 +203,7 @@ int gemm(r4_env* e, int slot, int act, int M, int N, int K, const float* A, int 
   p.bnt = bnt;
   p.A2 = A2; p.gather2 = gather2; p.k2_start = k2_start; p.g2_n = g2_n;
   p.tm_steps = tm_steps;
-  static const int sms = [] { int d = 0, n = 148; cudaGetDevice(&d); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d); return n; }();
+  const int sms = sm_count();
   int tiles = ((M + r4tc::G_BM - 1) / r4tc::G_BM) * ((N + bnt - 1) / bnt);
   // split-K when the output tiles leave SMs idle and K is long (each part keeps >= 16 K blocks): the head at 4096 rows
   static const bool no_splitk = getenv("R4_NO_SPLITK") != nullptr;
@@ -253,7 +254,7 @@ int build_cache(r4_env* e, int si, const int32_t* ids, int n, SeqCache& c, cudaS
       { ProfScope ps(e, SL_GRU1, st, (double)ns * MAXLEN * 2.0 * (EMB * 2 * EMB + EMB * EMB));
         r4tc::GruTcParams gp{xinT, w.gru_img, nullptr, ns};
         gp.hard = 1; gp.Hlast = reinterpret_cast<float*>(c.H.p) + (size_t)s0 * EMB; gp.ld_last = EMB;
-        r4tc::k_gru_tc<<<(ns + TM - 1) / TM, r4tc::NTHREADS, r4tc::G1_SMEM_BYTES, st>>>(gp); }
+        r4tc::k_gru_tc<<<(ns + r4tc::RC_ROWS - 1) / r4tc::RC_ROWS, r4tc::RC_THREADS, r4tc::G1_SMEM_BYTES, st>>>(gp); }
       R4_LAUNCH_CHECK(e, "k_gru_tc");
     }
     return R4_OK;
@@ -275,7 +276,7 @@ int build_cache(r4_env* e, int si, const int32_t* ids, int n, SeqCache& c, cudaS
                    w.gru_bx, nullptr, XIN_LD, st, ns, 0, XIN_LD, xinT, nullptr))) return rc;
     { ProfScope ps(e, SL_GRU1, st, (double)ns * MAXLEN * 2.0 * (EMB * 2 * EMB + EMB * EMB));
       r4tc::GruTcParams gp{xinT, w.gru_img, Hc, ns};
-      r4tc::k_gru_tc<<<(ns + TM - 1) / TM, r4tc::NTHREADS, r4tc::G1_SMEM_BYTES, st>>>(gp); }
+      r4tc::k_gru_tc<<<(ns + r4tc::RC_ROWS - 1) / r4tc::RC_ROWS, r4tc::RC_THREADS, r4tc::G1_SMEM_BYTES, st>>>(gp); }
     R4_LAUNCH_CHECK(e, "k_gru_tc");
     // H_t [Wgx | Wcx | Wk-Wd] + [bg | bc | 0]: AUGRU halves -> XT tiles, key half -> Kp
     if ((rc = gemm(e, SL_GEMM_XK, 0, ns * MAXLEN, XK_LD, EMB, Hc, EMB, nullptr, w.au_wx_img, w.au_bx, nullptr, XK_LD, st,
@@ -284,17 +285,16 @@ int build_cache(r4_env* e, int si, const int32_t* ids, int n, SeqCache& c, cudaS
   return R4_OK;
 }
 
-// Kernel-choice options (r4_set_option; the environment gives the initial values).
+// Kernel-choice options (r4_set_option; the environment gives the initial values).  There is one AUGRU kernel
+// (k_augru_tc) and one scores kernel (k_scores_tc2): force, pair_impl, cost_*, cluster and scores_impl are validated and
+// stored for ABI compatibility and select nothing (include/rl4rs_b200.h says so); cost_* only feed r4_augru_kernel_for.
 struct AugruOpts {
-  int force = 0;          // 0 rule, 2 pair kernel (one recurrence per pair), 3 ping-pong pair kernel (1 was the deleted one-CTA kernel)
-  int pair_impl = 1;      // k_augru_pair2<RELAY, TMAP>: 1 = <0,0> (default), 2 = <0,1>, 3 = <1,0>, 4 = <1,1>; k_augru_pp<RELAY> follows RELAY
-  // cost of one wave, measured (tools/augru_probe.cu, round 2, ms x 25): k_augru_pair2 0.51 ms per 74 tile-sequences,
-  // k_augru_pp 0.96 ms per 74 TILES (= 148 tile-sequences)
+  int force = 0;
+  int pair_impl = 1;
   int cost_pair = 13, cost_pp = 24;
-  int cluster = 2;        // CTAs per cluster of the pair kernel: 2, or 4 / 8 = weight stream shared by 2 / 4 pairs (multicast)
-  int scores_impl = 2;    // 2 = k_scores_tc2 (both attention layers on the tensor pipe), 1 = k_scores_tc (second layer as FFMA2)
-  int scores_shared_pct = 85;    // k_scores_tc2: CTA share of a shared (L2-resident) sequence, per cent of an even split (tools/scores_probe.cu,
-                                 // us per 4096-row pass: 100 % 98.5, 85 % 86.8, 75 % 90.1, 65 % 100.6, 55 % 120.8)
+  int cluster = 2;
+  int scores_impl = 2;
+  int scores_shared_pct = 85;    // k_scores_tc2: CTA share of a shared (L2-resident) sequence, per cent of an even split
   int pay_obs_reuse = 1;  // a paying step takes its observation from its reward pass (r4_step); 0 = separate observation pass
   AugruOpts() {
     if (getenv("R4_NO_PAY_OBS_REUSE")) pay_obs_reuse = 0;
@@ -310,9 +310,8 @@ struct AugruOpts {
 };
 AugruOpts& augru_opts() { static AugruOpts o; return o; }
 
-// Which AUGRU kernel runs `ctas` = 2 x row tiles (tile-sequences) of work: 2 = k_augru_pair2 (a CTA pair per tile-sequence),
-// 3 = k_augru_pp (a CTA pair per TILE, both sequences in flight).  The pair kernel finishes a tile sooner, the ping-pong
-// kernel keeps the tensor pipe busier but needs twice the tiles to fill the chip: compare wave counts x measured wave times.
+// r4_augru_kernel_for: wave counts x per-wave costs of two kernel shapes (2 = a CTA pair per tile-sequence, 3 = a CTA pair
+// per tile).  Kept as ABI arithmetic only: no launch consults it.
 static int augru_rule(int ctas, int sms) {
   const AugruOpts& o = augru_opts();
   const int pairs = sms / 2;
@@ -320,12 +319,6 @@ static int augru_rule(int ctas, int sms) {
   const long c3 = (long)o.cost_pp * (((ctas + 1) / 2 + pairs - 1) / pairs);
   return c3 <= c2 ? 3 : 2;
 }
-static int augru_choice(int ctas) {
-  static const int sms = [] { int d = 0, n = 148; cudaGetDevice(&d); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d); return n; }();
-  const int force = augru_opts().force;
-  return force ? force : augru_rule(ctas, sms);
-}
-static int augru_pair_impl() { return augru_opts().pair_impl; }
 
 // One simulator pass over `R` feature rows (cat/dense already assembled, chunk-local pointers).
 int forward_rows(r4_env* e, int R, int row0, int div, const int32_t* cat, const float* dense,
@@ -335,7 +328,7 @@ int forward_rows(r4_env* e, int R, int row0, int div, const int32_t* cat, const 
   if (e->sim == R4_SIM_LSTM) {
     // nets/lstm.py:29-36: all = [GRU(seq0) | GRU(seq1) | dense tower | GRU(E_c[cat]) | Flatten(E_c[cat])] -> Dense(256, ELU) =
     // simulator_obs -> softmax head.  The sequence GRUs' last states come from the caches; the category GRU (21 steps)
-    // runs per pass: E_c gather fused into its input projection, then the tcgen05 recurrence writes its last state
+    // runs per pass: E_c gather fused into its input projection, then the wgmma recurrence writes its last state
     // straight into the feature slab; the Flatten() part is gathered by the head GEMM's A staging (as in the dien head).
     const int TM = r4tc::TM, LD = 4 * EMB;                  // materialised part of the feature vector: 512 columns
     const int rtiles = (R + TM - 1) / TM;
@@ -354,7 +347,7 @@ int forward_rows(r4_env* e, int R, int row0, int div, const int32_t* cat, const 
     { ProfScope ps(e, SL_GRU1, st, (double)R * NCAT * 2.0 * (EMB * 2 * EMB + EMB * EMB));
       r4tc::GruTcParams gp{cgx, e->cg_img, nullptr, R};
       gp.steps = NCAT; gp.hard = 1; gp.Hlast = allf + 3 * EMB; gp.ld_last = LD;
-      r4tc::k_gru_tc<<<rtiles, r4tc::NTHREADS, r4tc::G1_SMEM_BYTES, st>>>(gp); }
+      r4tc::k_gru_tc<<<(R + r4tc::RC_ROWS - 1) / r4tc::RC_ROWS, r4tc::RC_THREADS, r4tc::G1_SMEM_BYTES, st>>>(gp); }
     R4_LAUNCH_CHECK(e, "k_gru_tc");
     if ((rc = gemm(e, SL_GEMM_DENSE, 1, R, HU, NDENSE, dense, NDENSE, nullptr, e->w1_img, e->b1, tmp, HU, st))) return rc;
     if ((rc = gemm(e, SL_GEMM_DENSE, 1, R, HU, HU, tmp, HU, nullptr, e->w2_img, e->b2, allf + 2 * EMB, LD, st))) return rc;
@@ -405,7 +398,7 @@ int forward_rows(r4_env* e, int R, int row0, int div, const int32_t* cat, const 
     if ((rc = reserve(e, e->ws_tmp, (size_t)R * OBSD * 4))) return rc;
     float* allf = reinterpret_cast<float*>(e->ws_allf.p);
     float* tmp = reinterpret_cast<float*>(e->ws_tmp.p);
-    static const int sms = [] { int d = 0, n = 148; cudaGetDevice(&d); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d); return n; }();
+    const int sms = sm_count();
     { ProfScope ps(e, SL_CAT, st, (double)R * (NCAT * 4 + NCAT * EMB * 4));       // work = algorithmic gather bytes
       const int blocks = std::max(1, std::min((R + POOL_WARPS - 1) / POOL_WARPS, 2 * sms));
       k_cat_pool<<<blocks, POOL_WARPS * 32, POOL_SMEM, st>>>(R, cat, e->emb_cat, allf, 2 * HU); }
@@ -451,7 +444,7 @@ int forward_rows(r4_env* e, int R, int row0, int div, const int32_t* cat, const 
     s.scoresT = scores + (size_t)i * sc_per_seq;
     s.shared = sh[i];
     r4tc::AugruTcSeq& q = rp.s[i];
-    q.XT = reinterpret_cast<const float*>(cs[i]->XT.p); q.Wimg = w.au_pair_img; q.scoresT = s.scoresT;
+    q.XT = reinterpret_cast<const float*>(cs[i]->XT.p); q.Wimg = w.au_img; q.scoresT = s.scoresT;
     q.out = allf + i * AUH; q.shared = sh[i];
   }
   sp.R = R; sp.row0 = row0; sp.div = div; sp.q = qbuf;
@@ -485,46 +478,14 @@ int forward_rows(r4_env* e, int R, int row0, int div, const int32_t* cat, const 
                                                 qbuf, qa0, qa1); }
   R4_LAUNCH_CHECK(e, "k_query");
   { ProfScope ps(e, SL_SCORES, st, (double)R * 2 * MAXLEN * 2.0 * (EMB * AH1 + AH1 * AH2 + AH2));
-    const int nt = (R + 1) / 2;
-    if (augru_opts().scores_impl == 1) r4tc::k_scores_tc<<<dim3(std::min(nt, 74), 2), r4tc::S_THREADS, r4tc::S_SMEM_BYTES, st>>>(sp, cat, e->emb_seq);
-    else {
-      const int ctas = std::min(2 * nt, 148);
-      r4tc::k_scores_tc2<false><<<ctas, r4tc::S2_THREADS, r4tc::S2_SMEM_BYTES, st>>>(
-          sp, r4tc::scores_grid_split(ctas, nt, sh[0], sh[1], augru_opts().scores_shared_pct));
-    } }
+    const int ctas = std::min(2 * R, 2 * sm_count());
+    r4tc::k_scores_tc2<<<ctas, r4tc::S2_THREADS, r4tc::S2_SMEM_BYTES, st>>>(
+        sp, r4tc::scores_grid_split(ctas, R, sh[0], sh[1], augru_opts().scores_shared_pct)); }
   R4_LAUNCH_CHECK(e, "k_scores_tc");
   if (!no_side && !side_early) R4_CUDA(e, cudaEventRecord(e->ev_fork, st));
   { ProfScope ps(e, SL_AUGRU, st, (double)R * 2 * MAXLEN * 2.0 * (AUH * 2 * AUH + AUH * AUH));
-    const dim3 pgrid(rtiles * 2, 2);
-    const int which = augru_choice(2 * rtiles);
-    if (which == 3) {
-      r4tc::AugruPairParams pp;
-      pp.b = rp; pp.tmap[0] = e->ps[0].au_pair_tmap; pp.tmap[1] = e->ps[1].au_pair_tmap;
-      if (augru_pair_impl() >= 3) r4tc::k_augru_pp<1><<<dim3(rtiles * 2), r4tc::NTHREADS, r4tc::PP_SMEM_BYTES, st>>>(pp);
-      else r4tc::k_augru_pp<0><<<dim3(rtiles * 2), r4tc::NTHREADS, r4tc::PP_SMEM_BYTES, st>>>(pp);
-    } else {
-      r4tc::AugruPairParams pp;
-      pp.b = rp; pp.tmap[0] = e->ps[0].au_pair_tmap; pp.tmap[1] = e->ps[1].au_pair_tmap;
-      // cluster size = CTAs sharing one weight stream (2 = one pair, 4 / 8 = 2 / 4 pairs: multicast ring)
-      const int cs = augru_opts().cluster;
-      cudaLaunchConfig_t lc = {};
-      cudaLaunchAttribute at[1];
-      at[0].id = cudaLaunchAttributeClusterDimension;
-      at[0].val.clusterDim.x = cs; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-      lc.gridDim = dim3((pgrid.x + cs - 1) / cs * cs, 2); lc.blockDim = dim3(r4tc::NTHREADS);
-      lc.dynamicSmemBytes = r4tc::P_SMEM_BYTES; lc.stream = st; lc.attrs = at; lc.numAttrs = 1;
-      cudaError_t le;
-      if (cs == 4) le = cudaLaunchKernelEx(&lc, r4tc::k_augru_pair2<0, 1, 4>, pp);
-      else if (cs == 8) le = cudaLaunchKernelEx(&lc, r4tc::k_augru_pair2<0, 1, 8>, pp);
-      else switch (augru_pair_impl()) {
-        case 2: le = cudaLaunchKernelEx(&lc, r4tc::k_augru_pair2<0, 1, 2>, pp); break;
-        case 3: le = cudaLaunchKernelEx(&lc, r4tc::k_augru_pair2<1, 0, 2>, pp); break;
-        case 4: le = cudaLaunchKernelEx(&lc, r4tc::k_augru_pair2<1, 1, 2>, pp); break;
-        default: le = cudaLaunchKernelEx(&lc, r4tc::k_augru_pair2<0, 0, 2>, pp); break;
-      }
-      (void)le;
-    } }
-  R4_LAUNCH_CHECK(e, augru_choice(2 * rtiles) == 3 ? "k_augru_pp" : "k_augru_pair2");
+    r4tc::k_augru_tc<<<dim3((R + r4tc::RC_ROWS - 1) / r4tc::RC_ROWS, 2), r4tc::RC_THREADS, r4tc::AU_SMEM_BYTES, st>>>(rp); }
+  R4_LAUNCH_CHECK(e, "k_augru_tc");
   if (!no_side && !side_early && (rc = side_work())) return rc;
   if (!no_side) R4_CUDA(e, cudaStreamWaitEvent(st, e->ev_join, 0));
   float* obs = obs_out;
@@ -697,17 +658,9 @@ int r4_create(const r4_config* cfg, int device, r4_env** out) {
             cudaMalloc(&e->sflag, (size_t)e->B) == cudaSuccess;
   if (!ok) { r4_destroy(e); return fail(nullptr, R4_ERR_NOMEM, "r4_create: cudaMalloc failed"); }
   cudaFuncSetAttribute(r4tc::k_gru_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, r4tc::G1_SMEM_BYTES);
-  cudaFuncSetAttribute(r4tc::k_augru_pair2<0, 1, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, r4tc::P_SMEM_BYTES);
-  cudaFuncSetAttribute(r4tc::k_augru_pair2<0, 1, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, r4tc::P_SMEM_BYTES);
-  cudaFuncSetAttribute(r4tc::k_augru_pp<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, r4tc::PP_SMEM_BYTES);
-  cudaFuncSetAttribute(r4tc::k_augru_pp<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, r4tc::PP_SMEM_BYTES);
-  cudaFuncSetAttribute(r4tc::k_augru_pair2<1, 1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, r4tc::P_SMEM_BYTES);
-  cudaFuncSetAttribute(r4tc::k_augru_pair2<0, 1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, r4tc::P_SMEM_BYTES);
-  cudaFuncSetAttribute(r4tc::k_augru_pair2<1, 0, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, r4tc::P_SMEM_BYTES);
-  cudaFuncSetAttribute(r4tc::k_augru_pair2<0, 0, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, r4tc::P_SMEM_BYTES);
+  cudaFuncSetAttribute(r4tc::k_augru_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, r4tc::AU_SMEM_BYTES);
   cudaFuncSetAttribute(r4tc::k_gemm_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, r4tc::G_SMEM_BYTES);
-  cudaFuncSetAttribute(r4tc::k_scores_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, r4tc::S_SMEM_BYTES);
-  cudaFuncSetAttribute(r4tc::k_scores_tc2<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, r4tc::S2_SMEM_BYTES);
+  cudaFuncSetAttribute(r4tc::k_scores_tc2, cudaFuncAttributeMaxDynamicSharedMemorySize, r4tc::S2_SMEM_BYTES);
   cudaFuncSetAttribute(k_cat_attn, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_CAT);
   cudaFuncSetAttribute(k_cat_pool, cudaFuncAttributeMaxDynamicSharedMemorySize, POOL_SMEM);
   st = cudaGetLastError();
@@ -820,7 +773,7 @@ int r4_finalize_weights(r4_env* e, void* stream) {
           }
       for (int g = 0; g < 3; ++g) for (int n = 0; n < EMB; ++n) bx[g * EMB + n] = b[src_of[g] + n];
       std::vector<uint8_t> gi(r4tc::G1_IMAGE_BYTES);
-      r4tc::build_gru_image(wgh.data(), wch.data(), gi.data());
+      r4tc::build_recur_image(r4tc::GH, wgh.data(), wch.data(), gi.data());
       int rc2;
       if ((rc2 = upload(e, gi, rec_img)) || (rc2 = upload(e, bx, bx_dev)) || (rc2 = upload_image(e, wx.data(), EMB, XIN_LD, wx_img))) return rc2;
       return R4_OK;
@@ -949,7 +902,7 @@ int r4_finalize_weights(r4_env* e, void* stream) {
     }
     {
       std::vector<uint8_t> gi(r4tc::G1_IMAGE_BYTES);
-      r4tc::build_gru_image(wgh.data(), wch.data(), gi.data());
+      r4tc::build_recur_image(r4tc::GH, wgh.data(), wch.data(), gi.data());
       if ((rc = upload(e, gi, &w.gru_img))) return rc;
     }
     if ((rc = upload_image(e, wx.data(), EMB, XIN_LD, &w.gru_wx_img)) ||
@@ -959,14 +912,9 @@ int r4_finalize_weights(r4_env* e, void* stream) {
       r4tc::build_scores_image2(wp.data(), aw2, wpi.data());
       if ((rc = upload(e, wpi, &w.wp_img))) return rc;
     }
-    std::vector<uint8_t> img(r4tc::W_IMAGE_BYTES);
-    r4tc::build_pair_image(awgh.data(), awch.data(), img.data());
-    if ((rc = upload(e, img, &w.au_pair_img))) return rc;
-    {
-      int trc = r4tc::make_pair_tensor_map(w.au_pair_img, &w.au_pair_tmap);
-      w.au_pair_tmap_ok = trc == 0;
-      if (trc) return fail(e, R4_ERR_CUDA, "r4_finalize_weights: cuTensorMapEncodeTiled failed for the AUGRU pair weight image");
-    }
+    std::vector<uint8_t> img(r4tc::AU_IMAGE_BYTES);
+    r4tc::build_recur_image(r4tc::HID, awgh.data(), awch.data(), img.data());
+    if ((rc = upload(e, img, &w.au_img))) return rc;
     std::vector<float> vb1(ab1, ab1 + AH1), vw2(aw2, aw2 + AH1 * AH2), vb2(ab2, ab2 + AH2), vkv(akv, akv + AH2);
     if ((rc = upload(e, wx, &w.gru_wx)) || (rc = upload(e, bx, &w.gru_bx)) || (rc = upload(e, wgh, &w.gru_wgh)) ||
         (rc = upload(e, wch, &w.gru_wch)) || (rc = upload(e, awx, &w.au_wx)) || (rc = upload(e, abx, &w.au_bx)) ||
@@ -1306,7 +1254,7 @@ int r4_ppo_epoch(float* params, const float* obs, const uint8_t* mask, const int
                  float* v, int step0, float lr, float beta1, float beta2, float eps, float grad_clip,
                  float* norm_scratch, void* stream) {
   if (!perm || n < 1 || mb < 1 || mb > n || step0 < 0) return fail(nullptr, R4_ERR_ARG, "r4_ppo_epoch: bad argument");
-  const int G = std::max(1, std::min((mb + r4ppo::TS - 1) / r4ppo::TS, 148));
+  const int G = std::max(1, std::min((mb + r4ppo::TS - 1) / r4ppo::TS, sm_count()));
   const int np = r4ppo::make_layout(action_size).n;
   int steps = 0;
   const bool fused = !(grad_clip > 0.f);      // global-norm clipping needs the reduced gradient first
@@ -1451,7 +1399,7 @@ int r4_ppo_epoch_dist(r4_comm* c, float* params, const float* obs, const uint8_t
                       void* stream) {
   if (!c || !params || !perm || !m || !v || !scratch || n < 1 || mb < 1 || mb > n || step0 < 0)
     return fail(nullptr, R4_ERR_ARG, "r4_ppo_epoch_dist: bad argument");
-  const int G = std::max(1, std::min((mb + r4ppo::TS - 1) / r4ppo::TS, 148));
+  const int G = std::max(1, std::min((mb + r4ppo::TS - 1) / r4ppo::TS, sm_count()));
   const int np = r4ppo::make_layout(action_size).n;
   const float inv = 1.0f / ((float)mb * (float)c->world);
   int steps = 0;

@@ -22,7 +22,7 @@ def _ptr(t):
 class Engine(object):
     def __init__(self, config, seq, catalog, weights, log, device=None):
         if not torch.cuda.is_available():
-            raise _capi.R4Error("rl4rs_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise _capi.R4Error("rl4rs_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.lib = _capi.load_library()
         self.config = config
         self.seq = bool(seq)

@@ -43,7 +43,8 @@ class KernelOps(object):
         assert self.lib.r4_policy_num_params(A) == n_params
         z = lambda k: torch.zeros(k, dtype=torch.float32, device=device)
         self.m, self.v, self.grad, self.stats, self.norm = z(n_params), z(n_params), z(n_params), z(5), z(1)
-        self.scratch = z(148 * (n_params + 5))
+        self.sms = torch.cuda.get_device_properties(device).multi_processor_count   # grid cap of the learner kernels
+        self.scratch = z(self.sms * (n_params + 5))
         self.step = 0
         self.counter = 0
         self.launches = 0                # kernels launched through this object (bench.py: gpu_launches)
@@ -65,7 +66,7 @@ class KernelOps(object):
 
     def policy_grad(self, mode, flat, data, idx, idx_offset, n, hp, inv_n, stat_scale, G=None):
         obs, mask, act, logp, logits, val, adv, target = data
-        G = G or max(1, min((n + 3) // 4, 148))          # 4 samples per CTA tile (r4_ppo.cuh: TS)
+        G = G or max(1, min((n + 3) // 4, self.sms))          # 4 samples per CTA tile (r4_ppo.cuh: TS)
         rc = self.lib.r4_policy_grad(mode, _p(flat), _p(obs), _p(mask), _p(act), _p(logp), _p(logits), _p(val), _p(adv),
                                      _p(target), _p(idx, idx_offset * 8) if idx is not None else C.c_void_p(0), n, self.A,
                                      hp["clip"], hp["vf_clip"], hp["vf_coeff"], hp["kl_coeff"], hp["ent_coeff"], inv_n,
@@ -103,7 +104,7 @@ class KernelOps(object):
     def policy_grad_exchange(self, comm, mode, flat, data, n, hp, inv_n, stat_scale):
         """One gradient over n local samples, summed over the ranks through peer memory into self.grad (A2C)."""
         obs, mask, act, logp, logits, val, adv, target = data
-        G = max(1, min((n + 3) // 4, 148))
+        G = max(1, min((n + 3) // 4, self.sms))
         rc = self.lib.r4_policy_grad_partial(mode, _p(flat), _p(obs), _p(mask), _p(act), _p(logp), _p(logits), _p(val), _p(adv),
                                              _p(target), C.c_void_p(0), n, self.A, hp["clip"], hp["vf_clip"], hp["vf_coeff"],
                                              hp["kl_coeff"], hp["ent_coeff"], inv_n, _p(self.scratch), G, self._stream())
@@ -257,6 +258,7 @@ class _TrainerBase(object):
                 buf.action[t].copy_(a); buf.logp[t].copy_(logp); buf.value[t].copy_(value); buf.logits[t].copy_(logits)
             obs, reward, done, info = env.step(a)
             buf.reward[t].copy_(reward)
+        self.final_step = (obs, done)          # what the episode's last step returned
         return buf
 
     def _gae(self, buf):

@@ -1,7 +1,7 @@
 """Vector adapter over the batched env (SURVEY.md section 8b item 4; reference `rl4rs/utils/rllib_vector_env.py:9-69`).
 
 The reference wraps ONE batched `RecEnvBase` as an RLlib `VectorEnv` of `batch_size` sub-envs so that RLlib's sampler
-can drive it.  ray is not part of this image and the B200 trainer does not need it (`rl4rs_b200.trainer` consumes the
+can drive it.  ray is not part of this image and the GPU trainer does not need it (`rl4rs_b200.trainer` consumes the
 batched env directly), so this class keeps the reference's method names and semantics without the ray base class:
 
 * `vector_reset()`             -> `env.reset()`                                  (rllib_vector_env.py:26-32)

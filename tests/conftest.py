@@ -12,7 +12,7 @@ _KEEP = []
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
     # The CPU suite is hundreds of small NumPy / torch products (the oracles).  With a BLAS thread per core they spend
     # their time handing 100-microsecond products to spinning worker threads, and glibc returns every temporary above
     # 128 KB to the kernel: on the 8-core build container the same suite takes 24 minutes that way and about 4 with two

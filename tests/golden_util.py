@@ -85,3 +85,28 @@ def assert_close_rel(got, ref, rtol=RTOL, what=""):
     bad = err > bound
     assert not bad.any(), "%s: %d/%d outside rtol=%g (worst err/bound %.3g)" % (
         what, int(bad.sum()), bad.size, rtol, float((err / bound).max()))
+
+
+REFERENCE_GOLDEN_DIR = os.path.join(GOLDEN_DIR, "reference")
+
+
+def reference_result(key, compute):
+    """What the reference's own code computes for one test case, stored under tests/golden/reference/<key>.npz.
+
+    `compute()` runs the reference (oracle/ref_harness.py, oracle/tf_eager_stub.py) and returns a dict of NumPy arrays and
+    JSON values.  It runs only to (re)write the stored result -- `RL4RS_WRITE_GOLDEN=1` with the reference tree present
+    (tests/golden/make_reference_golden.py) -- so the comparison itself needs nothing outside the repository."""
+    path = os.path.join(REFERENCE_GOLDEN_DIR, key + ".npz")
+    if os.environ.get("RL4RS_WRITE_GOLDEN"):
+        from oracle import ref_harness
+        assert ref_harness.reference_available(), "RL4RS_WRITE_GOLDEN needs the reference tree (RL4RS_REFERENCE_ROOT)"
+        out = compute()
+        arrays = {k: np.asarray(v) for k, v in out.items() if isinstance(v, np.ndarray)}
+        rest = {k: v for k, v in out.items() if not isinstance(v, np.ndarray)}
+        os.makedirs(REFERENCE_GOLDEN_DIR, exist_ok=True)
+        np.savez_compressed(path, __json__=np.frombuffer(json.dumps(rest).encode(), dtype=np.uint8), **arrays)
+    assert os.path.exists(path), "stored reference result missing: %s" % path
+    z = np.load(path)
+    out = json.loads(bytes(z["__json__"]).decode())
+    out.update({k: z[k] for k in z.files if k != "__json__"})
+    return out

@@ -66,11 +66,9 @@ def test_product_never_imports_oracle():
 
 
 def test_augru_kernel_choice_rule():
-    """r4_augru_kernel_for(ctas = 2 x row tiles, sms): 2 = k_augru_pair2 (a CTA pair per tile-sequence), 3 = k_augru_pp (a
-    CTA pair per tile, both sequences in flight) -- the cheaper by wave count x measured wave cost (defaults 13 : 24).
-    B200 (148 SMs): a 4096-row observation pass = 64 tile-sequences -> pair2 (one wave on 128 SMs beats one ping-pong wave
-    on 64); the 36 864-row reward pass = 576 and 8192-row passes = 128 -> ping-pong.  (1 was the round-1 one-CTA kernel,
-    deleted: it lost every regime.)"""
+    """r4_augru_kernel_for(ctas = 2 x row tiles, sms): the wave-count rule between two kernel shapes (2 = a CTA pair per
+    tile-sequence, 3 = a CTA pair per tile), kept in the ABI as host arithmetic.  No launch consults it: this build has one
+    AUGRU kernel (k_augru_tc), so this test holds the exported arithmetic and option validation only."""
     from rl4rs_b200 import _capi
     lib = _capi.load_library()
     f = lib.r4_augru_kernel_for

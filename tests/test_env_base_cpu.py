@@ -1,9 +1,10 @@
 """CPU: the gym layer (rl4rs_b200.env.base.RecEnvBase / build_spaces) over a fake simulator, held against the
-reference's OWN RecEnvBase (rl4rs/env/base.py:178-273, run through oracle/ref_harness.py) when /root/reference is
-present, and against the recorded expectations otherwise."""
+reference's OWN RecEnvBase (rl4rs/env/base.py:178-273, run through oracle/ref_harness.py; its record is stored under
+tests/golden/reference/) and against the recorded expectations."""
 import numpy as np
 import pytest
 
+from golden_util import reference_result
 from oracle import ref_harness
 from rl4rs_b200.env.base import RecEnvBase, build_spaces
 
@@ -119,11 +120,10 @@ def test_env_layer_matches_reference_env_layer(name, batch):
         assert [c[1] for c in ours["calls"] if c[0] == "step"] == [[7], [7]]        # a bare action is wrapped
     else:
         assert ours["user"] == [200, 201, 202] and ours["r1"][1] == [1.0, 2.0, 3.0]
-    if not ref_harness.reference_available():
-        pytest.skip("reference tree absent: recorded expectations only")
-    ref_base = ref_harness.install_stubs()[0]
-    ref = drive(ref_base.RecEnvBase, config)
-    assert ref == ours
+    # the reference's own RecEnvBase driven the same way; its record is stored (tests/golden/reference/), compared by repr
+    ref = reference_result("env_base_%s_%d" % (name, batch),
+                           lambda: {"repr": repr(drive(ref_harness.install_stubs()[0].RecEnvBase, config))})
+    assert repr(ours) == ref["repr"]
 
 
 def test_build_spaces_takes_the_widths_from_the_config():

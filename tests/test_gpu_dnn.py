@@ -1,6 +1,6 @@
 """GPU: the `dnn` simulator (config['algo'] = 'dnn'; rl4rs/env/slate.py:239-242 -> rl4rs/nets/dnn.py:8-45) through the
 same env API against the CPU oracle (oracle/dnn_np.py): the gather kernel k_cat_pool (bulk-TMA staged embedding rows),
-the dense tower and the two 256-wide FC layers on tcgen05, reward / violation / masks unchanged."""
+the dense tower and the two 256-wide FC layers on wgmma, reward / violation / masks unchanged."""
 import numpy as np
 import pytest
 

@@ -4,9 +4,9 @@
   zero biases, category_hash_size 100 000) on DISTINCT synthetic rows -- Slate, SeqSlate-27 and continuous-kNN at B=48;
 * full-size batches (4096 and 8192 rows per GPU, the BASELINE configs[1] / north-star per-GPU sizes): a 128-row oracle
   sample of the big env, rows compared by index;
-* every AUGRU kernel forced in turn (``r4_set_option('augru_kernel', ...)``): the simulator alone and env fixtures
-  through the pair kernel (one recurrence per CTA pair) and the ping-pong kernel (two per pair), every hand-over /
-  weight-ring variant of both, plus a launch big enough for the natural rule;
+* the AUGRU kernel under every historical kernel-choice option (``r4_set_option('augru_kernel' / 'augru_pair_impl', ...)``):
+  this build has one AUGRU kernel (k_augru_tc), the options are ABI no-ops, so these cases all run it -- the simulator
+  alone and env fixtures, plus a launch big enough for several waves;
 * the chunked sequence-cache build (> 8192 sequences) and the multi-wave persistent GEMM (tiles > SMs).
 
 Oracle = oracle/env_np.py + oracle/dien_np.py (f32), reference lines: rl4rs/nets/utils.py:117-125,
@@ -156,8 +156,8 @@ def test_dien_forward_each_augru_kernel(kernel, regime, augru_option):
 @pytest.mark.parametrize("impl", [2, 3, 4])
 @pytest.mark.parametrize("kernel", ["pair", "pp"])
 def test_dien_forward_each_pair_variant(kernel, impl, augru_option):
-    """The non-default hand-over / weight-ring variants of the pair kernels (r4_set_option('augru_pair_impl', 2..4):
-    tensor-map ring, relayed release.cluster hand-over, both) against the oracle; 300 rows = 3 tiles, a padding pair."""
+    """The simulator against the oracle with every value of the (no-op) 'augru_pair_impl' option set; 300 rows = 3 tiles
+    of 128 rows, 5 CTAs of 64 rows, a partial last CTA."""
     from oracle.dien_np import DienOracle
     from rl4rs_b200 import _capi
     cfg, cat, log, w = _default_regime(8, False)

@@ -3,13 +3,15 @@ scenarios -- env kind, episode length, mask mode, continuous / one-hot actions, 
 batch size, and per-step actions (logged, random, repeated, out-of-layer) are drawn from a seed; the reference is rolled
 through oracle/ref_harness.py exactly like the committed fixtures were, and everything it exposes per step must equal
 what the oracle computes (integers and feature rows bit-exact).  The ten committed fixtures pin ten hand-picked corners;
-this sweeps the product of the flags.  Skipped where /root/reference is absent (the GPU box)."""
+this sweeps the product of the flags.  What the reference computed is stored under tests/golden/reference/
+(golden_util.reference_result; tests/golden/make_reference_golden.py rewrites it), so these run on any machine."""
 import os
 import sys
 
 import numpy as np
 import pytest
 
+from golden_util import GOLDEN_DIR, reference_result
 from oracle import ref_harness
 from oracle.dnn_np import DnnOracle
 from oracle.env_np import OracleEnv
@@ -18,7 +20,7 @@ from rl4rs_b200.utils.datautil import FeatureUtil
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
 
-pytestmark = pytest.mark.skipif(not ref_harness.reference_available(), reason="reference tree absent")
+ITEM_FILE = os.path.join(GOLDEN_DIR, "item_info.csv")     # the reference's dataset/item_info.csv (data fixture)
 
 
 def draw_scenario(seed):
@@ -81,8 +83,9 @@ def test_oracle_env_equals_the_reference_env_on_a_random_scenario(seed):
     records = synth.render_records(log, cat)
     w = synth.make_dnn_weights(cfg, stress=2.0, bias_noise=0.2)
     np_seed = 77 + seed if train_mode else None
-    rec = make_golden.run_reference(dict(cfg), records, cat.to_text(), w, seq, action_source(cfg, aseed),
-                                    n_episodes=episodes, seed=np_seed, net=DnnOracle(w, np.float32))
+    rec = reference_result("random_scenario_%02d" % seed, lambda: make_golden.run_reference(
+        dict(cfg), records, cat.to_text(), w, seq, action_source(cfg, aseed), n_episodes=episodes, seed=np_seed,
+        net=DnnOracle(w, np.float32)))
     if np_seed is not None:
         np.random.seed(np_seed)
     env = OracleEnv(dict(cfg), FeatureUtil.parse_log(records, 64), cat, DnnOracle(w, np.float32), seq=seq)
@@ -110,10 +113,10 @@ def test_ingest_equals_the_reference_preprocessing_on_random_sessions(seed, tmp_
     the GLOBAL numpy RNG, `slate2trajectory` joins 4-page sessions and drops the last one."""
     import runpy
     from rl4rs_b200.utils import ingest
-    ref_harness.install_stubs()
-    script = os.path.join(ref_harness.REFERENCE_ROOT, "script", "data_preprocess.py")
 
     def run_stage(stage, lines):
+        ref_harness.install_stubs()
+        script = os.path.join(ref_harness.REFERENCE_ROOT, "script", "data_preprocess.py")
         src, dst = str(tmp_path / "in.csv"), str(tmp_path / ("out_%s.csv" % stage))
         open(src, "w").write("\n".join(lines))
         argv, sys.argv = sys.argv, [script, src, dst, stage]
@@ -135,13 +138,18 @@ def test_ingest_equals_the_reference_preprocessing_on_random_sessions(seed, tmp_
             f = recs[4 * s + p].split("@")
             ragged.append("@".join([str(1000 * s + p), base[1], str(p + 1), f[3], f[4], base[5], base[6], f[7], base[8]]))
     ragged.append("")
-    np.random.seed(40 + seed)
-    want_aug = run_stage("data_augment", ragged)
+
+    def reference():
+        np.random.seed(40 + seed)
+        aug = run_stage("data_augment", ragged)
+        full_ = [header] + aug[1:] + [""] if aug[0] == header else [header] + aug + [""]
+        return {"aug": aug, "traj": run_stage("slate2trajectory", full_)}
+    want = reference_result("ingest_%d" % seed, reference)
+    want_aug, want_traj = want["aug"], want["traj"]
     np.random.seed(40 + seed)
     got_aug = ingest.data_augment(ragged)
     assert got_aug == want_aug
     full = [header] + want_aug[1:] + [""] if want_aug[0] == header else [header] + want_aug + [""]
-    want_traj = run_stage("slate2trajectory", full)
     assert ingest.slate2trajectory(full) == want_traj
     assert 1 <= len(want_traj) < n_sess                      # the script drops the last session (and any it merges)
 
@@ -151,8 +159,6 @@ def test_trainer_defaults_are_the_reference_scripts_hyper_parameters():
     the script's own source with `ast`, against the defaults rl4rs_b200/trainer.py trains with."""
     import ast
     from rl4rs_b200 import trainer
-    src = open(os.path.join(ref_harness.REFERENCE_ROOT, "script", "modelfree_train.py")).read()
-    tree = ast.parse(src)
 
     def literal(node):
         """A dict literal with non-literal values (config[...] expressions) left out."""
@@ -166,13 +172,21 @@ def test_trainer_defaults_are_the_reference_scripts_hyper_parameters():
                 pass
         return out
 
-    branches = {}
-    for node in ast.walk(tree):
-        if isinstance(node, ast.If) and isinstance(node.test, ast.Compare) and isinstance(node.test.left, ast.Constant) \
-                and node.test.left.value in ("PPO", "A2C"):
-            first = node.body[0]
-            assert isinstance(first, ast.Assign) and first.targets[0].id == "cfg"
-            branches[node.test.left.value] = literal(first.value)
+    def reference():
+        src = open(os.path.join(ref_harness.REFERENCE_ROOT, "script", "modelfree_train.py")).read()
+        tree = ast.parse(src)
+        branches = {}
+        for node in ast.walk(tree):
+            if isinstance(node, ast.If) and isinstance(node.test, ast.Compare) and isinstance(node.test.left, ast.Constant) \
+                    and node.test.left.value in ("PPO", "A2C"):
+                first = node.body[0]
+                assert isinstance(first, ast.Assign) and first.targets[0].id == "cfg"
+                branches[node.test.left.value] = literal(first.value)
+        common = [literal(n) for n in ast.walk(tree) if isinstance(n, ast.Dict)]
+        return {"branches": branches, "common": [d for d in common if d.get("batch_mode") == "complete_episodes"],
+                "softq": '"type": "SoftQ"' in src}
+    stored = reference_result("modelfree_train_configs", reference)
+    branches, common = stored["branches"], stored["common"]
     assert set(branches) == {"PPO", "A2C"}
     for algo, ours in (("PPO", trainer.PPO_DEFAULTS), ("A2C", trainer.A2C_DEFAULTS)):
         ref = branches[algo]
@@ -182,11 +196,9 @@ def test_trainer_defaults_are_the_reference_scripts_hyper_parameters():
             assert ours[k] == ref[k], (algo, k, ours[k], ref[k])
     assert trainer.PPO_DEFAULTS["grad_clip"] is None and "grad_clip" not in branches["PPO"]       # commented out there
     # the dict every algorithm is merged into: gamma 1, SoftQ exploration, complete episodes
-    common = [literal(n) for n in ast.walk(tree) if isinstance(n, ast.Dict)]
-    common = [d for d in common if d.get("batch_mode") == "complete_episodes"]
     assert len(common) == 1 and common[0]["gamma"] == 1 and common[0]["explore"] is True
     assert trainer.PPO_DEFAULTS["gamma"] == trainer.A2C_DEFAULTS["gamma"] == 1.0
-    assert '"type": "SoftQ"' in src
+    assert stored["softq"]
 
 
 def test_static_helpers_on_the_real_catalog_and_random_knn_queries():
@@ -194,50 +206,76 @@ def test_static_helpers_on_the_real_catalog_and_random_knn_queries():
     reference's own dataset/item_info.csv, and the two nearest-neighbour statics on random queries (incl. ties and
     fully masked rows), reference class against mirror class."""
     from rl4rs_b200.env.slate import SlateState
-    ref_slate = ref_harness.install_stubs()[1]
-    item_file = os.path.join(ref_harness.REFERENCE_ROOT, "dataset", "item_info.csv")
-    info_r, emb_r = ref_slate.SlateState.get_iteminfo_from_file(item_file, 284)
-    info_o, emb_o = SlateState.get_iteminfo_from_file(item_file, 284)
-    np.testing.assert_array_equal(emb_o, emb_r)
-    assert set(info_o) == set(info_r)
-    for k in info_r:
-        assert info_o[k]["price"] == info_r[k]["price"] and info_o[k]["location"] == info_r[k]["location"], k
-        np.testing.assert_array_equal(np.asarray(info_o[k]["item_vec"], float), np.asarray(info_r[k]["item_vec"], float))
-    loc_r, sp_r = ref_slate.SlateState.get_mask_from_file(item_file, 284)
-    loc_o, sp_o = SlateState.get_mask_from_file(item_file, 284)
-    np.testing.assert_array_equal(loc_o, loc_r)
-    assert list(sp_o) == list(sp_r) and len(sp_r) > 0
-    rs = np.random.RandomState(4)
-    for trial in range(20):
-        q = rs.uniform(-1, 1, (16, 32))
-        q[0] = 0.0                                            # every score ties at 0: lowest index wins
-        q[1] = emb_r[1 + trial]                               # an item's own embedding
-        mask = (rs.rand(16, 284) < 0.3).astype(np.int64)
-        mask[2] = 0                                           # nothing allowed: all scores -2**31, index 0
-        np.testing.assert_array_equal(SlateState.get_nearest_neighbor(q, emb_o),
-                                      ref_slate.SlateState.get_nearest_neighbor(q, emb_r))
-        np.testing.assert_array_equal(SlateState.get_nearest_neighbor_with_mask(q, emb_o, mask),
-                                      ref_slate.SlateState.get_nearest_neighbor_with_mask(q, emb_r, mask))
+
+    def queries(emb):
+        rs = np.random.RandomState(4)
+        for trial in range(20):
+            q = rs.uniform(-1, 1, (16, 32))
+            q[0] = 0.0                                        # every score ties at 0: lowest index wins
+            q[1] = emb[1 + trial]                             # an item's own embedding
+            mask = (rs.rand(16, 284) < 0.3).astype(np.int64)
+            mask[2] = 0                                       # nothing allowed: all scores -2**31, index 0
+            yield q, mask
+
+    def reference():
+        ref_slate = ref_harness.install_stubs()[1]
+        item_file = os.path.join(ref_harness.REFERENCE_ROOT, "dataset", "item_info.csv")
+        info, emb = ref_slate.SlateState.get_iteminfo_from_file(item_file, 284)
+        loc, sp = ref_slate.SlateState.get_mask_from_file(item_file, 284)
+        keys = sorted(info, key=int)
+        nn = [(ref_slate.SlateState.get_nearest_neighbor(q, emb), ref_slate.SlateState.get_nearest_neighbor_with_mask(q, emb, m))
+              for q, m in queries(emb)]
+        return {"keys": [int(k) for k in keys], "price": np.array([info[k]["price"] for k in keys], np.float64),
+                "location": np.array([info[k]["location"] for k in keys], np.int64),
+                "item_vec": np.array([np.asarray(info[k]["item_vec"], float) for k in keys]), "emb": np.asarray(emb),
+                "loc": np.asarray(loc), "special": [int(x) for x in sp],
+                "nn": np.array([a for a, _ in nn]), "nn_mask": np.array([b for _, b in nn])}
+    ref = reference_result("static_helpers", reference)
+    info_o, emb_o = SlateState.get_iteminfo_from_file(ITEM_FILE, 284)
+    np.testing.assert_array_equal(emb_o, ref["emb"])
+    assert sorted(int(k) for k in info_o) == ref["keys"]
+    for i, k in enumerate(sorted(info_o, key=int)):
+        assert info_o[k]["price"] == ref["price"][i] and info_o[k]["location"] == ref["location"][i], k
+        np.testing.assert_array_equal(np.asarray(info_o[k]["item_vec"], float), ref["item_vec"][i])
+    loc_o, sp_o = SlateState.get_mask_from_file(ITEM_FILE, 284)
+    np.testing.assert_array_equal(loc_o, ref["loc"])
+    assert [int(x) for x in sp_o] == ref["special"] and len(ref["special"]) > 0
+    for trial, (q, mask) in enumerate(queries(emb_o)):
+        np.testing.assert_array_equal(SlateState.get_nearest_neighbor(q, emb_o), ref["nn"][trial])
+        np.testing.assert_array_equal(SlateState.get_nearest_neighbor_with_mask(q, emb_o, mask), ref["nn_mask"][trial])
 
 
 def test_feature_extraction_mirror_on_random_ragged_rows():
     """datautil.py:34-69: FeatureUtil.feature_extraction, reference method against the host mirror, on raw state rows
     with empty / short / over-long sequences, short and over-long dense and category lists."""
     from rl4rs_b200.utils.datautil import FeatureUtil
-    ref_datautil = ref_harness.install_stubs()[3]
     cfg = {"maxlen": 64, "batch_size": 5, "class_num": 2, "dense_feature_num": 432, "category_feature_num": 21,
            "category_hash_size": 100000, "seq_num": 2}
-    ours, ref = FeatureUtil(cfg), ref_datautil.FeatureUtil(cfg)
-    rs = np.random.RandomState(8)
-    for trial in range(12):
-        rows = []
-        for i in range(5):
-            seqs = [list(rs.randint(1, 284, rs.choice([0, 1, 7, 64, 65, 130]))) for _ in range(2)]
-            dense = list(rs.normal(0, 1, rs.choice([32, 72, 432, 440])).astype(np.float64))
-            cat = list(rs.randint(0, 100000, rs.choice([10, 12, 21, 25])).astype(np.float64))       # floats in the reference too
-            rows.append([0, seqs, dense, cat, [0] * 9, int(rs.randint(2))])
+
+    def trials():
+        rs = np.random.RandomState(8)
+        for trial in range(12):
+            rows = []
+            for i in range(5):
+                seqs = [list(rs.randint(1, 284, rs.choice([0, 1, 7, 64, 65, 130]))) for _ in range(2)]
+                dense = list(rs.normal(0, 1, rs.choice([32, 72, 432, 440])).astype(np.float64))
+                cat = list(rs.randint(0, 100000, rs.choice([10, 12, 21, 25])).astype(np.float64))       # floats in the reference too
+                rows.append([0, seqs, dense, cat, [0] * 9, int(rs.randint(2))])
+            yield rows
+
+    def reference():
+        ref = ref_harness.install_stubs()[3].FeatureUtil(cfg)
+        out = {}
+        for trial, rows in enumerate(trials()):
+            (s2, d2, c2, l2), y2 = ref.feature_extraction(rows)
+            out.update({"s%d" % trial: s2, "d%d" % trial: d2, "c%d" % trial: c2, "l%d" % trial: np.asarray(l2),
+                        "y%d" % trial: np.asarray(y2)})
+        return out
+    ref = reference_result("feature_extraction", reference)
+    ours = FeatureUtil(cfg)
+    for trial, rows in enumerate(trials()):
         (s1, d1, c1, l1), y1 = ours.feature_extraction(rows)
-        (s2, d2, c2, l2), y2 = ref.feature_extraction(rows)
-        np.testing.assert_array_equal(s1, s2); np.testing.assert_array_equal(d1, d2); np.testing.assert_array_equal(c1, c2)
-        np.testing.assert_array_equal(l1, l2)
-        assert y1 == y2 and d1.dtype == d2.dtype and c1.dtype == c2.dtype and s1.shape == (5, 2, 64)
+        np.testing.assert_array_equal(s1, ref["s%d" % trial]); np.testing.assert_array_equal(d1, ref["d%d" % trial])
+        np.testing.assert_array_equal(c1, ref["c%d" % trial]); np.testing.assert_array_equal(l1, ref["l%d" % trial])
+        np.testing.assert_array_equal(np.asarray(y1), ref["y%d" % trial])
+        assert d1.dtype == ref["d%d" % trial].dtype and c1.dtype == ref["c%d" % trial].dtype and s1.shape == (5, 2, 64)

@@ -142,9 +142,7 @@ def test_the_references_own_stack_reproduces_the_fixtures(name):
 def test_the_references_own_stack_with_the_other_simulators(algo, seq):
     """config['algo'] dispatch (slate.py:239-242) through the reference's own constructors for the other three graphs of
     rl4rs/nets/: a short logged-policy episode of the self-constructed reference env against the oracle env the GPU tests
-    use for that simulator (tests/test_gpu_dnn.py)."""
-    if not ref_harness.reference_available():
-        pytest.skip("reference tree absent")
+    use for that simulator (tests/test_gpu_dnn.py).  The reference's episode is stored under tests/golden/reference/."""
     sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
     import make_golden
     from oracle.env_np import OracleEnv
@@ -157,7 +155,9 @@ def test_the_references_own_stack_with_the_other_simulators(algo, seq):
     records = synth.render_records(log, cat)
     maker = {"dnn": synth.make_dnn_weights, "widedeep": synth.make_widedeep_weights, "lstm": synth.make_lstm_weights}[algo]
     w = maker(cfg, stress=2.0, bias_noise=0.2)
-    rec = make_golden.run_reference(cfg, records, cat.to_text(), w, seq, lambda env, ep, t, off: off, full_stack=True)
+    from golden_util import reference_result
+    rec = reference_result("other_simulator_%s" % algo, lambda: make_golden.run_reference(
+        cfg, records, cat.to_text(), w, seq, lambda env, ep, t, off: off, full_stack=True))
     from rl4rs_b200.utils.datautil import FeatureUtil
     ora = OracleEnv(cfg, FeatureUtil.parse_log(records, 64), cat, ORACLES[algo](w, np.float32), seq=seq)
     obs = ora.reset()
@@ -175,10 +175,10 @@ def test_the_references_own_stack_with_the_other_simulators(algo, seq):
 def test_rllib_policy_models_of_the_reference_against_the_torch_twins():
     """a22 / n4: rl4rs/nets/rllib/rllib_rawstate_model.py's TFModelWithRawState (its own Keras graph over nets/utils.py)
     and rllib_mask_model.py's MyMaskActionsModel.forward (the action masking), run from the reference tree over the
-    stand-ins, against rl4rs_b200/policy.py -- the twins the kernels k_policy_act / k_policy_grad are themselves held to."""
-    if not ref_harness.reference_available():
-        pytest.skip("reference tree absent")
+    stand-ins, against rl4rs_b200/policy.py -- the twins the kernels k_policy_act / k_policy_grad are themselves held to.
+    What the reference computes is stored under tests/golden/reference/."""
     import torch
+    from golden_util import reference_result
     from oracle import tf_eager_stub as stub
     from rl4rs_b200.policy import MaskedPolicy, RawStatePolicy
     cfg = {"category_hash_size": 600, "emb_size": 128, "hidden_units": 128, "category_feature_num": 21,
@@ -196,26 +196,32 @@ def test_rllib_policy_models_of_the_reference_against_the_torch_twins():
           "dense_1/bias": p["db2"], "embedding_1/embeddings": p["emb_seq"], "dense_2/kernel": p["wc"], "dense_2/bias": p["bc"],
           "fc_out/kernel": p["w2"], "fc_out/bias": p["b2"], "value_out/kernel": p["wv"], "value_out/bias": p["bv"]}
     cat, dense, seq = rs.randint(0, 600, (R, 21)), rs.normal(0, 2, (R, 432)).astype(np.float32), rs.randint(0, 284, (R, 2, 64))
-    out = stub.run_reference_rawstate_model(cfg, ck, cat.astype(np.float32), dense, seq.astype(np.float32), A)
-    scopes = [v[0] for v in out["variables"]]
-    assert not out["unused"]
-    assert [s_ for i, s_ in enumerate(scopes) if i == 0 or s_ != scopes[i - 1]] == \
-        ["embedding", "dense", "dense_1", "embedding_1", "dense_2", "fc_out", "value_out"]       # Keras creation order
     obs = pol.pack({"category_feature": torch.as_tensor(cat), "dense_feature": torch.as_tensor(dense), "sequence_feature": torch.as_tensor(seq)})
     with torch.no_grad():
         logits, value = pol.forward(obs, torch.ones(R, A))
         masked, _ = pol.forward(obs, torch.as_tensor(mask))
-    np.testing.assert_allclose(out["logits"], logits.numpy(), rtol=0, atol=2e-5)
-    np.testing.assert_allclose(out["value"], value.numpy(), rtol=0, atol=2e-5)
-    # the masking itself, by the reference's forward(): fed the twin's unmasked logits as the action_embed_model output
-    got = stub.run_reference_mask_forward(lambda o: logits.numpy(), obs.numpy(), mask, A)
-    np.testing.assert_array_equal(got, masked.numpy())
     # and for the 256-d observation policy of the benchmark configs
     mp = MaskedPolicy(A, "cpu", seed=5)
     o256 = torch.as_tensor(rs.normal(0, 1, (R, 256)).astype(np.float32))
     with torch.no_grad():
         raw, _ = mp.forward(o256, torch.ones(R, A))
         want, _ = mp.forward(o256, torch.as_tensor(mask))
-    got = stub.run_reference_mask_forward(lambda o: raw.numpy(), o256.numpy(), mask, A)
+
+    def reference():
+        out = stub.run_reference_rawstate_model(cfg, ck, cat.astype(np.float32), dense, seq.astype(np.float32), A)
+        # the masking itself, by the reference's forward(): fed the twins' unmasked logits as the action_embed_model output
+        return {"logits": np.asarray(out["logits"]), "value": np.asarray(out["value"]),
+                "scopes": [v[0] for v in out["variables"]], "unused": list(out["unused"]),
+                "masked": np.asarray(stub.run_reference_mask_forward(lambda o: logits.numpy(), obs.numpy(), mask, A)),
+                "masked256": np.asarray(stub.run_reference_mask_forward(lambda o: raw.numpy(), o256.numpy(), mask, A))}
+    out = reference_result("rllib_policy_models", reference)
+    scopes = out["scopes"]
+    assert not out["unused"]
+    assert [s_ for i, s_ in enumerate(scopes) if i == 0 or s_ != scopes[i - 1]] == \
+        ["embedding", "dense", "dense_1", "embedding_1", "dense_2", "fc_out", "value_out"]       # Keras creation order
+    np.testing.assert_allclose(out["logits"], logits.numpy(), rtol=0, atol=2e-5)
+    np.testing.assert_allclose(out["value"], value.numpy(), rtol=0, atol=2e-5)
+    np.testing.assert_array_equal(out["masked"], masked.numpy())
+    got = out["masked256"]
     np.testing.assert_array_equal(got, want.numpy())
     assert (got[mask == 0] < -1e38).all()
