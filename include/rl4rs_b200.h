@@ -256,6 +256,51 @@ int r4_policy_grad_partial(int mode, const float* params, const float* obs, cons
                            void* stream);
 int r4_grad_exchange(r4_comm* comm, const float* scratch, int G, int action_size, float* flat_grad, float* stats_accum,
                      float stat_scale, void* stream);
+/* r4_grad_exchange for a flat gradient of any length (the communicator's n_params): partial = f32 [G][n_params] followed by
+ * the statistics f32 [G][5]; flat_grad = the sum over the ranks, stats_accum += this rank's statistics * stat_scale. */
+int r4_grad_exchange_n(r4_comm* comm, const float* partial, int G, int n_params, float* flat_grad, float* stats_accum,
+                       float stat_scale, void* stream);
+
+/* ---- Gaussian policy + learner of the continuous-action env (PPO_conti / A2C_conti, modelfree_train.py:46-48,218-247,
+ * 270-290): RLlib's default FullyConnectedNetwork (fcnet_hiddens [256,256], tanh, vf_share_layers off) over obs f32[n,256],
+ * a DiagGaussian over action_dim = D (even, 2..64) dimensions.  Flat parameter layout (r4_gauss_num_params(D) floats):
+ * fc_1 w[256,256] b[256] | fc_2 w[256,256] b[256] | fc_out w[256,2D] b[2D] (mean | log_std) |
+ * fc_value_1 w[256,256] b[256] | fc_value_2 w[256,256] b[256] | value_out w[256] b[1].  Stateless, caller-owned DEVICE memory. */
+int r4_gauss_num_params(int action_dim);
+/* floats of the scratch that r4_gauss_grad / r4_gauss_ppo_epoch* need (any n: samples are processed in chunks); -1 for a
+ * bad action_dim */
+int64_t r4_gauss_scratch_size(int action_dim);
+/* forward + StochasticSampling (explore != 0: a = mean + exp(log_std) * N(0,1), counter-based noise keyed by seed, counter +
+ * row and dimension) or the mean (RLlib explore=False; modelfree_train.py:412-414) -> action f32[n,D] (unclipped: what the
+ * sample batch stores and logp is taken on), env_action f32[n,D] = clip(action, -1, 1) (clip_actions), logp f32[n], value
+ * f32[n], dist_inputs f32[n,2D] (mean | log_std; may be NULL). */
+int r4_gauss_act(const float* params, const float* obs, int n, int action_dim, int explore, uint64_t seed, uint64_t counter,
+                 float* action, float* env_action, float* logp, float* value, float* dist_inputs, void* stream);
+/* Gradient of the RLlib loss over samples idx[0..n) (NULL = 0..n-1) of a rollout, as r4_policy_grad but deterministic without
+ * per-CTA partials (one CTA owns each tile of every weight gradient): mode 0 PPO surrogate over the DiagGaussian (mean; needs
+ * old_logp, old_dist = the stored dist inputs f32[n,2D], old_value), mode 1 A2C (sums; old_* may be NULL).  flat_grad
+ * f32[num_params] receives the gradient; stats_accum f32[5] (may be NULL) += {policy_loss, vf_loss, kl, entropy, total} *
+ * stat_scale.  scratch: r4_gauss_scratch_size(D) floats. */
+int r4_gauss_grad(int mode, const float* params, const float* obs, const float* action, const float* old_logp,
+                  const float* old_dist, const float* old_value, const float* adv, const float* target, const int64_t* idx,
+                  int n, int action_dim, float clip, float vf_clip, float vf_coeff, float kl_coeff, float ent_coeff,
+                  float inv_n, float* scratch, float* flat_grad, float* stats_accum, float stat_scale, void* stream);
+/* One PPO SGD epoch of the Gaussian policy on a single GPU, as r4_ppo_epoch: per full minibatch perm[s .. s+mb),
+ * r4_gauss_grad (mode 0, mean over mb) then r4_adam_step (grad_clip <= 0: off).  Returns the steps done or a negative
+ * r4_status. */
+int r4_gauss_ppo_epoch(float* params, const float* obs, const float* action, const float* old_logp, const float* old_dist,
+                       const float* old_value, const float* adv, const float* target, const int64_t* perm, int n, int mb,
+                       int action_dim, float clip, float vf_clip, float vf_coeff, float kl_coeff, float ent_coeff,
+                       float* scratch, float* flat_grad, float* stats_accum, float* m, float* v, int step0, float lr,
+                       float beta1, float beta2, float eps, float grad_clip, float* norm_scratch, void* stream);
+/* The data-parallel epoch of the Gaussian policy, as r4_ppo_epoch_dist (mb = minibatch PER RANK, loss = mean over
+ * mb x world samples): per minibatch the gradient launches and ONE exchange + Adam kernel over peer memory.  The
+ * communicator must have been created with r4_gauss_num_params(action_dim). */
+int r4_gauss_ppo_epoch_dist(r4_comm* comm, float* params, const float* obs, const float* action, const float* old_logp,
+                            const float* old_dist, const float* old_value, const float* adv, const float* target,
+                            const int64_t* perm, int n, int mb, int action_dim, float clip, float vf_clip, float vf_coeff,
+                            float kl_coeff, float ent_coeff, float* scratch, float* flat_grad, float* stats_accum, float* m,
+                            float* v, int step0, float lr, float beta1, float beta2, float eps, void* stream);
 
 /* ---- the simulator alone (nets/dien.py:8-45), for parity tests and kernel benchmarks ------- */
 /* seq i32[R,2,64], dense f32[R,432], cat i32[R,21] (device) -> obs f32[R,256], probs f32[R,2]

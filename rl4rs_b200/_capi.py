@@ -72,6 +72,16 @@ EXPORTS = {
     "r4_policy_grad_partial": (C.c_int, [C.c_int] + [C.c_void_p] * 10 + [C.c_int, C.c_int] + [C.c_float] * 6 +
                                [C.c_void_p, C.c_int, C.c_void_p]),
     "r4_grad_exchange": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]),
+    "r4_grad_exchange_n": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]),
+    "r4_gauss_num_params": (C.c_int, [C.c_int]),
+    "r4_gauss_scratch_size": (C.c_int64, [C.c_int]),
+    "r4_gauss_act": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_uint64] + [C.c_void_p] * 6),
+    "r4_gauss_grad": (C.c_int, [C.c_int] + [C.c_void_p] * 9 + [C.c_int, C.c_int] + [C.c_float] * 6 +
+                      [C.c_void_p] * 3 + [C.c_float, C.c_void_p]),
+    "r4_gauss_ppo_epoch": (C.c_int, [C.c_void_p] * 9 + [C.c_int] * 3 + [C.c_float] * 5 + [C.c_void_p] * 5 + [C.c_int] +
+                           [C.c_float] * 5 + [C.c_void_p, C.c_void_p]),
+    "r4_gauss_ppo_epoch_dist": (C.c_int, [C.c_void_p] * 10 + [C.c_int] * 3 + [C.c_float] * 5 + [C.c_void_p] * 5 + [C.c_int] +
+                                [C.c_float] * 4 + [C.c_void_p]),
     "r4_adam_step": (C.c_int, [C.c_void_p] * 4 + [C.c_int, C.c_int] + [C.c_float] * 6 + [C.c_void_p, C.c_void_p]),
     "r4_dien_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
 }

@@ -8,6 +8,7 @@
 #include "r4_recur.cuh"
 #include "r4_ppo.cuh"
 #include "r4_comm.cuh"
+#include "r4_gauss.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -1411,6 +1412,127 @@ int r4_ppo_epoch_dist(r4_comm* c, float* params, const float* obs, const uint8_t
     // statistics stay per-rank means over this rank's mb samples (the trainer averages them over the ranks)
     rc = exchange_launch(c, scratch, G, np, flat_grad, stats_accum, 1.0f / (float)mb, 1, params, m, v, step0 + steps + 1, lr, beta1, beta2,
                          eps, stream);
+    if (rc) return rc;
+  }
+  return steps;
+}
+
+int r4_grad_exchange_n(r4_comm* c, const float* partial, int G, int n_params, float* flat_grad, float* stats_accum,
+                       float stat_scale, void* stream) {
+  if (!c || !partial || !flat_grad || G < 1 || n_params < 1) return fail(nullptr, R4_ERR_ARG, "r4_grad_exchange_n: bad argument");
+  return exchange_launch(c, partial, G, n_params, flat_grad, stats_accum, stat_scale, 0, nullptr, nullptr, nullptr, 0, 0.f, 0.f, 0.f,
+                         0.f, stream);
+}
+
+// ---- Gaussian policy of the continuous-action env (r4_gauss.cuh) -------------------------------------------
+int r4_gauss_num_params(int action_dim) { return r4gauss::make_layout(action_dim).n; }
+
+int64_t r4_gauss_scratch_size(int action_dim) {
+  return (action_dim < 2 || action_dim > r4gauss::MAXD || action_dim % 2) ? -1 : (int64_t)r4gauss::scratch_floats(action_dim);
+}
+
+static bool gauss_dim_ok(int D) { return D >= 2 && D <= r4gauss::MAXD && D % 2 == 0; }
+
+int r4_gauss_act(const float* params, const float* obs, int n, int action_dim, int explore, uint64_t seed, uint64_t counter,
+                 float* action, float* env_action, float* logp, float* value, float* dist_inputs, void* stream) {
+  if (!params || !obs || !action || !env_action || !logp || !value || n < 1 || !gauss_dim_ok(action_dim))
+    return fail(nullptr, R4_ERR_ARG, "r4_gauss_act: bad argument (action_dim even, 2..64)");
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t st = cudaFuncSetAttribute(r4gauss::k_gauss_act, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)r4gauss::ACT_SMEM);
+    if (st != cudaSuccess) return fail(nullptr, R4_ERR_CUDA, std::string("cudaFuncSetAttribute(k_gauss_act): ") + cudaGetErrorString(st));
+    attr = true;
+  }
+  r4gauss::k_gauss_act<<<(n + r4gauss::TS - 1) / r4gauss::TS, r4gauss::NT, r4gauss::ACT_SMEM, S(stream)>>>(
+      r4gauss::make_layout(action_dim), params, obs, n, explore, seed, counter, action, env_action, logp, value, dist_inputs);
+  R4_PCHECK("k_gauss_act");
+  return R4_OK;
+}
+
+// grad_out[np] = the gradient over samples idx[0..n) (chunks of CH, accumulated in order); stat_sum[5] = the raw statistic
+// sums; stats_accum (may be NULL) += stat_sum * stat_scale.
+static int gauss_grad_impl(int mode, const float* params, const float* obs, const float* action, const float* old_logp,
+                           const float* old_dist, const float* old_value, const float* adv, const float* target,
+                           const int64_t* idx, int n, int D, float clip, float vf_clip, float vf_coeff, float kl_coeff,
+                           float ent_coeff, float inv_n, float* scratch, float* grad_out, float* stat_sum, float* stats_accum,
+                           float stat_scale, void* stream) {
+  if (!params || !obs || !action || !adv || !target || !scratch || !grad_out || n < 1 || !gauss_dim_ok(D) ||
+      (mode == 0 && (!old_logp || !old_value || !old_dist)) || (mode != 0 && mode != 1))
+    return fail(nullptr, R4_ERR_ARG, "r4_gauss_grad: bad argument");
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t st = cudaFuncSetAttribute(r4gauss::k_gauss_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)r4gauss::ROWS_SMEM);
+    if (st != cudaSuccess) return fail(nullptr, R4_ERR_CUDA, std::string("cudaFuncSetAttribute(k_gauss_rows): ") + cudaGetErrorString(st));
+    attr = true;
+  }
+  const r4gauss::Layout L = r4gauss::make_layout(D);
+  const r4gauss::Hyper hp{mode, clip, vf_clip, vf_coeff, kl_coeff, ent_coeff, inv_n};
+  const r4gauss::Planes P = r4gauss::make_planes(scratch, D);
+  const r4gauss::Jobs J = r4gauss::make_jobs(L, P);
+  for (int c0 = 0; c0 < n; c0 += r4gauss::CH) {
+    const int cn = std::min(r4gauss::CH, n - c0);
+    const bool last = c0 + cn >= n;
+    r4gauss::k_gauss_rows<<<(cn + r4gauss::TS - 1) / r4gauss::TS, r4gauss::NT, r4gauss::ROWS_SMEM, S(stream)>>>(
+        L, hp, params, obs, action, old_logp, old_dist, old_value, adv, target, idx, c0, cn, P);
+    R4_PCHECK("k_gauss_rows");
+    r4gauss::k_gauss_wgrad<<<J.ntiles + 1, r4gauss::NT, 0, S(stream)>>>(J, cn, c0 == 0, grad_out, P.stats, stat_sum,
+                                                                        last ? stats_accum : nullptr, stat_scale);
+    R4_PCHECK("k_gauss_wgrad");
+  }
+  return R4_OK;
+}
+
+static float* gauss_gsum(float* scratch, int D) {           // [np] gradient + [5] statistics, then [5] raw statistics
+  return scratch + (size_t)r4gauss::CH * (r4gauss::NPLANE * r4gauss::H + 2 * D + 1 + 5);
+}
+
+int r4_gauss_grad(int mode, const float* params, const float* obs, const float* action, const float* old_logp,
+                  const float* old_dist, const float* old_value, const float* adv, const float* target, const int64_t* idx,
+                  int n, int action_dim, float clip, float vf_clip, float vf_coeff, float kl_coeff, float ent_coeff,
+                  float inv_n, float* scratch, float* flat_grad, float* stats_accum, float stat_scale, void* stream) {
+  if (!scratch || !gauss_dim_ok(action_dim)) return fail(nullptr, R4_ERR_ARG, "r4_gauss_grad: bad argument");
+  float* raw = gauss_gsum(scratch, action_dim) + r4gauss::make_layout(action_dim).n + 5;
+  return gauss_grad_impl(mode, params, obs, action, old_logp, old_dist, old_value, adv, target, idx, n, action_dim, clip, vf_clip,
+                         vf_coeff, kl_coeff, ent_coeff, inv_n, scratch, flat_grad, raw, stats_accum, stat_scale, stream);
+}
+
+int r4_gauss_ppo_epoch(float* params, const float* obs, const float* action, const float* old_logp, const float* old_dist,
+                       const float* old_value, const float* adv, const float* target, const int64_t* perm, int n, int mb,
+                       int action_dim, float clip, float vf_clip, float vf_coeff, float kl_coeff, float ent_coeff,
+                       float* scratch, float* flat_grad, float* stats_accum, float* m, float* v, int step0, float lr,
+                       float beta1, float beta2, float eps, float grad_clip, float* norm_scratch, void* stream) {
+  if (!perm || !params || !m || !v || !flat_grad || !scratch || n < 1 || mb < 1 || mb > n || step0 < 0 || !gauss_dim_ok(action_dim))
+    return fail(nullptr, R4_ERR_ARG, "r4_gauss_ppo_epoch: bad argument");
+  const int np = r4gauss::make_layout(action_dim).n;
+  int steps = 0;
+  for (int s = 0; s + mb <= n; s += mb, ++steps) {
+    int rc = r4_gauss_grad(0, params, obs, action, old_logp, old_dist, old_value, adv, target, perm + s, mb, action_dim, clip, vf_clip,
+                           vf_coeff, kl_coeff, ent_coeff, 1.0f / mb, scratch, flat_grad, stats_accum, 1.0f / mb, stream);
+    if (rc) return rc;
+    rc = r4_adam_step(params, flat_grad, m, v, np, step0 + steps + 1, lr, beta1, beta2, eps, 1.0f, grad_clip, norm_scratch, stream);
+    if (rc) return rc;
+  }
+  return steps;
+}
+
+int r4_gauss_ppo_epoch_dist(r4_comm* c, float* params, const float* obs, const float* action, const float* old_logp,
+                            const float* old_dist, const float* old_value, const float* adv, const float* target,
+                            const int64_t* perm, int n, int mb, int action_dim, float clip, float vf_clip, float vf_coeff,
+                            float kl_coeff, float ent_coeff, float* scratch, float* flat_grad, float* stats_accum, float* m,
+                            float* v, int step0, float lr, float beta1, float beta2, float eps, void* stream) {
+  if (!c || !params || !perm || !m || !v || !scratch || n < 1 || mb < 1 || mb > n || step0 < 0 || !gauss_dim_ok(action_dim))
+    return fail(nullptr, R4_ERR_ARG, "r4_gauss_ppo_epoch_dist: bad argument");
+  const int np = r4gauss::make_layout(action_dim).n;
+  const float inv = 1.0f / ((float)mb * (float)c->world);
+  float* gsum = gauss_gsum(scratch, action_dim);
+  int steps = 0;
+  for (int s = 0; s + mb <= n; s += mb, ++steps) {
+    int rc = gauss_grad_impl(0, params, obs, action, old_logp, old_dist, old_value, adv, target, perm + s, mb, action_dim, clip,
+                             vf_clip, vf_coeff, kl_coeff, ent_coeff, inv, scratch, gsum, gsum + np, nullptr, 0.f, stream);
+    if (rc) return rc;
+    // one "partial" (G = 1): the exchange sums it over the ranks in rank order and applies Adam; statistics stay per-rank means
+    rc = exchange_launch(c, gsum, 1, np, flat_grad, stats_accum, 1.0f / (float)mb, 1, params, m, v, step0 + steps + 1, lr, beta1,
+                         beta2, eps, stream);
     if (rc) return rc;
   }
   return steps;

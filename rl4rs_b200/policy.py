@@ -66,6 +66,72 @@ class MaskedPolicy(object):
         return a.to(torch.int32), logp_all.gather(1, a.long().unsqueeze(1)).squeeze(1), value, logits
 
 
+class GaussianPolicy(object):
+    """The policy RLlib builds for the continuous-action env (`PPO_conti` / `A2C_conti`, modelfree_train.py:46-48): the default
+    FullyConnectedNetwork (fcnet_hiddens [256, 256], tanh, vf_share_layers off) over obs(256):
+        fc_1 256 tanh -> fc_2 256 tanh -> fc_out 2D = mean | log_std      (DiagGaussian dist inputs, free_log_std off)
+        fc_value_1 256 tanh -> fc_value_2 256 tanh -> value_out 1
+    normc_initializer(1.0) for the hidden kernels, 0.01 for fc_out and value_out, zero biases.  Exploration is
+    StochasticSampling (a = mean + std * N(0, 1)); evaluation takes the mean.  The env receives clip(a, -1, 1)
+    (clip_actions), the sample batch stores a.  The flat layout is csrc/r4_gauss.cuh's; this torch twin is the CPU path and
+    the autograd cross-check of those kernels (tests/test_gpu_trainer_conti.py)."""
+
+    def __init__(self, action_dim=32, device="cuda", seed=0):
+        self.D = action_dim
+        self.device = torch.device(device)
+        D2 = 2 * action_dim
+        shapes = [("w1", (OBS, 256)), ("b1", (256,)), ("w2", (256, 256)), ("b2", (256,)), ("wo", (256, D2)), ("bo", (D2,)),
+                  ("vw1", (OBS, 256)), ("vb1", (256,)), ("vw2", (256, 256)), ("vb2", (256,)), ("vwo", (256, 1)), ("vbo", (1,))]
+        n = sum(math.prod(s) for _, s in shapes)
+        g = torch.Generator(device="cpu").manual_seed(seed)
+        self.flat = torch.zeros(n, dtype=torch.float32, device=self.device, requires_grad=True)
+        off = 0
+        with torch.no_grad():
+            for name, shape in shapes:
+                k = math.prod(shape)
+                if len(shape) == 2:       # normc_initializer
+                    w = torch.randn(shape, generator=g)
+                    std = 0.01 if name in ("wo", "vwo") else 1.0
+                    self.flat[off:off + k].view(shape).copy_((w * std / w.pow(2).sum(0, keepdim=True).sqrt()).to(self.device))
+                off += k
+        self._shapes, self.n_params = shapes, n
+
+    params = MaskedPolicy.params
+
+    def forward(self, obs):
+        """obs f32 [n,256] -> (dist inputs [n,2D] = mean | log_std, value [n])."""
+        p = self.params()
+        h = torch.tanh(torch.tanh(obs @ p["w1"] + p["b1"]) @ p["w2"] + p["b2"])
+        g = torch.tanh(torch.tanh(obs @ p["vw1"] + p["vb1"]) @ p["vw2"] + p["vb2"])
+        return h @ p["wo"] + p["bo"], (g @ p["vwo"] + p["vbo"]).squeeze(-1)
+
+    @staticmethod
+    def logp(dist_inputs, action):
+        """DiagGaussian log-likelihood summed over the action dimensions."""
+        mu, ls = dist_inputs.chunk(2, dim=-1)
+        return (-0.5 * ((action - mu) / ls.exp()) ** 2 - ls - 0.5 * math.log(2 * math.pi)).sum(-1)
+
+    @staticmethod
+    def entropy(dist_inputs):
+        ls = dist_inputs.chunk(2, dim=-1)[1]
+        return (ls + 0.5 * math.log(2 * math.pi * math.e)).sum(-1)
+
+    @staticmethod
+    def kl(old_inputs, new_inputs):
+        """KL(old || new) of two DiagGaussians (RLlib TorchDiagGaussian.kl)."""
+        mo, lo = old_inputs.chunk(2, dim=-1)
+        mn, ln = new_inputs.chunk(2, dim=-1)
+        return (ln - lo + ((2 * lo).exp() + (mo - mn) ** 2) / (2 * (2 * ln).exp()) - 0.5).sum(-1)
+
+    @torch.no_grad()
+    def act(self, obs, explore=True):
+        """-> (action [n,D] unclipped, env action [n,D] = clip(action, -1, 1), logp [n], value [n], dist inputs [n,2D])."""
+        d, value = self.forward(obs)
+        mu, ls = d.chunk(2, dim=-1)
+        a = mu + ls.exp() * torch.randn(mu.shape, device=mu.device) if explore else mu.clone()
+        return a, a.clamp(-1.0, 1.0), self.logp(d, a), value, d
+
+
 class RawStatePolicy(object):
     """RLlib 'mask_model_rawstate' (rl4rs/nets/rllib/rllib_mask_model.py:67-115 over rllib_rawstate_model.py:25-86): the
     policy reads the RAW state -- category ids [21], dense features [432], sequence ids [2,64] (`rawstate_as_obs`,

@@ -25,7 +25,7 @@ import ctypes as C
 import torch
 import torch.distributed as dist
 
-from .policy import MaskedPolicy, RawStatePolicy
+from .policy import GaussianPolicy, MaskedPolicy, RawStatePolicy
 
 
 def _p(t, byte_offset=0):
@@ -395,14 +395,17 @@ class PPOTrainer(_TrainerBase):
         total = (-surr + self.kl_coeff * kl + c["vf_loss_coeff"] * vf - c["entropy_coeff"] * entropy).mean()
         return total, {"policy_loss": (-surr).mean(), "vf_loss": vf.mean(), "kl": kl.mean(), "entropy": entropy.mean()}
 
+    def _columns(self, buf):
+        """The rollout as flat [n, ...] columns, in the order loss() takes them before (adv, target)."""
+        n = buf.T * buf.B
+        flat = lambda x: x.reshape((n,) + x.shape[2:])
+        return (flat(buf.obs), flat(buf.mask), flat(buf.action), flat(buf.logp), flat(buf.logits), flat(buf.value))
+
     def learn(self, buf):
         c = self.config
         target, adv = self._gae(buf)
         n = buf.T * buf.B
-        flat = lambda x: x.reshape((n,) + x.shape[2:])
-        obs, mask, act = flat(buf.obs), flat(buf.mask), flat(buf.action)
-        logp, logits, val = flat(buf.logp), flat(buf.logits), flat(buf.value)
-        adv, target = flat(adv), flat(target)
+        adv, target = adv.reshape(n), target.reshape(n)
         # StandardizeFields(["advantages"]) over the whole (global) train batch
         mean, sq = adv.mean(), (adv ** 2).mean()
         if _world() > 1:
@@ -411,7 +414,7 @@ class PPOTrainer(_TrainerBase):
         # RLlib: sgd_minibatch_size is the TOTAL over devices; every rank contributes sgd_minibatch_size / world samples
         # of its own shard to each SGD step (multi-GPU tower semantics) and the loss is the mean over all of them
         mb = min(max(c["sgd_minibatch_size"] // _world(), 1), n)
-        data = (obs, mask, act, logp, logits, val, adv, target)
+        data = self._columns(buf) + (adv, target)
         agg, steps = (self._sgd_kernels if self.use_kernels else self._sgd_eager)(data, n, mb)
         named = {k: v / max(steps, 1) for k, v in agg.items()}
         named["_episode_reward_mean"] = buf.reward.sum(0).mean()
@@ -541,8 +544,261 @@ class A2CTrainer(_TrainerBase):
         return out
 
 
+# ---- the continuous-action env: Gaussian policy (PPO_conti / A2C_conti) ------------------------------------------------
+class GaussKernelOps(KernelOps):
+    """ctypes front of the Gaussian-policy kernels (include/rl4rs_b200.h: r4_gauss_*).  Same method names and signatures as
+    KernelOps, so PPOTrainer._sgd_kernels drives either; `data` is (obs, action, logp, dist_inputs, value, adv, target)."""
+
+    def __init__(self, D, device, n_params):
+        from . import _capi
+        self.capi = _capi
+        self.lib = _capi.load_library()
+        self.A = self.D = D
+        self.device, self.n = device, n_params
+        assert self.lib.r4_gauss_num_params(D) == n_params
+        z = lambda k: torch.zeros(k, dtype=torch.float32, device=device)
+        self.m, self.v, self.grad, self.stats, self.norm = z(n_params), z(n_params), z(n_params), z(5), z(1)
+        self.gsum = z(n_params + 5)      # one rank's gradient + statistics, the partial r4_grad_exchange_n sums (A2C)
+        self.scratch = z(self.lib.r4_gauss_scratch_size(D))
+        self.step = 0
+        self.counter = 0
+        self.launches = 0
+
+    def act(self, flat, obs, explore, seed, action, env_action, logp, value, dist_inputs):
+        n = obs.shape[0]
+        rc = self.lib.r4_gauss_act(_p(flat), _p(obs), n, self.D, int(bool(explore)), seed, self.counter, _p(action),
+                                   _p(env_action), _p(logp), _p(value), _p(dist_inputs), self._stream())
+        self._check(rc, "r4_gauss_act")
+        self.counter += n
+        self.launches += 1
+
+    def _chunks(self, n):
+        return 2 * -(-n // 2048)         # k_gauss_rows + k_gauss_wgrad per chunk of 2048 samples (r4_gauss.cuh: CH)
+
+    def policy_grad(self, mode, flat, data, idx, idx_offset, n, hp, inv_n, stat_scale, grad=None, stats=None):
+        obs, act, logp, dist_inputs, val, adv, target = data
+        grad = self.grad if grad is None else grad
+        stats = self.stats if stats is None else stats
+        rc = self.lib.r4_gauss_grad(mode, _p(flat), _p(obs), _p(act), _p(logp), _p(dist_inputs), _p(val), _p(adv), _p(target),
+                                    _p(idx, idx_offset * 8) if idx is not None else C.c_void_p(0), n, self.D, hp["clip"],
+                                    hp["vf_clip"], hp["vf_coeff"], hp["kl_coeff"], hp["ent_coeff"], inv_n, _p(self.scratch),
+                                    _p(grad), _p(stats), stat_scale, self._stream())
+        self._check(rc, "r4_gauss_grad")
+        self.launches += self._chunks(n)
+
+    def ppo_epoch(self, flat, data, perm, n, mb, hp, lr, clip):
+        obs, act, logp, dist_inputs, val, adv, target = data
+        rc = self.lib.r4_gauss_ppo_epoch(_p(flat), _p(obs), _p(act), _p(logp), _p(dist_inputs), _p(val), _p(adv), _p(target),
+                                         _p(perm), n, mb, self.D, hp["clip"], hp["vf_clip"], hp["vf_coeff"], hp["kl_coeff"],
+                                         hp["ent_coeff"], _p(self.scratch), _p(self.grad), _p(self.stats), _p(self.m),
+                                         _p(self.v), self.step, lr, 0.9, 0.999, 1e-8, float(clip or 0.0), _p(self.norm),
+                                         self._stream())
+        if rc < 0:
+            self._check(rc, "r4_gauss_ppo_epoch")
+        self.step += rc
+        self.launches += rc * (self._chunks(mb) + (2 if clip else 1))
+        return rc
+
+    def ppo_epoch_dist(self, comm, flat, data, perm, n, mb_local, hp, lr):
+        obs, act, logp, dist_inputs, val, adv, target = data
+        rc = self.lib.r4_gauss_ppo_epoch_dist(comm.h, _p(flat), _p(obs), _p(act), _p(logp), _p(dist_inputs), _p(val), _p(adv),
+                                              _p(target), _p(perm), n, mb_local, self.D, hp["clip"], hp["vf_clip"],
+                                              hp["vf_coeff"], hp["kl_coeff"], hp["ent_coeff"], _p(self.scratch), _p(self.grad),
+                                              _p(self.stats), _p(self.m), _p(self.v), self.step, lr, 0.9, 0.999, 1e-8,
+                                              self._stream())
+        if rc < 0:
+            self._check(rc, "r4_gauss_ppo_epoch_dist")
+        self.step += rc
+        self.launches += rc * (self._chunks(mb_local) + 1)
+        return rc
+
+    def policy_grad_exchange(self, comm, mode, flat, data, n, hp, inv_n, stat_scale):
+        """One gradient over n local samples, summed over the ranks through peer memory into self.grad (A2C)."""
+        self.gsum[self.n:].zero_()
+        self.policy_grad(mode, flat, data, None, 0, n, hp, inv_n, 1.0, grad=self.gsum[:self.n], stats=self.gsum[self.n:])
+        rc = self.lib.r4_grad_exchange_n(comm.h, _p(self.gsum), 1, self.n, _p(self.grad), _p(self.stats), stat_scale,
+                                         self._stream())
+        self._check(rc, "r4_grad_exchange_n")
+        self.launches += 1
+
+
+class GaussRolloutBuffer(RolloutBuffer):
+    """[T, B, ...] device-resident sample batch of the continuous-action env: the unclipped action, the dist inputs
+    (mean | log_std, RLlib's stored 'action_dist_inputs'), no mask and no logits."""
+
+    def __init__(self, T, B, D, device, obs_dim=256):
+        z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=device)
+        self.obs, self.action, self.dist = z(T, B, obs_dim), z(T, B, D), z(T, B, 2 * D)
+        self.logp, self.value, self.reward = z(T, B), z(T, B), z(T, B)
+        self.T, self.B = T, B
+
+
+class _GaussMixin(object):
+    """Set-up, rollout and compute_actions of the Gaussian-policy trainers; train / evaluate / save / restore / GAE come from
+    _TrainerBase unchanged."""
+
+    def _setup(self, config, env, device, seed):
+        self.config = dict(self.DEFAULTS, **{k: v for k, v in (config or {}).items() if k in self.DEFAULTS})
+        self.env = env
+        self.T = env.config["max_steps"]
+        self.B = env.config["batch_size"]
+        self.D = env.config.get("action_emb_size", 32)
+        self.device = torch.device(device) if device is not None else env.sim.engine.device
+        self.rawstate = False
+        self.policy = GaussianPolicy(self.D, self.device, seed=seed)     # same init on every rank
+        self.use_kernels = self.device.type == "cuda" and (config or {}).get("use_kernels", True)
+        self.opt = torch.optim.Adam([self.policy.flat], lr=self.config["lr"])
+        self.ops = GaussKernelOps(self.D, self.device, self.policy.n_params) if self.use_kernels else None
+        self.comm = PeerComm(self.policy.n_params, self.device) if self.use_kernels else None
+        rank = dist.get_rank() if dist.is_available() and dist.is_initialized() else 0
+        self._seed = (seed * 1000003 + rank) & 0x7fffffffffffffff       # per-rank exploration noise (see _TrainerBase)
+        if rank and not self.use_kernels:
+            torch.manual_seed(seed * 1000003 + rank)
+        self.buf = GaussRolloutBuffer(self.T, self.B, self.D, self.device)
+        self._env_act = torch.zeros(self.B, self.D, dtype=torch.float32, device=self.device)
+        self.iteration = 0
+        self.timesteps_total = 0
+
+    @torch.no_grad()
+    def rollout(self, explore=True):
+        env, buf = self.env, self.buf
+        obs = env.reset()
+        for t in range(self.T):
+            buf.obs[t].copy_(obs["obs"] if isinstance(obs, dict) else obs)
+            if self.use_kernels:       # forward + sampling + clipping in ONE kernel, written straight into the rollout buffers
+                ea = self._env_act
+                self.ops.act(self.policy.flat, buf.obs[t], explore, self._seed, buf.action[t], ea, buf.logp[t], buf.value[t],
+                             buf.dist[t])
+            else:
+                a, ea, logp, value, d = self.policy.act(buf.obs[t], explore=explore)
+                buf.action[t].copy_(a); buf.logp[t].copy_(logp); buf.value[t].copy_(value); buf.dist[t].copy_(d)
+            obs, reward, done, info = env.step(ea)          # clip_actions: the env gets clip(a, -1, 1), the buffer keeps a
+            buf.reward[t].copy_(reward)
+        self.final_step = (obs, done)
+        return buf
+
+    @torch.no_grad()
+    def compute_actions(self, obs, explore=False):
+        """trainer.compute_actions: obs f32 [n,256] (array or tensor, or {'obs': ...}) or RLlib's {i: observation} dict
+        -> clipped actions f32 [n,D] (a dict keyed like the input for the RLlib form)."""
+        import numpy as np
+        if isinstance(obs, dict) and "obs" not in obs:      # RLlib's {env_id: observation} form
+            keys = list(obs.keys())
+            rows = [np.asarray(obs[k]["obs"] if isinstance(obs[k], dict) else obs[k], dtype=np.float32) for k in keys]
+            return dict(zip(keys, list(self.compute_actions(np.stack(rows), explore))))
+        if isinstance(obs, dict):
+            obs = obs["obs"]
+        o = torch.as_tensor(obs, dtype=torch.float32, device=self.device).contiguous()
+        if self.use_kernels:
+            n = o.shape[0]
+            e = lambda *s: torch.empty(*s, dtype=torch.float32, device=self.device)
+            ea = e(n, self.D)
+            self.ops.act(self.policy.flat, o, explore, self._seed, e(n, self.D), ea, e(n), e(n), None)
+            return ea.cpu().numpy()
+        return self.policy.act(o, explore=explore)[1].cpu().numpy()
+
+
+class GaussPPOTrainer(_GaussMixin, PPOTrainer):
+    """PPO_conti: RLlib 1.5 PPO over the DiagGaussian policy; the learner is PPOTrainer's (GAE, standardised advantages,
+    minibatch SGD, adaptive KL, peer-memory exchange) with the Gaussian loss and kernels."""
+    algo = "PPO_conti"
+
+    def __init__(self, config, env, device=None, seed=0):
+        self._setup(config, env, device, seed)
+        self.kl_coeff = self.config["kl_coeff"]
+        self._gen = torch.Generator(device=self.device if self.device.type == "cuda" else "cpu").manual_seed(seed)
+
+    def _columns(self, buf):
+        n = buf.T * buf.B
+        flat = lambda x: x.reshape((n,) + x.shape[2:])
+        return (flat(buf.obs), flat(buf.action), flat(buf.logp), flat(buf.dist), flat(buf.value))
+
+    def loss(self, obs, action, old_logp, old_dist, old_value, adv, target):
+        """RLlib 1.5 ppo_surrogate_loss over TorchDiagGaussian."""
+        c = self.config
+        d, value = self.policy.forward(obs)
+        logp = GaussianPolicy.logp(d, action)
+        kl = GaussianPolicy.kl(old_dist, d)
+        entropy = GaussianPolicy.entropy(d)
+        ratio = torch.exp(logp - old_logp)
+        surr = torch.min(adv * ratio, adv * torch.clamp(ratio, 1 - c["clip_param"], 1 + c["clip_param"]))
+        vf1 = (value - target) ** 2
+        vclip = old_value + torch.clamp(value - old_value, -c["vf_clip_param"], c["vf_clip_param"])
+        vf = torch.max(vf1, (vclip - target) ** 2)
+        total = (-surr + self.kl_coeff * kl + c["vf_loss_coeff"] * vf - c["entropy_coeff"] * entropy).mean()
+        return total, {"policy_loss": (-surr).mean(), "vf_loss": vf.mean(), "kl": kl.mean(), "entropy": entropy.mean()}
+
+
+class GaussA2CTrainer(_GaussMixin, A2CTrainer):
+    """A2C_conti: RLlib 1.5 A3C loss (summed) over the DiagGaussian policy, one gradient step per iteration."""
+    algo = "A2C_conti"
+
+    def __init__(self, config, env, device=None, seed=0):
+        self._setup(config, env, device, seed)
+
+    def loss(self, obs, action, adv, target):
+        c = self.config
+        d, value = self.policy.forward(obs)
+        pi_loss = -(GaussianPolicy.logp(d, action) * adv).sum()
+        vf_loss = 0.5 * ((value - target) ** 2).sum()
+        entropy = GaussianPolicy.entropy(d).sum()
+        total = pi_loss + c["vf_loss_coeff"] * vf_loss - c["entropy_coeff"] * entropy
+        return total, {"policy_loss": pi_loss, "vf_loss": vf_loss, "entropy": entropy}
+
+    def learn(self, buf):
+        c = self.config
+        target, adv = self._gae(buf)
+        n = buf.T * buf.B
+        obs, act = buf.obs.reshape(n, -1), buf.action.reshape(n, -1)
+        adv, target = adv.reshape(n).contiguous(), target.reshape(n).contiguous()
+        w = _world()
+        if self.use_kernels:
+            ops = self.ops
+            data = (obs, act, None, None, None, adv, target)
+            hp = {"clip": 0.0, "vf_clip": 0.0, "vf_coeff": c["vf_loss_coeff"], "kl_coeff": 0.0, "ent_coeff": c["entropy_coeff"]}
+            ops.stats.zero_()
+            if w > 1 and self.comm is not None and self.comm.ok:
+                ops.policy_grad_exchange(self.comm, 1, self.policy.flat, data, n, hp, 1.0, 1.0)   # summed over the ranks
+            else:
+                ops.policy_grad(1, self.policy.flat, data, None, 0, n, hp, 1.0, 1.0)
+                if w > 1:
+                    dist.all_reduce(ops.grad, op=dist.ReduceOp.SUM)            # summed loss over the global batch
+            gn = ops.grad.norm()
+            ops.adam(self.policy.flat, c["lr"], 1.0, c["grad_clip"])
+            st = ops.stats
+            g = self._global_means({"policy_loss": st[0], "vf_loss": st[1], "entropy": st[3], "total_loss": st[4], "gn": gn,
+                                    "_episode_reward_mean": buf.reward.sum(0).mean()})
+            return {"policy_loss": g["policy_loss"] * w, "vf_loss": g["vf_loss"] * w, "entropy": g["entropy"] * w,
+                    "total_loss": g["total_loss"] * w, "grad_gnorm": g["gn"], "sgd_steps": 1,
+                    "_episode_reward_mean": g["_episode_reward_mean"]}
+        if self.policy.flat.grad is not None:
+            self.policy.flat.grad.zero_()
+        total, st = self.loss(obs, act, adv, target)
+        total.backward()
+        self._allreduce_grad(average=False)          # summed loss over the global batch
+        gn = torch.nn.utils.clip_grad_norm_([self.policy.flat], c["grad_clip"]) if c["grad_clip"] else torch.zeros(())
+        self.opt.step()
+        out = {k: self._global_mean(v) * w for k, v in st.items()}
+        out.update({"total_loss": self._global_mean(total) * w, "grad_gnorm": float(gn), "sgd_steps": 1})
+        return out
+
+
 def get_rl_model(algo, rllib_config, env=None, **kw):
-    """script/modelfree_trainer.py:11-36.  Only the algorithms of the BASELINE configs are built."""
+    """script/modelfree_trainer.py:11-36.  Only the algorithms of the BASELINE configs are built.  On an env built with
+    support_conti_env, PPO / A2C (and PPO_conti / A2C_conti, modelfree_train.py:46-48) train the Gaussian policy."""
+    conti = env is not None and bool(env.config.get("support_conti_env", False))
+    if algo.endswith("_conti") or (conti and algo in ("PPO", "A2C")):
+        base = algo[:-len("_conti")] if algo.endswith("_conti") else algo
+        if base not in ("PPO", "A2C"):
+            raise NotImplementedError("%s is outside the hot-path scope (SURVEY.md section 2, row 11)" % algo)
+        if not conti:
+            raise ValueError("%s needs an env built with support_conti_env=True" % algo)
+        if env.config.get("rawstate_as_obs", False):
+            raise NotImplementedError("%s on a rawstate_as_obs env (model_rawstate) is not built" % algo)
+        if env.config.get("support_rllib_mask", False):
+            raise ValueError("%s takes the plain observation: build the env with support_rllib_mask=False "
+                             "(the reference turns the mask off for *_conti, modelfree_train.py:46-48)" % algo)
+        return (GaussPPOTrainer if base == "PPO" else GaussA2CTrainer)(rllib_config, env, **kw)
     if algo in ("PPO", "PPO_rawstate"):        # '*_rawstate' = the same trainer on an env built with rawstate_as_obs (modelfree_train.py:55-56)
         return PPOTrainer(rllib_config, env, **kw)
     if algo in ("A2C", "A2C_rawstate"):
