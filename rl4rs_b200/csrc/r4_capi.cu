@@ -1387,9 +1387,7 @@ static int exchange_launch(r4_comm* c, const float* scratch, int G, int np, floa
 
 int r4_grad_exchange(r4_comm* c, const float* scratch, int G, int action_size, float* flat_grad, float* stats_accum,
                      float stat_scale, void* stream) {
-  if (!c || !scratch || !flat_grad || G < 1) return fail(nullptr, R4_ERR_ARG, "r4_grad_exchange: bad argument");
-  return exchange_launch(c, scratch, G, r4ppo::make_layout(action_size).n, flat_grad, stats_accum, stat_scale, 0, nullptr, nullptr,
-                         nullptr, 0, 0.f, 0.f, 0.f, 0.f, stream);
+  return r4_grad_exchange_n(c, scratch, G, r4ppo::make_layout(action_size).n, flat_grad, stats_accum, stat_scale, stream);
 }
 
 int r4_ppo_epoch_dist(r4_comm* c, float* params, const float* obs, const uint8_t* mask, const int64_t* action,
@@ -1466,7 +1464,7 @@ static int gauss_grad_impl(int mode, const float* params, const float* obs, cons
     attr = true;
   }
   const r4gauss::Layout L = r4gauss::make_layout(D);
-  const r4gauss::Hyper hp{mode, clip, vf_clip, vf_coeff, kl_coeff, ent_coeff, inv_n};
+  const r4ppo::LossHyper hp{mode, clip, vf_clip, vf_coeff, kl_coeff, ent_coeff, inv_n};
   const r4gauss::Planes P = r4gauss::make_planes(scratch, D);
   const r4gauss::Jobs J = r4gauss::make_jobs(L, P);
   for (int c0 = 0; c0 < n; c0 += r4gauss::CH) {

@@ -172,10 +172,6 @@ __global__ void __launch_bounds__(NT) k_gauss_act(Layout L, const float* __restr
 // gradient, part 1: per-sample rows.  Positions p = c0 .. c0+cn of the sample list (idx[p], or p when idx == nullptr);
 // row q = p - c0 of every plane.  mode 0 = PPO (loss mean: inv_n), mode 1 = A2C (sums).
 // ------------------------------------------------------------------------------------------------
-struct Hyper {
-  int mode;
-  float clip, vf_clip, vf_coeff, kl_coeff, ent_coeff, inv_n;
-};
 struct Planes {
   float *x, *h1, *h2, *g1, *g2, *d1, *d2, *e1, *e2, *dout, *dv, *stats;
 };
@@ -190,7 +186,7 @@ __host__ __device__ inline Planes make_planes(float* scratch, int D) {
   return P;
 }
 
-__global__ void __launch_bounds__(NT) k_gauss_rows(Layout L, Hyper hp, const float* __restrict__ prm, const float* __restrict__ obs,
+__global__ void __launch_bounds__(NT) k_gauss_rows(Layout L, r4ppo::LossHyper hp, const float* __restrict__ prm, const float* __restrict__ obs,
                                                    const float* __restrict__ action, const float* __restrict__ old_logp,
                                                    const float* __restrict__ old_dist, const float* __restrict__ old_value,
                                                    const float* __restrict__ adv, const float* __restrict__ target,
@@ -227,47 +223,25 @@ __global__ void __launch_bounds__(NT) k_gauss_rows(Layout L, Hyper hp, const flo
     const float logp = -0.5f * q - sls - HALF_LOG_2PI * D;
     const float ent = sls + HALF_LOG_2PIE * D;
     const float advv = adv[r], tg = target[r], v = val[s];
-    float ca, ckl = 0.f, cent = hp.ent_coeff, dv, pl, vl;
-    if (hp.mode == 0) {                                    // same surrogate / value clip algebra as r4ppo::k_policy_grad
-      const float ratio = expf(logp - old_logp[r]);
-      const float lo = 1.f - hp.clip, hi = 1.f + hp.clip;
-      const float t1 = advv * ratio, t2 = advv * fminf(fmaxf(ratio, lo), hi);
-      const float g2c = (ratio >= lo && ratio <= hi) ? advv : 0.f;
-      const float g = t1 < t2 ? advv : (t2 < t1 ? g2c : 0.5f * (advv + g2c));     // torch.min ties split evenly
-      ca = -g * ratio * hp.inv_n;
-      ckl = hp.kl_coeff * hp.inv_n;
-      cent *= hp.inv_n;
-      const float vo = old_value[r], d = v - vo;
-      const float dcl = fminf(fmaxf(d, -hp.vf_clip), hp.vf_clip), vcl = vo + dcl;
-      const float vf1 = (v - tg) * (v - tg), vf2 = (vcl - tg) * (vcl - tg);
-      const float gv1 = 2.f * (v - tg), gv2 = (fabsf(d) <= hp.vf_clip) ? 2.f * (vcl - tg) : 0.f;
-      const float gv = vf1 > vf2 ? gv1 : (vf2 > vf1 ? gv2 : 0.5f * (gv1 + gv2));
-      dv = hp.vf_coeff * gv * hp.inv_n;
-      pl = -fminf(t1, t2); vl = fmaxf(vf1, vf2);
-    } else {
-      ca = -advv;
-      dv = hp.vf_coeff * (v - tg);
-      pl = -logp * advv; vl = 0.5f * (v - tg) * (v - tg);
-    }
+    const r4ppo::SampleLoss sl = r4ppo::sample_loss(hp, logp, hp.mode == 0 ? old_logp[r] : 0.f, advv, tg, v,
+                                                    hp.mode == 0 ? old_value[r] : 0.f, kl, ent);
     // d logp / d mu = z / sd, d logp / d ls = z^2 - 1; d ent / d ls = 1;
     // d kl / d mu = (mu - mu_o) / sd^2, d kl / d ls = 1 - (sd_o^2 + (mu_o - mu)^2) / sd^2
     for (int i = lane; i < D; i += 32) {
       const float mu = od[i], ls = od[D + i], sd = expf(ls), z = (__ldg(action + r * D + i) - mu) / sd;
-      float gm = ca * (z / sd), gl = ca * (z * z - 1.f) - cent;
-      if (old_dist && ckl != 0.f) {
+      float gm = sl.ca * (z / sd), gl = sl.ca * (z * z - 1.f) - sl.cent;
+      if (old_dist && sl.ckl != 0.f) {
         const float muo = __ldg(old_dist + r * N2 + i), so = expf(__ldg(old_dist + r * N2 + D + i));
         const float dm = muo - mu, s2 = expf(2.f * ls);
-        gm = fmaf(ckl, -dm / s2, gm);
-        gl = fmaf(ckl, 1.f - (so * so + dm * dm) / s2, gl);
+        gm = fmaf(sl.ckl, -dm / s2, gm);
+        gl = fmaf(sl.ckl, 1.f - (so * so + dm * dm) / s2, gl);
       }
       od[i] = gm; od[D + i] = gl;
     }
     if (lane == 0) {
-      dvs[s] = dv;
-      const float tot = hp.mode == 0 ? (pl + hp.kl_coeff * kl + hp.vf_coeff * vl - hp.ent_coeff * ent)
-                                     : (pl + hp.vf_coeff * vl - hp.ent_coeff * ent);
+      dvs[s] = sl.dv;
       float* st = P.stats + (size_t)(q0 + s) * 5;
-      st[0] = pl; st[1] = vl; st[2] = kl; st[3] = ent; st[4] = tot;
+      st[0] = sl.pl; st[1] = sl.vl; st[2] = sl.kl; st[3] = sl.ent; st[4] = sl.total;
     }
   }
   __syncthreads();

@@ -181,6 +181,43 @@ struct LossHyper {
   float clip, vf_clip, vf_coeff, kl_coeff, ent_coeff, inv_n;
 };
 
+// The per-sample scalars of the loss, for both policies' gradient kernels (k_policy_grad, r4gauss::k_gauss_rows): from the
+// sample's logp of the taken action, value, KL and entropy, the loss derivatives d/dlogp = ca, d/dkl = ckl,
+// d/dentropy = -cent, d/dvalue = dv, and the statistics pl, vl, kl, ent, total.  old_logp and old_value are used in mode 0 only.
+struct SampleLoss {
+  float ca, ckl, cent, dv, pl, vl, kl, ent, total;
+};
+__device__ __forceinline__ SampleLoss sample_loss(const LossHyper& hp, float logp, float old_logp, float adv, float target,
+                                                  float value, float old_value, float kl, float ent) {
+  SampleLoss o;
+  const float v = value, tg = target;
+  o.ckl = 0.f; o.cent = hp.ent_coeff; o.kl = kl; o.ent = ent;
+  if (hp.mode == 0) {
+    const float ratio = expf(logp - old_logp);
+    const float lo = 1.f - hp.clip, hi = 1.f + hp.clip;
+    const float t1 = adv * ratio, t2 = adv * fminf(fmaxf(ratio, lo), hi);
+    const float g2 = (ratio >= lo && ratio <= hi) ? adv : 0.f;
+    const float g = t1 < t2 ? adv : (t2 < t1 ? g2 : 0.5f * (adv + g2));     // torch.min ties split evenly
+    o.ca = -g * ratio * hp.inv_n;
+    o.ckl = hp.kl_coeff * hp.inv_n;
+    o.cent *= hp.inv_n;
+    const float vo = old_value, d = v - vo;
+    const float dcl = fminf(fmaxf(d, -hp.vf_clip), hp.vf_clip), vcl = vo + dcl;
+    const float vf1 = (v - tg) * (v - tg), vf2 = (vcl - tg) * (vcl - tg);
+    const float gv1 = 2.f * (v - tg), gv2 = (fabsf(d) <= hp.vf_clip) ? 2.f * (vcl - tg) : 0.f;
+    const float gv = vf1 > vf2 ? gv1 : (vf2 > vf1 ? gv2 : 0.5f * (gv1 + gv2));
+    o.dv = hp.vf_coeff * gv * hp.inv_n;
+    o.pl = -fminf(t1, t2); o.vl = fmaxf(vf1, vf2);
+  } else {
+    o.ca = -adv;
+    o.dv = hp.vf_coeff * (v - tg);
+    o.pl = -logp * adv; o.vl = 0.5f * (v - tg) * (v - tg);
+  }
+  o.total = hp.mode == 0 ? (o.pl + hp.kl_coeff * kl + hp.vf_coeff * o.vl - hp.ent_coeff * ent)
+                         : (o.pl + hp.vf_coeff * o.vl - hp.ent_coeff * ent);
+  return o;
+}
+
 // SINGLE = true: the grid has exactly one tile per CTA (a PPO minibatch): no shared-memory gradient accumulator;
 // instead both weight matrices are staged in shared memory once (136 KB) so every inner loop reads shared memory, and
 // each gradient element is stored straight to this CTA's partial row by its owner thread.
@@ -277,40 +314,18 @@ __global__ void __launch_bounds__(NT) k_policy_grad(Layout L, LossHyper hp, cons
         if (p > 0.f) ent -= p * lp;
       }
       kl = warp_sum(kl); ent = warp_sum(ent);
-      float ca, ckl = 0.f, cent = hp.ent_coeff, dv, pl, vl;
-      if (hp.mode == 0) {
-        const float ratio = expf(logp - old_logp[r]);
-        const float lo = 1.f - hp.clip, hi = 1.f + hp.clip;
-        const float t1 = advv * ratio, t2 = advv * fminf(fmaxf(ratio, lo), hi);
-        const float g2 = (ratio >= lo && ratio <= hi) ? advv : 0.f;
-        const float g = t1 < t2 ? advv : (t2 < t1 ? g2 : 0.5f * (advv + g2));     // torch.min ties split evenly
-        ca = -g * ratio * hp.inv_n;
-        ckl = hp.kl_coeff * hp.inv_n;
-        cent *= hp.inv_n;
-        const float vo = old_value[r], d = v - vo;
-        const float dcl = fminf(fmaxf(d, -hp.vf_clip), hp.vf_clip), vcl = vo + dcl;
-        const float vf1 = (v - tg) * (v - tg), vf2 = (vcl - tg) * (vcl - tg);
-        const float gv1 = 2.f * (v - tg), gv2 = (fabsf(d) <= hp.vf_clip) ? 2.f * (vcl - tg) : 0.f;
-        const float gv = vf1 > vf2 ? gv1 : (vf2 > vf1 ? gv2 : 0.5f * (gv1 + gv2));
-        dv = hp.vf_coeff * gv * hp.inv_n;
-        pl = -fminf(t1, t2); vl = fmaxf(vf1, vf2);
-      } else {
-        ca = -advv;
-        dv = hp.vf_coeff * (v - tg);
-        pl = -logp * advv; vl = 0.5f * (v - tg) * (v - tg);
-      }
+      const SampleLoss o = sample_loss(hp, logp, hp.mode == 0 ? old_logp[r] : 0.f, advv, tg, v,
+                                       hp.mode == 0 ? old_value[r] : 0.f, kl, ent);
       // dlogits_j = ca (delta_ja - p_j) + ckl (p_j - p_old_j) + cent p_j (logp_j + H)
       for (int c = lane; c < L.A; c += 32) {
         float lp = lg[c] - lse, p = expf(lp), po = expf(__ldg(ol + c) - lso);
-        float dz = ca * ((c == a ? 1.f : 0.f) - p) + ckl * (p - po);
-        if (cent != 0.f && p > 0.f) dz += cent * p * (lp + ent);
+        float dz = o.ca * ((c == a ? 1.f : 0.f) - p) + o.ckl * (p - po);
+        if (o.cent != 0.f && p > 0.f) dz += o.cent * p * (lp + ent);
         lg[c] = dz;
       }
       if (lane == 0) {
-        dv_s[s] = dv;
-        float tot = hp.mode == 0 ? (pl + hp.kl_coeff * kl + hp.vf_coeff * vl - hp.ent_coeff * ent)
-                                 : (pl + hp.vf_coeff * vl - hp.ent_coeff * ent);
-        stat_t[s][0] = pl; stat_t[s][1] = vl; stat_t[s][2] = kl; stat_t[s][3] = ent; stat_t[s][4] = tot;
+        dv_s[s] = o.dv;
+        stat_t[s][0] = o.pl; stat_t[s][1] = o.vl; stat_t[s][2] = o.kl; stat_t[s][3] = o.ent; stat_t[s][4] = o.total;
       }
     }
     __syncthreads();

@@ -54,6 +54,20 @@ class MaskedPolicy(object):
         value = (h @ p["wv"] + p["bv"]).squeeze(-1)
         return logits + inf_mask, value
 
+    def inputs(self, obs):
+        """env observation {'obs', 'action_mask'} -> the inputs of forward()."""
+        return obs["obs"], obs["action_mask"]
+
+    def terms(self, logits, action, old_logits=None):
+        """Categorical over masked logits -> (logp(action), KL(old || new) or None without old_logits, entropy) per sample."""
+        logp_all = torch.log_softmax(logits, -1)
+        logp = logp_all.gather(1, action.unsqueeze(1)).squeeze(1)
+        kl = None
+        if old_logits is not None:
+            old_logp_all = torch.log_softmax(old_logits, -1)
+            kl = (old_logp_all.exp() * (old_logp_all - logp_all)).sum(-1)
+        return logp, kl, -(logp_all.exp() * logp_all).sum(-1)
+
     @torch.no_grad()
     def act(self, obs, mask, explore=True):
         """-> (action i32 [B], logp [B], value [B], masked logits [B,A])."""
@@ -104,6 +118,14 @@ class GaussianPolicy(object):
         h = torch.tanh(torch.tanh(obs @ p["w1"] + p["b1"]) @ p["w2"] + p["b2"])
         g = torch.tanh(torch.tanh(obs @ p["vw1"] + p["vb1"]) @ p["vw2"] + p["vb2"])
         return h @ p["wo"] + p["bo"], (g @ p["vwo"] + p["vbo"]).squeeze(-1)
+
+    def inputs(self, obs):
+        """env observation (the obs vector, or {'obs': ...}) -> the inputs of forward()."""
+        return (obs["obs"] if isinstance(obs, dict) else obs,)
+
+    def terms(self, dist_inputs, action, old_dist=None):
+        """-> (logp(action), KL(old || new) or None without old_dist, entropy) per sample."""
+        return self.logp(dist_inputs, action), None if old_dist is None else self.kl(old_dist, dist_inputs), self.entropy(dist_inputs)
 
     @staticmethod
     def logp(dist_inputs, action):
@@ -184,6 +206,9 @@ class RawStatePolicy(object):
         return torch.cat([obs["category_feature"].reshape(B, -1).to(torch.float32), obs["dense_feature"].reshape(B, -1).to(torch.float32),
                           obs["sequence_feature"].reshape(B, -1).to(torch.float32)], dim=1)
 
+    def inputs(self, obs):
+        return self.pack(obs), obs["action_mask"]
+
     def forward(self, obs, mask):
         p = self.params()
         C, D = self.C, self.D
@@ -199,4 +224,4 @@ class RawStatePolicy(object):
         inf_mask = torch.clamp(torch.log(mask.to(torch.float32)), min=FLOAT_MIN)
         return logits + inf_mask, (ctx @ p["wv"] + p["bv"]).squeeze(-1)
 
-    act = MaskedPolicy.act
+    act, terms = MaskedPolicy.act, MaskedPolicy.terms

@@ -11,7 +11,8 @@ Differences from the reference, by design (north_star):
 On a CUDA device the policy forward + sampling, the loss gradients (hand-derived backward) and Adam
 are the library's own kernels (csrc/r4_ppo.cuh through the C-ABI: r4_policy_act / r4_policy_grad /
 r4_adam_step), 2 launches per SGD step; the torch implementation below is kept as the CPU path of
-the tests and as the autograd cross-check of the kernels (tests/test_gpu_trainer.py).
+the tests and as the autograd cross-check of the kernels (tests/test_gpu_trainer.py).  The Gaussian policy of the
+continuous-action env (GaussPPOTrainer / GaussA2CTrainer) runs the same learner over csrc/r4_gauss.cuh (GaussKernelOps).
 
 RLlib semantics kept: gamma = 1, GAE(lambda = 1) advantages from complete episodes, SoftQ(T=1)
 exploration = sampling from softmax(masked logits), argmax for evaluation; PPO: standardised
@@ -32,22 +33,39 @@ def _p(t, byte_offset=0):
     return C.c_void_p(t.data_ptr() + byte_offset) if t is not None else C.c_void_p(0)
 
 
+def _hp(hp):
+    """The loss hyper-parameters in the argument order of the gradient entry points."""
+    return hp["clip"], hp["vf_clip"], hp["vf_coeff"], hp["kl_coeff"], hp["ent_coeff"]
+
+
 class KernelOps(object):
-    """ctypes front of the K12 kernels (include/rl4rs_b200.h: r4_policy_act / r4_policy_grad / r4_adam_step)."""
+    """ctypes front of the K12 kernels (include/rl4rs_b200.h: r4_policy_act / r4_policy_grad / r4_adam_step).  `data` is
+    (obs, mask, action, logp, logits, value, adv, target), the argument order of the gradient entry points."""
 
     def __init__(self, A, device, n_params):
+        self.A = A
+        self._init(device, n_params)
+
+    def _init(self, device, n_params):
+        """The Adam, gradient and statistics buffers, the learner scratch and the counters, for either policy."""
         from . import _capi
         self.capi = _capi
         self.lib = _capi.load_library()
-        self.A, self.device, self.n = A, device, n_params
-        assert self.lib.r4_policy_num_params(A) == n_params
+        self.device, self.n = device, n_params
+        assert self._num_params() == n_params
         z = lambda k: torch.zeros(k, dtype=torch.float32, device=device)
         self.m, self.v, self.grad, self.stats, self.norm = z(n_params), z(n_params), z(n_params), z(5), z(1)
         self.sms = torch.cuda.get_device_properties(device).multi_processor_count   # grid cap of the learner kernels
-        self.scratch = z(self.sms * (n_params + 5))
+        self.scratch = z(self._scratch_floats())
         self.step = 0
         self.counter = 0
         self.launches = 0                # kernels launched through this object (bench.py: gpu_launches)
+
+    def _num_params(self):
+        return self.lib.r4_policy_num_params(self.A)
+
+    def _scratch_floats(self):
+        return self.sms * (self.n + 5)   # one partial gradient + statistics per CTA
 
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
@@ -65,53 +83,50 @@ class KernelOps(object):
         self.launches += 1
 
     def policy_grad(self, mode, flat, data, idx, idx_offset, n, hp, inv_n, stat_scale, G=None):
-        obs, mask, act, logp, logits, val, adv, target = data
         G = G or max(1, min((n + 3) // 4, self.sms))          # 4 samples per CTA tile (r4_ppo.cuh: TS)
-        rc = self.lib.r4_policy_grad(mode, _p(flat), _p(obs), _p(mask), _p(act), _p(logp), _p(logits), _p(val), _p(adv),
-                                     _p(target), _p(idx, idx_offset * 8) if idx is not None else C.c_void_p(0), n, self.A,
-                                     hp["clip"], hp["vf_clip"], hp["vf_coeff"], hp["kl_coeff"], hp["ent_coeff"], inv_n,
+        rc = self.lib.r4_policy_grad(mode, _p(flat), *map(_p, data), _p(idx, idx_offset * 8), n, self.A, *_hp(hp), inv_n,
                                      _p(self.scratch), G, _p(self.grad), _p(self.stats), stat_scale, self._stream())
         self._check(rc, "r4_policy_grad")
         self.launches += 2               # k_policy_grad + k_grad_reduce
 
     def ppo_epoch(self, flat, data, perm, n, mb, hp, lr, clip):
         """All minibatch steps of one SGD epoch in ONE library call (single-GPU learner)."""
-        obs, mask, act, logp, logits, val, adv, target = data
-        rc = self.lib.r4_ppo_epoch(_p(flat), _p(obs), _p(mask), _p(act), _p(logp), _p(logits), _p(val), _p(adv), _p(target),
-                                   _p(perm), n, mb, self.A, hp["clip"], hp["vf_clip"], hp["vf_coeff"], hp["kl_coeff"],
-                                   hp["ent_coeff"], _p(self.scratch), _p(self.grad), _p(self.stats), _p(self.m), _p(self.v),
-                                   self.step, lr, 0.9, 0.999, 1e-8, float(clip or 0.0), _p(self.norm), self._stream())
-        if rc < 0:
-            self._check(rc, "r4_ppo_epoch")
-        self.step += rc
+        rc = self._epoch("r4_ppo_epoch", (), self.A, flat, data, perm, n, mb, hp, lr, (float(clip or 0.0), _p(self.norm)))
         self.launches += rc * (4 if clip else 2)   # k_policy_grad + k_reduce_adam, or + k_grad_reduce, k_sumsq, k_adam
         return rc
 
     def ppo_epoch_dist(self, comm, flat, data, perm, n, mb_local, hp, lr):
         """All minibatch steps of one SGD epoch of a data-parallel learner in ONE library call: per step the gradient
         kernel + the fused peer-memory exchange / Adam kernel (csrc/r4_comm.cuh); no NCCL, no host round trip."""
-        obs, mask, act, logp, logits, val, adv, target = data
-        rc = self.lib.r4_ppo_epoch_dist(comm.h, _p(flat), _p(obs), _p(mask), _p(act), _p(logp), _p(logits), _p(val), _p(adv),
-                                        _p(target), _p(perm), n, mb_local, self.A, hp["clip"], hp["vf_clip"], hp["vf_coeff"],
-                                        hp["kl_coeff"], hp["ent_coeff"], _p(self.scratch), _p(self.grad), _p(self.stats),
-                                        _p(self.m), _p(self.v), self.step, lr, 0.9, 0.999, 1e-8, self._stream())
-        if rc < 0:
-            self._check(rc, "r4_ppo_epoch_dist")
-        self.step += rc
+        rc = self._epoch("r4_ppo_epoch_dist", (comm.h,), self.A, flat, data, perm, n, mb_local, hp, lr, ())
         self.launches += rc * 2          # k_policy_grad + k_exchange_adam
+        return rc
+
+    def _epoch(self, fn, head, dim, flat, data, perm, n, mb, hp, lr, tail):
+        """One call of an epoch entry point (r4_ppo_epoch, r4_gauss_ppo_epoch and their _dist forms): the argument lists differ
+        only in the leading communicator, the policy's columns and size, and the trailing gradient clip."""
+        rc = getattr(self.lib, fn)(*head, _p(flat), *map(_p, data), _p(perm), n, mb, dim, *_hp(hp), _p(self.scratch),
+                                   _p(self.grad), _p(self.stats), _p(self.m), _p(self.v), self.step, lr, 0.9, 0.999, 1e-8,
+                                   *tail, self._stream())
+        if rc < 0:
+            self._check(rc, fn)
+        self.step += rc
         return rc
 
     def policy_grad_exchange(self, comm, mode, flat, data, n, hp, inv_n, stat_scale):
         """One gradient over n local samples, summed over the ranks through peer memory into self.grad (A2C)."""
-        obs, mask, act, logp, logits, val, adv, target = data
         G = max(1, min((n + 3) // 4, self.sms))
-        rc = self.lib.r4_policy_grad_partial(mode, _p(flat), _p(obs), _p(mask), _p(act), _p(logp), _p(logits), _p(val), _p(adv),
-                                             _p(target), C.c_void_p(0), n, self.A, hp["clip"], hp["vf_clip"], hp["vf_coeff"],
-                                             hp["kl_coeff"], hp["ent_coeff"], inv_n, _p(self.scratch), G, self._stream())
+        rc = self.lib.r4_policy_grad_partial(mode, _p(flat), *map(_p, data), C.c_void_p(0), n, self.A, *_hp(hp), inv_n,
+                                             _p(self.scratch), G, self._stream())
         self._check(rc, "r4_policy_grad_partial")
-        rc = self.lib.r4_grad_exchange(comm.h, _p(self.scratch), G, self.A, _p(self.grad), _p(self.stats), stat_scale, self._stream())
-        self._check(rc, "r4_grad_exchange")
+        self._exchange(comm, self.scratch, G, stat_scale)
         self.launches += 2
+
+    def _exchange(self, comm, partial, G, stat_scale):
+        """self.grad = the sum over the ranks of this rank's G partial gradients in `partial` (then their statistics)."""
+        rc = self.lib.r4_grad_exchange_n(comm.h, _p(partial), G, self.n, _p(self.grad), _p(self.stats), stat_scale,
+                                         self._stream())
+        self._check(rc, "r4_grad_exchange_n")
 
     def gae(self, reward, value, gamma, lam):
         """-> (target, adv) of a [T, B] rollout in one launch (r4_gae)."""
@@ -127,6 +142,60 @@ class KernelOps(object):
                                    1e-8, grad_scale, float(clip or 0.0), _p(self.norm), self._stream())
         self._check(rc, "r4_adam_step")
         self.launches += 2 if clip else 1
+
+
+class GaussKernelOps(KernelOps):
+    """ctypes front of the Gaussian-policy kernels (include/rl4rs_b200.h: r4_gauss_*), with KernelOps's methods, so the
+    same learner drives either; `data` is (obs, action, logp, dist_inputs, value, adv, target)."""
+
+    def __init__(self, D, device, n_params):
+        self.D = D
+        self._init(device, n_params)
+        # one rank's gradient + statistics, the partial r4_grad_exchange_n sums (A2C)
+        self.gsum = torch.zeros(n_params + 5, dtype=torch.float32, device=device)
+
+    def _num_params(self):
+        return self.lib.r4_gauss_num_params(self.D)
+
+    def _scratch_floats(self):
+        return self.lib.r4_gauss_scratch_size(self.D)
+
+    def act(self, flat, obs, explore, seed, action, env_action, logp, value, dist_inputs):
+        n = obs.shape[0]
+        rc = self.lib.r4_gauss_act(_p(flat), _p(obs), n, self.D, int(bool(explore)), seed, self.counter, _p(action),
+                                   _p(env_action), _p(logp), _p(value), _p(dist_inputs), self._stream())
+        self._check(rc, "r4_gauss_act")
+        self.counter += n
+        self.launches += 1
+
+    def _chunks(self, n):
+        return 2 * -(-n // 2048)         # k_gauss_rows + k_gauss_wgrad per chunk of 2048 samples (r4_gauss.cuh: CH)
+
+    def policy_grad(self, mode, flat, data, idx, idx_offset, n, hp, inv_n, stat_scale, grad=None, stats=None):
+        grad = self.grad if grad is None else grad
+        stats = self.stats if stats is None else stats
+        rc = self.lib.r4_gauss_grad(mode, _p(flat), *map(_p, data), _p(idx, idx_offset * 8), n, self.D, *_hp(hp), inv_n,
+                                    _p(self.scratch), _p(grad), _p(stats), stat_scale, self._stream())
+        self._check(rc, "r4_gauss_grad")
+        self.launches += self._chunks(n)
+
+    def ppo_epoch(self, flat, data, perm, n, mb, hp, lr, clip):
+        rc = self._epoch("r4_gauss_ppo_epoch", (), self.D, flat, data, perm, n, mb, hp, lr, (float(clip or 0.0), _p(self.norm)))
+        self.launches += rc * (self._chunks(mb) + (2 if clip else 1))
+        return rc
+
+    def ppo_epoch_dist(self, comm, flat, data, perm, n, mb_local, hp, lr):
+        rc = self._epoch("r4_gauss_ppo_epoch_dist", (comm.h,), self.D, flat, data, perm, n, mb_local, hp, lr, ())
+        self.launches += rc * (self._chunks(mb_local) + 1)
+        return rc
+
+    def policy_grad_exchange(self, comm, mode, flat, data, n, hp, inv_n, stat_scale):
+        """One gradient over n local samples, summed over the ranks through peer memory into self.grad (A2C)."""
+        self.gsum[self.n:].zero_()
+        self.policy_grad(mode, flat, data, None, 0, n, hp, inv_n, 1.0, grad=self.gsum[:self.n], stats=self.gsum[self.n:])
+        self._exchange(comm, self.gsum, 1, stat_scale)
+        self.launches += 1
+
 
 class PeerComm(object):
     """The learner's gradient exchange over NVLink peer memory (include/rl4rs_b200.h: r4_comm_*).  Every rank exports
@@ -185,7 +254,7 @@ def _world():
 
 
 class RolloutBuffer(object):
-    """[T, B, ...] device-resident sample batch of one vector episode."""
+    """[T, B, ...] device-resident sample batch of one vector episode of the mask policy."""
 
     def __init__(self, T, B, A, device, obs_dim=256):
         z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=device)
@@ -193,6 +262,25 @@ class RolloutBuffer(object):
         self.action, self.logp, self.value = z(T, B, dt=torch.int64), z(T, B), z(T, B)
         self.logits, self.reward = z(T, B, A), z(T, B)
         self.T, self.B = T, B
+
+    def observe(self, t, obs, mask):
+        """Stores the policy inputs of step t -> the stored copies."""
+        self.obs[t].copy_(obs); self.mask[t].copy_(mask)
+        return self.obs[t], self.mask[t]
+
+    def _flat(self, *cols):
+        n = self.T * self.B
+        return tuple(x.reshape((n,) + x.shape[2:]) for x in cols)
+
+    def columns(self):
+        """The rollout as flat [n, ...] columns: the policy inputs, action, logp, dist inputs, value -- the order in which the
+        losses and the gradient entry points take them before (adv, target)."""
+        return self._flat(self.obs, self.mask, self.action, self.logp, self.logits, self.value)
+
+    def a2c_columns(self):
+        """columns() with what the A2C gradient does not read left out (r4_policy_grad reads the logits in every mode)."""
+        obs, mask, action, _, logits, _ = self.columns()
+        return obs, mask, action, None, logits, None
 
     def returns_and_advantages(self, gamma, lam):
         """GAE (RLlib compute_advantages, complete episodes => bootstrap value 0)."""
@@ -207,12 +295,36 @@ class RolloutBuffer(object):
         return adv + self.value, adv
 
 
+class GaussRolloutBuffer(RolloutBuffer):
+    """[T, B, ...] device-resident sample batch of the continuous-action env: the unclipped action, the dist inputs
+    (mean | log_std, RLlib's stored 'action_dist_inputs'), no mask and no logits."""
+
+    def __init__(self, T, B, D, device, obs_dim=256):
+        z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=device)
+        self.obs, self.action, self.dist = z(T, B, obs_dim), z(T, B, D), z(T, B, 2 * D)
+        self.logp, self.value, self.reward = z(T, B), z(T, B), z(T, B)
+        self.T, self.B = T, B
+
+    def observe(self, t, obs):
+        self.obs[t].copy_(obs)
+        return (self.obs[t],)
+
+    def columns(self):
+        return self._flat(self.obs, self.action, self.logp, self.dist, self.value)
+
+    def a2c_columns(self):
+        """No dist inputs: with them r4_gauss_grad would add a KL pass that A2C does not use."""
+        obs, action = self.columns()[:2]
+        return obs, action, None, None, None
+
+
 class _TrainerBase(object):
     algo = None
+    conti = False          # True: the Gaussian policy of the continuous-action env (PPO_conti / A2C_conti)
 
     def __init__(self, config, env, device=None, seed=0):
-        """config: RLlib-style hyper-parameter dict (unknown keys ignored); env: a RecEnvBase built
-        with output_format='torch' and support_rllib_mask=True (or any object with that protocol)."""
+        """config: RLlib-style hyper-parameter dict (unknown keys ignored); env: a RecEnvBase built with output_format='torch'
+        and support_rllib_mask=True, or with support_conti_env=True for the Gaussian policy (or any object with that protocol)."""
         self.config = dict(self.DEFAULTS, **{k: v for k, v in (config or {}).items() if k in self.DEFAULTS})
         self.env = env
         self.T = env.config["max_steps"]
@@ -221,42 +333,57 @@ class _TrainerBase(object):
         self.device = torch.device(device) if device is not None else env.sim.engine.device
         # `*_rawstate` algorithms / rawstate_as_obs (modelfree_train.py:218,235-240,270,287-298): the policy embeds the raw
         # state itself ('mask_model_rawstate'); that twin is plain torch + autograd, the kernels serve the 256-d obs policy
-        self.rawstate = bool(env.config.get("rawstate_as_obs", False))
-        if self.rawstate:
-            self.policy = RawStatePolicy(self.A, self.device, seed=seed, config=env.config)
+        self.rawstate = not self.conti and bool(env.config.get("rawstate_as_obs", False))
+        # same init on every rank; _env_action is what the act kernel hands the env: the sampled index, or clip(a, -1, 1)
+        if self.conti:
+            self.D = env.config.get("action_emb_size", 32)
+            self.policy = GaussianPolicy(self.D, self.device, seed=seed)
+            self.buf = GaussRolloutBuffer(self.T, self.B, self.D, self.device)
+            self._env_action = torch.zeros(self.B, self.D, dtype=torch.float32, device=self.device)
         else:
-            self.policy = MaskedPolicy(self.A, self.device, seed=seed)     # same init on every rank
+            if self.rawstate:
+                self.policy = RawStatePolicy(self.A, self.device, seed=seed, config=env.config)
+            else:
+                self.policy = MaskedPolicy(self.A, self.device, seed=seed)
+            self.buf = RolloutBuffer(self.T, self.B, self.A, self.device, obs_dim=self.policy.obs_dim if self.rawstate else 256)
+            self._env_action = torch.zeros(self.B, dtype=torch.int32, device=self.device)
         self.use_kernels = self.device.type == "cuda" and (config or {}).get("use_kernels", True) and not self.rawstate
         self.opt = torch.optim.Adam([self.policy.flat], lr=self.config["lr"])
-        self.ops = KernelOps(self.A, self.device, self.policy.n_params) if self.use_kernels else None
+        self.ops = None
+        if self.use_kernels:
+            self.ops = (GaussKernelOps(self.D, self.device, self.policy.n_params) if self.conti
+                        else KernelOps(self.A, self.device, self.policy.n_params))
         self.comm = PeerComm(self.policy.n_params, self.device) if self.use_kernels else None
-        self._act_i32 = torch.zeros(self.B, dtype=torch.int32, device=self.device)
         # shared `seed` for the parameter init and the minibatch permutation; the exploration noise is per rank
         # (k_policy_act hashes seed ^ counter+row: the same seed would give rank r row i the noise of rank 0 row i)
         rank = dist.get_rank() if dist.is_available() and dist.is_initialized() else 0
         self._seed = (seed * 1000003 + rank) & 0x7fffffffffffffff
         if rank and not self.use_kernels:
             torch.manual_seed(seed * 1000003 + rank)
-        self.buf = RolloutBuffer(self.T, self.B, self.A, self.device, obs_dim=self.policy.obs_dim if self.rawstate else 256)
         self.iteration = 0
         self.timesteps_total = 0
 
     # ---- rollout ------------------------------------------------------------------------------
     @torch.no_grad()
     def rollout(self, explore=True):
-        env, buf = self.env, self.buf
+        env, buf, flat = self.env, self.buf, self.policy.flat
         obs = env.reset()
         for t in range(self.T):
-            buf.obs[t].copy_(self.policy.pack(obs) if self.rawstate else obs["obs"]); buf.mask[t].copy_(obs["action_mask"])
+            inputs = buf.observe(t, *self.policy.inputs(obs))
             if self.use_kernels:       # forward + sampling in ONE kernel, written straight into the rollout buffers
-                a = self._act_i32
-                self.ops.act(self.policy.flat, buf.obs[t], buf.mask[t], explore, self._seed, a,
-                             buf.logp[t], buf.value[t], buf.logits[t])
-                buf.action[t].copy_(a)
+                a = self._env_action
+                if self.conti:
+                    self.ops.act(flat, *inputs, explore, self._seed, buf.action[t], a, buf.logp[t], buf.value[t], buf.dist[t])
+                else:
+                    self.ops.act(flat, *inputs, explore, self._seed, a, buf.logp[t], buf.value[t], buf.logits[t])
+                    buf.action[t].copy_(a)
+            elif self.conti:
+                sample, a, logp, value, d = self.policy.act(*inputs, explore=explore)
+                buf.action[t].copy_(sample); buf.logp[t].copy_(logp); buf.value[t].copy_(value); buf.dist[t].copy_(d)
             else:
-                a, logp, value, logits = self.policy.act(buf.obs[t], obs["action_mask"], explore=explore)
+                a, logp, value, logits = self.policy.act(*inputs, explore=explore)
                 buf.action[t].copy_(a); buf.logp[t].copy_(logp); buf.value[t].copy_(value); buf.logits[t].copy_(logits)
-            obs, reward, done, info = env.step(a)
+            obs, reward, done, info = env.step(a)      # clip_actions: the env gets clip(a, -1, 1), the buffer keeps a
             buf.reward[t].copy_(reward)
         self.final_step = (obs, done)          # what the episode's last step returned
         return buf
@@ -314,26 +441,33 @@ class _TrainerBase(object):
 
     @torch.no_grad()
     def compute_actions(self, obs, explore=False):
-        """trainer.compute_actions (modelfree_train.py:454): obs = {'obs': [n,256], 'action_mask': [n,A]}
-        (arrays or tensors) or RLlib's {i: {'obs':..,'action_mask':..}} dict."""
+        """trainer.compute_actions (modelfree_train.py:454): one batch of observations in the env's format (arrays or
+        tensors), or RLlib's {env_id: observation} dict -> the actions: i32 [n] of the mask policy, clipped f32 [n, D] of the
+        Gaussian policy (a dict keyed like the input for the RLlib form)."""
         import numpy as np
-        if isinstance(obs, dict) and "action_mask" not in obs:      # RLlib's {env_id: observation} form
+        if isinstance(obs, dict) and not {"obs", "action_mask"} & obs.keys():      # RLlib's {env_id: observation} form
             keys = list(obs.keys())
-            fields = [f for f in obs[keys[0]]]
-            a = self.compute_actions({f: np.stack([np.asarray(obs[k][f]) for k in keys]) for f in fields}, explore)
-            return dict(zip(keys, a.tolist()))
-        if self.rawstate:
-            o = self.policy.pack({k: torch.as_tensor(obs[k], device=self.device) for k in ("category_feature", "dense_feature", "sequence_feature")})
+            rows = [obs[k] for k in keys]
+            if isinstance(rows[0], dict):
+                a = self.compute_actions({f: np.stack([np.asarray(r[f]) for r in rows]) for f in rows[0]}, explore)
+            else:
+                a = self.compute_actions(np.stack([np.asarray(r) for r in rows]), explore)
+            return dict(zip(keys, a.tolist() if a.ndim == 1 else list(a)))
+        if isinstance(obs, dict):
+            obs = {k: torch.as_tensor(v, device=self.device) for k, v in obs.items()}
+        o, *mask = self.policy.inputs(obs)
+        o = torch.as_tensor(o, dtype=torch.float32, device=self.device).contiguous()
+        mask = [m.to(torch.uint8).contiguous() for m in mask]
+        n = o.shape[0]
+        e = lambda *s: torch.empty(*s, dtype=torch.float32, device=self.device)
+        if not self.use_kernels:
+            a = self.policy.act(o, *mask, explore=explore)[1 if self.conti else 0]
+        elif self.conti:
+            a = e(n, self.D)
+            self.ops.act(self.policy.flat, o, explore, self._seed, e(n, self.D), a, e(n), e(n), None)
         else:
-            o = torch.as_tensor(obs["obs"], dtype=torch.float32, device=self.device).contiguous()
-        m = torch.as_tensor(obs["action_mask"], device=self.device)
-        if self.use_kernels:
-            n = o.shape[0]
             a = torch.empty(n, dtype=torch.int32, device=self.device)
-            lp, v = torch.empty(n, device=self.device), torch.empty(n, device=self.device)
-            self.ops.act(self.policy.flat, o, m.to(torch.uint8).contiguous(), explore, self._seed, a, lp, v, None)
-            return a.cpu().numpy()
-        a, _, _, _ = self.policy.act(o, m, explore=explore)
+            self.ops.act(self.policy.flat, o, *mask, explore, self._seed, a, e(n), e(n), None)
         return a.cpu().numpy()
 
     # ---- checkpoint / resume (trainer.save / restore, modelfree_train.py:421-435) -----------------
@@ -377,16 +511,13 @@ class PPOTrainer(_TrainerBase):
         # minibatch permutations are drawn on the device the rollout lives on (a CPU randperm + copy stalled the GPU ~1 ms per epoch)
         self._gen = torch.Generator(device=self.device if self.device.type == "cuda" else "cpu").manual_seed(seed)
 
-    def loss(self, obs, mask, action, old_logp, old_logits, old_value, adv, target):
-        """RLlib 1.5 ppo_surrogate_loss."""
+    def loss(self, *args):
+        """RLlib 1.5 ppo_surrogate_loss: loss(*inputs, action, old_logp, old_dist, old_value, adv, target), where inputs are
+        the policy's forward() inputs and old_dist its stored dist inputs."""
+        *inputs, action, old_logp, old_dist, old_value, adv, target = args
         c = self.config
-        logits, value = self.policy.forward(obs, mask)
-        logp_all = torch.log_softmax(logits, -1)
-        logp = logp_all.gather(1, action.unsqueeze(1)).squeeze(1)
-        old_logp_all = torch.log_softmax(old_logits, -1)
-        p_old = old_logp_all.exp()
-        kl = (p_old * (old_logp_all - logp_all)).sum(-1)
-        entropy = -(logp_all.exp() * logp_all).sum(-1)
+        d, value = self.policy.forward(*inputs)
+        logp, kl, entropy = self.policy.terms(d, action, old_dist)
         ratio = torch.exp(logp - old_logp)
         surr = torch.min(adv * ratio, adv * torch.clamp(ratio, 1 - c["clip_param"], 1 + c["clip_param"]))
         vf1 = (value - target) ** 2
@@ -394,12 +525,6 @@ class PPOTrainer(_TrainerBase):
         vf = torch.max(vf1, (vclip - target) ** 2)
         total = (-surr + self.kl_coeff * kl + c["vf_loss_coeff"] * vf - c["entropy_coeff"] * entropy).mean()
         return total, {"policy_loss": (-surr).mean(), "vf_loss": vf.mean(), "kl": kl.mean(), "entropy": entropy.mean()}
-
-    def _columns(self, buf):
-        """The rollout as flat [n, ...] columns, in the order loss() takes them before (adv, target)."""
-        n = buf.T * buf.B
-        flat = lambda x: x.reshape((n,) + x.shape[2:])
-        return (flat(buf.obs), flat(buf.mask), flat(buf.action), flat(buf.logp), flat(buf.logits), flat(buf.value))
 
     def learn(self, buf):
         c = self.config
@@ -414,7 +539,7 @@ class PPOTrainer(_TrainerBase):
         # RLlib: sgd_minibatch_size is the TOTAL over devices; every rank contributes sgd_minibatch_size / world samples
         # of its own shard to each SGD step (multi-GPU tower semantics) and the loss is the mean over all of them
         mb = min(max(c["sgd_minibatch_size"] // _world(), 1), n)
-        data = self._columns(buf) + (adv, target)
+        data = buf.columns() + (adv, target)
         agg, steps = (self._sgd_kernels if self.use_kernels else self._sgd_eager)(data, n, mb)
         named = {k: v / max(steps, 1) for k, v in agg.items()}
         named["_episode_reward_mean"] = buf.reward.sum(0).mean()
@@ -495,15 +620,15 @@ class A2CTrainer(_TrainerBase):
     algo = "A2C"
     DEFAULTS = A2C_DEFAULTS
 
-    def loss(self, obs, mask, action, adv, target):
-        """RLlib 1.5 A3CLoss: summed terms."""
+    def loss(self, *args):
+        """RLlib 1.5 A3CLoss, summed terms: loss(*inputs, action, adv, target)."""
+        *inputs, action, adv, target = args
         c = self.config
-        logits, value = self.policy.forward(obs, mask)
-        logp_all = torch.log_softmax(logits, -1)
-        logp = logp_all.gather(1, action.unsqueeze(1)).squeeze(1)
+        d, value = self.policy.forward(*inputs)
+        logp, _, entropy = self.policy.terms(d, action)
         pi_loss = -(logp * adv).sum()
         vf_loss = 0.5 * ((value - target) ** 2).sum()
-        entropy = -(logp_all.exp() * logp_all).sum()
+        entropy = entropy.sum()
         total = pi_loss + c["vf_loss_coeff"] * vf_loss - c["entropy_coeff"] * entropy
         return total, {"policy_loss": pi_loss, "vf_loss": vf_loss, "entropy": entropy}
 
@@ -511,250 +636,11 @@ class A2CTrainer(_TrainerBase):
         c = self.config
         target, adv = self._gae(buf)
         n = buf.T * buf.B
-        flat = lambda x: x.reshape((n,) + x.shape[2:])
-        if self.use_kernels:
-            ops, w = self.ops, _world()
-            data = (flat(buf.obs), flat(buf.mask), flat(buf.action), None, flat(buf.logits), None,
-                    flat(adv).contiguous(), flat(target).contiguous())
-            hp = {"clip": 0.0, "vf_clip": 0.0, "vf_coeff": c["vf_loss_coeff"], "kl_coeff": 0.0, "ent_coeff": c["entropy_coeff"]}
-            ops.stats.zero_()
-            if w > 1 and self.comm is not None and self.comm.ok:
-                ops.policy_grad_exchange(self.comm, 1, self.policy.flat, data, n, hp, 1.0, 1.0)   # summed over the ranks
-            else:
-                ops.policy_grad(1, self.policy.flat, data, None, 0, n, hp, 1.0, 1.0)
-                if w > 1:
-                    dist.all_reduce(ops.grad, op=dist.ReduceOp.SUM)            # summed loss over the global batch
-            gn = ops.grad.norm()
-            ops.adam(self.policy.flat, c["lr"], 1.0, c["grad_clip"])
-            st = ops.stats
-            g = self._global_means({"policy_loss": st[0], "vf_loss": st[1], "entropy": st[3], "total_loss": st[4], "gn": gn,
-                                    "_episode_reward_mean": buf.reward.sum(0).mean()})
-            return {"policy_loss": g["policy_loss"] * w, "vf_loss": g["vf_loss"] * w, "entropy": g["entropy"] * w,
-                    "total_loss": g["total_loss"] * w, "grad_gnorm": g["gn"], "sgd_steps": 1,
-                    "_episode_reward_mean": g["_episode_reward_mean"]}
-        if self.policy.flat.grad is not None:
-            self.policy.flat.grad.zero_()
-        total, st = self.loss(flat(buf.obs), flat(buf.mask), flat(buf.action), flat(adv), flat(target))
-        total.backward()
-        self._allreduce_grad(average=False)          # summed loss over the global batch
-        gn = torch.nn.utils.clip_grad_norm_([self.policy.flat], c["grad_clip"]) if c["grad_clip"] else torch.zeros(())
-        self.opt.step()
-        out = {k: self._global_mean(v) * _world() for k, v in st.items()}
-        out.update({"total_loss": self._global_mean(total) * _world(), "grad_gnorm": float(gn), "sgd_steps": 1})
-        return out
-
-
-# ---- the continuous-action env: Gaussian policy (PPO_conti / A2C_conti) ------------------------------------------------
-class GaussKernelOps(KernelOps):
-    """ctypes front of the Gaussian-policy kernels (include/rl4rs_b200.h: r4_gauss_*).  Same method names and signatures as
-    KernelOps, so PPOTrainer._sgd_kernels drives either; `data` is (obs, action, logp, dist_inputs, value, adv, target)."""
-
-    def __init__(self, D, device, n_params):
-        from . import _capi
-        self.capi = _capi
-        self.lib = _capi.load_library()
-        self.A = self.D = D
-        self.device, self.n = device, n_params
-        assert self.lib.r4_gauss_num_params(D) == n_params
-        z = lambda k: torch.zeros(k, dtype=torch.float32, device=device)
-        self.m, self.v, self.grad, self.stats, self.norm = z(n_params), z(n_params), z(n_params), z(5), z(1)
-        self.gsum = z(n_params + 5)      # one rank's gradient + statistics, the partial r4_grad_exchange_n sums (A2C)
-        self.scratch = z(self.lib.r4_gauss_scratch_size(D))
-        self.step = 0
-        self.counter = 0
-        self.launches = 0
-
-    def act(self, flat, obs, explore, seed, action, env_action, logp, value, dist_inputs):
-        n = obs.shape[0]
-        rc = self.lib.r4_gauss_act(_p(flat), _p(obs), n, self.D, int(bool(explore)), seed, self.counter, _p(action),
-                                   _p(env_action), _p(logp), _p(value), _p(dist_inputs), self._stream())
-        self._check(rc, "r4_gauss_act")
-        self.counter += n
-        self.launches += 1
-
-    def _chunks(self, n):
-        return 2 * -(-n // 2048)         # k_gauss_rows + k_gauss_wgrad per chunk of 2048 samples (r4_gauss.cuh: CH)
-
-    def policy_grad(self, mode, flat, data, idx, idx_offset, n, hp, inv_n, stat_scale, grad=None, stats=None):
-        obs, act, logp, dist_inputs, val, adv, target = data
-        grad = self.grad if grad is None else grad
-        stats = self.stats if stats is None else stats
-        rc = self.lib.r4_gauss_grad(mode, _p(flat), _p(obs), _p(act), _p(logp), _p(dist_inputs), _p(val), _p(adv), _p(target),
-                                    _p(idx, idx_offset * 8) if idx is not None else C.c_void_p(0), n, self.D, hp["clip"],
-                                    hp["vf_clip"], hp["vf_coeff"], hp["kl_coeff"], hp["ent_coeff"], inv_n, _p(self.scratch),
-                                    _p(grad), _p(stats), stat_scale, self._stream())
-        self._check(rc, "r4_gauss_grad")
-        self.launches += self._chunks(n)
-
-    def ppo_epoch(self, flat, data, perm, n, mb, hp, lr, clip):
-        obs, act, logp, dist_inputs, val, adv, target = data
-        rc = self.lib.r4_gauss_ppo_epoch(_p(flat), _p(obs), _p(act), _p(logp), _p(dist_inputs), _p(val), _p(adv), _p(target),
-                                         _p(perm), n, mb, self.D, hp["clip"], hp["vf_clip"], hp["vf_coeff"], hp["kl_coeff"],
-                                         hp["ent_coeff"], _p(self.scratch), _p(self.grad), _p(self.stats), _p(self.m),
-                                         _p(self.v), self.step, lr, 0.9, 0.999, 1e-8, float(clip or 0.0), _p(self.norm),
-                                         self._stream())
-        if rc < 0:
-            self._check(rc, "r4_gauss_ppo_epoch")
-        self.step += rc
-        self.launches += rc * (self._chunks(mb) + (2 if clip else 1))
-        return rc
-
-    def ppo_epoch_dist(self, comm, flat, data, perm, n, mb_local, hp, lr):
-        obs, act, logp, dist_inputs, val, adv, target = data
-        rc = self.lib.r4_gauss_ppo_epoch_dist(comm.h, _p(flat), _p(obs), _p(act), _p(logp), _p(dist_inputs), _p(val), _p(adv),
-                                              _p(target), _p(perm), n, mb_local, self.D, hp["clip"], hp["vf_clip"],
-                                              hp["vf_coeff"], hp["kl_coeff"], hp["ent_coeff"], _p(self.scratch), _p(self.grad),
-                                              _p(self.stats), _p(self.m), _p(self.v), self.step, lr, 0.9, 0.999, 1e-8,
-                                              self._stream())
-        if rc < 0:
-            self._check(rc, "r4_gauss_ppo_epoch_dist")
-        self.step += rc
-        self.launches += rc * (self._chunks(mb_local) + 1)
-        return rc
-
-    def policy_grad_exchange(self, comm, mode, flat, data, n, hp, inv_n, stat_scale):
-        """One gradient over n local samples, summed over the ranks through peer memory into self.grad (A2C)."""
-        self.gsum[self.n:].zero_()
-        self.policy_grad(mode, flat, data, None, 0, n, hp, inv_n, 1.0, grad=self.gsum[:self.n], stats=self.gsum[self.n:])
-        rc = self.lib.r4_grad_exchange_n(comm.h, _p(self.gsum), 1, self.n, _p(self.grad), _p(self.stats), stat_scale,
-                                         self._stream())
-        self._check(rc, "r4_grad_exchange_n")
-        self.launches += 1
-
-
-class GaussRolloutBuffer(RolloutBuffer):
-    """[T, B, ...] device-resident sample batch of the continuous-action env: the unclipped action, the dist inputs
-    (mean | log_std, RLlib's stored 'action_dist_inputs'), no mask and no logits."""
-
-    def __init__(self, T, B, D, device, obs_dim=256):
-        z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=device)
-        self.obs, self.action, self.dist = z(T, B, obs_dim), z(T, B, D), z(T, B, 2 * D)
-        self.logp, self.value, self.reward = z(T, B), z(T, B), z(T, B)
-        self.T, self.B = T, B
-
-
-class _GaussMixin(object):
-    """Set-up, rollout and compute_actions of the Gaussian-policy trainers; train / evaluate / save / restore / GAE come from
-    _TrainerBase unchanged."""
-
-    def _setup(self, config, env, device, seed):
-        self.config = dict(self.DEFAULTS, **{k: v for k, v in (config or {}).items() if k in self.DEFAULTS})
-        self.env = env
-        self.T = env.config["max_steps"]
-        self.B = env.config["batch_size"]
-        self.D = env.config.get("action_emb_size", 32)
-        self.device = torch.device(device) if device is not None else env.sim.engine.device
-        self.rawstate = False
-        self.policy = GaussianPolicy(self.D, self.device, seed=seed)     # same init on every rank
-        self.use_kernels = self.device.type == "cuda" and (config or {}).get("use_kernels", True)
-        self.opt = torch.optim.Adam([self.policy.flat], lr=self.config["lr"])
-        self.ops = GaussKernelOps(self.D, self.device, self.policy.n_params) if self.use_kernels else None
-        self.comm = PeerComm(self.policy.n_params, self.device) if self.use_kernels else None
-        rank = dist.get_rank() if dist.is_available() and dist.is_initialized() else 0
-        self._seed = (seed * 1000003 + rank) & 0x7fffffffffffffff       # per-rank exploration noise (see _TrainerBase)
-        if rank and not self.use_kernels:
-            torch.manual_seed(seed * 1000003 + rank)
-        self.buf = GaussRolloutBuffer(self.T, self.B, self.D, self.device)
-        self._env_act = torch.zeros(self.B, self.D, dtype=torch.float32, device=self.device)
-        self.iteration = 0
-        self.timesteps_total = 0
-
-    @torch.no_grad()
-    def rollout(self, explore=True):
-        env, buf = self.env, self.buf
-        obs = env.reset()
-        for t in range(self.T):
-            buf.obs[t].copy_(obs["obs"] if isinstance(obs, dict) else obs)
-            if self.use_kernels:       # forward + sampling + clipping in ONE kernel, written straight into the rollout buffers
-                ea = self._env_act
-                self.ops.act(self.policy.flat, buf.obs[t], explore, self._seed, buf.action[t], ea, buf.logp[t], buf.value[t],
-                             buf.dist[t])
-            else:
-                a, ea, logp, value, d = self.policy.act(buf.obs[t], explore=explore)
-                buf.action[t].copy_(a); buf.logp[t].copy_(logp); buf.value[t].copy_(value); buf.dist[t].copy_(d)
-            obs, reward, done, info = env.step(ea)          # clip_actions: the env gets clip(a, -1, 1), the buffer keeps a
-            buf.reward[t].copy_(reward)
-        self.final_step = (obs, done)
-        return buf
-
-    @torch.no_grad()
-    def compute_actions(self, obs, explore=False):
-        """trainer.compute_actions: obs f32 [n,256] (array or tensor, or {'obs': ...}) or RLlib's {i: observation} dict
-        -> clipped actions f32 [n,D] (a dict keyed like the input for the RLlib form)."""
-        import numpy as np
-        if isinstance(obs, dict) and "obs" not in obs:      # RLlib's {env_id: observation} form
-            keys = list(obs.keys())
-            rows = [np.asarray(obs[k]["obs"] if isinstance(obs[k], dict) else obs[k], dtype=np.float32) for k in keys]
-            return dict(zip(keys, list(self.compute_actions(np.stack(rows), explore))))
-        if isinstance(obs, dict):
-            obs = obs["obs"]
-        o = torch.as_tensor(obs, dtype=torch.float32, device=self.device).contiguous()
-        if self.use_kernels:
-            n = o.shape[0]
-            e = lambda *s: torch.empty(*s, dtype=torch.float32, device=self.device)
-            ea = e(n, self.D)
-            self.ops.act(self.policy.flat, o, explore, self._seed, e(n, self.D), ea, e(n), e(n), None)
-            return ea.cpu().numpy()
-        return self.policy.act(o, explore=explore)[1].cpu().numpy()
-
-
-class GaussPPOTrainer(_GaussMixin, PPOTrainer):
-    """PPO_conti: RLlib 1.5 PPO over the DiagGaussian policy; the learner is PPOTrainer's (GAE, standardised advantages,
-    minibatch SGD, adaptive KL, peer-memory exchange) with the Gaussian loss and kernels."""
-    algo = "PPO_conti"
-
-    def __init__(self, config, env, device=None, seed=0):
-        self._setup(config, env, device, seed)
-        self.kl_coeff = self.config["kl_coeff"]
-        self._gen = torch.Generator(device=self.device if self.device.type == "cuda" else "cpu").manual_seed(seed)
-
-    def _columns(self, buf):
-        n = buf.T * buf.B
-        flat = lambda x: x.reshape((n,) + x.shape[2:])
-        return (flat(buf.obs), flat(buf.action), flat(buf.logp), flat(buf.dist), flat(buf.value))
-
-    def loss(self, obs, action, old_logp, old_dist, old_value, adv, target):
-        """RLlib 1.5 ppo_surrogate_loss over TorchDiagGaussian."""
-        c = self.config
-        d, value = self.policy.forward(obs)
-        logp = GaussianPolicy.logp(d, action)
-        kl = GaussianPolicy.kl(old_dist, d)
-        entropy = GaussianPolicy.entropy(d)
-        ratio = torch.exp(logp - old_logp)
-        surr = torch.min(adv * ratio, adv * torch.clamp(ratio, 1 - c["clip_param"], 1 + c["clip_param"]))
-        vf1 = (value - target) ** 2
-        vclip = old_value + torch.clamp(value - old_value, -c["vf_clip_param"], c["vf_clip_param"])
-        vf = torch.max(vf1, (vclip - target) ** 2)
-        total = (-surr + self.kl_coeff * kl + c["vf_loss_coeff"] * vf - c["entropy_coeff"] * entropy).mean()
-        return total, {"policy_loss": (-surr).mean(), "vf_loss": vf.mean(), "kl": kl.mean(), "entropy": entropy.mean()}
-
-
-class GaussA2CTrainer(_GaussMixin, A2CTrainer):
-    """A2C_conti: RLlib 1.5 A3C loss (summed) over the DiagGaussian policy, one gradient step per iteration."""
-    algo = "A2C_conti"
-
-    def __init__(self, config, env, device=None, seed=0):
-        self._setup(config, env, device, seed)
-
-    def loss(self, obs, action, adv, target):
-        c = self.config
-        d, value = self.policy.forward(obs)
-        pi_loss = -(GaussianPolicy.logp(d, action) * adv).sum()
-        vf_loss = 0.5 * ((value - target) ** 2).sum()
-        entropy = GaussianPolicy.entropy(d).sum()
-        total = pi_loss + c["vf_loss_coeff"] * vf_loss - c["entropy_coeff"] * entropy
-        return total, {"policy_loss": pi_loss, "vf_loss": vf_loss, "entropy": entropy}
-
-    def learn(self, buf):
-        c = self.config
-        target, adv = self._gae(buf)
-        n = buf.T * buf.B
-        obs, act = buf.obs.reshape(n, -1), buf.action.reshape(n, -1)
         adv, target = adv.reshape(n).contiguous(), target.reshape(n).contiguous()
         w = _world()
         if self.use_kernels:
             ops = self.ops
-            data = (obs, act, None, None, None, adv, target)
+            data = buf.a2c_columns() + (adv, target)
             hp = {"clip": 0.0, "vf_clip": 0.0, "vf_coeff": c["vf_loss_coeff"], "kl_coeff": 0.0, "ent_coeff": c["entropy_coeff"]}
             ops.stats.zero_()
             if w > 1 and self.comm is not None and self.comm.ok:
@@ -773,7 +659,7 @@ class GaussA2CTrainer(_GaussMixin, A2CTrainer):
                     "_episode_reward_mean": g["_episode_reward_mean"]}
         if self.policy.flat.grad is not None:
             self.policy.flat.grad.zero_()
-        total, st = self.loss(obs, act, adv, target)
+        total, st = self.loss(*buf.columns()[:-3], adv, target)       # the policy inputs and the action
         total.backward()
         self._allreduce_grad(average=False)          # summed loss over the global batch
         gn = torch.nn.utils.clip_grad_norm_([self.policy.flat], c["grad_clip"]) if c["grad_clip"] else torch.zeros(())
@@ -781,6 +667,18 @@ class GaussA2CTrainer(_GaussMixin, A2CTrainer):
         out = {k: self._global_mean(v) * w for k, v in st.items()}
         out.update({"total_loss": self._global_mean(total) * w, "grad_gnorm": float(gn), "sgd_steps": 1})
         return out
+
+
+class GaussPPOTrainer(PPOTrainer):
+    """PPO_conti: PPOTrainer over the DiagGaussian policy of the continuous-action env."""
+    algo = "PPO_conti"
+    conti = True
+
+
+class GaussA2CTrainer(A2CTrainer):
+    """A2C_conti: A2CTrainer over the DiagGaussian policy of the continuous-action env."""
+    algo = "A2C_conti"
+    conti = True
 
 
 def get_rl_model(algo, rllib_config, env=None, **kw):
