@@ -43,9 +43,8 @@ struct SeqCache {   // one cached (sequence, weight-set): GRU-1 outputs + AUGRU/
 };
 
 struct PerSeq {
-  float *gru_wx = nullptr, *gru_bx = nullptr, *gru_wgh = nullptr, *gru_wch = nullptr;
-  float *au_wx = nullptr, *au_bx = nullptr, *au_wgh = nullptr, *au_wch = nullptr;
-  float *wqd = nullptr, *wp = nullptr, *ab1 = nullptr, *aw2 = nullptr, *ab2 = nullptr, *akv = nullptr;
+  float *gru_bx = nullptr, *au_bx = nullptr;
+  float *wqd = nullptr, *ab1 = nullptr, *aw2 = nullptr, *ab2 = nullptr, *akv = nullptr;
   uint8_t *gru_wx_img = nullptr, *au_wx_img = nullptr, *wp_img = nullptr, *gru_img = nullptr;   // pre-tiled bf16 hi/lo images of the input projections
   uint8_t* au_img = nullptr;   // the same weights as the recurrence kernel's weight stream (r4_recur.cuh)
   float abk = 0.f;
@@ -68,8 +67,8 @@ struct r4_env {
   bool items_ready = false;
   // weights
   std::map<std::string, std::vector<float>> hw;
-  float *emb_cat = nullptr, *emb_seq = nullptr, *w1 = nullptr, *b1 = nullptr, *w2 = nullptr, *b2 = nullptr;
-  float *wo = nullptr, *bo = nullptr, *wr = nullptr, *br = nullptr;
+  float *emb_cat = nullptr, *emb_seq = nullptr, *b1 = nullptr, *b2 = nullptr;
+  float *bo = nullptr, *wr = nullptr, *br = nullptr;
   uint8_t *w1_img = nullptr, *w2_img = nullptr, *wo_img = nullptr;   // tensor-core images (r4_gemm_tc.cuh)
   int sim = R4_SIM_DIEN;                                             // config['algo']: which simulator graph
   float* fcb = nullptr; uint8_t *fc_img = nullptr;                   // dnn: the unnamed Dense(256, ELU) of nets/dnn.py:34; widedeep: nets/widedeep.py:34
@@ -88,7 +87,6 @@ struct r4_env {
   const int32_t* log_seq = nullptr;
   const int32_t* log_items = nullptr;
   const uint8_t* log_fb = nullptr;
-  int64_t log_n = 0;
   int log_slots = 0;
   // episode state
   int32_t* row_idx = nullptr;
@@ -182,33 +180,25 @@ int upload(r4_env* e, const std::vector<T>& h, T** dptr) {
 
 inline cudaStream_t S(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
-// n-tile width of the observation-head GEMM (K = 3456, N = 256): 128 doubles its CTA count (64 at batch 4096).
-// n-tile width of the observation head's weight image.  256: every 128-row tile converts its A rows (fp32 -> bf16 hi/mid/lo,
-// the producers' work and the kernel's limiter) ONCE, and split-K (4 parts at 4096 rows: 32 tiles x 4 = 128 CTAs) fills the
-// SMs; 128 (R4_HEAD_BNT=128, the earlier default) converted every A row twice for 64 tiles x 2 K parts.
-static int head_bnt() {
-  static const int v = [] { const char* e = getenv("R4_HEAD_BNT"); int x = e ? atoi(e) : 256; return (x == 128 || x == 256) ? x : 256; }();
-  return v;
-}
-#define HEAD_BNT head_bnt()
-
+// Every weight image, and so every GEMM, uses n-tiles of r4tc::G_BNMAX = 256 columns.  For the observation head
+// (K = 3456, N = 256) that means every 128-row tile converts its A rows (fp32 -> bf16 hi/mid/lo, the producers' work and
+// the kernel's limiter) ONCE, and split-K (4 parts at 4096 rows: 32 tiles x 4 = 128 CTAs) fills the SMs; 128-column
+// tiles (the earlier default) doubled the CTA count but converted every A row twice for 64 tiles x 2 K parts.
 int gemm(r4_env* e, int slot, int act, int M, int N, int K, const float* A, int lda, const int32_t* gather,
          const uint8_t* Wimg, const float* bias, float* C, int ldc, cudaStream_t st, int tm_ns = 0, int cr_base = 0,
-         int ldT = 0, float* outT = nullptr, float* outK = nullptr, int bnt = r4tc::G_BNMAX,
+         int ldT = 0, float* outT = nullptr, float* outK = nullptr,
          const float* A2 = nullptr, const int32_t* gather2 = nullptr, int k2_start = 0, int g2_n = 0, int tm_steps = MAXLEN,
          int ksplit_max = 1) {
   if (M <= 0) return R4_OK;
   if ((N & 15) || (K & 7) || (lda & 3) || (ldc & 3)) return fail(e, R4_ERR_ARG, "gemm: unaligned shape");
   ProfScope ps(e, slot, st, 2.0 * M * N * K);
   r4tc::GemmTcParams p{A, lda, gather, Wimg, bias, C, ldc, M, N, K, act, tm_ns, cr_base, ldT, outT, outK};
-  p.bnt = bnt;
   p.A2 = A2; p.gather2 = gather2; p.k2_start = k2_start; p.g2_n = g2_n;
   p.tm_steps = tm_steps;
   const int sms = sm_count();
-  int tiles = ((M + r4tc::G_BM - 1) / r4tc::G_BM) * ((N + bnt - 1) / bnt);
+  int tiles = ((M + r4tc::G_BM - 1) / r4tc::G_BM) * ((N + r4tc::G_BNMAX - 1) / r4tc::G_BNMAX);
   // split-K when the output tiles leave SMs idle and K is long (each part keeps >= 16 K blocks): the head at 4096 rows
-  static const bool no_splitk = getenv("R4_NO_SPLITK") != nullptr;
-  const int ksplit = no_splitk ? 1 : std::max(1, std::min(std::min(ksplit_max, sms / std::max(tiles, 1)), K / (16 * r4tc::G_BK)));
+  const int ksplit = std::max(1, std::min(std::min(ksplit_max, sms / std::max(tiles, 1)), K / (16 * r4tc::G_BK)));
   if (ksplit > 1) {
     if (tm_ns > 0 || !C || (N & 3)) return fail(e, R4_ERR_ARG, "gemm: split-K needs a plain row-major output");
     int rc;
@@ -226,9 +216,9 @@ int gemm(r4_env* e, int slot, int act, int M, int N, int K, const float* A, int 
   return R4_OK;
 }
 
-int upload_image(r4_env* e, const float* W, int K, int N, uint8_t** out, int bnt = r4tc::G_BNMAX) {
-  std::vector<uint8_t> img(r4tc::gemm_image_bytes(K, N, bnt));
-  r4tc::build_gemm_image(W, K, N, img.data(), bnt);
+int upload_image(r4_env* e, const float* W, int K, int N, uint8_t** out) {
+  std::vector<uint8_t> img(r4tc::gemm_image_bytes(K, N));
+  r4tc::build_gemm_image(W, K, N, img.data());
   return upload(e, img, out);
 }
 
@@ -239,30 +229,15 @@ constexpr int SMEM_CAT = 4 * (NCAT * CAT_LD + NCAT * 24) * 4;
 int build_cache(r4_env* e, int si, const int32_t* ids, int n, SeqCache& c, cudaStream_t st) {
   int rc;
   const int TM = r4tc::TM;
-  if (e->sim == R4_SIM_LSTM) {
-    // nets/utils.py:90-92: Keras GRU over Embedding(seq_i), only the LAST state is used -> c.H is [n, 128]
-    if ((rc = reserve(e, c.H, (size_t)n * EMB * 4))) return rc;
-    c.n = n;
-    const PerSeq& w = e->ps[si];
-    const int chunk = 8192;
-    const int nsmax = std::min(n, chunk);
-    if ((rc = reserve(e, e->ws_xin, (size_t)((nsmax + TM - 1) / TM) * MAXLEN * r4tc::G1_XT_COLS * TM * 4))) return rc;
-    float* xinT = reinterpret_cast<float*>(e->ws_xin.p);
-    for (int s0 = 0; s0 < n; s0 += chunk) {
-      const int ns = std::min(chunk, n - s0);
-      if ((rc = gemm(e, SL_GEMM_XIN, 0, ns * MAXLEN, XIN_LD, EMB, e->emb_seq, EMB, ids + (size_t)s0 * MAXLEN, w.gru_wx_img,
-                     w.gru_bx, nullptr, XIN_LD, st, ns, 0, XIN_LD, xinT, nullptr))) return rc;
-      { ProfScope ps(e, SL_GRU1, st, (double)ns * MAXLEN * 2.0 * (EMB * 2 * EMB + EMB * EMB));
-        r4tc::GruTcParams gp{xinT, w.gru_img, nullptr, ns};
-        gp.hard = 1; gp.Hlast = reinterpret_cast<float*>(c.H.p) + (size_t)s0 * EMB; gp.ld_last = EMB;
-        r4tc::k_gru_tc<<<(ns + r4tc::RC_ROWS - 1) / r4tc::RC_ROWS, r4tc::RC_THREADS, r4tc::G1_SMEM_BYTES, st>>>(gp); }
-      R4_LAUNCH_CHECK(e, "k_gru_tc");
-    }
-    return R4_OK;
+  // lstm (nets/utils.py:90-92): Keras GRU over Embedding(seq_i), only the LAST state is used -> c.H is [n, 128], and
+  // there is no AUGRU / attention input projection
+  const bool last_only = e->sim == R4_SIM_LSTM;
+  const int h_steps = last_only ? 1 : MAXLEN;             // GRU states kept per sequence
+  if ((rc = reserve(e, c.H, (size_t)n * h_steps * EMB * 4))) return rc;
+  if (!last_only) {
+    if ((rc = reserve(e, c.Kp, (size_t)n * MAXLEN * AH1 * 4))) return rc;
+    if ((rc = reserve(e, c.XT, (size_t)((n + TM - 1) / TM) * MAXLEN * r4tc::XT_COLS * TM * 4))) return rc;
   }
-  if ((rc = reserve(e, c.H, (size_t)n * MAXLEN * EMB * 4))) return rc;
-  if ((rc = reserve(e, c.Kp, (size_t)n * MAXLEN * AH1 * 4))) return rc;
-  if ((rc = reserve(e, c.XT, (size_t)((n + TM - 1) / TM) * MAXLEN * r4tc::XT_COLS * TM * 4))) return rc;
   c.n = n;
   const PerSeq& w = e->ps[si];
   const int chunk = 8192;
@@ -271,14 +246,16 @@ int build_cache(r4_env* e, int si, const int32_t* ids, int n, SeqCache& c, cudaS
   float* xinT = reinterpret_cast<float*>(e->ws_xin.p);
   for (int s0 = 0; s0 < n; s0 += chunk) {
     int ns = std::min(chunk, n - s0);
-    float* Hc = reinterpret_cast<float*>(c.H.p) + (size_t)s0 * MAXLEN * EMB;
+    float* Hc = reinterpret_cast<float*>(c.H.p) + (size_t)s0 * h_steps * EMB;
     // x_t [Wgx | Wcx] + [bg | bc]: Embedding gather fused into the A operand, output in lane-major tiles
     if ((rc = gemm(e, SL_GEMM_XIN, 0, ns * MAXLEN, XIN_LD, EMB, e->emb_seq, EMB, ids + (size_t)s0 * MAXLEN, w.gru_wx_img,
                    w.gru_bx, nullptr, XIN_LD, st, ns, 0, XIN_LD, xinT, nullptr))) return rc;
     { ProfScope ps(e, SL_GRU1, st, (double)ns * MAXLEN * 2.0 * (EMB * 2 * EMB + EMB * EMB));
-      r4tc::GruTcParams gp{xinT, w.gru_img, Hc, ns};
+      r4tc::GruTcParams gp{xinT, w.gru_img, last_only ? nullptr : Hc, ns};
+      if (last_only) { gp.hard = 1; gp.Hlast = Hc; gp.ld_last = EMB; }
       r4tc::k_gru_tc<<<(ns + r4tc::RC_ROWS - 1) / r4tc::RC_ROWS, r4tc::RC_THREADS, r4tc::G1_SMEM_BYTES, st>>>(gp); }
     R4_LAUNCH_CHECK(e, "k_gru_tc");
+    if (last_only) continue;
     // H_t [Wgx | Wcx | Wk-Wd] + [bg | bc | 0]: AUGRU halves -> XT tiles, key half -> Kp
     if ((rc = gemm(e, SL_GEMM_XK, 0, ns * MAXLEN, XK_LD, EMB, Hc, EMB, nullptr, w.au_wx_img, w.au_bx, nullptr, XK_LD, st,
                    ns, s0, r4tc::XT_COLS, reinterpret_cast<float*>(c.XT.p), reinterpret_cast<float*>(c.Kp.p)))) return rc;
@@ -326,6 +303,11 @@ int forward_rows(r4_env* e, int R, int row0, int div, const int32_t* cat, const 
                  const SeqCache& c0, int shared0, const SeqCache& c1, int shared1, float* obs_out,
                  float* p1_out, float* probs_out, cudaStream_t st) {
   int rc;
+  float* obs = obs_out;                                     // simulator_obs [R, obs_dim]
+  if (!obs) {
+    if ((rc = reserve(e, e->ws_obs, (size_t)R * e->obs_dim * 4))) return rc;
+    obs = reinterpret_cast<float*>(e->ws_obs.p);
+  }
   if (e->sim == R4_SIM_LSTM) {
     // nets/lstm.py:29-36: all = [GRU(seq0) | GRU(seq1) | dense tower | GRU(E_c[cat]) | Flatten(E_c[cat])] -> Dense(256, ELU) =
     // simulator_obs -> softmax head.  The sequence GRUs' last states come from the caches; the category GRU (21 steps)
@@ -344,7 +326,7 @@ int forward_rows(r4_env* e, int R, int row0, int div, const int32_t* cat, const 
                                                           reinterpret_cast<const float*>(c1.H.p), shared1, allf, LD); }
     R4_LAUNCH_CHECK(e, "k_seq_last_rows");
     if ((rc = gemm(e, SL_GEMM_XK, 0, R * NCAT, XIN_LD, EMB, e->emb_cat, EMB, cat, e->cg_wx_img, e->cg_bx, nullptr, XIN_LD, st,
-                   R, 0, XIN_LD, cgx, nullptr, r4tc::G_BNMAX, nullptr, nullptr, 0, 0, NCAT))) return rc;
+                   R, 0, XIN_LD, cgx, nullptr, nullptr, nullptr, 0, 0, NCAT))) return rc;
     { ProfScope ps(e, SL_GRU1, st, (double)R * NCAT * 2.0 * (EMB * 2 * EMB + EMB * EMB));
       r4tc::GruTcParams gp{cgx, e->cg_img, nullptr, R};
       gp.steps = NCAT; gp.hard = 1; gp.Hlast = allf + 3 * EMB; gp.ld_last = LD;
@@ -352,32 +334,15 @@ int forward_rows(r4_env* e, int R, int row0, int div, const int32_t* cat, const 
     R4_LAUNCH_CHECK(e, "k_gru_tc");
     if ((rc = gemm(e, SL_GEMM_DENSE, 1, R, HU, NDENSE, dense, NDENSE, nullptr, e->w1_img, e->b1, tmp, HU, st))) return rc;
     if ((rc = gemm(e, SL_GEMM_DENSE, 1, R, HU, HU, tmp, HU, nullptr, e->w2_img, e->b2, allf + 2 * EMB, LD, st))) return rc;
-    float* obs = obs_out;
-    if (!obs) {
-      if ((rc = reserve(e, e->ws_obs, (size_t)R * OBSD * 4))) return rc;
-      obs = reinterpret_cast<float*>(e->ws_obs.p);
-    }
     if ((rc = gemm(e, SL_GEMM_HEAD, 1, R, OBSD, LD + NCAT * EMB, allf, LD, nullptr, e->wo_img, e->bo, obs, OBSD, st, 0, 0, 0, nullptr,
-                   nullptr, HEAD_BNT, e->emb_cat, cat, LD, NCAT, MAXLEN, 4))) return rc;
-    if (p1_out || probs_out) {
-      { ProfScope ps(e, SL_RHEAD, st, (double)R * 2.0 * OBSD * 2);
-        k_reward_head<<<(R + 3) / 4, 128, 0, st>>>(R, obs, e->wr, e->br, p1_out, probs_out); }
-      R4_LAUNCH_CHECK(e, "k_reward_head");
-    }
-    return R4_OK;
-  }
-  if (e->sim == R4_SIM_WIDEDEEP) {
+                   nullptr, e->emb_cat, cat, LD, NCAT, MAXLEN, 4))) return rc;
+  } else if (e->sim == R4_SIM_WIDEDEEP) {
     // nets/widedeep.py:31-38: simulator_obs = [Dense256(ELU)(seq mean-pools) | dense tower | Flatten(E_c[cat])]; softmax head on it.
     // The sequence ids of the pass rows are in e->ws_seq (obs / reward passes: k_seq_ids_rows; r4_dien_forward: the caller's).
     if ((rc = reserve(e, e->ws_allf, (size_t)R * 2 * EMB * 4))) return rc;
     if ((rc = reserve(e, e->ws_tmp, (size_t)R * HU * 4))) return rc;
     float* pooled = reinterpret_cast<float*>(e->ws_allf.p);
     float* tmp = reinterpret_cast<float*>(e->ws_tmp.p);
-    float* obs = obs_out;
-    if (!obs) {
-      if ((rc = reserve(e, e->ws_obs, (size_t)R * OBSD_WD * 4))) return rc;
-      obs = reinterpret_cast<float*>(e->ws_obs.p);
-    }
     { ProfScope ps(e, SL_CAT, st, (double)R * (2 * MAXLEN * EMB * 4 + NCAT * EMB * 4));
       k_seq_pool<<<(R + 3) / 4, 128, 0, st>>>(R, reinterpret_cast<const int32_t*>(e->ws_seq.p), e->emb_seq, pooled);
       k_cat_flatten<<<(R + 3) / 4, 128, 0, st>>>(R, cat, e->emb_cat, obs + 2 * EMB + HU, OBSD_WD); }
@@ -386,14 +351,7 @@ int forward_rows(r4_env* e, int R, int row0, int div, const int32_t* cat, const 
     if ((rc = gemm(e, SL_GEMM_HEAD, 1, R, 2 * EMB, 2 * EMB, pooled, 2 * EMB, nullptr, e->fc_img, e->fcb, obs, OBSD_WD, st))) return rc;
     if ((rc = gemm(e, SL_GEMM_DENSE, 1, R, HU, NDENSE, dense, NDENSE, nullptr, e->w1_img, e->b1, tmp, HU, st))) return rc;
     if ((rc = gemm(e, SL_GEMM_DENSE, 1, R, HU, HU, tmp, HU, nullptr, e->w2_img, e->b2, obs + 2 * EMB, OBSD_WD, st))) return rc;
-    if (p1_out || probs_out) {
-      { ProfScope ps(e, SL_RHEAD, st, (double)R * 2.0 * OBSD_WD * 2);
-        k_reward_head<<<(R + 3) / 4, 128, 0, st>>>(R, obs, e->wr, e->br, p1_out, probs_out, OBSD_WD); }
-      R4_LAUNCH_CHECK(e, "k_reward_head");
-    }
-    return R4_OK;
-  }
-  if (e->sim == R4_SIM_DNN) {
+  } else if (e->sim == R4_SIM_DNN) {
     // nets/dnn.py:31-37: all = [mean_t E_c[cat] | dense tower]; Dense(256, ELU); simulator_obs Dense(256, ELU); softmax head
     if ((rc = reserve(e, e->ws_allf, (size_t)R * 2 * HU * 4))) return rc;
     if ((rc = reserve(e, e->ws_tmp, (size_t)R * OBSD * 4))) return rc;
@@ -407,99 +365,81 @@ int forward_rows(r4_env* e, int R, int row0, int div, const int32_t* cat, const 
     if ((rc = gemm(e, SL_GEMM_DENSE, 1, R, HU, NDENSE, dense, NDENSE, nullptr, e->w1_img, e->b1, tmp, HU, st))) return rc;
     if ((rc = gemm(e, SL_GEMM_DENSE, 1, R, HU, HU, tmp, HU, nullptr, e->w2_img, e->b2, allf + HU, 2 * HU, st))) return rc;
     if ((rc = gemm(e, SL_GEMM_DENSE, 1, R, OBSD, 2 * HU, allf, 2 * HU, nullptr, e->fc_img, e->fcb, tmp, OBSD, st))) return rc;
-    float* obs = obs_out;
-    if (!obs) {
-      if ((rc = reserve(e, e->ws_obs, (size_t)R * OBSD * 4))) return rc;
-      obs = reinterpret_cast<float*>(e->ws_obs.p);
-    }
     if ((rc = gemm(e, SL_GEMM_HEAD, 1, R, OBSD, OBSD, tmp, OBSD, nullptr, e->wo_img, e->bo, obs, OBSD, st))) return rc;
-    if (p1_out || probs_out) {
-      { ProfScope ps(e, SL_RHEAD, st, (double)R * 2.0 * OBSD * 2);
-        k_reward_head<<<(R + 3) / 4, 128, 0, st>>>(R, obs, e->wr, e->br, p1_out, probs_out); }
-      R4_LAUNCH_CHECK(e, "k_reward_head");
+  } else {
+    const int rtiles = (R + r4tc::TM - 1) / r4tc::TM;
+    const size_t sc_per_seq = (size_t)rtiles * r4tc::TM * MAXLEN;
+    if ((rc = reserve(e, e->ws_scores, 2 * sc_per_seq * 4))) return rc;
+    if ((rc = reserve(e, e->ws_allf, (size_t)R * ALLF_LD * 4))) return rc;
+    if ((rc = reserve(e, e->ws_tmp, (size_t)R * HU * 4))) return rc;
+    if ((rc = reserve(e, e->ws_q, (size_t)R * (r4tc::S_K + 2 * r4tc::S_N) * 4))) return rc;
+    float* qbuf = reinterpret_cast<float*>(e->ws_q.p);
+    float* qa0 = qbuf + (size_t)R * r4tc::S_K;
+    float* qa1 = qa0 + (size_t)R * r4tc::S_N;
+    float* scores = reinterpret_cast<float*>(e->ws_scores.p);
+    float* allf = reinterpret_cast<float*>(e->ws_allf.p);
+    float* tmp = reinterpret_cast<float*>(e->ws_tmp.p);
+    const SeqCache* cs[2] = {&c0, &c1};
+    int sh[2] = {shared0, shared1};
+    r4tc::ScoreTcParams sp{};
+    r4tc::AugruTcParams rp{};
+    for (int i = 0; i < 2; ++i) {
+      const PerSeq& w = e->ps[i];
+      r4tc::ScoreTcSeq& s = sp.s[i];
+      s.H = reinterpret_cast<const float*>(cs[i]->H.p);
+      s.Kp = reinterpret_cast<const float*>(cs[i]->Kp.p);
+      s.qa = i ? qa1 : qa0; s.WpImg = w.wp_img; s.Wqd = w.wqd; s.b1 = w.ab1; s.W2 = w.aw2; s.b2 = w.ab2; s.kv = w.akv; s.bk = w.abk;
+      s.scoresT = scores + (size_t)i * sc_per_seq;
+      s.shared = sh[i];
+      r4tc::AugruTcSeq& q = rp.s[i];
+      q.XT = reinterpret_cast<const float*>(cs[i]->XT.p); q.Wimg = w.au_img; q.scoresT = s.scoresT;
+      q.out = allf + i * AUH; q.shared = sh[i];
     }
-    return R4_OK;
-  }
-  const int rtiles = (R + r4tc::TM - 1) / r4tc::TM;
-  const size_t sc_per_seq = (size_t)rtiles * r4tc::TM * MAXLEN;
-  if ((rc = reserve(e, e->ws_scores, 2 * sc_per_seq * 4))) return rc;
-  if ((rc = reserve(e, e->ws_allf, (size_t)R * ALLF_LD * 4))) return rc;
-  if ((rc = reserve(e, e->ws_tmp, (size_t)R * HU * 4))) return rc;
-  if ((rc = reserve(e, e->ws_q, (size_t)R * (r4tc::S_K + 2 * r4tc::S_N) * 4))) return rc;
-  float* qbuf = reinterpret_cast<float*>(e->ws_q.p);
-  float* qa0 = qbuf + (size_t)R * r4tc::S_K;
-  float* qa1 = qa0 + (size_t)R * r4tc::S_N;
-  float* scores = reinterpret_cast<float*>(e->ws_scores.p);
-  float* allf = reinterpret_cast<float*>(e->ws_allf.p);
-  float* tmp = reinterpret_cast<float*>(e->ws_tmp.p);
-  const SeqCache* cs[2] = {&c0, &c1};
-  int sh[2] = {shared0, shared1};
-  r4tc::ScoreTcParams sp{};
-  r4tc::AugruTcParams rp{};
-  for (int i = 0; i < 2; ++i) {
-    const PerSeq& w = e->ps[i];
-    r4tc::ScoreTcSeq& s = sp.s[i];
-    s.H = reinterpret_cast<const float*>(cs[i]->H.p);
-    s.Kp = reinterpret_cast<const float*>(cs[i]->Kp.p);
-    s.qa = i ? qa1 : qa0; s.WpImg = w.wp_img; s.Wqd = w.wqd; s.b1 = w.ab1; s.W2 = w.aw2; s.b2 = w.ab2; s.kv = w.akv; s.bk = w.abk;
-    s.scoresT = scores + (size_t)i * sc_per_seq;
-    s.shared = sh[i];
-    r4tc::AugruTcSeq& q = rp.s[i];
-    q.XT = reinterpret_cast<const float*>(cs[i]->XT.p); q.Wimg = w.au_img; q.scoresT = s.scoresT;
-    q.out = allf + i * AUH; q.shared = sh[i];
-  }
-  sp.R = R; sp.row0 = row0; sp.div = div; sp.q = qbuf;
-  rp.R = R; rp.row0 = row0; rp.div = div; rp.out_ld = ALLF_LD;
-  // The side stream (lowest priority) does the AUGRU-independent half of the feature vector: category attention +
-  // dense tower.  It forks AFTER k_scores_tc and is fed after the AUGRU launch, so the AUGRU pairs (1 CTA per SM,
-  // 128 SMs at 4096 rows) are resident first and the side kernels fill the remaining SMs instead of delaying them.
-  // R4_NO_SIDE_STREAM / the per-kernel breakdown mode (r4_profile(2)) serialise everything on one stream: event pairs
-  // around a kernel on the low-priority side stream would time its wait for free SMs, not the kernel.
-  static const bool no_side_env = getenv("R4_NO_SIDE_STREAM") != nullptr;
-  const bool no_side = no_side_env || e->prof_mode == 2;
-  static const bool side_early = getenv("R4_SIDE_EARLY") != nullptr;    // diagnostics: fork before k_query (old schedule)
-  auto side_work = [&]() -> int {
-    cudaStream_t ss = no_side ? st : e->side;
-    if (!no_side) R4_CUDA(e, cudaStreamWaitEvent(e->side, e->ev_fork, 0));
-    { ProfScope ps(e, SL_CAT, ss, (double)R * 2.0 * (NCAT * NCAT * EMB * 2));
-      k_cat_attn<<<(R + 3) / 4, 128, SMEM_CAT, ss>>>(R, cat, e->emb_cat, allf); }
-    R4_LAUNCH_CHECK(e, "k_cat_attn");
-    int rc2;
-    if ((rc2 = gemm(e, SL_GEMM_DENSE, 1, R, HU, NDENSE, dense, NDENSE, nullptr, e->w1_img, e->b1, tmp, HU, ss))) return rc2;
-    if ((rc2 = gemm(e, SL_GEMM_DENSE, 1, R, HU, HU, tmp, HU, nullptr, e->w2_img, e->b2, allf + 2 * AUH, ALLF_LD, ss))) return rc2;
-    if (!no_side) R4_CUDA(e, cudaEventRecord(e->ev_join, ss));
-    return R4_OK;
-  };
-  if (no_side || side_early) {
+    sp.R = R; sp.row0 = row0; sp.div = div; sp.q = qbuf;
+    rp.R = R; rp.row0 = row0; rp.div = div; rp.out_ld = ALLF_LD;
+    // The side stream (lowest priority) does the AUGRU-independent half of the feature vector: category attention +
+    // dense tower.  It forks AFTER k_scores_tc and is fed after the AUGRU launch, so the AUGRU pairs (1 CTA per SM,
+    // 128 SMs at 4096 rows) are resident first and the side kernels fill the remaining SMs instead of delaying them.
+    // The per-kernel breakdown mode (r4_profile(2)) serialises everything on one stream: event pairs around a kernel
+    // on the low-priority side stream would time its wait for free SMs, not the kernel.
+    const bool no_side = e->prof_mode == 2;
+    auto side_work = [&]() -> int {
+      cudaStream_t ss = no_side ? st : e->side;
+      if (!no_side) R4_CUDA(e, cudaStreamWaitEvent(e->side, e->ev_fork, 0));
+      { ProfScope ps(e, SL_CAT, ss, (double)R * 2.0 * (NCAT * NCAT * EMB * 2));
+        k_cat_attn<<<(R + 3) / 4, 128, SMEM_CAT, ss>>>(R, cat, e->emb_cat, allf); }
+      R4_LAUNCH_CHECK(e, "k_cat_attn");
+      int rc2;
+      if ((rc2 = gemm(e, SL_GEMM_DENSE, 1, R, HU, NDENSE, dense, NDENSE, nullptr, e->w1_img, e->b1, tmp, HU, ss))) return rc2;
+      if ((rc2 = gemm(e, SL_GEMM_DENSE, 1, R, HU, HU, tmp, HU, nullptr, e->w2_img, e->b2, allf + 2 * AUH, ALLF_LD, ss))) return rc2;
+      if (!no_side) R4_CUDA(e, cudaEventRecord(e->ev_join, ss));
+      return R4_OK;
+    };
+    if (no_side && (rc = side_work())) return rc;
+    { ProfScope ps(e, SL_MISC, st, (double)R);
+      r4tc::k_query<<<(R + 7) / 8, 128, 0, st>>>(R, cat, e->emb_seq, e->ps[0].wqd, e->ps[0].ab1, e->ps[1].wqd, e->ps[1].ab1,
+                                                  qbuf, qa0, qa1); }
+    R4_LAUNCH_CHECK(e, "k_query");
+    { ProfScope ps(e, SL_SCORES, st, (double)R * 2 * MAXLEN * 2.0 * (EMB * AH1 + AH1 * AH2 + AH2));
+      const int ctas = std::min(2 * R, 2 * sm_count());
+      r4tc::k_scores_tc2<<<ctas, r4tc::S2_THREADS, r4tc::S2_SMEM_BYTES, st>>>(
+          sp, r4tc::scores_grid_split(ctas, R, sh[0], sh[1], augru_opts().scores_shared_pct)); }
+    R4_LAUNCH_CHECK(e, "k_scores_tc");
     if (!no_side) R4_CUDA(e, cudaEventRecord(e->ev_fork, st));
-    if ((rc = side_work())) return rc;
+    { ProfScope ps(e, SL_AUGRU, st, (double)R * 2 * MAXLEN * 2.0 * (AUH * 2 * AUH + AUH * AUH));
+      r4tc::k_augru_tc<<<dim3((R + r4tc::RC_ROWS - 1) / r4tc::RC_ROWS, 2), r4tc::RC_THREADS, r4tc::AU_SMEM_BYTES, st>>>(rp); }
+    R4_LAUNCH_CHECK(e, "k_augru_tc");
+    if (!no_side) {
+      if ((rc = side_work())) return rc;
+      R4_CUDA(e, cudaStreamWaitEvent(st, e->ev_join, 0));
+    }
+    // head: K = 768 materialised columns + 21 x 128 gathered from the category embedding table by `cat`
+    if ((rc = gemm(e, SL_GEMM_HEAD, 1, R, OBSD, ALLF, allf, ALLF_LD, nullptr, e->wo_img, e->bo, obs, OBSD, st, 0, 0, 0, nullptr, nullptr,
+                   e->emb_cat, cat, ALLF_LD, NCAT, MAXLEN, 4))) return rc;
   }
-  { ProfScope ps(e, SL_MISC, st, (double)R);
-    r4tc::k_query<<<(R + 7) / 8, 128, 0, st>>>(R, cat, e->emb_seq, e->ps[0].wqd, e->ps[0].ab1, e->ps[1].wqd, e->ps[1].ab1,
-                                                qbuf, qa0, qa1); }
-  R4_LAUNCH_CHECK(e, "k_query");
-  { ProfScope ps(e, SL_SCORES, st, (double)R * 2 * MAXLEN * 2.0 * (EMB * AH1 + AH1 * AH2 + AH2));
-    const int ctas = std::min(2 * R, 2 * sm_count());
-    r4tc::k_scores_tc2<<<ctas, r4tc::S2_THREADS, r4tc::S2_SMEM_BYTES, st>>>(
-        sp, r4tc::scores_grid_split(ctas, R, sh[0], sh[1], augru_opts().scores_shared_pct)); }
-  R4_LAUNCH_CHECK(e, "k_scores_tc");
-  if (!no_side && !side_early) R4_CUDA(e, cudaEventRecord(e->ev_fork, st));
-  { ProfScope ps(e, SL_AUGRU, st, (double)R * 2 * MAXLEN * 2.0 * (AUH * 2 * AUH + AUH * AUH));
-    r4tc::k_augru_tc<<<dim3((R + r4tc::RC_ROWS - 1) / r4tc::RC_ROWS, 2), r4tc::RC_THREADS, r4tc::AU_SMEM_BYTES, st>>>(rp); }
-  R4_LAUNCH_CHECK(e, "k_augru_tc");
-  if (!no_side && !side_early && (rc = side_work())) return rc;
-  if (!no_side) R4_CUDA(e, cudaStreamWaitEvent(st, e->ev_join, 0));
-  float* obs = obs_out;
-  if (!obs) {
-    if ((rc = reserve(e, e->ws_obs, (size_t)R * OBSD * 4))) return rc;
-    obs = reinterpret_cast<float*>(e->ws_obs.p);
-  }
-  // head: K = 768 materialised columns + 21 x 128 gathered from the category embedding table by `cat`
-  if ((rc = gemm(e, SL_GEMM_HEAD, 1, R, OBSD, ALLF, allf, ALLF_LD, nullptr, e->wo_img, e->bo, obs, OBSD, st, 0, 0, 0, nullptr, nullptr, HEAD_BNT,
-                 e->emb_cat, cat, ALLF_LD, NCAT, MAXLEN, 4))) return rc;
   if (p1_out || probs_out) {
-    { ProfScope ps(e, SL_RHEAD, st, (double)R * 2.0 * OBSD * 2);
-    k_reward_head<<<(R + 3) / 4, 128, 0, st>>>(R, obs, e->wr, e->br, p1_out, probs_out); }
+    { ProfScope ps(e, SL_RHEAD, st, (double)R * 2.0 * e->obs_dim * 2);
+      k_reward_head<<<(R + 3) / 4, 128, 0, st>>>(R, obs, e->wr, e->br, p1_out, probs_out, e->obs_dim); }
     R4_LAUNCH_CHECK(e, "k_reward_head");
   }
   return R4_OK;
@@ -613,6 +553,54 @@ const float* hw_get(r4_env* e, const std::string& name, size_t n) {
   auto it = e->hw.find(name);
   if (it == e->hw.end() || it->second.size() != n) return nullptr;
   return it->second.data();
+}
+
+// The simulators that cache GRU-1 (dien) / last-GRU-state (lstm) results per sequence (SeqCache)
+bool has_seq_cache(const r4_env* e) { return e->sim == R4_SIM_DIEN || e->sim == R4_SIM_LSTM; }
+
+// One tensor of a simulator's W-table (names and shapes of rl4rs_b200/synth.py *weight_shapes): uploaded as it is to
+// *dst, or as a k_gemm_tc image [K, N] to *img, or neither when only a derivation in r4_finalize_weights reads it.
+struct WEntry {
+  std::string name;
+  size_t n;
+  float** dst = nullptr;
+  uint8_t** img = nullptr;
+  int K = 0, N = 0;
+};
+
+// A GRU of the W-table -> the recurrence kernel's weights (r4_recur.cuh): gate columns [r | u | c], the x-side
+// projection wx [128, 384] carries the whole bias bx, the h-side is wgh [128, 256] (r | u) and wch [128, 128] (c).
+// Uploads the recurrence image, bx and the k_gemm_tc image of wx.
+//  - TF1 GRUCell (dien gru0/1): gate kernel `pre`_wg [x;h] x [r|u] + `pre`_bg, candidate kernel `pre`_wc [x;h] x c + `pre`_bc.
+//  - Keras GRU (lstm cgru, sgru0/1): kernel `pre`_k [128, 384], recurrent kernel `pre`_rk [128, 384], ONE bias `pre`_b
+//    [384], gate columns [z | r | h] (u = Keras z).
+int upload_gru(r4_env* e, const std::string& pre, bool keras, uint8_t** wx_img, float** bx_dev, uint8_t** rec_img) {
+  struct Gate { const float *x, *h, *b; int ld; };          // one gate's column block: x-side rows, h-side rows, bias
+  Gate g[3];                                                // [r, u, c]
+  if (keras) {
+    const float* k = e->hw[pre + "_k"].data(); const float* rk = e->hw[pre + "_rk"].data(); const float* b = e->hw[pre + "_b"].data();
+    const int src_of[3] = {EMB, 0, 2 * EMB};            // ours [r | u | c] <- Keras [z | r | h] column blocks
+    for (int j = 0; j < 3; ++j) g[j] = {k + src_of[j], rk + src_of[j], b + src_of[j], 3 * EMB};
+  } else {
+    const float* wg = e->hw[pre + "_wg"].data(); const float* bg = e->hw[pre + "_bg"].data();
+    const float* wc = e->hw[pre + "_wc"].data(); const float* bc = e->hw[pre + "_bc"].data();
+    for (int j = 0; j < 2; ++j) g[j] = {wg + j * EMB, wg + (size_t)EMB * 2 * EMB + j * EMB, bg + j * EMB, 2 * EMB};
+    g[2] = {wc, wc + (size_t)EMB * EMB, bc, EMB};
+  }
+  std::vector<float> wx((size_t)EMB * XIN_LD), bx(XIN_LD), wgh((size_t)EMB * 2 * EMB), wch((size_t)EMB * EMB);
+  for (int kk = 0; kk < EMB; ++kk)
+    for (int j = 0; j < 3; ++j)
+      for (int n = 0; n < EMB; ++n) {
+        wx[(size_t)kk * XIN_LD + j * EMB + n] = g[j].x[(size_t)kk * g[j].ld + n];
+        const float r = g[j].h[(size_t)kk * g[j].ld + n];
+        if (j < 2) wgh[(size_t)kk * 2 * EMB + j * EMB + n] = r; else wch[(size_t)kk * EMB + n] = r;
+      }
+  for (int j = 0; j < 3; ++j) for (int n = 0; n < EMB; ++n) bx[j * EMB + n] = g[j].b[n];
+  std::vector<uint8_t> gi(r4tc::G1_IMAGE_BYTES);
+  r4tc::build_recur_image(r4tc::GH, wgh.data(), wch.data(), gi.data());
+  int rc;
+  if ((rc = upload(e, gi, rec_img)) || (rc = upload(e, bx, bx_dev)) || (rc = upload_image(e, wx.data(), EMB, XIN_LD, wx_img))) return rc;
+  return R4_OK;
 }
 
 }  // namespace
@@ -738,196 +726,109 @@ int r4_finalize_weights(r4_env* e, void* stream) {
   if (!e) return R4_ERR_ARG;
   R4_CUDA(e, cudaSetDevice(e->device));
   const size_t Hh = (size_t)e->hash;
-  struct Need { const char* n; size_t sz; };
-  if (e->sim == R4_SIM_LSTM) {
-    // W-table of nets/lstm.py:8-45 (rl4rs_b200/synth.py: lstm_weight_shapes): Keras GRU layers = kernel [128, 384],
-    // recurrent kernel [128, 384], ONE bias [384], gate columns [z | r | h].  The recurrence kernel wants [r | u | c]
-    // (u = Keras z), the x-side projection carries the whole bias.
-    std::vector<Need> need = {{"emb_cat", Hh * EMB}, {"emb_seq", Hh * EMB}, {"dense_w1", (size_t)NDENSE * HU}, {"dense_b1", HU},
-                              {"dense_w2", (size_t)HU * HU}, {"dense_b2", HU}, {"cgru_k", (size_t)EMB * 3 * EMB},
-                              {"cgru_rk", (size_t)EMB * 3 * EMB}, {"cgru_b", 3 * EMB}, {"sgru0_k", (size_t)EMB * 3 * EMB},
-                              {"sgru0_rk", (size_t)EMB * 3 * EMB}, {"sgru0_b", 3 * EMB}, {"sgru1_k", (size_t)EMB * 3 * EMB},
-                              {"sgru1_rk", (size_t)EMB * 3 * EMB}, {"sgru1_b", 3 * EMB},
-                              {"obs_w", (size_t)(4 * EMB + NCAT * EMB) * OBSD}, {"obs_b", OBSD}, {"rew_w", OBSD * 2}, {"rew_b", 2}};
-    for (auto& nd : need)
-      if (!hw_get(e, nd.n, nd.sz)) return fail(e, R4_ERR_ARG, std::string("r4_finalize_weights(lstm): missing or mis-shaped ") + nd.n);
-    for (void* p : e->owned) cudaFree(p);
-    e->owned.clear();
-    int rc;
-    if ((rc = upload(e, e->hw["emb_cat"], &e->emb_cat)) || (rc = upload(e, e->hw["emb_seq"], &e->emb_seq)) ||
-        (rc = upload(e, e->hw["dense_b1"], &e->b1)) || (rc = upload(e, e->hw["dense_b2"], &e->b2)) ||
-        (rc = upload(e, e->hw["obs_b"], &e->bo)) || (rc = upload(e, e->hw["rew_w"], &e->wr)) ||
-        (rc = upload(e, e->hw["rew_b"], &e->br)) ||
-        (rc = upload_image(e, e->hw["dense_w1"].data(), NDENSE, HU, &e->w1_img)) ||
-        (rc = upload_image(e, e->hw["dense_w2"].data(), HU, HU, &e->w2_img)) ||
-        (rc = upload_image(e, e->hw["obs_w"].data(), 4 * EMB + NCAT * EMB, OBSD, &e->wo_img, HEAD_BNT))) return rc;
-    auto keras_gru = [&](const std::string& pre, uint8_t** wx_img, float** bx_dev, uint8_t** rec_img) -> int {
-      const float* k = e->hw[pre + "_k"].data(); const float* rk = e->hw[pre + "_rk"].data(); const float* b = e->hw[pre + "_b"].data();
-      std::vector<float> wx((size_t)EMB * XIN_LD), bx(XIN_LD), wgh((size_t)EMB * 2 * EMB), wch((size_t)EMB * EMB);
-      const int src_of[3] = {EMB, 0, 2 * EMB};            // ours [r | u | c] <- Keras [z | r | h] column blocks
-      for (int kk = 0; kk < EMB; ++kk)
-        for (int g = 0; g < 3; ++g)
-          for (int n = 0; n < EMB; ++n) {
-            wx[(size_t)kk * XIN_LD + g * EMB + n] = k[(size_t)kk * 3 * EMB + src_of[g] + n];
-            const float r = rk[(size_t)kk * 3 * EMB + src_of[g] + n];
-            if (g < 2) wgh[(size_t)kk * 2 * EMB + g * EMB + n] = r; else wch[(size_t)kk * EMB + n] = r;
-          }
-      for (int g = 0; g < 3; ++g) for (int n = 0; n < EMB; ++n) bx[g * EMB + n] = b[src_of[g] + n];
-      std::vector<uint8_t> gi(r4tc::G1_IMAGE_BYTES);
-      r4tc::build_recur_image(r4tc::GH, wgh.data(), wch.data(), gi.data());
-      int rc2;
-      if ((rc2 = upload(e, gi, rec_img)) || (rc2 = upload(e, bx, bx_dev)) || (rc2 = upload_image(e, wx.data(), EMB, XIN_LD, wx_img))) return rc2;
-      return R4_OK;
-    };
-    if ((rc = keras_gru("cgru", &e->cg_wx_img, &e->cg_bx, &e->cg_img)) ||
-        (rc = keras_gru("sgru0", &e->ps[0].gru_wx_img, &e->ps[0].gru_bx, &e->ps[0].gru_img)) ||
-        (rc = keras_gru("sgru1", &e->ps[1].gru_wx_img, &e->ps[1].gru_bx, &e->ps[1].gru_img))) return rc;
-    e->hw.clear();
-    e->weights_ready = true;
-    // SlateRecEnv's second sequence is the constant [0] (slate.py:75 -> 64 x id 0): cache its last GRU state once
-    cudaStream_t st = S(stream);
-    if ((rc = reserve(e, e->ws_ids1, (size_t)std::max(e->B, 1) * MAXLEN * 4))) return rc;
-    R4_CUDA(e, cudaMemsetAsync(e->ws_ids1.p, 0, (size_t)MAXLEN * 4, st));
-    if ((rc = build_cache(e, 1, reinterpret_cast<const int32_t*>(e->ws_ids1.p), 1, e->c1const, st))) return rc;
-    return R4_OK;
+  // every simulator: emb_cat [H,128], dense tower, simulator_reward [obs_dim, 2]
+  std::vector<WEntry> tab = {{"emb_cat", Hh * EMB, &e->emb_cat},
+                             {"dense_w1", (size_t)NDENSE * HU, nullptr, &e->w1_img, NDENSE, HU}, {"dense_b1", HU, &e->b1},
+                             {"dense_w2", (size_t)HU * HU, nullptr, &e->w2_img, HU, HU}, {"dense_b2", HU, &e->b2},
+                             {"rew_w", (size_t)e->obs_dim * 2, &e->wr}, {"rew_b", 2, &e->br}};
+  // the dnn graph's second Embedding (sequence_input_concat) feeds nothing; widedeep has ONE emb_seq for both sequences
+  if (e->sim != R4_SIM_DNN) tab.push_back({"emb_seq", Hh * EMB, &e->emb_seq});
+  if (e->sim == R4_SIM_DIEN) {
+    // W-table of nets/dien.py:8-45 (rl4rs_b200/synth.py: weight_shapes): observation head, then per sequence GRU-1
+    // (TF1 GRUCell), the attention MLP and the AUGRU (VecAttGRUCell)
+    tab.insert(tab.end(), {{"obs_w", (size_t)ALLF * OBSD, nullptr, &e->wo_img, ALLF, OBSD}, {"obs_b", OBSD, &e->bo}});
+    for (int i = 0; i < 2; ++i) {
+      const std::string si = std::to_string(i);
+      PerSeq& w = e->ps[i];
+      tab.insert(tab.end(), {{"gru" + si + "_wg", (size_t)2 * EMB * 2 * EMB}, {"gru" + si + "_bg", 2 * EMB},
+                             {"gru" + si + "_wc", (size_t)2 * EMB * EMB}, {"gru" + si + "_bc", EMB},
+                             {"att" + si + "_w1", (size_t)4 * EMB * AH1}, {"att" + si + "_b1", AH1, &w.ab1},
+                             {"att" + si + "_w2", (size_t)AH1 * AH2, &w.aw2}, {"att" + si + "_b2", AH2, &w.ab2},
+                             {"att" + si + "_k", AH2, &w.akv}, {"att" + si + "_b", 1},
+                             {"augru" + si + "_wg", (size_t)(EMB + AUH) * 2 * AUH}, {"augru" + si + "_bg", 2 * AUH},
+                             {"augru" + si + "_wc", (size_t)(EMB + AUH) * AUH}, {"augru" + si + "_bc", AUH}});
+    }
+  } else if (e->sim == R4_SIM_DNN) {
+    // W-table of nets/dnn.py:8-45: fc [256,256] (the unnamed Dense of :34), simulator_obs [256,256]
+    tab.insert(tab.end(), {{"fc_w", (size_t)2 * HU * OBSD, nullptr, &e->fc_img, 2 * HU, OBSD}, {"fc_b", OBSD, &e->fcb},
+                           {"obs_w", (size_t)OBSD * OBSD, nullptr, &e->wo_img, OBSD, OBSD}, {"obs_b", OBSD, &e->bo}});
+  } else if (e->sim == R4_SIM_WIDEDEEP) {
+    // W-table of nets/widedeep.py:8-45: fc [256,256] (the Dense on the pooled sequences, :34); 'simulator_obs' is a
+    // Concatenate (no weights)
+    tab.insert(tab.end(), {{"fc_w", (size_t)2 * EMB * 2 * EMB, nullptr, &e->fc_img, 2 * EMB, 2 * EMB}, {"fc_b", 2 * EMB, &e->fcb}});
+  } else {
+    // W-table of nets/lstm.py:8-45 (rl4rs_b200/synth.py: lstm_weight_shapes): the category GRU and the two sequence GRUs
+    // (Keras GRU layers: kernel [128, 384], recurrent kernel [128, 384], ONE bias [384]), observation head
+    for (const char* gru : {"cgru", "sgru0", "sgru1"}) {
+      const std::string p(gru);
+      tab.insert(tab.end(), {{p + "_k", (size_t)EMB * 3 * EMB}, {p + "_rk", (size_t)EMB * 3 * EMB}, {p + "_b", 3 * EMB}});
+    }
+    tab.insert(tab.end(), {{"obs_w", (size_t)(4 * EMB + NCAT * EMB) * OBSD, nullptr, &e->wo_img, 4 * EMB + NCAT * EMB, OBSD},
+                           {"obs_b", OBSD, &e->bo}});
   }
-  if (e->sim == R4_SIM_WIDEDEEP) {
-    // W-table of nets/widedeep.py:8-45: emb_cat, dense tower, emb_seq (ONE table for both sequences), fc [256,256] (the
-    // Dense on the pooled sequences, :34), simulator_reward [3072,2]; 'simulator_obs' is a Concatenate (no weights)
-    std::vector<Need> need = {{"emb_cat", Hh * EMB}, {"emb_seq", Hh * EMB}, {"dense_w1", (size_t)NDENSE * HU}, {"dense_b1", HU},
-                              {"dense_w2", (size_t)HU * HU}, {"dense_b2", HU}, {"fc_w", (size_t)2 * EMB * 2 * EMB}, {"fc_b", 2 * EMB},
-                              {"rew_w", (size_t)OBSD_WD * 2}, {"rew_b", 2}};
-    for (auto& nd : need)
-      if (!hw_get(e, nd.n, nd.sz)) return fail(e, R4_ERR_ARG, std::string("r4_finalize_weights(widedeep): missing or mis-shaped ") + nd.n);
-    for (void* p : e->owned) cudaFree(p);
-    e->owned.clear();
-    int rc;
-    if ((rc = upload(e, e->hw["emb_cat"], &e->emb_cat)) || (rc = upload(e, e->hw["emb_seq"], &e->emb_seq)) ||
-        (rc = upload(e, e->hw["dense_b1"], &e->b1)) || (rc = upload(e, e->hw["dense_b2"], &e->b2)) ||
-        (rc = upload(e, e->hw["fc_b"], &e->fcb)) || (rc = upload(e, e->hw["rew_w"], &e->wr)) ||
-        (rc = upload(e, e->hw["rew_b"], &e->br)) ||
-        (rc = upload_image(e, e->hw["dense_w1"].data(), NDENSE, HU, &e->w1_img)) ||
-        (rc = upload_image(e, e->hw["dense_w2"].data(), HU, HU, &e->w2_img)) ||
-        (rc = upload_image(e, e->hw["fc_w"].data(), 2 * EMB, 2 * EMB, &e->fc_img))) return rc;
-    e->hw.clear();
-    e->weights_ready = true;
-    return R4_OK;
-  }
-  if (e->sim == R4_SIM_DNN) {
-    // W-table of nets/dnn.py:8-45: emb_cat [H,128], dense tower, fc [256,256] (the unnamed Dense of :34), simulator_obs
-    // [256,256], simulator_reward [256,2].  The graph's second Embedding (sequence_input_concat) feeds nothing.
-    std::vector<Need> need = {{"emb_cat", Hh * EMB}, {"dense_w1", (size_t)NDENSE * HU}, {"dense_b1", HU},
-                              {"dense_w2", (size_t)HU * HU}, {"dense_b2", HU}, {"fc_w", (size_t)2 * HU * OBSD}, {"fc_b", OBSD},
-                              {"obs_w", (size_t)OBSD * OBSD}, {"obs_b", OBSD}, {"rew_w", OBSD * 2}, {"rew_b", 2}};
-    for (auto& nd : need)
-      if (!hw_get(e, nd.n, nd.sz)) return fail(e, R4_ERR_ARG, std::string("r4_finalize_weights(dnn): missing or mis-shaped ") + nd.n);
-    for (void* p : e->owned) cudaFree(p);
-    e->owned.clear();
-    int rc;
-    if ((rc = upload(e, e->hw["emb_cat"], &e->emb_cat)) || (rc = upload(e, e->hw["dense_b1"], &e->b1)) ||
-        (rc = upload(e, e->hw["dense_b2"], &e->b2)) || (rc = upload(e, e->hw["fc_b"], &e->fcb)) ||
-        (rc = upload(e, e->hw["obs_b"], &e->bo)) || (rc = upload(e, e->hw["rew_w"], &e->wr)) ||
-        (rc = upload(e, e->hw["rew_b"], &e->br)) ||
-        (rc = upload_image(e, e->hw["dense_w1"].data(), NDENSE, HU, &e->w1_img)) ||
-        (rc = upload_image(e, e->hw["dense_w2"].data(), HU, HU, &e->w2_img)) ||
-        (rc = upload_image(e, e->hw["fc_w"].data(), 2 * HU, OBSD, &e->fc_img)) ||
-        (rc = upload_image(e, e->hw["obs_w"].data(), OBSD, OBSD, &e->wo_img))) return rc;
-    e->hw.clear();
-    e->weights_ready = true;
-    return R4_OK;
-  }
-  std::vector<Need> need = {{"emb_cat", Hh * EMB}, {"emb_seq", Hh * EMB}, {"dense_w1", (size_t)NDENSE * HU},
-                            {"dense_b1", HU}, {"dense_w2", (size_t)HU * HU}, {"dense_b2", HU},
-                            {"obs_w", (size_t)ALLF * OBSD}, {"obs_b", OBSD}, {"rew_w", OBSD * 2}, {"rew_b", 2}};
-  for (auto& nd : need)
-    if (!hw_get(e, nd.n, nd.sz)) return fail(e, R4_ERR_ARG, std::string("r4_finalize_weights: missing or mis-shaped ") + nd.n);
+  static const char* const SIM_NAMES[] = {"dien", "dnn", "widedeep", "lstm"};     // indexed by R4_SIM_*
+  for (const WEntry& t : tab)
+    if (!hw_get(e, t.name, t.n))
+      return fail(e, R4_ERR_ARG, std::string("r4_finalize_weights(") + SIM_NAMES[e->sim] + "): missing or mis-shaped " + t.name);
   for (void* p : e->owned) cudaFree(p);
   e->owned.clear();
   int rc;
-#define UP(dst, nm) if ((rc = upload(e, e->hw[nm], &(dst)))) return rc;
-  UP(e->emb_cat, "emb_cat"); UP(e->emb_seq, "emb_seq"); UP(e->w1, "dense_w1"); UP(e->b1, "dense_b1");
-  UP(e->w2, "dense_w2"); UP(e->b2, "dense_b2"); UP(e->wo, "obs_w"); UP(e->bo, "obs_b");
-  UP(e->wr, "rew_w"); UP(e->br, "rew_b");
-#undef UP
-  if ((rc = upload_image(e, e->hw["dense_w1"].data(), NDENSE, HU, &e->w1_img)) ||
-      (rc = upload_image(e, e->hw["dense_w2"].data(), HU, HU, &e->w2_img)) ||
-      (rc = upload_image(e, e->hw["obs_w"].data(), ALLF, OBSD, &e->wo_img, HEAD_BNT))) return rc;
-  for (int i = 0; i < 2; ++i) {
-    std::string si = std::to_string(i);
-    const float* gwg = hw_get(e, "gru" + si + "_wg", (size_t)2 * EMB * 2 * EMB);
-    const float* gbg = hw_get(e, "gru" + si + "_bg", 2 * EMB);
-    const float* gwc = hw_get(e, "gru" + si + "_wc", (size_t)2 * EMB * EMB);
-    const float* gbc = hw_get(e, "gru" + si + "_bc", EMB);
-    const float* aw1 = hw_get(e, "att" + si + "_w1", (size_t)4 * EMB * AH1);
-    const float* ab1 = hw_get(e, "att" + si + "_b1", AH1);
-    const float* aw2 = hw_get(e, "att" + si + "_w2", (size_t)AH1 * AH2);
-    const float* ab2 = hw_get(e, "att" + si + "_b2", AH2);
-    const float* akv = hw_get(e, "att" + si + "_k", AH2);
-    const float* abk = hw_get(e, "att" + si + "_b", 1);
-    const float* uwg = hw_get(e, "augru" + si + "_wg", (size_t)(EMB + AUH) * 2 * AUH);
-    const float* ubg = hw_get(e, "augru" + si + "_bg", 2 * AUH);
-    const float* uwc = hw_get(e, "augru" + si + "_wc", (size_t)(EMB + AUH) * AUH);
-    const float* ubc = hw_get(e, "augru" + si + "_bc", AUH);
-    if (!gwg || !gbg || !gwc || !gbc || !aw1 || !ab1 || !aw2 || !ab2 || !akv || !abk || !uwg || !ubg || !uwc || !ubc)
-      return fail(e, R4_ERR_ARG, "r4_finalize_weights: missing or mis-shaped per-sequence weight (seq " + si + ")");
-    PerSeq& w = e->ps[i];
-    // GRU-1 (TF1 GRUCell): gate kernel [x;h] x [r|u], candidate kernel [x;h] x c
-    std::vector<float> wx((size_t)EMB * XIN_LD), bx(XIN_LD), wgh((size_t)EMB * 2 * EMB), wch((size_t)EMB * EMB);
-    for (int k = 0; k < EMB; ++k) {
-      for (int n = 0; n < 2 * EMB; ++n) wx[(size_t)k * XIN_LD + n] = gwg[(size_t)k * 2 * EMB + n];
-      for (int n = 0; n < EMB; ++n) wx[(size_t)k * XIN_LD + 2 * EMB + n] = gwc[(size_t)k * EMB + n];
-      for (int n = 0; n < 2 * EMB; ++n) wgh[(size_t)k * 2 * EMB + n] = gwg[(size_t)(EMB + k) * 2 * EMB + n];
-      for (int n = 0; n < EMB; ++n) wch[(size_t)k * EMB + n] = gwc[(size_t)(EMB + k) * EMB + n];
-    }
-    for (int n = 0; n < 2 * EMB; ++n) bx[n] = gbg[n];
-    for (int n = 0; n < EMB; ++n) bx[2 * EMB + n] = gbc[n];
-    // AUGRU (VecAttGRUCell) input halves + attention key half
-    std::vector<float> awx((size_t)EMB * XK_LD), abx(XK_LD, 0.f), awgh((size_t)AUH * 2 * AUH), awch((size_t)AUH * AUH);
-    std::vector<float> wqd((size_t)EMB * AH1), wp((size_t)EMB * AH1);
-    for (int k = 0; k < EMB; ++k) {
-      for (int n = 0; n < 2 * AUH; ++n) awx[(size_t)k * XK_LD + n] = uwg[(size_t)k * 2 * AUH + n];
-      for (int n = 0; n < AUH; ++n) awx[(size_t)k * XK_LD + XK_C + n] = uwc[(size_t)k * AUH + n];
-      for (int n = 0; n < AH1; ++n) {
-        float wq = aw1[(size_t)k * AH1 + n], wk = aw1[(size_t)(EMB + k) * AH1 + n];
-        float wd = aw1[(size_t)(2 * EMB + k) * AH1 + n], wpp = aw1[(size_t)(3 * EMB + k) * AH1 + n];
-        awx[(size_t)k * XK_LD + XK_K + n] = wk - wd;        // keys * (Wk - Wd)
-        wqd[(size_t)k * AH1 + n] = wq + wd;                 // query * (Wq + Wd)
-        wp[(size_t)k * AH1 + n] = wpp;                      // (query*keys) * Wp
+  for (const WEntry& t : tab) {
+    const std::vector<float>& v = e->hw[t.name];
+    if (t.dst && (rc = upload(e, v, t.dst))) return rc;
+    if (t.img && (rc = upload_image(e, v.data(), t.K, t.N, t.img))) return rc;
+  }
+  if (e->sim == R4_SIM_LSTM) {
+    if ((rc = upload_gru(e, "cgru", true, &e->cg_wx_img, &e->cg_bx, &e->cg_img)) ||
+        (rc = upload_gru(e, "sgru0", true, &e->ps[0].gru_wx_img, &e->ps[0].gru_bx, &e->ps[0].gru_img)) ||
+        (rc = upload_gru(e, "sgru1", true, &e->ps[1].gru_wx_img, &e->ps[1].gru_bx, &e->ps[1].gru_img))) return rc;
+  }
+  if (e->sim == R4_SIM_DIEN) {
+    for (int i = 0; i < 2; ++i) {
+      const std::string si = std::to_string(i);
+      PerSeq& w = e->ps[i];
+      if ((rc = upload_gru(e, "gru" + si, false, &w.gru_wx_img, &w.gru_bx, &w.gru_img))) return rc;
+      const float* aw1 = e->hw["att" + si + "_w1"].data();
+      const float* uwg = e->hw["augru" + si + "_wg"].data();
+      const float* ubg = e->hw["augru" + si + "_bg"].data();
+      const float* uwc = e->hw["augru" + si + "_wc"].data();
+      const float* ubc = e->hw["augru" + si + "_bc"].data();
+      // AUGRU (VecAttGRUCell) input halves + attention key half
+      std::vector<float> awx((size_t)EMB * XK_LD), abx(XK_LD, 0.f), awgh((size_t)AUH * 2 * AUH), awch((size_t)AUH * AUH);
+      std::vector<float> wqd((size_t)EMB * AH1), wp((size_t)EMB * AH1);
+      for (int k = 0; k < EMB; ++k) {
+        for (int n = 0; n < 2 * AUH; ++n) awx[(size_t)k * XK_LD + n] = uwg[(size_t)k * 2 * AUH + n];
+        for (int n = 0; n < AUH; ++n) awx[(size_t)k * XK_LD + XK_C + n] = uwc[(size_t)k * AUH + n];
+        for (int n = 0; n < AH1; ++n) {
+          float wq = aw1[(size_t)k * AH1 + n], wk = aw1[(size_t)(EMB + k) * AH1 + n];
+          float wd = aw1[(size_t)(2 * EMB + k) * AH1 + n], wpp = aw1[(size_t)(3 * EMB + k) * AH1 + n];
+          awx[(size_t)k * XK_LD + XK_K + n] = wk - wd;        // keys * (Wk - Wd)
+          wqd[(size_t)k * AH1 + n] = wq + wd;                 // query * (Wq + Wd)
+          wp[(size_t)k * AH1 + n] = wpp;                      // (query*keys) * Wp
+        }
       }
+      for (int n = 0; n < 2 * AUH; ++n) abx[n] = ubg[n];
+      for (int n = 0; n < AUH; ++n) abx[XK_C + n] = ubc[n];
+      for (int k = 0; k < AUH; ++k) {
+        for (int n = 0; n < 2 * AUH; ++n) awgh[(size_t)k * 2 * AUH + n] = uwg[(size_t)(EMB + k) * 2 * AUH + n];
+        for (int n = 0; n < AUH; ++n) awch[(size_t)k * AUH + n] = uwc[(size_t)(EMB + k) * AUH + n];
+      }
+      if ((rc = upload_image(e, awx.data(), EMB, XK_LD, &w.au_wx_img))) return rc;
+      {
+        std::vector<uint8_t> wpi(r4tc::S_IMG_BYTES);      // Wp image, then the W2 image of k_scores_tc2
+        r4tc::build_scores_image2(wp.data(), e->hw["att" + si + "_w2"].data(), wpi.data());
+        if ((rc = upload(e, wpi, &w.wp_img))) return rc;
+      }
+      std::vector<uint8_t> img(r4tc::AU_IMAGE_BYTES);
+      r4tc::build_recur_image(r4tc::HID, awgh.data(), awch.data(), img.data());
+      if ((rc = upload(e, img, &w.au_img)) || (rc = upload(e, abx, &w.au_bx)) || (rc = upload(e, wqd, &w.wqd))) return rc;
+      w.abk = e->hw["att" + si + "_b"][0];
     }
-    for (int n = 0; n < 2 * AUH; ++n) abx[n] = ubg[n];
-    for (int n = 0; n < AUH; ++n) abx[XK_C + n] = ubc[n];
-    for (int k = 0; k < AUH; ++k) {
-      for (int n = 0; n < 2 * AUH; ++n) awgh[(size_t)k * 2 * AUH + n] = uwg[(size_t)(EMB + k) * 2 * AUH + n];
-      for (int n = 0; n < AUH; ++n) awch[(size_t)k * AUH + n] = uwc[(size_t)(EMB + k) * AUH + n];
-    }
-    {
-      std::vector<uint8_t> gi(r4tc::G1_IMAGE_BYTES);
-      r4tc::build_recur_image(r4tc::GH, wgh.data(), wch.data(), gi.data());
-      if ((rc = upload(e, gi, &w.gru_img))) return rc;
-    }
-    if ((rc = upload_image(e, wx.data(), EMB, XIN_LD, &w.gru_wx_img)) ||
-        (rc = upload_image(e, awx.data(), EMB, XK_LD, &w.au_wx_img))) return rc;
-    {
-      std::vector<uint8_t> wpi(r4tc::S_IMG_BYTES);      // Wp image, then the W2 image of k_scores_tc2
-      r4tc::build_scores_image2(wp.data(), aw2, wpi.data());
-      if ((rc = upload(e, wpi, &w.wp_img))) return rc;
-    }
-    std::vector<uint8_t> img(r4tc::AU_IMAGE_BYTES);
-    r4tc::build_recur_image(r4tc::HID, awgh.data(), awch.data(), img.data());
-    if ((rc = upload(e, img, &w.au_img))) return rc;
-    std::vector<float> vb1(ab1, ab1 + AH1), vw2(aw2, aw2 + AH1 * AH2), vb2(ab2, ab2 + AH2), vkv(akv, akv + AH2);
-    if ((rc = upload(e, wx, &w.gru_wx)) || (rc = upload(e, bx, &w.gru_bx)) || (rc = upload(e, wgh, &w.gru_wgh)) ||
-        (rc = upload(e, wch, &w.gru_wch)) || (rc = upload(e, awx, &w.au_wx)) || (rc = upload(e, abx, &w.au_bx)) ||
-        (rc = upload(e, awgh, &w.au_wgh)) || (rc = upload(e, awch, &w.au_wch)) || (rc = upload(e, wqd, &w.wqd)) ||
-        (rc = upload(e, wp, &w.wp)) || (rc = upload(e, vb1, &w.ab1)) || (rc = upload(e, vw2, &w.aw2)) ||
-        (rc = upload(e, vb2, &w.ab2)) || (rc = upload(e, vkv, &w.akv)))
-      return rc;
-    w.abk = abk[0];
   }
   e->hw.clear();
   e->weights_ready = true;
-  // SlateRecEnv's second sequence is the constant [0] (slate.py:75 -> 64 x id 0): cache it once.
+  if (!has_seq_cache(e)) return R4_OK;
+  // SlateRecEnv's second sequence is the constant [0] (slate.py:75 -> 64 x id 0): cache it once (lstm: its last GRU state).
   cudaStream_t st = S(stream);
   if ((rc = reserve(e, e->ws_ids1, (size_t)std::max(e->B, 1) * MAXLEN * 4))) return rc;
   R4_CUDA(e, cudaMemsetAsync(e->ws_ids1.p, 0, (size_t)MAXLEN * 4, st));
@@ -941,7 +842,7 @@ int r4_load_log(r4_env* e, const int32_t* user_cat, const float* user_dense, con
     return fail(e, R4_ERR_ARG, "r4_load_log: bad argument");
   if (n_rows > 0x7fffffffLL) return fail(e, R4_ERR_ARG, "r4_load_log: more than 2^31-1 rows");
   e->log_cat = user_cat; e->log_dense = user_dense; e->log_seq = user_seq; e->log_items = logged_items;
-  e->log_fb = feedback; e->log_n = n_rows; e->log_slots = n_slots;
+  e->log_fb = feedback; e->log_slots = n_slots;
   e->has_reset = false;
   return R4_OK;
 }
@@ -967,7 +868,7 @@ int r4_reset(r4_env* e, const int32_t* row_idx, const r4_out* out, void* stream)
   e->has_reset = true;
   // user-history GRU-1 + input projections: once per episode (they do not depend on the actions); the dnn simulator
   // has no sequence branch
-  if ((e->sim == R4_SIM_DIEN || e->sim == R4_SIM_LSTM) && (rc = build_cache(e, 0, (const int32_t*)e->ws_ids0.p, B, e->c0, st))) return rc;
+  if (has_seq_cache(e) && (rc = build_cache(e, 0, (const int32_t*)e->ws_ids0.p, B, e->c0, st))) return rc;
   if ((rc = obs_pass(e, 0, 0, out, st))) return rc;
   if (out && out->reward) { k_fill_f64<<<(B + 255) / 256, 256, 0, st>>>(B, 0.0, out->reward); R4_LAUNCH_CHECK(e, "k_fill_f64"); }
   if (out && out->done) { k_fill_u8<<<(B + 255) / 256, 256, 0, st>>>(B, 0, out->done); R4_LAUNCH_CHECK(e, "k_fill_u8"); }
@@ -987,7 +888,7 @@ int r4_step(r4_env* e, const void* action, int action_is_f64, const r4_out* out,
   bool conti = (e->cfg.flags & R4_FLAG_CONTI) != 0;
   // SeqSlate: entering a new page, the second sequence becomes the items of all previous pages
   // (seqslate.py:109-110) -> rebuild its GRU-1 cache once per page.
-  if ((e->sim == R4_SIM_DIEN || e->sim == R4_SIM_LSTM) && e->seq && cur > 0 && cur % e->P == 0) {
+  if (has_seq_cache(e) && e->seq && cur > 0 && cur % e->P == 0) {
     if ((rc = reserve(e, e->ws_ids1, (size_t)B * MAXLEN * 4))) return rc;
     k_seq_ids<<<(B * MAXLEN + 255) / 256, 256, 0, st>>>(B, e->T, cur, e->row_idx, e->log_seq, e->prev_actions,
                                                          nullptr, (int32_t*)e->ws_ids1.p, nullptr);
@@ -1259,25 +1160,20 @@ int r4_ppo_epoch(float* params, const float* obs, const uint8_t* mask, const int
   const int np = r4ppo::make_layout(action_size).n;
   int steps = 0;
   const bool fused = !(grad_clip > 0.f);      // global-norm clipping needs the reduced gradient first
-  // programmatic dependent launch for the grad / optimiser chain of the epoch (R4_NO_PDL=1: plain stream order)
-  static const bool pdl = getenv("R4_NO_PDL") == nullptr;
   if (!params || !m || !v || !flat_grad || !scratch) return fail(nullptr, R4_ERR_ARG, "r4_ppo_epoch: bad argument");
   for (int s = 0; s + mb <= n; s += mb, ++steps) {
+    // programmatic dependent launch for the grad / optimiser chain of the fused epoch
     int rc = policy_grad_impl(0, params, obs, mask, action, old_logp, old_logits, old_value, adv, target, perm + s, mb,
                               action_size, clip, vf_clip, vf_coeff, kl_coeff, ent_coeff, 1.0f / mb, scratch, G, flat_grad,
-                              stats_accum, 1.0f / mb, stream, !fused, fused && pdl);
+                              stats_accum, 1.0f / mb, stream, !fused, fused);
     if (rc) return rc;
-    if (fused && pdl) {
+    if (fused) {
       cudaLaunchConfig_t lc = {};
       cudaLaunchAttribute at[1];
       at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
       lc.gridDim = dim3((np + 255) / 256); lc.blockDim = dim3(256); lc.dynamicSmemBytes = 0; lc.stream = S(stream); lc.attrs = at; lc.numAttrs = 1;
       cudaLaunchKernelEx(&lc, r4ppo::k_reduce_adam, np, G, (const float*)scratch, flat_grad, (const float*)(scratch + (size_t)G * np), stats_accum,
                          1.0f / mb, params, m, v, step0 + steps + 1, lr, beta1, beta2, eps);
-      R4_PCHECK("k_reduce_adam");
-    } else if (fused) {
-      r4ppo::k_reduce_adam<<<(np + 255) / 256, 256, 0, S(stream)>>>(np, G, scratch, flat_grad, scratch + (size_t)G * np, stats_accum,
-                                                                    1.0f / mb, params, m, v, step0 + steps + 1, lr, beta1, beta2, eps);
       R4_PCHECK("k_reduce_adam");
     } else {
       rc = r4_adam_step(params, flat_grad, m, v, np, step0 + steps + 1, lr, beta1, beta2, eps, 1.0f, grad_clip, norm_scratch, stream);
@@ -1542,36 +1438,30 @@ int r4_dien_forward(r4_env* e, const int32_t* seq, const float* dense, const int
   if (!e->weights_ready) return fail(e, R4_ERR_STATE, "r4_dien_forward: load + finalize weights first");
   R4_CUDA(e, cudaSetDevice(e->device));
   cudaStream_t st = S(stream);
-  int rc;
-  if (e->sim == R4_SIM_DNN || e->sim == R4_SIM_WIDEDEEP) {          // dnn: no sequence branch; widedeep: raw ids, no sequence cache
-    rc = R4_OK;
-    int chunk = std::min(n_rows, e->max_rows);
-    for (int r0 = 0; !rc && r0 < n_rows; r0 += chunk) {
-      int nr = std::min(chunk, n_rows - r0);
-      if (e->sim == R4_SIM_WIDEDEEP) {
-        if ((rc = reserve(e, e->ws_seq, (size_t)nr * 2 * MAXLEN * 4))) return rc;
-        R4_CUDA(e, cudaMemcpyAsync(e->ws_seq.p, seq + (size_t)r0 * 2 * MAXLEN, (size_t)nr * 2 * MAXLEN * 4, cudaMemcpyDeviceToDevice, st));
-      }
-      rc = forward_rows(e, nr, r0, 1, cat + (size_t)r0 * NCAT, dense + (size_t)r0 * NDENSE, e->c0, 0, e->c0, 0,
-                        obs ? obs + (size_t)r0 * e->obs_dim : nullptr, nullptr, probs ? probs + (size_t)r0 * 2 : nullptr, st);
-    }
-    return rc;
-  }
+  int rc = R4_OK;
+  // dien / lstm: temporary sequence caches of the rows' own sequences; dnn has no sequence branch, widedeep reads raw ids
   SeqCache t0, t1;
   DevBuf ids;
-  if ((rc = reserve(e, ids, (size_t)2 * n_rows * MAXLEN * 4))) return rc;
-  int32_t* i0 = (int32_t*)ids.p;
-  int32_t* i1 = i0 + (size_t)n_rows * MAXLEN;
-  R4_CUDA(e, cudaMemcpy2DAsync(i0, MAXLEN * 4, seq, 2 * MAXLEN * 4, MAXLEN * 4, n_rows, cudaMemcpyDeviceToDevice, st));
-  R4_CUDA(e, cudaMemcpy2DAsync(i1, MAXLEN * 4, seq + MAXLEN, 2 * MAXLEN * 4, MAXLEN * 4, n_rows, cudaMemcpyDeviceToDevice, st));
-  rc = build_cache(e, 0, i0, n_rows, t0, st);
-  if (!rc) rc = build_cache(e, 1, i1, n_rows, t1, st);
+  if (has_seq_cache(e)) {
+    if ((rc = reserve(e, ids, (size_t)2 * n_rows * MAXLEN * 4))) return rc;
+    int32_t* i0 = (int32_t*)ids.p;
+    int32_t* i1 = i0 + (size_t)n_rows * MAXLEN;
+    R4_CUDA(e, cudaMemcpy2DAsync(i0, MAXLEN * 4, seq, 2 * MAXLEN * 4, MAXLEN * 4, n_rows, cudaMemcpyDeviceToDevice, st));
+    R4_CUDA(e, cudaMemcpy2DAsync(i1, MAXLEN * 4, seq + MAXLEN, 2 * MAXLEN * 4, MAXLEN * 4, n_rows, cudaMemcpyDeviceToDevice, st));
+    rc = build_cache(e, 0, i0, n_rows, t0, st);
+    if (!rc) rc = build_cache(e, 1, i1, n_rows, t1, st);
+  }
   int chunk = std::min(n_rows, e->max_rows);
   for (int r0 = 0; !rc && r0 < n_rows; r0 += chunk) {
     int nr = std::min(chunk, n_rows - r0);
+    if (e->sim == R4_SIM_WIDEDEEP) {
+      if ((rc = reserve(e, e->ws_seq, (size_t)nr * 2 * MAXLEN * 4))) return rc;
+      R4_CUDA(e, cudaMemcpyAsync(e->ws_seq.p, seq + (size_t)r0 * 2 * MAXLEN, (size_t)nr * 2 * MAXLEN * 4, cudaMemcpyDeviceToDevice, st));
+    }
     rc = forward_rows(e, nr, r0, 1, cat + (size_t)r0 * NCAT, dense + (size_t)r0 * NDENSE, t0, 0, t1, 0,
-                      obs ? obs + (size_t)r0 * OBSD : nullptr, nullptr, probs ? probs + (size_t)r0 * 2 : nullptr, st);
+                      obs ? obs + (size_t)r0 * e->obs_dim : nullptr, nullptr, probs ? probs + (size_t)r0 * 2 : nullptr, st);
   }
+  if (!has_seq_cache(e)) return rc;
   cudaStreamSynchronize(st);
   DevBuf* tmp[] = {&t0.H, &t0.Kp, &t0.XT, &t1.H, &t1.Kp, &t1.XT, &ids};
   for (DevBuf* b : tmp) if (b->p) cudaFree(b->p);
