@@ -33,11 +33,12 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo, uint
 }
 // D[64 x N] (+)= A[64 x 16] . B[16 x N]^T, bf16 in, fp32 accumulators in the registers of the issuing warpgroup.  Register
 // i of a thread (warp w of the warpgroup, lane l) holds row 16 w + l / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (l % 4) + i % 2.
-__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uint64_t db) {
+// scale_d = 0: D = A . B (the accumulators' old values are not read).
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uint64_t db, int scale_d = 1) {
   asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
                "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-               : "l"(da), "l"(db), "r"(1) : "memory");
+               : "l"(da), "l"(db), "r"(scale_d) : "memory");
 }
 __device__ __forceinline__ void wgmma_m64n16k16_rs(float (&d)[8], const uint32_t (&a)[4], uint64_t db) {
   asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
@@ -58,6 +59,13 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
                "@p bra DONE;\n\tbra WAIT_LOOP;\n\tDONE:\n\t}\n"
                :: "r"(smem_u32(bar)), "r"(parity) : "memory");
 }
+// An opaque 0, read from a shared word that holds 0: an address offset by it cannot be computed before the read, nor
+// shared with another read.  (volatile + memory clobber keep the read after the preceding barrier wait.)
+__device__ __forceinline__ uint32_t lds_opaque(const uint32_t* p) {
+  uint32_t z;
+  asm volatile("ld.volatile.shared.u32 %0, [%1];" : "=r"(z) : "r"(smem_u32(p)) : "memory");
+  return z;
+}
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory");
 }
@@ -70,6 +78,9 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
 }
 // generic-proxy shared-memory stores -> visible to the async proxy (wgmma operand reads, bulk copies)
 __device__ __forceinline__ void proxy_fence() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void sts32(uint32_t saddr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" :: "r"(saddr), "r"(v) : "memory");
+}
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" :: "r"(id), "r"(nthreads) : "memory");
 }
