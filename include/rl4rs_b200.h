@@ -302,6 +302,69 @@ int r4_gauss_ppo_epoch_dist(r4_comm* comm, float* params, const float* obs, cons
                             float kl_coeff, float ent_coeff, float* scratch, float* flat_grad, float* stats_accum, float* m,
                             float* v, int step0, float lr, float beta1, float beta2, float eps, void* stream);
 
+/* ---- DDPG / TD3 on the continuous-action env (modelfree_train.py:46-48,79-105; modelfree_trainer.py:25-28; RLlib 1.5
+ * ddpg / td3 defaults, INTEGRATION.md section 3): a deterministic actor obs(256) -> 400 relu -> 300 relu -> D, squashed
+ * to Box(-1, 1) as tanh, and a critic concat(obs, a) -> 400 relu -> 300 relu -> 1 (TD3: plus a twin critic), action_dim
+ * = D in 2..32.  Flat parameter layout (r4_ddpg_num_params(D, twin) floats):
+ * actor  w1[256,400] b1[400] w2[400,300] b2[300] w3[300,D] b3[D] |
+ * critic w1[256+D,400] b1[400] w2[400,300] b2[300] w3[300] b3[1] | twin critic as the critic (twin != 0 only).
+ * The target parameters have the same layout.  Stateless: every pointer is caller-owned DEVICE memory. */
+int r4_ddpg_num_params(int action_dim, int twin);
+/* floats of the scratch r4_ddpg_grad / r4_ddpg_train_step need for batches of up to n samples; -1 for bad arguments */
+int64_t r4_ddpg_scratch_size(int action_dim, int twin, int n);
+/* The actor on obs f32[n,256] -> action f32[n,D], the env action and what the replay stores.  mode 0: the actor output
+ * (DDPG's StochasticSampling over a deterministic distribution, and explore=False).  mode 1: OrnsteinUhlenbeckNoise with ONE
+ * state f32[D] shared by every row: x' = x + theta (-x) + sigma N(0, I), a = clip(actor + noise_scale x', -1, 1), where the
+ * caller passes noise_scale = scale * ou_base_scale * (high - low); ou_out receives x' (ou_out != ou_in: alternate two
+ * buffers).  mode 2: the random phase, a = U(-1, 1) per row and dimension.  The draws are counter-based: splitmix64 keyed by
+ * seed and ((counter + row) << 6) + dim (row 0 for the OU state), so the same seed and counter reproduce the actions. */
+int r4_ddpg_act(const float* params, const float* obs, int n, int action_dim, int mode, uint64_t seed, uint64_t counter,
+                const float* ou_in, float* ou_out, float ou_theta, float ou_sigma, float noise_scale, float* action,
+                void* stream);
+/* Replay (RLlib ReplayBuffer / PrioritizedReplayBuffer): a ring of `capacity` transitions in caller-owned arrays obs
+ * f32[C,256], action f32[C,D], reward f32[C], new_obs f32[C,256], done u8[C] and, for prioritized replay, prio f32[C] (the
+ * stored p^alpha) with max_prio f32[1] (the running maximum of |td| + eps, initially 1).
+ * r4_replay_store: the [T,B] rollout rows r = t*B + b (obs f32[T*B,256], action f32[T*B,D], reward f32[T*B], done u8[T*B])
+ * go to slot (pos + r) % capacity, pos = transitions stored before; new_obs = the obs of row r + B, or final_obs f32[B,256]
+ * (what the last step returned) on the last step.  New items get max_prio^alpha (prio may be NULL: uniform replay). */
+int r4_replay_store(float* r_obs, float* r_action, float* r_reward, float* r_new_obs, uint8_t* r_done, float* r_prio,
+                    const float* max_prio, int capacity, int action_dim, int64_t pos, float alpha, const float* obs,
+                    const float* final_obs, const float* action, const float* reward, const uint8_t* done, int T, int B,
+                    void* stream);
+/* n indices over the first `size` slots from the caller's uniforms u f32[n] in [0, 1): prio == NULL uniform, idx =
+ * floor(u size), weight 1; else proportional with replacement, idx = the first i whose prefix sum of prio exceeds u * total
+ * (float64 sums in a fixed order), weight = (p_i N)^-beta / (p_min N)^-beta with p = prio / total, N = size. */
+int r4_replay_sample(const float* prio, int size, int n, float beta, const float* u, int64_t* idx, float* weights, void* stream);
+/* prio[idx[i]] = (|td[i]| + eps)^alpha, the later position winning for a repeated index (RLlib's sequential loop), and
+ * max_prio = max(max_prio, |td[i]| + eps). */
+int r4_replay_update_priorities(float* prio, float* max_prio, const int64_t* idx, const float* td, int n, float alpha,
+                                float eps, void* stream);
+/* Gradient of the DDPG / TD3 losses over the replay rows idx[0..n) (weights f32[n] may be NULL = 1):
+ * critic loss sum_i w_i (td1_i^2 + td2_i^2) / 2 * inv_n, td_k = Q_k(s, a) - (r + gamma (1 - done) min_k Q'_k(s', a')),
+ * a' = clip(pi'(s') + clip(target_noise smooth_noise, -noise_clip, noise_clip), -1, 1) (smooth_noise f32[n,D] N(0,1)
+ * draws, NULL: a' = pi'(s')); actor loss -sum_i Q1(s_i, pi(s_i)) * inv_n, applied to the actor weights only.  No l2 terms
+ * (r4_ddpg_apply adds them).  grad f32[num_params] receives the gradient (deterministic: one writer per element), td f32[n]
+ * (may be NULL) td1, stats f32[3] (may be NULL) {critic loss, actor loss, mean Q1(s, pi(s))}.  2 launches. */
+int r4_ddpg_grad(const float* params, const float* target, int action_dim, int twin, const float* r_obs, const float* r_action,
+                 const float* r_reward, const float* r_new_obs, const uint8_t* r_done, const int64_t* idx, const float* weights,
+                 const float* smooth_noise, int n, float gamma, float target_noise, float noise_clip, float inv_n,
+                 float* scratch, float* grad, float* td, float* stats, void* stream);
+/* The optimiser step of both networks in one launch: g = grad * grad_scale + l2_reg * w on the kernels (not the biases);
+ * torch.optim.Adam (betas 0.9 / 0.999, eps 1e-8) with one moment pair m, v f32[num_params] split by region: the actor with
+ * actor_lr at 1-based actor_step (0: the actor is left unchanged, TD3's delayed steps), the critic(s) with critic_lr at
+ * critic_step; then the soft target update target = tau params + (1 - tau) target over the whole buffer. */
+int r4_ddpg_apply(float* params, float* target, const float* grad, float* m, float* v, int action_dim, int twin, int actor_step,
+                  int critic_step, float actor_lr, float critic_lr, float l2_reg, float tau, float grad_scale, void* stream);
+/* One SGD step with no host round trip: r4_replay_sample (n indices from u), r4_ddpg_grad, over peer memory the sum over the
+ * ranks (comm != NULL; loss = mean over n x world samples; comm created with r4_ddpg_num_params), r4_ddpg_apply and, with
+ * prio != NULL, r4_replay_update_priorities from td1.  stats (may be NULL) as r4_ddpg_grad.  5 launches. */
+int r4_ddpg_train_step(r4_comm* comm, float* params, float* target, float* m, float* v, int action_dim, int twin,
+                       const float* r_obs, const float* r_action, const float* r_reward, const float* r_new_obs,
+                       const uint8_t* r_done, float* r_prio, float* max_prio, int size, int n, const float* u,
+                       const float* smooth_noise, float beta, float alpha, float prio_eps, float gamma, float target_noise,
+                       float noise_clip, int actor_step, int critic_step, float actor_lr, float critic_lr, float l2_reg,
+                       float tau, float* scratch, float* stats, void* stream);
+
 /* ---- the simulator alone (nets/dien.py:8-45), for parity tests and kernel benchmarks ------- */
 /* seq i32[R,2,64], dense f32[R,432], cat i32[R,21] (device) -> obs f32[R,256], probs f32[R,2]
  * (either may be NULL).  Runs the uncached path: GRU-1 is recomputed for every row. */

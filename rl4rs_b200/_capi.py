@@ -82,7 +82,20 @@ EXPORTS = {
                            [C.c_float] * 5 + [C.c_void_p, C.c_void_p]),
     "r4_gauss_ppo_epoch_dist": (C.c_int, [C.c_void_p] * 10 + [C.c_int] * 3 + [C.c_float] * 5 + [C.c_void_p] * 5 + [C.c_int] +
                                 [C.c_float] * 4 + [C.c_void_p]),
-    "r4_adam_step": (C.c_int, [C.c_void_p] * 4 + [C.c_int, C.c_int] + [C.c_float] * 6 + [C.c_void_p, C.c_void_p]),
+    "r4_ddpg_num_params": (C.c_int, [C.c_int, C.c_int]),
+    "r4_ddpg_scratch_size": (C.c_int64, [C.c_int, C.c_int, C.c_int]),
+    "r4_ddpg_act": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p] +
+                    [C.c_float] * 3 + [C.c_void_p, C.c_void_p]),
+    "r4_replay_store": (C.c_int, [C.c_void_p] * 7 + [C.c_int, C.c_int, C.c_int64, C.c_float] + [C.c_void_p] * 5 +
+                        [C.c_int, C.c_int, C.c_void_p]),
+    "r4_replay_sample": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "r4_replay_update_priorities": (C.c_int, [C.c_void_p] * 4 + [C.c_int, C.c_float, C.c_float, C.c_void_p]),
+    "r4_ddpg_grad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 8 + [C.c_int] + [C.c_float] * 4 +
+                     [C.c_void_p] * 5),
+    "r4_ddpg_apply": (C.c_int, [C.c_void_p] * 5 + [C.c_int] * 4 + [C.c_float] * 5 + [C.c_void_p]),
+    "r4_ddpg_train_step": (C.c_int, [C.c_void_p] * 5 + [C.c_int, C.c_int] + [C.c_void_p] * 7 + [C.c_int, C.c_int] +
+                           [C.c_void_p] * 2 + [C.c_float] * 6 + [C.c_int, C.c_int] + [C.c_float] * 4 + [C.c_void_p] * 3),
+    "r4_adam_step": (C.c_int,[C.c_void_p] * 4 + [C.c_int, C.c_int] + [C.c_float] * 6 + [C.c_void_p, C.c_void_p]),
     "r4_dien_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 

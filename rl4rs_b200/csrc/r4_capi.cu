@@ -9,6 +9,7 @@
 #include "r4_ppo.cuh"
 #include "r4_comm.cuh"
 #include "r4_gauss.cuh"
+#include "r4_ddpg.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -1430,6 +1431,132 @@ int r4_gauss_ppo_epoch_dist(r4_comm* c, float* params, const float* obs, const f
     if (rc) return rc;
   }
   return steps;
+}
+
+// ---- DDPG / TD3 (r4_ddpg.cuh) ---------------------------------------------------------------------------------
+static bool ddpg_dim_ok(int D) { return D >= 2 && D <= r4ddpg::MAXD; }
+
+int r4_ddpg_num_params(int action_dim, int twin) { return ddpg_dim_ok(action_dim) ? r4ddpg::make_layout(action_dim, twin != 0).n : -1; }
+
+int64_t r4_ddpg_scratch_size(int action_dim, int twin, int n) {
+  return (!ddpg_dim_ok(action_dim) || n < 1) ? -1 : (int64_t)r4ddpg::scratch_floats(action_dim, twin != 0, n);
+}
+
+static int ddpg_smem(const void* fn, size_t bytes, const char* name, bool& done) {
+  if (done) return R4_OK;
+  cudaError_t st = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  if (st != cudaSuccess) return fail(nullptr, R4_ERR_CUDA, std::string("cudaFuncSetAttribute(") + name + "): " + cudaGetErrorString(st));
+  done = true;
+  return R4_OK;
+}
+
+int r4_ddpg_act(const float* params, const float* obs, int n, int action_dim, int mode, uint64_t seed, uint64_t counter,
+                const float* ou_in, float* ou_out, float ou_theta, float ou_sigma, float noise_scale, float* action,
+                void* stream) {
+  if (!params || !obs || !action || n < 1 || !ddpg_dim_ok(action_dim) || mode < 0 || mode > 2 ||
+      (mode == 1 && (!ou_in || !ou_out || ou_in == ou_out)))
+    return fail(nullptr, R4_ERR_ARG, "r4_ddpg_act: bad argument (action_dim 2..32, mode 0..2, OU needs two state buffers)");
+  static bool attr = false;
+  if (int rc = ddpg_smem((const void*)r4ddpg::k_ddpg_act, r4ddpg::ACT_SMEM, "k_ddpg_act", attr)) return rc;
+  r4ddpg::k_ddpg_act<<<(n + r4ddpg::TS - 1) / r4ddpg::TS, r4ddpg::NT, r4ddpg::ACT_SMEM, S(stream)>>>(
+      r4ddpg::make_layout(action_dim, 0), params, obs, n, mode, seed, counter, ou_in, ou_out, ou_theta, ou_sigma, noise_scale,
+      action);
+  R4_PCHECK("k_ddpg_act");
+  return R4_OK;
+}
+
+int r4_replay_store(float* r_obs, float* r_action, float* r_reward, float* r_new_obs, uint8_t* r_done, float* r_prio,
+                    const float* max_prio, int capacity, int action_dim, int64_t pos, float alpha, const float* obs,
+                    const float* final_obs, const float* action, const float* reward, const uint8_t* done, int T, int B,
+                    void* stream) {
+  if (!r_obs || !r_action || !r_reward || !r_new_obs || !r_done || (r_prio && !max_prio) || capacity < 1 || pos < 0 ||
+      !ddpg_dim_ok(action_dim) || !obs || !final_obs || !action || !reward || !done || T < 1 || B < 1)
+    return fail(nullptr, R4_ERR_ARG, "r4_replay_store: bad argument");
+  const int64_t rows = std::min<int64_t>((int64_t)T * B, capacity);
+  r4ddpg::k_replay_store<<<(unsigned)rows, 64, 0, S(stream)>>>(r_obs, r_action, r_reward, r_new_obs, r_done, r_prio, max_prio,
+                                                              capacity, action_dim, pos, alpha, obs, final_obs, action, reward,
+                                                              done, T, B);
+  R4_PCHECK("k_replay_store");
+  return R4_OK;
+}
+
+int r4_replay_sample(const float* prio, int size, int n, float beta, const float* u, int64_t* idx, float* weights, void* stream) {
+  if (size < 1 || n < 1 || !u || !idx || !weights) return fail(nullptr, R4_ERR_ARG, "r4_replay_sample: bad argument");
+  r4ddpg::k_replay_sample<<<1, r4ddpg::SNT, 0, S(stream)>>>(prio, size, n, beta, u, idx, weights);
+  R4_PCHECK("k_replay_sample");
+  return R4_OK;
+}
+
+int r4_replay_update_priorities(float* prio, float* max_prio, const int64_t* idx, const float* td, int n, float alpha,
+                                float eps, void* stream) {
+  if (!prio || !max_prio || !idx || !td || n < 1) return fail(nullptr, R4_ERR_ARG, "r4_replay_update_priorities: bad argument");
+  r4ddpg::k_replay_priorities<<<1, r4ddpg::SNT, 0, S(stream)>>>(prio, max_prio, idx, td, n, alpha, eps);
+  R4_PCHECK("k_replay_priorities");
+  return R4_OK;
+}
+
+int r4_ddpg_grad(const float* params, const float* target, int action_dim, int twin, const float* r_obs, const float* r_action,
+                 const float* r_reward, const float* r_new_obs, const uint8_t* r_done, const int64_t* idx, const float* weights,
+                 const float* smooth_noise, int n, float gamma, float target_noise, float noise_clip, float inv_n,
+                 float* scratch, float* grad, float* td, float* stats, void* stream) {
+  if (!params || !target || !ddpg_dim_ok(action_dim) || !r_obs || !r_action || !r_reward || !r_new_obs || !r_done || !idx ||
+      n < 1 || !scratch || !grad)
+    return fail(nullptr, R4_ERR_ARG, "r4_ddpg_grad: bad argument");
+  static bool attr = false;
+  if (int rc = ddpg_smem((const void*)r4ddpg::k_ddpg_rows, r4ddpg::ROWS_SMEM, "k_ddpg_rows", attr)) return rc;
+  const r4ddpg::Layout L = r4ddpg::make_layout(action_dim, twin != 0);
+  r4ddpg::Planes P = r4ddpg::make_planes(scratch, action_dim, twin != 0, n);
+  if (td) P.td = td;
+  const r4ddpg::Jobs J = r4ddpg::make_jobs(L, P);
+  const r4ddpg::Replay R{r_obs, r_action, r_reward, r_new_obs, r_done};
+  const r4ddpg::Hyper hp{gamma, target_noise, noise_clip, inv_n};
+  r4ddpg::k_ddpg_rows<<<(n + r4ddpg::TS - 1) / r4ddpg::TS, r4ddpg::NT, r4ddpg::ROWS_SMEM, S(stream)>>>(
+      L, hp, params, target, R, idx, weights, smooth_noise, n, P);
+  R4_PCHECK("k_ddpg_rows");
+  r4ddpg::k_ddpg_wgrad<<<J.ntiles + 1, r4ddpg::NT, 0, S(stream)>>>(J, n, grad, P.stats, stats, inv_n);
+  R4_PCHECK("k_ddpg_wgrad");
+  return R4_OK;
+}
+
+int r4_ddpg_apply(float* params, float* target, const float* grad, float* m, float* v, int action_dim, int twin, int actor_step,
+                  int critic_step, float actor_lr, float critic_lr, float l2_reg, float tau, float grad_scale, void* stream) {
+  if (!params || !target || !grad || !m || !v || !ddpg_dim_ok(action_dim) || actor_step < 0 || critic_step < 1)
+    return fail(nullptr, R4_ERR_ARG, "r4_ddpg_apply: bad argument");
+  const r4ddpg::Layout L = r4ddpg::make_layout(action_dim, twin != 0);
+  r4ddpg::k_ddpg_apply<<<(L.n + 255) / 256, 256, 0, S(stream)>>>(L, params, target, grad, m, v, actor_step, critic_step, actor_lr,
+                                                                  critic_lr, l2_reg, tau, grad_scale);
+  R4_PCHECK("k_ddpg_apply");
+  return R4_OK;
+}
+
+int r4_ddpg_train_step(r4_comm* comm, float* params, float* target, float* m, float* v, int action_dim, int twin,
+                       const float* r_obs, const float* r_action, const float* r_reward, const float* r_new_obs,
+                       const uint8_t* r_done, float* r_prio, float* max_prio, int size, int n, const float* u,
+                       const float* smooth_noise, float beta, float alpha, float prio_eps, float gamma, float target_noise,
+                       float noise_clip, int actor_step, int critic_step, float actor_lr, float critic_lr, float l2_reg,
+                       float tau, float* scratch, float* stats, void* stream) {
+  if (!scratch || !ddpg_dim_ok(action_dim) || n < 1 || (r_prio && !max_prio))
+    return fail(nullptr, R4_ERR_ARG, "r4_ddpg_train_step: bad argument");
+  const int np = r4ddpg::make_layout(action_dim, twin != 0).n;
+  const r4ddpg::Planes P = r4ddpg::make_planes(scratch, action_dim, twin != 0, n);
+  const int world = comm ? comm->world : 1;
+  int rc = r4_replay_sample(r_prio, size, n, beta, u, P.idx, P.weights, stream);
+  if (rc) return rc;
+  rc = r4_ddpg_grad(params, target, action_dim, twin, r_obs, r_action, r_reward, r_new_obs, r_done, P.idx,
+                    r_prio ? P.weights : nullptr, smooth_noise, n, gamma, target_noise, noise_clip, 1.0f / ((float)n * world),
+                    scratch, P.grad, nullptr, stats, stream);
+  if (rc) return rc;
+  const float* g = P.grad;
+  if (comm) {        // one partial (G = 1) per rank, summed in rank order into the scratch's second gradient
+    float* sum = P.grad + np + 5;
+    if ((rc = exchange_launch(comm, P.grad, 1, np, sum, nullptr, 0.f, 0, nullptr, nullptr, nullptr, 0, 0.f, 0.f, 0.f, 0.f, stream)))
+      return rc;
+    g = sum;
+  }
+  rc = r4_ddpg_apply(params, target, g, m, v, action_dim, twin, actor_step, critic_step, actor_lr, critic_lr, l2_reg, tau, 1.0f,
+                     stream);
+  if (rc || !r_prio) return rc;
+  return r4_replay_update_priorities(r_prio, max_prio, P.idx, P.td, n, alpha, prio_eps, stream);
 }
 
 int r4_dien_forward(r4_env* e, const int32_t* seq, const float* dense, const int32_t* cat, int n_rows,

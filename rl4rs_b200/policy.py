@@ -154,6 +154,130 @@ class GaussianPolicy(object):
         return a, a.clamp(-1.0, 1.0), self.logp(d, a), value, d
 
 
+def _splitmix64(x):
+    """csrc/r4_ppo.cuh splitmix64 over a uint64 array (wrapping arithmetic)."""
+    import numpy as np
+    x = x + np.uint64(0x9E3779B97F4A7C15)
+    x = (x ^ (x >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+    x = (x ^ (x >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+    return x ^ (x >> np.uint64(31))
+
+
+def counter_draws(seed, counter, rows, dims):
+    """The exploration draws of csrc/r4_ddpg.cuh for rows 0..rows-1 and dims 0..dims-1, keyed by (seed, counter):
+    -> (uniform in [-1, 1), standard normal), both float64 [rows, dims]."""
+    import numpy as np
+    with np.errstate(over="ignore"):
+        r = np.arange(rows, dtype=np.uint64)[:, None]
+        d = np.arange(dims, dtype=np.uint64)[None, :]
+        key = ((np.uint64(counter) + r) << np.uint64(6)) + d
+        x = _splitmix64(np.uint64(seed) ^ _splitmix64(key))
+    hi = (x >> np.uint64(40)).astype(np.float64)
+    u1 = (hi + 0.5) / 16777216.0
+    u2 = ((x >> np.uint64(16)) & np.uint64(0xFFFFFF)).astype(np.float64) / 16777216.0
+    return hi * (2.0 / 16777216.0) - 1.0, np.sqrt(-2.0 * np.log(u1)) * np.cos(2.0 * np.pi * u2)
+
+
+class DeterministicActorCritic(object):
+    """The networks RLlib 1.5 builds for DDPG / TD3 (modelfree_trainer.py:25-28, actor_hiddens = critic_hiddens = [400, 300],
+    relu): an actor obs(256) -> 400 -> 300 -> D squashed to Box(-1, 1) by (high - low) sigmoid(2x) + low = tanh(x), and a
+    critic concat(obs, a) -> 400 -> 300 -> 1; TD3 (twin) adds a second critic.  Keras glorot-uniform kernels, zero biases.
+    One flat buffer [actor | critic | twin] (csrc/r4_ddpg.cuh's layout) and a target copy of it (hard copy at construction).
+    This torch twin is the CPU path of DDPGTrainer / TD3Trainer and the autograd cross-check of the kernels
+    (tests/test_gpu_trainer_ddpg.py)."""
+
+    H1, H2 = 400, 300
+
+    def __init__(self, action_dim=32, device="cuda", seed=0, twin=False):
+        self.D, self.twin = action_dim, bool(twin)
+        self.device = torch.device(device)
+        D, H1, H2 = action_dim, self.H1, self.H2
+
+        def net(p, K, N3):
+            return [(p + "w1", (K, H1)), (p + "b1", (H1,)), (p + "w2", (H1, H2)), (p + "b2", (H2,)), (p + "w3", (H2, N3)),
+                    (p + "b3", (N3,))]
+        shapes = net("a_", OBS, D) + net("q1_", OBS + D, 1) + (net("q2_", OBS + D, 1) if twin else [])
+        n = sum(math.prod(s) for _, s in shapes)
+        g = torch.Generator(device="cpu").manual_seed(seed)
+        self.flat = torch.zeros(n, dtype=torch.float32, device=self.device, requires_grad=True)
+        off = 0
+        with torch.no_grad():
+            for name, shape in shapes:
+                k = math.prod(shape)
+                if len(shape) == 2:       # glorot uniform
+                    lim = math.sqrt(6.0 / (shape[0] + shape[1]))
+                    self.flat[off:off + k].view(shape).copy_(((torch.rand(shape, generator=g) * 2 - 1) * lim).to(self.device))
+                off += k
+        self._shapes, self.n_params = shapes, n
+        self.n_actor = sum(math.prod(s) for name, s in shapes if name.startswith("a_"))
+        self.target = self.flat.detach().clone()
+        mask = torch.zeros(n, dtype=torch.bool)
+        off = 0
+        for name, shape in shapes:
+            k = math.prod(shape)
+            mask[off:off + k] = len(shape) == 2
+            off += k
+        self.kernel_mask = mask.to(self.device)      # the l2 terms cover the kernels, not the biases
+
+    def params(self, flat=None):
+        flat = self.flat if flat is None else flat
+        out, off = {}, 0
+        for name, shape in self._shapes:
+            k = math.prod(shape)
+            out[name] = flat[off:off + k].view(shape)
+            off += k
+        return out
+
+    @staticmethod
+    def _mlp(p, pre, x):
+        return torch.relu(torch.relu(x @ p[pre + "w1"] + p[pre + "b1"]) @ p[pre + "w2"] + p[pre + "b2"]) @ p[pre + "w3"] + p[pre + "b3"]
+
+    def actor(self, obs, flat=None):
+        """obs f32 [n,256] -> the deterministic action [n,D] in (-1, 1)."""
+        return torch.tanh(self._mlp(self.params(flat), "a_", obs))
+
+    def critic(self, obs, a, k=1, flat=None):
+        """Q_k(obs, a) [n] (k = 1, or 2 for the twin)."""
+        return self._mlp(self.params(flat), "q%d_" % k, torch.cat([obs, a], dim=1)).squeeze(-1)
+
+    def inputs(self, obs):
+        return (obs["obs"] if isinstance(obs, dict) else obs,)
+
+    def losses(self, obs, action, reward, new_obs, done, weights=None, smooth_noise=None, gamma=1.0, target_noise=0.2,
+               noise_clip=0.5, inv_n=None):
+        """The RLlib DDPG / TD3 losses without the l2 terms (r4_ddpg_grad's definition), as sums over the batch times inv_n
+        (default 1/n): -> (critic loss, actor loss, td1 [n]).  The actor loss reads the critic with its weights detached,
+        so its gradient reaches the actor weights only."""
+        n = obs.shape[0]
+        inv_n = 1.0 / n if inv_n is None else inv_n
+        w = torch.ones(n, device=obs.device) if weights is None else weights
+        with torch.no_grad():
+            a2 = self.actor(new_obs, self.target)
+            if smooth_noise is not None:
+                a2 = (a2 + (target_noise * smooth_noise).clamp(-noise_clip, noise_clip)).clamp(-1.0, 1.0)
+            qt = self.critic(new_obs, a2, 1, self.target)
+            if self.twin:
+                qt = torch.min(qt, self.critic(new_obs, a2, 2, self.target))
+            y = reward + gamma * (1.0 - done.to(torch.float32)) * qt
+        td1 = self.critic(obs, action, 1) - y
+        err = 0.5 * td1 ** 2
+        if self.twin:
+            err = err + 0.5 * (self.critic(obs, action, 2) - y) ** 2
+        critic_loss = (w * err).sum() * inv_n
+        frozen = self.flat.detach()
+        actor_loss = -self.critic(obs, self.actor(obs), 1, frozen).sum() * inv_n
+        return critic_loss, actor_loss, td1.detach()
+
+    def l2_loss(self, l2):
+        """l2 * sum(w^2) / 2 over the kernels of the actor and of the critic(s) (the two losses' l2 terms added)."""
+        return l2 * 0.5 * (self.flat[self.kernel_mask] ** 2).sum()
+
+    @torch.no_grad()
+    def soft_update(self, tau):
+        """target = tau * online + (1 - tau) * target."""
+        self.target.copy_(tau * self.flat.detach() + (1.0 - tau) * self.target)
+
+
 class RawStatePolicy(object):
     """RLlib 'mask_model_rawstate' (rl4rs/nets/rllib/rllib_mask_model.py:67-115 over rllib_rawstate_model.py:25-86): the
     policy reads the RAW state -- category ids [21], dense features [432], sequence ids [2,64] (`rawstate_as_obs`,

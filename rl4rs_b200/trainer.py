@@ -26,7 +26,7 @@ import ctypes as C
 import torch
 import torch.distributed as dist
 
-from .policy import GaussianPolicy, MaskedPolicy, RawStatePolicy
+from .policy import DeterministicActorCritic, GaussianPolicy, MaskedPolicy, RawStatePolicy, counter_draws
 
 
 def _p(t, byte_offset=0):
@@ -681,10 +681,404 @@ class GaussA2CTrainer(A2CTrainer):
     conti = True
 
 
+# ---- DDPG / TD3 ------------------------------------------------------------------------------------------------------
+# RLlib 1.5 ddpg / td3 defaults as modelfree_train.py leaves them (INTEGRATION.md section 3).  train_batch_size None =
+# min(B * max_steps, 1024) over the global batch; exploration_config None = the actor output itself (the DDPG quirk,
+# INTEGRATION.md section 4), or {"type": "OrnsteinUhlenbeckNoise", ...} over OU_DEFAULTS.
+DDPG_DEFAULTS = {"gamma": 1.0, "actor_lr": 1e-3, "critic_lr": 1e-3, "tau": 0.002, "l2_reg": 1e-6, "twin_q": False,
+                 "policy_delay": 1, "smooth_target_policy": False, "target_noise": 0.2, "target_noise_clip": 0.5,
+                 "prioritized_replay": True, "prioritized_replay_alpha": 0.6, "prioritized_replay_beta": 0.4,
+                 "prioritized_replay_eps": 1e-6, "buffer_size": 50000, "learning_starts": 1500,
+                 "timesteps_per_iteration": 1000, "train_batch_size": None, "exploration_config": None}
+TD3_DEFAULTS = dict(DDPG_DEFAULTS, tau=0.005, l2_reg=0.0, twin_q=True, policy_delay=2, smooth_target_policy=True,
+                    prioritized_replay=False, buffer_size=1000000, learning_starts=10000,
+                    exploration_config={"type": "OrnsteinUhlenbeckNoise", "random_timesteps": 10000})
+OU_DEFAULTS = {"ou_theta": 0.15, "ou_sigma": 0.2, "ou_base_scale": 0.1, "initial_scale": 1.0, "final_scale": 0.02,
+               "scale_timesteps": 10000, "random_timesteps": 1000}
+
+
+class ReplayBuffer(object):
+    """RLlib's ReplayBuffer (uniform) / PrioritizedReplayBuffer (proportional) as a device ring: obs f32[C,256], action
+    f32[C,D], reward f32[C], new_obs f32[C,256], done u8[C] and, prioritized, prio f32[C] = p^alpha with max_prio f32[1]
+    (the running max of |td| + eps).  With `ops` (DDPGKernelOps) the csrc/r4_ddpg.cuh kernels do the work; without, this
+    torch code (the CPU path, and the reference of the tests).  The draws are the caller's: u in [0, 1) per sample."""
+
+    def __init__(self, capacity, D, device, prioritized, alpha=0.6, ops=None):
+        e = lambda *s, dt=torch.float32: torch.empty(*s, dtype=dt, device=device)   # untouched slots are never read
+        self.C, self.D, self.device, self.alpha, self.ops = int(capacity), D, device, alpha, ops
+        self.obs, self.action, self.reward = e(self.C, 256), e(self.C, D), e(self.C)
+        self.new_obs, self.done = e(self.C, 256), e(self.C, dt=torch.uint8)
+        self.prio = e(self.C) if prioritized else None
+        self.max_prio = torch.ones(1, dtype=torch.float32, device=device)
+        self.added = 0                      # transitions stored since construction
+
+    @property
+    def size(self):
+        return min(self.added, self.C)
+
+    def store(self, obs, final_obs, action, reward, done):
+        """A [T, B] rollout: row t*B + b -> slot (added + t*B + b) % C, new_obs = the next step's obs, or final_obs."""
+        T, B = reward.shape
+        n = T * B
+        if self.ops is not None:
+            self.ops.replay_store(self, obs, final_obs, action, reward, done)
+        else:
+            nxt = torch.cat([obs[1:].reshape(-1, 256), final_obs.reshape(B, 256)])
+            first = max(0, n - self.C)
+            rows = torch.arange(first, n, device=self.device)
+            slots = (self.added + rows) % self.C
+            for dst, src in ((self.obs, obs.reshape(n, 256)), (self.new_obs, nxt), (self.action, action.reshape(n, -1)),
+                             (self.reward, reward.reshape(n)), (self.done, done.reshape(n))):
+                dst[slots] = src[rows].to(dst.dtype)
+            if self.prio is not None:
+                self.prio[slots] = self.max_prio.pow(self.alpha)
+        self.added += n
+
+    def sample(self, u, beta):
+        """-> (idx i64 [n], importance weights f32 [n]) from the uniforms u [n]."""
+        N = self.size
+        if self.ops is not None:
+            return self.ops.replay_sample(self, u, beta)
+        if self.prio is None:
+            return (u.double() * N).long().clamp(max=N - 1), torch.ones_like(u)
+        p = self.prio[:N].double()
+        cum = torch.cumsum(p, 0)
+        total = cum[-1]
+        idx = torch.searchsorted(cum, u.double() * total, right=True).clamp(max=N - 1)
+        maxw = (p.min() / total * N) ** -beta
+        return idx, ((p[idx] / total * N) ** -beta / maxw).to(torch.float32)
+
+    def update_priorities(self, idx, td, eps):
+        """prio[idx] = (|td| + eps)^alpha, the later position winning for a repeated index."""
+        if self.ops is not None:
+            return self.ops.replay_priorities(self, idx, td, eps)
+        import numpy as np
+        p = td.abs() + eps
+        ix = idx.cpu().numpy()
+        _, rev = np.unique(ix[::-1], return_index=True)
+        keep = torch.as_tensor(len(ix) - 1 - rev, device=self.device)
+        self.prio[idx[keep]] = p[keep].pow(self.alpha)
+        self.max_prio.copy_(torch.maximum(self.max_prio, p.max().reshape(1)))
+
+    def gather(self, idx):
+        return self.obs[idx], self.action[idx], self.reward[idx], self.new_obs[idx], self.done[idx]
+
+
+class DDPGKernelOps(object):
+    """ctypes front of the DDPG / TD3 kernels (include/rl4rs_b200.h: r4_ddpg_* / r4_replay_*): the moments m, v of both
+    Adams (one buffer, split by region), the learner scratch for n samples per step, the loss statistics."""
+
+    def __init__(self, D, twin, device, n_params, n):
+        from . import _capi
+        self.capi, self.lib = _capi, _capi.load_library()
+        self.D, self.twin, self.device, self.n, self.np = D, int(bool(twin)), device, n, n_params
+        assert self.lib.r4_ddpg_num_params(D, self.twin) == n_params
+        z = lambda k: torch.zeros(k, dtype=torch.float32, device=device)
+        self.m, self.v, self.stats = z(n_params), z(n_params), z(3)
+        self.grad, self.td = z(n_params), z(n)
+        self.scratch = z(self.lib.r4_ddpg_scratch_size(D, self.twin, n))
+        self.launches = 0
+
+    _stream = KernelOps._stream
+    _check = KernelOps._check
+
+    def act(self, flat, obs, mode, seed, counter, ou_in, ou_out, theta, sigma, ns, action):
+        rc = self.lib.r4_ddpg_act(_p(flat), _p(obs), obs.shape[0], self.D, mode, seed, counter, _p(ou_in), _p(ou_out), theta,
+                                  sigma, ns, _p(action), self._stream())
+        self._check(rc, "r4_ddpg_act")
+        self.launches += 1
+
+    def _replay(self, rb):
+        return _p(rb.obs), _p(rb.action), _p(rb.reward), _p(rb.new_obs), _p(rb.done)
+
+    def replay_store(self, rb, obs, final_obs, action, reward, done):
+        T, B = reward.shape
+        rc = self.lib.r4_replay_store(*self._replay(rb), _p(rb.prio), _p(rb.max_prio), rb.C, self.D, rb.added, rb.alpha,
+                                      _p(obs), _p(final_obs), _p(action), _p(reward), _p(done), T, B, self._stream())
+        self._check(rc, "r4_replay_store")
+        self.launches += 1
+
+    def replay_sample(self, rb, u, beta):
+        n = u.shape[0]
+        idx = torch.empty(n, dtype=torch.int64, device=self.device)
+        w = torch.empty(n, dtype=torch.float32, device=self.device)
+        rc = self.lib.r4_replay_sample(_p(rb.prio), rb.size, n, beta, _p(u), _p(idx), _p(w), self._stream())
+        self._check(rc, "r4_replay_sample")
+        self.launches += 1
+        return idx, w
+
+    def replay_priorities(self, rb, idx, td, eps):
+        rc = self.lib.r4_replay_update_priorities(_p(rb.prio), _p(rb.max_prio), _p(idx), _p(td), idx.shape[0], rb.alpha, eps,
+                                                  self._stream())
+        self._check(rc, "r4_replay_update_priorities")
+        self.launches += 1
+
+    def grad_(self, pol, rb, idx, weights, noise, hp, inv_n):
+        """self.grad, self.td, self.stats = r4_ddpg_grad over replay rows idx."""
+        rc = self.lib.r4_ddpg_grad(_p(pol.flat), _p(pol.target), self.D, self.twin, *self._replay(rb), _p(idx), _p(weights),
+                                   _p(noise), idx.shape[0], hp["gamma"], hp["target_noise"], hp["noise_clip"], inv_n,
+                                   _p(self.scratch), _p(self.grad), _p(self.td), _p(self.stats), self._stream())
+        self._check(rc, "r4_ddpg_grad")
+        self.launches += 2
+
+    def apply(self, pol, actor_step, critic_step, hp, grad_scale=1.0):
+        rc = self.lib.r4_ddpg_apply(_p(pol.flat), _p(pol.target), _p(self.grad), _p(self.m), _p(self.v), self.D, self.twin,
+                                    actor_step, critic_step, hp["actor_lr"], hp["critic_lr"], hp["l2_reg"], hp["tau"],
+                                    grad_scale, self._stream())
+        self._check(rc, "r4_ddpg_apply")
+        self.launches += 1
+
+    def train_step(self, comm, pol, rb, u, noise, actor_step, critic_step, hp):
+        """One whole SGD step in one library call (sample, gradient, exchange over peer memory, Adams + soft update,
+        priorities)."""
+        rc = self.lib.r4_ddpg_train_step(comm.h if comm is not None else None, _p(pol.flat), _p(pol.target), _p(self.m),
+                                         _p(self.v), self.D, self.twin, *self._replay(rb), _p(rb.prio), _p(rb.max_prio),
+                                         rb.size, u.shape[0], _p(u), _p(noise), hp["beta"], rb.alpha, hp["eps"], hp["gamma"],
+                                         hp["target_noise"], hp["noise_clip"], actor_step, critic_step, hp["actor_lr"],
+                                         hp["critic_lr"], hp["l2_reg"], hp["tau"], _p(self.scratch), _p(self.stats),
+                                         self._stream())
+        self._check(rc, "r4_ddpg_train_step")
+        self.launches += 5 if rb.prio is not None else 4
+        self.launches += 1 if comm is not None else 0
+
+
+class DDPGTrainer(_TrainerBase):
+    """DDPG (RLlib 1.5 DDPGTrainer as modelfree_train.py configures it) over the deterministic actor-critic of the
+    continuous-action env: rollout -> store in the replay -> one SGD step per stored vector episode once `learning_starts`
+    transitions were stored (RLlib's 1:1 round robin); an iteration rolls episodes until it sampled
+    `timesteps_per_iteration`.  On CUDA: the act kernel, the replay kernels and r4_ddpg_train_step (no host round trip per
+    step); on CPU the torch twin.  Data parallel: every rank keeps its own replay and OU state and samples
+    train_batch_size / world per step; the gradient is summed over the ranks (peer memory, or NCCL / gloo all-reduce).
+    The replay is not checkpointed (RLlib 1.5's default): after restore, learning waits for `learning_starts` again."""
+    algo = "DDPG"
+    DEFAULTS = DDPG_DEFAULTS
+
+    def __init__(self, config, env, device=None, seed=0):
+        cfg = config or {}
+        self.config = c = dict(self.DEFAULTS, **{k: v for k, v in cfg.items() if k in self.DEFAULTS})
+        self.env = env
+        self.T, self.B = env.config["max_steps"], env.config["batch_size"]
+        self.D = env.config.get("action_emb_size", 32)
+        self.device = torch.device(device) if device is not None else env.sim.engine.device
+        world = _world()
+        rank = dist.get_rank() if world > 1 else 0
+        ex = dict(self.DEFAULTS["exploration_config"] or {}, **(cfg.get("exploration_config") or {}))
+        self.ou = dict(OU_DEFAULTS, **{k: v for k, v in ex.items() if k != "type"}) \
+            if ex.get("type") == "OrnsteinUhlenbeckNoise" else None
+        self.policy = DeterministicActorCritic(self.D, self.device, seed=seed, twin=c["twin_q"])
+        tb = c["train_batch_size"] or min(self.B * world * self.T, 1024)
+        self.n_local = max(1, tb // world)
+        self.use_kernels = self.device.type == "cuda" and cfg.get("use_kernels", True)
+        self.ops = DDPGKernelOps(self.D, c["twin_q"], self.device, self.policy.n_params, self.n_local) if self.use_kernels else None
+        self.comm = PeerComm(self.policy.n_params, self.device) if self.use_kernels else None
+        self.replay = ReplayBuffer(c["buffer_size"], self.D, self.device, c["prioritized_replay"],
+                                   c["prioritized_replay_alpha"], self.ops)
+        na = self.policy.n_actor
+        self._pa = torch.nn.Parameter(self.policy.flat.data[:na])     # the two optimisers update the flat buffer in place
+        self._pc = torch.nn.Parameter(self.policy.flat.data[na:])
+        self.opt_actor = torch.optim.Adam([self._pa], lr=c["actor_lr"])
+        self.opt_critic = torch.optim.Adam([self._pc], lr=c["critic_lr"])
+        z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=self.device)
+        self.buf_obs, self.buf_action, self.buf_reward = z(self.T, self.B, 256), z(self.T, self.B, self.D), z(self.T, self.B)
+        self.buf_done, self.final_obs = z(self.T, self.B, dt=torch.uint8), z(self.B, 256)
+        self.ou_state = z(2, self.D)        # the OU state and its next value: the act kernel reads one, writes the other
+        self._ou_slot = 0
+        # exploration draws are per rank; the sampling / smoothing draws come from a per-rank generator on the device
+        self._seed = (seed * 1000003 + rank) & 0x7fffffffffffffff
+        self.gen = torch.Generator(device=self.device).manual_seed(seed * 1000003 + rank + 1)
+        self.counter = 0                    # draw counter of the act kernel
+        self.policy_ts = 0                  # global exploring timesteps: the OU scale / random-phase schedule
+        self.actor_steps = self.critic_steps = 0
+        self.iteration = self.timesteps_total = 0
+
+    # ---- acting -------------------------------------------------------------------------------------------------
+    def _ou_scale(self):
+        o = self.ou
+        f = min(max((self.policy_ts - o["random_timesteps"]) / max(o["scale_timesteps"], 1), 0.0), 1.0)
+        return o["initial_scale"] + (o["final_scale"] - o["initial_scale"]) * f
+
+    @torch.no_grad()
+    def _act(self, obs, explore, out):
+        """out [n, D] = the action of obs [n, 256]: the actor output, or OU / random-phase exploration when configured."""
+        n, D = obs.shape[0], self.D
+        mode = 0
+        if explore and self.ou is not None:
+            mode = 2 if self.policy_ts <= self.ou["random_timesteps"] else 1
+        theta, sigma = (self.ou["ou_theta"], self.ou["ou_sigma"]) if self.ou else (0.0, 0.0)
+        ns = self._ou_scale() * self.ou["ou_base_scale"] * 2.0 if mode == 1 else 0.0      # (high - low) = 2
+        x_in, x_out = self.ou_state[self._ou_slot], self.ou_state[1 - self._ou_slot]
+        if self.use_kernels:
+            self.ops.act(self.policy.flat, obs, mode, self._seed, self.counter, x_in, x_out, theta, sigma, ns, out)
+        elif mode == 2:
+            out.copy_(torch.as_tensor(counter_draws(self._seed, self.counter, n, D)[0], dtype=torch.float32))
+        else:
+            a = self.policy.actor(obs)
+            if mode == 1:
+                z = torch.as_tensor(counter_draws(self._seed, self.counter, 1, D)[1][0], dtype=torch.float32, device=obs.device)
+                x_out.copy_(x_in + (theta * -x_in + sigma * z))
+                a = (a + ns * x_out).clamp(-1.0, 1.0)
+            out.copy_(a)
+        if mode == 1:
+            self._ou_slot ^= 1
+        self.counter += n
+        if explore:
+            self.policy_ts += n * _world()
+        return out
+
+    @torch.no_grad()
+    def rollout(self, explore=True):
+        env = self.env
+        obs = env.reset()
+        for t in range(self.T):
+            self.buf_obs[t].copy_(self.policy.inputs(obs)[0])
+            a = self._act(self.buf_obs[t], explore, self.buf_action[t])
+            obs, reward, done, info = env.step(a)
+            self.buf_reward[t].copy_(reward)
+            self.buf_done[t].copy_(torch.as_tensor(done))
+        self.final_obs.copy_(self.policy.inputs(obs)[0])
+        self.reward = self.buf_reward
+        return self
+
+    @torch.no_grad()
+    def compute_actions(self, obs, explore=False):
+        if isinstance(obs, dict) and "obs" not in obs:                 # RLlib's {env_id: observation} form
+            return super().compute_actions(obs, explore)
+        o = torch.as_tensor(self.policy.inputs(obs)[0], dtype=torch.float32, device=self.device).contiguous()
+        out = torch.empty(o.shape[0], self.D, dtype=torch.float32, device=self.device)
+        return self._act(o, explore, out).cpu().numpy()
+
+    # ---- learning -----------------------------------------------------------------------------------------------
+    def _hp(self):
+        c = self.config
+        return {"gamma": c["gamma"], "target_noise": c["target_noise"], "noise_clip": c["target_noise_clip"],
+                "actor_lr": c["actor_lr"], "critic_lr": c["critic_lr"], "l2_reg": c["l2_reg"], "tau": c["tau"],
+                "beta": c["prioritized_replay_beta"], "eps": c["prioritized_replay_eps"]}
+
+    def draws(self):
+        """The caller-side draws of one SGD step: sampling uniforms [n], smoothing normals [n, D] (TD3) or None."""
+        u = torch.rand(self.n_local, generator=self.gen, device=self.device)
+        noise = (torch.randn(self.n_local, self.D, generator=self.gen, device=self.device)
+                 if self.config["smooth_target_policy"] else None)
+        return u, noise
+
+    def sgd_step(self, u, noise):
+        """One SGD step on this rank's replay with the given draws -> the statistics tensor [3] (critic loss, actor loss,
+        mean Q1(s, pi(s)))."""
+        c, hp, rb, w = self.config, self._hp(), self.replay, _world()
+        update_actor = self.critic_steps % c["policy_delay"] == 0
+        self.critic_steps += 1
+        self.actor_steps += int(update_actor)
+        a_step = self.actor_steps if update_actor else 0
+        if self.use_kernels and (w == 1 or self.comm.ok):
+            self.ops.train_step(self.comm if w > 1 else None, self.policy, rb, u, noise, a_step, self.critic_steps, hp)
+            return self.ops.stats
+        idx, wt = rb.sample(u, hp["beta"])
+        weights = wt if rb.prio is not None else None
+        if self.use_kernels:                # NCCL between the gradient and the optimiser
+            self.ops.grad_(self.policy, rb, idx, weights, noise, hp, 1.0 / (self.n_local * w))
+            dist.all_reduce(self.ops.grad, op=dist.ReduceOp.SUM)
+            self.ops.apply(self.policy, a_step, self.critic_steps, hp)
+            td, stats = self.ops.td, self.ops.stats
+        else:
+            td, stats = self.twin_step(*rb.gather(idx), weights, noise, update_actor)
+        if rb.prio is not None:
+            rb.update_priorities(idx, td, hp["eps"])
+        return stats
+
+    def twin_step(self, obs, action, reward, new_obs, done, weights, noise, update_actor):
+        """The torch twin's step over an explicit batch: losses (mean over the global batch), gradient summed over the ranks,
+        l2 terms, torch.optim.Adam for the critic(s) and, unless delayed, the actor, then the soft target update."""
+        c, pol, w = self.config, self.policy, _world()
+        if pol.flat.grad is not None:
+            pol.flat.grad.zero_()
+        cl, al, td = pol.losses(obs, action, reward, new_obs, done, weights, noise, c["gamma"], c["target_noise"],
+                                c["target_noise_clip"], 1.0 / (obs.shape[0] * w))
+        (cl + al).backward()
+        self._allreduce_grad(average=False)
+        g = pol.flat.grad
+        if c["l2_reg"]:
+            g.add_(c["l2_reg"] * pol.flat.detach() * pol.kernel_mask)
+        na = pol.n_actor
+        self._pa.grad, self._pc.grad = g[:na], g[na:]
+        if update_actor:
+            self.opt_actor.step()
+        self.opt_critic.step()
+        pol.soft_update(c["tau"])
+        return td, torch.stack([cl.detach(), al.detach(), -al.detach()])
+
+    def train(self):
+        c, w = self.config, _world()
+        sampled = steps = 0
+        rew, stats = [], torch.zeros(3, dtype=torch.float64, device=self.device)
+        while sampled < c["timesteps_per_iteration"]:
+            self.rollout(explore=True)
+            self.replay.store(self.buf_obs, self.final_obs, self.buf_action, self.buf_reward, self.buf_done)
+            sampled += self.T * self.B * w
+            rew.append(self.buf_reward.sum(0).mean())
+            if self.replay.added * w >= c["learning_starts"]:
+                stats += self.sgd_step(*self.draws()).double()
+                steps += 1
+        self.iteration += 1
+        self.timesteps_total += sampled
+        nan = float("nan")
+        g = self._global_means({"r": torch.stack(rew).mean(), "c": stats[0], "a": stats[1], "q": stats[2]})
+        k = max(steps, 1) / w              # each rank's statistics are its share of the global mean
+        return {"episode_reward_mean": g["r"], "training_iteration": self.iteration, "timesteps_this_iter": sampled,
+                "timesteps_total": self.timesteps_total, "episodes_this_iter": len(rew) * self.B * w, "sgd_steps": steps,
+                "num_steps_trained": self.critic_steps * self.n_local * w, "replay_size": self.replay.size,
+                "critic_loss": g["c"] / k if steps else nan, "actor_loss": g["a"] / k if steps else nan,
+                "mean_q": g["q"] / k if steps else nan}
+
+    # ---- checkpoint ---------------------------------------------------------------------------------------------
+    def save(self, checkpoint_dir):
+        os.makedirs(checkpoint_dir, exist_ok=True)
+        path = os.path.join(checkpoint_dir, "checkpoint_%06d.pt" % self.iteration)
+        kst = {"m": self.ops.m.cpu(), "v": self.ops.v.cpu()} if self.use_kernels else None
+        torch.save({"algo": self.algo, "flat": self.policy.flat.detach().cpu(), "target": self.policy.target.cpu(),
+                    "opt_actor": self.opt_actor.state_dict(), "opt_critic": self.opt_critic.state_dict(), "kernel_adam": kst,
+                    "ou_state": self.ou_state.cpu(), "ou_slot": self._ou_slot, "counter": self.counter,
+                    "policy_ts": self.policy_ts, "actor_steps": self.actor_steps, "critic_steps": self.critic_steps,
+                    "gen": self.gen.get_state(), "iteration": self.iteration, "timesteps_total": self.timesteps_total}, path)
+        return path
+
+    def restore(self, path):
+        st = torch.load(path, map_location="cpu")
+        assert st["algo"] == self.algo
+        with torch.no_grad():
+            self.policy.flat.copy_(st["flat"].to(self.device))
+            self.policy.target.copy_(st["target"].to(self.device))
+            self.ou_state.copy_(st["ou_state"].to(self.device))
+        self.opt_actor.load_state_dict(st["opt_actor"])
+        self.opt_critic.load_state_dict(st["opt_critic"])
+        if self.use_kernels and st.get("kernel_adam"):
+            self.ops.m.copy_(st["kernel_adam"]["m"]); self.ops.v.copy_(st["kernel_adam"]["v"])
+        self.gen.set_state(st["gen"])
+        for k in ("counter", "policy_ts", "actor_steps", "critic_steps", "iteration", "timesteps_total"):
+            setattr(self, k, st[k])
+        self._ou_slot = st["ou_slot"]
+
+
+class TD3Trainer(DDPGTrainer):
+    """TD3: DDPGTrainer with RLlib 1.5's TD3 defaults (twin critics with the min target, policy_delay 2, target policy
+    smoothing, uniform replay of 10^6, OU exploration after 10 000 random timesteps)."""
+    algo = "TD3"
+    DEFAULTS = TD3_DEFAULTS
+
+
 def get_rl_model(algo, rllib_config, env=None, **kw):
     """script/modelfree_trainer.py:11-36.  Only the algorithms of the BASELINE configs are built.  On an env built with
-    support_conti_env, PPO / A2C (and PPO_conti / A2C_conti, modelfree_train.py:46-48) train the Gaussian policy."""
+    support_conti_env, PPO / A2C (and PPO_conti / A2C_conti, modelfree_train.py:46-48) train the Gaussian policy, and
+    DDPG / TD3 (modelfree_trainer.py:25-28) the deterministic actor-critic."""
     conti = env is not None and bool(env.config.get("support_conti_env", False))
+    if algo.replace("_rawstate", "") in ("DDPG", "TD3"):
+        if algo.endswith("_rawstate") or (env is not None and env.config.get("rawstate_as_obs", False)):
+            raise NotImplementedError("%s on a rawstate_as_obs env (model_rawstate) is not built" % algo)
+        if not conti:
+            raise ValueError("%s needs an env built with support_conti_env=True (modelfree_train.py:46-48)" % algo)
+        if env.config.get("support_rllib_mask", False):
+            raise ValueError("%s takes the plain observation: build the env with support_rllib_mask=False "
+                             "(the reference turns the mask off for DDPG / TD3, modelfree_train.py:46-48)" % algo)
+        return (DDPGTrainer if algo == "DDPG" else TD3Trainer)(rllib_config, env, **kw)
     if algo.endswith("_conti") or (conti and algo in ("PPO", "A2C")):
         base = algo[:-len("_conti")] if algo.endswith("_conti") else algo
         if base not in ("PPO", "A2C"):
