@@ -365,6 +365,54 @@ int r4_ddpg_train_step(r4_comm* comm, float* params, float* target, float* m, fl
                        float noise_clip, int actor_step, int critic_step, float actor_lr, float critic_lr, float l2_reg,
                        float tau, float* scratch, float* stats, void* stream);
 
+/* ---- RAINBOW on the discrete env (modelfree_train.py:50-51,146-178; RLlib 1.5 DQN defaults with num_atoms 8, v_min 0,
+ * v_max 1000, n_step 3, noisy off, INTEGRATION.md section 3): the plain obs(256) -> 256 tanh -> 256 tanh trunk, an
+ * advantage stream -> 128 relu -> A x atoms and a state-score stream -> 128 relu -> atoms, combined as
+ * logits[a][k] = score[k] + adv[a][k] - mean_a adv[a][k]; Q(s, a) = sum_k z_k softmax(logits[a])_k with
+ * z_k = v_min + k (v_max - v_min) / (atoms - 1).  A = num_actions in 2..512, atoms in 2..32, A x atoms <= 4096.
+ * Flat parameter layout (r4_rainbow_num_params(A, atoms) floats; 491 496 at A = 284, atoms = 8):
+ * trunk     w1[256,256] b1[256] w2[256,256] b2[256] |
+ * advantage aw1[256,128] ab1[128] aw2[128,A*atoms] ab2[A*atoms] |
+ * score     sw1[256,128] sb1[128] sw2[128,atoms] sb2[atoms].
+ * The target parameters have the same layout.  Stateless: every pointer is caller-owned DEVICE memory. */
+int r4_rainbow_num_params(int num_actions, int num_atoms);
+/* floats of the scratch r4_rainbow_grad / r4_rainbow_train_step need for batches of up to n samples; -1 for bad arguments */
+int64_t r4_rainbow_scratch_size(int num_actions, int num_atoms, int n);
+/* The network on obs f32[n,256] -> action i32[n] and, when q != NULL, Q f32[n,A].  explore 0: the first argmax of Q.
+ * explore 1: SoftQ (temperature 1), a ~ softmax(Q) by inverse CDF over one uniform per row, the top 24 bits of splitmix64
+ * keyed by seed and (counter + row) << 6, so the same seed and counter reproduce the actions. */
+int r4_rainbow_act(const float* params, const float* obs, int n, int num_actions, int num_atoms, float v_min, float v_max,
+                   int explore, uint64_t seed, uint64_t counter, int32_t* action, float* q, void* stream);
+/* The replay store of r4_replay_store with integer actions (action ring i32[C], rollout action i32[T*B]) and RLlib's
+ * n-step fold per episode: row t keeps sum_{j < n_step, t + j < T} gamma^j reward[t + j] (the original rewards, added in j
+ * order), and the new_obs and done of row min(t + n_step - 1, T - 1).  n_step = 1 stores the rows as they are. */
+int r4_replay_store_nstep(float* r_obs, int32_t* r_action, float* r_reward, float* r_new_obs, uint8_t* r_done, float* r_prio,
+                          const float* max_prio, int capacity, int64_t pos, float alpha, int n_step, float gamma,
+                          const float* obs, const float* final_obs, const int32_t* action, const float* reward,
+                          const uint8_t* done, int T, int B, void* stream);
+/* Gradient of the distributional loss over the replay rows idx[0..n) (weights f32[n] may be NULL = 1): a* = argmax of the
+ * online Q(s', .), p' = the target net's distribution at (s', a*), m = its projection of clip(r + gamma_n (1 - done) z,
+ * v_min, v_max) onto the support (RLlib's QLoss, gamma_n = gamma^n_step), td = -sum_k m_k log p(s, a)_k, loss =
+ * sum_i w_i td_i * inv_n.  grad f32[num_params] receives the gradient (deterministic: one writer per element), td f32[n]
+ * (may be NULL) the td errors, stats f32[3] (may be NULL) {loss, mean td, mean Q(s, a)}, each sum times inv_n.  2 launches. */
+int r4_rainbow_grad(const float* params, const float* target, int num_actions, int num_atoms, float v_min, float v_max,
+                    const float* r_obs, const int32_t* r_action, const float* r_reward, const float* r_new_obs,
+                    const uint8_t* r_done, const int64_t* idx, const float* weights, int n, float gamma_n, float inv_n,
+                    float* scratch, float* grad, float* td, float* stats, void* stream);
+/* The optimiser step in one launch: each of the 12 tensors' gradient scaled by grad_clip / ||g|| where its norm exceeds
+ * grad_clip (per tensor, RLlib's minimize_and_clip; grad_clip <= 0: off), torch.optim.Adam (betas 0.9 / 0.999, eps
+ * adam_eps) at the 1-based step, then target = params when copy_target != 0 (the hard target update). */
+int r4_rainbow_apply(float* params, float* target, const float* grad, float* m, float* v, int num_actions, int num_atoms,
+                     int step, float lr, float adam_eps, float grad_clip, int copy_target, void* stream);
+/* One SGD step with no host round trip: r4_replay_sample (n indices from u), r4_rainbow_grad, over peer memory the sum over
+ * the ranks (comm != NULL; loss = mean over n x world samples; comm created with r4_rainbow_num_params), r4_rainbow_apply
+ * and, with prio != NULL, r4_replay_update_priorities from td.  stats (may be NULL) as r4_rainbow_grad.  5 launches. */
+int r4_rainbow_train_step(r4_comm* comm, float* params, float* target, float* m, float* v, int num_actions, int num_atoms,
+                          float v_min, float v_max, const float* r_obs, const int32_t* r_action, const float* r_reward,
+                          const float* r_new_obs, const uint8_t* r_done, float* r_prio, float* max_prio, int size, int n,
+                          const float* u, float beta, float alpha, float prio_eps, float gamma_n, int step, float lr,
+                          float adam_eps, float grad_clip, int copy_target, float* scratch, float* stats, void* stream);
+
 /* ---- the simulator alone (nets/dien.py:8-45), for parity tests and kernel benchmarks ------- */
 /* seq i32[R,2,64], dense f32[R,432], cat i32[R,21] (device) -> obs f32[R,256], probs f32[R,2]
  * (either may be NULL).  Runs the uncached path: GRU-1 is recomputed for every row. */

@@ -95,6 +95,18 @@ EXPORTS = {
     "r4_ddpg_apply": (C.c_int, [C.c_void_p] * 5 + [C.c_int] * 4 + [C.c_float] * 5 + [C.c_void_p]),
     "r4_ddpg_train_step": (C.c_int, [C.c_void_p] * 5 + [C.c_int, C.c_int] + [C.c_void_p] * 7 + [C.c_int, C.c_int] +
                            [C.c_void_p] * 2 + [C.c_float] * 6 + [C.c_int, C.c_int] + [C.c_float] * 4 + [C.c_void_p] * 3),
+    "r4_rainbow_num_params": (C.c_int, [C.c_int, C.c_int]),
+    "r4_rainbow_scratch_size": (C.c_int64, [C.c_int, C.c_int, C.c_int]),
+    "r4_rainbow_act": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int, C.c_uint64,
+                                 C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "r4_replay_store_nstep": (C.c_int, [C.c_void_p] * 7 + [C.c_int, C.c_int64, C.c_float, C.c_int, C.c_float] +
+                              [C.c_void_p] * 5 + [C.c_int, C.c_int, C.c_void_p]),
+    "r4_rainbow_grad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float] + [C.c_void_p] * 7 +
+                        [C.c_int, C.c_float, C.c_float] + [C.c_void_p] * 5),
+    "r4_rainbow_apply": (C.c_int, [C.c_void_p] * 5 + [C.c_int] * 3 + [C.c_float] * 3 + [C.c_int, C.c_void_p]),
+    "r4_rainbow_train_step": (C.c_int, [C.c_void_p] * 5 + [C.c_int, C.c_int, C.c_float, C.c_float] + [C.c_void_p] * 7 +
+                              [C.c_int, C.c_int, C.c_void_p] + [C.c_float] * 4 + [C.c_int, C.c_float, C.c_float, C.c_float,
+                                                                                  C.c_int] + [C.c_void_p] * 3),
     "r4_adam_step": (C.c_int,[C.c_void_p] * 4 + [C.c_int, C.c_int] + [C.c_float] * 6 + [C.c_void_p, C.c_void_p]),
     "r4_dien_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
 }

@@ -10,6 +10,7 @@
 #include "r4_comm.cuh"
 #include "r4_gauss.cuh"
 #include "r4_ddpg.cuh"
+#include "r4_rainbow.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -1555,6 +1556,112 @@ int r4_ddpg_train_step(r4_comm* comm, float* params, float* target, float* m, fl
   }
   rc = r4_ddpg_apply(params, target, g, m, v, action_dim, twin, actor_step, critic_step, actor_lr, critic_lr, l2_reg, tau, 1.0f,
                      stream);
+  if (rc || !r_prio) return rc;
+  return r4_replay_update_priorities(r_prio, max_prio, P.idx, P.td, n, alpha, prio_eps, stream);
+}
+
+// ---- RAINBOW (r4_rainbow.cuh) ---------------------------------------------------------------------------------
+static bool rainbow_dims_ok(int A, int Z) {
+  return A >= 2 && A <= r4rb::MAXA && Z >= 2 && Z <= r4rb::MAXZ && A * Z <= r4rb::MAXAZ;
+}
+
+int r4_rainbow_num_params(int num_actions, int num_atoms) {
+  return rainbow_dims_ok(num_actions, num_atoms) ? r4rb::make_layout(num_actions, num_atoms).n : -1;
+}
+
+int64_t r4_rainbow_scratch_size(int num_actions, int num_atoms, int n) {
+  if (!rainbow_dims_ok(num_actions, num_atoms) || n < 1) return -1;
+  return (int64_t)r4rb::scratch_floats(r4rb::make_layout(num_actions, num_atoms), n);
+}
+
+int r4_rainbow_act(const float* params, const float* obs, int n, int num_actions, int num_atoms, float v_min, float v_max,
+                   int explore, uint64_t seed, uint64_t counter, int32_t* action, float* q, void* stream) {
+  if (!params || !obs || !action || n < 1 || !rainbow_dims_ok(num_actions, num_atoms) || !(v_max > v_min))
+    return fail(nullptr, R4_ERR_ARG, "r4_rainbow_act: bad argument (actions 2..512, atoms 2..32, actions x atoms <= 4096)");
+  static bool attr = false;
+  if (int rc = ddpg_smem((const void*)r4rb::k_rainbow_act, r4rb::act_smem(r4rb::MAXA, r4rb::MAXAZ), "k_rainbow_act", attr))
+    return rc;
+  const r4rb::Layout L = r4rb::make_layout(num_actions, num_atoms);
+  r4rb::k_rainbow_act<<<(n + r4rb::TS - 1) / r4rb::TS, r4rb::NT, r4rb::act_smem(L.A, L.AZ), S(stream)>>>(
+      L, params, obs, n, v_min, (v_max - v_min) / (float)(num_atoms - 1), explore != 0, seed, counter, action, q);
+  R4_PCHECK("k_rainbow_act");
+  return R4_OK;
+}
+
+int r4_replay_store_nstep(float* r_obs, int32_t* r_action, float* r_reward, float* r_new_obs, uint8_t* r_done, float* r_prio,
+                          const float* max_prio, int capacity, int64_t pos, float alpha, int n_step, float gamma,
+                          const float* obs, const float* final_obs, const int32_t* action, const float* reward,
+                          const uint8_t* done, int T, int B, void* stream) {
+  if (!r_obs || !r_action || !r_reward || !r_new_obs || !r_done || (r_prio && !max_prio) || capacity < 1 || pos < 0 ||
+      n_step < 1 || !obs || !final_obs || !action || !reward || !done || T < 1 || B < 1)
+    return fail(nullptr, R4_ERR_ARG, "r4_replay_store_nstep: bad argument");
+  const int64_t rows = std::min<int64_t>((int64_t)T * B, capacity);
+  r4rb::k_replay_store_nstep<<<(unsigned)rows, 64, 0, S(stream)>>>(r_obs, r_action, r_reward, r_new_obs, r_done, r_prio,
+                                                                   max_prio, capacity, pos, alpha, n_step, gamma, obs,
+                                                                   final_obs, action, reward, done, T, B);
+  R4_PCHECK("k_replay_store_nstep");
+  return R4_OK;
+}
+
+int r4_rainbow_grad(const float* params, const float* target, int num_actions, int num_atoms, float v_min, float v_max,
+                    const float* r_obs, const int32_t* r_action, const float* r_reward, const float* r_new_obs,
+                    const uint8_t* r_done, const int64_t* idx, const float* weights, int n, float gamma_n, float inv_n,
+                    float* scratch, float* grad, float* td, float* stats, void* stream) {
+  if (!params || !target || !rainbow_dims_ok(num_actions, num_atoms) || !(v_max > v_min) || !r_obs || !r_action ||
+      !r_reward || !r_new_obs || !r_done || !idx || n < 1 || !scratch || !grad)
+    return fail(nullptr, R4_ERR_ARG, "r4_rainbow_grad: bad argument");
+  static bool attr = false;
+  if (int rc = ddpg_smem((const void*)r4rb::k_rainbow_rows, r4rb::rows_smem(r4rb::MAXA, r4rb::MAXAZ), "k_rainbow_rows", attr))
+    return rc;
+  const r4rb::Layout L = r4rb::make_layout(num_actions, num_atoms);
+  r4rb::Planes P = r4rb::make_planes(scratch, L, n);
+  if (td) P.td = td;
+  const r4ddpg::Jobs J = r4rb::make_jobs(L, P);
+  const r4rb::Replay R{r_obs, r_action, r_reward, r_new_obs, r_done};
+  const r4rb::Hyper hp{v_min, v_max, (v_max - v_min) / (float)(num_atoms - 1), gamma_n, inv_n};
+  r4rb::k_rainbow_rows<<<(n + r4rb::TS - 1) / r4rb::TS, r4rb::NT, r4rb::rows_smem(L.A, L.AZ), S(stream)>>>(
+      L, hp, params, target, R, idx, weights, n, P);
+  R4_PCHECK("k_rainbow_rows");
+  r4ddpg::k_ddpg_wgrad<<<J.ntiles + 1, r4ddpg::NT, 0, S(stream)>>>(J, n, grad, P.stats, stats, inv_n);
+  R4_PCHECK("k_ddpg_wgrad");
+  return R4_OK;
+}
+
+int r4_rainbow_apply(float* params, float* target, const float* grad, float* m, float* v, int num_actions, int num_atoms,
+                     int step, float lr, float adam_eps, float grad_clip, int copy_target, void* stream) {
+  if (!params || !target || !grad || !m || !v || !rainbow_dims_ok(num_actions, num_atoms) || step < 1)
+    return fail(nullptr, R4_ERR_ARG, "r4_rainbow_apply: bad argument");
+  const r4rb::Split Sp = r4rb::make_split(r4rb::make_layout(num_actions, num_atoms));
+  r4rb::k_rainbow_apply<<<Sp.cta0[r4rb::NTEN], r4rb::ANT, 0, S(stream)>>>(Sp, params, target, grad, m, v, step, lr, adam_eps,
+                                                                        grad_clip, copy_target != 0);
+  R4_PCHECK("k_rainbow_apply");
+  return R4_OK;
+}
+
+int r4_rainbow_train_step(r4_comm* comm, float* params, float* target, float* m, float* v, int num_actions, int num_atoms,
+                          float v_min, float v_max, const float* r_obs, const int32_t* r_action, const float* r_reward,
+                          const float* r_new_obs, const uint8_t* r_done, float* r_prio, float* max_prio, int size, int n,
+                          const float* u, float beta, float alpha, float prio_eps, float gamma_n, int step, float lr,
+                          float adam_eps, float grad_clip, int copy_target, float* scratch, float* stats, void* stream) {
+  if (!scratch || !rainbow_dims_ok(num_actions, num_atoms) || n < 1 || (r_prio && !max_prio))
+    return fail(nullptr, R4_ERR_ARG, "r4_rainbow_train_step: bad argument");
+  const r4rb::Layout L = r4rb::make_layout(num_actions, num_atoms);
+  const r4rb::Planes P = r4rb::make_planes(scratch, L, n);
+  const int world = comm ? comm->world : 1;
+  int rc = r4_replay_sample(r_prio, size, n, beta, u, P.idx, P.weights, stream);
+  if (rc) return rc;
+  rc = r4_rainbow_grad(params, target, num_actions, num_atoms, v_min, v_max, r_obs, r_action, r_reward, r_new_obs, r_done,
+                       P.idx, r_prio ? P.weights : nullptr, n, gamma_n, 1.0f / ((float)n * world), scratch, P.grad, nullptr,
+                       stats, stream);
+  if (rc) return rc;
+  const float* g = P.grad;
+  if (comm) {        // one partial (G = 1) per rank, summed in rank order into the scratch's second gradient
+    float* sum = P.grad + L.n + 5;
+    if ((rc = exchange_launch(comm, P.grad, 1, L.n, sum, nullptr, 0.f, 0, nullptr, nullptr, nullptr, 0, 0.f, 0.f, 0.f, 0.f, stream)))
+      return rc;
+    g = sum;
+  }
+  rc = r4_rainbow_apply(params, target, g, m, v, num_actions, num_atoms, step, lr, adam_eps, grad_clip, copy_target, stream);
   if (rc || !r_prio) return rc;
   return r4_replay_update_priorities(r_prio, max_prio, P.idx, P.td, n, alpha, prio_eps, stream);
 }

@@ -278,6 +278,120 @@ class DeterministicActorCritic(object):
         self.target.copy_(tau * self.flat.detach() + (1.0 - tau) * self.target)
 
 
+class DistributionalQNetwork(object):
+    """The Q network RLlib 1.5 builds for RAINBOW on the plain 256-d observation (modelfree_train.py:146-178, no custom
+    model): the default FullyConnectedNetwork with no_final_linear, obs(256) -> 256 tanh -> 256 tanh (normc(1.0) kernels,
+    zero biases), and the dueling distributional head (hiddens [128], Keras glorot-uniform kernels, zero biases):
+        advantage   256 -> 128 relu -> A * atoms          state score   256 -> 128 relu -> atoms
+        logits[a][k] = score[k] + (adv[a][k] - mean_a adv[a][k]),  Q(s, a) = sum_k z_k softmax(logits[a])_k,
+    z = v_min + k dz, dz = (v_max - v_min) / (atoms - 1) in float32.  One flat buffer (csrc/r4_rainbow.cuh's layout) and a
+    target copy of it (hard copy at construction).  This torch twin is the CPU path of RainbowTrainer and the autograd
+    cross-check of the kernels (tests/test_gpu_trainer_rainbow.py)."""
+
+    HT, HQ = 256, 128
+
+    def __init__(self, action_size=284, device="cuda", seed=0, num_atoms=8, v_min=0.0, v_max=1000.0):
+        import numpy as np
+        self.A, self.atoms, self.v_min, self.v_max = action_size, num_atoms, float(v_min), float(v_max)
+        self.device = torch.device(device)
+        A, Z, HT, HQ = action_size, num_atoms, self.HT, self.HQ
+        shapes = [("w1", (OBS, HT)), ("b1", (HT,)), ("w2", (HT, HT)), ("b2", (HT,)),
+                  ("aw1", (HT, HQ)), ("ab1", (HQ,)), ("aw2", (HQ, A * Z)), ("ab2", (A * Z,)),
+                  ("sw1", (HT, HQ)), ("sb1", (HQ,)), ("sw2", (HQ, Z)), ("sb2", (Z,))]
+        n = sum(math.prod(s) for _, s in shapes)
+        g = torch.Generator(device="cpu").manual_seed(seed)
+        self.flat = torch.zeros(n, dtype=torch.float32, device=self.device, requires_grad=True)
+        self.slices, off = [], 0
+        with torch.no_grad():
+            for name, shape in shapes:
+                k = math.prod(shape)
+                v = self.flat[off:off + k].view(shape)
+                if name in ("w1", "w2"):               # normc_initializer(1.0)
+                    w = torch.randn(shape, generator=g)
+                    v.copy_((w / w.pow(2).sum(0, keepdim=True).sqrt()).to(self.device))
+                elif len(shape) == 2:                  # glorot uniform
+                    lim = math.sqrt(6.0 / (shape[0] + shape[1]))
+                    v.copy_(((torch.rand(shape, generator=g) * 2 - 1) * lim).to(self.device))
+                self.slices.append((off, off + k))
+                off += k
+        self._shapes, self.n_params = shapes, n
+        self.target = self.flat.detach().clone()
+        # the support in float32, formed as the kernels form it (the projection's floor / ceil must agree bit for bit)
+        dz = np.float32(np.float32(self.v_max) - np.float32(self.v_min)) / np.float32(Z - 1)
+        self.dz = torch.tensor(dz, dtype=torch.float32, device=self.device)
+        self.z = torch.tensor(np.float32(self.v_min), device=self.device) + torch.arange(Z, dtype=torch.float32,
+                                                                                          device=self.device) * self.dz
+
+    params = DeterministicActorCritic.params
+
+    def forward(self, obs, flat=None):
+        """obs f32 [n,256] -> (support logits [n, A, atoms], Q [n, A])."""
+        p = self.params(flat)
+        h = torch.tanh(torch.tanh(obs @ p["w1"] + p["b1"]) @ p["w2"] + p["b2"])
+        adv = (torch.relu(h @ p["aw1"] + p["ab1"]) @ p["aw2"] + p["ab2"]).view(-1, self.A, self.atoms)
+        score = torch.relu(h @ p["sw1"] + p["sb1"]) @ p["sw2"] + p["sb2"]
+        logits = score.unsqueeze(1) + (adv - adv.mean(1, keepdim=True))
+        return logits, (torch.softmax(logits, -1) * self.z).sum(-1)
+
+    def inputs(self, obs):
+        return (obs["obs"] if isinstance(obs, dict) else obs,)
+
+    def project(self, reward, done, probs, gamma_n):
+        """RLlib QLoss's categorical projection: the target distribution probs [n, atoms] moved to r + gamma_n (1 - done) z,
+        clipped to [v_min, v_max], split over the neighbouring atoms -> m [n, atoms].  Mass on an index off the support is
+        dropped, as tf.one_hot drops it."""
+        Z = self.atoms
+        nd = gamma_n * (1.0 - done.to(torch.float32))
+        rt = (reward.to(torch.float32).unsqueeze(1) + nd.unsqueeze(1) * self.z).clamp(self.v_min, self.v_max)
+        b = (rt - self.v_min) / self.dz
+        lb, ub = torch.floor(b), torch.ceil(b)
+        feq = (ub - lb < 0.5).to(torch.float32)
+        ml, mu = probs * (ub - b + feq), probs * (b - lb)
+        m = torch.zeros_like(probs)
+        for j in range(Z):                             # in atom order, as the kernel adds them
+            for i, w in ((lb[:, j].long(), ml[:, j]), (ub[:, j].long(), mu[:, j])):
+                ok = (i >= 0) & (i < Z)
+                m.scatter_add_(1, i.clamp(0, Z - 1).unsqueeze(1), torch.where(ok, w, torch.zeros_like(w)).unsqueeze(1))
+        return m
+
+    def loss(self, obs, action, reward, new_obs, done, weights=None, gamma_n=1.0, inv_n=None):
+        """The distributional double-Q loss sum_i w_i td_i * inv_n (default 1/n), td = softmax cross entropy of the projected
+        target (labels) and the taken action's logits -> (loss, td [n])."""
+        n = obs.shape[0]
+        inv_n = 1.0 / n if inv_n is None else inv_n
+        rows = torch.arange(n, device=obs.device)
+        with torch.no_grad():
+            a_star = self.forward(new_obs)[1].argmax(1)
+            pt = torch.softmax(self.forward(new_obs, self.target)[0][rows, a_star], -1)
+            m = self.project(reward, done, pt, gamma_n)
+        logits = self.forward(obs)[0][rows, action.long()]
+        td = -(m * torch.log_softmax(logits, -1)).sum(-1)
+        w = torch.ones(n, device=obs.device) if weights is None else weights
+        return (w * td).sum() * inv_n, td.detach()
+
+    @torch.no_grad()
+    def clip_per_tensor(self, grad, clip):
+        """RLlib's minimize_and_clip: every tensor's gradient whose norm exceeds clip is scaled to norm clip, on its own."""
+        if clip:
+            for lo, hi in self.slices:
+                g = grad[lo:hi]
+                norm = g.norm()
+                if float(norm) > clip:
+                    g.mul_(clip / norm)
+
+    @torch.no_grad()
+    def act(self, obs, explore, seed=0, counter=0):
+        """-> (action i32 [n], Q [n, A]): argmax Q, or SoftQ (a ~ softmax(Q)) over csrc/r4_rainbow.cuh's uniform per row."""
+        import numpy as np
+        q = self.forward(obs)[1]
+        if not explore:
+            return q.argmax(1).to(torch.int32), q
+        u = (counter_draws(seed, counter, q.shape[0], 1)[0][:, 0] + 1.0) / 2.0       # the top 24 bits / 2^24
+        cdf = np.cumsum(torch.softmax(q.double(), 1).cpu().numpy(), 1)
+        a = np.minimum((cdf <= (u * cdf[:, -1])[:, None]).sum(1), self.A - 1)
+        return torch.as_tensor(a, dtype=torch.int32, device=q.device), q
+
+
 class RawStatePolicy(object):
     """RLlib 'mask_model_rawstate' (rl4rs/nets/rllib/rllib_mask_model.py:67-115 over rllib_rawstate_model.py:25-86): the
     policy reads the RAW state -- category ids [21], dense features [432], sequence ids [2,64] (`rawstate_as_obs`,
