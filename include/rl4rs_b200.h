@@ -413,6 +413,68 @@ int r4_rainbow_train_step(r4_comm* comm, float* params, float* target, float* m,
                           const float* u, float beta, float alpha, float prio_eps, float gamma_n, int step, float lr,
                           float adam_eps, float grad_clip, int copy_target, float* scratch, float* stats, void* stream);
 
+/* ---- batch RL on the logged dataset (batchrl_trainer.py:34-90; d3rlpy 0.91 DiscreteBC / DiscreteBCQ / DiscreteCQL as the
+ * reference configures them, INTEGRATION.md section 3).  algo 0 BC, 1 BCQ, 2 CQL; obs_dim K in 11..4096 (the d3rl
+ * observation: simulator obs | 9 prev actions | cur_steps), A = action_size in 2..512, with the shared planes within
+ * 226 KB (every K at A = 284; K <= 2998 at A = 512).  Flat parameter layout:
+ * masked net  w1[K,256] b1[256] emb[A,32] w2[576,A] b2[A] w3[A,A] b3[A]   (the custom encoder with_q + d3rlpy's head)
+ * plain net   w1[K,256] b1[256] w2[256,256] b2[256] w3[256,A] b3[A]      (d3rlpy's default encoder + head)
+ * BC: masked (imitator); BCQ: masked (Q) | masked (imitator); CQL: plain.  The target holds the Q part only
+ * (r4_batchrl_target_size floats: 0 for BC).  Stateless: every pointer is caller-owned DEVICE memory. */
+typedef struct {
+  const float* obs;            /* f32[N, K] */
+  const int32_t* action;       /* i32[N] */
+  const float* reward;         /* f32[N] */
+  const uint8_t* terminal;     /* u8[N] */
+  const int64_t* transitions;  /* i64[T] from r4_batchrl_transitions */
+  const uint8_t* location_mask;/* u8[3, A]: 1 where the page layer allows the item */
+  const uint8_t* special;      /* u8[A]: 1 for the special items */
+} r4_batchrl_data;
+typedef struct {
+  float gamma;                 /* discount */
+  float beta;                  /* the imitator's penalty beta * mean(z^2) (BC 0 in the script, BCQ 0.5) */
+  float alpha;                 /* CQL's conservative weight */
+  float log_flex;              /* log(action_flexibility) of BCQ (log 0.3) */
+  float reward_mean, reward_den;   /* CQL's reward scaler r' = (r - mean) / den (0, 1: off) */
+} r4_batchrl_hyper;
+int r4_batchrl_num_params(int algo, int obs_dim, int action_size);
+int r4_batchrl_target_size(int algo, int obs_dim, int action_size);
+/* floats of the scratch r4_batchrl_grad / r4_batchrl_epoch need for minibatches of up to n samples; -1 for bad arguments */
+int64_t r4_batchrl_scratch_size(int algo, int obs_dim, int action_size, int n);
+/* index i64[N] receives, in order, every entry i with terminal[i] == 0 that lies before the last terminal entry (the first
+ * entry of each transition (obs[i], action[i], reward[i + 1], obs[i + 1], terminal[i + 1]) of d3rlpy's episodes, split at
+ * the terminals); count i64[1] (device) receives how many.  1 launch. */
+int r4_batchrl_transitions(const uint8_t* terminal, int64_t N, int64_t* index, int64_t* count, void* stream);
+/* The gradient of the algorithm's loss (the minibatch mean) over the transitions data->transitions[idx[0..n)] -> grad
+ * f32[num_params] (deterministic: one writer per element) and stats f32[3] (may be NULL): {loss, td or nll term, Q(s, a)
+ * or the imitator's mean z^2}, each a minibatch mean.  3 launches. */
+int r4_batchrl_grad(int algo, int obs_dim, int action_size, const float* params, const float* target,
+                    const r4_batchrl_data* data, const r4_batchrl_hyper* hp, const int64_t* idx, int n, float* scratch,
+                    float* grad, float* stats, void* stream);
+/* torch.optim.Adam (betas 0.9 / 0.999, no clipping) at the 1-based step, then target = the Q part of params when
+ * copy_target != 0.  1 launch. */
+int r4_batchrl_apply(int algo, int obs_dim, int action_size, float* params, float* target, const float* grad, float* m,
+                     float* v, int step, float lr, float adam_eps, int copy_target, void* stream);
+/* One epoch of d3rlpy's RoundIterator with no host round trip: minibatch k is perm[k mb .. (k + 1) mb) for k < n_perm / mb
+ * (the last partial minibatch dropped); each runs r4_batchrl_grad and r4_batchrl_apply at step step0 + k + 1, copying the
+ * target after the steps whose 0-based index is a multiple of target_interval (target_interval <= 0: never).  stats
+ * (may be NULL) receives f32[steps, 3].  Chained by programmatic dependent launch.  Returns the number of steps, or an
+ * r4_status. */
+int r4_batchrl_epoch(int algo, int obs_dim, int action_size, float* params, float* target, float* m, float* v,
+                     const r4_batchrl_data* data, const r4_batchrl_hyper* hp, const int64_t* perm, int64_t n_perm, int mb,
+                     int step0, float lr, float adam_eps, int target_interval, float* scratch, float* stats, void* stream);
+/* kernels launched so far by the r4_batchrl_* entry points in this process (for launch-count measurements) */
+int64_t r4_batchrl_launch_count(void);
+/* The act rule on n observations (obs_f64 != 0: f64[n, K], as the env's 'torch' output; else f32[n, K]) -> action
+ * i32[n].  mode 0: rl4rs policy_model.predict_with_mask (action_probs = BC's log-probs or softmax(Q), -2^15 where the
+ * location layer cur_steps % 9 / 3, the 9 prev actions or, when one of them is special, the special items rule an item
+ * out, the first argmax); mode 1: d3rlpy's predict (BC argmax log-prob, BCQ the imitator-filtered argmax of Q, CQL argmax Q).
+ * probs f32[n, A] (may be NULL) receives action_probs, values f32[n, A] (may be NULL) the raw output (BC logits, else Q).
+ * Only data->location_mask and data->special are read.  1 launch. */
+int r4_batchrl_act(int algo, int obs_dim, int action_size, const float* params, const void* obs, int obs_f64, int n,
+                   const r4_batchrl_data* data, int mode, float log_flex, int32_t* action, float* probs, float* values,
+                   void* stream);
+
 /* ---- the simulator alone (nets/dien.py:8-45), for parity tests and kernel benchmarks ------- */
 /* seq i32[R,2,64], dense f32[R,432], cat i32[R,21] (device) -> obs f32[R,256], probs f32[R,2]
  * (either may be NULL).  Runs the uncached path: GRU-1 is recomputed for every row. */

@@ -28,6 +28,14 @@ class R4Out(C.Structure):
         "masked_actions")]
 
 
+class BatchRLData(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("obs", "action", "reward", "terminal", "transitions", "location_mask", "special")]
+
+
+class BatchRLHyper(C.Structure):
+    _fields_ = [(n, C.c_float) for n in ("gamma", "beta", "alpha", "log_flex", "reward_mean", "reward_den")]
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     "r4_create": (C.c_int, [C.POINTER(R4Config), C.c_int, C.POINTER(C.c_void_p)]),
@@ -107,6 +115,19 @@ EXPORTS = {
     "r4_rainbow_train_step": (C.c_int, [C.c_void_p] * 5 + [C.c_int, C.c_int, C.c_float, C.c_float] + [C.c_void_p] * 7 +
                               [C.c_int, C.c_int, C.c_void_p] + [C.c_float] * 4 + [C.c_int, C.c_float, C.c_float, C.c_float,
                                                                                   C.c_int] + [C.c_void_p] * 3),
+    "r4_batchrl_num_params": (C.c_int, [C.c_int] * 3),
+    "r4_batchrl_target_size": (C.c_int, [C.c_int] * 3),
+    "r4_batchrl_scratch_size": (C.c_int64, [C.c_int] * 4),
+    "r4_batchrl_transitions": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "r4_batchrl_grad": (C.c_int, [C.c_int] * 3 + [C.c_void_p, C.c_void_p, C.POINTER(BatchRLData), C.POINTER(BatchRLHyper),
+                                                  C.c_void_p, C.c_int] + [C.c_void_p] * 4),
+    "r4_batchrl_apply": (C.c_int, [C.c_int] * 3 + [C.c_void_p] * 5 + [C.c_int, C.c_float, C.c_float, C.c_int, C.c_void_p]),
+    "r4_batchrl_epoch": (C.c_int, [C.c_int] * 3 + [C.c_void_p] * 4 + [C.POINTER(BatchRLData), C.POINTER(BatchRLHyper),
+                                                                   C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_float,
+                                                                   C.c_float, C.c_int] + [C.c_void_p] * 3),
+    "r4_batchrl_launch_count": (C.c_int64, []),
+    "r4_batchrl_act": (C.c_int, [C.c_int] * 3 + [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(BatchRLData), C.c_int,
+                                                  C.c_float] + [C.c_void_p] * 4),
     "r4_adam_step": (C.c_int,[C.c_void_p] * 4 + [C.c_int, C.c_int] + [C.c_float] * 6 + [C.c_void_p, C.c_void_p]),
     "r4_dien_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
 }

@@ -1,0 +1,468 @@
+"""Batch (offline) RL on the logged dataset: the ``train`` and ``eval`` stages of ``script/batchrl_train.py:109-128`` for
+the three discrete algorithms of ``script/batchrl_trainer.py:get_model`` -- BC, BCQ and CQL -- over the dataset
+``rl4rs_b200.dataset`` writes (Slate and SeqSlate).
+
+The names are the reference's, so the script changes only its imports:
+  get_model(config, algo)       -> a model with d3rlpy's AlgoBase surface the scripts call: fit, save_model, load_model,
+                                   predict, predict_value
+  build_with_dataset(model, ds) -> builds the networks for the dataset's observation width and fits CQL's reward scaler
+  policy_model(model, config)   -> rl4rs/policy/policy_model.py: predict_with_mask, predict, action_probs, predict_q
+  evaluate(config, policy)      -> batchrl_trainer.py:395-426 on the GPU env; returns the average reward
+  load_dataset(path)            -> the writer's .npz (fit also takes the dict data_generate_* returns)
+
+On a CUDA device the dataset is uploaded once and stays there; an epoch is one device permutation and one library call
+(r4_batchrl_epoch: every minibatch's gradient and Adam step chained on the device, csrc/r4_batchrl.cuh), and acting is
+r4_batchrl_act.  On the CPU the torch twin (policy.BatchRLNet) runs the same algorithm.  The d3rlpy 0.91 semantics
+restated here are listed in INTEGRATION.md section 3 as not verified (d3rlpy is not in this
+project's environment).
+"""
+import ctypes as C
+import math
+
+import numpy as np
+import torch
+
+from .policy import BatchRLNet
+
+ALGOS = {"BC": 0, "BCQ": 1, "CQL": 2}
+NOT_BUILT = {
+    "dynamics": "the ProbabilisticEnsembleDynamics model",
+    "BCQ-conti": "continuous-action BCQ",
+    "CQL-conti": "continuous-action CQL",
+    "MOPO": "MOPO (needs the dynamics model)",
+    "COMBO": "COMBO (needs the dynamics model)",
+}
+# d3rlpy 0.91 defaults as batchrl_trainer.py:34-90 leaves or sets them (INTEGRATION.md section 3, not verified)
+DEFAULTS = {
+    "BC": {"batch_size": 256, "learning_rate": 1e-3, "eps": 1e-8, "beta": 0.0},
+    "BCQ": {"batch_size": 256, "learning_rate": 6.25e-5, "eps": 1e-8, "gamma": 0.99, "beta": 0.5,
+            "action_flexibility": 0.3, "target_update_interval": 8000},
+    "CQL": {"batch_size": 256, "learning_rate": 6.25e-5, "eps": 1e-8, "gamma": 1.0, "alpha": 1.0,
+            "target_update_interval": 8000, "reward_scaler": "standard"},
+}
+
+
+def _p(t):
+    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
+
+
+def get_model(config, algo, dynamics=None):
+    """batchrl_trainer.get_model: 'BC', 'BCQ' or 'CQL' (alpha = config['CQL_alpha']).  The other names of the reference raise
+    NotImplementedError; any other name fails its assert."""
+    if algo in NOT_BUILT:
+        raise NotImplementedError("%s: %s is not built in this project" % (algo, NOT_BUILT[algo]))
+    assert algo in ("BC", "BCQ", "CQL", "MOPO", "COMBO")
+    cls = {"BC": DiscreteBC, "BCQ": DiscreteBCQ, "CQL": DiscreteCQL}[algo]
+    extra = {"alpha": float(config["CQL_alpha"])} if algo == "CQL" and "CQL_alpha" in config else {}
+    return cls(config, **extra)
+
+
+def build_with_dataset(model, dataset):
+    """batchrl_trainer.build_with_dataset: the networks for the dataset's observation width, then the reward scaler."""
+    model.build_with_dataset(dataset)
+    return model
+
+
+def load_dataset(path):
+    """The .npz rl4rs_b200.dataset writes -> a dict of its arrays."""
+    with np.load(path) as z:
+        return {k: z[k] for k in z.files}
+
+
+def d3rlpy_eval(*args, **kwargs):
+    raise NotImplementedError("d3rlpy_eval: the soft_opc / discrete_action_match scorers are not built in this project")
+
+
+def ope_eval(*args, **kwargs):
+    raise NotImplementedError("ope: the off-policy evaluation stage is not built in this project")
+
+
+def _masks(config, A):
+    """(location_mask [4, A], special_items) from the config (batchrl_train.py:32-40 puts them there), else from the
+    catalog the env is built from, else from config['iteminfo_file'] (SlateState.get_mask_from_file)."""
+    from .env.slate import SlateState
+    if config.get("location_mask") is not None and config.get("special_items") is not None:
+        return np.asarray(config["location_mask"]), [int(i) for i in config["special_items"]]
+    if config.get("catalog") is not None:
+        return SlateState._location_mask(A), [int(i) for i in config["catalog"].special_items]
+    return SlateState.get_mask_from_file(config["iteminfo_file"], A)
+
+
+def transitions_host(terminals):
+    """The transition list of d3rlpy's episodes (split at the terminals): every entry i with terminals[i] == 0 before the last
+    terminal entry.  The same rule as r4_batchrl_transitions, for the CPU path and the tests."""
+    t = torch.as_tensor(np.asarray(terminals)).reshape(-1) != 0
+    idx = torch.nonzero(t).reshape(-1)
+    if idx.numel() == 0:
+        return torch.zeros(0, dtype=torch.int64)
+    last = int(idx[-1])
+    return torch.nonzero(~t[:last]).reshape(-1).to(torch.int64)
+
+
+class DeviceDataset(object):
+    """The dataset where the learner runs: obs f32 [N, K], action i32 [N], reward f32 [N], terminal u8 [N] and the
+    transition entries i64 [T].  On CUDA it is uploaded once; a dataset that does not fit raises MemoryError."""
+
+    def __init__(self, dataset, device):
+        obs = np.asarray(dataset["observations"], dtype=np.float32)
+        N = obs.shape[0]
+        act = np.asarray(dataset["actions"]).reshape(N)
+        if np.any(act != np.round(act)) or act.min(initial=0) < 0:
+            raise ValueError("batch RL here is discrete: the dataset's actions must be item ids")
+        self.device, self.N, self.K = torch.device(device), N, obs.shape[1]
+        need = N * (self.K * 4 + 4 + 4 + 1 + 8)
+        if self.device.type == "cuda":
+            free = torch.cuda.mem_get_info(self.device)[0]
+            if need > free:
+                raise MemoryError("the dataset needs %d bytes on %s, %d are free" % (need, self.device, free))
+        try:
+            self.obs = torch.from_numpy(obs).to(self.device)
+            self.action = torch.from_numpy(act.astype(np.int32)).to(self.device)
+            self.reward = torch.from_numpy(np.asarray(dataset["rewards"], dtype=np.float32).reshape(N)).to(self.device)
+            self.terminal = torch.from_numpy((np.asarray(dataset["terminals"]).reshape(N) != 0).astype(np.uint8)).to(self.device)
+            if self.device.type == "cuda":
+                from . import _capi
+                lib = _capi.load_library()
+                index = torch.empty(N, dtype=torch.int64, device=self.device)
+                count = torch.zeros(1, dtype=torch.int64, device=self.device)
+                rc = lib.r4_batchrl_transitions(_p(self.terminal), N, _p(index), _p(count),
+                                                C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+                if rc != 0:
+                    raise _capi.R4Error("r4_batchrl_transitions failed (%d): %s" % (rc, (lib.r4_last_error(None) or b"?").decode()))
+                self.transitions = index[:int(count)]
+            else:
+                self.transitions = transitions_host(self.terminal)
+        except torch.OutOfMemoryError as exc:
+            raise MemoryError("the dataset needs %d bytes on %s: %s" % (need, self.device, exc)) from exc
+        self.n = int(self.transitions.numel())
+
+    def batch(self, pos):
+        """(obs, action, reward, next_obs, terminal) of the transitions at positions pos of the transition list."""
+        e = self.transitions[pos]
+        return self.obs[e], self.action[e], self.reward[e + 1], self.obs[e + 1], self.terminal[e + 1]
+
+
+class BatchRLModel(object):
+    """d3rlpy AlgoBase's surface the scripts use, over policy.BatchRLNet (CPU) or the r4_batchrl_* kernels (CUDA)."""
+
+    algo = None
+
+    def __init__(self, config, device=None, seed=0, use_kernels=None, **overrides):
+        self.config = dict(config)
+        self.hp = dict(DEFAULTS[self.algo], **overrides)
+        self.batch_size = int(self.hp["batch_size"])
+        if device is None:
+            device = "cuda" if torch.cuda.is_available() and config.get("gpu", True) else "cpu"
+        self.device = torch.device(device)
+        self.use_kernels = (self.device.type == "cuda") if use_kernels is None else bool(use_kernels)
+        self.A = int(config.get("action_size", 284))
+        if int(config.get("page_items", 9)) != 9:
+            raise ValueError("the custom encoder reads 9 prev actions (page_items = 9)")
+        self.location_mask, self.special_items = _masks(config, self.A)
+        self.seed = seed
+        self.net = None
+        self.reward_mean, self.reward_std = 0.0, 1.0
+        self.reward_scaler = None
+        self._data, self._data_src = None, None
+        self.step = 0
+
+    # ---- building ------------------------------------------------------------------------------------
+    def create_impl(self, obs_dim):
+        self.net = BatchRLNet(self.algo, obs_dim, self.location_mask, self.special_items, self.A, self.device, self.seed)
+        z = lambda: torch.zeros(self.net.n_params, dtype=torch.float32, device=self.device)
+        self.m, self.v = z(), z()
+        self.step = 0
+        self._gen = torch.Generator(device=self.device).manual_seed(self.seed)
+        if self.use_kernels:
+            from . import _capi
+            self.capi, self.lib = _capi, _capi.load_library()
+            k = ALGOS[self.algo]
+            assert self.lib.r4_batchrl_num_params(k, obs_dim, self.A) == self.net.n_params
+            assert self.lib.r4_batchrl_target_size(k, obs_dim, self.A) == self.net.n_target
+            self.grad = z()
+            self.stats = torch.zeros(3, dtype=torch.float32, device=self.device)
+            n = self.lib.r4_batchrl_scratch_size(k, obs_dim, self.A, self.batch_size)
+            if n < 0:
+                raise ValueError("obs_dim %d / action_size %d is outside the kernels' range" % (obs_dim, self.A))
+            self.scratch = torch.zeros(n, dtype=torch.float32, device=self.device)
+            self._tables = BatchRLDataPtrs(self.net)
+
+    def build_with_dataset(self, dataset):
+        obs = dataset["observations"]
+        if self.net is None or self.net.K != obs.shape[1]:
+            self.create_impl(obs.shape[1])
+        if self.hp.get("reward_scaler") == "standard":
+            self.fit_reward_scaler(dataset)
+
+    def fit_reward_scaler(self, dataset):
+        """d3rlpy StandardRewardScaler.fit: mean and (population) std of the transitions' rewards, rewards[i] over the
+        transition entries i."""
+        idx = transitions_host(dataset["terminals"]).numpy()
+        r = np.asarray(dataset["rewards"], dtype=np.float64).reshape(-1)[idx]
+        self.reward_mean, self.reward_std = float(r.mean()), float(r.std())
+        self.reward_scaler = "standard"
+
+    def _hyper(self):
+        hp = self.hp
+        return {"gamma": float(hp.get("gamma", 0.0)), "beta": float(hp.get("beta", 0.0)), "alpha": float(hp.get("alpha", 0.0)),
+                "log_flex": float(np.float32(math.log(hp.get("action_flexibility", 0.3)))),
+                "reward_mean": self.reward_mean if self.reward_scaler else 0.0,
+                "reward_den": (self.reward_std + 1e-3) if self.reward_scaler else 1.0}
+
+    # ---- training ------------------------------------------------------------------------------------
+    def _device_data(self, dataset):
+        if self._data_src is not dataset:
+            self._data = None                       # release the previous upload first
+            self._data = DeviceDataset(dataset, self.device)
+            self._data_src = dataset
+        return self._data
+
+    def fit(self, dataset, n_epochs=1, eval_episodes=None, show_progress=False, **kwargs):
+        """d3rlpy fit with its RoundIterator: per epoch one permutation of the transitions (drawn on the device) and
+        floor(n / batch_size) minibatches in order.  eval_episodes is accepted and not scored (no scorers are passed).
+        CQL's reward scaler is fitted here only when it has not been fitted yet (on the first dataset, or by
+        build_with_dataset): a later fit on another dataset keeps those statistics; build_with_dataset refits them.
+        Returns [(epoch, {'loss', 'td' or 'nll', 'q' or 'penalty'})]."""
+        if self.net is None or self.net.K != dataset["observations"].shape[1]:
+            self.build_with_dataset(dataset)
+        elif self.hp.get("reward_scaler") == "standard" and self.reward_scaler is None:
+            self.fit_reward_scaler(dataset)
+        data = self._device_data(dataset)
+        mb = self.batch_size
+        if data.n < mb:
+            raise ValueError("the dataset has %d transitions, fewer than one minibatch of %d" % (data.n, mb))
+        out = []
+        for epoch in range(1, int(n_epochs) + 1):
+            perm = torch.randperm(data.n, generator=self._gen, device=self.device)
+            st = self._epoch_kernels(data, perm) if self.use_kernels else self._epoch_twin(data, perm)
+            names = ("loss", "nll", "penalty") if self.algo == "BC" else ("loss", "td", "q")
+            out.append((epoch, dict(zip(names, st))))
+            if show_progress:
+                print("epoch %d %s" % (epoch, out[-1][1]))
+        return out
+
+    def _epoch_twin(self, data, perm):
+        hp, mb = self._hyper(), self.batch_size
+        acc = torch.zeros(3, dtype=torch.float64)
+        steps = data.n // mb
+        for k in range(steps):
+            self.train_step_twin(data.batch(perm[k * mb:(k + 1) * mb]), hp)
+            acc += self._last_stats.double().cpu()
+        return [float(v) for v in acc / max(steps, 1)]
+
+    def train_step_twin(self, batch, hp=None):
+        """One SGD step of the twin: autograd gradient, the kernels' Adam, the hard target copy when due."""
+        hp = hp or self._hyper()
+        net = self.net
+        if net.flat.grad is not None:
+            net.flat.grad.zero_()
+        loss, st = net.loss(*batch, hp)
+        loss.backward()
+        self.step += 1
+        with torch.no_grad():
+            adam_(net.flat.data, net.flat.grad, self.m, self.v, self.step, self.hp["learning_rate"], self.hp["eps"])
+            if self._copy_due(self.step):
+                net.target.copy_(net.flat.detach()[:net.n_target])
+        self._last_stats = st
+        return st
+
+    def _copy_due(self, step):
+        ti = int(self.hp.get("target_update_interval", 0))
+        return self.net.n_target > 0 and ti > 0 and (step - 1) % ti == 0
+
+    def _epoch_kernels(self, data, perm):
+        mb = self.batch_size
+        steps = data.n // mb
+        stats = torch.zeros(steps * 3, dtype=torch.float32, device=self.device)
+        rc = self.lib.r4_batchrl_epoch(ALGOS[self.algo], self.net.K, self.A, _p(self.net.flat), _p(self.net.target),
+                                       _p(self.m), _p(self.v), C.byref(self._tables.data(data)), C.byref(self._hyper_c()),
+                                       _p(perm), perm.numel(), mb, self.step, self.hp["learning_rate"], self.hp["eps"],
+                                       int(self.hp.get("target_update_interval", 0)), _p(self.scratch), _p(stats),
+                                       self._stream())
+        if rc < 0:
+            self._check(rc, "r4_batchrl_epoch")
+        self.step += rc
+        return [float(v) for v in stats.view(steps, 3).double().mean(0)]
+
+    def _hyper_c(self):
+        h = self._hyper()
+        return self.capi.BatchRLHyper(h["gamma"], h["beta"], h["alpha"], h["log_flex"], h["reward_mean"], h["reward_den"])
+
+    def _stream(self):
+        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def _check(self, rc, what):
+        if rc != 0:
+            raise self.capi.R4Error("%s failed (%d): %s" % (what, rc, (self.lib.r4_last_error(None) or b"?").decode()))
+
+    def grad_kernels(self, data, pos):
+        """r4_batchrl_grad over the transitions at positions pos (i64, device) -> self.grad, self.stats."""
+        rc = self.lib.r4_batchrl_grad(ALGOS[self.algo], self.net.K, self.A, _p(self.net.flat), _p(self.net.target),
+                                      C.byref(self._tables.data(data)), C.byref(self._hyper_c()), _p(pos), pos.numel(),
+                                      _p(self.scratch), _p(self.grad), _p(self.stats), self._stream())
+        self._check(rc, "r4_batchrl_grad")
+
+    # ---- acting --------------------------------------------------------------------------------------
+    def act(self, obs, mode=0, want_probs=False, want_values=False):
+        """The act rule on observations (numpy or torch, f32 or f64 [n, K]) -> (action i32 [n], probs or None, values or
+        None) as device tensors.  mode 0: predict_with_mask's rule; mode 1: d3rlpy's predict."""
+        x = torch.as_tensor(obs, device=self.device)
+        if x.dtype not in (torch.float32, torch.float64):
+            x = x.to(torch.float32)
+        x = x.reshape(-1, self.net.K).contiguous()
+        log_flex = self._hyper()["log_flex"]
+        if not self.use_kernels:
+            a, probs, raw = self.net.act(x, mode, log_flex)
+            return a, probs if want_probs else None, raw if want_values else None
+        n = x.shape[0]
+        a = torch.empty(n, dtype=torch.int32, device=self.device)
+        probs = torch.empty(n, self.A, dtype=torch.float32, device=self.device) if want_probs else None
+        vals = torch.empty(n, self.A, dtype=torch.float32, device=self.device) if want_values else None
+        rc = self.lib.r4_batchrl_act(ALGOS[self.algo], self.net.K, self.A, _p(self.net.flat), _p(x),
+                                     int(x.dtype == torch.float64), n, C.byref(self._tables.tables()), mode, log_flex,
+                                     _p(a), _p(probs), _p(vals), self._stream())
+        self._check(rc, "r4_batchrl_act")
+        return a, probs, vals
+
+    def predict(self, x):
+        """d3rlpy predict: the greedy action of the algorithm (no location mask) -> int array [n]."""
+        return self.act(x, 1)[0].long().cpu().numpy()
+
+    def predict_value(self, x, action):
+        """d3rlpy predict_value: Q(s, a) in the scaled reward units (BC: its logit of a)."""
+        vals = self.act(x, 1, want_values=True)[2]
+        a = torch.as_tensor(np.asarray(action), device=self.device).long().reshape(-1)
+        return vals[torch.arange(vals.shape[0], device=self.device), a].cpu().numpy()
+
+    # ---- checkpoints ---------------------------------------------------------------------------------
+    def save_model(self, fname):
+        """torch.save of the flat parameters, the target, the Adam moments, the step counter and the reward scaler."""
+        torch.save({"algo": self.algo, "obs_dim": self.net.K, "action_size": self.A, "params": self.net.flat.detach().cpu(),
+                    "target": self.net.target.cpu(), "m": self.m.cpu(), "v": self.v.cpu(), "step": self.step,
+                    "reward_scaler": self.reward_scaler, "reward_mean": self.reward_mean, "reward_std": self.reward_std},
+                   fname)
+
+    def load_model(self, fname):
+        ck = torch.load(fname, map_location="cpu")
+        if ck["algo"] != self.algo or ck["action_size"] != self.A:
+            raise ValueError("%s holds a %s model for %d actions" % (fname, ck["algo"], ck["action_size"]))
+        if self.net is None or self.net.K != ck["obs_dim"]:
+            self.create_impl(ck["obs_dim"])
+        with torch.no_grad():
+            self.net.flat.copy_(ck["params"].to(self.device))
+            self.net.target.copy_(ck["target"].to(self.device))
+            self.m.copy_(ck["m"].to(self.device))
+            self.v.copy_(ck["v"].to(self.device))
+        self.step = int(ck["step"])
+        self.reward_scaler, self.reward_mean, self.reward_std = ck["reward_scaler"], ck["reward_mean"], ck["reward_std"]
+
+
+class DiscreteBC(BatchRLModel):
+    algo = "BC"
+
+
+class DiscreteBCQ(BatchRLModel):
+    algo = "BCQ"
+
+
+class DiscreteCQL(BatchRLModel):
+    algo = "CQL"
+
+
+class BatchRLDataPtrs(object):
+    """The r4_batchrl_data structure: the device dataset's planes and the net's masking tables."""
+
+    def __init__(self, net):
+        self.net = net
+
+    def tables(self):
+        from ._capi import BatchRLData
+        d = BatchRLData()
+        d.location_mask, d.special = self.net.location_mask.data_ptr(), self.net.special.data_ptr()
+        return d
+
+    def data(self, ds):
+        d = self.tables()
+        d.obs, d.action, d.reward = ds.obs.data_ptr(), ds.action.data_ptr(), ds.reward.data_ptr()
+        d.terminal, d.transitions = ds.terminal.data_ptr(), ds.transitions.data_ptr()
+        return d
+
+
+@torch.no_grad()
+def adam_(p, g, m, v, step, lr, eps, b1=0.9, b2=0.999):
+    """torch.optim.Adam's update in the operation order of csrc/r4_ppo.cuh adam_update."""
+    m.mul_(b1).add_((1 - b1) * g)
+    v.mul_(b2).add_((1 - b2) * g * g)
+    bc1, bc2 = 1 - b1 ** step, 1 - b2 ** step
+    p.sub_((lr / bc1) * (m / (v.sqrt() / math.sqrt(bc2) + eps)))
+
+
+class policy_model(object):
+    """rl4rs/policy/policy_model.py over a batch-RL model."""
+
+    def __init__(self, model, config={}):
+        self.policy = model
+        self.config = config
+        self.page_items = int(config.get("page_items", 9))
+        self.mask_size = self.page_items + 1
+        self.location_mask = config.get("location_mask", None)
+        self.special_items = config.get("special_items", None)
+
+    def predict_with_mask(self, obs):
+        """policy_model.py:17-36: action_probs, -2^15 where the location layer, the prev actions or the special-item rule
+        exclude an item, the first argmax.  A device tensor in gives a device tensor out, else a numpy array."""
+        if self.config.get("support_conti_env", False):
+            return self.predict(obs)
+        a = self.policy.act(obs, 0)[0]
+        return a if hasattr(obs, "is_cuda") else a.long().cpu().numpy()
+
+    def predict(self, obs):
+        return self.policy.predict(obs)
+
+    def predict_q(self, obs, action):
+        q = self.policy.predict_value(obs, action)
+        if self.policy.reward_scaler is not None:
+            return q * (self.policy.reward_std + 1e-3) + self.policy.reward_mean
+        return q
+
+    def action_probs(self, obs):
+        """BC: the imitator's log-probs; BCQ / CQL: softmax(Q)."""
+        return self.policy.act(obs, 0, want_probs=True)[1].cpu().numpy()
+
+
+def make_eval_env(config, batch_size=2048):
+    """The eval env of batchrl_trainer.evaluate: is_eval, the given batch, the d3rl mask and the 'torch' output format."""
+    from . import gymshim as gym
+    from .env.seqslate import SeqSlateRecEnv, SeqSlateState
+    from .env.slate import SlateRecEnv, SlateState
+    cfg = dict(config, is_eval=True, batch_size=batch_size, support_d3rl_mask=True, support_rllib_mask=False,
+               output_format="torch")
+    cfg.setdefault("cache_size", batch_size)
+    name = cfg.get("env", "SlateRecEnv-v0")
+    assert name in ("SlateRecEnv-v0", "SeqSlateRecEnv-v0")
+    if name == "SeqSlateRecEnv-v0":
+        return gym.make(name, recsim=SeqSlateRecEnv(cfg, state_cls=SeqSlateState))
+    return gym.make(name, recsim=SlateRecEnv(cfg, state_cls=SlateState))
+
+
+def evaluate(config, policy, batch_size=2048, episodes=4, env=None):
+    """batchrl_trainer.evaluate (:395-426): `episodes` episodes of max_steps steps at `batch_size` with
+    predict_with_mask; prints the reference's lines and returns the average episode reward."""
+    env = env if env is not None else make_eval_env(config, batch_size)
+    T = config["max_steps"]
+    total, rmax, rmin, B = 0.0, -math.inf, math.inf, batch_size
+    for i in range(episodes):
+        obs = env.reset()
+        print("test batch at ", i)
+        ep = None
+        for _ in range(T):
+            action = policy.predict_with_mask(obs)
+            obs, reward, done, info = env.step(action)
+            r = torch.as_tensor(reward).to(torch.float64)
+            ep = r if ep is None else ep + r
+        total, B = total + float(ep.sum()), ep.numel()
+        rmax, rmin = max(rmax, float(ep.max())), min(rmin, float(ep.min()))
+    print("reward max min", rmax, rmin)
+    avg = total / B / episodes
+    print("avg reward", avg)
+    return avg

@@ -11,6 +11,7 @@
 #include "r4_gauss.cuh"
 #include "r4_ddpg.cuh"
 #include "r4_rainbow.cuh"
+#include "r4_batchrl.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -1664,6 +1665,160 @@ int r4_rainbow_train_step(r4_comm* comm, float* params, float* target, float* m,
   rc = r4_rainbow_apply(params, target, g, m, v, num_actions, num_atoms, step, lr, adam_eps, grad_clip, copy_target, stream);
   if (rc || !r_prio) return rc;
   return r4_replay_update_priorities(r_prio, max_prio, P.idx, P.td, n, alpha, prio_eps, stream);
+}
+
+// ---- batch RL: discrete BC / BCQ / CQL (r4_batchrl.cuh) -----------------------------------------------------------
+// kernels launched by the r4_batchrl_* entry points in this process (r4_batchrl_launch_count)
+static int64_t g_bq_launches = 0;
+
+int64_t r4_batchrl_launch_count(void) { return g_bq_launches; }
+
+int r4_batchrl_num_params(int algo, int obs_dim, int action_size) {
+  return r4bq::dims_ok(algo, obs_dim, action_size) ? r4bq::make_layout(algo, obs_dim, action_size).n : -1;
+}
+
+int r4_batchrl_target_size(int algo, int obs_dim, int action_size) {
+  return r4bq::dims_ok(algo, obs_dim, action_size) ? r4bq::make_layout(algo, obs_dim, action_size).ntgt : -1;
+}
+
+int64_t r4_batchrl_scratch_size(int algo, int obs_dim, int action_size, int n) {
+  if (!r4bq::dims_ok(algo, obs_dim, action_size) || n < 1) return -1;
+  return (int64_t)r4bq::scratch_floats(r4bq::make_layout(algo, obs_dim, action_size), n);
+}
+
+int r4_batchrl_transitions(const uint8_t* terminal, int64_t N, int64_t* index, int64_t* count, void* stream) {
+  if (!terminal || N < 1 || !index || !count) return fail(nullptr, R4_ERR_ARG, "r4_batchrl_transitions: bad argument");
+  r4bq::k_bq_transitions<<<1, r4bq::TRT, 0, S(stream)>>>(terminal, N, index, count);
+  ++g_bq_launches;
+  R4_PCHECK("k_bq_transitions");
+  return R4_OK;
+}
+
+// raise a kernel's dynamic shared-memory limit to bytes when the last setting was lower
+static int bq_smem(const void* fn, size_t bytes, const char* name, size_t& cur) {
+  if (bytes <= cur) return R4_OK;
+  cudaError_t st = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  if (st != cudaSuccess) return fail(nullptr, R4_ERR_CUDA, std::string("cudaFuncSetAttribute(") + name + "): " + cudaGetErrorString(st));
+  cur = bytes;
+  return R4_OK;
+}
+
+static r4bq::Data bq_data(const r4_batchrl_data* d) {
+  return r4bq::Data{d->obs, d->action, d->reward, d->terminal, d->transitions, d->location_mask, d->special};
+}
+
+// the kernels of one SGD step; pdl: launch the chain with programmatic dependent launch (r4_batchrl_epoch)
+static int bq_launch(const void* fn, dim3 grid, int threads, size_t smem, cudaStream_t st, bool pdl, void** args) {
+  cudaLaunchConfig_t lc = {};
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
+  lc.gridDim = grid; lc.blockDim = dim3(threads); lc.dynamicSmemBytes = smem; lc.stream = st; lc.attrs = at; lc.numAttrs = pdl ? 1 : 0;
+  ++g_bq_launches;
+  return cudaLaunchKernelExC(&lc, fn, args) == cudaSuccess ? R4_OK : R4_ERR_CUDA;
+}
+
+static int bq_grad(int algo, int K, int A, const float* params, const float* target, const r4_batchrl_data* data,
+                   const r4_batchrl_hyper* h, const int64_t* idx, int n, float* scratch, float* grad, float* stats,
+                   cudaStream_t st, bool pdl) {
+  const void* rows[3] = {(const void*)r4bq::k_bq_rows<r4bq::BC>, (const void*)r4bq::k_bq_rows<r4bq::BCQ>,
+                         (const void*)r4bq::k_bq_rows<r4bq::CQL>};
+  static size_t attr[3] = {0, 0, 0};
+  const size_t smem = r4bq::rows_smem(K, A);
+  if (int rc = bq_smem(rows[algo], smem, "k_bq_rows", attr[algo])) return rc;
+  r4bq::Layout L = r4bq::make_layout(algo, K, A);
+  r4bq::Planes P = r4bq::make_planes(scratch, L, n);
+  P.grad = grad;
+  r4bq::Hyper hp{h->gamma, 1.0f / (float)n, h->beta, h->alpha, h->log_flex, h->reward_mean, h->reward_den};
+  r4bq::Data D = bq_data(data);
+  void* a1[] = {&L, &hp, (void*)&params, (void*)&target, &D, (void*)&idx, &n, &P};
+  if (bq_launch(rows[algo], dim3((n + r4bq::TS - 1) / r4bq::TS), r4bq::NT, smem, st, pdl, a1))
+    return fail(nullptr, R4_ERR_CUDA, std::string("k_bq_rows: ") + cudaGetErrorString(cudaGetLastError()));
+  R4_PCHECK("k_bq_rows");
+  const r4ddpg::Jobs J = r4bq::make_jobs(L, P);
+  r4ddpg::k_ddpg_wgrad<<<J.ntiles + 1, r4ddpg::NT, 0, st>>>(J, n, grad, P.stats, stats, 1.0f / (float)n);
+  ++g_bq_launches;
+  R4_PCHECK("k_ddpg_wgrad");
+  const int nets = r4bq::n_mnets(algo);
+  if (nets) {
+    int per = (A * r4bq::E + r4bq::EGT - 1) / r4bq::EGT;
+    void* a3[] = {&L, &P, &n, &per};
+    if (bq_launch((const void*)r4bq::k_bq_embgrad, dim3(nets * per), r4bq::EGT, 0, st, pdl, a3))
+      return fail(nullptr, R4_ERR_CUDA, std::string("k_bq_embgrad: ") + cudaGetErrorString(cudaGetLastError()));
+    R4_PCHECK("k_bq_embgrad");
+  }
+  return R4_OK;
+}
+
+static int bq_apply(int algo, int K, int A, float* params, float* target, const float* grad, float* m, float* v, int step,
+                    float lr, float eps, int copy, cudaStream_t st, bool pdl) {
+  const r4bq::Layout L = r4bq::make_layout(algo, K, A);
+  int np = L.n, nt = L.ntgt;
+  void* a[] = {&np, &nt, &params, &target, (void*)&grad, &m, &v, &step, &lr, &eps, &copy};
+  if (bq_launch((const void*)r4bq::k_bq_apply, dim3((np + 255) / 256), 256, 0, st, pdl, a))
+    return fail(nullptr, R4_ERR_CUDA, std::string("k_bq_apply: ") + cudaGetErrorString(cudaGetLastError()));
+  R4_PCHECK("k_bq_apply");
+  return R4_OK;
+}
+
+static bool bq_data_ok(const r4_batchrl_data* d) {
+  return d && d->obs && d->action && d->reward && d->terminal && d->transitions && d->location_mask && d->special;
+}
+
+int r4_batchrl_grad(int algo, int obs_dim, int action_size, const float* params, const float* target,
+                    const r4_batchrl_data* data, const r4_batchrl_hyper* hp, const int64_t* idx, int n, float* scratch,
+                    float* grad, float* stats, void* stream) {
+  if (!r4bq::dims_ok(algo, obs_dim, action_size) || !params || (algo != r4bq::BC && !target) || !bq_data_ok(data) || !hp ||
+      !idx || n < 1 || !scratch || !grad)
+    return fail(nullptr, R4_ERR_ARG, "r4_batchrl_grad: bad argument (algo 0..2, obs_dim 11..4096, action_size 2..512, shared planes <= 226 KB)");
+  return bq_grad(algo, obs_dim, action_size, params, target, data, hp, idx, n, scratch, grad, stats, S(stream), false);
+}
+
+int r4_batchrl_apply(int algo, int obs_dim, int action_size, float* params, float* target, const float* grad, float* m,
+                     float* v, int step, float lr, float adam_eps, int copy_target, void* stream) {
+  if (!r4bq::dims_ok(algo, obs_dim, action_size) || !params || !grad || !m || !v || step < 1 || (copy_target && algo != r4bq::BC && !target))
+    return fail(nullptr, R4_ERR_ARG, "r4_batchrl_apply: bad argument");
+  return bq_apply(algo, obs_dim, action_size, params, target, grad, m, v, step, lr, adam_eps, copy_target, S(stream), false);
+}
+
+int r4_batchrl_epoch(int algo, int obs_dim, int action_size, float* params, float* target, float* m, float* v,
+                     const r4_batchrl_data* data, const r4_batchrl_hyper* hp, const int64_t* perm, int64_t n_perm, int mb,
+                     int step0, float lr, float adam_eps, int target_interval, float* scratch, float* stats, void* stream) {
+  if (!r4bq::dims_ok(algo, obs_dim, action_size) || !params || (algo != r4bq::BC && !target) || !m || !v || !bq_data_ok(data) ||
+      !hp || !perm || n_perm < 1 || mb < 1 || step0 < 0 || !scratch)
+    return fail(nullptr, R4_ERR_ARG, "r4_batchrl_epoch: bad argument");
+  const int64_t steps = n_perm / mb;
+  if (steps > (int64_t)0x7fffffff - step0) return fail(nullptr, R4_ERR_ARG, "r4_batchrl_epoch: too many steps");
+  const r4bq::Layout L = r4bq::make_layout(algo, obs_dim, action_size);
+  float* grad = r4bq::make_planes(scratch, L, mb).grad;
+  cudaStream_t st = S(stream);
+  for (int64_t k = 0; k < steps; ++k) {
+    const int step = step0 + (int)k + 1;
+    const int copy = L.ntgt > 0 && target_interval > 0 && (step - 1) % target_interval == 0;
+    int rc = bq_grad(algo, obs_dim, action_size, params, target, data, hp, perm + k * mb, mb, scratch, grad,
+                     stats ? stats + 3 * k : nullptr, st, true);
+    if (rc) return rc;
+    if ((rc = bq_apply(algo, obs_dim, action_size, params, target, grad, m, v, step, lr, adam_eps, copy, st, true))) return rc;
+  }
+  return (int)steps;
+}
+
+int r4_batchrl_act(int algo, int obs_dim, int action_size, const float* params, const void* obs, int obs_f64, int n,
+                   const r4_batchrl_data* data, int mode, float log_flex, int32_t* action, float* probs, float* values,
+                   void* stream) {
+  if (!r4bq::dims_ok(algo, obs_dim, action_size) || !params || !obs || n < 1 || !data || !data->location_mask ||
+      !data->special || mode < 0 || mode > 1 || !action)
+    return fail(nullptr, R4_ERR_ARG, "r4_batchrl_act: bad argument");
+  static size_t attr = 0;
+  if (int rc = bq_smem((const void*)r4bq::k_bq_act, r4bq::act_smem(obs_dim, action_size), "k_bq_act", attr)) return rc;
+  const r4bq::Layout L = r4bq::make_layout(algo, obs_dim, action_size);
+  r4bq::Data D{};
+  D.locm = data->location_mask; D.special = data->special;
+  r4bq::k_bq_act<<<(n + r4bq::TS - 1) / r4bq::TS, r4bq::NT, r4bq::act_smem(obs_dim, action_size), S(stream)>>>(
+      L, params, obs_f64 ? nullptr : (const float*)obs, obs_f64 ? (const double*)obs : nullptr, n, D, mode, log_flex, action,
+      probs, values);
+  ++g_bq_launches;
+  R4_PCHECK("k_bq_act");
+  return R4_OK;
 }
 
 int r4_dien_forward(r4_env* e, const int32_t* seq, const float* dense, const int32_t* cat, int n_rows,

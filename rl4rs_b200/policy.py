@@ -9,6 +9,7 @@ Parameters live in one flat f32 buffer so the data-parallel gradient all-reduce 
 """
 import math
 
+import numpy as np
 import torch
 
 OBS, HID = 256, 64
@@ -463,3 +464,159 @@ class RawStatePolicy(object):
         return logits + inf_mask, (ctx @ p["wv"] + p["bv"]).squeeze(-1)
 
     act, terms = MaskedPolicy.act, MaskedPolicy.terms
+
+
+class BatchRLNet(object):
+    """The networks of the discrete batch-RL learners (script/batchrl_trainer.py:34-90, d3rlpy 0.91 as the script configures
+    it), in csrc/r4_batchrl.cuh's flat layout.  The masked net M (BC's imitator; BCQ's Q function and, separately, its
+    imitator) is rl4rs/nets/cql/encoder.py CustomVectorEncoder with_q plus d3rlpy's Linear(A, A) head:
+        h = relu(x W1 + b1) [256] ; e = flatten(Emb[x[:, -10:]]) [10 x 32] (the 9 prev actions and cur_steps)
+        f = ([h | e] W2 + b2), set to 0 where keep is 0 ; z = f W3 + b3
+    keep: location_mask[cur_steps % 9 // 3], 0 for the 9 prev actions, and 0 for every special item of a row whose prev
+    actions hold one.  CQL's plain net is d3rlpy's default encoder (256 relu, 256 relu) and Linear(256, A).  Init is torch's
+    default (Linear: U(+-1/sqrt(fan_in)) for weight and bias; Embedding: N(0, 1)).  The target is a copy of the Q part
+    (BCQ: its Q net; CQL: the whole net; BC has none).  This twin is the CPU path of rl4rs_b200.batchrl and the autograd
+    cross-check of the kernels (tests/test_gpu_batchrl.py)."""
+
+    H, E, W, PW = 256, 32, 10, 9
+    ALGOS = ("BC", "BCQ", "CQL")
+
+    def __init__(self, algo, obs_dim, location_mask, special_items, action_size=284, device="cuda", seed=0):
+        assert algo in self.ALGOS
+        self.algo, self.K, self.A = algo, int(obs_dim), int(action_size)
+        self.device = torch.device(device)
+        K, A, H, E, W = self.K, self.A, self.H, self.E, self.W
+
+        def mnet(p):
+            return [(p + "w1", (K, H)), (p + "b1", (H,)), (p + "emb", (A, E)), (p + "w2", (H + W * E, A)), (p + "b2", (A,)),
+                    (p + "w3", (A, A)), (p + "b3", (A,))]
+        cnet = [("w1", (K, H)), ("b1", (H,)), ("w2", (H, H)), ("b2", (H,)), ("w3", (H, A)), ("b3", (A,))]
+        shapes = {"BC": mnet("i_"), "BCQ": mnet("q_") + mnet("i_"), "CQL": cnet}[algo]
+        n = sum(math.prod(s) for _, s in shapes)
+        self.n_target = {"BC": 0, "BCQ": n // 2, "CQL": n}[algo]
+        g = torch.Generator(device="cpu").manual_seed(seed)
+        self.flat = torch.zeros(n, dtype=torch.float32, device=self.device, requires_grad=True)
+        off, fan = 0, 1
+        with torch.no_grad():
+            for name, shape in shapes:
+                k = math.prod(shape)
+                v = self.flat[off:off + k].view(shape)
+                if name.endswith("emb"):
+                    v.copy_(torch.randn(shape, generator=g).to(self.device))
+                else:
+                    fan = shape[0] if len(shape) == 2 else fan          # a bias follows its weight
+                    bound = 1.0 / math.sqrt(fan)
+                    v.copy_(((torch.rand(shape, generator=g) * 2 - 1) * bound).to(self.device))
+                off += k
+        self._shapes, self.n_params = shapes, n
+        self.target = self.flat.detach()[:self.n_target].clone()
+        lm = torch.as_tensor(np.asarray(location_mask)[:3] >= 0.01, dtype=torch.uint8)
+        self.location_mask = lm.to(self.device)
+        sp = torch.zeros(A, dtype=torch.uint8)
+        sp[torch.as_tensor(np.asarray(list(special_items), dtype=np.int64))] = 1
+        self.special = sp.to(self.device)
+
+    def params(self, flat=None):
+        flat = self.flat if flat is None else flat
+        out, off = {}, 0
+        for name, shape in self._shapes:
+            k = math.prod(shape)
+            if off + k > flat.numel():
+                break
+            out[name] = flat[off:off + k].view(shape)
+            off += k
+        return out
+
+    def keep(self, x):
+        """bool [n, A]: the custom encoder's mask (encoder.py:43-65), the same as the eval rule's (policy_model.py:24-33)."""
+        prev = x[:, -self.W:-1].to(torch.long)
+        layer = x[:, -1].to(torch.long) % self.PW // 3
+        mask = self.location_mask[layer].clone()
+        mask.scatter_(1, prev, 0)
+        has = self.special[prev].bool().any(1)
+        mask[has.unsqueeze(1) & self.special.bool().unsqueeze(0)] = 0
+        return mask.bool()
+
+    def features(self, x, prefix, flat=None, keep=None):
+        """The custom encoder's output (encoder.py:42-67 with_q): the masked features f [n, A] of the masked net."""
+        p = self.params(flat)
+        keep = self.keep(x) if keep is None else keep
+        h = torch.relu(x @ p[prefix + "w1"] + p[prefix + "b1"])
+        e = torch.nn.functional.embedding(x[:, -self.W:].to(torch.long), p[prefix + "emb"]).flatten(1)
+        f = torch.cat([h, e], 1) @ p[prefix + "w2"] + p[prefix + "b2"]
+        return torch.where(keep, f, torch.zeros_like(f))
+
+    def mnet(self, x, prefix, flat=None, keep=None):
+        """The masked net on x [n, K] -> z [n, A] (d3rlpy's Linear head on the encoder's features)."""
+        p = self.params(flat)
+        return self.features(x, prefix, flat, keep) @ p[prefix + "w3"] + p[prefix + "b3"]
+
+    def cnet(self, x, flat=None):
+        p = self.params(flat)
+        h = torch.relu(torch.relu(x @ p["w1"] + p["b1"]) @ p["w2"] + p["b2"])
+        return h @ p["w3"] + p["b3"]
+
+    def q(self, x, flat=None):
+        """The Q function (BCQ, CQL) [n, A]."""
+        return self.cnet(x, flat) if self.algo == "CQL" else self.mnet(x, "q_", flat)
+
+    def imitator(self, x, flat=None):
+        """The imitator's logits (BC, BCQ) [n, A]."""
+        return self.mnet(x, "i_", flat)
+
+    def bcq_filtered(self, x, log_flex):
+        """d3rlpy DiscreteBCQ's action rule: (Q - min Q) * [log pi - max log pi > log_flex] (first argmax picks)."""
+        lp = torch.log_softmax(self.imitator(x), 1)
+        mask = ((lp - lp.max(1, keepdim=True).values) > log_flex).to(torch.float32)
+        q = self.q(x)
+        return (q - q.min(1, keepdim=True).values) * mask
+
+    def loss(self, obs, action, reward, next_obs, terminal, hp):
+        """The minibatch loss of the algorithm -> (loss, stats [3]) in r4_batchrl_grad's statistics order.  hp: gamma, beta,
+        alpha, log_flex, reward_mean, reward_den."""
+        n = obs.shape[0]
+        rows = torch.arange(n, device=obs.device)
+        a = action.long()
+
+        def huber(d):
+            return torch.where(d.abs() < 1.0, 0.5 * d * d, d.abs() - 0.5)
+
+        def bc_terms(z):
+            nll = -torch.log_softmax(z, 1)[rows, a]
+            pen = (z * z).mean(1)
+            return nll + hp["beta"] * pen, nll, pen
+        if self.algo == "BC":
+            tot, nll, pen = bc_terms(self.imitator(obs))
+            return tot.mean(), torch.stack([tot.mean(), nll.mean(), pen.mean()]).detach()
+        with torch.no_grad():
+            if self.algo == "BCQ":
+                a_star = self.bcq_filtered(next_obs, hp["log_flex"]).argmax(1)
+                r = reward
+            else:
+                a_star = self.q(next_obs).argmax(1)
+                r = (reward - hp["reward_mean"]) / hp["reward_den"]
+            qt = self.q(next_obs, self.target)[rows, a_star]
+            y = r + hp["gamma"] * (1.0 - terminal.to(torch.float32)) * qt
+        q = self.q(obs)
+        qa = q[rows, a]
+        td = huber(qa - y)
+        if self.algo == "BCQ":
+            tot = td + bc_terms(self.imitator(obs))[0]
+        else:
+            tot = td + hp["alpha"] * (torch.logsumexp(q, 1) - qa)
+        return tot.mean(), torch.stack([tot.mean(), td.mean(), qa.mean()]).detach()
+
+    @torch.no_grad()
+    def act(self, obs, mode=0, log_flex=math.log(0.3)):
+        """r4_batchrl_act's rule -> (action i32 [n], action_probs [n, A], raw output [n, A]).  mode 0: predict_with_mask
+        (policy_model.py:17-36); mode 1: d3rlpy's predict."""
+        x = obs.to(torch.float32)
+        raw = self.imitator(x) if self.algo == "BC" else self.q(x)
+        probs = torch.log_softmax(raw, 1) if self.algo == "BC" else torch.softmax(raw, 1)
+        if mode == 0:
+            pick = torch.where(self.keep(x), probs, torch.full_like(probs, -2.0 ** 15))
+        elif self.algo == "BCQ":
+            pick = self.bcq_filtered(x, log_flex)
+        else:
+            pick = probs
+        return pick.argmax(1).to(torch.int32), probs, raw
