@@ -190,6 +190,7 @@ int r4_set_option(const char* key, int value);
 /* ---- policy + learner (K12): MyMaskActionsModel (rllib_mask_model.py:41-62) and the RLlib PPO / A2C losses ----
  * Stateless: every pointer is caller-owned DEVICE memory.  Flat parameter layout:
  * w1[256,64] b1[64] w2[64,A] b2[A] wv[64] bv[1]  (r4_policy_num_params(A) floats). */
+/* -1 for an action_size outside 2..512 */
 int r4_policy_num_params(int action_size);
 /* forward + SoftQ(T=1) sampling (explore != 0) or argmax (modelfree_train.py:398-402,412-414); obs f32[n,256],
  * mask u8[n,A] -> action i32[n], logp f32[n], value f32[n], logits f32[n,A] (masked logits; may be NULL). */
@@ -266,6 +267,7 @@ int r4_grad_exchange_n(r4_comm* comm, const float* partial, int G, int n_params,
  * a DiagGaussian over action_dim = D (even, 2..64) dimensions.  Flat parameter layout (r4_gauss_num_params(D) floats):
  * fc_1 w[256,256] b[256] | fc_2 w[256,256] b[256] | fc_out w[256,2D] b[2D] (mean | log_std) |
  * fc_value_1 w[256,256] b[256] | fc_value_2 w[256,256] b[256] | value_out w[256] b[1].  Stateless, caller-owned DEVICE memory. */
+/* -1 for a bad action_dim */
 int r4_gauss_num_params(int action_dim);
 /* floats of the scratch that r4_gauss_grad / r4_gauss_ppo_epoch* need (any n: samples are processed in chunks); -1 for a
  * bad action_dim */

@@ -1059,7 +1059,7 @@ int r4_copy_prev_actions(r4_env* e, int32_t* out, void* stream) {
     if (_st != cudaSuccess) return fail(nullptr, R4_ERR_CUDA, std::string(name) + ": " + cudaGetErrorString(_st)); \
   } while (0)
 
-int r4_policy_num_params(int action_size) { return r4ppo::make_layout(action_size).n; }
+int r4_policy_num_params(int action_size) { return (action_size < 2 || action_size > 512) ? -1 : r4ppo::make_layout(action_size).n; }
 
 int r4_policy_act(const float* params, const float* obs, const uint8_t* mask, int n, int action_size, int explore,
                   uint64_t seed, uint64_t counter, int32_t* action, float* logp, float* value, float* logits,
@@ -1322,13 +1322,13 @@ int r4_grad_exchange_n(r4_comm* c, const float* partial, int G, int n_params, fl
 }
 
 // ---- Gaussian policy of the continuous-action env (r4_gauss.cuh) -------------------------------------------
-int r4_gauss_num_params(int action_dim) { return r4gauss::make_layout(action_dim).n; }
+static bool gauss_dim_ok(int D) { return D >= 2 && D <= r4gauss::MAXD && D % 2 == 0; }
+
+int r4_gauss_num_params(int action_dim) { return gauss_dim_ok(action_dim) ? r4gauss::make_layout(action_dim).n : -1; }
 
 int64_t r4_gauss_scratch_size(int action_dim) {
-  return (action_dim < 2 || action_dim > r4gauss::MAXD || action_dim % 2) ? -1 : (int64_t)r4gauss::scratch_floats(action_dim);
+  return gauss_dim_ok(action_dim) ? (int64_t)r4gauss::scratch_floats(action_dim) : -1;
 }
-
-static bool gauss_dim_ok(int D) { return D >= 2 && D <= r4gauss::MAXD && D % 2 == 0; }
 
 int r4_gauss_act(const float* params, const float* obs, int n, int action_dim, int explore, uint64_t seed, uint64_t counter,
                  float* action, float* env_action, float* logp, float* value, float* dist_inputs, void* stream) {

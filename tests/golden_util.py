@@ -53,7 +53,16 @@ MARGINS = {}
 
 def _record(what, err, bound, ref):
     key = what.split(" step ")[0]
-    key = "".join(c for c in key if not c.isdigit()).strip() or "?"
+    _record_key("".join(c for c in key if not c.isdigit()).strip() or "?", err, bound, ref)
+
+
+def record_margin(key, err, bound, ref):
+    """Record one comparison under `key` as given: digits are kept, so a key can name the shape it was measured at
+    (the learner grid's `learner rainbow A284 Z8 ... sb2` rows)."""
+    _record_key(key, np.asarray(err, dtype=np.float64), np.asarray(bound, dtype=np.float64), np.asarray(ref, dtype=np.float64))
+
+
+def _record_key(key, err, bound, ref):
     nz = np.abs(ref) > 0
     plain = np.zeros_like(err)
     plain[nz] = err[nz] / np.abs(ref[nz])
