@@ -483,6 +483,53 @@ int r4_batchrl_act(int algo, int obs_dim, int action_size, const float* params, 
 int r4_dien_forward(r4_env* env, const int32_t* seq, const float* dense, const int32_t* cat,
                     int n_rows, float* obs, float* probs, void* stream);
 
+/* ---- training the DIEN simulator (nets/dien.py:8-45 in training mode, supervised_train.py <train> <test> <model> dien 0) on
+ * item samples: sample i of the per-record store is (record i / 9, exposed item i % 9) (data_preprocess.py:91-131,
+ * INTEGRATION.md section 8).  emb_size 128, hidden_units 128, maxlen 64, 432 dense and 21 category features, seq_num 2;
+ * hash_size H = category_hash_size in 1..4000000.  Flat parameter layout (tf_checkpoint.dien_layer_plan order, row-major):
+ *   emb_cat[H,128] dense_w1[432,128] dense_b1[128] dense_w2[128,128] dense_b2[128] emb_seq[H,128]
+ *   then for sequence i = 0, 1: gru_wg[256,256] gru_bg[256] gru_wc[256,128] gru_bc[128] att_w1[512,64] att_b1[64]
+ *     att_w2[64,16] att_b2[16] att_k[16,1] att_b[1] augru_wg[384,512] augru_bg[512] augru_wc[384,256] augru_bc[256]
+ *   obs_w[3456,256] obs_b[256] rew_w[256,2] rew_b[2]
+ * Stateless: every pointer is caller-owned DEVICE memory.  Every id must lie in [0, H) (checked where the store is built). */
+typedef struct {
+  const int32_t* user_cat;     /* i32[N, 10] portrait ids */
+  const float* user_dense;     /* f32[N, 32] portrait dense features */
+  const int32_t* sequence_id;  /* i32[N] */
+  const int32_t* items;        /* i32[N, 9] exposed items */
+  const uint8_t* feedback;     /* u8[N, 9] labels */
+  const float* item_feature;   /* f32[N, 360] the record's item features (9 x 40) */
+  const int32_t* seq;          /* i32[N, 2, 64] user_seqfeature | the earlier pages' items, pre-padded / pre-truncated */
+} r4_simtrain_data;
+/* floats of the flat parameters (27 413 956 at H = 100000); -1 for H out of range */
+int64_t r4_simtrain_num_params(int hash_size);
+/* BYTES of the scratch r4_simtrain_grad / _step / _eval need for n samples (n in 1..4096); -1 out of range */
+int64_t r4_simtrain_scratch_size(int n);
+/* The gradient of the loss (Keras binary_crossentropy of the softmax output on one_hot(label, 2), p clipped to
+ * [1e-7, 1 - 1e-7], mean over both columns and the n samples idx[0..n)) -> grad f32[num_params].  The embedding tables of
+ * grad must be zero on entry (r4_simtrain_apply leaves them so); only the rows the samples touch are written.  Dropout on
+ * the two dense-tower outputs: keep_in (may be NULL) u8[n, 256] (layer-major, 1 = kept), else a unit is kept when the
+ * counter-based draw of (seed, counter, sample, unit) is >= drop_rate; kept units are scaled by 1 / (1 - drop_rate).
+ * keep_out (may be NULL) receives the bits used.  stats (may be NULL) f32[2] = {mean loss, mean binary accuracy};
+ * acc (may be NULL) f64[405] accumulates {loss sum, accuracy sum, samples, positives[201], negatives[201]}, where bin b counts
+ * the probabilities above exactly b of Keras's 200 AUC thresholds (both one-hot columns).  Deterministic. */
+int r4_simtrain_grad(int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n, uint64_t seed,
+                     uint64_t counter, float drop_rate, const uint8_t* keep_in, uint8_t* keep_out, void* scratch, float* grad,
+                     float* stats, double* acc, void* stream);
+/* Keras Adam over every parameter at the 1-based step: m += (g - m)(1 - beta1), v += (g^2 - v)(1 - beta2),
+ * p -= lr sqrt(1 - beta2^step) / (1 - beta1^step) m / (sqrt(v) + eps).  Clears the embedding rows of grad.  1 launch. */
+int r4_simtrain_apply(int hash_size, float* params, float* grad, float* m, float* v, int step, float lr, float beta1, float beta2,
+                      float eps, void* stream);
+/* r4_simtrain_grad (keep bits drawn) then r4_simtrain_apply, with no host round trip. */
+int r4_simtrain_step(int hash_size, float* params, float* grad, float* m, float* v, const r4_simtrain_data* data,
+                     const int64_t* idx, int n, uint64_t seed, uint64_t counter, float drop_rate, int step, float lr, float beta1,
+                     float beta2, float eps, void* scratch, float* stats, double* acc, void* stream);
+/* The forward without dropout -> probs f32[n, 2] (may be NULL); acc (may be NULL) accumulates as in r4_simtrain_grad. */
+int r4_simtrain_eval(int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n, void* scratch,
+                     float* probs, double* acc, void* stream);
+/* kernels launched so far by the r4_simtrain_* entry points in this process (the radix sort counted once) */
+int64_t r4_simtrain_launch_count(void);
+
 #ifdef __cplusplus
 }
 #endif

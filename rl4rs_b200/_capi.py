@@ -32,6 +32,10 @@ class BatchRLData(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("obs", "action", "reward", "terminal", "transitions", "location_mask", "special")]
 
 
+class SimTrainData(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("user_cat", "user_dense", "sequence_id", "items", "feedback", "item_feature", "seq")]
+
+
 class BatchRLHyper(C.Structure):
     _fields_ = [(n, C.c_float) for n in ("gamma", "beta", "alpha", "log_flex", "reward_mean", "reward_den")]
 
@@ -130,6 +134,16 @@ EXPORTS = {
                                                   C.c_float] + [C.c_void_p] * 4),
     "r4_adam_step": (C.c_int,[C.c_void_p] * 4 + [C.c_int, C.c_int] + [C.c_float] * 6 + [C.c_void_p, C.c_void_p]),
     "r4_dien_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "r4_simtrain_num_params": (C.c_int64, [C.c_int]),
+    "r4_simtrain_scratch_size": (C.c_int64, [C.c_int]),
+    "r4_simtrain_grad": (C.c_int, [C.c_int, C.c_void_p, C.POINTER(SimTrainData), C.c_void_p, C.c_int, C.c_uint64, C.c_uint64,
+                                   C.c_float] + [C.c_void_p] * 7),
+    "r4_simtrain_apply": (C.c_int, [C.c_int] + [C.c_void_p] * 4 + [C.c_int] + [C.c_float] * 4 + [C.c_void_p]),
+    "r4_simtrain_step": (C.c_int, [C.c_int] + [C.c_void_p] * 4 + [C.POINTER(SimTrainData), C.c_void_p, C.c_int, C.c_uint64,
+                                                                C.c_uint64, C.c_float, C.c_int] + [C.c_float] * 4 +
+                         [C.c_void_p] * 4),
+    "r4_simtrain_eval": (C.c_int, [C.c_int, C.c_void_p, C.POINTER(SimTrainData), C.c_void_p, C.c_int] + [C.c_void_p] * 4),
+    "r4_simtrain_launch_count": (C.c_int64, []),
 }
 
 _lib = None

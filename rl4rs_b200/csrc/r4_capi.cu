@@ -12,8 +12,10 @@
 #include "r4_ddpg.cuh"
 #include "r4_rainbow.cuh"
 #include "r4_batchrl.cuh"
+#include "r4_simtrain.cuh"
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <cstdlib>
@@ -1858,3 +1860,231 @@ int r4_dien_forward(r4_env* e, const int32_t* seq, const float* dense, const int
 }
 
 }  // extern "C"
+
+// ---- training the DIEN simulator (r4_simtrain.cuh) -------------------------------------------------------------------
+// kernels launched by the r4_simtrain_* entry points in this process (the radix sort counted once)
+static int64_t g_st_launches = 0;
+
+int64_t r4_simtrain_launch_count(void) { return g_st_launches; }
+
+static bool st_hash_ok(int H) { return H >= 1 && H <= r4st::MAXH; }
+
+int64_t r4_simtrain_num_params(int hash_size) { return st_hash_ok(hash_size) ? r4st::make_layout(hash_size).n : -1; }
+
+int64_t r4_simtrain_scratch_size(int n) { return (n < 1 || n > r4st::MAXN) ? -1 : (int64_t)r4st::scratch_bytes(n); }
+
+#define R4_ST_CHECK(name)                                                                   \
+  do {                                                                                      \
+    ++g_st_launches;                                                                        \
+    cudaError_t _st = cudaGetLastError();                                                   \
+    if (_st != cudaSuccess) return fail(nullptr, R4_ERR_CUDA, std::string(name) + ": " + cudaGetErrorString(_st)); \
+  } while (0)
+
+static r4st::Data st_data(const r4_simtrain_data* d) {
+  return r4st::Data{d->user_cat, d->user_dense, d->sequence_id, d->items, d->feedback, d->item_feature, d->seq};
+}
+static bool st_data_ok(const r4_simtrain_data* d) {
+  return d && d->user_cat && d->user_dense && d->sequence_id && d->items && d->feedback && d->item_feature && d->seq;
+}
+
+static int st_gemm(bool tb, const float* A, int lda, const float* B, int ldb, const float* bias, float* C, int ldc, int M, int N,
+                   int K, int epi, cudaStream_t st, const float* aux = nullptr, const float* mul = nullptr, float* pre = nullptr,
+                   int accum = 0) {
+  r4st::Gemm g{A, lda, B, ldb, bias, C, ldc, M, N, K, epi, accum, aux, mul, pre};
+  dim3 grid((N + r4st::GT - 1) / r4st::GT, (M + r4st::GT - 1) / r4st::GT);
+  if (tb) r4st::k_st_gemm<true><<<grid, r4st::NTH, 0, st>>>(g);
+  else r4st::k_st_gemm<false><<<grid, r4st::NTH, 0, st>>>(g);
+  R4_ST_CHECK("k_st_gemm");
+  return R4_OK;
+}
+
+// The forward with saved activations: gather, towers, both sequences (GRU-1, attention, AUGRU), the head and the loss.
+static int st_forward(const r4st::Layout& L, const float* prm, const r4st::Data& D, const int64_t* idx, int n, uint64_t seed,
+                      uint64_t counter, float rate, const uint8_t* keep_in, uint8_t* keep_out, const r4st::Planes& P,
+                      bool with_grad, float* stats, double* acc, float* probs, cudaStream_t st) {
+  using namespace r4st;
+  const int R = n * T;
+  GatherArgs ga{L, D, idx, n, seed, counter, rate, keep_in, keep_out};
+  k_st_gather<<<n, E, 0, st>>>(ga, prm, P);
+  R4_ST_CHECK("k_st_gather");
+  int rc;
+  const float* keep0 = P.keep;
+  const float* keep1 = P.keep + (size_t)n * U;
+  if ((rc = st_gemm(false, P.dense, ND, prm + L.dw1, U, prm + L.db1, P.T1d, U, n, U, ND, EP_ELU, st, nullptr, keep0, P.T1))) return rc;
+  if ((rc = st_gemm(false, P.T1d, U, prm + L.dw2, U, prm + L.db2, P.allf + F_DENSE, FEAT, n, U, U, EP_ELU, st, nullptr, keep1, P.T2)))
+    return rc;
+  for (int i = 0; i < 2; ++i) {
+    const Seq& w = L.s[i];
+    const SeqPlanes& s = P.sp[i];
+    if ((rc = st_gemm(false, s.X, E, prm + w.gwg, 2 * E, prm + w.gbg, s.XG1, 2 * E, R, 2 * E, E, EP_LIN, st))) return rc;
+    if ((rc = st_gemm(false, s.X, E, prm + w.gwc, E, prm + w.gbc, s.XC1, E, R, E, E, EP_LIN, st))) return rc;
+    RecArgs<E> g1{prm + w.gwg + E * 2 * E, prm + w.gwc + E * E, s.XG1, s.XC1, nullptr, s.Hp1, s.G1, s.C1, s.RH1, s.H1, nullptr, 0, n};
+    k_st_gru_fwd<E><<<(n + SB - 1) / SB, NTH, 0, st>>>(g1);
+    R4_ST_CHECK("k_st_gru_fwd<128>");
+    k_st_attin<<<(unsigned)(((size_t)R * E + 255) / 256), 256, 0, st>>>(P.q, s.H1, s.Ain, n);
+    R4_ST_CHECK("k_st_attin");
+    if ((rc = st_gemm(false, s.Ain, 4 * E, prm + w.aw1, A1, prm + w.ab1, s.At1, A1, R, A1, 4 * E, EP_SIG, st))) return rc;
+    if ((rc = st_gemm(false, s.At1, A1, prm + w.aw2, A2, prm + w.ab2, s.At2, A2, R, A2, A1, EP_SIG, st))) return rc;
+    if ((rc = st_gemm(false, s.At2, A2, prm + w.ak, 1, prm + w.ab, s.S, 1, R, 1, A2, EP_LIN, st))) return rc;
+    if ((rc = st_gemm(false, s.H1, E, prm + w.uwg, 4 * E, prm + w.ubg, s.XG2, 4 * E, R, 4 * E, E, EP_LIN, st))) return rc;
+    if ((rc = st_gemm(false, s.H1, E, prm + w.uwc, 2 * E, prm + w.ubc, s.XC2, 2 * E, R, 2 * E, E, EP_LIN, st))) return rc;
+    RecArgs<HA> g2{prm + w.uwg + E * 4 * E, prm + w.uwc + E * 2 * E, s.XG2, s.XC2, s.S, s.Hp2, s.G2, s.C2, s.RH2, nullptr,
+                   P.allf + i * HA, FEAT, n};
+    k_st_gru_fwd<HA><<<(n + SB - 1) / SB, NTH, 0, st>>>(g2);
+    R4_ST_CHECK("k_st_gru_fwd<256>");
+  }
+  if ((rc = st_gemm(false, P.allf, FEAT, prm + L.ow, OBS, prm + L.ob, P.O, OBS, n, OBS, FEAT, EP_ELU, st))) return rc;
+  if ((rc = st_gemm(false, P.O, OBS, prm + L.rw, 2, prm + L.rb, P.Z, 2, n, 2, OBS, EP_LIN, st))) return rc;
+  k_st_loss<<<1, NTH, 0, st>>>(D, idx, n, P.Z, with_grad ? P.dZ : nullptr, P.stats, stats, acc, probs);
+  R4_ST_CHECK("k_st_loss");
+  return R4_OK;
+}
+
+static r4ddpg::Job st_job(const float* X, int ldx, const float* Z, int M, int N, int64_t off) {
+  return r4ddpg::Job{X, Z, ldx, M, N, (int)off, 0};
+}
+static int st_wgrad(r4ddpg::Jobs J, int njob, int rows, float* grad, cudaStream_t st) {
+  J.njob = njob;
+  int t = 0;
+  for (int i = 0; i < njob; ++i) {
+    J.j[i].tile0 = t;
+    t += ((J.j[i].M + r4ddpg::WT - 1) / r4ddpg::WT) * ((J.j[i].N + r4ddpg::WT - 1) / r4ddpg::WT);
+  }
+  J.ntiles = t;
+  r4ddpg::k_ddpg_wgrad<<<t, r4ddpg::NT, 0, st>>>(J, rows, grad, nullptr, nullptr, 0.f);
+  R4_ST_CHECK("k_ddpg_wgrad");
+  return R4_OK;
+}
+
+static int st_backward(const r4st::Layout& L, const float* prm, const r4st::Data& D, const int64_t* idx, int n,
+                       const r4st::Planes& P, float* grad, cudaStream_t st) {
+  using namespace r4st;
+  const int R = n * T;
+  int rc;
+  // head: dO = dZ rew_w^T elu'(O); dAllf = dO obs_w^T; the dense tower's columns again with its activation and dropout
+  if ((rc = st_gemm(true, P.dZ, 2, prm + L.rw, 2, nullptr, P.dO, OBS, n, OBS, 2, EP_DELU, st, P.O))) return rc;
+  if ((rc = st_gemm(true, P.dO, OBS, prm + L.ow, OBS, nullptr, P.dAllf, FEAT, n, FEAT, OBS, EP_LIN, st))) return rc;
+  if ((rc = st_gemm(true, P.dO, OBS, prm + L.ow + (int64_t)F_DENSE * OBS, OBS, nullptr, P.dT2, U, n, U, OBS, EP_DELU, st, P.T2,
+                    P.keep + (size_t)n * U)))
+    return rc;
+  if ((rc = st_gemm(true, P.dT2, U, prm + L.dw2, U, nullptr, P.dT1, U, n, U, U, EP_DELU, st, P.T1, P.keep))) return rc;
+  k_st_cat_bwd<<<n, E, 0, st>>>(P.allf, P.P, P.dAllf, P.dEcat);
+  R4_ST_CHECK("k_st_cat_bwd");
+  for (int i = 0; i < 2; ++i) {
+    const Seq& w = L.s[i];
+    const SeqPlanes& s = P.sp[i];
+    RecBack<HA> b2{prm + w.uwg + E * 4 * E, prm + w.uwc + E * 2 * E, s.Hp2, s.G2, s.C2, s.S, nullptr, P.dAllf + i * HA, FEAT,
+                   s.XG2, s.XC2, s.dS, n};
+    k_st_gru_bwd<HA><<<(n + SB - 1) / SB, NTH, 0, st>>>(b2);
+    R4_ST_CHECK("k_st_gru_bwd<256>");
+    if ((rc = st_gemm(true, s.XG2, 4 * E, prm + w.uwg, 4 * E, nullptr, s.dH1, E, R, E, 4 * E, EP_LIN, st))) return rc;
+    if ((rc = st_gemm(true, s.XC2, 2 * E, prm + w.uwc, 2 * E, nullptr, s.dH1, E, R, E, 2 * E, EP_LIN, st, nullptr, nullptr,
+                      nullptr, 1)))
+      return rc;
+    if ((rc = st_gemm(true, s.dS, 1, prm + w.ak, 1, nullptr, s.dA2, A2, R, A2, 1, EP_DSIG, st, s.At2))) return rc;
+    if ((rc = st_gemm(true, s.dA2, A2, prm + w.aw2, A2, nullptr, s.dA1, A1, R, A1, A2, EP_DSIG, st, s.At1))) return rc;
+    if ((rc = st_gemm(true, s.dA1, A1, prm + w.aw1, A1, nullptr, s.dAin, 4 * E, R, 4 * E, A1, EP_LIN, st))) return rc;
+    k_st_attin_bwd<<<n, E, 0, st>>>(P.q, s.H1, s.dAin, s.dH1, s.dq);
+    R4_ST_CHECK("k_st_attin_bwd");
+    RecBack<E> b1{prm + w.gwg + E * 2 * E, prm + w.gwc + E * E, s.Hp1, s.G1, s.C1, nullptr, s.dH1, nullptr, 0, s.XG1, s.XC1,
+                  nullptr, n};
+    k_st_gru_bwd<E><<<(n + SB - 1) / SB, NTH, 0, st>>>(b1);
+    R4_ST_CHECK("k_st_gru_bwd<128>");
+    if ((rc = st_gemm(true, s.XG1, 2 * E, prm + w.gwg, 2 * E, nullptr, s.dX, E, R, E, 2 * E, EP_LIN, st))) return rc;
+    if ((rc = st_gemm(true, s.XC1, E, prm + w.gwc, E, nullptr, s.dX, E, R, E, E, EP_LIN, st, nullptr, nullptr, nullptr, 1)))
+      return rc;
+  }
+  // dense weight gradients: one launch over the n-row jobs, one per sequence over its 64 n-row jobs
+  r4ddpg::Jobs J;
+  int k = 0;
+  J.j[k++] = st_job(P.dense, ND, P.dT1, ND, U, L.dw1);  J.j[k++] = st_job(nullptr, 1, P.dT1, 1, U, L.db1);
+  J.j[k++] = st_job(P.T1d, U, P.dT2, U, U, L.dw2);      J.j[k++] = st_job(nullptr, 1, P.dT2, 1, U, L.db2);
+  J.j[k++] = st_job(P.allf, FEAT, P.dO, FEAT, OBS, L.ow); J.j[k++] = st_job(nullptr, 1, P.dO, 1, OBS, L.ob);
+  J.j[k++] = st_job(P.O, OBS, P.dZ, OBS, 2, L.rw);      J.j[k++] = st_job(nullptr, 1, P.dZ, 1, 2, L.rb);
+  if ((rc = st_wgrad(J, k, n, grad, st))) return rc;
+  for (int i = 0; i < 2; ++i) {
+    const Seq& w = L.s[i];
+    const SeqPlanes& s = P.sp[i];
+    k = 0;
+    J.j[k++] = st_job(s.X, E, s.XG1, E, 2 * E, w.gwg);   J.j[k++] = st_job(s.Hp1, E, s.XG1, E, 2 * E, w.gwg + E * 2 * E);
+    J.j[k++] = st_job(nullptr, 1, s.XG1, 1, 2 * E, w.gbg);
+    J.j[k++] = st_job(s.X, E, s.XC1, E, E, w.gwc);       J.j[k++] = st_job(s.RH1, E, s.XC1, E, E, w.gwc + E * E);
+    J.j[k++] = st_job(nullptr, 1, s.XC1, 1, E, w.gbc);
+    J.j[k++] = st_job(s.Ain, 4 * E, s.dA1, 4 * E, A1, w.aw1); J.j[k++] = st_job(nullptr, 1, s.dA1, 1, A1, w.ab1);
+    J.j[k++] = st_job(s.At1, A1, s.dA2, A1, A2, w.aw2);  J.j[k++] = st_job(nullptr, 1, s.dA2, 1, A2, w.ab2);
+    J.j[k++] = st_job(s.At2, A2, s.dS, A2, 1, w.ak);     J.j[k++] = st_job(nullptr, 1, s.dS, 1, 1, w.ab);
+    J.j[k++] = st_job(s.H1, E, s.XG2, E, 4 * E, w.uwg);  J.j[k++] = st_job(s.Hp2, HA, s.XG2, HA, 4 * E, w.uwg + E * 4 * E);
+    J.j[k++] = st_job(nullptr, 1, s.XG2, 1, 4 * E, w.ubg);
+    J.j[k++] = st_job(s.H1, E, s.XC2, E, 2 * E, w.uwc);  J.j[k++] = st_job(s.RH2, HA, s.XC2, HA, 2 * E, w.uwc + E * 2 * E);
+    J.j[k++] = st_job(nullptr, 1, s.XC2, 1, 2 * E, w.ubc);
+    if ((rc = st_wgrad(J, k, R, grad, st))) return rc;
+  }
+  // embedding gradients: keys, a stable radix sort by (table, id), one ordered sum per run
+  const int total = n * NSLOT;
+  k_st_dq<<<(n * E + 255) / 256, 256, 0, st>>>(P.sp[0].dq, P.sp[1].dq, P.dqs, n);
+  R4_ST_CHECK("k_st_dq");
+  k_st_embkeys<<<(total + 255) / 256, 256, 0, st>>>(L, D, idx, n, P.cat, P.keys, P.vals);
+  R4_ST_CHECK("k_st_embkeys");
+  int bits = 1;
+  while (bits < 32 && ((uint64_t)1 << bits) < (uint64_t)(2 * L.H)) ++bits;
+  cub::DoubleBuffer<uint32_t> kb(P.keys, P.keys2);
+  cub::DoubleBuffer<int32_t> vb(P.vals, P.vals2);
+  size_t need = 0;
+  if (cub::DeviceRadixSort::SortPairs(nullptr, need, kb, vb, total, 0, bits, st) != cudaSuccess || need > P.cub_bytes)
+    return fail(nullptr, R4_ERR_NOMEM, "r4_simtrain: radix sort temporary storage exceeds the scratch reserve");
+  size_t have = P.cub_bytes;
+  if (cub::DeviceRadixSort::SortPairs(P.cub_tmp, have, kb, vb, total, 0, bits, st) != cudaSuccess)
+    return fail(nullptr, R4_ERR_CUDA, std::string("cub::DeviceRadixSort: ") + cudaGetErrorString(cudaGetLastError()));
+  R4_ST_CHECK("cub::DeviceRadixSort::SortPairs");
+  k_st_embsum<<<total, EST, 0, st>>>(L, kb.Current(), vb.Current(), total, P.dEcat, P.sp[0].dX, P.sp[1].dX, P.dqs, grad);
+  R4_ST_CHECK("k_st_embsum");
+  return R4_OK;
+}
+
+static int st_apply(int H, float* params, float* grad, float* m, float* v, int step, float lr, float b1, float b2, float eps,
+                    cudaStream_t st) {
+  const r4st::Layout L = r4st::make_layout(H);
+  const double alpha = (double)lr * std::sqrt(1.0 - std::pow((double)b2, step)) / (1.0 - std::pow((double)b1, step));
+  r4st::k_st_apply<<<(unsigned)((L.n + 255) / 256), 256, 0, st>>>(L, params, grad, m, v, (float)alpha, b1, b2, eps);
+  R4_ST_CHECK("k_st_apply");
+  return R4_OK;
+}
+
+int r4_simtrain_grad(int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n, uint64_t seed,
+                     uint64_t counter, float drop_rate, const uint8_t* keep_in, uint8_t* keep_out, void* scratch, float* grad,
+                     float* stats, double* acc, void* stream) {
+  if (!st_hash_ok(hash_size) || !params || !st_data_ok(data) || !idx || n < 1 || n > r4st::MAXN || !(drop_rate >= 0.f) ||
+      !(drop_rate < 1.f) || !scratch || !grad)
+    return fail(nullptr, R4_ERR_ARG, "r4_simtrain_grad: bad argument (hash_size 1..4000000, n 1..4096, drop_rate in [0, 1))");
+  const r4st::Layout L = r4st::make_layout(hash_size);
+  const r4st::Planes P = r4st::make_planes(scratch, n);
+  const r4st::Data D = st_data(data);
+  cudaStream_t st = S(stream);
+  int rc = st_forward(L, params, D, idx, n, seed, counter, drop_rate, keep_in, keep_out, P, true, stats, acc, nullptr, st);
+  return rc ? rc : st_backward(L, params, D, idx, n, P, grad, st);
+}
+
+int r4_simtrain_apply(int hash_size, float* params, float* grad, float* m, float* v, int step, float lr, float beta1, float beta2,
+                      float eps, void* stream) {
+  if (!st_hash_ok(hash_size) || !params || !grad || !m || !v || step < 1)
+    return fail(nullptr, R4_ERR_ARG, "r4_simtrain_apply: bad argument");
+  return st_apply(hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, S(stream));
+}
+
+int r4_simtrain_step(int hash_size, float* params, float* grad, float* m, float* v, const r4_simtrain_data* data,
+                     const int64_t* idx, int n, uint64_t seed, uint64_t counter, float drop_rate, int step, float lr, float beta1,
+                     float beta2, float eps, void* scratch, float* stats, double* acc, void* stream) {
+  if (!m || !v || step < 1) return fail(nullptr, R4_ERR_ARG, "r4_simtrain_step: bad argument");
+  int rc = r4_simtrain_grad(hash_size, params, data, idx, n, seed, counter, drop_rate, nullptr, nullptr, scratch, grad, stats, acc,
+                            stream);
+  return rc ? rc : st_apply(hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, S(stream));
+}
+
+int r4_simtrain_eval(int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n, void* scratch,
+                     float* probs, double* acc, void* stream) {
+  if (!st_hash_ok(hash_size) || !params || !st_data_ok(data) || !idx || n < 1 || n > r4st::MAXN || !scratch)
+    return fail(nullptr, R4_ERR_ARG, "r4_simtrain_eval: bad argument");
+  const r4st::Layout L = r4st::make_layout(hash_size);
+  const r4st::Planes P = r4st::make_planes(scratch, n);
+  return st_forward(L, params, st_data(data), idx, n, 0, 0, 0.f, nullptr, nullptr, P, false, nullptr, acc, probs, S(stream));
+}
