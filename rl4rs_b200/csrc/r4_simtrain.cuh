@@ -106,22 +106,18 @@ struct Planes {
   int32_t *vals, *vals2;
   void* cub_tmp;
   size_t cub_bytes;
+  size_t bytes;                          // the end of the radix sort's reserve: the scratch size the layout needs
 };
-__host__ __device__ inline size_t seq_row_floats() {
-  return (size_t)E + 2 * E + E + E + E + 2 * E + E + E + 4 * E + A1 + A2 + 1 + 4 * E + 2 * E + HA + 2 * HA + HA + HA + 1 + E +
-         A2 + A1 + 4 * E + E;
-}
-__host__ __device__ inline size_t sample_floats() {
-  return (size_t)NC + ND + 2 * U + U + U + U + FEAT + NC * NC + E + OBS + 2 + 2 + OBS + FEAT + U + U + NC * E + E + 2 +
-         2 * E + 2 * T * seq_row_floats() + 4 * NSLOT;
-}
 __host__ inline size_t cub_reserve(int n) { return ((size_t)4 << 20) + (size_t)16 * n * NSLOT; }
-__host__ inline size_t scratch_bytes(int n) { return (size_t)n * sample_floats() * 4 + cub_reserve(n) + 256; }
 
+// The planes are cut from the scratch in this order, each rounded up to 256 bytes, and the radix sort's reserve follows.
+// With base = nullptr only the offsets are formed: scratch_bytes is the end of the same cuts, so the size a caller
+// allocates and the layout a launch uses cannot disagree.
 __host__ inline Planes make_planes(void* base, int n) {
   Planes P;
-  char* p = reinterpret_cast<char*>(base);
-  auto take = [&](size_t floats) { float* q = reinterpret_cast<float*>(p); p += ((floats * 4 + 255) / 256) * 256; return q; };
+  const uintptr_t b = reinterpret_cast<uintptr_t>(base);
+  size_t o = 0;
+  auto take = [&](size_t floats) { float* q = reinterpret_cast<float*>(b + o); o += ((floats * 4 + 255) / 256) * 256; return q; };
   const size_t R = (size_t)n * T;
   P.cat = reinterpret_cast<int32_t*>(take((size_t)n * NC));
   P.dense = take((size_t)n * ND); P.keep = take((size_t)n * 2 * U);
@@ -142,10 +138,12 @@ __host__ inline Planes make_planes(void* base, int n) {
   }
   P.keys = reinterpret_cast<uint32_t*>(take((size_t)n * NSLOT)); P.keys2 = reinterpret_cast<uint32_t*>(take((size_t)n * NSLOT));
   P.vals = reinterpret_cast<int32_t*>(take((size_t)n * NSLOT)); P.vals2 = reinterpret_cast<int32_t*>(take((size_t)n * NSLOT));
-  P.cub_tmp = p;
+  P.cub_tmp = reinterpret_cast<void*>(b + o);
   P.cub_bytes = cub_reserve(n);
+  P.bytes = o + P.cub_bytes;
   return P;
 }
+__host__ inline size_t scratch_bytes(int n) { return make_planes(nullptr, n).bytes; }
 
 __device__ __forceinline__ float sigm(float x) { return 1.f / (1.f + expf(-x)); }
 __device__ __forceinline__ float elu(float x) { return x > 0.f ? x : expm1f(x); }

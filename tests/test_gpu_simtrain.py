@@ -61,7 +61,7 @@ def _kernel_grad(tr, samples, idx, rate, keep_in=None):
 
 
 @pytest.mark.parametrize("kind", ["default", "stress"])
-@pytest.mark.parametrize("n", [1, 7, 33, 256, 257])
+@pytest.mark.parametrize("n", [1, 7, 8, 9, 33, 63, 64, 65, 256, 257])
 @pytest.mark.parametrize("rate", [0.0, 0.2])
 def test_gradient_parity_per_tensor(samples, kind, n, rate):
     w = _weights(kind)

@@ -198,3 +198,69 @@ def test_size_functions_reject_out_of_range():
     assert lib.r4_simtrain_num_params(0) == -1 and lib.r4_simtrain_num_params(4000001) == -1
     assert lib.r4_simtrain_scratch_size(0) == -1 and lib.r4_simtrain_scratch_size(4097) == -1
     assert 0 < lib.r4_simtrain_scratch_size(1) < lib.r4_simtrain_scratch_size(256) < lib.r4_simtrain_scratch_size(4096)
+    for H in (1, 9, 4000000):
+        assert lib.r4_simtrain_num_params(H) == R.num_params(H)
+
+
+@pytest.mark.parametrize("n", list(range(1, 131)) + [4095, 4096])
+def test_scratch_size_is_the_end_of_the_layout(n):
+    """The scratch size is where the radix sort's reserve ends after the planes make_planes cuts, each rounded up to 256
+    bytes (R.scratch_cuts restates that take sequence): a smaller size lets the sort's storage run past the buffer
+    whenever a plane is not a multiple of 256 bytes (n not a multiple of 64)."""
+    from rl4rs_b200 import _capi
+    assert _capi.load_library().r4_simtrain_scratch_size(n) == R.scratch_bytes(n)
+
+
+def test_compact_reference_equals_full_reference():
+    """The reference over the ids a batch touches (compacted tables) gives the full reference's touched rows, and the full
+    reference is exactly zero on every other row; chunking the batch changes nothing but the rounding."""
+    H = 700
+    cfg = {"category_hash_size": H}
+    s = R.make_edge_samples(4, H, seed=3)
+    idx = np.array([0, 5, 13, 22, 30])
+    w = synth.make_weights(cfg, seed=8, stress=2.0, bias_noise=0.1, bounded_scores=True)
+    keep = R.keep_bits(3, 4, len(idx), 0.2)
+    loss, full, probs = R.ref_grad(cfg, simtrain.flatten(w, cfg), s, idx, keep, 0.2)
+    ids, sc, ic = R.compact(s, idx)
+    assert len(ids) < H and sc.hash_size == len(ids)
+    ccfg = {"category_hash_size": len(ids)}
+    closs, cg, cprobs = R.ref_grad(ccfg, simtrain.flatten(R.compact_weights(w, ids), ccfg), sc, ic, keep, 0.2, chunk=2)
+    assert abs(closs - loss) <= 1e-12 * abs(loss) and np.abs(cprobs - probs).max() <= 1e-12
+    ft, ct = simtrain.unflatten(full, cfg), simtrain.unflatten(cg, ccfg)
+    for name in ft:
+        got = ft[name][ids] if name.startswith("emb_") else ft[name]
+        assert np.abs(got - ct[name]).max() <= 1e-12 * np.abs(ct[name]).max(), name
+    rows = R.touched_rows(s, idx)
+    for name in ("emb_cat", "emb_seq"):
+        mask = np.ones(H, bool)
+        mask[ids] = False
+        assert not ft[name][mask].any(), name
+        assert set(np.flatnonzero(np.abs(ft[name]).sum(1))) == set(rows[name]), name
+
+
+def test_keep_bits_restatement():
+    """The NumPy restatement of the kernel's dropout draw: rate 0 keeps everything, the kept share is 1 - rate, the draw
+    depends on the seed, the counter and the sample, and a lower rate keeps a superset."""
+    assert R.keep_bits(5, 7, 9, 0.0).all()
+    k = R.keep_bits(5, 7, 4096, 0.2)
+    assert k.shape == (4096, 256) and k.dtype == np.uint8
+    assert abs(k.mean() - 0.8) < 3e-3                               # 1M draws: sigma 4e-4
+    assert abs(R.keep_bits(2 ** 63 + 3, 2 ** 32 + 1, 4096, 0.5).mean() - 0.5) < 3e-3
+    assert not np.array_equal(k, R.keep_bits(6, 7, 4096, 0.2)) and not np.array_equal(k, R.keep_bits(5, 8, 4096, 0.2))
+    assert not np.array_equal(k[:64], k[64:128])
+    assert np.all(R.keep_bits(5, 7, 4096, 0.1) >= k)
+
+
+def test_edge_samples_cover_the_edges():
+    for H in (9, 3000):
+        s = R.make_edge_samples(64, H, seed=1)
+        cat, _, seq, _ = s.features(np.arange(len(s)))
+        assert cat.min() == 0 and cat.max() == H - 1 and seq.min() == 0 and seq.max() == H - 1
+        for col in (s.user_cat, s.sequence_id, s.items, s.seq[:, 0], s.seq[:, 1]):
+            assert col.min() == 0 and (col == H - 1).any()
+        assert not s.seq[:, 1].any(1).all() and not s.seq[:, 0].any(1).all()       # empty sequences
+        both = [r for r in range(s.n_records) if set(s.user_cat[r]) & set(s.items[r]) & set(s.seq[r, 0]) & set(s.seq[r, 1])]
+        assert len(both) >= s.n_records // 4
+    r = R.make_range_samples(20, 100, 50, 100)
+    cat, _, seq, _ = r.features(np.arange(len(r)))
+    assert cat.min() >= 50 and seq.min() >= 50 and cat.max() < 100
