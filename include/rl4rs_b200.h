@@ -529,6 +529,10 @@ int r4_simtrain_eval(int hash_size, const float* params, const r4_simtrain_data*
                      float* probs, double* acc, void* stream);
 /* kernels launched so far by the r4_simtrain_* entry points in this process (the radix sort counted once) */
 int64_t r4_simtrain_launch_count(void);
+/* kernels launched so far by every learner entry point in this process (r4_policy_*, r4_gae, r4_adam_step, r4_ppo_epoch*,
+ * r4_grad_exchange*, r4_gauss_*, r4_ddpg_*, r4_replay_*, r4_rainbow_*, r4_batchrl_*, r4_simtrain_*): the sum of the batch
+ * RL and simulator-trainer counts above and the online learners'. */
+int64_t r4_learner_launch_count(void);
 
 #ifdef __cplusplus
 }

@@ -144,6 +144,7 @@ EXPORTS = {
                          [C.c_void_p] * 4),
     "r4_simtrain_eval": (C.c_int, [C.c_int, C.c_void_p, C.POINTER(SimTrainData), C.c_void_p, C.c_int] + [C.c_void_p] * 4),
     "r4_simtrain_launch_count": (C.c_int64, []),
+    "r4_learner_launch_count": (C.c_int64, []),
 }
 
 _lib = None

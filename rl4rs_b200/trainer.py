@@ -60,7 +60,13 @@ class KernelOps(object):
         self.scratch = z(self._scratch_floats())
         self.step = 0
         self.counter = 0
-        self.launches = 0                # kernels launched through this object (bench.py: gpu_launches)
+        self._launch0 = self.lib.r4_learner_launch_count()
+
+    @property
+    def launches(self):
+        """Kernels launched by every learner entry point of this process since this object was made, as the library counts
+        them (r4_learner_launch_count; bench.py's gpu_launches).  In a process that drives one learner, those are its own."""
+        return self.lib.r4_learner_launch_count() - self._launch0
 
     def _num_params(self):
         return self.lib.r4_policy_num_params(self.A)
@@ -81,26 +87,22 @@ class KernelOps(object):
                                     _p(action_i32), _p(logp), _p(value), _p(logits), self._stream())
         self._check(rc, "r4_policy_act")
         self.counter += n
-        self.launches += 1
 
     def policy_grad(self, mode, flat, data, idx, idx_offset, n, hp, inv_n, stat_scale, G=None):
         G = G or max(1, min((n + 3) // 4, self.sms))          # 4 samples per CTA tile (r4_ppo.cuh: TS)
         rc = self.lib.r4_policy_grad(mode, _p(flat), *map(_p, data), _p(idx, idx_offset * 8), n, self.A, *_hp(hp), inv_n,
                                      _p(self.scratch), G, _p(self.grad), _p(self.stats), stat_scale, self._stream())
         self._check(rc, "r4_policy_grad")
-        self.launches += 2               # k_policy_grad + k_grad_reduce
 
     def ppo_epoch(self, flat, data, perm, n, mb, hp, lr, clip):
         """All minibatch steps of one SGD epoch in ONE library call (single-GPU learner)."""
         rc = self._epoch("r4_ppo_epoch", (), self.A, flat, data, perm, n, mb, hp, lr, (float(clip or 0.0), _p(self.norm)))
-        self.launches += rc * (4 if clip else 2)   # k_policy_grad + k_reduce_adam, or + k_grad_reduce, k_sumsq, k_adam
         return rc
 
     def ppo_epoch_dist(self, comm, flat, data, perm, n, mb_local, hp, lr):
         """All minibatch steps of one SGD epoch of a data-parallel learner in ONE library call: per step the gradient
         kernel + the fused peer-memory exchange / Adam kernel (csrc/r4_comm.cuh); no NCCL, no host round trip."""
         rc = self._epoch("r4_ppo_epoch_dist", (comm.h,), self.A, flat, data, perm, n, mb_local, hp, lr, ())
-        self.launches += rc * 2          # k_policy_grad + k_exchange_adam
         return rc
 
     def _epoch(self, fn, head, dim, flat, data, perm, n, mb, hp, lr, tail):
@@ -121,7 +123,6 @@ class KernelOps(object):
                                              _p(self.scratch), G, self._stream())
         self._check(rc, "r4_policy_grad_partial")
         self._exchange(comm, self.scratch, G, stat_scale)
-        self.launches += 2
 
     def _exchange(self, comm, partial, G, stat_scale):
         """self.grad = the sum over the ranks of this rank's G partial gradients in `partial` (then their statistics)."""
@@ -134,7 +135,6 @@ class KernelOps(object):
         adv, target = torch.empty_like(reward), torch.empty_like(reward)
         rc = self.lib.r4_gae(_p(reward), _p(value), reward.shape[0], reward.shape[1], gamma, gamma * lam, _p(adv), _p(target), self._stream())
         self._check(rc, "r4_gae")
-        self.launches += 1
         return target, adv
 
     def adam(self, flat, lr, grad_scale, clip):
@@ -142,7 +142,6 @@ class KernelOps(object):
         rc = self.lib.r4_adam_step(_p(flat), _p(self.grad), _p(self.m), _p(self.v), self.n, self.step, lr, 0.9, 0.999,
                                    1e-8, grad_scale, float(clip or 0.0), _p(self.norm), self._stream())
         self._check(rc, "r4_adam_step")
-        self.launches += 2 if clip else 1
 
 
 class GaussKernelOps(KernelOps):
@@ -167,10 +166,6 @@ class GaussKernelOps(KernelOps):
                                    _p(env_action), _p(logp), _p(value), _p(dist_inputs), self._stream())
         self._check(rc, "r4_gauss_act")
         self.counter += n
-        self.launches += 1
-
-    def _chunks(self, n):
-        return 2 * -(-n // 2048)         # k_gauss_rows + k_gauss_wgrad per chunk of 2048 samples (r4_gauss.cuh: CH)
 
     def policy_grad(self, mode, flat, data, idx, idx_offset, n, hp, inv_n, stat_scale, grad=None, stats=None):
         grad = self.grad if grad is None else grad
@@ -178,16 +173,13 @@ class GaussKernelOps(KernelOps):
         rc = self.lib.r4_gauss_grad(mode, _p(flat), *map(_p, data), _p(idx, idx_offset * 8), n, self.D, *_hp(hp), inv_n,
                                     _p(self.scratch), _p(grad), _p(stats), stat_scale, self._stream())
         self._check(rc, "r4_gauss_grad")
-        self.launches += self._chunks(n)
 
     def ppo_epoch(self, flat, data, perm, n, mb, hp, lr, clip):
         rc = self._epoch("r4_gauss_ppo_epoch", (), self.D, flat, data, perm, n, mb, hp, lr, (float(clip or 0.0), _p(self.norm)))
-        self.launches += rc * (self._chunks(mb) + (2 if clip else 1))
         return rc
 
     def ppo_epoch_dist(self, comm, flat, data, perm, n, mb_local, hp, lr):
         rc = self._epoch("r4_gauss_ppo_epoch_dist", (comm.h,), self.D, flat, data, perm, n, mb_local, hp, lr, ())
-        self.launches += rc * (self._chunks(mb_local) + 1)
         return rc
 
     def policy_grad_exchange(self, comm, mode, flat, data, n, hp, inv_n, stat_scale):
@@ -195,7 +187,6 @@ class GaussKernelOps(KernelOps):
         self.gsum[self.n:].zero_()
         self.policy_grad(mode, flat, data, None, 0, n, hp, inv_n, 1.0, grad=self.gsum[:self.n], stats=self.gsum[self.n:])
         self._exchange(comm, self.gsum, 1, stat_scale)
-        self.launches += 1
 
 
 class PeerComm(object):
@@ -800,16 +791,16 @@ class DDPGKernelOps(object):
         self.m, self.v, self.stats = z(n_params), z(n_params), z(3)
         self.grad, self.td = z(n_params), z(n)
         self.scratch = z(self.lib.r4_ddpg_scratch_size(D, self.twin, n))
-        self.launches = 0
+        self._launch0 = self.lib.r4_learner_launch_count()
 
     _stream = KernelOps._stream
     _check = KernelOps._check
+    launches = KernelOps.launches
 
     def act(self, flat, obs, mode, seed, counter, ou_in, ou_out, theta, sigma, ns, action):
         rc = self.lib.r4_ddpg_act(_p(flat), _p(obs), obs.shape[0], self.D, mode, seed, counter, _p(ou_in), _p(ou_out), theta,
                                   sigma, ns, _p(action), self._stream())
         self._check(rc, "r4_ddpg_act")
-        self.launches += 1
 
     def _replay(self, rb):
         return _p(rb.obs), _p(rb.action), _p(rb.reward), _p(rb.new_obs), _p(rb.done)
@@ -819,7 +810,6 @@ class DDPGKernelOps(object):
         rc = self.lib.r4_replay_store(*self._replay(rb), _p(rb.prio), _p(rb.max_prio), rb.C, self.D, rb.added, rb.alpha,
                                       _p(obs), _p(final_obs), _p(action), _p(reward), _p(done), T, B, self._stream())
         self._check(rc, "r4_replay_store")
-        self.launches += 1
 
     def replay_sample(self, rb, u, beta):
         n = u.shape[0]
@@ -827,14 +817,12 @@ class DDPGKernelOps(object):
         w = torch.empty(n, dtype=torch.float32, device=self.device)
         rc = self.lib.r4_replay_sample(_p(rb.prio), rb.size, n, beta, _p(u), _p(idx), _p(w), self._stream())
         self._check(rc, "r4_replay_sample")
-        self.launches += 1
         return idx, w
 
     def replay_priorities(self, rb, idx, td, eps):
         rc = self.lib.r4_replay_update_priorities(_p(rb.prio), _p(rb.max_prio), _p(idx), _p(td), idx.shape[0], rb.alpha, eps,
                                                   self._stream())
         self._check(rc, "r4_replay_update_priorities")
-        self.launches += 1
 
     def grad_(self, pol, rb, idx, weights, noise, hp, inv_n):
         """self.grad, self.td, self.stats = r4_ddpg_grad over replay rows idx."""
@@ -842,14 +830,12 @@ class DDPGKernelOps(object):
                                    _p(noise), idx.shape[0], hp["gamma"], hp["target_noise"], hp["noise_clip"], inv_n,
                                    _p(self.scratch), _p(self.grad), _p(self.td), _p(self.stats), self._stream())
         self._check(rc, "r4_ddpg_grad")
-        self.launches += 2
 
     def apply(self, pol, actor_step, critic_step, hp, grad_scale=1.0):
         rc = self.lib.r4_ddpg_apply(_p(pol.flat), _p(pol.target), _p(self.grad), _p(self.m), _p(self.v), self.D, self.twin,
                                     actor_step, critic_step, hp["actor_lr"], hp["critic_lr"], hp["l2_reg"], hp["tau"],
                                     grad_scale, self._stream())
         self._check(rc, "r4_ddpg_apply")
-        self.launches += 1
 
     def train_step(self, comm, pol, rb, u, noise, actor_step, critic_step, hp):
         """One whole SGD step in one library call (sample, gradient, exchange over peer memory, Adams + soft update,
@@ -861,8 +847,6 @@ class DDPGKernelOps(object):
                                          hp["critic_lr"], hp["l2_reg"], hp["tau"], _p(self.scratch), _p(self.stats),
                                          self._stream())
         self._check(rc, "r4_ddpg_train_step")
-        self.launches += 5 if rb.prio is not None else 4
-        self.launches += 1 if comm is not None else 0
 
 
 class DDPGTrainer(_TrainerBase):
@@ -1113,10 +1097,11 @@ class RainbowKernelOps(object):
         self.m, self.v, self.stats = z(n_params), z(n_params), z(3)
         self.grad, self.td = z(n_params), z(n)
         self.scratch = z(self.lib.r4_rainbow_scratch_size(A, atoms, n))
-        self.launches = 0
+        self._launch0 = self.lib.r4_learner_launch_count()
 
     _stream = KernelOps._stream
     _check = KernelOps._check
+    launches = KernelOps.launches
     _replay = DDPGKernelOps._replay
     replay_sample = DDPGKernelOps.replay_sample
     replay_priorities = DDPGKernelOps.replay_priorities
@@ -1125,7 +1110,6 @@ class RainbowKernelOps(object):
         rc = self.lib.r4_rainbow_act(_p(pol.flat), _p(obs), obs.shape[0], self.A, self.atoms, pol.v_min, pol.v_max,
                                      int(bool(explore)), seed, counter, _p(action), _p(q), self._stream())
         self._check(rc, "r4_rainbow_act")
-        self.launches += 1
 
     def replay_store(self, rb, obs, final_obs, action, reward, done):
         T, B = reward.shape
@@ -1133,7 +1117,6 @@ class RainbowKernelOps(object):
                                             rb.n_step, rb.gamma, _p(obs), _p(final_obs), _p(action), _p(reward), _p(done),
                                             T, B, self._stream())
         self._check(rc, "r4_replay_store_nstep")
-        self.launches += 1
 
     def grad_(self, pol, rb, idx, weights, gamma_n, inv_n):
         """self.grad, self.td, self.stats = r4_rainbow_grad over replay rows idx."""
@@ -1141,14 +1124,12 @@ class RainbowKernelOps(object):
                                       *self._replay(rb), _p(idx), _p(weights), idx.shape[0], gamma_n, inv_n,
                                       _p(self.scratch), _p(self.grad), _p(self.td), _p(self.stats), self._stream())
         self._check(rc, "r4_rainbow_grad")
-        self.launches += 2
 
     def apply(self, pol, step, hp, copy_target):
         rc = self.lib.r4_rainbow_apply(_p(pol.flat), _p(pol.target), _p(self.grad), _p(self.m), _p(self.v), self.A,
                                        self.atoms, step, hp["lr"], hp["adam_eps"], hp["grad_clip"], int(copy_target),
                                        self._stream())
         self._check(rc, "r4_rainbow_apply")
-        self.launches += 1
 
     def train_step(self, comm, pol, rb, u, step, copy_target, hp):
         """One whole SGD step in one library call (sample, gradient, exchange over peer memory, clip + Adam + target copy,
@@ -1159,8 +1140,6 @@ class RainbowKernelOps(object):
                                             hp["eps"], hp["gamma_n"], step, hp["lr"], hp["adam_eps"], hp["grad_clip"],
                                             int(copy_target), _p(self.scratch), _p(self.stats), self._stream())
         self._check(rc, "r4_rainbow_train_step")
-        self.launches += 5 if rb.prio is not None else 4
-        self.launches += 1 if comm is not None else 0
 
 
 class RainbowTrainer(DDPGTrainer):
