@@ -89,8 +89,8 @@ typedef struct {
   int32_t* cat;          /* i32 [B,21]    category_feature of the new state (datautil.py:59-65) */
   float*   dense;        /* f32 [B,432]   dense_feature (datautil.py:52-58) */
   int32_t* seq;          /* i32 [B,2,64]  sequence_feature (datautil.py:43-47) */
-  float*   click_p;      /* f32 [B,9]     probs[:,1] of the reward pass (slate.py:298-301); written
-                                          only on steps that compute a reward */
+  float*   click_p;      /* f32 [B,R]     probs[:,1] of the reward pass (slate.py:298-301), R = 9 (SeqSlate) or
+                                          max_steps (Slate) rows per env; written only on steps that compute a reward */
   int32_t* masked_actions; /* i32 [B,9|max_steps] d3rl 'masked_actions' (slate.py:98-104, seqslate.py:18-23) */
 } r4_out;
 
@@ -131,7 +131,12 @@ int r4_reset(r4_env* env, const int32_t* row_idx, const r4_out* out, void* strea
 int r4_step(r4_env* env, const void* action, int action_is_f64, const r4_out* out, void* stream);
 
 /* SlateState.offline_action / offline_reward (slate.py:149-174, seqslate.py:71-86).
- * items: i32[B]; emb (conti mode, may be NULL): f64[B,emb_dim]; reward: f64[B]. */
+ * items: i32[B]; emb (conti mode, may be NULL): f64[B,emb_dim]; reward: f64[B].
+ * An env longer than its log rows (n_slots of r4_load_log) has no logged slot to give where the reference raises:
+ * r4_offline_action returns R4_ERR_STATE at cur_steps >= n_slots while cur_steps < max_steps (the record split's
+ * IndexError, slate.py:156), r4_offline_reward at a SeqSlate page end cur_steps > n_slots (the (B, 9) x (B, 0)
+ * broadcast, seqslate.py:77-85).  At cur_steps == max_steps offline_action is item 0, and the Slate offline_reward after
+ * the last step sums every logged slot, whatever max_steps is. */
 int r4_offline_action(r4_env* env, int32_t* items, double* emb, void* stream);
 int r4_offline_reward(r4_env* env, double* reward, void* stream);
 

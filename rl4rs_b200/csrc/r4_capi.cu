@@ -921,6 +921,9 @@ int r4_step(r4_env* e, const void* action, int action_is_f64, const r4_out* out,
 int r4_offline_action(r4_env* e, int32_t* items, double* emb, void* stream) {
   if (!e || (!items && !emb)) return fail(e, R4_ERR_ARG, "r4_offline_action: null argument");
   if (!e->has_reset) return fail(e, R4_ERR_STATE, "r4_offline_action: reset first");
+  if (e->cur_steps < e->T && e->cur_steps >= e->log_slots)      // the reference's record split raises IndexError (slate.py:156)
+    return fail(e, R4_ERR_STATE, "r4_offline_action: step " + std::to_string(e->cur_steps) + " is past the " +
+                                 std::to_string(e->log_slots) + " logged slots of the log rows");
   R4_CUDA(e, cudaSetDevice(e->device));
   k_offline_action<<<(e->B + 3) / 4, 128, 0, S(stream)>>>(e->B, e->log_slots, e->cur_steps, e->T, e->emb_dim,
                                                          e->row_idx, e->log_items, e->action_emb, items, emb);
@@ -934,9 +937,14 @@ int r4_offline_reward(r4_env* e, double* reward, void* stream) {
   R4_CUDA(e, cudaSetDevice(e->device));
   int c = e->cur_steps, lo = 0, hi = 0;
   if (e->seq) {                       // seqslate.py:71-86 (hard-coded 9 at :74)
-    if (c % 9 == 0 && c > 0) { lo = c - e->P; hi = c; }
+    if (c % 9 == 0 && c > 0) {
+      // a page end past the log: the reference multiplies (B, 9) prices by (B, 0) labels and raises ValueError (:77-85)
+      if (c > e->log_slots)
+        return fail(e, R4_ERR_STATE, "r4_offline_reward: page end " + std::to_string(c) + " is past the " +
+                                     std::to_string(e->log_slots) + " logged slots of the log rows");
+      lo = c - e->P; hi = c;
+    }
   } else if (c >= e->T) { lo = 0; hi = e->log_slots; }   // slate.py:164-174: every logged slot
-  if (hi > e->log_slots) hi = e->log_slots;
   k_offline_reward<<<(e->B + 127) / 128, 128, 0, S(stream)>>>(e->B, e->log_slots, lo, hi, e->row_idx, e->log_items,
                                                               e->log_fb, e->price, reward);
   R4_LAUNCH_CHECK(e, "k_offline_reward");

@@ -89,9 +89,13 @@ class Engine(object):
 
     def _load_weights(self, weights):
         for name, arr in weights.items():
-            a = np.ascontiguousarray(arr, dtype=np.float32)
-            shape = (C.c_int64 * a.ndim)(*a.shape)
-            rc = self.lib.r4_load_weight(self.h, name.encode(), a.ctypes.data, shape, a.ndim)
+            if isinstance(arr, torch.Tensor):        # host or device tensor: r4_load_weight reads either pointer
+                a = arr.detach().to(torch.float32).contiguous()
+                shape, ptr = (C.c_int64 * a.dim())(*a.shape), a.data_ptr()
+            else:
+                a = np.ascontiguousarray(arr, dtype=np.float32)
+                shape, ptr = (C.c_int64 * a.ndim)(*a.shape), a.ctypes.data
+            rc = self.lib.r4_load_weight(self.h, name.encode(), ptr, shape, len(shape))
             _capi.check(self.lib, self.h, rc, "r4_load_weight(%s)" % name)
         rc = self.lib.r4_finalize_weights(self.h, self._sp())
         _capi.check(self.lib, self.h, rc, "r4_finalize_weights")
@@ -131,7 +135,8 @@ class Engine(object):
         self.cat = z((B, int(c.get("category_feature_num", 21))), torch.int32) if self.raw else None
         self.dense = z((B, int(c.get("dense_feature_num", 432))), torch.float32) if self.raw else None
         self.seqf = z((B, int(c.get("seq_num", 2)), int(c.get("maxlen", 64))), torch.int32) if self.raw else None
-        self.click_p = z((B, self.P), torch.float32) if self.info_fetch else None
+        # one click probability per reward row: a page (SeqSlate) or the whole slate of max_steps items (Slate)
+        self.click_p = z((B, self.P if self.seq else self.T), torch.float32) if self.info_fetch else None
         self.masked = z((B, self.P if self.seq else self.T), torch.int32) if self.d3rl else None
         self.out = _capi.R4Out(
             obs=_ptr(self.obs), action_mask=_ptr(self.mask), reward=_ptr(self.reward), done=None,

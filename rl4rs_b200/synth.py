@@ -126,7 +126,8 @@ def _page_items(rs, n, catalog):
     for k, (lo, hi) in enumerate(bounds):
         keys = rs.random_sample((n, hi - lo + 1))
         keys[:, is_sp[lo:hi + 1]] += 2.0                     # non-special ids sort first
-        out[:, 3 * k:3 * k + 3] = np.argsort(keys, axis=1)[:, :3] + lo
+        pick = np.argsort(keys, axis=1)[:, :3]
+        out[:, 3 * k:3 * k + 3] = pick[:, np.arange(3) % pick.shape[1]] + lo    # a layer of 1-2 ids repeats them
     # half of the pages carry exactly one special item, in a random slot of the matching layer
     with_sp = rs.random_sample(n) < 0.5
     slot = rs.randint(0, 9, n)

@@ -40,6 +40,41 @@ def test_create_rejects_bad_config_without_gpu_work():
     assert b"maxlen=64" in lib.r4_last_error(None)
 
 
+R4_ERR_ARG = -1                     # include/rl4rs_b200.h
+
+
+def test_create_admits_exactly_the_range_the_env_grid_spans():
+    """r4_create checks the config before it touches a device: R4_ERR_ARG on the outer side of each edge the GPU grid
+    (tests/test_gpu_env_shapes.py) is built from, anything else on the inner side (0 with a device, R4_ERR_CUDA without)."""
+    import ctypes as C
+    from test_gpu_env_shapes import A_MIN, A_MAX, SLATE_T_MIN, SLATE_T_MAX, SEQ_T_STEP
+    from test_oracle_vs_reference_random import SHAPE_SCENARIOS
+    lib = _capi.load_library()
+
+    def rc(seq=False, T=9, A=284, H=5000):
+        cfg = _capi.R4Config(env_kind=_capi.ENV_SEQSLATE if seq else _capi.ENV_SLATE, flags=0, batch_size=2, max_steps=T,
+                             page_items=9, action_size=A, action_emb_size=32, maxlen=64, seq_num=2, dense_feature_num=432,
+                             category_feature_num=21, category_hash_size=H, emb_size=128, hidden_units=128,
+                             max_rows_per_pass=0, simulator=_capi.SIMULATORS["dnn"])
+        h = C.c_void_p()
+        r = lib.r4_create(C.byref(cfg), 0, C.byref(h))
+        if h.value:
+            lib.r4_destroy(h)
+        return r
+
+    for outside, inside in (({"A": A_MIN - 1}, {"A": A_MIN}), ({"A": A_MAX + 1}, {"A": A_MAX}),
+                            ({"T": SLATE_T_MIN - 1}, {"T": SLATE_T_MIN}), ({"T": SLATE_T_MAX + 1}, {"T": SLATE_T_MAX}),
+                            ({"seq": True, "T": 2 * SEQ_T_STEP - 1}, {"seq": True, "T": 2 * SEQ_T_STEP}),
+                            ({"A": 300, "H": 299}, {"A": 300, "H": 300})):
+        assert rc(**outside) == R4_ERR_ARG, outside
+        assert rc(**inside) != R4_ERR_ARG, (inside, lib.r4_last_error(None))
+    # the stored scenarios reach both ends of each range
+    assert {s["A"] for s in SHAPE_SCENARIOS} >= {A_MIN, A_MAX}
+    assert {s["T"] for s in SHAPE_SCENARIOS if not s["seq"]} >= {SLATE_T_MIN, SLATE_T_MAX}
+    assert all(s["T"] % SEQ_T_STEP == 0 for s in SHAPE_SCENARIOS if s["seq"])
+    assert any(s.get("H") == s["A"] for s in SHAPE_SCENARIOS)
+
+
 def test_no_cpu_fallback():
     """Constructing an env without a CUDA device must fail loudly, not fall back."""
     import torch

@@ -264,17 +264,19 @@ def test_full_batch_properties():
 
 def test_row_chunking_is_invisible():
     """max_rows_per_pass bounds the simulator rows per launch group (obs and reward passes are chunked);
-    results must not depend on it.  B=48 with 40-row chunks: ragged obs chunks (40 + 8) and 4-env reward chunks."""
-    B = 48
-    cfg, cat, log, w = _synthetic(B, False, support_rllib_mask=True, simulator_info_fetch=True)
-    runs = []
-    for mr in (0, 40):
-        env = make_env(dict(cfg, max_rows_per_pass=mr), False, cat, log, w, output_format="numpy")
-        o = env.reset(reset_file=True)
-        tr = [o["obs"].copy()]
-        for t in range(9):
-            o, rew, _, info = env.step(env.offline_action)
-            tr.append(o["obs"].copy())
-        runs.append((np.stack(tr), np.asarray(rew), info["click_p"].copy()))
-    for a, b in zip(runs[0], runs[1]):
-        np.testing.assert_array_equal(a, b)
+    results must not depend on it.  40-row chunks: ragged obs chunks (40 + 8 / 40 + 7); reward chunks of 4 envs (Slate 9,
+    SeqSlate pages), and of 3 envs with a ragged last chunk of 2 at Slate 11."""
+    for seq, T, B in ((False, 9, 48), (False, 11, 47), (True, 81, 47)):
+        cfg, cat, log, w = _synthetic(B, seq, pages=-(-T // 9), support_rllib_mask=True, simulator_info_fetch=True,
+                                      max_steps=T)
+        runs = []
+        for mr in (0, 40):
+            env = make_env(dict(cfg, max_rows_per_pass=mr), seq, cat, log, w, output_format="numpy")
+            o = env.reset(reset_file=True)
+            tr = [o["obs"].copy()]
+            for t in range(T):
+                o, rew, _, info = env.step(env.offline_action)
+                tr.append(o["obs"].copy())
+            runs.append((np.stack(tr), np.asarray(rew), info["click_p"].copy()))
+        for what, a, b in zip(("obs", "reward", "click_p"), runs[0], runs[1]):
+            np.testing.assert_array_equal(a, b, err_msg="%s, %s %d, B=%d" % (what, "SeqSlate" if seq else "Slate", T, B))

@@ -35,7 +35,8 @@ def _default_regime(B, seq, n_log=None, **flags):
     from rl4rs_b200 import synth
     cfg = _cfg(B, seq, **flags)
     cat = synth.make_catalog()
-    log = synth.make_log(n_log or 4 * B, pages=4 if seq else 1, catalog=cat, hash_size=100000, corrupt_frac=0.1)
+    pages = max(4 if seq else 1, -(-cfg["max_steps"] // 9))          # a logged slot at every step
+    log = synth.make_log(n_log or 4 * B, pages=pages, catalog=cat, hash_size=100000, corrupt_frac=0.1)
     return cfg, cat, log, synth.make_weights(cfg)
 
 
@@ -249,17 +250,19 @@ def test_augru_kernels_agree_bit_patterns_under_load():
     assert_close_rel(outs[0], base, what="pair vs ping-pong kernel")
 
 
-@pytest.mark.parametrize("kind", ["slate", "seqslate27"])
+@pytest.mark.parametrize("kind", ["slate", "seqslate27", "slate11", "seqslate81"])
 def test_pay_step_observation_comes_from_the_reward_pass(kind):
     """A paying step's state is the last complete state of its page (slate.py:203-213 vs :117-131, seqslate.py:104-122 vs
     :27-50), so r4_step takes that step's observation from its reward pass instead of launching a second pass over the
     same feature rows (r4_set_option('pay_obs_reuse', 1), the default).  A/B against the separate observation pass:
     same rewards, masks and observations (different AUGRU kernel / tile shapes: fp32 rounding only), and the option
-    does change the launch count."""
+    does change the launch count.  At Slate 11 the observation is row 10 of 11 reward rows per env; at SeqSlate 81 the
+    reward pass reads the page cache of up to 64 of 72 previous items."""
     from rl4rs_b200 import _capi
-    seq = kind == "seqslate27"
+    seq = kind.startswith("seq")
+    T = {"slate": 9, "seqslate27": 27, "slate11": 11, "seqslate81": 81}[kind]
     B = 48
-    cfg, cat, log, w = _default_regime(B, seq, support_rllib_mask=True)
+    cfg, cat, log, w = _default_regime(B, seq, support_rllib_mask=True, max_steps=T)
     runs = {}
     try:
         for reuse in (1, 0):
@@ -282,5 +285,7 @@ def test_pay_step_observation_comes_from_the_reward_pass(kind):
         assert_close_rel(o1, o0, what="%s pay-step reuse obs step %d" % (kind, t))
         assert_close_rel(r1, r0, what="%s pay-step reuse reward step %d" % (kind, t))
         paid += int((r0 != 0).any())
-    assert paid >= 1                            # (a page of 48 random-replaced slates can be all violations: reward 0)
+    # (a page of 48 random-replaced slates can be all violations: reward 0; a Slate of 11 always violates, since steps 9
+    # and 10 may only hold item 0)
+    assert paid >= 1 or kind == "slate11"
     assert runs[1][1] < runs[0][1], (runs[1][1], runs[0][1])        # one observation pass fewer per paying step

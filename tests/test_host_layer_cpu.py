@@ -35,11 +35,12 @@ def obs_arrays(obs):
 
 
 def host(x):
-    return x.numpy() if hasattr(x, "is_cuda") else np.asarray(x)
+    return x.cpu().numpy() if hasattr(x, "is_cuda") else np.asarray(x)
 
 
-def replay_through_host_layer(env, cfg, a, n_episodes, name, fmt):
-    """Replay recorded actions through the product's env classes and hold what they hand out to the record."""
+def replay_through_host_layer(env, cfg, a, n_episodes, name, fmt, floor_rewards=False):
+    """Replay recorded actions through the product's env classes and hold what they hand out to the record.
+    floor_rewards: a step's rewards are bounded like an observation row, 1e-4 of max(|ref|, rms of the step's rewards)."""
     def arrays(obs):
         if fmt == "torch" and not isinstance(obs, dict):
             obs = {"obs": host(obs)}
@@ -68,7 +69,9 @@ def replay_through_host_layer(env, cfg, a, n_episodes, name, fmt):
                     assert_close_rel(val, ref, what="host %s obs step %d" % (name, k))
                 else:
                     np.testing.assert_array_equal(val, ref, err_msg="%s step %d" % (key, k))
-            assert_close_rel(np.asarray(host(reward), dtype=np.float64), a["reward"][k], what="host %s reward step %d" % (name, k))
+            rew = np.asarray(host(reward), dtype=np.float64).reshape(-1)
+            assert_close_rel(rew[None] if floor_rewards else rew, a["reward"][k][None] if floor_rewards else a["reward"][k],
+                             what="host %s reward step %d" % (name, k))
             assert_close_rel(np.asarray(host(env.offline_reward), dtype=np.float64), a["offline_reward"][k], rtol=1e-12,
                              what="host offline_reward")
             if "click_p" in a and t == T - 1:

@@ -72,38 +72,103 @@ def action_source(cfg, seed):
     return pick
 
 
-@pytest.mark.parametrize("seed", range(32))
-def test_oracle_env_equals_the_reference_env_on_a_random_scenario(seed):
+# The configuration edges r4_create admits, as a fixed list rather than a draw, so every value is covered by construction:
+# action_size 149 (layer 2 holds item 148 alone), 150, 160, 255-257, 288 and 511 / 512 (the last and the 16th mask word,
+# full or partial), Slate lengths 3-11 (post-padded and post-truncated feature rows, layer 3 at steps 9 and 10), SeqSlate
+# 9 to 81 (more than 64 previous items, Q9 walking pages 4-8), and category_hash_size == action_size.  The log carries
+# ceil(T / 9) pages, so the reference finds a logged slot at every step.  A Slate slate of 11 always violates (steps 9 and
+# 10 may only hold item 0, and twice in a row is a repeat), so there the reward pass is held to the record by click_p.
+SHAPE_SCENARIOS = [
+    dict(A=149, seq=False, T=10, B=3, mode="rllib", conti=True),
+    dict(A=150, seq=False, T=3, B=2, mode="plain", H=150),
+    dict(A=160, seq=False, T=4, B=5, mode="d3rl", info=True),
+    dict(A=255, seq=False, T=5, B=4, mode="rllib", raw=True, train=True),
+    dict(A=256, seq=False, T=8, B=3, mode="both", conti=True, info=True),
+    dict(A=257, seq=False, T=11, B=4, mode="rllib", info=True),
+    dict(A=288, seq=False, T=11, B=2, mode="d3rl", conti=True),
+    dict(A=511, seq=False, T=10, B=5, mode="plain", info=True, train=True),
+    dict(A=512, seq=False, T=8, B=3, mode="rllib", conti=True, onehot=True),
+    dict(A=256, seq=False, T=3, B=2, mode="rllib", raw=True, info=True, H=256),
+    dict(A=288, seq=True, T=9, B=2, mode="rllib", conti=True, info=True),
+    dict(A=511, seq=True, T=18, B=5, mode="d3rl", info=True),
+    dict(A=160, seq=True, T=45, B=3, mode="plain", raw=True),
+    dict(A=512, seq=True, T=45, B=3, mode="rllib", conti=True, onehot=True),
+    dict(A=512, seq=True, T=81, B=2, mode="plain", info=True, train=True),
+    dict(A=149, seq=True, T=81, B=4, mode="both", conti=True),
+]
+
+
+def shape_scenario(i):
+    s = dict({"H": 5000, "conti": False, "onehot": False, "raw": False, "info": False, "train": False}, **SHAPE_SCENARIOS[i])
+    B = s["B"]
+    cfg = {"epoch": 1, "maxlen": 64, "action_size": s["A"], "class_num": 2, "dense_feature_num": 432,
+           "category_feature_num": 21, "category_hash_size": s["H"], "seq_num": 2, "emb_size": 128, "page_items": 9,
+           "hidden_units": 128, "action_emb_size": 32, "batch_size": B, "algo": "dnn", "max_steps": s["T"],
+           "is_eval": not s["train"], "cache_size": 2 * B if s["train"] else B}
+    for key, on in (("support_rllib_mask", s["mode"] in ("rllib", "both")), ("support_d3rl_mask", s["mode"] in ("d3rl", "both")),
+                    ("support_conti_env", s["conti"]), ("support_onehot_action", s["onehot"]),
+                    ("rawstate_as_obs", s["raw"]), ("simulator_info_fetch", s["info"])):
+        if on:
+            cfg[key] = True
+    episodes = 2 if s["T"] <= 18 else 1
+    return cfg, s["seq"], 2 * cfg["cache_size"] + 1, episodes, 3000 + i, (300 + i if s["train"] else None)
+
+
+def scenario(kind, i):
+    """Inputs of random_scenario_NN / shape_scenario_NN and what the reference's own env computed on them:
+    (cfg, seq, catalog, records, dnn weights, episodes, numpy seed of the sampler or None, record)."""
     import make_golden
-    from test_oracle_golden import check_oracle_against_record
-    cfg, seq, n_rows, episodes, aseed, train_mode = draw_scenario(seed)
-    cat = synth.make_catalog()
-    log = synth.make_log(n_rows, pages=4 if seq else 1, catalog=cat, hash_size=5000, corrupt_frac=0.25, keep_hist=True,
-                         seed=synth.LOG_SEED + seed)
+    if kind == "random":
+        cfg, seq, n_rows, episodes, aseed, train_mode = draw_scenario(i)
+        cat = synth.make_catalog()
+        log = synth.make_log(n_rows, pages=4 if seq else 1, catalog=cat, hash_size=5000, corrupt_frac=0.25, keep_hist=True,
+                             seed=synth.LOG_SEED + i)
+        np_seed = 77 + i if train_mode else None
+        w = synth.make_dnn_weights(cfg, stress=2.0, bias_noise=0.2)
+    else:
+        cfg, seq, n_rows, episodes, aseed, np_seed = shape_scenario(i)
+        cat = synth.make_catalog(n_items=cfg["action_size"] - 1)
+        log = synth.make_log(n_rows, pages=-(-cfg["max_steps"] // 9), catalog=cat, hash_size=cfg["category_hash_size"],
+                             corrupt_frac=0.25, keep_hist=True, seed=synth.LOG_SEED + 100 + i)
+        w = synth.make_dnn_weights(cfg, stress=1.0, bias_noise=0.2)     # the env's edges are under test, not the network's
     records = synth.render_records(log, cat)
-    w = synth.make_dnn_weights(cfg, stress=2.0, bias_noise=0.2)
-    np_seed = 77 + seed if train_mode else None
-    rec = reference_result("random_scenario_%02d" % seed, lambda: make_golden.run_reference(
+    rec = reference_result("%s_scenario_%02d" % (kind, i), lambda: make_golden.run_reference(
         dict(cfg), records, cat.to_text(), w, seq, action_source(cfg, aseed), n_episodes=episodes, seed=np_seed,
         net=DnnOracle(w, np.float32)))
+    return cfg, seq, cat, records, w, episodes, np_seed, rec
+
+
+def check_scenario(kind, i, fmt):
+    """The oracle env, then the product's own env classes (gym layer, sampler, obs / reward formatting) over the engine
+    stand-in, against the stored reference record of one scenario."""
+    from test_oracle_golden import check_oracle_against_record
+    cfg, seq, cat, records, w, episodes, np_seed, rec = scenario(kind, i)
     if np_seed is not None:
         np.random.seed(np_seed)
     env = OracleEnv(dict(cfg), FeatureUtil.parse_log(records, 64), cat, DnnOracle(w, np.float32), seq=seq)
-    check_oracle_against_record(env, cfg, rec, episodes, "random scenario %d" % seed)
-    # ... and the product's own env classes (gym layer, sampler, obs / reward formatting) over the engine stand-in
+    check_oracle_against_record(env, cfg, rec, episodes, "%s scenario %d" % (kind, i))
     import rl4rs_b200.engine as engine_mod
     from oracle_engine import OracleEngine
     from test_host_layer_cpu import make_env, replay_through_host_layer
     real = engine_mod.Engine
     engine_mod.Engine = OracleEngine
     try:
-        fmt = ("list", "numpy", "torch")[seed % 3]
         if np_seed is not None:
             np.random.seed(np_seed)
         host_env = make_env(dict(cfg), seq, cat, FeatureUtil.parse_log(records, 64), w, output_format=fmt)
-        replay_through_host_layer(host_env, cfg, rec, episodes, "random scenario %d (host layer, %s)" % (seed, fmt), fmt)
+        replay_through_host_layer(host_env, cfg, rec, episodes, "%s scenario %d (host layer, %s)" % (kind, i, fmt), fmt)
     finally:
         engine_mod.Engine = real
+
+
+@pytest.mark.parametrize("seed", range(32))
+def test_oracle_env_equals_the_reference_env_on_a_random_scenario(seed):
+    check_scenario("random", seed, ("list", "numpy", "torch")[seed % 3])
+
+
+@pytest.mark.parametrize("idx", range(len(SHAPE_SCENARIOS)))
+def test_oracle_env_equals_the_reference_env_on_a_shape_scenario(idx):
+    check_scenario("shape", idx, ("list", "numpy", "torch")[idx % 3])
 
 
 @pytest.mark.parametrize("seed", range(8))
