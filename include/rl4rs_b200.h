@@ -309,6 +309,44 @@ int r4_gauss_ppo_epoch_dist(r4_comm* comm, float* params, const float* obs, cons
                             float kl_coeff, float ent_coeff, float* scratch, float* flat_grad, float* stats_accum, float* m,
                             float* v, int step0, float lr, float beta1, float beta2, float eps, void* stream);
 
+/* ---- IMPALA (modelfree_train.py:345-390; RLlib 1.5 vtrace_torch_policy.py) over either policy ----------------------------
+ * A rollout is B complete episodes of T steps (1..81), time-major: element [t * B + b] of every f32 [T, B] buffer; done at
+ * T - 1 only.  Stateless, caller-owned DEVICE memory. */
+/* The forward at stored actions (no sampling): obs f32[n,256], mask u8[n,A], action i64[n] -> logp f32[n] of the action
+ * under params, value f32[n].  Equal, bit for bit, to what r4_policy_act wrote for its own sample on the same params. */
+int r4_policy_eval(const float* params, const float* obs, const uint8_t* mask, const int64_t* action, int n, int action_size,
+                   float* logp, float* value, void* stream);
+/* The same for the Gaussian policy: action f32[n,D] (the unclipped sample r4_gauss_act stored). */
+int r4_gauss_eval(const float* params, const float* obs, const float* action, int n, int action_dim, float* logp, float* value,
+                  void* stream);
+/* V-trace (vtrace.from_importance_weights), one thread per episode: rho = exp(target_logp - behaviour_logp), c = min(1, rho),
+ * vs_t - V_t = min(rho_bar, rho_t) (r_t + g_t V_{t+1} - V_t) + g_t c_t (vs_{t+1} - V_{t+1}),
+ * pg_adv_t = min(rho_pg_bar, rho_t) (r_t + g_t vs_{t+1} - V_t), g_t = gamma (0 at t = T - 1).  drop_last != 0 (RLlib 1.5): steps
+ * 0..T-2 with the bootstrap V(s_{T-1}) = value[T-1], and vs[T-1] = value[T-1], pg_adv[T-1] = 0; drop_last = 0: every step,
+ * bootstrap 0.  T 2..81 with drop_last, gamma in [0, 1], thresholds > 0.  Deterministic. */
+int r4_vtrace(const float* behaviour_logp, const float* target_logp, const float* value, const float* reward, int T, int B,
+              float gamma, float rho_bar, float rho_pg_bar, int drop_last, float* vs, float* pg_adv, void* stream);
+/* One IMPALA learner step of the mask policy, with no host round trip: r4_policy_eval over all T * B rows (-> logp, value),
+ * r4_vtrace (behaviour_logp = the logp r4_policy_act stored; -> vs, pg_adv), the A2C-mode gradient of r4_policy_grad with
+ * adv = pg_adv and target = vs over the kept rows (the first T - 1 time steps with drop_last, else all), the exchange over
+ * peer memory (comm; NULL = one GPU: the loss is summed over the global batch), the global-norm clip (grad_clip <= 0: off;
+ * norm_scratch f32[1]; the norm is summed in a fixed order) and Adam (step is 1-based).  logits = the stored masked logits
+ * (the KL statistic).  scratch: f32[G * (num_params + 5)], G = min(ceil(kept rows / 4), the device's SM count).
+ * stats_accum f32[5] += the sums {policy_loss, vf_loss, kl, entropy, total}. */
+int r4_impala_step(r4_comm* comm, float* params, const float* obs, const uint8_t* mask, const int64_t* action,
+                   const float* behaviour_logp, const float* logits, const float* reward, int T, int B, int action_size,
+                   float gamma, float rho_bar, float rho_pg_bar, int drop_last, float vf_coeff, float ent_coeff, float* logp,
+                   float* value, float* vs, float* pg_adv, float* scratch, float* flat_grad, float* stats_accum, float* m,
+                   float* v, int step, float lr, float beta1, float beta2, float eps, float grad_clip, float* norm_scratch,
+                   void* stream);
+/* r4_impala_step for the Gaussian policy over r4_gauss_eval and r4_gauss_grad (mode 1); scratch: r4_gauss_scratch_size(D)
+ * floats; kl is reported as 0. */
+int r4_gauss_impala_step(r4_comm* comm, float* params, const float* obs, const float* action, const float* behaviour_logp,
+                         const float* reward, int T, int B, int action_dim, float gamma, float rho_bar, float rho_pg_bar,
+                         int drop_last, float vf_coeff, float ent_coeff, float* logp, float* value, float* vs, float* pg_adv,
+                         float* scratch, float* flat_grad, float* stats_accum, float* m, float* v, int step, float lr,
+                         float beta1, float beta2, float eps, float grad_clip, float* norm_scratch, void* stream);
+
 /* ---- DDPG / TD3 on the continuous-action env (modelfree_train.py:46-48,79-105; modelfree_trainer.py:25-28; RLlib 1.5
  * ddpg / td3 defaults, INTEGRATION.md section 3): a deterministic actor obs(256) -> 400 relu -> 300 relu -> D, squashed
  * to Box(-1, 1) as tanh, and a critic concat(obs, a) -> 400 relu -> 300 relu -> 1 (TD3: plus a twin critic), action_dim
@@ -535,7 +573,7 @@ int r4_simtrain_eval(int hash_size, const float* params, const r4_simtrain_data*
 /* kernels launched so far by the r4_simtrain_* entry points in this process (the radix sort counted once) */
 int64_t r4_simtrain_launch_count(void);
 /* kernels launched so far by every learner entry point in this process (r4_policy_*, r4_gae, r4_adam_step, r4_ppo_epoch*,
- * r4_grad_exchange*, r4_gauss_*, r4_ddpg_*, r4_replay_*, r4_rainbow_*, r4_batchrl_*, r4_simtrain_*): the sum of the batch
+ * r4_grad_exchange*, r4_gauss_*, r4_vtrace, r4_impala_step, r4_ddpg_*, r4_replay_*, r4_rainbow_*, r4_batchrl_*, r4_simtrain_*): the sum of the batch
  * RL and simulator-trainer counts above and the online learners'. */
 int64_t r4_learner_launch_count(void);
 

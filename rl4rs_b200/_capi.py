@@ -94,6 +94,13 @@ EXPORTS = {
                            [C.c_float] * 5 + [C.c_void_p, C.c_void_p]),
     "r4_gauss_ppo_epoch_dist": (C.c_int, [C.c_void_p] * 10 + [C.c_int] * 3 + [C.c_float] * 5 + [C.c_void_p] * 5 + [C.c_int] +
                                 [C.c_float] * 4 + [C.c_void_p]),
+    "r4_policy_eval": (C.c_int, [C.c_void_p] * 4 + [C.c_int, C.c_int] + [C.c_void_p] * 3),
+    "r4_gauss_eval": (C.c_int, [C.c_void_p] * 3 + [C.c_int, C.c_int] + [C.c_void_p] * 3),
+    "r4_vtrace": (C.c_int, [C.c_void_p] * 4 + [C.c_int, C.c_int] + [C.c_float] * 3 + [C.c_int] + [C.c_void_p] * 3),
+    "r4_impala_step": (C.c_int, [C.c_void_p] * 8 + [C.c_int] * 3 + [C.c_float] * 3 + [C.c_int] + [C.c_float] * 2 +
+                       [C.c_void_p] * 9 + [C.c_int] + [C.c_float] * 5 + [C.c_void_p] * 2),
+    "r4_gauss_impala_step": (C.c_int, [C.c_void_p] * 6 + [C.c_int] * 3 + [C.c_float] * 3 + [C.c_int] + [C.c_float] * 2 +
+                             [C.c_void_p] * 9 + [C.c_int] + [C.c_float] * 5 + [C.c_void_p] * 2),
     "r4_ddpg_num_params": (C.c_int, [C.c_int, C.c_int]),
     "r4_ddpg_scratch_size": (C.c_int64, [C.c_int, C.c_int, C.c_int]),
     "r4_ddpg_act": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p] +

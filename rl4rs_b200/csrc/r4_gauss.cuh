@@ -168,6 +168,33 @@ __global__ void __launch_bounds__(NT) k_gauss_act(Layout L, const float* __restr
   }
 }
 
+// IMPALA's learner forward at the stored (unclipped) actions -> logp, value for rows 0..n-1: k_gauss_act's log-likelihood
+// in its order, so on the parameters that acted logp equals the stored logp bit for bit.
+__global__ void __launch_bounds__(NT) k_gauss_eval(Layout L, const float* __restrict__ prm, const float* __restrict__ obs,
+                                                   const float* __restrict__ action, int n, float* __restrict__ logp,
+                                                   float* __restrict__ value) {
+  extern __shared__ __align__(16) float sm[];
+  float *x = sm, *h1 = x + TS * H, *h2 = h1 + TS * H, *g1 = h2 + TS * H, *g2 = g1 + TS * H;
+  float *o = g2 + TS * H, *val = o + TS * 2 * MAXD;
+  __shared__ int64_t src[TS];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, D = L.D;
+  const int s0 = blockIdx.x * TS, nvalid = min(TS, n - s0);
+  if (tid < TS) src[tid] = min(s0 + tid, n - 1);
+  __syncthreads();
+  forward_rows(L, prm, obs, src, nvalid, x, h1, h2, g1, g2, o, val);
+  for (int s = warp; s < nvalid; s += NT / 32) {
+    const int64_t row = s0 + s;
+    float q = 0.f, sls = 0.f;
+    for (int i = lane; i < D; i += 32) {
+      const float mu = o[s * 2 * D + i], ls = o[s * 2 * D + D + i];
+      const float z = (__ldg(action + row * D + i) - mu) / expf(ls);
+      q = fmaf(z, z, q); sls += ls;
+    }
+    q = r4ppo::warp_sum(q); sls = r4ppo::warp_sum(sls);
+    if (lane == 0) { logp[row] = -0.5f * q - sls - HALF_LOG_2PI * D; value[row] = val[s]; }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // gradient, part 1: per-sample rows.  Positions p = c0 .. c0+cn of the sample list (idx[p], or p when idx == nullptr);
 // row q = p - c0 of every plane.  mode 0 = PPO (loss mean: inv_n), mode 1 = A2C (sums).

@@ -363,6 +363,114 @@ int r4_gauss_ppo_epoch_dist(r4_comm* c, float* params, const float* obs, const f
   return steps;
 }
 
+// ---- IMPALA: forward at the stored actions, V-trace, the fused learner step (r4_ppo.cuh, r4_gauss.cuh) ----------------------------
+static bool vtrace_args_ok(int T, int B, float gamma, float rho_bar, float rho_pg_bar, int drop_last) {
+  return T >= (drop_last ? 2 : 1) && T <= r4ppo::MAXT && B >= 1 && (int64_t)T * B <= 0x7fffffff && gamma >= 0.f &&
+         gamma <= 1.f && rho_bar > 0.f && rho_pg_bar > 0.f && std::isfinite(rho_bar) && std::isfinite(rho_pg_bar);
+}
+
+static size_t policy_eval_smem(int A) {
+  return (size_t)(r4ppo::TS * r4ppo::OBS + r4ppo::TS * r4ppo::HID + r4ppo::TS * A + r4ppo::TS) * 4;
+}
+
+int r4_policy_eval(const float* params, const float* obs, const uint8_t* mask, const int64_t* action, int n, int action_size,
+                   float* logp, float* value, void* stream) {
+  if (!params || !obs || !mask || !action || !logp || !value || n < 1 || action_size < 2 || action_size > 512)
+    return fail(R4_ERR_ARG, "r4_policy_eval: bad argument");
+  return launch(FAM_ONLINE, "k_policy_eval", r4ppo::k_policy_eval, (n + r4ppo::TS - 1) / r4ppo::TS, r4ppo::NT,
+                policy_eval_smem(action_size), S(stream), false, r4ppo::make_layout(action_size), params, obs, mask, action, n,
+                logp, value);
+}
+
+int r4_gauss_eval(const float* params, const float* obs, const float* action, int n, int action_dim, float* logp, float* value,
+                  void* stream) {
+  if (!params || !obs || !action || !logp || !value || n < 1 || !gauss_dim_ok(action_dim))
+    return fail(R4_ERR_ARG, "r4_gauss_eval: bad argument (action_dim even, 2..64)");
+  return launch(FAM_ONLINE, "k_gauss_eval", r4gauss::k_gauss_eval, (n + r4gauss::TS - 1) / r4gauss::TS, r4gauss::NT,
+                r4gauss::ACT_SMEM, S(stream), false, r4gauss::make_layout(action_dim), params, obs, action, n, logp, value);
+}
+
+int r4_vtrace(const float* behaviour_logp, const float* target_logp, const float* value, const float* reward, int T, int B,
+              float gamma, float rho_bar, float rho_pg_bar, int drop_last, float* vs, float* pg_adv, void* stream) {
+  if (!behaviour_logp || !target_logp || !value || !reward || !vs || !pg_adv ||
+      !vtrace_args_ok(T, B, gamma, rho_bar, rho_pg_bar, drop_last))
+    return fail(R4_ERR_ARG, "r4_vtrace: bad argument (T 1..81, 2..81 with drop_last, gamma in [0, 1], thresholds > 0)");
+  return launch(FAM_ONLINE, "k_vtrace", r4ppo::k_vtrace, (B + 255) / 256, 256, 0, S(stream), false, T, B, behaviour_logp,
+                target_logp, value, reward, gamma, rho_bar, rho_pg_bar, (int)(drop_last != 0), vs, pg_adv);
+}
+
+// The tail of both fused IMPALA steps: (the exchange of this rank's partials over peer memory,) the global-norm clip in a
+// fixed order and Adam.
+static int impala_tail(r4_comm* comm, const float* partial, int G, int np, float* params, float* flat_grad, float* stats_accum,
+                       float* m, float* v, int step, float lr, float b1, float b2, float eps, float grad_clip,
+                       float* norm_scratch, cudaStream_t st) {
+  int rc = R4_OK;
+  if (comm && (rc = exchange_launch(comm, partial, G, np, flat_grad, stats_accum, 1.f, 0, nullptr, nullptr, nullptr, 0, 0.f, 0.f,
+                                    0.f, 0.f, st)))
+    return rc;
+  if (grad_clip > 0.f &&
+      (rc = launch(FAM_ONLINE, "k_sumsq_one", r4ppo::k_sumsq_one, 1, r4ppo::SQT, 0, st, false, np, flat_grad, norm_scratch)))
+    return rc;
+  return launch(FAM_ONLINE, "k_adam", r4ppo::k_adam, (np + 255) / 256, 256, 0, st, false, np, params, flat_grad, m, v, step, lr,
+                b1, b2, eps, 1.f, grad_clip > 0.f ? norm_scratch : nullptr, grad_clip);
+}
+
+static bool impala_comm_ok(r4_comm* comm, int np) { return !comm || (comm->ready && comm->n == np); }
+
+int r4_impala_step(r4_comm* comm, float* params, const float* obs, const uint8_t* mask, const int64_t* action,
+                   const float* behaviour_logp, const float* logits, const float* reward, int T, int B, int action_size,
+                   float gamma, float rho_bar, float rho_pg_bar, int drop_last, float vf_coeff, float ent_coeff, float* logp,
+                   float* value, float* vs, float* pg_adv, float* scratch, float* flat_grad, float* stats_accum, float* m,
+                   float* v, int step, float lr, float beta1, float beta2, float eps, float grad_clip, float* norm_scratch,
+                   void* stream) {
+  if (!params || !obs || !mask || !action || !behaviour_logp || !logits || !reward || !logp || !value || !vs || !pg_adv ||
+      !scratch || !flat_grad || !m || !v || step < 1 || (grad_clip > 0.f && !norm_scratch) || action_size < 2 ||
+      action_size > 512 || !vtrace_args_ok(T, B, gamma, rho_bar, rho_pg_bar, drop_last) ||
+      !impala_comm_ok(comm, r4ppo::make_layout(action_size).n))
+    return fail(R4_ERR_ARG, "r4_impala_step: bad argument");
+  const int n = T * B, nk = (drop_last ? T - 1 : T) * B;          // the kept rows are the first T - 1 (or T) time steps
+  const int np = r4ppo::make_layout(action_size).n;
+  const int G = std::max(1, std::min((nk + r4ppo::TS - 1) / r4ppo::TS, sm_count()));
+  cudaStream_t st = S(stream);
+  int rc = r4_policy_eval(params, obs, mask, action, n, action_size, logp, value, stream);
+  if (!rc) rc = r4_vtrace(behaviour_logp, logp, value, reward, T, B, gamma, rho_bar, rho_pg_bar, drop_last, vs, pg_adv, stream);
+  // A2C mode: -sum logp pg_adv + vf_coeff * 0.5 sum (V - vs)^2 - ent_coeff * sum H over the kept rows
+  if (!rc) rc = policy_grad_impl(1, params, obs, mask, action, nullptr, logits, nullptr, pg_adv, vs, nullptr, nk, action_size, 0.f,
+                                 0.f, vf_coeff, 0.f, ent_coeff, 1.f, scratch, G, flat_grad, stats_accum, 1.f, stream, !comm);
+  if (rc) return rc;
+  return impala_tail(comm, scratch, G, np, params, flat_grad, stats_accum, m, v, step, lr, beta1, beta2, eps, grad_clip,
+                     norm_scratch, st);
+}
+
+int r4_gauss_impala_step(r4_comm* comm, float* params, const float* obs, const float* action, const float* behaviour_logp,
+                         const float* reward, int T, int B, int action_dim, float gamma, float rho_bar, float rho_pg_bar,
+                         int drop_last, float vf_coeff, float ent_coeff, float* logp, float* value, float* vs, float* pg_adv,
+                         float* scratch, float* flat_grad, float* stats_accum, float* m, float* v, int step, float lr,
+                         float beta1, float beta2, float eps, float grad_clip, float* norm_scratch, void* stream) {
+  if (!params || !obs || !action || !behaviour_logp || !reward || !logp || !value || !vs || !pg_adv || !scratch || !flat_grad ||
+      !m || !v || step < 1 || (grad_clip > 0.f && !norm_scratch) || !gauss_dim_ok(action_dim) ||
+      !vtrace_args_ok(T, B, gamma, rho_bar, rho_pg_bar, drop_last) ||
+      !impala_comm_ok(comm, r4gauss::make_layout(action_dim).n))
+    return fail(R4_ERR_ARG, "r4_gauss_impala_step: bad argument");
+  const int n = T * B, nk = (drop_last ? T - 1 : T) * B;
+  const int np = r4gauss::make_layout(action_dim).n;
+  float* gsum = gauss_gsum(scratch, action_dim);
+  cudaStream_t st = S(stream);
+  int rc = r4_gauss_eval(params, obs, action, n, action_dim, logp, value, stream);
+  if (!rc) rc = r4_vtrace(behaviour_logp, logp, value, reward, T, B, gamma, rho_bar, rho_pg_bar, drop_last, vs, pg_adv, stream);
+  if (!rc) {
+    if (comm)      // one partial (G = 1): the gradient and its statistics, summed over the ranks by the exchange
+      rc = gauss_grad_impl(1, params, obs, action, nullptr, nullptr, nullptr, pg_adv, vs, nullptr, nk, action_dim, 0.f, 0.f,
+                           vf_coeff, 0.f, ent_coeff, 1.f, scratch, gsum, gsum + np, nullptr, 0.f, stream);
+    else
+      rc = gauss_grad_impl(1, params, obs, action, nullptr, nullptr, nullptr, pg_adv, vs, nullptr, nk, action_dim, 0.f, 0.f,
+                           vf_coeff, 0.f, ent_coeff, 1.f, scratch, flat_grad, gsum + np + 5, stats_accum, 1.f, stream);
+  }
+  if (rc) return rc;
+  return impala_tail(comm, gsum, 1, np, params, flat_grad, stats_accum, m, v, step, lr, beta1, beta2, eps, grad_clip,
+                     norm_scratch, st);
+}
+
 // ---- DDPG / TD3 (r4_ddpg.cuh) ---------------------------------------------------------------------------------
 static bool ddpg_dim_ok(int D) { return D >= 2 && D <= r4ddpg::MAXD; }
 

@@ -509,4 +509,86 @@ __global__ void k_sumsq(int n, const float* __restrict__ x, float* __restrict__ 
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// IMPALA (RLlib 1.5 vtrace_torch_policy.py): the learner forward at the stored actions, V-trace, and the clip's norm.
+// ------------------------------------------------------------------------------------------------
+constexpr int MAXT = 81;               // the longest episode the IMPALA entry points take (SeqSlate 9 pages x 9 steps)
+constexpr int SQT = 1024;              // threads of k_sumsq_one
+
+// forward_tile at the rollout's own actions -> logp(a), value for rows 0..n-1 (no sampling).  The log-softmax is
+// k_policy_act's, in its order, so on the parameters that acted logp equals the stored logp bit for bit.
+__global__ void __launch_bounds__(NT) k_policy_eval(Layout L, const float* __restrict__ prm, const float* __restrict__ obs,
+                                                    const uint8_t* __restrict__ mask, const int64_t* __restrict__ action, int n,
+                                                    float* __restrict__ logp, float* __restrict__ value) {
+  extern __shared__ __align__(16) float sm[];
+  float* obs_s = sm; float* h_s = obs_s + TS * OBS; float* lg_s = h_s + TS * HID; float* val_s = lg_s + TS * L.A;
+  __shared__ int64_t src[TS];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int s0 = blockIdx.x * TS;
+  const int nvalid = min(TS, n - s0);
+  if (tid < TS) src[tid] = min(s0 + tid, n - 1);
+  __syncthreads();
+  forward_tile<false>(L, prm, prm + L.o_w1, prm + L.o_w2, obs, mask, src, nvalid, obs_s, h_s, lg_s, val_s);
+  for (int s = warp; s < nvalid; s += NT / 32) {
+    const float* lg = lg_s + s * L.A;
+    float m = -INFINITY;
+    for (int c = lane; c < L.A; c += 32) m = fmaxf(m, lg[c]);
+    m = warp_max(m);
+    float se = 0.f;
+    for (int c = lane; c < L.A; c += 32) se += expf(lg[c] - m);
+    se = warp_sum(se);
+    if (lane == 0) {
+      const int64_t r = s0 + s;
+      logp[r] = lg[action[r]] - (m + logf(se));
+      value[r] = val_s[s];
+    }
+  }
+}
+
+// V-trace (vtrace.from_importance_weights) over complete episodes of T steps (done at T - 1 only), element [t * B + b] of
+// every buffer, one thread per episode b.  drop_last: the loss covers t < T - 1 and V(s_{T-1}) is the bootstrap value
+// (RLlib 1.5 drops the last step of the time-major batch); then vs[T-1] = V(s_{T-1}) and pg_adv[T-1] = 0.  Otherwise the
+// loss covers every step and the bootstrap is 0.
+//     rho_t = exp(target_logp - behaviour_logp), c_t = min(1, rho_t), disc_t = gamma (t < T - 1) or 0 (t = T - 1)
+//     vs_t - V_t = min(rho_bar, rho_t) (r_t + disc_t V_{t+1} - V_t) + disc_t c_t (vs_{t+1} - V_{t+1})
+//     pg_adv_t   = min(rho_pg_bar, rho_t) (r_t + disc_t vs_{t+1} - V_t)
+// Every product and sum is rounded on its own (no contraction), in the order from_importance_weights writes them.
+__global__ void k_vtrace(int T, int B, const float* __restrict__ blogp, const float* __restrict__ tlogp,
+                         const float* __restrict__ value, const float* __restrict__ reward, float gamma, float rho_bar,
+                         float rho_pg_bar, int drop_last, float* __restrict__ vs, float* __restrict__ pg_adv) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const int K = drop_last ? T - 1 : T;
+  const float boot = drop_last ? value[(size_t)(T - 1) * B + b] : 0.f;
+  if (drop_last) { vs[(size_t)(T - 1) * B + b] = boot; pg_adv[(size_t)(T - 1) * B + b] = 0.f; }
+  float acc = 0.f, v_next = boot, vs_next = boot;
+  for (int t = K - 1; t >= 0; --t) {
+    const size_t i = (size_t)t * B + b;
+    const float disc = t == T - 1 ? 0.f : gamma;
+    const float rho = expf(__fadd_rn(tlogp[i], -blogp[i]));
+    const float v = value[i], r = reward[i];
+    const float delta = __fmul_rn(fminf(rho_bar, rho), __fadd_rn(__fadd_rn(r, __fmul_rn(disc, v_next)), -v));
+    acc = __fadd_rn(delta, __fmul_rn(__fmul_rn(disc, fminf(1.f, rho)), acc));
+    const float vsi = __fadd_rn(acc, v);
+    pg_adv[i] = __fmul_rn(fminf(rho_pg_bar, rho), __fadd_rn(__fadd_rn(r, __fmul_rn(disc, vs_next)), -v));
+    vs[i] = vsi;
+    v_next = v; vs_next = vsi;
+  }
+}
+
+// out[0] = sum x_i^2 in ONE CTA and a fixed order (thread k adds i = k, k + SQT, ..., then a fixed tree over the warps):
+// k_sumsq adds its 32 CTAs' sums with atomics, whose order varies between runs, so IMPALA's clipped step uses this one.
+__global__ void __launch_bounds__(SQT) k_sumsq_one(int n, const float* __restrict__ x, float* __restrict__ out) {
+  __shared__ float red[SQT / 32];
+  float s = 0.f;
+  for (int i = threadIdx.x; i < n; i += SQT) s = fmaf(x[i], x[i], s);
+  s = warp_sum(s);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    s = warp_sum(red[threadIdx.x]);
+    if (threadIdx.x == 0) out[0] = s;
+  }
+}
+
 }  // namespace r4ppo

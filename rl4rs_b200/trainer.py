@@ -143,6 +143,34 @@ class KernelOps(object):
                                    1e-8, grad_scale, float(clip or 0.0), _p(self.norm), self._stream())
         self._check(rc, "r4_adam_step")
 
+    # ---- IMPALA ----
+    def eval(self, flat, inputs, action, logp, value):
+        """logp [n] of the stored actions and value [n] under flat, in one launch (r4_policy_eval)."""
+        rc = self.lib.r4_policy_eval(_p(flat), *map(_p, inputs), _p(action), action.shape[0], self.A, _p(logp), _p(value),
+                                     self._stream())
+        self._check(rc, "r4_policy_eval")
+
+    def vtrace(self, behaviour_logp, target_logp, value, reward, hp, vs, pg_adv):
+        """vs, pg_adv [T, B] of a rollout (r4_vtrace); hp = IMPALATrainer._hp()."""
+        T, B = reward.shape
+        rc = self.lib.r4_vtrace(_p(behaviour_logp), _p(target_logp), _p(value), _p(reward), T, B, *hp[:4], _p(vs), _p(pg_adv),
+                                self._stream())
+        self._check(rc, "r4_vtrace")
+
+    def _impala_cols(self, buf):
+        """-> (the fused step's entry point, the rollout columns it takes, the policy's size argument)."""
+        return "r4_impala_step", (buf.obs, buf.mask, buf.action, buf.logp, buf.logits, buf.reward), self.A
+
+    def impala_step(self, comm, flat, buf, hp, lr, clip, work):
+        """One IMPALA learner step in ONE library call (r4_impala_step / r4_gauss_impala_step): forward, V-trace, gradient,
+        the exchange over peer memory when comm is given, clip and Adam.  work = (logp, value, vs, pg_adv) [T, B]."""
+        fn, cols, dim = self._impala_cols(buf)
+        rc = getattr(self.lib, fn)(comm.h if comm is not None else None, _p(flat), *map(_p, cols), buf.T, buf.B, dim, *hp, *map(_p, work), _p(self.scratch), _p(self.grad), _p(self.stats), _p(self.m),
+                                   _p(self.v), self.step + 1, lr, 0.9, 0.999, 1e-8, float(clip or 0.0), _p(self.norm),
+                                   self._stream())
+        self._check(rc, fn)
+        self.step += 1
+
 
 class GaussKernelOps(KernelOps):
     """ctypes front of the Gaussian-policy kernels (include/rl4rs_b200.h: r4_gauss_*), with KernelOps's methods, so the
@@ -181,6 +209,14 @@ class GaussKernelOps(KernelOps):
     def ppo_epoch_dist(self, comm, flat, data, perm, n, mb_local, hp, lr):
         rc = self._epoch("r4_gauss_ppo_epoch_dist", (comm.h,), self.D, flat, data, perm, n, mb_local, hp, lr, ())
         return rc
+
+    def eval(self, flat, inputs, action, logp, value):
+        rc = self.lib.r4_gauss_eval(_p(flat), *map(_p, inputs), _p(action), action.shape[0], self.D, _p(logp), _p(value),
+                                    self._stream())
+        self._check(rc, "r4_gauss_eval")
+
+    def _impala_cols(self, buf):
+        return "r4_gauss_impala_step", (buf.obs, buf.action, buf.logp, buf.reward), self.D
 
     def policy_grad_exchange(self, comm, mode, flat, data, n, hp, inv_n, stat_scale):
         """One gradient over n local samples, summed over the ranks through peer memory into self.grad (A2C)."""
@@ -670,6 +706,189 @@ class GaussPPOTrainer(PPOTrainer):
 class GaussA2CTrainer(A2CTrainer):
     """A2C_conti: A2CTrainer over the DiagGaussian policy of the continuous-action env."""
     algo = "A2C_conti"
+    conti = True
+
+
+# ---- PG / IMPALA -----------------------------------------------------------------------------------------------------
+# RLlib 1.5 pg / impala defaults as modelfree_train.py:306-390 leaves them (INTEGRATION.md section 3).  IMPALA's
+# vtrace_drop_last_ts True reproduces RLlib 1.5, whose loss drops the last step of every episode (INTEGRATION.md section 3).
+PG_DEFAULTS = {"gamma": 1.0, "lr": 4e-4}
+IMPALA_DEFAULTS = {"gamma": 1.0, "lr": 1e-4, "grad_clip": 10.0, "opt_type": "adam", "vf_loss_coeff": 0.5,
+                   "entropy_coeff": 0.01, "vtrace_clip_rho_threshold": 1.0, "vtrace_clip_pg_rho_threshold": 1.0,
+                   "vtrace_drop_last_ts": True, "num_sgd_iter": 1}
+
+
+class PGTrainer(_TrainerBase):
+    """PG (RLlib 1.5 PGTrainer): one step per vector episode on -mean(logp(a) * G), G the discounted reward-to-go
+    (compute_advantages without GAE or critic); no value loss, no entropy, no clip.  On CUDA the A2C-mode gradient kernel with
+    the value and entropy coefficients at 0 over r4_gae's returns for zero values, and Adam scaled by 1 / (world * n)."""
+    algo = "PG"
+    DEFAULTS = PG_DEFAULTS
+
+    def loss(self, *args):
+        """pg_torch_policy's loss: loss(*inputs, action, returns)."""
+        *inputs, action, ret = args
+        d, _ = self.policy.forward(*inputs)
+        total = -(self.policy.terms(d, action)[0] * ret).mean()
+        return total, {"policy_loss": total}
+
+    def returns(self, buf):
+        """The discounted reward-to-go [T, B] of a rollout of complete episodes."""
+        gamma = self.config["gamma"]
+        if self.use_kernels:
+            return self.ops.gae(buf.reward, torch.zeros_like(buf.reward), gamma, 1.0)[1]
+        ret, last = torch.zeros_like(buf.reward), torch.zeros_like(buf.reward[0])
+        for t in reversed(range(buf.T)):
+            last = buf.reward[t] + gamma * last
+            ret[t] = last
+        return ret
+
+    def learn(self, buf):
+        c = self.config
+        n, w = buf.T * buf.B, _world()
+        ret = self.returns(buf).reshape(n).contiguous()
+        if self.use_kernels:
+            ops = self.ops
+            data = buf.a2c_columns() + (ret, ret)      # adv = the return; the target is unread at vf_coeff 0
+            hp = {"clip": 0.0, "vf_clip": 0.0, "vf_coeff": 0.0, "kl_coeff": 0.0, "ent_coeff": 0.0}
+            ops.stats.zero_()
+            if w > 1 and self.comm is not None and self.comm.ok:
+                ops.policy_grad_exchange(self.comm, 1, self.policy.flat, data, n, hp, 1.0, 1.0 / n)
+            else:
+                ops.policy_grad(1, self.policy.flat, data, None, 0, n, hp, 1.0, 1.0 / n)
+                if w > 1:
+                    dist.all_reduce(ops.grad, op=dist.ReduceOp.SUM)
+            ops.adam(self.policy.flat, c["lr"], 1.0 / (w * n), None)      # the summed gradient -> the global mean's
+            g = self._global_means({"policy_loss": ops.stats[0], "entropy": ops.stats[3],
+                                    "_episode_reward_mean": buf.reward.sum(0).mean()})
+            g.update({"total_loss": g["policy_loss"], "sgd_steps": 1})
+            return g
+        if self.policy.flat.grad is not None:
+            self.policy.flat.grad.zero_()
+        total, st = self.loss(*buf.columns()[:-3], ret)
+        total.backward()
+        self._allreduce_grad(average=True)          # the mean over the global batch
+        self.opt.step()
+        return {"policy_loss": self._global_mean(total), "total_loss": self._global_mean(total), "sgd_steps": 1}
+
+
+class IMPALATrainer(_TrainerBase):
+    """IMPALA (RLlib 1.5 ImpalaTrainer's learner as modelfree_train.py configures it): per vector episode, num_sgd_iter
+    steps on the V-trace loss -sum logp(a) pg_adv + 0.5 vf_coeff sum (V - vs)^2 - ent_coeff sum H over the kept steps, the
+    global batch summed, global-norm clip, Adam.  The behaviour policy mu is the logp the act kernel stored; passes after the
+    first are off-policy and V-trace corrects them.  On CUDA one library call per step (r4_impala_step), the exchange over
+    peer memory included; the torch code below is the CPU / rawstate path and the autograd cross-check."""
+    algo = "IMPALA"
+    DEFAULTS = IMPALA_DEFAULTS
+
+    def __init__(self, config, env, device=None, seed=0):
+        c = dict(self.DEFAULTS, **{k: v for k, v in (config or {}).items() if k in self.DEFAULTS})
+        if c["opt_type"] != "adam":
+            raise NotImplementedError("IMPALA opt_type %r: only 'adam' (modelfree_train.py:345-390) is built" % c["opt_type"])
+        if c["vtrace_drop_last_ts"] and env.config["max_steps"] < 2:
+            raise ValueError("IMPALA with vtrace_drop_last_ts drops the last step of every episode: max_steps = 1 leaves "
+                             "nothing to learn from (set vtrace_drop_last_ts=False)")
+        super().__init__(config, env, device, seed)
+        self._work = None
+        if self.use_kernels:            # logp, value, vs, pg_adv of the learner's forward, [T, B]
+            self._work = tuple(torch.zeros(self.T, self.B, dtype=torch.float32, device=self.device) for _ in range(4))
+
+    def _hp(self):
+        """(gamma, rho_bar, rho_pg_bar, drop_last, vf_coeff, ent_coeff) in the argument order of r4_impala_step."""
+        c = self.config
+        return (c["gamma"], c["vtrace_clip_rho_threshold"], c["vtrace_clip_pg_rho_threshold"], int(bool(c["vtrace_drop_last_ts"])),
+                c["vf_loss_coeff"], c["entropy_coeff"])
+
+    def kept(self, T):
+        """Time steps the loss covers: T - 1 with vtrace_drop_last_ts (RLlib 1.5), else T."""
+        return T - 1 if self.config["vtrace_drop_last_ts"] else T
+
+    def vtrace(self, behaviour_logp, target_logp, value, reward):
+        """vtrace.from_importance_weights over [T, B] episodes (done at T - 1), in float32 and in k_vtrace's order ->
+        (vs, pg_adv); with vtrace_drop_last_ts, bootstrapped at V(s_{T-1}) and vs[T-1] = V, pg_adv[T-1] = 0."""
+        gamma, rho_bar, rho_pg_bar, drop = self._hp()[:4]
+        T = reward.shape[0]
+        rho = torch.exp(target_logp - behaviour_logp)
+        vs, pg = value.clone(), torch.zeros_like(value)
+        boot = value[T - 1] if drop else torch.zeros_like(value[0])
+        acc, v_next, vs_next = torch.zeros_like(boot), boot, boot
+        for t in reversed(range(self.kept(T))):
+            disc = 0.0 if t == T - 1 else gamma
+            delta = torch.clamp(rho[t], max=rho_bar) * (reward[t] + disc * v_next - value[t])
+            acc = delta + disc * torch.clamp(rho[t], max=1.0) * acc
+            vs[t] = acc + value[t]
+            pg[t] = torch.clamp(rho[t], max=rho_pg_bar) * (reward[t] + disc * vs_next - value[t])
+            v_next, vs_next = value[t], vs[t]
+        return vs, pg
+
+    def loss(self, *args):
+        """RLlib 1.5 VTraceLoss, summed terms: loss(*inputs, action, behaviour_logp [T, B], reward [T, B]) over T * B rows."""
+        *inputs, action, behaviour_logp, reward = args
+        c = self.config
+        T, B = reward.shape
+        d, value = self.policy.forward(*inputs)
+        logp, _, entropy = self.policy.terms(d, action)
+        with torch.no_grad():
+            vs, pg_adv = self.vtrace(behaviour_logp, logp.detach().view(T, B), value.detach().view(T, B), reward)
+        k = self.kept(T) * B
+        pi_loss = -(logp[:k] * pg_adv.reshape(-1)[:k]).sum()
+        vf_loss = 0.5 * ((value[:k] - vs.reshape(-1)[:k]) ** 2).sum()
+        entropy = entropy[:k].sum()
+        total = pi_loss + c["vf_loss_coeff"] * vf_loss - c["entropy_coeff"] * entropy
+        return total, {"policy_loss": pi_loss, "vf_loss": vf_loss, "entropy": entropy}
+
+    def learn(self, buf):
+        c = self.config
+        for _ in range(c["num_sgd_iter"]):
+            out = self._step_kernels(buf) if self.use_kernels else self._step_eager(buf)
+        out["sgd_steps"] = c["num_sgd_iter"]
+        return out
+
+    def _step_eager(self, buf):
+        c, w = self.config, _world()
+        if self.policy.flat.grad is not None:
+            self.policy.flat.grad.zero_()
+        total, st = self.loss(*buf.columns()[:-3], buf.logp, buf.reward)
+        total.backward()
+        self._allreduce_grad(average=False)          # summed loss over the global batch
+        gn = torch.nn.utils.clip_grad_norm_([self.policy.flat], c["grad_clip"]) if c["grad_clip"] else torch.zeros(())
+        self.opt.step()
+        out = {k: self._global_mean(v) * w for k, v in st.items()}
+        out.update({"total_loss": self._global_mean(total) * w, "grad_gnorm": float(gn)})
+        return out
+
+    def _step_kernels(self, buf):
+        c, w, ops = self.config, _world(), self.ops
+        ops.stats.zero_()
+        if w == 1 or (self.comm is not None and self.comm.ok):
+            ops.impala_step(self.comm if w > 1 else None, self.policy.flat, buf, self._hp(), c["lr"], c["grad_clip"], self._work)
+        else:           # no peer memory: the same kernels with an NCCL all-reduce before the clip and Adam
+            logp, value, vs, pg_adv = self._work
+            n, k = buf.T * buf.B, self.kept(buf.T) * buf.B
+            cols = buf.a2c_columns()            # the policy inputs, the action, ...
+            ninp = 1 if self.conti else 2
+            ops.eval(self.policy.flat, cols[:ninp], cols[ninp], logp, value)
+            ops.vtrace(buf.logp, logp, value, buf.reward, self._hp(), vs, pg_adv)
+            hp = {"clip": 0.0, "vf_clip": 0.0, "vf_coeff": c["vf_loss_coeff"], "kl_coeff": 0.0, "ent_coeff": c["entropy_coeff"]}
+            ops.policy_grad(1, self.policy.flat, cols + (pg_adv.reshape(n), vs.reshape(n)), None, 0, k, hp, 1.0, 1.0)
+            dist.all_reduce(ops.grad, op=dist.ReduceOp.SUM)
+            ops.adam(self.policy.flat, c["lr"], 1.0, c["grad_clip"])
+        st = ops.stats
+        g = self._global_means({"policy_loss": st[0], "vf_loss": st[1], "entropy": st[3], "total_loss": st[4],
+                                "gn": ops.grad.norm(), "_episode_reward_mean": buf.reward.sum(0).mean()})
+        return {"policy_loss": g["policy_loss"] * w, "vf_loss": g["vf_loss"] * w, "entropy": g["entropy"] * w,
+                "total_loss": g["total_loss"] * w, "grad_gnorm": g["gn"], "_episode_reward_mean": g["_episode_reward_mean"]}
+
+
+class GaussPGTrainer(PGTrainer):
+    """PG_conti: PGTrainer over the DiagGaussian policy of the continuous-action env."""
+    algo = "PG_conti"
+    conti = True
+
+
+class GaussIMPALATrainer(IMPALATrainer):
+    """IMPALA_conti: IMPALATrainer over the DiagGaussian policy of the continuous-action env."""
+    algo = "IMPALA_conti"
     conti = True
 
 
@@ -1287,8 +1506,8 @@ class RainbowTrainer(DDPGTrainer):
 
 def get_rl_model(algo, rllib_config, env=None, **kw):
     """script/modelfree_trainer.py:11-36.  Only the algorithms of the BASELINE configs are built.  On an env built with
-    support_conti_env, PPO / A2C (and PPO_conti / A2C_conti, modelfree_train.py:46-48) train the Gaussian policy, and
-    DDPG / TD3 (modelfree_trainer.py:25-28) the deterministic actor-critic."""
+    support_conti_env, PPO / A2C / PG / IMPALA (and their *_conti names, modelfree_train.py:46-48) train the Gaussian
+    policy, and DDPG / TD3 (modelfree_trainer.py:25-28) the deterministic actor-critic."""
     conti = env is not None and bool(env.config.get("support_conti_env", False))
     if algo.replace("_rawstate", "") in ("DDPG", "TD3"):
         if algo.endswith("_rawstate") or (env is not None and env.config.get("rawstate_as_obs", False)):
@@ -1308,9 +1527,10 @@ def get_rl_model(algo, rllib_config, env=None, **kw):
             raise ValueError("RAINBOW takes the plain observation: build the env with support_rllib_mask=False "
                              "(the reference turns the mask off for RAINBOW, modelfree_train.py:50-51)")
         return RainbowTrainer(rllib_config, env, **kw)
-    if algo.endswith("_conti") or (conti and algo in ("PPO", "A2C")):
+    gauss = {"PPO": GaussPPOTrainer, "A2C": GaussA2CTrainer, "PG": GaussPGTrainer, "IMPALA": GaussIMPALATrainer}
+    if algo.endswith("_conti") or (conti and algo in gauss):
         base = algo[:-len("_conti")] if algo.endswith("_conti") else algo
-        if base not in ("PPO", "A2C"):
+        if base not in gauss:
             raise NotImplementedError("%s is outside the hot-path scope (SURVEY.md section 2, row 11)" % algo)
         if not conti:
             raise ValueError("%s needs an env built with support_conti_env=True" % algo)
@@ -1319,11 +1539,15 @@ def get_rl_model(algo, rllib_config, env=None, **kw):
         if env.config.get("support_rllib_mask", False):
             raise ValueError("%s takes the plain observation: build the env with support_rllib_mask=False "
                              "(the reference turns the mask off for *_conti, modelfree_train.py:46-48)" % algo)
-        return (GaussPPOTrainer if base == "PPO" else GaussA2CTrainer)(rllib_config, env, **kw)
+        return gauss[base](rllib_config, env, **kw)
     if algo in ("PPO", "PPO_rawstate"):        # '*_rawstate' = the same trainer on an env built with rawstate_as_obs (modelfree_train.py:55-56)
         return PPOTrainer(rllib_config, env, **kw)
     if algo in ("A2C", "A2C_rawstate"):
         return A2CTrainer(rllib_config, env, **kw)
+    if algo in ("PG", "PG_rawstate"):
+        return PGTrainer(rllib_config, env, **kw)
+    if algo in ("IMPALA", "IMPALA_rawstate"):
+        return IMPALATrainer(rllib_config, env, **kw)
     algo = algo.replace("_rawstate", "")
     assert algo in ("PPO", "DQN", "A2C", "A3C", "PG", "IMPALA", "TD3", "RAINBOW", "SLATEQ", "DDPG")
     raise NotImplementedError("%s is outside the hot-path scope (SURVEY.md section 2, row 11)" % algo)
