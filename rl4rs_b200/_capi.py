@@ -7,6 +7,8 @@ with the reason; if it loads but no CUDA device is present, creating an env fail
 import ctypes as C
 import os
 
+import torch
+
 LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "lib", "librl4rs_b200.so")
 
 FLAG_RLLIB_MASK, FLAG_D3RL_MASK, FLAG_CONTI, FLAG_ONEHOT, FLAG_RAWSTATE, FLAG_INFO_FETCH = 1, 2, 4, 8, 16, 32
@@ -177,6 +179,16 @@ def load_library(path=None):
         fn.argtypes = args
     _lib = lib
     return lib
+
+
+def ptr(t, byte_offset=0):
+    """The device (or host) address of tensor t plus byte_offset as a void* argument; NULL for None."""
+    return C.c_void_p(t.data_ptr() + byte_offset) if t is not None else C.c_void_p(0)
+
+
+def stream(device):
+    """The current torch stream of device as the cudaStream_t argument every entry point ends with."""
+    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
 def check(lib, handle, rc, what):

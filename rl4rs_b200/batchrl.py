@@ -22,6 +22,8 @@ import math
 import numpy as np
 import torch
 
+from . import _capi
+from ._capi import ptr
 from .policy import BatchRLNet
 
 ALGOS = {"BC": 0, "BCQ": 1, "CQL": 2}
@@ -40,10 +42,6 @@ DEFAULTS = {
     "CQL": {"batch_size": 256, "learning_rate": 6.25e-5, "eps": 1e-8, "gamma": 1.0, "alpha": 1.0,
             "target_update_interval": 8000, "reward_scaler": "standard"},
 }
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
 def get_model(config, algo, dynamics=None):
@@ -121,14 +119,11 @@ class DeviceDataset(object):
             self.reward = torch.from_numpy(np.asarray(dataset["rewards"], dtype=np.float32).reshape(N)).to(self.device)
             self.terminal = torch.from_numpy((np.asarray(dataset["terminals"]).reshape(N) != 0).astype(np.uint8)).to(self.device)
             if self.device.type == "cuda":
-                from . import _capi
                 lib = _capi.load_library()
                 index = torch.empty(N, dtype=torch.int64, device=self.device)
                 count = torch.zeros(1, dtype=torch.int64, device=self.device)
-                rc = lib.r4_batchrl_transitions(_p(self.terminal), N, _p(index), _p(count),
-                                                C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
-                if rc != 0:
-                    raise _capi.R4Error("r4_batchrl_transitions failed (%d): %s" % (rc, (lib.r4_last_error(None) or b"?").decode()))
+                rc = lib.r4_batchrl_transitions(ptr(self.terminal), N, ptr(index), ptr(count), _capi.stream(self.device))
+                _capi.check(lib, None, rc, "r4_batchrl_transitions")
                 self.transitions = index[:int(count)]
             else:
                 self.transitions = transitions_host(self.terminal)
@@ -174,8 +169,7 @@ class BatchRLModel(object):
         self.step = 0
         self._gen = torch.Generator(device=self.device).manual_seed(self.seed)
         if self.use_kernels:
-            from . import _capi
-            self.capi, self.lib = _capi, _capi.load_library()
+            self.lib = _capi.load_library()
             k = ALGOS[self.algo]
             assert self.lib.r4_batchrl_num_params(k, obs_dim, self.A) == self.net.n_params
             assert self.lib.r4_batchrl_target_size(k, obs_dim, self.A) == self.net.n_target
@@ -274,10 +268,10 @@ class BatchRLModel(object):
         mb = self.batch_size
         steps = data.n // mb
         stats = torch.zeros(steps * 3, dtype=torch.float32, device=self.device)
-        rc = self.lib.r4_batchrl_epoch(ALGOS[self.algo], self.net.K, self.A, _p(self.net.flat), _p(self.net.target),
-                                       _p(self.m), _p(self.v), C.byref(self._tables.data(data)), C.byref(self._hyper_c()),
-                                       _p(perm), perm.numel(), mb, self.step, self.hp["learning_rate"], self.hp["eps"],
-                                       int(self.hp.get("target_update_interval", 0)), _p(self.scratch), _p(stats),
+        rc = self.lib.r4_batchrl_epoch(ALGOS[self.algo], self.net.K, self.A, ptr(self.net.flat), ptr(self.net.target),
+                                       ptr(self.m), ptr(self.v), C.byref(self._tables.data(data)), C.byref(self._hyper_c()),
+                                       ptr(perm), perm.numel(), mb, self.step, self.hp["learning_rate"], self.hp["eps"],
+                                       int(self.hp.get("target_update_interval", 0)), ptr(self.scratch), ptr(stats),
                                        self._stream())
         if rc < 0:
             self._check(rc, "r4_batchrl_epoch")
@@ -286,20 +280,19 @@ class BatchRLModel(object):
 
     def _hyper_c(self):
         h = self._hyper()
-        return self.capi.BatchRLHyper(h["gamma"], h["beta"], h["alpha"], h["log_flex"], h["reward_mean"], h["reward_den"])
+        return _capi.BatchRLHyper(h["gamma"], h["beta"], h["alpha"], h["log_flex"], h["reward_mean"], h["reward_den"])
 
     def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        return _capi.stream(self.device)
 
     def _check(self, rc, what):
-        if rc != 0:
-            raise self.capi.R4Error("%s failed (%d): %s" % (what, rc, (self.lib.r4_last_error(None) or b"?").decode()))
+        _capi.check(self.lib, None, rc, what)
 
     def grad_kernels(self, data, pos):
         """r4_batchrl_grad over the transitions at positions pos (i64, device) -> self.grad, self.stats."""
-        rc = self.lib.r4_batchrl_grad(ALGOS[self.algo], self.net.K, self.A, _p(self.net.flat), _p(self.net.target),
-                                      C.byref(self._tables.data(data)), C.byref(self._hyper_c()), _p(pos), pos.numel(),
-                                      _p(self.scratch), _p(self.grad), _p(self.stats), self._stream())
+        rc = self.lib.r4_batchrl_grad(ALGOS[self.algo], self.net.K, self.A, ptr(self.net.flat), ptr(self.net.target),
+                                      C.byref(self._tables.data(data)), C.byref(self._hyper_c()), ptr(pos), pos.numel(),
+                                      ptr(self.scratch), ptr(self.grad), ptr(self.stats), self._stream())
         self._check(rc, "r4_batchrl_grad")
 
     # ---- acting --------------------------------------------------------------------------------------
@@ -318,9 +311,9 @@ class BatchRLModel(object):
         a = torch.empty(n, dtype=torch.int32, device=self.device)
         probs = torch.empty(n, self.A, dtype=torch.float32, device=self.device) if want_probs else None
         vals = torch.empty(n, self.A, dtype=torch.float32, device=self.device) if want_values else None
-        rc = self.lib.r4_batchrl_act(ALGOS[self.algo], self.net.K, self.A, _p(self.net.flat), _p(x),
+        rc = self.lib.r4_batchrl_act(ALGOS[self.algo], self.net.K, self.A, ptr(self.net.flat), ptr(x),
                                      int(x.dtype == torch.float64), n, C.byref(self._tables.tables()), mode, log_flex,
-                                     _p(a), _p(probs), _p(vals), self._stream())
+                                     ptr(a), ptr(probs), ptr(vals), self._stream())
         self._check(rc, "r4_batchrl_act")
         return a, probs, vals
 

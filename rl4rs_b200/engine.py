@@ -15,10 +15,6 @@ from .synth import Catalog, LogSoA
 OBS_DIM = 256
 
 
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
-
-
 class Engine(object):
     def __init__(self, config, seq, catalog, weights, log, device=None):
         if not torch.cuda.is_available():
@@ -69,9 +65,6 @@ class Engine(object):
         self.env_launches0 = 0
 
     # ---- static data -------------------------------------------------------------------------
-    def _sp(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-
     def _load_items(self, catalog):
         assert isinstance(catalog, Catalog)
         if catalog.action_size != self.A:
@@ -97,7 +90,7 @@ class Engine(object):
                 shape, ptr = (C.c_int64 * a.ndim)(*a.shape), a.ctypes.data
             rc = self.lib.r4_load_weight(self.h, name.encode(), ptr, shape, len(shape))
             _capi.check(self.lib, self.h, rc, "r4_load_weight(%s)" % name)
-        rc = self.lib.r4_finalize_weights(self.h, self._sp())
+        rc = self.lib.r4_finalize_weights(self.h, _capi.stream(self.device))
         _capi.check(self.lib, self.h, rc, "r4_finalize_weights")
 
     def _load_log(self, log):
@@ -119,8 +112,8 @@ class Engine(object):
         self.d_seq = torch.from_numpy(np.ascontiguousarray(log.user_seq, dtype=np.int32)).to(dev)
         self.d_items = torch.from_numpy(np.ascontiguousarray(log.items, dtype=np.int32)).to(dev)
         self.d_fb = torch.from_numpy(np.ascontiguousarray(log.feedback, dtype=np.uint8)).to(dev)
-        rc = self.lib.r4_load_log(self.h, _ptr(self.d_cat), _ptr(self.d_dense), _ptr(self.d_seq),
-                                  _ptr(self.d_items), _ptr(self.d_fb), log.n, log.items.shape[1])
+        rc = self.lib.r4_load_log(self.h, _capi.ptr(self.d_cat), _capi.ptr(self.d_dense), _capi.ptr(self.d_seq),
+                                  _capi.ptr(self.d_items), _capi.ptr(self.d_fb), log.n, log.items.shape[1])
         _capi.check(self.lib, self.h, rc, "r4_load_log")
 
     def _alloc_outputs(self):
@@ -139,9 +132,9 @@ class Engine(object):
         self.click_p = z((B, self.P if self.seq else self.T), torch.float32) if self.info_fetch else None
         self.masked = z((B, self.P if self.seq else self.T), torch.int32) if self.d3rl else None
         self.out = _capi.R4Out(
-            obs=_ptr(self.obs), action_mask=_ptr(self.mask), reward=_ptr(self.reward), done=None,
-            chosen=_ptr(self.chosen), cat=_ptr(self.cat), dense=_ptr(self.dense), seq=_ptr(self.seqf),
-            click_p=_ptr(self.click_p), masked_actions=_ptr(self.masked))
+            obs=_capi.ptr(self.obs), action_mask=_capi.ptr(self.mask), reward=_capi.ptr(self.reward), done=None,
+            chosen=_capi.ptr(self.chosen), cat=_capi.ptr(self.cat), dense=_capi.ptr(self.dense), seq=_capi.ptr(self.seqf),
+            click_p=_capi.ptr(self.click_p), masked_actions=_capi.ptr(self.masked))
         self.act_i32 = z((B,), torch.int32)
         self.act_f32 = z((B, self.emb_dim), torch.float32) if self.conti else None
         self.act_f64 = z((B, self.emb_dim), torch.float64) if self.conti else None
@@ -169,7 +162,7 @@ class Engine(object):
             self.pin_rows.numpy()[:] = rows
             self.rows.copy_(self.pin_rows, non_blocking=True)
             self._ev_rows.record()
-        rc = self.lib.r4_reset(self.h, _ptr(self.rows), C.byref(self.out), self._sp())
+        rc = self.lib.r4_reset(self.h, _capi.ptr(self.rows), C.byref(self.out), _capi.stream(self.device))
         _capi.check(self.lib, self.h, rc, "r4_reset")
         self.paid = False
 
@@ -208,7 +201,7 @@ class Engine(object):
                 a = self.act_i32
         self._keep = a
         cur = self.cur_steps
-        rc = self.lib.r4_step(self.h, _ptr(a), is_f64, C.byref(self.out), self._sp())
+        rc = self.lib.r4_step(self.h, _capi.ptr(a), is_f64, C.byref(self.out), _capi.stream(self.device))
         _capi.check(self.lib, self.h, rc, "r4_step")
         nxt = cur + 1
         self.paid = (nxt % self.P == 0) if self.seq else (nxt >= self.T)
@@ -220,26 +213,26 @@ class Engine(object):
     def prev_actions(self):
         """Copy of SlateState.prev_actions as a device tensor i32 [B, max_steps]."""
         t = torch.empty((self.B, self.T), dtype=torch.int32, device=self.device)
-        rc = self.lib.r4_copy_prev_actions(self.h, _ptr(t), self._sp())
+        rc = self.lib.r4_copy_prev_actions(self.h, _capi.ptr(t), _capi.stream(self.device))
         _capi.check(self.lib, self.h, rc, "r4_copy_prev_actions")
         return t
 
     def offline_action(self):
         items = torch.empty((self.B,), dtype=torch.int32, device=self.device)
         emb = torch.empty((self.B, self.emb_dim), dtype=torch.float64, device=self.device) if self.conti else None
-        rc = self.lib.r4_offline_action(self.h, _ptr(items), _ptr(emb), self._sp())
+        rc = self.lib.r4_offline_action(self.h, _capi.ptr(items), _capi.ptr(emb), _capi.stream(self.device))
         _capi.check(self.lib, self.h, rc, "r4_offline_action")
         return items, emb
 
     def offline_reward(self):
         out = torch.empty((self.B,), dtype=torch.float64, device=self.device)
-        rc = self.lib.r4_offline_reward(self.h, _ptr(out), self._sp())
+        rc = self.lib.r4_offline_reward(self.h, _capi.ptr(out), _capi.stream(self.device))
         _capi.check(self.lib, self.h, rc, "r4_offline_reward")
         return out
 
     def violation(self):
         out = torch.empty((self.B,), dtype=torch.int32, device=self.device)
-        rc = self.lib.r4_violation(self.h, _ptr(out), self._sp())
+        rc = self.lib.r4_violation(self.h, _capi.ptr(out), _capi.stream(self.device))
         _capi.check(self.lib, self.h, rc, "r4_violation")
         return out
 
@@ -261,14 +254,14 @@ class Engine(object):
         cat = torch.empty((self.B, int(c.get("category_feature_num", 21))), dtype=torch.int32, device=self.device)
         dense = torch.empty((self.B, int(c.get("dense_feature_num", 432))), dtype=torch.float32, device=self.device)
         seq = torch.empty((self.B, int(c.get("seq_num", 2)), int(c.get("maxlen", 64))), dtype=torch.int32, device=self.device)
-        rc = self.lib.r4_features(self.h, _ptr(cat), _ptr(dense), _ptr(seq), self._sp())
+        rc = self.lib.r4_features(self.h, _capi.ptr(cat), _capi.ptr(dense), _capi.ptr(seq), _capi.stream(self.device))
         _capi.check(self.lib, self.h, rc, "r4_features")
         return cat, dense, seq
 
     def nearest_neighbor(self, actions):
         a = torch.as_tensor(np.ascontiguousarray(actions, dtype=np.float64)).to(self.device)
         out = torch.empty((a.shape[0],), dtype=torch.int32, device=self.device)
-        rc = self.lib.r4_nearest_neighbor(self.h, _ptr(a), 1, a.shape[0], _ptr(out), self._sp())
+        rc = self.lib.r4_nearest_neighbor(self.h, _capi.ptr(a), 1, a.shape[0], _capi.ptr(out), _capi.stream(self.device))
         _capi.check(self.lib, self.h, rc, "r4_nearest_neighbor")
         return out
 
@@ -281,7 +274,8 @@ class Engine(object):
         n = seq.shape[0]
         obs = torch.empty((n, self.obs_dim), dtype=torch.float32, device=dev)
         probs = torch.empty((n, 2), dtype=torch.float32, device=dev)
-        rc = self.lib.r4_dien_forward(self.h, _ptr(seq), _ptr(dense), _ptr(cat), n, _ptr(obs), _ptr(probs), self._sp())
+        rc = self.lib.r4_dien_forward(self.h, _capi.ptr(seq), _capi.ptr(dense), _capi.ptr(cat), n, _capi.ptr(obs),
+                                      _capi.ptr(probs), _capi.stream(dev))
         _capi.check(self.lib, self.h, rc, "r4_dien_forward")
         return obs, probs
 

@@ -17,7 +17,8 @@ import math
 import numpy as np
 import torch
 
-from . import synth
+from . import _capi, synth
+from ._capi import ptr
 from .utils import tf_checkpoint
 from .utils.datautil import FeatureUtil
 
@@ -314,10 +315,6 @@ class Metrics(object):
 
 
 # ---- the trainer ----------------------------------------------------------------------------------------------------
-def _p(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
-
-
 class _Stream(object):
     """An endless stream of minibatches cut from consecutive seeded permutations of the sample set (tf.data's
     shuffle(10000).repeat() cannot be reproduced; INTEGRATION.md section 8)."""
@@ -352,7 +349,6 @@ class SimulatorTrainer(object):
         self.v = torch.zeros_like(flat)
         self._uploaded = {}
         if self.device.type == "cuda":
-            from . import _capi
             self.lib = _capi.load_library()
             if self.lib.r4_simtrain_num_params(self.H) != flat.numel():
                 raise ValueError("category_hash_size %d is outside the library's range" % self.H)
@@ -396,7 +392,6 @@ class SimulatorTrainer(object):
         if key not in self._uploaded:
             if samples.hash_size > self.H:
                 raise ValueError("samples were checked against category_hash_size %d > %d" % (samples.hash_size, self.H))
-            from . import _capi
             ts = [torch.from_numpy(np.ascontiguousarray(getattr(samples, k))).to(self.device) for k in ItemSamples.FIELDS]
             self._uploaded[key] = (samples, ts, _capi.SimTrainData(*[t.data_ptr() for t in ts]))
         return self._uploaded[key][2]
@@ -411,7 +406,6 @@ class SimulatorTrainer(object):
         return self.scratch
 
     def _check(self, rc, what):
-        from . import _capi
         _capi.check(self.lib, None, rc, what)
 
     # -- one step / one evaluation batch --
@@ -423,10 +417,10 @@ class SimulatorTrainer(object):
         n = int(idx.numel())
         if self.device.type == "cuda":
             d = self._data(samples)
-            rc = self.lib.r4_simtrain_step(self.H, _p(self.params), _p(self.grad), _p(self.m), _p(self.v), C.byref(d), _p(idx), n,
+            rc = self.lib.r4_simtrain_step(self.H, ptr(self.params), ptr(self.grad), ptr(self.m), ptr(self.v), C.byref(d), ptr(idx), n,
                                            self.data_seed, counter, rate, self.step, ADAM["lr"], ADAM["beta1"], ADAM["beta2"],
-                                           ADAM["eps"], _p(self._scratch(n)), _p(self.stats), _p(self.acc),
-                                           C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+                                           ADAM["eps"], ptr(self._scratch(n)), ptr(self.stats), ptr(self.acc),
+                                           _capi.stream(self.device))
             self._check(rc, "r4_simtrain_step")
             return
         cat, dense, seq, y = samples.features(idx.numpy())
@@ -447,8 +441,8 @@ class SimulatorTrainer(object):
         if self.device.type == "cuda":
             d = self._data(samples)
             probs = torch.empty(n, 2, dtype=torch.float32, device=self.device)
-            rc = self.lib.r4_simtrain_eval(self.H, _p(self.params), C.byref(d), _p(idx), n, _p(self._scratch(n)), _p(probs),
-                                           _p(self.acc), C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+            rc = self.lib.r4_simtrain_eval(self.H, ptr(self.params), C.byref(d), ptr(idx), n, ptr(self._scratch(n)), ptr(probs),
+                                           ptr(self.acc), _capi.stream(self.device))
             self._check(rc, "r4_simtrain_eval")
             return probs
         cat, dense, seq, y = samples.features(idx.numpy())

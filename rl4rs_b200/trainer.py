@@ -26,12 +26,10 @@ import ctypes as C
 import torch
 import torch.distributed as dist
 
+from . import _capi
+from ._capi import ptr
 from .policy import (DeterministicActorCritic, DistributionalQNetwork, GaussianPolicy, MaskedPolicy, RawStatePolicy,
                      counter_draws)
-
-
-def _p(t, byte_offset=0):
-    return C.c_void_p(t.data_ptr() + byte_offset) if t is not None else C.c_void_p(0)
 
 
 def _hp(hp):
@@ -39,27 +37,15 @@ def _hp(hp):
     return hp["clip"], hp["vf_clip"], hp["vf_coeff"], hp["kl_coeff"], hp["ent_coeff"]
 
 
-class KernelOps(object):
-    """ctypes front of the K12 kernels (include/rl4rs_b200.h: r4_policy_act / r4_policy_grad / r4_adam_step).  `data` is
-    (obs, mask, action, logp, logits, value, adv, target), the argument order of the gradient entry points."""
+class _LearnerOps(object):
+    """What every ctypes front of the learner kernels holds: the library, the device, the Adam moments m and v, the
+    gradient, the loss statistics and the learner scratch (sized by the subclass), and the launch-count baseline."""
 
-    def __init__(self, A, device, n_params):
-        self.A = A
-        self._init(device, n_params)
-
-    def _init(self, device, n_params):
-        """The Adam, gradient and statistics buffers, the learner scratch and the counters, for either policy."""
-        from . import _capi
-        self.capi = _capi
+    def __init__(self, device, n_params, n_stats, n_scratch):
         self.lib = _capi.load_library()
-        self.device, self.n = device, n_params
-        assert self._num_params() == n_params
+        self.device = device
         z = lambda k: torch.zeros(k, dtype=torch.float32, device=device)
-        self.m, self.v, self.grad, self.stats, self.norm = z(n_params), z(n_params), z(n_params), z(5), z(1)
-        self.sms = torch.cuda.get_device_properties(device).multi_processor_count   # grid cap of the learner kernels
-        self.scratch = z(self._scratch_floats())
-        self.step = 0
-        self.counter = 0
+        self.m, self.v, self.grad, self.stats, self.scratch = z(n_params), z(n_params), z(n_params), z(n_stats), z(n_scratch)
         self._launch0 = self.lib.r4_learner_launch_count()
 
     @property
@@ -68,35 +54,47 @@ class KernelOps(object):
         them (r4_learner_launch_count; bench.py's gpu_launches).  In a process that drives one learner, those are its own."""
         return self.lib.r4_learner_launch_count() - self._launch0
 
-    def _num_params(self):
-        return self.lib.r4_policy_num_params(self.A)
-
-    def _scratch_floats(self):
-        return self.sms * (self.n + 5)   # one partial gradient + statistics per CTA
-
     def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        return _capi.stream(self.device)
 
     def _check(self, rc, what):
-        if rc != 0:
-            raise self.capi.R4Error("%s failed (%d): %s" % (what, rc, (self.lib.r4_last_error(None) or b"?").decode()))
+        _capi.check(self.lib, None, rc, what)
+
+
+class KernelOps(_LearnerOps):
+    """ctypes front of the K12 kernels (include/rl4rs_b200.h: r4_policy_act / r4_policy_grad / r4_adam_step).  `data` is
+    (obs, mask, action, logp, logits, value, adv, target), the argument order of the gradient entry points."""
+
+    def __init__(self, A, device, n_params):
+        self.A = A
+        assert _capi.load_library().r4_policy_num_params(A) == n_params
+        self.sms = torch.cuda.get_device_properties(device).multi_processor_count   # grid cap of the learner kernels
+        self._init(device, n_params, self.sms * (n_params + 5))   # one partial gradient + statistics per CTA
+
+    def _init(self, device, n_params, n_scratch):
+        """The buffers of either policy's learner (5 statistics), the clip's norm and the Adam and draw counters."""
+        super().__init__(device, n_params, 5, n_scratch)
+        self.n = n_params
+        self.norm = torch.zeros(1, dtype=torch.float32, device=device)
+        self.step = 0
+        self.counter = 0
 
     def act(self, flat, obs, mask, explore, seed, action_i32, logp, value, logits):
         n = obs.shape[0]
-        rc = self.lib.r4_policy_act(_p(flat), _p(obs), _p(mask), n, self.A, int(bool(explore)), seed, self.counter,
-                                    _p(action_i32), _p(logp), _p(value), _p(logits), self._stream())
+        rc = self.lib.r4_policy_act(ptr(flat), ptr(obs), ptr(mask), n, self.A, int(bool(explore)), seed, self.counter,
+                                    ptr(action_i32), ptr(logp), ptr(value), ptr(logits), self._stream())
         self._check(rc, "r4_policy_act")
         self.counter += n
 
     def policy_grad(self, mode, flat, data, idx, idx_offset, n, hp, inv_n, stat_scale, G=None):
         G = G or max(1, min((n + 3) // 4, self.sms))          # 4 samples per CTA tile (r4_ppo.cuh: TS)
-        rc = self.lib.r4_policy_grad(mode, _p(flat), *map(_p, data), _p(idx, idx_offset * 8), n, self.A, *_hp(hp), inv_n,
-                                     _p(self.scratch), G, _p(self.grad), _p(self.stats), stat_scale, self._stream())
+        rc = self.lib.r4_policy_grad(mode, ptr(flat), *map(ptr, data), ptr(idx, idx_offset * 8), n, self.A, *_hp(hp), inv_n,
+                                     ptr(self.scratch), G, ptr(self.grad), ptr(self.stats), stat_scale, self._stream())
         self._check(rc, "r4_policy_grad")
 
     def ppo_epoch(self, flat, data, perm, n, mb, hp, lr, clip):
         """All minibatch steps of one SGD epoch in ONE library call (single-GPU learner)."""
-        rc = self._epoch("r4_ppo_epoch", (), self.A, flat, data, perm, n, mb, hp, lr, (float(clip or 0.0), _p(self.norm)))
+        rc = self._epoch("r4_ppo_epoch", (), self.A, flat, data, perm, n, mb, hp, lr, (float(clip or 0.0), ptr(self.norm)))
         return rc
 
     def ppo_epoch_dist(self, comm, flat, data, perm, n, mb_local, hp, lr):
@@ -108,8 +106,8 @@ class KernelOps(object):
     def _epoch(self, fn, head, dim, flat, data, perm, n, mb, hp, lr, tail):
         """One call of an epoch entry point (r4_ppo_epoch, r4_gauss_ppo_epoch and their _dist forms): the argument lists differ
         only in the leading communicator, the policy's columns and size, and the trailing gradient clip."""
-        rc = getattr(self.lib, fn)(*head, _p(flat), *map(_p, data), _p(perm), n, mb, dim, *_hp(hp), _p(self.scratch),
-                                   _p(self.grad), _p(self.stats), _p(self.m), _p(self.v), self.step, lr, 0.9, 0.999, 1e-8,
+        rc = getattr(self.lib, fn)(*head, ptr(flat), *map(ptr, data), ptr(perm), n, mb, dim, *_hp(hp), ptr(self.scratch),
+                                   ptr(self.grad), ptr(self.stats), ptr(self.m), ptr(self.v), self.step, lr, 0.9, 0.999, 1e-8,
                                    *tail, self._stream())
         if rc < 0:
             self._check(rc, fn)
@@ -119,41 +117,41 @@ class KernelOps(object):
     def policy_grad_exchange(self, comm, mode, flat, data, n, hp, inv_n, stat_scale):
         """One gradient over n local samples, summed over the ranks through peer memory into self.grad (A2C)."""
         G = max(1, min((n + 3) // 4, self.sms))
-        rc = self.lib.r4_policy_grad_partial(mode, _p(flat), *map(_p, data), C.c_void_p(0), n, self.A, *_hp(hp), inv_n,
-                                             _p(self.scratch), G, self._stream())
+        rc = self.lib.r4_policy_grad_partial(mode, ptr(flat), *map(ptr, data), C.c_void_p(0), n, self.A, *_hp(hp), inv_n,
+                                             ptr(self.scratch), G, self._stream())
         self._check(rc, "r4_policy_grad_partial")
         self._exchange(comm, self.scratch, G, stat_scale)
 
     def _exchange(self, comm, partial, G, stat_scale):
         """self.grad = the sum over the ranks of this rank's G partial gradients in `partial` (then their statistics)."""
-        rc = self.lib.r4_grad_exchange_n(comm.h, _p(partial), G, self.n, _p(self.grad), _p(self.stats), stat_scale,
+        rc = self.lib.r4_grad_exchange_n(comm.h, ptr(partial), G, self.n, ptr(self.grad), ptr(self.stats), stat_scale,
                                          self._stream())
         self._check(rc, "r4_grad_exchange_n")
 
     def gae(self, reward, value, gamma, lam):
         """-> (target, adv) of a [T, B] rollout in one launch (r4_gae)."""
         adv, target = torch.empty_like(reward), torch.empty_like(reward)
-        rc = self.lib.r4_gae(_p(reward), _p(value), reward.shape[0], reward.shape[1], gamma, gamma * lam, _p(adv), _p(target), self._stream())
+        rc = self.lib.r4_gae(ptr(reward), ptr(value), reward.shape[0], reward.shape[1], gamma, gamma * lam, ptr(adv), ptr(target), self._stream())
         self._check(rc, "r4_gae")
         return target, adv
 
     def adam(self, flat, lr, grad_scale, clip):
         self.step += 1
-        rc = self.lib.r4_adam_step(_p(flat), _p(self.grad), _p(self.m), _p(self.v), self.n, self.step, lr, 0.9, 0.999,
-                                   1e-8, grad_scale, float(clip or 0.0), _p(self.norm), self._stream())
+        rc = self.lib.r4_adam_step(ptr(flat), ptr(self.grad), ptr(self.m), ptr(self.v), self.n, self.step, lr, 0.9, 0.999,
+                                   1e-8, grad_scale, float(clip or 0.0), ptr(self.norm), self._stream())
         self._check(rc, "r4_adam_step")
 
     # ---- IMPALA ----
     def eval(self, flat, inputs, action, logp, value):
         """logp [n] of the stored actions and value [n] under flat, in one launch (r4_policy_eval)."""
-        rc = self.lib.r4_policy_eval(_p(flat), *map(_p, inputs), _p(action), action.shape[0], self.A, _p(logp), _p(value),
+        rc = self.lib.r4_policy_eval(ptr(flat), *map(ptr, inputs), ptr(action), action.shape[0], self.A, ptr(logp), ptr(value),
                                      self._stream())
         self._check(rc, "r4_policy_eval")
 
     def vtrace(self, behaviour_logp, target_logp, value, reward, hp, vs, pg_adv):
         """vs, pg_adv [T, B] of a rollout (r4_vtrace); hp = IMPALATrainer._hp()."""
         T, B = reward.shape
-        rc = self.lib.r4_vtrace(_p(behaviour_logp), _p(target_logp), _p(value), _p(reward), T, B, *hp[:4], _p(vs), _p(pg_adv),
+        rc = self.lib.r4_vtrace(ptr(behaviour_logp), ptr(target_logp), ptr(value), ptr(reward), T, B, *hp[:4], ptr(vs), ptr(pg_adv),
                                 self._stream())
         self._check(rc, "r4_vtrace")
 
@@ -165,8 +163,8 @@ class KernelOps(object):
         """One IMPALA learner step in ONE library call (r4_impala_step / r4_gauss_impala_step): forward, V-trace, gradient,
         the exchange over peer memory when comm is given, clip and Adam.  work = (logp, value, vs, pg_adv) [T, B]."""
         fn, cols, dim = self._impala_cols(buf)
-        rc = getattr(self.lib, fn)(comm.h if comm is not None else None, _p(flat), *map(_p, cols), buf.T, buf.B, dim, *hp, *map(_p, work), _p(self.scratch), _p(self.grad), _p(self.stats), _p(self.m),
-                                   _p(self.v), self.step + 1, lr, 0.9, 0.999, 1e-8, float(clip or 0.0), _p(self.norm),
+        rc = getattr(self.lib, fn)(comm.h if comm is not None else None, ptr(flat), *map(ptr, cols), buf.T, buf.B, dim, *hp, *map(ptr, work), ptr(self.scratch), ptr(self.grad), ptr(self.stats), ptr(self.m),
+                                   ptr(self.v), self.step + 1, lr, 0.9, 0.999, 1e-8, float(clip or 0.0), ptr(self.norm),
                                    self._stream())
         self._check(rc, fn)
         self.step += 1
@@ -178,32 +176,28 @@ class GaussKernelOps(KernelOps):
 
     def __init__(self, D, device, n_params):
         self.D = D
-        self._init(device, n_params)
+        lib = _capi.load_library()
+        assert lib.r4_gauss_num_params(D) == n_params
+        self._init(device, n_params, lib.r4_gauss_scratch_size(D))
         # one rank's gradient + statistics, the partial r4_grad_exchange_n sums (A2C)
         self.gsum = torch.zeros(n_params + 5, dtype=torch.float32, device=device)
 
-    def _num_params(self):
-        return self.lib.r4_gauss_num_params(self.D)
-
-    def _scratch_floats(self):
-        return self.lib.r4_gauss_scratch_size(self.D)
-
     def act(self, flat, obs, explore, seed, action, env_action, logp, value, dist_inputs):
         n = obs.shape[0]
-        rc = self.lib.r4_gauss_act(_p(flat), _p(obs), n, self.D, int(bool(explore)), seed, self.counter, _p(action),
-                                   _p(env_action), _p(logp), _p(value), _p(dist_inputs), self._stream())
+        rc = self.lib.r4_gauss_act(ptr(flat), ptr(obs), n, self.D, int(bool(explore)), seed, self.counter, ptr(action),
+                                   ptr(env_action), ptr(logp), ptr(value), ptr(dist_inputs), self._stream())
         self._check(rc, "r4_gauss_act")
         self.counter += n
 
     def policy_grad(self, mode, flat, data, idx, idx_offset, n, hp, inv_n, stat_scale, grad=None, stats=None):
         grad = self.grad if grad is None else grad
         stats = self.stats if stats is None else stats
-        rc = self.lib.r4_gauss_grad(mode, _p(flat), *map(_p, data), _p(idx, idx_offset * 8), n, self.D, *_hp(hp), inv_n,
-                                    _p(self.scratch), _p(grad), _p(stats), stat_scale, self._stream())
+        rc = self.lib.r4_gauss_grad(mode, ptr(flat), *map(ptr, data), ptr(idx, idx_offset * 8), n, self.D, *_hp(hp), inv_n,
+                                    ptr(self.scratch), ptr(grad), ptr(stats), stat_scale, self._stream())
         self._check(rc, "r4_gauss_grad")
 
     def ppo_epoch(self, flat, data, perm, n, mb, hp, lr, clip):
-        rc = self._epoch("r4_gauss_ppo_epoch", (), self.D, flat, data, perm, n, mb, hp, lr, (float(clip or 0.0), _p(self.norm)))
+        rc = self._epoch("r4_gauss_ppo_epoch", (), self.D, flat, data, perm, n, mb, hp, lr, (float(clip or 0.0), ptr(self.norm)))
         return rc
 
     def ppo_epoch_dist(self, comm, flat, data, perm, n, mb_local, hp, lr):
@@ -211,7 +205,7 @@ class GaussKernelOps(KernelOps):
         return rc
 
     def eval(self, flat, inputs, action, logp, value):
-        rc = self.lib.r4_gauss_eval(_p(flat), *map(_p, inputs), _p(action), action.shape[0], self.D, _p(logp), _p(value),
+        rc = self.lib.r4_gauss_eval(ptr(flat), *map(ptr, inputs), ptr(action), action.shape[0], self.D, ptr(logp), ptr(value),
                                     self._stream())
         self._check(rc, "r4_gauss_eval")
 
@@ -232,7 +226,6 @@ class PeerComm(object):
     box -- the trainer then keeps the NCCL all-reduce per step and says so."""
 
     def __init__(self, n_params, device):
-        from . import _capi
         self.lib = _capi.load_library()
         self.h, self.ok, self.why = None, False, ""
         if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size() < 2 or device.type != "cuda":
@@ -279,6 +272,10 @@ A2C_DEFAULTS = {"gamma": 1.0, "lambda": 1.0, "grad_clip": 10.0, "lr": 1e-4, "vf_
 
 def _world():
     return dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+
+
+def _rank():
+    return dist.get_rank() if dist.is_available() and dist.is_initialized() else 0
 
 
 class RolloutBuffer(object):
@@ -384,7 +381,7 @@ class _TrainerBase(object):
         self.comm = PeerComm(self.policy.n_params, self.device) if self.use_kernels else None
         # shared `seed` for the parameter init and the minibatch permutation; the exploration noise is per rank
         # (k_policy_act hashes seed ^ counter+row: the same seed would give rank r row i the noise of rank 0 row i)
-        rank = dist.get_rank() if dist.is_available() and dist.is_initialized() else 0
+        rank = _rank()
         self._seed = (seed * 1000003 + rank) & 0x7fffffffffffffff
         if rank and not self.use_kernels:
             torch.manual_seed(seed * 1000003 + rank)
@@ -429,6 +426,38 @@ class _TrainerBase(object):
             dist.all_reduce(self.policy.flat.grad, op=dist.ReduceOp.SUM)     # the ONE collective
             if average:
                 self.policy.flat.grad.div_(w)
+
+    def _torch_step(self, total, average, clip):
+        """One torch.optim step on the loss `total`: its gradient summed (or, with `average`, averaged) over the ranks and
+        clipped to the global norm `clip` when set -> the gradient norm (0 without a clip)."""
+        flat = self.policy.flat
+        if flat.grad is not None:
+            flat.grad.zero_()
+        total.backward()
+        self._allreduce_grad(average)
+        gn = torch.nn.utils.clip_grad_norm_([flat], clip) if clip else torch.zeros(())
+        self.opt.step()
+        return gn
+
+    def _kernel_grad(self, data, n, hp, stat_scale):
+        """ops.grad, ops.stats = the A2C-mode gradient of this rank's n rows, summed over the global batch: one exchange over
+        peer memory, or the gradient and an all-reduce."""
+        ops = self.ops
+        ops.stats.zero_()
+        if _world() > 1 and self.comm is not None and self.comm.ok:
+            ops.policy_grad_exchange(self.comm, 1, self.policy.flat, data, n, hp, 1.0, stat_scale)
+        else:
+            ops.policy_grad(1, self.policy.flat, data, None, 0, n, hp, 1.0, stat_scale)
+            if _world() > 1:
+                dist.all_reduce(ops.grad, op=dist.ReduceOp.SUM)
+
+    def _kernel_stats(self, buf, gn):
+        """The kernel learner's summed losses over the global batch and the gradient norm gn (A2C's and IMPALA's result)."""
+        st, w = self.ops.stats, _world()
+        g = self._global_means({"policy_loss": st[0], "vf_loss": st[1], "entropy": st[3], "total_loss": st[4], "gn": gn,
+                                "_episode_reward_mean": buf.reward.sum(0).mean()})
+        return {"policy_loss": g["policy_loss"] * w, "vf_loss": g["vf_loss"] * w, "entropy": g["entropy"] * w,
+                "total_loss": g["total_loss"] * w, "grad_gnorm": g["gn"], "_episode_reward_mean": g["_episode_reward_mean"]}
 
     def _global_mean(self, x):
         x = x.detach().clone().to(torch.float64)
@@ -502,12 +531,10 @@ class _TrainerBase(object):
     def save(self, checkpoint_dir):
         os.makedirs(checkpoint_dir, exist_ok=True)
         path = os.path.join(checkpoint_dir, "checkpoint_%06d.pt" % self.iteration)
-        kst = None
-        if self.use_kernels:
-            kst = {"m": self.ops.m.cpu(), "v": self.ops.v.cpu(), "step": self.ops.step}
-        torch.save({"algo": self.algo, "flat": self.policy.flat.detach().cpu(), "opt": self.opt.state_dict(), "kernel_adam": kst,
-                    "iteration": self.iteration, "timesteps_total": self.timesteps_total,
-                    "extra": self._extra_state()}, path)
+        kst = {"m": self.ops.m.cpu(), "v": self.ops.v.cpu()} if self.use_kernels else None
+        st = {"algo": self.algo, "flat": self.policy.flat.detach().cpu(), "kernel_adam": kst, "iteration": self.iteration,
+              "timesteps_total": self.timesteps_total}
+        torch.save(dict(st, **self._state(kst)), path)
         return path
 
     def restore(self, path):
@@ -515,11 +542,21 @@ class _TrainerBase(object):
         assert st["algo"] == self.algo
         with torch.no_grad():
             self.policy.flat.copy_(st["flat"].to(self.device))
+        if self.use_kernels and st.get("kernel_adam"):
+            self.ops.m.copy_(st["kernel_adam"]["m"]); self.ops.v.copy_(st["kernel_adam"]["v"])
+        self.iteration, self.timesteps_total = st["iteration"], st["timesteps_total"]
+        self._load_state(st)
+
+    def _state(self, kernel_adam):
+        """The algorithm's own checkpoint entries; kernel_adam (the kernels' Adam moments, or None) takes its step count."""
+        if kernel_adam is not None:
+            kernel_adam["step"] = self.ops.step
+        return {"opt": self.opt.state_dict(), "extra": self._extra_state()}
+
+    def _load_state(self, st):
         self.opt.load_state_dict(st["opt"])
         if self.use_kernels and st.get("kernel_adam"):
-            k = st["kernel_adam"]
-            self.ops.m.copy_(k["m"]); self.ops.v.copy_(k["v"]); self.ops.step = k["step"]
-        self.iteration, self.timesteps_total = st["iteration"], st["timesteps_total"]
+            self.ops.step = st["kernel_adam"]["step"]
         self._load_extra_state(st["extra"])
 
     def _extra_state(self):
@@ -593,14 +630,8 @@ class PPOTrainer(_TrainerBase):
             perm = self._perm(n, data[0].device)
             for s in range(0, n - mb + 1, mb):
                 idx = perm[s:s + mb]
-                if self.policy.flat.grad is not None:
-                    self.policy.flat.grad.zero_()
                 total, st = self.loss(*[d[idx] for d in data])
-                total.backward()
-                self._allreduce_grad(average=True)
-                if c["grad_clip"]:
-                    torch.nn.utils.clip_grad_norm_([self.policy.flat], c["grad_clip"])
-                self.opt.step()
+                self._torch_step(total, True, c["grad_clip"])
                 steps += 1
                 for k, v in st.items():
                     agg[k] = agg.get(k, 0.0) + v.detach()
@@ -667,31 +698,13 @@ class A2CTrainer(_TrainerBase):
         adv, target = adv.reshape(n).contiguous(), target.reshape(n).contiguous()
         w = _world()
         if self.use_kernels:
-            ops = self.ops
-            data = buf.a2c_columns() + (adv, target)
             hp = {"clip": 0.0, "vf_clip": 0.0, "vf_coeff": c["vf_loss_coeff"], "kl_coeff": 0.0, "ent_coeff": c["entropy_coeff"]}
-            ops.stats.zero_()
-            if w > 1 and self.comm is not None and self.comm.ok:
-                ops.policy_grad_exchange(self.comm, 1, self.policy.flat, data, n, hp, 1.0, 1.0)   # summed over the ranks
-            else:
-                ops.policy_grad(1, self.policy.flat, data, None, 0, n, hp, 1.0, 1.0)
-                if w > 1:
-                    dist.all_reduce(ops.grad, op=dist.ReduceOp.SUM)            # summed loss over the global batch
-            gn = ops.grad.norm()
-            ops.adam(self.policy.flat, c["lr"], 1.0, c["grad_clip"])
-            st = ops.stats
-            g = self._global_means({"policy_loss": st[0], "vf_loss": st[1], "entropy": st[3], "total_loss": st[4], "gn": gn,
-                                    "_episode_reward_mean": buf.reward.sum(0).mean()})
-            return {"policy_loss": g["policy_loss"] * w, "vf_loss": g["vf_loss"] * w, "entropy": g["entropy"] * w,
-                    "total_loss": g["total_loss"] * w, "grad_gnorm": g["gn"], "sgd_steps": 1,
-                    "_episode_reward_mean": g["_episode_reward_mean"]}
-        if self.policy.flat.grad is not None:
-            self.policy.flat.grad.zero_()
+            self._kernel_grad(buf.a2c_columns() + (adv, target), n, hp, 1.0)
+            gn = self.ops.grad.norm()
+            self.ops.adam(self.policy.flat, c["lr"], 1.0, c["grad_clip"])
+            return dict(self._kernel_stats(buf, gn), sgd_steps=1)
         total, st = self.loss(*buf.columns()[:-3], adv, target)       # the policy inputs and the action
-        total.backward()
-        self._allreduce_grad(average=False)          # summed loss over the global batch
-        gn = torch.nn.utils.clip_grad_norm_([self.policy.flat], c["grad_clip"]) if c["grad_clip"] else torch.zeros(())
-        self.opt.step()
+        gn = self._torch_step(total, False, c["grad_clip"])           # summed loss over the global batch
         out = {k: self._global_mean(v) * w for k, v in st.items()}
         out.update({"total_loss": self._global_mean(total) * w, "grad_gnorm": float(gn), "sgd_steps": 1})
         return out
@@ -749,26 +762,15 @@ class PGTrainer(_TrainerBase):
         ret = self.returns(buf).reshape(n).contiguous()
         if self.use_kernels:
             ops = self.ops
-            data = buf.a2c_columns() + (ret, ret)      # adv = the return; the target is unread at vf_coeff 0
             hp = {"clip": 0.0, "vf_clip": 0.0, "vf_coeff": 0.0, "kl_coeff": 0.0, "ent_coeff": 0.0}
-            ops.stats.zero_()
-            if w > 1 and self.comm is not None and self.comm.ok:
-                ops.policy_grad_exchange(self.comm, 1, self.policy.flat, data, n, hp, 1.0, 1.0 / n)
-            else:
-                ops.policy_grad(1, self.policy.flat, data, None, 0, n, hp, 1.0, 1.0 / n)
-                if w > 1:
-                    dist.all_reduce(ops.grad, op=dist.ReduceOp.SUM)
+            self._kernel_grad(buf.a2c_columns() + (ret, ret), n, hp, 1.0 / n)   # adv = the return; the target is unread
             ops.adam(self.policy.flat, c["lr"], 1.0 / (w * n), None)      # the summed gradient -> the global mean's
             g = self._global_means({"policy_loss": ops.stats[0], "entropy": ops.stats[3],
                                     "_episode_reward_mean": buf.reward.sum(0).mean()})
             g.update({"total_loss": g["policy_loss"], "sgd_steps": 1})
             return g
-        if self.policy.flat.grad is not None:
-            self.policy.flat.grad.zero_()
         total, st = self.loss(*buf.columns()[:-3], ret)
-        total.backward()
-        self._allreduce_grad(average=True)          # the mean over the global batch
-        self.opt.step()
+        self._torch_step(total, True, None)          # the mean over the global batch
         return {"policy_loss": self._global_mean(total), "total_loss": self._global_mean(total), "sgd_steps": 1}
 
 
@@ -845,22 +847,17 @@ class IMPALATrainer(_TrainerBase):
         return out
 
     def _step_eager(self, buf):
-        c, w = self.config, _world()
-        if self.policy.flat.grad is not None:
-            self.policy.flat.grad.zero_()
+        w = _world()
         total, st = self.loss(*buf.columns()[:-3], buf.logp, buf.reward)
-        total.backward()
-        self._allreduce_grad(average=False)          # summed loss over the global batch
-        gn = torch.nn.utils.clip_grad_norm_([self.policy.flat], c["grad_clip"]) if c["grad_clip"] else torch.zeros(())
-        self.opt.step()
+        gn = self._torch_step(total, False, self.config["grad_clip"])          # summed loss over the global batch
         out = {k: self._global_mean(v) * w for k, v in st.items()}
         out.update({"total_loss": self._global_mean(total) * w, "grad_gnorm": float(gn)})
         return out
 
     def _step_kernels(self, buf):
         c, w, ops = self.config, _world(), self.ops
-        ops.stats.zero_()
         if w == 1 or (self.comm is not None and self.comm.ok):
+            ops.stats.zero_()
             ops.impala_step(self.comm if w > 1 else None, self.policy.flat, buf, self._hp(), c["lr"], c["grad_clip"], self._work)
         else:           # no peer memory: the same kernels with an NCCL all-reduce before the clip and Adam
             logp, value, vs, pg_adv = self._work
@@ -870,14 +867,9 @@ class IMPALATrainer(_TrainerBase):
             ops.eval(self.policy.flat, cols[:ninp], cols[ninp], logp, value)
             ops.vtrace(buf.logp, logp, value, buf.reward, self._hp(), vs, pg_adv)
             hp = {"clip": 0.0, "vf_clip": 0.0, "vf_coeff": c["vf_loss_coeff"], "kl_coeff": 0.0, "ent_coeff": c["entropy_coeff"]}
-            ops.policy_grad(1, self.policy.flat, cols + (pg_adv.reshape(n), vs.reshape(n)), None, 0, k, hp, 1.0, 1.0)
-            dist.all_reduce(ops.grad, op=dist.ReduceOp.SUM)
+            self._kernel_grad(cols + (pg_adv.reshape(n), vs.reshape(n)), k, hp, 1.0)
             ops.adam(self.policy.flat, c["lr"], 1.0, c["grad_clip"])
-        st = ops.stats
-        g = self._global_means({"policy_loss": st[0], "vf_loss": st[1], "entropy": st[3], "total_loss": st[4],
-                                "gn": ops.grad.norm(), "_episode_reward_mean": buf.reward.sum(0).mean()})
-        return {"policy_loss": g["policy_loss"] * w, "vf_loss": g["vf_loss"] * w, "entropy": g["entropy"] * w,
-                "total_loss": g["total_loss"] * w, "grad_gnorm": g["gn"], "_episode_reward_mean": g["_episode_reward_mean"]}
+        return self._kernel_stats(buf, ops.grad.norm())
 
 
 class GaussPGTrainer(PGTrainer):
@@ -997,61 +989,61 @@ class ReplayBuffer(object):
         return self.obs[idx], self.action[idx], self.reward[idx], self.new_obs[idx], self.done[idx]
 
 
-class DDPGKernelOps(object):
-    """ctypes front of the DDPG / TD3 kernels (include/rl4rs_b200.h: r4_ddpg_* / r4_replay_*): the moments m, v of both
-    Adams (one buffer, split by region), the learner scratch for n samples per step, the loss statistics."""
+class _ReplayOps(_LearnerOps):
+    """_LearnerOps with what the replay learners add: the TD errors of one SGD step over n samples, 3 loss statistics, and
+    the sampling and priority kernels of the device replay (include/rl4rs_b200.h: r4_replay_*)."""
 
-    def __init__(self, D, twin, device, n_params, n):
-        from . import _capi
-        self.capi, self.lib = _capi, _capi.load_library()
-        self.D, self.twin, self.device, self.n, self.np = D, int(bool(twin)), device, n, n_params
-        assert self.lib.r4_ddpg_num_params(D, self.twin) == n_params
-        z = lambda k: torch.zeros(k, dtype=torch.float32, device=device)
-        self.m, self.v, self.stats = z(n_params), z(n_params), z(3)
-        self.grad, self.td = z(n_params), z(n)
-        self.scratch = z(self.lib.r4_ddpg_scratch_size(D, self.twin, n))
-        self._launch0 = self.lib.r4_learner_launch_count()
-
-    _stream = KernelOps._stream
-    _check = KernelOps._check
-    launches = KernelOps.launches
-
-    def act(self, flat, obs, mode, seed, counter, ou_in, ou_out, theta, sigma, ns, action):
-        rc = self.lib.r4_ddpg_act(_p(flat), _p(obs), obs.shape[0], self.D, mode, seed, counter, _p(ou_in), _p(ou_out), theta,
-                                  sigma, ns, _p(action), self._stream())
-        self._check(rc, "r4_ddpg_act")
+    def __init__(self, device, n_params, n, n_scratch):
+        super().__init__(device, n_params, 3, n_scratch)
+        self.td = torch.zeros(n, dtype=torch.float32, device=device)
 
     def _replay(self, rb):
-        return _p(rb.obs), _p(rb.action), _p(rb.reward), _p(rb.new_obs), _p(rb.done)
-
-    def replay_store(self, rb, obs, final_obs, action, reward, done):
-        T, B = reward.shape
-        rc = self.lib.r4_replay_store(*self._replay(rb), _p(rb.prio), _p(rb.max_prio), rb.C, self.D, rb.added, rb.alpha,
-                                      _p(obs), _p(final_obs), _p(action), _p(reward), _p(done), T, B, self._stream())
-        self._check(rc, "r4_replay_store")
+        return ptr(rb.obs), ptr(rb.action), ptr(rb.reward), ptr(rb.new_obs), ptr(rb.done)
 
     def replay_sample(self, rb, u, beta):
         n = u.shape[0]
         idx = torch.empty(n, dtype=torch.int64, device=self.device)
         w = torch.empty(n, dtype=torch.float32, device=self.device)
-        rc = self.lib.r4_replay_sample(_p(rb.prio), rb.size, n, beta, _p(u), _p(idx), _p(w), self._stream())
+        rc = self.lib.r4_replay_sample(ptr(rb.prio), rb.size, n, beta, ptr(u), ptr(idx), ptr(w), self._stream())
         self._check(rc, "r4_replay_sample")
         return idx, w
 
     def replay_priorities(self, rb, idx, td, eps):
-        rc = self.lib.r4_replay_update_priorities(_p(rb.prio), _p(rb.max_prio), _p(idx), _p(td), idx.shape[0], rb.alpha, eps,
+        rc = self.lib.r4_replay_update_priorities(ptr(rb.prio), ptr(rb.max_prio), ptr(idx), ptr(td), idx.shape[0], rb.alpha, eps,
                                                   self._stream())
         self._check(rc, "r4_replay_update_priorities")
 
+
+class DDPGKernelOps(_ReplayOps):
+    """ctypes front of the DDPG / TD3 kernels (include/rl4rs_b200.h: r4_ddpg_* / r4_replay_*): the moments m, v of both
+    Adams (one buffer, split by region), the learner scratch for n samples per step, the loss statistics."""
+
+    def __init__(self, D, twin, device, n_params, n):
+        self.D, self.twin = D, int(bool(twin))
+        lib = _capi.load_library()
+        assert lib.r4_ddpg_num_params(D, self.twin) == n_params
+        super().__init__(device, n_params, n, lib.r4_ddpg_scratch_size(D, self.twin, n))
+
+    def act(self, flat, obs, mode, seed, counter, ou_in, ou_out, theta, sigma, ns, action):
+        rc = self.lib.r4_ddpg_act(ptr(flat), ptr(obs), obs.shape[0], self.D, mode, seed, counter, ptr(ou_in), ptr(ou_out), theta,
+                                  sigma, ns, ptr(action), self._stream())
+        self._check(rc, "r4_ddpg_act")
+
+    def replay_store(self, rb, obs, final_obs, action, reward, done):
+        T, B = reward.shape
+        rc = self.lib.r4_replay_store(*self._replay(rb), ptr(rb.prio), ptr(rb.max_prio), rb.C, self.D, rb.added, rb.alpha,
+                                      ptr(obs), ptr(final_obs), ptr(action), ptr(reward), ptr(done), T, B, self._stream())
+        self._check(rc, "r4_replay_store")
+
     def grad_(self, pol, rb, idx, weights, noise, hp, inv_n):
         """self.grad, self.td, self.stats = r4_ddpg_grad over replay rows idx."""
-        rc = self.lib.r4_ddpg_grad(_p(pol.flat), _p(pol.target), self.D, self.twin, *self._replay(rb), _p(idx), _p(weights),
-                                   _p(noise), idx.shape[0], hp["gamma"], hp["target_noise"], hp["noise_clip"], inv_n,
-                                   _p(self.scratch), _p(self.grad), _p(self.td), _p(self.stats), self._stream())
+        rc = self.lib.r4_ddpg_grad(ptr(pol.flat), ptr(pol.target), self.D, self.twin, *self._replay(rb), ptr(idx), ptr(weights),
+                                   ptr(noise), idx.shape[0], hp["gamma"], hp["target_noise"], hp["noise_clip"], inv_n,
+                                   ptr(self.scratch), ptr(self.grad), ptr(self.td), ptr(self.stats), self._stream())
         self._check(rc, "r4_ddpg_grad")
 
     def apply(self, pol, actor_step, critic_step, hp, grad_scale=1.0):
-        rc = self.lib.r4_ddpg_apply(_p(pol.flat), _p(pol.target), _p(self.grad), _p(self.m), _p(self.v), self.D, self.twin,
+        rc = self.lib.r4_ddpg_apply(ptr(pol.flat), ptr(pol.target), ptr(self.grad), ptr(self.m), ptr(self.v), self.D, self.twin,
                                     actor_step, critic_step, hp["actor_lr"], hp["critic_lr"], hp["l2_reg"], hp["tau"],
                                     grad_scale, self._stream())
         self._check(rc, "r4_ddpg_apply")
@@ -1059,43 +1051,114 @@ class DDPGKernelOps(object):
     def train_step(self, comm, pol, rb, u, noise, actor_step, critic_step, hp):
         """One whole SGD step in one library call (sample, gradient, exchange over peer memory, Adams + soft update,
         priorities)."""
-        rc = self.lib.r4_ddpg_train_step(comm.h if comm is not None else None, _p(pol.flat), _p(pol.target), _p(self.m),
-                                         _p(self.v), self.D, self.twin, *self._replay(rb), _p(rb.prio), _p(rb.max_prio),
-                                         rb.size, u.shape[0], _p(u), _p(noise), hp["beta"], rb.alpha, hp["eps"], hp["gamma"],
+        rc = self.lib.r4_ddpg_train_step(comm.h if comm is not None else None, ptr(pol.flat), ptr(pol.target), ptr(self.m),
+                                         ptr(self.v), self.D, self.twin, *self._replay(rb), ptr(rb.prio), ptr(rb.max_prio),
+                                         rb.size, u.shape[0], ptr(u), ptr(noise), hp["beta"], rb.alpha, hp["eps"], hp["gamma"],
                                          hp["target_noise"], hp["noise_clip"], actor_step, critic_step, hp["actor_lr"],
-                                         hp["critic_lr"], hp["l2_reg"], hp["tau"], _p(self.scratch), _p(self.stats),
+                                         hp["critic_lr"], hp["l2_reg"], hp["tau"], ptr(self.scratch), ptr(self.stats),
                                          self._stream())
         self._check(rc, "r4_ddpg_train_step")
 
 
-class DDPGTrainer(_TrainerBase):
-    """DDPG (RLlib 1.5 DDPGTrainer as modelfree_train.py configures it) over the deterministic actor-critic of the
-    continuous-action env: rollout -> store in the replay -> one SGD step per stored vector episode once `learning_starts`
-    transitions were stored (RLlib's 1:1 round robin); an iteration rolls episodes until it sampled
-    `timesteps_per_iteration`.  On CUDA: the act kernel, the replay kernels and r4_ddpg_train_step (no host round trip per
-    step); on CPU the torch twin.  Data parallel: every rank keeps its own replay and OU state and samples
-    train_batch_size / world per step; the gradient is summed over the ranks (peer memory, or NCCL / gloo all-reduce).
-    The replay is not checkpointed (RLlib 1.5's default): after restore, learning waits for `learning_starts` again."""
-    algo = "DDPG"
-    DEFAULTS = DDPG_DEFAULTS
-    STATS = ("critic_loss", "actor_loss", "mean_q")     # the names of sgd_step's three statistics in train()'s result
+class _ReplayTrainer(_TrainerBase):
+    """The schedule of the replay learners (DDPG / TD3 and RAINBOW, RLlib 1.5's as modelfree_train.py configures them):
+    rollout -> store in the replay -> one SGD step per stored vector episode once `learning_starts` transitions were stored
+    (RLlib's 1:1 round robin); an iteration rolls episodes until it sampled `timesteps_per_iteration`.  Data parallel:
+    every rank keeps its own replay and samples train_batch_size / world per step; the gradient is summed over the ranks
+    (peer memory, or NCCL / gloo all-reduce).  The replay is not checkpointed (RLlib 1.5's default): after restore,
+    learning waits for `learning_starts` again.  A subclass builds its policy, ops, comm, replay and optimisers after this
+    constructor, and gives the action buffer (_actions), the act rule (_act), _hp, draws, sgd_step and twin_step."""
 
     def __init__(self, config, env, device=None, seed=0):
         cfg = config or {}
         self.config = c = dict(self.DEFAULTS, **{k: v for k, v in cfg.items() if k in self.DEFAULTS})
         self.env = env
         self.T, self.B = env.config["max_steps"], env.config["batch_size"]
-        self.D = env.config.get("action_emb_size", 32)
         self.device = torch.device(device) if device is not None else env.sim.engine.device
-        world = _world()
-        rank = dist.get_rank() if world > 1 else 0
-        ex = dict(self.DEFAULTS["exploration_config"] or {}, **(cfg.get("exploration_config") or {}))
-        self.ou = dict(OU_DEFAULTS, **{k: v for k, v in ex.items() if k != "type"}) \
-            if ex.get("type") == "OrnsteinUhlenbeckNoise" else None
-        self.policy = DeterministicActorCritic(self.D, self.device, seed=seed, twin=c["twin_q"])
+        world, rank = _world(), _rank()
         tb = c["train_batch_size"] or min(self.B * world * self.T, 1024)
         self.n_local = max(1, tb // world)
         self.use_kernels = self.device.type == "cuda" and cfg.get("use_kernels", True)
+        z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=self.device)
+        self.buf_obs, self.buf_action, self.buf_reward = z(self.T, self.B, 256), self._actions(self.T, self.B), z(self.T, self.B)
+        self.buf_done, self.final_obs = z(self.T, self.B, dt=torch.uint8), z(self.B, 256)
+        # exploration draws are per rank; the sampling / smoothing draws come from a per-rank generator on the device
+        self._seed = (seed * 1000003 + rank) & 0x7fffffffffffffff
+        self.gen = torch.Generator(device=self.device).manual_seed(seed * 1000003 + rank + 1)
+        self.counter = 0                    # draw counter of the act kernel
+        self.policy_ts = 0                  # global exploring timesteps: the exploration and target-copy schedules
+        self.iteration = self.timesteps_total = 0
+
+    @torch.no_grad()
+    def rollout(self, explore=True):
+        env = self.env
+        obs = env.reset()
+        for t in range(self.T):
+            self.buf_obs[t].copy_(self.policy.inputs(obs)[0])
+            a = self._act(self.buf_obs[t], explore, self.buf_action[t])
+            obs, reward, done, info = env.step(a)
+            self.buf_reward[t].copy_(reward)
+            self.buf_done[t].copy_(torch.as_tensor(done))
+        self.final_obs.copy_(self.policy.inputs(obs)[0])
+        self.reward = self.buf_reward
+        return self
+
+    @torch.no_grad()
+    def compute_actions(self, obs, explore=False):
+        if isinstance(obs, dict) and "obs" not in obs:                 # RLlib's {env_id: observation} form
+            return super().compute_actions(obs, explore)
+        o = torch.as_tensor(self.policy.inputs(obs)[0], dtype=torch.float32, device=self.device).contiguous()
+        return self._act(o, explore, self._actions(o.shape[0])).cpu().numpy()
+
+    def train(self):
+        c, w = self.config, _world()
+        sampled = steps = 0
+        rew, stats = [], torch.zeros(3, dtype=torch.float64, device=self.device)
+        while sampled < c["timesteps_per_iteration"]:
+            self.rollout(explore=True)
+            self.replay.store(self.buf_obs, self.final_obs, self.buf_action, self.buf_reward, self.buf_done)
+            sampled += self.T * self.B * w
+            rew.append(self.buf_reward.sum(0).mean())
+            if self.replay.added * w >= c["learning_starts"]:
+                stats += self.sgd_step(*self.draws()).double()
+                steps += 1
+        self.iteration += 1
+        self.timesteps_total += sampled
+        g = self._global_means(dict({"_r": torch.stack(rew).mean()}, **{s: stats[i] for i, s in enumerate(self.STATS)}))
+        k = max(steps, 1) / w              # each rank's statistics are its share of the global mean
+        out = {"episode_reward_mean": g["_r"], "training_iteration": self.iteration, "timesteps_this_iter": sampled,
+               "timesteps_total": self.timesteps_total, "episodes_this_iter": len(rew) * self.B * w, "sgd_steps": steps,
+               "num_steps_trained": self.critic_steps * self.n_local * w, "replay_size": self.replay.size}
+        out.update({s: g[s] / k if steps else float("nan") for s in self.STATS})
+        return out
+
+    def _state(self, kernel_adam):
+        return {"target": self.policy.target.cpu(), "counter": self.counter, "policy_ts": self.policy_ts,
+                "gen": self.gen.get_state()}
+
+    def _load_state(self, st):
+        with torch.no_grad():
+            self.policy.target.copy_(st["target"].to(self.device))
+        self.gen.set_state(st["gen"])
+        self.counter, self.policy_ts = st["counter"], st["policy_ts"]
+
+
+class DDPGTrainer(_ReplayTrainer):
+    """DDPG (RLlib 1.5 DDPGTrainer as modelfree_train.py configures it) over the deterministic actor-critic of the
+    continuous-action env, on _ReplayTrainer's schedule.  On CUDA: the act kernel, the replay kernels and
+    r4_ddpg_train_step (no host round trip per step); on CPU the torch twin.  Every rank keeps its own OU state."""
+    algo = "DDPG"
+    DEFAULTS = DDPG_DEFAULTS
+    STATS = ("critic_loss", "actor_loss", "mean_q")     # the names of sgd_step's three statistics in train()'s result
+
+    def __init__(self, config, env, device=None, seed=0):
+        self.D = env.config.get("action_emb_size", 32)
+        super().__init__(config, env, device, seed)
+        c = self.config
+        ex = dict(self.DEFAULTS["exploration_config"] or {}, **((config or {}).get("exploration_config") or {}))
+        self.ou = dict(OU_DEFAULTS, **{k: v for k, v in ex.items() if k != "type"}) \
+            if ex.get("type") == "OrnsteinUhlenbeckNoise" else None
+        self.policy = DeterministicActorCritic(self.D, self.device, seed=seed, twin=c["twin_q"])
         self.ops = DDPGKernelOps(self.D, c["twin_q"], self.device, self.policy.n_params, self.n_local) if self.use_kernels else None
         self.comm = PeerComm(self.policy.n_params, self.device) if self.use_kernels else None
         self.replay = ReplayBuffer(c["buffer_size"], self.D, self.device, c["prioritized_replay"],
@@ -1105,18 +1168,13 @@ class DDPGTrainer(_TrainerBase):
         self._pc = torch.nn.Parameter(self.policy.flat.data[na:])
         self.opt_actor = torch.optim.Adam([self._pa], lr=c["actor_lr"])
         self.opt_critic = torch.optim.Adam([self._pc], lr=c["critic_lr"])
-        z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=self.device)
-        self.buf_obs, self.buf_action, self.buf_reward = z(self.T, self.B, 256), z(self.T, self.B, self.D), z(self.T, self.B)
-        self.buf_done, self.final_obs = z(self.T, self.B, dt=torch.uint8), z(self.B, 256)
-        self.ou_state = z(2, self.D)        # the OU state and its next value: the act kernel reads one, writes the other
+        # the OU state and its next value: the act kernel reads one, writes the other
+        self.ou_state = torch.zeros(2, self.D, dtype=torch.float32, device=self.device)
         self._ou_slot = 0
-        # exploration draws are per rank; the sampling / smoothing draws come from a per-rank generator on the device
-        self._seed = (seed * 1000003 + rank) & 0x7fffffffffffffff
-        self.gen = torch.Generator(device=self.device).manual_seed(seed * 1000003 + rank + 1)
-        self.counter = 0                    # draw counter of the act kernel
-        self.policy_ts = 0                  # global exploring timesteps: the OU scale / random-phase schedule
         self.actor_steps = self.critic_steps = 0
-        self.iteration = self.timesteps_total = 0
+
+    def _actions(self, *lead):
+        return torch.zeros(*lead, self.D, dtype=torch.float32, device=self.device)
 
     # ---- acting -------------------------------------------------------------------------------------------------
     def _ou_scale(self):
@@ -1151,28 +1209,6 @@ class DDPGTrainer(_TrainerBase):
         if explore:
             self.policy_ts += n * _world()
         return out
-
-    @torch.no_grad()
-    def rollout(self, explore=True):
-        env = self.env
-        obs = env.reset()
-        for t in range(self.T):
-            self.buf_obs[t].copy_(self.policy.inputs(obs)[0])
-            a = self._act(self.buf_obs[t], explore, self.buf_action[t])
-            obs, reward, done, info = env.step(a)
-            self.buf_reward[t].copy_(reward)
-            self.buf_done[t].copy_(torch.as_tensor(done))
-        self.final_obs.copy_(self.policy.inputs(obs)[0])
-        self.reward = self.buf_reward
-        return self
-
-    @torch.no_grad()
-    def compute_actions(self, obs, explore=False):
-        if isinstance(obs, dict) and "obs" not in obs:                 # RLlib's {env_id: observation} form
-            return super().compute_actions(obs, explore)
-        o = torch.as_tensor(self.policy.inputs(obs)[0], dtype=torch.float32, device=self.device).contiguous()
-        out = torch.empty(o.shape[0], self.D, dtype=torch.float32, device=self.device)
-        return self._act(o, explore, out).cpu().numpy()
 
     # ---- learning -----------------------------------------------------------------------------------------------
     def _hp(self):
@@ -1233,55 +1269,18 @@ class DDPGTrainer(_TrainerBase):
         pol.soft_update(c["tau"])
         return td, torch.stack([cl.detach(), al.detach(), -al.detach()])
 
-    def train(self):
-        c, w = self.config, _world()
-        sampled = steps = 0
-        rew, stats = [], torch.zeros(3, dtype=torch.float64, device=self.device)
-        while sampled < c["timesteps_per_iteration"]:
-            self.rollout(explore=True)
-            self.replay.store(self.buf_obs, self.final_obs, self.buf_action, self.buf_reward, self.buf_done)
-            sampled += self.T * self.B * w
-            rew.append(self.buf_reward.sum(0).mean())
-            if self.replay.added * w >= c["learning_starts"]:
-                stats += self.sgd_step(*self.draws()).double()
-                steps += 1
-        self.iteration += 1
-        self.timesteps_total += sampled
-        g = self._global_means(dict({"_r": torch.stack(rew).mean()}, **{s: stats[i] for i, s in enumerate(self.STATS)}))
-        k = max(steps, 1) / w              # each rank's statistics are its share of the global mean
-        out = {"episode_reward_mean": g["_r"], "training_iteration": self.iteration, "timesteps_this_iter": sampled,
-               "timesteps_total": self.timesteps_total, "episodes_this_iter": len(rew) * self.B * w, "sgd_steps": steps,
-               "num_steps_trained": self.critic_steps * self.n_local * w, "replay_size": self.replay.size}
-        out.update({s: g[s] / k if steps else float("nan") for s in self.STATS})
-        return out
+    def _state(self, kernel_adam):
+        return dict(super()._state(kernel_adam), opt_actor=self.opt_actor.state_dict(), opt_critic=self.opt_critic.state_dict(),
+                    ou_state=self.ou_state.cpu(), ou_slot=self._ou_slot, actor_steps=self.actor_steps,
+                    critic_steps=self.critic_steps)
 
-    # ---- checkpoint ---------------------------------------------------------------------------------------------
-    def save(self, checkpoint_dir):
-        os.makedirs(checkpoint_dir, exist_ok=True)
-        path = os.path.join(checkpoint_dir, "checkpoint_%06d.pt" % self.iteration)
-        kst = {"m": self.ops.m.cpu(), "v": self.ops.v.cpu()} if self.use_kernels else None
-        torch.save({"algo": self.algo, "flat": self.policy.flat.detach().cpu(), "target": self.policy.target.cpu(),
-                    "opt_actor": self.opt_actor.state_dict(), "opt_critic": self.opt_critic.state_dict(), "kernel_adam": kst,
-                    "ou_state": self.ou_state.cpu(), "ou_slot": self._ou_slot, "counter": self.counter,
-                    "policy_ts": self.policy_ts, "actor_steps": self.actor_steps, "critic_steps": self.critic_steps,
-                    "gen": self.gen.get_state(), "iteration": self.iteration, "timesteps_total": self.timesteps_total}, path)
-        return path
-
-    def restore(self, path):
-        st = torch.load(path, map_location="cpu")
-        assert st["algo"] == self.algo
+    def _load_state(self, st):
+        super()._load_state(st)
         with torch.no_grad():
-            self.policy.flat.copy_(st["flat"].to(self.device))
-            self.policy.target.copy_(st["target"].to(self.device))
             self.ou_state.copy_(st["ou_state"].to(self.device))
         self.opt_actor.load_state_dict(st["opt_actor"])
         self.opt_critic.load_state_dict(st["opt_critic"])
-        if self.use_kernels and st.get("kernel_adam"):
-            self.ops.m.copy_(st["kernel_adam"]["m"]); self.ops.v.copy_(st["kernel_adam"]["v"])
-        self.gen.set_state(st["gen"])
-        for k in ("counter", "policy_ts", "actor_steps", "critic_steps", "iteration", "timesteps_total"):
-            setattr(self, k, st[k])
-        self._ou_slot = st["ou_slot"]
+        self._ou_slot, self.actor_steps, self.critic_steps = st["ou_slot"], st["actor_steps"], st["critic_steps"]
 
 
 class TD3Trainer(DDPGTrainer):
@@ -1302,50 +1301,38 @@ RAINBOW_DEFAULTS = {"gamma": 1.0, "lr": 5e-4, "adam_epsilon": 1e-8, "grad_clip":
                     "train_batch_size": None}
 
 
-class RainbowKernelOps(object):
+class RainbowKernelOps(_ReplayOps):
     """ctypes front of the RAINBOW kernels (include/rl4rs_b200.h: r4_rainbow_* / r4_replay_store_nstep, and the sampling
     and priority kernels of the DDPG replay): the Adam moments m, v, the learner scratch for n samples per step, the loss
     statistics."""
 
     def __init__(self, A, atoms, device, n_params, n):
-        from . import _capi
-        self.capi, self.lib = _capi, _capi.load_library()
-        self.A, self.atoms, self.device, self.n, self.np = A, atoms, device, n, n_params
-        assert self.lib.r4_rainbow_num_params(A, atoms) == n_params
-        z = lambda k: torch.zeros(k, dtype=torch.float32, device=device)
-        self.m, self.v, self.stats = z(n_params), z(n_params), z(3)
-        self.grad, self.td = z(n_params), z(n)
-        self.scratch = z(self.lib.r4_rainbow_scratch_size(A, atoms, n))
-        self._launch0 = self.lib.r4_learner_launch_count()
-
-    _stream = KernelOps._stream
-    _check = KernelOps._check
-    launches = KernelOps.launches
-    _replay = DDPGKernelOps._replay
-    replay_sample = DDPGKernelOps.replay_sample
-    replay_priorities = DDPGKernelOps.replay_priorities
+        self.A, self.atoms = A, atoms
+        lib = _capi.load_library()
+        assert lib.r4_rainbow_num_params(A, atoms) == n_params
+        super().__init__(device, n_params, n, lib.r4_rainbow_scratch_size(A, atoms, n))
 
     def act(self, pol, obs, explore, seed, counter, action, q=None):
-        rc = self.lib.r4_rainbow_act(_p(pol.flat), _p(obs), obs.shape[0], self.A, self.atoms, pol.v_min, pol.v_max,
-                                     int(bool(explore)), seed, counter, _p(action), _p(q), self._stream())
+        rc = self.lib.r4_rainbow_act(ptr(pol.flat), ptr(obs), obs.shape[0], self.A, self.atoms, pol.v_min, pol.v_max,
+                                     int(bool(explore)), seed, counter, ptr(action), ptr(q), self._stream())
         self._check(rc, "r4_rainbow_act")
 
     def replay_store(self, rb, obs, final_obs, action, reward, done):
         T, B = reward.shape
-        rc = self.lib.r4_replay_store_nstep(*self._replay(rb), _p(rb.prio), _p(rb.max_prio), rb.C, rb.added, rb.alpha,
-                                            rb.n_step, rb.gamma, _p(obs), _p(final_obs), _p(action), _p(reward), _p(done),
+        rc = self.lib.r4_replay_store_nstep(*self._replay(rb), ptr(rb.prio), ptr(rb.max_prio), rb.C, rb.added, rb.alpha,
+                                            rb.n_step, rb.gamma, ptr(obs), ptr(final_obs), ptr(action), ptr(reward), ptr(done),
                                             T, B, self._stream())
         self._check(rc, "r4_replay_store_nstep")
 
     def grad_(self, pol, rb, idx, weights, gamma_n, inv_n):
         """self.grad, self.td, self.stats = r4_rainbow_grad over replay rows idx."""
-        rc = self.lib.r4_rainbow_grad(_p(pol.flat), _p(pol.target), self.A, self.atoms, pol.v_min, pol.v_max,
-                                      *self._replay(rb), _p(idx), _p(weights), idx.shape[0], gamma_n, inv_n,
-                                      _p(self.scratch), _p(self.grad), _p(self.td), _p(self.stats), self._stream())
+        rc = self.lib.r4_rainbow_grad(ptr(pol.flat), ptr(pol.target), self.A, self.atoms, pol.v_min, pol.v_max,
+                                      *self._replay(rb), ptr(idx), ptr(weights), idx.shape[0], gamma_n, inv_n,
+                                      ptr(self.scratch), ptr(self.grad), ptr(self.td), ptr(self.stats), self._stream())
         self._check(rc, "r4_rainbow_grad")
 
     def apply(self, pol, step, hp, copy_target):
-        rc = self.lib.r4_rainbow_apply(_p(pol.flat), _p(pol.target), _p(self.grad), _p(self.m), _p(self.v), self.A,
+        rc = self.lib.r4_rainbow_apply(ptr(pol.flat), ptr(pol.target), ptr(self.grad), ptr(self.m), ptr(self.v), self.A,
                                        self.atoms, step, hp["lr"], hp["adam_eps"], hp["grad_clip"], int(copy_target),
                                        self._stream())
         self._check(rc, "r4_rainbow_apply")
@@ -1353,57 +1340,42 @@ class RainbowKernelOps(object):
     def train_step(self, comm, pol, rb, u, step, copy_target, hp):
         """One whole SGD step in one library call (sample, gradient, exchange over peer memory, clip + Adam + target copy,
         priorities)."""
-        rc = self.lib.r4_rainbow_train_step(comm.h if comm is not None else None, _p(pol.flat), _p(pol.target), _p(self.m),
-                                            _p(self.v), self.A, self.atoms, pol.v_min, pol.v_max, *self._replay(rb),
-                                            _p(rb.prio), _p(rb.max_prio), rb.size, u.shape[0], _p(u), hp["beta"], rb.alpha,
+        rc = self.lib.r4_rainbow_train_step(comm.h if comm is not None else None, ptr(pol.flat), ptr(pol.target), ptr(self.m),
+                                            ptr(self.v), self.A, self.atoms, pol.v_min, pol.v_max, *self._replay(rb),
+                                            ptr(rb.prio), ptr(rb.max_prio), rb.size, u.shape[0], ptr(u), hp["beta"], rb.alpha,
                                             hp["eps"], hp["gamma_n"], step, hp["lr"], hp["adam_eps"], hp["grad_clip"],
-                                            int(copy_target), _p(self.scratch), _p(self.stats), self._stream())
+                                            int(copy_target), ptr(self.scratch), ptr(self.stats), self._stream())
         self._check(rc, "r4_rainbow_train_step")
 
 
-class RainbowTrainer(DDPGTrainer):
+class RainbowTrainer(_ReplayTrainer):
     """RAINBOW (RLlib 1.5 DQNTrainer as modelfree_train.py configures it: distributional, dueling, double Q, n-step 3,
     prioritized replay, noisy off) over the plain observation of the discrete env, acting in Discrete(A) with SoftQ(T = 1)
-    exploration and argmax evaluation.  DDPGTrainer's schedule: rollout -> n-step store -> one SGD step per stored vector
-    episode once `learning_starts` transitions were stored; an iteration rolls episodes until it sampled
-    `timesteps_per_iteration`.  The target net is hard-copied after the SGD step at which target_network_update_freq
-    timesteps were sampled since the last copy (RLlib's UpdateTargetNetwork; the first step copies).  On CUDA: the act
-    kernel, the replay kernels and r4_rainbow_train_step; on CPU the torch twin.  Data parallel as DDPGTrainer: per-rank
-    replay, train_batch_size / world samples per rank, the gradient summed over the ranks before the per-tensor clip.
-    The replay is not checkpointed."""
+    exploration and argmax evaluation, on _ReplayTrainer's schedule with an n-step store.  The target net is hard-copied
+    after the SGD step at which target_network_update_freq timesteps were sampled since the last copy (RLlib's
+    UpdateTargetNetwork; the first step copies).  On CUDA: the act kernel, the replay kernels and r4_rainbow_train_step;
+    on CPU the torch twin.  The gradient is summed over the ranks before the per-tensor clip."""
     algo = "RAINBOW"
     DEFAULTS = RAINBOW_DEFAULTS
     STATS = ("loss", "mean_td_error", "mean_q")
 
     def __init__(self, config, env, device=None, seed=0):
-        cfg = config or {}
-        self.config = c = dict(self.DEFAULTS, **{k: v for k, v in cfg.items() if k in self.DEFAULTS})
-        self.env = env
-        self.T, self.B, self.A = env.config["max_steps"], env.config["batch_size"], env.config["action_size"]
-        self.device = torch.device(device) if device is not None else env.sim.engine.device
-        world = _world()
-        rank = dist.get_rank() if world > 1 else 0
+        super().__init__(config, env, device, seed)
+        c = self.config
+        self.A = env.config["action_size"]
         self.policy = DistributionalQNetwork(self.A, self.device, seed=seed, num_atoms=c["num_atoms"], v_min=c["v_min"],
                                              v_max=c["v_max"])
-        tb = c["train_batch_size"] or min(self.B * world * self.T, 1024)
-        self.n_local = max(1, tb // world)
-        self.use_kernels = self.device.type == "cuda" and cfg.get("use_kernels", True)
         self.ops = (RainbowKernelOps(self.A, c["num_atoms"], self.device, self.policy.n_params, self.n_local)
                     if self.use_kernels else None)
         self.comm = PeerComm(self.policy.n_params, self.device) if self.use_kernels else None
         self.replay = ReplayBuffer(c["buffer_size"], None, self.device, c["prioritized_replay"], c["prioritized_replay_alpha"],
                                    self.ops, n_step=c["n_step"], gamma=c["gamma"])
         self.opt = torch.optim.Adam([self.policy.flat], lr=c["lr"], eps=c["adam_epsilon"])
-        z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=self.device)
-        self.buf_obs, self.buf_action, self.buf_reward = z(self.T, self.B, 256), z(self.T, self.B, dt=torch.int32), z(self.T, self.B)
-        self.buf_done, self.final_obs = z(self.T, self.B, dt=torch.uint8), z(self.B, 256)
-        self._seed = (seed * 1000003 + rank) & 0x7fffffffffffffff
-        self.gen = torch.Generator(device=self.device).manual_seed(seed * 1000003 + rank + 1)
-        self.counter = 0                    # draw counter of the act kernel
-        self.policy_ts = 0                  # global exploring timesteps: RLlib's sampled-steps counter
         self.last_target_update = 0         # policy_ts at the last hard target copy
         self.critic_steps = 0               # SGD steps taken (the Adam step count)
-        self.iteration = self.timesteps_total = 0
+
+    def _actions(self, *lead):
+        return torch.zeros(*lead, dtype=torch.int32, device=self.device)
 
     @torch.no_grad()
     def _act(self, obs, explore, out):
@@ -1417,14 +1389,6 @@ class RainbowTrainer(DDPGTrainer):
         if explore:
             self.policy_ts += n * _world()
         return out
-
-    @torch.no_grad()
-    def compute_actions(self, obs, explore=False):
-        if isinstance(obs, dict) and "obs" not in obs:                 # RLlib's {env_id: observation} form
-            return _TrainerBase.compute_actions(self, obs, explore)
-        o = torch.as_tensor(self.policy.inputs(obs)[0], dtype=torch.float32, device=self.device).contiguous()
-        out = torch.empty(o.shape[0], dtype=torch.int32, device=self.device)
-        return self._act(o, explore, out).cpu().numpy()
 
     def _hp(self):
         c = self.config
@@ -1479,29 +1443,14 @@ class RainbowTrainer(DDPGTrainer):
                 pol.target.copy_(pol.flat.detach())
         return td, torch.stack([loss.detach(), td.sum() * inv_n, q])
 
-    def save(self, checkpoint_dir):
-        os.makedirs(checkpoint_dir, exist_ok=True)
-        path = os.path.join(checkpoint_dir, "checkpoint_%06d.pt" % self.iteration)
-        kst = {"m": self.ops.m.cpu(), "v": self.ops.v.cpu()} if self.use_kernels else None
-        torch.save({"algo": self.algo, "flat": self.policy.flat.detach().cpu(), "target": self.policy.target.cpu(),
-                    "opt": self.opt.state_dict(), "kernel_adam": kst, "counter": self.counter, "policy_ts": self.policy_ts,
-                    "last_target_update": self.last_target_update, "sgd_steps": self.critic_steps,
-                    "gen": self.gen.get_state(), "iteration": self.iteration, "timesteps_total": self.timesteps_total}, path)
-        return path
+    def _state(self, kernel_adam):
+        return dict(super()._state(kernel_adam), opt=self.opt.state_dict(), last_target_update=self.last_target_update,
+                    sgd_steps=self.critic_steps)
 
-    def restore(self, path):
-        st = torch.load(path, map_location="cpu")
-        assert st["algo"] == self.algo
-        with torch.no_grad():
-            self.policy.flat.copy_(st["flat"].to(self.device))
-            self.policy.target.copy_(st["target"].to(self.device))
+    def _load_state(self, st):
+        super()._load_state(st)
         self.opt.load_state_dict(st["opt"])
-        if self.use_kernels and st.get("kernel_adam"):
-            self.ops.m.copy_(st["kernel_adam"]["m"]); self.ops.v.copy_(st["kernel_adam"]["v"])
-        self.gen.set_state(st["gen"])
-        for k in ("counter", "policy_ts", "last_target_update", "iteration", "timesteps_total"):
-            setattr(self, k, st[k])
-        self.critic_steps = st["sgd_steps"]
+        self.last_target_update, self.critic_steps = st["last_target_update"], st["sgd_steps"]
 
 
 def get_rl_model(algo, rllib_config, env=None, **kw):

@@ -32,7 +32,8 @@ def main():
     g.build()
     from rl4rs_b200 import synth, gymshim, _capi
     from rl4rs_b200.env.slate import SlateRecEnv, SlateState
-    from rl4rs_b200.trainer import PPOTrainer, PeerComm, _p
+    from rl4rs_b200._capi import ptr as _p
+    from rl4rs_b200.trainer import PPOTrainer, PeerComm
     lib = _capi.load_library()
     out = {"world": world}
 
