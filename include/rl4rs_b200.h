@@ -570,6 +570,31 @@ int r4_simtrain_step(int hash_size, float* params, float* grad, float* m, float*
 /* The forward without dropout -> probs f32[n, 2] (may be NULL); acc (may be NULL) accumulates as in r4_simtrain_grad. */
 int r4_simtrain_eval(int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n, void* scratch,
                      float* probs, double* acc, void* stream);
+/* ---- the slate-label heads on the same backbone (nets/dien_slate.py, nets/dien_slate_multiclass.py; supervised_train.py
+ * <train> <test> <model> dien_slate[_multiclass] 1).  head selects simulator_reward's width C and the loss:
+ *   R4_SIMHEAD_ITEM (C = 2): the r4_simtrain_* entry points above, exactly (they forward here).
+ *   R4_SIMHEAD_SLATE (C = 9): sigmoid output against the page's 9 clicks; binary cross-entropy from the logits (no clip),
+ *     mean over the 9 columns and the n samples.  acc f64[408] = the 405 of the item head (accuracy: binary accuracy at
+ *     0.5 per column; histograms over all 9 columns) then {TP, FP, FN} at p > 0.5.
+ *   R4_SIMHEAD_SLATE_MULTICLASS (C = 22): softmax output against the class sum_j y_j [1,2,4,1,2,4,1,2,4]_j; categorical
+ *     cross-entropy from the logits, mean over the n samples.  acc f64[3] = {loss sum, hits (first argmax == class), samples}.
+ * For the slate heads idx holds RECORD indices: sample s is record idx[s] (data_preprocess.py tfrecord_slate): cat = portrait
+ * ids + [sequence_id] + the 9 items + the pad id 0, dense = portrait dense + item features + 40 zeros.  The flat layout is the
+ * item head's with rew_w [256, C], rew_b [C]; scratch_size depends on the head.  Each entry point has the signature of its
+ * r4_simtrain_* namesake with head first; probs is f32[n, C].  Bad head, hash_size or n: -1 or R4_ERR_ARG, nothing written. */
+enum { R4_SIMHEAD_ITEM = 0, R4_SIMHEAD_SLATE = 1, R4_SIMHEAD_SLATE_MULTICLASS = 2 };
+int64_t r4_simtrain_head_num_params(int head, int hash_size);
+int64_t r4_simtrain_head_scratch_size(int head, int n);
+int r4_simtrain_head_grad(int head, int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n,
+                          uint64_t seed, uint64_t counter, float drop_rate, const uint8_t* keep_in, uint8_t* keep_out,
+                          void* scratch, float* grad, float* stats, double* acc, void* stream);
+int r4_simtrain_head_apply(int head, int hash_size, float* params, float* grad, float* m, float* v, int step, float lr,
+                           float beta1, float beta2, float eps, void* stream);
+int r4_simtrain_head_step(int head, int hash_size, float* params, float* grad, float* m, float* v, const r4_simtrain_data* data,
+                          const int64_t* idx, int n, uint64_t seed, uint64_t counter, float drop_rate, int step, float lr,
+                          float beta1, float beta2, float eps, void* scratch, float* stats, double* acc, void* stream);
+int r4_simtrain_head_eval(int head, int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n,
+                          void* scratch, float* probs, double* acc, void* stream);
 /* kernels launched so far by the r4_simtrain_* entry points in this process (the radix sort counted once) */
 int64_t r4_simtrain_launch_count(void);
 /* kernels launched so far by every learner entry point in this process (r4_policy_*, r4_gae, r4_adam_step, r4_ppo_epoch*,

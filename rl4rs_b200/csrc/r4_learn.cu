@@ -789,10 +789,16 @@ int r4_batchrl_act(int algo, int obs_dim, int action_size, const float* params, 
 int64_t r4_simtrain_launch_count(void) { return g_launches[FAM_SIMTRAIN].load(std::memory_order_relaxed); }
 
 static bool st_hash_ok(int H) { return H >= 1 && H <= r4st::MAXH; }
+static bool st_head_ok(int head) { return head >= 0 && head < r4st::NHEAD; }
 
-int64_t r4_simtrain_num_params(int hash_size) { return st_hash_ok(hash_size) ? r4st::make_layout(hash_size).n : -1; }
-
-int64_t r4_simtrain_scratch_size(int n) { return (n < 1 || n > r4st::MAXN) ? -1 : (int64_t)r4st::scratch_bytes(n); }
+int64_t r4_simtrain_head_num_params(int head, int hash_size) {
+  return st_head_ok(head) && st_hash_ok(hash_size) ? r4st::make_layout(hash_size, r4st::head_classes(head)).n : -1;
+}
+int64_t r4_simtrain_head_scratch_size(int head, int n) {
+  return (!st_head_ok(head) || n < 1 || n > r4st::MAXN) ? -1 : (int64_t)r4st::scratch_bytes(n, r4st::head_classes(head));
+}
+int64_t r4_simtrain_num_params(int hash_size) { return r4_simtrain_head_num_params(R4_SIMHEAD_ITEM, hash_size); }
+int64_t r4_simtrain_scratch_size(int n) { return r4_simtrain_head_scratch_size(R4_SIMHEAD_ITEM, n); }
 
 template <typename... P, typename... A>
 static int st_launch(const char* name, void (*kernel)(P...), dim3 grid, int threads, cudaStream_t st, A&&... args) {
@@ -815,12 +821,12 @@ static int st_gemm(bool tb, const float* A, int lda, const float* B, int ldb, co
 }
 
 // The forward with saved activations: gather, towers, both sequences (GRU-1, attention, AUGRU), the head and the loss.
-static int st_forward(const r4st::Layout& L, const float* prm, const r4st::Data& D, const int64_t* idx, int n, uint64_t seed,
-                      uint64_t counter, float rate, const uint8_t* keep_in, uint8_t* keep_out, const r4st::Planes& P,
+static int st_forward(int head, const r4st::Layout& L, const float* prm, const r4st::Data& D, const int64_t* idx, int n,
+                      uint64_t seed, uint64_t counter, float rate, const uint8_t* keep_in, uint8_t* keep_out, const r4st::Planes& P,
                       bool with_grad, float* stats, double* acc, float* probs, cudaStream_t st) {
   using namespace r4st;
-  const int R = n * T;
-  const GatherArgs ga{L, D, idx, n, seed, counter, rate, keep_in, keep_out};
+  const int R = n * T, C = head_classes(head);
+  const GatherArgs ga{L, D, idx, n, seed, counter, rate, keep_in, keep_out, head != HEAD_ITEM};
   int rc;
   if ((rc = st_launch("k_st_gather", k_st_gather, n, E, st, ga, prm, P))) return rc;
   const float* keep0 = P.keep;
@@ -846,8 +852,13 @@ static int st_forward(const r4st::Layout& L, const float* prm, const r4st::Data&
     if ((rc = st_launch("k_st_gru_fwd<256>", k_st_gru_fwd<HA>, (n + SB - 1) / SB, NTH, st, g2))) return rc;
   }
   if ((rc = st_gemm(false, P.allf, FEAT, prm + L.ow, OBS, prm + L.ob, P.O, OBS, n, OBS, FEAT, EP_ELU, st))) return rc;
-  if ((rc = st_gemm(false, P.O, OBS, prm + L.rw, 2, prm + L.rb, P.Z, 2, n, 2, OBS, EP_LIN, st))) return rc;
-  return st_launch("k_st_loss", k_st_loss, 1, NTH, st, D, idx, n, P.Z, with_grad ? P.dZ : nullptr, P.stats, stats, acc, probs);
+  if ((rc = st_gemm(false, P.O, OBS, prm + L.rw, C, prm + L.rb, P.Z, C, n, C, OBS, EP_LIN, st))) return rc;
+  float* dZ = with_grad ? P.dZ : nullptr;
+  if (head == HEAD_SLATE)
+    return st_launch("k_st_loss_slate<9>", k_st_loss_slate<NS>, 1, NTH, st, D, idx, n, P.Z, dZ, P.stats, stats, acc, probs);
+  if (head == HEAD_SLATE_MULTICLASS)
+    return st_launch("k_st_loss_slate<22>", k_st_loss_slate<NMC>, 1, NTH, st, D, idx, n, P.Z, dZ, P.stats, stats, acc, probs);
+  return st_launch("k_st_loss", k_st_loss, 1, NTH, st, D, idx, n, P.Z, dZ, P.stats, stats, acc, probs);
 }
 
 static r4ddpg::Job st_job(const float* X, int ldx, const float* Z, int M, int N, int64_t off) {
@@ -864,13 +875,13 @@ static int st_wgrad(r4ddpg::Jobs J, int njob, int rows, float* grad, cudaStream_
   return st_launch("k_ddpg_wgrad", r4ddpg::k_ddpg_wgrad, t, r4ddpg::NT, st, J, rows, grad, nullptr, nullptr, 0.f);
 }
 
-static int st_backward(const r4st::Layout& L, const float* prm, const r4st::Data& D, const int64_t* idx, int n,
+static int st_backward(int head, const r4st::Layout& L, const float* prm, const r4st::Data& D, const int64_t* idx, int n,
                        const r4st::Planes& P, float* grad, cudaStream_t st) {
   using namespace r4st;
-  const int R = n * T;
+  const int R = n * T, C = head_classes(head);
   int rc;
   // head: dO = dZ rew_w^T elu'(O); dAllf = dO obs_w^T; the dense tower's columns again with its activation and dropout
-  if ((rc = st_gemm(true, P.dZ, 2, prm + L.rw, 2, nullptr, P.dO, OBS, n, OBS, 2, EP_DELU, st, P.O))) return rc;
+  if ((rc = st_gemm(true, P.dZ, C, prm + L.rw, C, nullptr, P.dO, OBS, n, OBS, C, EP_DELU, st, P.O))) return rc;
   if ((rc = st_gemm(true, P.dO, OBS, prm + L.ow, OBS, nullptr, P.dAllf, FEAT, n, FEAT, OBS, EP_LIN, st))) return rc;
   if ((rc = st_gemm(true, P.dO, OBS, prm + L.ow + (int64_t)F_DENSE * OBS, OBS, nullptr, P.dT2, U, n, U, OBS, EP_DELU, st, P.T2,
                     P.keep + (size_t)n * U)))
@@ -904,7 +915,7 @@ static int st_backward(const r4st::Layout& L, const float* prm, const r4st::Data
   J.j[k++] = st_job(P.dense, ND, P.dT1, ND, U, L.dw1);  J.j[k++] = st_job(nullptr, 1, P.dT1, 1, U, L.db1);
   J.j[k++] = st_job(P.T1d, U, P.dT2, U, U, L.dw2);      J.j[k++] = st_job(nullptr, 1, P.dT2, 1, U, L.db2);
   J.j[k++] = st_job(P.allf, FEAT, P.dO, FEAT, OBS, L.ow); J.j[k++] = st_job(nullptr, 1, P.dO, 1, OBS, L.ob);
-  J.j[k++] = st_job(P.O, OBS, P.dZ, OBS, 2, L.rw);      J.j[k++] = st_job(nullptr, 1, P.dZ, 1, 2, L.rb);
+  J.j[k++] = st_job(P.O, OBS, P.dZ, OBS, C, L.rw);      J.j[k++] = st_job(nullptr, 1, P.dZ, 1, C, L.rb);
   if ((rc = st_wgrad(J, k, n, grad, st))) return rc;
   for (int i = 0; i < 2; ++i) {
     const Seq& w = L.s[i];
@@ -926,7 +937,8 @@ static int st_backward(const r4st::Layout& L, const float* prm, const r4st::Data
   // embedding gradients: keys, a stable radix sort by (table, id), one ordered sum per run
   const int total = n * NSLOT;
   if ((rc = st_launch("k_st_dq", k_st_dq, (n * E + 255) / 256, 256, st, P.sp[0].dq, P.sp[1].dq, P.dqs, n))) return rc;
-  if ((rc = st_launch("k_st_embkeys", k_st_embkeys, (total + 255) / 256, 256, st, L, D, idx, n, P.cat, P.keys, P.vals))) return rc;
+  if ((rc = st_launch("k_st_embkeys", k_st_embkeys, (total + 255) / 256, 256, st, L, D, idx, n, (int)(head != HEAD_ITEM), P.cat, P.keys,
+                       P.vals))) return rc;
   int bits = 1;
   while (bits < 32 && ((uint64_t)1 << bits) < (uint64_t)(2 * L.H)) ++bits;
   cub::DoubleBuffer<uint32_t> kb(P.keys, P.keys2);
@@ -942,49 +954,76 @@ static int st_backward(const r4st::Layout& L, const float* prm, const r4st::Data
                    P.sp[1].dX, P.dqs, grad);
 }
 
-static int st_apply(int H, float* params, float* grad, float* m, float* v, int step, float lr, float b1, float b2, float eps,
-                    cudaStream_t st) {
-  const r4st::Layout L = r4st::make_layout(H);
+static int st_apply(int head, int H, float* params, float* grad, float* m, float* v, int step, float lr, float b1, float b2,
+                    float eps, cudaStream_t st) {
+  const r4st::Layout L = r4st::make_layout(H, r4st::head_classes(head));
   const double alpha = (double)lr * std::sqrt(1.0 - std::pow((double)b2, step)) / (1.0 - std::pow((double)b1, step));
   return st_launch("k_st_apply", r4st::k_st_apply, (unsigned)((L.n + 255) / 256), 256, st, L, params, grad, m, v, (float)alpha,
                    b1, b2, eps);
 }
 
+int r4_simtrain_head_grad(int head, int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n,
+                          uint64_t seed, uint64_t counter, float drop_rate, const uint8_t* keep_in, uint8_t* keep_out,
+                          void* scratch, float* grad, float* stats, double* acc, void* stream) {
+  if (!st_head_ok(head) || !st_hash_ok(hash_size) || !params || !st_data_ok(data) || !idx || n < 1 || n > r4st::MAXN ||
+      !(drop_rate >= 0.f) || !(drop_rate < 1.f) || !scratch || !grad)
+    return fail(R4_ERR_ARG, "r4_simtrain_grad: bad argument (head 0..2, hash_size 1..4000000, n 1..4096, drop_rate in [0, 1))");
+  const int C = r4st::head_classes(head);
+  const r4st::Layout L = r4st::make_layout(hash_size, C);
+  const r4st::Planes P = r4st::make_planes(scratch, n, C);
+  const r4st::Data D = st_data(data);
+  cudaStream_t st = S(stream);
+  int rc = st_forward(head, L, params, D, idx, n, seed, counter, drop_rate, keep_in, keep_out, P, true, stats, acc, nullptr, st);
+  return rc ? rc : st_backward(head, L, params, D, idx, n, P, grad, st);
+}
+
+int r4_simtrain_head_apply(int head, int hash_size, float* params, float* grad, float* m, float* v, int step, float lr,
+                           float beta1, float beta2, float eps, void* stream) {
+  if (!st_head_ok(head) || !st_hash_ok(hash_size) || !params || !grad || !m || !v || step < 1)
+    return fail(R4_ERR_ARG, "r4_simtrain_apply: bad argument");
+  return st_apply(head, hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, S(stream));
+}
+
+int r4_simtrain_head_step(int head, int hash_size, float* params, float* grad, float* m, float* v, const r4_simtrain_data* data,
+                          const int64_t* idx, int n, uint64_t seed, uint64_t counter, float drop_rate, int step, float lr,
+                          float beta1, float beta2, float eps, void* scratch, float* stats, double* acc, void* stream) {
+  if (!m || !v || step < 1) return fail(R4_ERR_ARG, "r4_simtrain_step: bad argument");
+  int rc = r4_simtrain_head_grad(head, hash_size, params, data, idx, n, seed, counter, drop_rate, nullptr, nullptr, scratch, grad,
+                                 stats, acc, stream);
+  return rc ? rc : st_apply(head, hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, S(stream));
+}
+
+int r4_simtrain_head_eval(int head, int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n,
+                          void* scratch, float* probs, double* acc, void* stream) {
+  if (!st_head_ok(head) || !st_hash_ok(hash_size) || !params || !st_data_ok(data) || !idx || n < 1 || n > r4st::MAXN || !scratch)
+    return fail(R4_ERR_ARG, "r4_simtrain_eval: bad argument");
+  const int C = r4st::head_classes(head);
+  const r4st::Layout L = r4st::make_layout(hash_size, C);
+  const r4st::Planes P = r4st::make_planes(scratch, n, C);
+  return st_forward(head, L, params, st_data(data), idx, n, 0, 0, 0.f, nullptr, nullptr, P, false, nullptr, acc, probs, S(stream));
+}
+
+// the item head's entry points
 int r4_simtrain_grad(int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n, uint64_t seed,
                      uint64_t counter, float drop_rate, const uint8_t* keep_in, uint8_t* keep_out, void* scratch, float* grad,
                      float* stats, double* acc, void* stream) {
-  if (!st_hash_ok(hash_size) || !params || !st_data_ok(data) || !idx || n < 1 || n > r4st::MAXN || !(drop_rate >= 0.f) ||
-      !(drop_rate < 1.f) || !scratch || !grad)
-    return fail(R4_ERR_ARG, "r4_simtrain_grad: bad argument (hash_size 1..4000000, n 1..4096, drop_rate in [0, 1))");
-  const r4st::Layout L = r4st::make_layout(hash_size);
-  const r4st::Planes P = r4st::make_planes(scratch, n);
-  const r4st::Data D = st_data(data);
-  cudaStream_t st = S(stream);
-  int rc = st_forward(L, params, D, idx, n, seed, counter, drop_rate, keep_in, keep_out, P, true, stats, acc, nullptr, st);
-  return rc ? rc : st_backward(L, params, D, idx, n, P, grad, st);
+  return r4_simtrain_head_grad(R4_SIMHEAD_ITEM, hash_size, params, data, idx, n, seed, counter, drop_rate, keep_in, keep_out,
+                               scratch, grad, stats, acc, stream);
 }
 
 int r4_simtrain_apply(int hash_size, float* params, float* grad, float* m, float* v, int step, float lr, float beta1, float beta2,
                       float eps, void* stream) {
-  if (!st_hash_ok(hash_size) || !params || !grad || !m || !v || step < 1)
-    return fail(R4_ERR_ARG, "r4_simtrain_apply: bad argument");
-  return st_apply(hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, S(stream));
+  return r4_simtrain_head_apply(R4_SIMHEAD_ITEM, hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, stream);
 }
 
 int r4_simtrain_step(int hash_size, float* params, float* grad, float* m, float* v, const r4_simtrain_data* data,
                      const int64_t* idx, int n, uint64_t seed, uint64_t counter, float drop_rate, int step, float lr, float beta1,
                      float beta2, float eps, void* scratch, float* stats, double* acc, void* stream) {
-  if (!m || !v || step < 1) return fail(R4_ERR_ARG, "r4_simtrain_step: bad argument");
-  int rc = r4_simtrain_grad(hash_size, params, data, idx, n, seed, counter, drop_rate, nullptr, nullptr, scratch, grad, stats, acc,
-                            stream);
-  return rc ? rc : st_apply(hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, S(stream));
+  return r4_simtrain_head_step(R4_SIMHEAD_ITEM, hash_size, params, grad, m, v, data, idx, n, seed, counter, drop_rate, step, lr,
+                               beta1, beta2, eps, scratch, stats, acc, stream);
 }
 
 int r4_simtrain_eval(int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n, void* scratch,
                      float* probs, double* acc, void* stream) {
-  if (!st_hash_ok(hash_size) || !params || !st_data_ok(data) || !idx || n < 1 || n > r4st::MAXN || !scratch)
-    return fail(R4_ERR_ARG, "r4_simtrain_eval: bad argument");
-  const r4st::Layout L = r4st::make_layout(hash_size);
-  const r4st::Planes P = r4st::make_planes(scratch, n);
-  return st_forward(L, params, st_data(data), idx, n, 0, 0, 0.f, nullptr, nullptr, P, false, nullptr, acc, probs, S(stream));
+  return r4_simtrain_head_eval(R4_SIMHEAD_ITEM, hash_size, params, data, idx, n, scratch, probs, acc, stream);
 }

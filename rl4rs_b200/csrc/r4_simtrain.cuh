@@ -17,6 +17,8 @@
 //   k_st_attin(_bwd) the DIN attention input [q, k, q - k, q k] and its backward (dq summed over t, dk into dH)
 //   k_st_loss        softmax output, Keras binary_crossentropy on one_hot(label, 2) with the clip, dlogits, the batch
 //                    statistics and the AUC histograms (one CTA, samples summed in order)
+//   k_st_loss_slate  the slate-label heads (nets/dien_slate.py, dien_slate_multiclass.py): 9 sigmoid columns against the
+//                    page's clicks, or a 22-way softmax against the click pattern's class; same one-CTA ordered sums
 //   k_st_cat_bwd     the category self-attention backward
 //   r4ddpg::k_ddpg_wgrad  every dW = X^T dZ and bias, one CTA per 64 x 64 tile walking the rows in order
 //   k_st_embkeys + a stable CUB radix sort + k_st_embsum   the two embedding tables' gradients: (table, id) keys of every
@@ -47,6 +49,14 @@ constexpr int MAXN = 4096;                      // samples per pass
 constexpr int MAXH = 4000000;                   // category_hash_size
 constexpr int NTH = 256;
 
+// ---- the heads: the item head of nets/dien.py and the two slate-label heads ----
+// A head sets the width C of simulator_reward ([OBS, C] + [C]) and whether a sample is (record idx / 9, item idx % 9) or the
+// record idx itself (the slate samples of data_preprocess.py tfrecord_slate: cat slot 20 and dense 392..431 are padding).
+enum { HEAD_ITEM = 0, HEAD_SLATE = 1, HEAD_SLATE_MULTICLASS = 2, NHEAD = 3 };
+constexpr int NS = 9;            // slate columns: one per exposed item
+constexpr int NMC = 22;          // click-pattern classes: sum_j y_j [1, 2, 4, 1, 2, 4, 1, 2, 4]_j in 0..21
+__host__ __device__ constexpr int head_classes(int head) { return head == HEAD_SLATE ? NS : head == HEAD_SLATE_MULTICLASS ? NMC : 2; }
+
 // ---- the flat parameter layout: tf_checkpoint.dien_layer_plan order ----
 struct Seq {
   int64_t gwg, gbg, gwc, gbc;                 // GRU-1: wg [2E, 2E], bg [2E], wc [2E, E], bc [E]
@@ -59,7 +69,7 @@ struct Layout {
   Seq s[2];
   int64_t ow, ob, rw, rb, n;
 };
-__host__ __device__ inline Layout make_layout(int64_t H) {
+__host__ __device__ inline Layout make_layout(int64_t H, int C = 2) {
   Layout L;
   int64_t o = 0;
   auto take = [&](int64_t k) { int64_t r = o; o += k; return r; };
@@ -75,12 +85,13 @@ __host__ __device__ inline Layout make_layout(int64_t H) {
     s.uwg = take(3 * E * 4 * E); s.ubg = take(4 * E); s.uwc = take(3 * E * 2 * E); s.ubc = take(2 * E);
   }
   L.ow = take((int64_t)FEAT * OBS); L.ob = take(OBS);
-  L.rw = take(OBS * 2); L.rb = take(2);
+  L.rw = take(OBS * C); L.rb = take(C);
   L.n = o;
   return L;
 }
 
-// ---- the per-record sample store (ItemSamples): sample i is (record i / 9, exposed item i % 9) ----
+// ---- the per-record sample store (ItemSamples): item sample i is (record i / 9, exposed item i % 9), slate sample i is
+// record i ----
 struct Data {
   const int32_t* ucat;     // [N][10] portrait ids
   const float* udense;     // [N][32] portrait dense
@@ -112,8 +123,8 @@ __host__ inline size_t cub_reserve(int n) { return ((size_t)4 << 20) + (size_t)1
 
 // The planes are cut from the scratch in this order, each rounded up to 256 bytes, and the radix sort's reserve follows.
 // With base = nullptr only the offsets are formed: scratch_bytes is the end of the same cuts, so the size a caller
-// allocates and the layout a launch uses cannot disagree.
-__host__ inline Planes make_planes(void* base, int n) {
+// allocates and the layout a launch uses cannot disagree.  C is the head's width: the logits Z and dZ are [n][C].
+__host__ inline Planes make_planes(void* base, int n, int C = 2) {
   Planes P;
   const uintptr_t b = reinterpret_cast<uintptr_t>(base);
   size_t o = 0;
@@ -123,7 +134,7 @@ __host__ inline Planes make_planes(void* base, int n) {
   P.dense = take((size_t)n * ND); P.keep = take((size_t)n * 2 * U);
   P.T1 = take((size_t)n * U); P.T1d = take((size_t)n * U); P.T2 = take((size_t)n * U);
   P.allf = take((size_t)n * FEAT); P.P = take((size_t)n * NC * NC); P.q = take((size_t)n * E);
-  P.O = take((size_t)n * OBS); P.Z = take((size_t)n * 2); P.dZ = take((size_t)n * 2); P.dO = take((size_t)n * OBS);
+  P.O = take((size_t)n * OBS); P.Z = take((size_t)n * C); P.dZ = take((size_t)n * C); P.dO = take((size_t)n * OBS);
   P.dAllf = take((size_t)n * FEAT); P.dT1 = take((size_t)n * U); P.dT2 = take((size_t)n * U);
   P.dEcat = take((size_t)n * NC * E); P.dqs = take((size_t)n * E); P.stats = take((size_t)n * 2);
   for (int i = 0; i < 2; ++i) {
@@ -143,7 +154,7 @@ __host__ inline Planes make_planes(void* base, int n) {
   P.bytes = o + P.cub_bytes;
   return P;
 }
-__host__ inline size_t scratch_bytes(int n) { return make_planes(nullptr, n).bytes; }
+__host__ inline size_t scratch_bytes(int n, int C = 2) { return make_planes(nullptr, n, C).bytes; }
 
 __device__ __forceinline__ float sigm(float x) { return 1.f / (1.f + expf(-x)); }
 __device__ __forceinline__ float elu(float x) { return x > 0.f ? x : expm1f(x); }
@@ -156,7 +167,8 @@ __device__ __forceinline__ float drop_u(uint64_t seed, uint64_t counter, int s, 
 }
 
 // ------------------------------------------------------------------------------------------------
-// k_st_gather: one CTA (128 threads) per sample s of the batch (sample index idx[s]).
+// k_st_gather: one CTA (128 threads) per sample s of the batch (sample index idx[s]).  slate: the sample is record idx[s],
+// its cat slot 20 the pad id 0 and its dense features 392..431 zero (pad_sequences post-padding of tfrecord_slate's rows).
 // keep: keep_in != NULL -> keep_in[s][256] (u8, 1 = kept); else the draw of (seed, counter, s, unit) >= rate.  The keep
 // scale is 1 / (1 - rate) (inverted dropout); rate 0 keeps every unit at scale 1.  keep_out (may be NULL) receives the bits.
 // ------------------------------------------------------------------------------------------------
@@ -169,6 +181,7 @@ struct GatherArgs {
   float rate;
   const uint8_t* keep_in;
   uint8_t* keep_out;
+  int slate;
 };
 __global__ void __launch_bounds__(E) k_st_gather(GatherArgs g, const float* __restrict__ prm, Planes P) {
   __shared__ float Es[NC][E + 1];
@@ -176,18 +189,18 @@ __global__ void __launch_bounds__(E) k_st_gather(GatherArgs g, const float* __re
   __shared__ int ids[NC];
   __shared__ float w[NC];
   const int s = blockIdx.x, c = threadIdx.x;
-  const int64_t smp = g.idx[s], rec = smp / 9;
-  const int j = (int)(smp % 9);
+  const int64_t smp = g.idx[s], rec = g.slate ? smp : smp / 9;
+  const int j = g.slate ? -1 : (int)(smp % 9);
   const Data& D = g.D;
   const Layout& L = g.L;
   if (c < NC) {
-    int id = c < 10 ? D.ucat[rec * 10 + c] : c == 10 ? D.seqid[rec] : c < 20 ? D.items[rec * 9 + c - 11] : D.items[rec * 9 + j];
+    int id = c < 10 ? D.ucat[rec * 10 + c] : c == 10 ? D.seqid[rec] : c < 20 ? D.items[rec * 9 + c - 11] : j < 0 ? 0 : D.items[rec * 9 + j];
     id = clampid(id, L.H);
     ids[c] = id;
     P.cat[(size_t)s * NC + c] = id;
   }
   for (int k = c; k < ND; k += E) {
-    const float v = k < 32 ? D.udense[rec * 32 + k] : k < 392 ? D.ifeat[rec * 360 + k - 32] : D.ifeat[rec * 360 + j * 40 + k - 392];
+    const float v = k < 32 ? D.udense[rec * 32 + k] : k < 392 ? D.ifeat[rec * 360 + k - 32] : j < 0 ? 0.f : D.ifeat[rec * 360 + j * 40 + k - 392];
     P.dense[(size_t)s * ND + k] = v;
   }
   for (int u = c; u < 2 * U; u += E) {
@@ -603,6 +616,87 @@ __global__ void __launch_bounds__(NTH) k_st_loss(Data D, const int64_t* __restri
 }
 
 // ------------------------------------------------------------------------------------------------
+// k_st_loss_slate<C> (one CTA), sample s = record idx[s] with the page's clicks y[9]; Keras takes the logits path for a
+// Sigmoid / Softmax output (no clip, INTEGRATION.md section 8).
+//   C = 9:  p = sigmoid(z), loss = mean over the 9 columns and the batch of max(z, 0) - z y + log(1 + exp(-|z|)),
+//           dz = (p - y) / (9 n).  acc (may be NULL) f64[NACC_SLATE] accumulates {loss sum, binary accuracy sum, samples,
+//           positives[201], negatives[201] (the k_st_loss histograms over all 9 columns), TP, FP, FN at p > 0.5}.
+//   C = 22: class = sum_j y_j [1, 2, 4, 1, 2, 4, 1, 2, 4]_j, p = softmax(z), loss = mean of logsumexp(z) - z_class,
+//           dz = (p - one_hot(class)) / n.  acc f64[NACC_MC] accumulates {loss sum, hits, samples}: a hit is the first
+//           argmax of p (tf.argmax) at the class.
+// stats (may be NULL) f32[2] = {mean loss, mean binary accuracy | categorical accuracy}; probs (may be NULL) [n][C].
+// ------------------------------------------------------------------------------------------------
+constexpr int NACC_SLATE = NACC + 3, NACC_MC = 3;
+template <int C>
+__global__ void __launch_bounds__(NTH) k_st_loss_slate(Data D, const int64_t* __restrict__ idx, int n, const float* __restrict__ Z,
+                                                       float* __restrict__ dZ, float* __restrict__ srow, float* __restrict__ stats,
+                                                       double* __restrict__ acc, float* __restrict__ probs) {
+  __shared__ unsigned int hist[2][NBIN];
+  __shared__ unsigned int cnt[3];
+  const int tid = threadIdx.x;
+  for (int i = tid; i < 2 * NBIN; i += NTH) hist[i / NBIN][i % NBIN] = 0u;
+  if (tid < 3) cnt[tid] = 0u;
+  __syncthreads();
+  const float inv = 1.f / ((float)n * (C == NS ? (float)NS : 1.f));
+  for (int s = tid; s < n; s += NTH) {
+    const uint8_t* y = D.label + idx[s] * 9;
+    const float* z = Z + (size_t)s * C;
+    if constexpr (C == NS) {
+      float loss = 0.f, hit = 0.f;
+#pragma unroll
+      for (int j = 0; j < NS; ++j) {
+        const bool yj = y[j] != 0;
+        const float zj = z[j], e = expf(-fabsf(zj));
+        const float p = zj >= 0.f ? 1.f / (1.f + e) : e / (1.f + e);
+        loss += fmaxf(zj, 0.f) - (yj ? zj : 0.f) + log1pf(e);
+        if (dZ) dZ[(size_t)s * C + j] = (p - (yj ? 1.f : 0.f)) * inv;
+        if (probs) probs[(size_t)s * C + j] = p;
+        const bool pos = p > 0.5f;
+        hit += pos == yj ? 1.f : 0.f;
+        if (acc) {
+          atomicAdd(&hist[yj ? 0 : 1][auc_bin(p)], 1u);
+          if (pos || yj) atomicAdd(&cnt[pos ? (yj ? 0 : 1) : 2], 1u);
+        }
+      }
+      srow[2 * s] = loss / (float)NS;
+      srow[2 * s + 1] = hit / (float)NS;
+    } else {
+      int cls = 0;
+#pragma unroll
+      for (int j = 0; j < NS; ++j) cls += y[j] != 0 ? 1 << (j % 3) : 0;
+      float m = -INFINITY;
+#pragma unroll
+      for (int k = 0; k < C; ++k) m = fmaxf(m, z[k]);
+      float e[C], den = 0.f;
+#pragma unroll
+      for (int k = 0; k < C; ++k) { e[k] = expf(z[k] - m); den += e[k]; }
+      int am = 0;
+      float best = -1.f;
+#pragma unroll
+      for (int k = 0; k < C; ++k) {
+        const float p = e[k] / den;
+        if (p > best) { best = p; am = k; }
+        if (dZ) dZ[(size_t)s * C + k] = (p - (k == cls ? 1.f : 0.f)) * inv;
+        if (probs) probs[(size_t)s * C + k] = p;
+      }
+      srow[2 * s] = m + logf(den) - z[cls];
+      srow[2 * s + 1] = am == cls ? 1.f : 0.f;
+    }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    double l = 0.0, h = 0.0;
+    for (int s = 0; s < n; ++s) { l += srow[2 * s]; h += srow[2 * s + 1]; }
+    if (stats) { stats[0] = (float)(l / n); stats[1] = (float)(h / n); }
+    if (acc) { acc[0] += l; acc[1] += h; acc[2] += n; }
+  }
+  if (acc && C == NS) {
+    for (int i = tid; i < 2 * NBIN; i += NTH) acc[3 + i] += (double)hist[i / NBIN][i % NBIN];
+    if (tid < 3) acc[NACC + tid] += (double)cnt[tid];
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // k_st_cat_bwd: one CTA (128 threads) per sample.  c1 = (1/21) sum_i sum_j P_ij E_j; dE_j = d(flatten)_j
 //   + (w_j / 21) dc1 + sum_i dS_ij E_i + sum_i dS_ji E_i   with w_j = sum_i P_ij, a_j = (dc1 . E_j) / 21,
 //   dS_ij = P_ij (a_j - sum_k P_ik a_k).
@@ -653,9 +747,10 @@ __global__ void k_st_dq(const float* __restrict__ dq0, const float* __restrict__
 // ------------------------------------------------------------------------------------------------
 // The embedding gradients.  Entry e = s * NSLOT + k of sample s: k < 21 the emb_cat slot k (source row dEcat[s][k]);
 // 21 <= k < 149 emb_seq for sequence (k - 21) / 64, step (k - 21) % 64 (source dX); k >= 149 emb_seq of cat slot 11 + (k - 149)
-// (the query, source dqs[s]).  key = table * H + id; a stable radix sort keeps equal keys in (s, k) order.
+// (the query, source dqs[s]).  key = table * H + id; a stable radix sort keeps equal keys in (s, k) order.  slate: the
+// sequences are record idx[s]'s, and the pad id 0 of cat slot 20 (in the query too) keys row 0 like any other id.
 // ------------------------------------------------------------------------------------------------
-__global__ void k_st_embkeys(Layout L, Data D, const int64_t* __restrict__ idx, int n, const int32_t* __restrict__ cat,
+__global__ void k_st_embkeys(Layout L, Data D, const int64_t* __restrict__ idx, int n, int slate, const int32_t* __restrict__ cat,
                              uint32_t* __restrict__ keys, int32_t* __restrict__ vals) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= n * NSLOT) return;
@@ -665,7 +760,7 @@ __global__ void k_st_embkeys(Layout L, Data D, const int64_t* __restrict__ idx, 
     key = (uint32_t)cat[s * NC + k];
   } else if (k < NC + 2 * T) {
     const int i = (k - NC) / T, t = (k - NC) % T;
-    const int64_t rec = idx[s] / 9;
+    const int64_t rec = slate ? idx[s] : idx[s] / 9;
     key = (uint32_t)(L.H + clampid(D.seq[(rec * 2 + i) * T + t], L.H));
   } else {
     key = (uint32_t)(L.H + cat[s * NC + NC - 10 + (k - NC - 2 * T)]);

@@ -1,9 +1,10 @@
 """Time simulator training (csrc/r4_simtrain.cuh) on the GPU at the reference's sizes (category_hash_size 100000):
 ms per optimiser step at batch 256 and 1024 over back-to-back steps, with the launches per step (counted by the library)
 and samples/s; one steps_per_epoch epoch (2343 steps of 256) plus its validation (1562 batches); the torch twin's step on
-the same card; and peak device memory.  Prints the card name and power limit read in the same run.
+the same card; and peak device memory.  Prints the card name and power limit read in the same run.  --model dien_slate /
+dien_slate_multiclass times the slate-label nets instead (one sample per record, so samples/s reads records/s; no twin).
 
-    python tools/simtrain_time.py [--steps 50] [--epoch-steps 2343] [--val-steps 1562] [--records 20000]
+    python tools/simtrain_time.py [--model dien] [--steps 50] [--epoch-steps 2343] [--val-steps 1562] [--records 20000]
 """
 import argparse
 import os
@@ -26,6 +27,7 @@ def card():
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--model", default="dien", choices=["dien", "dien_slate", "dien_slate_multiclass"])
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--epoch-steps", type=int, default=600000 // 256)
     ap.add_argument("--val-steps", type=int, default=400000 // 256)
@@ -40,9 +42,14 @@ def main():
     print("card:", card())
     cfg = {"category_hash_size": 100000}
     samples = R.make_samples(a.records, 100000, seed=0)
+    slate = a.model != "dien"
+    if slate:
+        samples = simtrain.SlateSamples.view(samples)
+        print("model:", a.model)
+    unit = "records" if slate else "samples"
     lib = _capi.load_library()
     for B in (256, 1024):
-        tr = simtrain.SimulatorTrainer(cfg, device="cuda")
+        tr = simtrain.get_model(cfg, a.model, device="cuda")
         st = simtrain._Stream(len(samples), B, 0, torch.device("cuda"))
         for _ in range(3):
             tr.train_step(samples, st.next())
@@ -55,11 +62,13 @@ def main():
         torch.cuda.synchronize()
         dt = (time.perf_counter() - t) / a.steps
         launches = (lib.r4_simtrain_launch_count() - l0) / a.steps
-        print("batch %d: %.2f ms/step, %.0f launches/step, %.0f samples/s" % (B, dt * 1e3, launches, B / dt))
+        print("batch %d: %.2f ms/step, %.0f launches/step, %.0f %s/s" % (B, dt * 1e3, launches, B / dt, unit))
         del tr
     torch.cuda.reset_peak_memory_stats()
-    tr = simtrain.SimulatorTrainer(cfg, device="cuda")
+    tr = simtrain.get_model(cfg, a.model, device="cuda")
     test = R.make_samples(max(a.records // 4, 100), 100000, seed=1)
+    if slate:
+        test = simtrain.SlateSamples.view(test)
     torch.cuda.synchronize()
     t = time.perf_counter()
     h = tr.fit(samples, test, epochs=1, steps_per_epoch=a.epoch_steps, validation_steps=a.val_steps)
@@ -68,6 +77,8 @@ def main():
           % (a.epoch_steps, a.val_steps, time.perf_counter() - t, h["loss"][0], h["val_loss"][0]))
     print("peak device memory: %.2f GB" % (torch.cuda.max_memory_allocated() / 1e9))
     del tr
+    if slate:
+        return
     net = simtrain.SimulatorNet(cfg).cuda()
     m, v = torch.zeros_like(net.flat.data), torch.zeros_like(net.flat.data)
     idx = np.arange(256)
