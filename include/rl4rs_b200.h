@@ -595,6 +595,37 @@ int r4_simtrain_head_step(int head, int hash_size, float* params, float* grad, f
                           float beta1, float beta2, float eps, void* scratch, float* stats, double* acc, void* stream);
 int r4_simtrain_head_eval(int head, int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n,
                           void* scratch, float* probs, double* acc, void* stream);
+/* ---- the other backbones and adversarial_slate (nets/dnn*.py, widedeep*.py, lstm*.py, adversarial_slate.py).  net is
+ * an R4_SIM_* value or R4_SIMNET_ADVERSARIAL_SLATE; nets 0..3 take heads 0..2, net 4 only R4_SIMHEAD_ADVERSARIAL.  Each entry
+ * point takes the arguments of its r4_simtrain_head_* namesake after net; net R4_SIM_DIEN forwards to it unchanged.  A bad
+ * pair, hash_size or n: -1 or R4_ERR_ARG, nothing written.  The samples, keep bits, dropout, heads, acc layouts and Adam are
+ * the DIEN heads' (R4_SIMHEAD_ADVERSARIAL: the R4_SIMHEAD_SLATE acc layout, f64[408]).  The flat layouts, with H =
+ * hash_size, E = U = 128 and C the head's width (2, 9, 22; adversarial 9), in tf_checkpoint.*_layer_plan order:
+ *   dnn       emb_cat[H,E] dense_w1[432,128] dense_b1 dense_w2[128,128] dense_b2 fc_w[256,256] fc_b obs_w[256,256] obs_b
+ *             rew_w[256,C] rew_b[C]                                  (dnn.py's second Embedding feeds nothing: not held)
+ *   widedeep  emb_cat dense_w1 dense_b1 dense_w2 dense_b2 emb_seq[H,E] fc_w[256,256] fc_b rew_w[3072,C] rew_b[C]
+ *   lstm      emb_cat cgru_k[128,384] cgru_rk[128,384] cgru_b[384] dense_w1 dense_b1 dense_w2 dense_b2 emb_seq
+ *             sgru0_k sgru0_rk sgru0_b sgru1_k sgru1_rk sgru1_b obs_w[3200,256] obs_b rew_w[256,C] rew_b[C]
+ *   adversarial_slate  emb_cat dense_w1 dense_b1 dense_w2 dense_b2 emb_seq w[512,9] b[9]
+ * The lstm GRUs are Keras-v1 GRUs (hard sigmoid, reset_after = False, gates [z | r | h]; its slope is taken as 0.2 at both
+ * kinks).  adversarial_slate's loss per record: 0.1 mean_j BCE(y_j, sigmoid(z_j)) + sum_j softmax(sigmoid(z))_j (1 - y_j).
+ * Launches per step (grad + apply; the radix sort counted once): dnn 18, widedeep 17, lstm 34, adversarial_slate 14; eval:
+ * dnn 7, widedeep 6, lstm 12, adversarial_slate 5. */
+enum { R4_SIMNET_ADVERSARIAL_SLATE = 4 };
+enum { R4_SIMHEAD_ADVERSARIAL = 3 };
+int64_t r4_simtrain_net_num_params(int net, int head, int hash_size);
+int64_t r4_simtrain_net_scratch_size(int net, int head, int n);
+int r4_simtrain_net_grad(int net, int head, int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx,
+                         int n, uint64_t seed, uint64_t counter, float drop_rate, const uint8_t* keep_in, uint8_t* keep_out,
+                         void* scratch, float* grad, float* stats, double* acc, void* stream);
+int r4_simtrain_net_apply(int net, int head, int hash_size, float* params, float* grad, float* m, float* v, int step, float lr,
+                          float beta1, float beta2, float eps, void* stream);
+int r4_simtrain_net_step(int net, int head, int hash_size, float* params, float* grad, float* m, float* v,
+                         const r4_simtrain_data* data, const int64_t* idx, int n, uint64_t seed, uint64_t counter, float drop_rate,
+                         int step, float lr, float beta1, float beta2, float eps, void* scratch, float* stats, double* acc,
+                         void* stream);
+int r4_simtrain_net_eval(int net, int head, int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx,
+                         int n, void* scratch, float* probs, double* acc, void* stream);
 /* kernels launched so far by the r4_simtrain_* entry points in this process (the radix sort counted once) */
 int64_t r4_simtrain_launch_count(void);
 /* kernels launched so far by every learner entry point in this process (r4_policy_*, r4_gae, r4_adam_step, r4_ppo_epoch*,

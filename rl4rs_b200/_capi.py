@@ -162,6 +162,17 @@ EXPORTS = {
                               [C.c_float] * 4 + [C.c_void_p] * 4),
     "r4_simtrain_head_eval": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.POINTER(SimTrainData), C.c_void_p, C.c_int] +
                               [C.c_void_p] * 4),
+    "r4_simtrain_net_num_params": (C.c_int64, [C.c_int, C.c_int, C.c_int]),
+    "r4_simtrain_net_scratch_size": (C.c_int64, [C.c_int, C.c_int, C.c_int]),
+    "r4_simtrain_net_grad": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.POINTER(SimTrainData), C.c_void_p, C.c_int,
+                                       C.c_uint64, C.c_uint64, C.c_float] + [C.c_void_p] * 7),
+    "r4_simtrain_net_apply": (C.c_int, [C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 4 + [C.c_int] + [C.c_float] * 4 + [C.c_void_p]),
+    "r4_simtrain_net_step": (C.c_int, [C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 4 + [C.POINTER(SimTrainData), C.c_void_p,
+                                                                                        C.c_int, C.c_uint64, C.c_uint64, C.c_float,
+                                                                                        C.c_int] +
+                             [C.c_float] * 4 + [C.c_void_p] * 4),
+    "r4_simtrain_net_eval": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.POINTER(SimTrainData), C.c_void_p, C.c_int] +
+                             [C.c_void_p] * 4),
     "r4_simtrain_launch_count": (C.c_int64, []),
     "r4_learner_launch_count": (C.c_int64, []),
 }

@@ -1027,3 +1027,251 @@ int r4_simtrain_eval(int hash_size, const float* params, const r4_simtrain_data*
                      float* probs, double* acc, void* stream) {
   return r4_simtrain_head_eval(R4_SIMHEAD_ITEM, hash_size, params, data, idx, n, scratch, probs, acc, stream);
 }
+
+// ---- the other simulator backbones (dnn, widedeep, lstm) and adversarial_slate (r4_simtrain.cuh) -----------------------
+static bool st_pair_ok(int net, int head) {
+  if (net == r4st::NET_ADV) return head == r4st::HEAD_ADV;
+  return net >= 0 && net < r4st::NET_ADV && st_head_ok(head);
+}
+static int st_net_classes(int head) { return head == r4st::HEAD_ADV ? r4st::NS : r4st::head_classes(head); }
+
+int64_t r4_simtrain_net_num_params(int net, int head, int hash_size) {
+  if (!st_pair_ok(net, head) || !st_hash_ok(hash_size)) return -1;
+  if (net == r4st::NET_DIEN) return r4_simtrain_head_num_params(head, hash_size);
+  return r4st::make_nlayout(net, hash_size, st_net_classes(head)).n;
+}
+int64_t r4_simtrain_net_scratch_size(int net, int head, int n) {
+  if (!st_pair_ok(net, head) || n < 1 || n > r4st::MAXN) return -1;
+  if (net == r4st::NET_DIEN) return r4_simtrain_head_scratch_size(head, n);
+  return (int64_t)r4st::make_nplanes(nullptr, r4st::make_nlayout(net, 1, st_net_classes(head)), n).bytes;
+}
+
+// The forward with saved activations: the embedding front, the dense tower, lstm's three GRUs, the net's dense layers,
+// the head and the loss.
+static int sn_forward(int head, const r4st::NLayout& L, const float* prm, const r4st::Data& D, const int64_t* idx, int n,
+                      uint64_t seed, uint64_t counter, float rate, const uint8_t* keep_in, uint8_t* keep_out,
+                      const r4st::NPlanes& P, bool with_grad, float* stats, double* acc, float* probs, cudaStream_t st) {
+  using namespace r4st;
+  Layout LH{};
+  LH.H = L.H;
+  const GatherArgs ga{LH, D, idx, n, seed, counter, rate, keep_in, keep_out, head != HEAD_ITEM};
+  Front f{};
+  f.ncp = L.ncp;
+  if (L.net == NET_DNN) { f.cpool = P.A; f.ldc = L.FA; }
+  if (L.net == NET_ADV) { f.cpool = P.A + 2 * E + U; f.ldc = L.FA; }
+  if (L.net == NET_WIDEDEEP) { f.flat = P.O + OBS + U; f.ldf = L.FO; }
+  if (L.net == NET_LSTM) { f.flat = P.A + 4 * U; f.ldf = L.FA; f.xc = P.g[0].X; f.xs0 = P.g[1].X; f.xs1 = P.g[2].X; }
+  if (L.net == NET_WIDEDEEP || L.net == NET_ADV) { f.spool = P.A; f.lds = L.FA; }
+  int rc;
+  if ((rc = st_launch("k_st_front", k_st_front, n, E, st, ga, L.emb_cat, L.emb_seq, prm, P.cat, P.dense, P.keep, f))) return rc;
+  float* tower = L.A_tower >= 0 ? P.A + L.A_tower : P.O + L.O_tower;
+  const int ldt = L.A_tower >= 0 ? L.FA : L.FO;
+  if ((rc = st_gemm(false, P.dense, ND, prm + L.dw1, U, prm + L.db1, P.T1d, U, n, U, ND, EP_ELU, st, nullptr, P.keep, P.T1))) return rc;
+  if ((rc = st_gemm(false, P.T1d, U, prm + L.dw2, U, prm + L.db2, tower, ldt, n, U, U, EP_ELU, st, nullptr, P.keep + (size_t)n * U,
+                    P.T2)))
+    return rc;
+  if (L.net == NET_LSTM) {
+    const int col[3] = {3 * U, 0, U};             // the category GRU's state after the tower; the sequence GRUs first
+    for (int i = 0; i < 3; ++i) {
+      const GruPlanes& g = P.g[i];
+      const int nt = i ? T : NC, R = n * nt;
+      if ((rc = st_gemm(false, g.X, E, prm + L.g[i].k, NG3, prm + L.g[i].b, g.XG, NG3, R, NG3, E, EP_LIN, st))) return rc;
+      const KGru a{prm + L.g[i].rk, g.XG, g.Hp, g.A, g.HH, g.RH, P.A + col[i], L.FA, n, nt};
+      if ((rc = st_launch("k_st_kgru_fwd", k_st_kgru_fwd, (n + SB - 1) / SB, NTH, st, a))) return rc;
+    }
+  }
+  if (L.net == NET_DNN) {
+    if ((rc = st_gemm(false, P.A, L.FA, prm + L.fcw, OBS, prm + L.fcb, P.F, OBS, n, OBS, L.FA, EP_ELU, st))) return rc;
+    if ((rc = st_gemm(false, P.F, OBS, prm + L.ow, OBS, prm + L.ob, P.O, OBS, n, OBS, OBS, EP_ELU, st))) return rc;
+  } else if (L.net == NET_WIDEDEEP) {             // O[:, :256], its activations kept apart in F for the backward
+    if ((rc = st_gemm(false, P.A, L.FA, prm + L.fcw, OBS, prm + L.fcb, P.O, L.FO, n, OBS, L.FA, EP_ELU, st, nullptr, nullptr, P.F)))
+      return rc;
+  } else if (L.net == NET_LSTM) {
+    if ((rc = st_gemm(false, P.A, L.FA, prm + L.ow, OBS, prm + L.ob, P.O, OBS, n, OBS, L.FA, EP_ELU, st))) return rc;
+  }
+  const float* hin = L.FO ? P.O : P.A;
+  if ((rc = st_gemm(false, hin, L.FH, prm + L.rw, L.C, prm + L.rb, P.Z, L.C, n, L.C, L.FH, EP_LIN, st))) return rc;
+  float* dZ = with_grad ? P.dZ : nullptr;
+  if (head == HEAD_ADV) return st_launch("k_st_loss_adv", k_st_loss_adv, 1, NTH, st, D, idx, n, P.Z, dZ, P.srow, stats, acc, probs);
+  if (head == HEAD_SLATE)
+    return st_launch("k_st_loss_slate<9>", k_st_loss_slate<NS>, 1, NTH, st, D, idx, n, P.Z, dZ, P.srow, stats, acc, probs);
+  if (head == HEAD_SLATE_MULTICLASS)
+    return st_launch("k_st_loss_slate<22>", k_st_loss_slate<NMC>, 1, NTH, st, D, idx, n, P.Z, dZ, P.srow, stats, acc, probs);
+  return st_launch("k_st_loss", k_st_loss, 1, NTH, st, D, idx, n, P.Z, dZ, P.srow, stats, acc, probs);
+}
+
+static int sn_backward(int head, const r4st::NLayout& L, const float* prm, const r4st::Data& D, const int64_t* idx, int n,
+                       const r4st::NPlanes& P, float* grad, cudaStream_t st) {
+  using namespace r4st;
+  const int C = L.C;
+  const float* keep0 = P.keep;
+  const float* keep1 = P.keep + (size_t)n * U;
+  int rc;
+  // the head and dense layers down to dA (the front's and GRUs' columns) and dT2 (the tower's output, with its activation
+  // and dropout); Wt(w, r0) is the weight w from its row r0 on, read transposed
+  auto Wt = [&](int64_t w, int r0, int ld) { return prm + w + (int64_t)r0 * ld; };
+  int tower_r0 = 0, tower_ld = 0;
+  const float* dtop = nullptr;
+  if (L.net == NET_DNN) {
+    if ((rc = st_gemm(true, P.dZ, C, Wt(L.rw, 0, C), C, nullptr, P.dO, OBS, n, OBS, C, EP_DELU, st, P.O))) return rc;
+    if ((rc = st_gemm(true, P.dO, OBS, Wt(L.ow, 0, OBS), OBS, nullptr, P.dF, OBS, n, OBS, OBS, EP_DELU, st, P.F))) return rc;
+    if ((rc = st_gemm(true, P.dF, OBS, Wt(L.fcw, 0, OBS), OBS, nullptr, P.dA, L.FA, n, E, OBS, EP_LIN, st))) return rc;
+    dtop = P.dF; tower_r0 = E; tower_ld = OBS;
+  } else if (L.net == NET_WIDEDEEP) {
+    if ((rc = st_gemm(true, P.dZ, C, Wt(L.rw, 0, C), C, nullptr, P.dF, OBS, n, OBS, C, EP_DELU, st, P.F))) return rc;
+    if ((rc = st_gemm(true, P.dZ, C, Wt(L.rw, OBS + U, C), C, nullptr, P.dO + OBS + U, L.FO, n, NC * E, C, EP_LIN, st))) return rc;
+    if ((rc = st_gemm(true, P.dF, OBS, Wt(L.fcw, 0, OBS), OBS, nullptr, P.dA, L.FA, n, L.FA, OBS, EP_LIN, st))) return rc;
+    dtop = P.dZ; tower_r0 = OBS; tower_ld = C;
+  } else if (L.net == NET_LSTM) {
+    if ((rc = st_gemm(true, P.dZ, C, Wt(L.rw, 0, C), C, nullptr, P.dO, OBS, n, OBS, C, EP_DELU, st, P.O))) return rc;
+    if ((rc = st_gemm(true, P.dO, OBS, Wt(L.ow, 0, OBS), OBS, nullptr, P.dA, L.FA, n, L.FA, OBS, EP_LIN, st))) return rc;
+    dtop = P.dO; tower_r0 = L.A_tower; tower_ld = OBS;
+  } else {
+    if ((rc = st_gemm(true, P.dZ, C, Wt(L.rw, 0, C), C, nullptr, P.dA, L.FA, n, L.FA, C, EP_LIN, st))) return rc;
+    dtop = P.dZ; tower_r0 = L.A_tower; tower_ld = C;
+  }
+  const int64_t tw = L.net == NET_DNN ? L.fcw : L.net == NET_LSTM ? L.ow : L.rw;
+  if ((rc = st_gemm(true, dtop, tower_ld, Wt(tw, tower_r0, tower_ld), tower_ld, nullptr, P.dT2, U, n, U, tower_ld, EP_DELU, st, P.T2,
+                    keep1)))
+    return rc;
+  if ((rc = st_gemm(true, P.dT2, U, prm + L.dw2, U, nullptr, P.dT1, U, n, U, U, EP_DELU, st, P.T1, keep0))) return rc;
+  // the embedding front: pools and Flatten; lstm's GRUs (BPTT) and their input gradients
+  FrontBack fb{};
+  fb.ncp = L.ncp;
+  if (L.net == NET_DNN) { fb.dcpool = P.dA; fb.ldc = L.FA; }
+  if (L.net == NET_ADV) { fb.dcpool = P.dA + 2 * E + U; fb.ldc = L.FA; }
+  if (L.net == NET_WIDEDEEP) { fb.dflat = P.dO + OBS + U; fb.ldf = L.FO; }
+  if (L.net == NET_LSTM) { fb.dflat = P.dA + 4 * U; fb.ldf = L.FA; }
+  if (L.net == NET_WIDEDEEP || L.net == NET_ADV) { fb.dspool = P.dA; fb.lds = L.FA; }
+  if ((rc = st_launch("k_st_front_bwd", k_st_front_bwd, n, E, st, fb, P.dEcat, P.dX[0], P.dX[1]))) return rc;
+  if (L.net == NET_LSTM) {
+    const int col[3] = {3 * U, 0, U};
+    for (int i = 0; i < 3; ++i) {
+      const GruPlanes& g = P.g[i];
+      const int nt = i ? T : NC, R = n * nt;
+      const KGruBack b{prm + L.g[i].rk, g.Hp, g.A, g.HH, P.dA + col[i], L.FA, g.dZR, g.dHH, n, nt};
+      if ((rc = st_launch("k_st_kgru_bwd", k_st_kgru_bwd, (n + SB - 1) / SB, NTH, st, b))) return rc;
+      float* dX = i ? P.dX[i - 1] : P.dEcat;      // the category GRU's input gradient adds to the Flatten one
+      if ((rc = st_gemm(true, g.dZR, 2 * U, prm + L.g[i].k, NG3, nullptr, dX, E, R, E, 2 * U, EP_LIN, st, nullptr, nullptr, nullptr,
+                        i ? 0 : 1)))
+        return rc;
+      if ((rc = st_gemm(true, g.dHH, U, prm + L.g[i].k + 2 * U, NG3, nullptr, dX, E, R, E, U, EP_LIN, st, nullptr, nullptr, nullptr, 1)))
+        return rc;
+    }
+  }
+  // dense weight gradients over the n-row jobs
+  r4ddpg::Jobs J;
+  int k = 0;
+  J.j[k++] = st_job(P.dense, ND, P.dT1, ND, U, L.dw1);  J.j[k++] = st_job(nullptr, 1, P.dT1, 1, U, L.db1);
+  J.j[k++] = st_job(P.T1d, U, P.dT2, U, U, L.dw2);      J.j[k++] = st_job(nullptr, 1, P.dT2, 1, U, L.db2);
+  if (L.net == NET_DNN) {
+    J.j[k++] = st_job(P.A, L.FA, P.dF, L.FA, OBS, L.fcw); J.j[k++] = st_job(nullptr, 1, P.dF, 1, OBS, L.fcb);
+    J.j[k++] = st_job(P.F, OBS, P.dO, OBS, OBS, L.ow);    J.j[k++] = st_job(nullptr, 1, P.dO, 1, OBS, L.ob);
+  } else if (L.net == NET_WIDEDEEP) {
+    J.j[k++] = st_job(P.A, L.FA, P.dF, L.FA, OBS, L.fcw); J.j[k++] = st_job(nullptr, 1, P.dF, 1, OBS, L.fcb);
+  } else if (L.net == NET_LSTM) {
+    J.j[k++] = st_job(P.A, L.FA, P.dO, L.FA, OBS, L.ow);  J.j[k++] = st_job(nullptr, 1, P.dO, 1, OBS, L.ob);
+  }
+  const float* hin = L.FO ? P.O : P.A;
+  J.j[k++] = st_job(hin, L.FH, P.dZ, L.FH, C, L.rw);    J.j[k++] = st_job(nullptr, 1, P.dZ, 1, C, L.rb);
+  if ((rc = st_wgrad(J, k, n, grad, st))) return rc;
+  if (L.net == NET_LSTM) {
+    // each GRU's [z | r] and h column blocks into gtmp, the category GRU's (21 n rows) then both sequence GRUs' (64 n rows)
+    auto gru_jobs = [&](int i, int& kk) {
+      const GruPlanes& g = P.g[i];
+      const int64_t zr = (int64_t)i * GROWS * NG3, hc = zr + (int64_t)GROWS * 2 * U;
+      J.j[kk++] = st_job(g.X, E, g.dZR, E, 2 * U, zr);  J.j[kk++] = st_job(g.Hp, U, g.dZR, U, 2 * U, zr + (int64_t)E * 2 * U);
+      J.j[kk++] = st_job(nullptr, 1, g.dZR, 1, 2 * U, zr + (int64_t)(E + U) * 2 * U);
+      J.j[kk++] = st_job(g.X, E, g.dHH, E, U, hc);      J.j[kk++] = st_job(g.RH, U, g.dHH, U, U, hc + (int64_t)E * U);
+      J.j[kk++] = st_job(nullptr, 1, g.dHH, 1, U, hc + (int64_t)(E + U) * U);
+    };
+    k = 0;
+    gru_jobs(0, k);
+    if ((rc = st_wgrad(J, k, n * NC, P.gtmp, st))) return rc;
+    k = 0;
+    gru_jobs(1, k);
+    gru_jobs(2, k);
+    if ((rc = st_wgrad(J, k, n * T, P.gtmp, st))) return rc;
+    if ((rc = st_launch("k_st_kgru_merge", k_st_kgru_merge, (3 * GROWS * NG3 + 255) / 256, 256, st, (const float*)P.gtmp, grad,
+                        L.g[0].k, L.g[1].k, L.g[2].k)))
+      return rc;
+  }
+  // embedding gradients: keys, a stable radix sort by (table, id), one ordered sum per run
+  const int ns = nslots(L), total = n * ns;
+  if ((rc = st_launch("k_st_nembkeys", k_st_nembkeys, (total + 255) / 256, 256, st, L.H, D, idx, n, (int)(head != HEAD_ITEM), L.ncp,
+                       ns, P.cat, P.keys, P.vals)))
+    return rc;
+  int bits = 1;
+  while (bits < 32 && ((uint64_t)1 << bits) < (uint64_t)(2 * L.H)) ++bits;
+  cub::DoubleBuffer<uint32_t> kb(P.keys, P.keys2);
+  cub::DoubleBuffer<int32_t> vb(P.vals, P.vals2);
+  size_t need = 0;
+  if (cub::DeviceRadixSort::SortPairs(nullptr, need, kb, vb, total, 0, bits, st) != cudaSuccess || need > P.cub_bytes)
+    return fail(R4_ERR_NOMEM, "r4_simtrain: radix sort temporary storage exceeds the scratch reserve");
+  size_t have = P.cub_bytes;
+  if (cub::DeviceRadixSort::SortPairs(P.cub_tmp, have, kb, vb, total, 0, bits, st) != cudaSuccess)
+    return fail(R4_ERR_CUDA, std::string("cub::DeviceRadixSort: ") + cudaGetErrorString(cudaGetLastError()));
+  count_launch(FAM_SIMTRAIN);
+  return st_launch("k_st_nembsum", k_st_nembsum, total, EST, st, L.H, L.emb_cat, L.emb_seq, L.ncp, ns, kb.Current(), vb.Current(),
+                   total, (const float*)P.dEcat, (const float*)P.dX[0], (const float*)P.dX[1], grad);
+}
+
+int r4_simtrain_net_grad(int net, int head, int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx,
+                         int n, uint64_t seed, uint64_t counter, float drop_rate, const uint8_t* keep_in, uint8_t* keep_out,
+                         void* scratch, float* grad, float* stats, double* acc, void* stream) {
+  if (!st_pair_ok(net, head))
+    return fail(R4_ERR_ARG, "r4_simtrain_net_grad: bad (net, head): nets 0..3 take heads 0..2, net 4 head 3");
+  if (net == r4st::NET_DIEN)
+    return r4_simtrain_head_grad(head, hash_size, params, data, idx, n, seed, counter, drop_rate, keep_in, keep_out, scratch, grad,
+                                 stats, acc, stream);
+  if (!st_hash_ok(hash_size) || !params || !st_data_ok(data) || !idx || n < 1 || n > r4st::MAXN || !(drop_rate >= 0.f) ||
+      !(drop_rate < 1.f) || !scratch || !grad)
+    return fail(R4_ERR_ARG, "r4_simtrain_net_grad: bad argument (hash_size 1..4000000, n 1..4096, drop_rate in [0, 1))");
+  const r4st::NLayout L = r4st::make_nlayout(net, hash_size, st_net_classes(head));
+  const r4st::NPlanes P = r4st::make_nplanes(scratch, L, n);
+  const r4st::Data D = st_data(data);
+  cudaStream_t st = S(stream);
+  int rc = sn_forward(head, L, params, D, idx, n, seed, counter, drop_rate, keep_in, keep_out, P, true, stats, acc, nullptr, st);
+  return rc ? rc : sn_backward(head, L, params, D, idx, n, P, grad, st);
+}
+
+static int sn_apply(int net, int head, int H, float* params, float* grad, float* m, float* v, int step, float lr, float b1, float b2,
+                    float eps, cudaStream_t st) {
+  const r4st::Layout L = r4st::apply_layout(r4st::make_nlayout(net, H, st_net_classes(head)));
+  const double alpha = (double)lr * std::sqrt(1.0 - std::pow((double)b2, step)) / (1.0 - std::pow((double)b1, step));
+  return st_launch("k_st_apply", r4st::k_st_apply, (unsigned)((L.n + 255) / 256), 256, st, L, params, grad, m, v, (float)alpha,
+                   b1, b2, eps);
+}
+
+int r4_simtrain_net_apply(int net, int head, int hash_size, float* params, float* grad, float* m, float* v, int step, float lr,
+                          float beta1, float beta2, float eps, void* stream) {
+  if (!st_pair_ok(net, head)) return fail(R4_ERR_ARG, "r4_simtrain_net_apply: bad (net, head)");
+  if (net == r4st::NET_DIEN) return r4_simtrain_head_apply(head, hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, stream);
+  if (!st_hash_ok(hash_size) || !params || !grad || !m || !v || step < 1) return fail(R4_ERR_ARG, "r4_simtrain_net_apply: bad argument");
+  return sn_apply(net, head, hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, S(stream));
+}
+
+int r4_simtrain_net_step(int net, int head, int hash_size, float* params, float* grad, float* m, float* v,
+                         const r4_simtrain_data* data, const int64_t* idx, int n, uint64_t seed, uint64_t counter, float drop_rate,
+                         int step, float lr, float beta1, float beta2, float eps, void* scratch, float* stats, double* acc,
+                         void* stream) {
+  if (!st_pair_ok(net, head)) return fail(R4_ERR_ARG, "r4_simtrain_net_step: bad (net, head)");
+  if (net == r4st::NET_DIEN)
+    return r4_simtrain_head_step(head, hash_size, params, grad, m, v, data, idx, n, seed, counter, drop_rate, step, lr, beta1, beta2,
+                                 eps, scratch, stats, acc, stream);
+  if (!m || !v || step < 1) return fail(R4_ERR_ARG, "r4_simtrain_net_step: bad argument");
+  int rc = r4_simtrain_net_grad(net, head, hash_size, params, data, idx, n, seed, counter, drop_rate, nullptr, nullptr, scratch, grad,
+                                stats, acc, stream);
+  return rc ? rc : sn_apply(net, head, hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, S(stream));
+}
+
+int r4_simtrain_net_eval(int net, int head, int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx,
+                         int n, void* scratch, float* probs, double* acc, void* stream) {
+  if (!st_pair_ok(net, head)) return fail(R4_ERR_ARG, "r4_simtrain_net_eval: bad (net, head)");
+  if (net == r4st::NET_DIEN) return r4_simtrain_head_eval(head, hash_size, params, data, idx, n, scratch, probs, acc, stream);
+  if (!st_hash_ok(hash_size) || !params || !st_data_ok(data) || !idx || n < 1 || n > r4st::MAXN || !scratch)
+    return fail(R4_ERR_ARG, "r4_simtrain_net_eval: bad argument");
+  const r4st::NLayout L = r4st::make_nlayout(net, hash_size, st_net_classes(head));
+  const r4st::NPlanes P = r4st::make_nplanes(scratch, L, n);
+  return sn_forward(head, L, params, st_data(data), idx, n, 0, 0, 0.f, nullptr, nullptr, P, false, nullptr, acc, probs, S(stream));
+}

@@ -817,4 +817,514 @@ __global__ void k_st_apply(Layout L, float* __restrict__ prm, float* __restrict_
   if (emb && g != 0.f) grad[i] = 0.f;
 }
 
+// ================================================================================================
+// The other backbones: nets/dnn*.py, widedeep*.py, lstm*.py and adversarial_slate.py on the same samples, dense tower,
+// heads, GEMM, weight-gradient jobs, embedding key sort and Adam.  What a backbone adds is its embedding front (mean
+// pools, Flatten, the GRU inputs) with its backward, and for lstm the Keras-v1 GRU with its BPTT.
+//   dnn       A = [mean_21 E_c[cat] | tower] (256); F = ELU(A fc_w + fc_b); O = ELU(F obs_w + obs_b); head on O
+//   widedeep  A = [mean_64 E_s[seq0] | mean_64 E_s[seq1]] (256); O = [ELU(A fc_w + fc_b) | tower | Flatten E_c[cat]] (3072);
+//             head on O
+//   lstm      A = [gru1(E_s[seq0]) | gru2(E_s[seq1]) | tower | gru0(E_c[cat]) | Flatten E_c[cat]] (3200);
+//             O = ELU(A obs_w + obs_b); head on O
+//   adversarial  A = [mean E_s[seq0] | mean E_s[seq1] | tower | mean_20 E_c[cat[:20]]] (512); p = sigmoid(A W + b) (9)
+// ================================================================================================
+enum { NET_DIEN = 0, NET_DNN = 1, NET_WIDEDEEP = 2, NET_LSTM = 3, NET_ADV = 4, NNET = 5 };
+enum { HEAD_ADV = 3 };
+constexpr int NG3 = 3 * U;                       // a Keras GRU's fused gate width [z | r | h]
+constexpr int GROWS = E + U + 1;                 // a GRU's parameter rows: kernel [E], recurrent_kernel [U], bias [1]
+constexpr int ADV_NCAT = NC - 1;                 // adversarial_slate pools the first 20 cat slots
+
+struct NGru { int64_t k, rk, b; };               // kernel [E, 3U], recurrent_kernel [U, 3U], bias [3U] (contiguous)
+struct NLayout {
+  int net, C;
+  int64_t H;
+  int64_t emb_cat, emb_seq;                      // emb_seq < 0: the net has no sequence table (dnn)
+  int64_t dw1, db1, dw2, db2;
+  int64_t fcw, fcb;                              // dnn / widedeep: the unnamed Dense(256)
+  NGru g[3];                                     // lstm: the category GRU, then one per sequence
+  int64_t ow, ob;                                // dnn / lstm: simulator_obs
+  int64_t rw, rb;                                // the head (adversarial: dense_2)
+  int FA, FO, FH;                                // widths of A, of O (0: none) and of the head's input
+  int A_tower, O_tower;                          // the tower's column in A or O (-1: not there)
+  int ncp, nseq;                                 // pooled / keyed cat slots; keyed sequence slots (0 or 2 T)
+  int64_t n;
+};
+__host__ __device__ inline NLayout make_nlayout(int net, int64_t H, int C) {
+  NLayout L{};
+  int64_t o = 0;
+  auto take = [&](int64_t k) { int64_t r = o; o += k; return r; };
+  L.net = net; L.C = C; L.H = H;
+  L.emb_seq = L.fcw = L.fcb = L.ow = L.ob = -1;
+  for (int i = 0; i < 3; ++i) L.g[i] = NGru{-1, -1, -1};
+  auto gru = [&](NGru& g) { g.k = take((int64_t)E * NG3); g.rk = take((int64_t)U * NG3); g.b = take(NG3); };
+  auto tower = [&]() { L.dw1 = take((int64_t)ND * U); L.db1 = take(U); L.dw2 = take((int64_t)U * U); L.db2 = take(U); };
+  L.emb_cat = take(H * E);
+  L.A_tower = L.O_tower = -1;
+  L.ncp = NC; L.nseq = 2 * T;
+  if (net == NET_DNN) {
+    tower();
+    L.fcw = take((int64_t)(E + U) * OBS); L.fcb = take(OBS);
+    L.ow = take((int64_t)OBS * OBS); L.ob = take(OBS);
+    L.FA = E + U; L.FO = OBS; L.FH = OBS; L.A_tower = E; L.nseq = 0;
+  } else if (net == NET_WIDEDEEP) {
+    tower();
+    L.emb_seq = take(H * E);
+    L.fcw = take((int64_t)2 * E * OBS); L.fcb = take(OBS);
+    L.FA = 2 * E; L.FO = OBS + U + NC * E; L.FH = L.FO; L.O_tower = OBS;
+  } else if (net == NET_LSTM) {
+    gru(L.g[0]);
+    tower();
+    L.emb_seq = take(H * E);
+    gru(L.g[1]); gru(L.g[2]);
+    L.ow = take((int64_t)(2 * U + U + U + NC * E) * OBS); L.ob = take(OBS);
+    L.FA = 4 * U + NC * E; L.FO = OBS; L.FH = OBS; L.A_tower = 2 * U;
+  } else {                                       // NET_ADV
+    tower();
+    L.emb_seq = take(H * E);
+    L.FA = 2 * E + U + E; L.FO = 0; L.FH = L.FA; L.A_tower = 2 * E; L.ncp = ADV_NCAT;
+  }
+  L.rw = take((int64_t)L.FH * C); L.rb = take(C);
+  L.n = o;
+  return L;
+}
+__host__ __device__ inline int nslots(const NLayout& L) { return L.ncp + L.nseq; }
+// the DIEN Layout k_st_apply reads: the parameter count and the tables whose gradient rows it clears (a net without a
+// sequence table names its category table twice)
+__host__ inline Layout apply_layout(const NLayout& N) {
+  Layout L{};
+  L.H = N.H; L.emb_cat = N.emb_cat; L.emb_seq = N.emb_seq >= 0 ? N.emb_seq : N.emb_cat; L.n = N.n;
+  return L;
+}
+
+struct GruPlanes { float *X, *XG, *Hp, *A, *HH, *RH, *dZR, *dHH; };   // R = T n rows ([R][E], [R][3U], [R][U], [R][2U] ...)
+struct NPlanes {
+  int32_t* cat;
+  float *dense, *keep, *T1, *T1d, *T2, *A, *dA, *F, *dF, *O, *dO, *Z, *dZ, *dT1, *dT2, *dEcat, *srow;   // NULL: not in the net
+  float* dX[2];                                  // [n][T][E] the sequence slots' gradient rows
+  GruPlanes g[3];                                // lstm: the category GRU (21 steps, X = E_c[cat]), the two sequence GRUs
+  float* gtmp;                                   // [3][GROWS][3U]: each GRU's [z|r] and h weight gradients before the merge
+  uint32_t *keys, *keys2;
+  int32_t *vals, *vals2;
+  void* cub_tmp;
+  size_t cub_bytes, bytes;
+};
+__host__ inline size_t ncub_reserve(int n, int nslot) { return ((size_t)4 << 20) + (size_t)16 * n * nslot; }
+__host__ inline NPlanes make_nplanes(void* base, const NLayout& L, int n) {
+  NPlanes P{};
+  const uintptr_t b = reinterpret_cast<uintptr_t>(base);
+  size_t o = 0;
+  auto take = [&](size_t floats) { float* q = reinterpret_cast<float*>(b + o); o += ((floats * 4 + 255) / 256) * 256; return q; };
+  const size_t N = (size_t)n;
+  P.cat = reinterpret_cast<int32_t*>(take(N * NC));
+  P.dense = take(N * ND); P.keep = take(N * 2 * U);
+  P.T1 = take(N * U); P.T1d = take(N * U); P.T2 = take(N * U);
+  P.A = take(N * L.FA); P.dA = take(N * L.FA);
+  if (L.net == NET_DNN || L.net == NET_WIDEDEEP) { P.F = take(N * OBS); P.dF = take(N * OBS); }   // Dense(256)'s ELU and its gradient
+  if (L.FO) { P.O = take(N * L.FO); P.dO = take(N * L.FO); }
+  P.Z = take(N * L.C); P.dZ = take(N * L.C);
+  P.dT1 = take(N * U); P.dT2 = take(N * U);
+  P.dEcat = take(N * NC * E); P.srow = take(N * 2);
+  if (L.nseq) for (int i = 0; i < 2; ++i) P.dX[i] = take(N * T * E);
+  if (L.net == NET_LSTM) {
+    for (int i = 0; i < 3; ++i) {
+      const size_t R = N * (i ? T : NC);
+      GruPlanes& g = P.g[i];
+      g.X = take(R * E);
+      g.XG = take(R * NG3); g.Hp = take(R * U); g.A = take(R * 2 * U); g.HH = take(R * U); g.RH = take(R * U);
+      g.dZR = take(R * 2 * U); g.dHH = take(R * U);
+    }
+    P.gtmp = take((size_t)3 * GROWS * NG3);
+  }
+  const int ns = nslots(L);
+  P.keys = reinterpret_cast<uint32_t*>(take(N * ns)); P.keys2 = reinterpret_cast<uint32_t*>(take(N * ns));
+  P.vals = reinterpret_cast<int32_t*>(take(N * ns)); P.vals2 = reinterpret_cast<int32_t*>(take(N * ns));
+  P.cub_tmp = reinterpret_cast<void*>(b + o);
+  P.cub_bytes = ncub_reserve(n, ns);
+  P.bytes = o + P.cub_bytes;
+  return P;
+}
+
+// ------------------------------------------------------------------------------------------------
+// k_st_front: one CTA (128 threads) per sample: the sample's cat ids, dense features and keep scales (as k_st_gather),
+// then the net's embedding front.  Each output (may be NULL) is a plane with its column offset applied and a row stride:
+//   cpool  mean of E_c over cat slots 0..ncp-1       flat  Flatten(E_c[cat]) (21 E)      xc  E_c rows [n][21][E]
+//   spool  [mean_t E_s[seq0] | mean_t E_s[seq1]]      xs0 / xs1  E_s rows [n][64][E]
+// ------------------------------------------------------------------------------------------------
+struct Front {
+  int ncp;
+  float* cpool; int ldc;
+  float* flat; int ldf;
+  float* spool; int lds;
+  float *xc, *xs0, *xs1;
+};
+__global__ void __launch_bounds__(E) k_st_front(GatherArgs g, int64_t emb_cat, int64_t emb_seq, const float* __restrict__ prm,
+                                                int32_t* __restrict__ catp, float* __restrict__ densep, float* __restrict__ keepp,
+                                                Front f) {
+  __shared__ int ids[NC];
+  const int s = blockIdx.x, c = threadIdx.x;
+  const int64_t smp = g.idx[s], rec = g.slate ? smp : smp / 9;
+  const int j = g.slate ? -1 : (int)(smp % 9);
+  const Data& D = g.D;
+  if (c < NC) {
+    int id = c < 10 ? D.ucat[rec * 10 + c] : c == 10 ? D.seqid[rec] : c < 20 ? D.items[rec * 9 + c - 11] : j < 0 ? 0 : D.items[rec * 9 + j];
+    id = clampid(id, g.L.H);
+    ids[c] = id;
+    catp[(size_t)s * NC + c] = id;
+  }
+  for (int k = c; k < ND; k += E) {
+    const float v = k < 32 ? D.udense[rec * 32 + k] : k < 392 ? D.ifeat[rec * 360 + k - 32] : j < 0 ? 0.f : D.ifeat[rec * 360 + j * 40 + k - 392];
+    densep[(size_t)s * ND + k] = v;
+  }
+  for (int u = c; u < 2 * U; u += E) {
+    bool kept;
+    if (g.keep_in) kept = g.keep_in[(size_t)s * 2 * U + u] != 0;
+    else kept = g.rate <= 0.f || drop_u(g.seed, g.counter, s, u) >= g.rate;
+    if (g.keep_out) g.keep_out[(size_t)s * 2 * U + u] = kept ? 1 : 0;
+    keepp[((size_t)(u / U) * g.n + s) * U + u % U] = kept ? 1.f / (1.f - g.rate) : 0.f;
+  }
+  __syncthreads();
+  float pool = 0.f;
+  for (int r = 0; r < NC; ++r) {
+    const float v = __ldg(prm + emb_cat + (int64_t)ids[r] * E + c);
+    if (r < f.ncp) pool += v;
+    if (f.flat) f.flat[(size_t)s * f.ldf + r * E + c] = v;
+    if (f.xc) f.xc[((size_t)s * NC + r) * E + c] = v;
+  }
+  if (f.cpool) f.cpool[(size_t)s * f.ldc + c] = pool / (float)f.ncp;
+  if (!f.spool && !f.xs0) return;
+  for (int i = 0; i < 2; ++i) {
+    float* xs = i ? f.xs1 : f.xs0;
+    float sum = 0.f;
+    for (int t = 0; t < T; ++t) {
+      const int id = clampid(D.seq[(rec * 2 + i) * T + t], g.L.H);
+      const float v = __ldg(prm + emb_seq + (int64_t)id * E + c);
+      sum += v;
+      if (xs) xs[((size_t)s * T + t) * E + c] = v;
+    }
+    if (f.spool) f.spool[(size_t)s * f.lds + i * E + c] = sum / (float)T;
+  }
+}
+
+// The front's backward for the pools and Flatten: dEcat[s][k] = d(flat)_k + [k < ncp] d(cpool) / ncp for every cat slot,
+// and, with spool, dX[i][s][t] = d(spool_i) / 64 for every step.  (lstm adds the category GRU's input gradient to dEcat
+// and writes its sequence slots' rows with the GRU input GEMMs.)
+struct FrontBack {
+  int ncp;
+  const float* dcpool; int ldc;
+  const float* dflat; int ldf;
+  const float* dspool; int lds;
+};
+__global__ void __launch_bounds__(E) k_st_front_bwd(FrontBack f, float* __restrict__ dEcat, float* __restrict__ dX0,
+                                                    float* __restrict__ dX1) {
+  const int s = blockIdx.x, c = threadIdx.x;
+  const float dp = f.dcpool ? f.dcpool[(size_t)s * f.ldc + c] / (float)f.ncp : 0.f;
+  for (int k = 0; k < NC; ++k) {
+    float v = k < f.ncp ? dp : 0.f;
+    if (f.dflat) v += f.dflat[(size_t)s * f.ldf + k * E + c];
+    dEcat[((size_t)s * NC + k) * E + c] = v;
+  }
+  if (!f.dspool) return;
+  for (int i = 0; i < 2; ++i) {
+    const float d = f.dspool[(size_t)s * f.lds + i * E + c] / (float)T;
+    float* dX = i ? dX1 : dX0;
+    for (int t = 0; t < T; ++t) dX[((size_t)s * T + t) * E + c] = d;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// The Keras-v1 GRU of nets/lstm*.py (TF 1.15 keras recurrent.GRU: reset_after = False, one bias, gate order [z | r | h],
+// h0 = 0, no masking, the last state only).  Hidden U = 128, input XG = x kernel + bias [R][3U] precomputed, nt steps:
+//   a = 0.2 (XG[:2U] + h rk[:, :2U]) + 0.5,  [z | r] = clip(a, 0, 1)  (hard sigmoid),
+//   hh = tanh(XG[2U:] + (r h) rk[:, 2U:]),   h' = z h + (1 - z) hh.
+// SB samples per CTA, h / r h / gates in shared memory, rk read from global memory (L2-resident).  Stores h_{t-1}, the
+// hard-sigmoid arguments a (the backward's kink test needs a itself: a gate at 0 or 1 does not say on which side of the
+// kink it was clipped), hh and r h; the last state goes to hT (ld ldT).
+// ------------------------------------------------------------------------------------------------
+struct KGru {
+  const float* rk; const float* XG;
+  float *Hp, *A, *HH, *RH;
+  float* hT; int ldT;
+  int n, nt;
+};
+__device__ __forceinline__ float hsig_arg(float x) { return fmaf(0.2f, x, 0.5f); }
+__device__ __forceinline__ float hsig(float a) { return fminf(fmaxf(a, 0.f), 1.f); }
+// the hard sigmoid's slope: 0.2 where 0 <= a <= 1, both ends included (clip_by_value = minimum / maximum, whose gradients
+// send ties to x; INTEGRATION.md section 8)
+__device__ __forceinline__ float hsig_d(float a) { return (a >= 0.f && a <= 1.f) ? 0.2f : 0.f; }
+
+__global__ void __launch_bounds__(NTH) k_st_kgru_fwd(KGru a) {
+  __shared__ float h[SB][U];
+  __shared__ float rh[SB][U];
+  __shared__ float gs[SB][2 * U];
+  const int tid = threadIdx.x, s0 = blockIdx.x * SB;
+  const int nv = min(SB, a.n - s0);
+  for (int i = tid; i < SB * U; i += NTH) h[i / U][i % U] = 0.f;
+  __syncthreads();
+  for (int t = 0; t < a.nt; ++t) {
+    for (int j = tid; j < 2 * U; j += NTH) {
+      float acc[SB];
+#pragma unroll
+      for (int s = 0; s < SB; ++s) acc[s] = 0.f;
+#pragma unroll 4
+      for (int k = 0; k < U; ++k) {
+        const float w = __ldg(a.rk + (size_t)k * NG3 + j);
+#pragma unroll
+        for (int s = 0; s < SB; ++s) acc[s] = fmaf(h[s][k], w, acc[s]);
+      }
+#pragma unroll
+      for (int s = 0; s < SB; ++s) {
+        if (s >= nv) { gs[s][j] = 0.f; continue; }
+        const size_t row = (size_t)(s0 + s) * a.nt + t;
+        const float ar = hsig_arg(a.XG[row * NG3 + j] + acc[s]);
+        gs[s][j] = hsig(ar);
+        a.A[row * 2 * U + j] = ar;
+      }
+    }
+    __syncthreads();
+    for (int i = tid; i < SB * U; i += NTH) {
+      const int s = i / U, k = i % U;
+      const float v = gs[s][U + k] * h[s][k];
+      rh[s][k] = v;
+      if (s < nv) {
+        const size_t row = (size_t)(s0 + s) * a.nt + t;
+        a.RH[row * U + k] = v;
+        a.Hp[row * U + k] = h[s][k];
+      }
+    }
+    __syncthreads();
+    for (int j = tid; j < U; j += NTH) {
+      float acc[SB];
+#pragma unroll
+      for (int s = 0; s < SB; ++s) acc[s] = 0.f;
+#pragma unroll 4
+      for (int k = 0; k < U; ++k) {
+        const float w = __ldg(a.rk + (size_t)k * NG3 + 2 * U + j);
+#pragma unroll
+        for (int s = 0; s < SB; ++s) acc[s] = fmaf(rh[s][k], w, acc[s]);
+      }
+#pragma unroll
+      for (int s = 0; s < SB; ++s) {
+        if (s >= nv) continue;
+        const size_t row = (size_t)(s0 + s) * a.nt + t;
+        const float hh = tanhf(a.XG[row * NG3 + 2 * U + j] + acc[s]);
+        const float z = gs[s][j];
+        a.HH[row * U + j] = hh;
+        h[s][j] = z * h[s][j] + (1.f - z) * hh;          // only this thread reads h[s][j] in this phase
+      }
+    }
+    __syncthreads();
+  }
+  for (int i = tid; i < nv * U; i += NTH) a.hT[(size_t)(s0 + i / U) * a.ldT + i % U] = h[i / U][i % U];
+}
+
+// BPTT of k_st_kgru_fwd: dh starts at dT (ld ldT) with no per-step input; writes dZR [R][2U] = d(z, r pre-activations) and
+// dHH [R][U] = d(candidate pre-activation).
+struct KGruBack {
+  const float* rk;
+  const float *Hp, *A, *HH, *dT;
+  int ldT;
+  float *dZR, *dHH;
+  int n, nt;
+};
+__global__ void __launch_bounds__(NTH) k_st_kgru_bwd(KGruBack a) {
+  __shared__ float dh[SB][U];
+  __shared__ float dgp[SB][2 * U];
+  __shared__ float dcp[SB][U];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, s0 = blockIdx.x * SB;
+  const int nv = min(SB, a.n - s0);
+  for (int i = tid; i < SB * U; i += NTH) {
+    const int s = i / U, k = i % U;
+    dh[s][k] = s < nv ? a.dT[(size_t)(s0 + s) * a.ldT + k] : 0.f;
+  }
+  __syncthreads();
+  for (int t = a.nt - 1; t >= 0; --t) {
+    // the cell output: dh -> d(z) (pre-activation), d(hh) (pre-activation), the carried dh z
+    for (int i = tid; i < SB * U; i += NTH) {
+      const int s = i / U, k = i % U;
+      if (s >= nv) { dcp[s][k] = 0.f; dgp[s][k] = 0.f; continue; }
+      const size_t row = (size_t)(s0 + s) * a.nt + t;
+      const float d = dh[s][k];
+      const float hp = a.Hp[row * U + k], az = a.A[row * 2 * U + k], hh = a.HH[row * U + k];
+      const float z = hsig(az);
+      const float dc = d * (1.f - z) * (1.f - hh * hh);
+      dgp[s][k] = d * (hp - hh) * hsig_d(az);
+      dcp[s][k] = dc;
+      dh[s][k] = d * z;
+      a.dHH[row * U + k] = dc;
+    }
+    __syncthreads();
+    // d(r h) = dhh rk_h^T: one warp per row k of rk
+    for (int k = warp; k < U; k += NTH / 32) {
+      float p[SB];
+#pragma unroll
+      for (int s = 0; s < SB; ++s) p[s] = 0.f;
+      for (int j = lane; j < U; j += 32) {
+        const float w = __ldg(a.rk + (size_t)k * NG3 + 2 * U + j);
+#pragma unroll
+        for (int s = 0; s < SB; ++s) p[s] = fmaf(dcp[s][j], w, p[s]);
+      }
+#pragma unroll
+      for (int s = 0; s < SB; ++s) p[s] = r4ppo::warp_sum(p[s]);
+      if (lane < SB && lane < nv) {
+        float drh = 0.f;
+#pragma unroll
+        for (int s = 0; s < SB; ++s) if (s == lane) drh = p[s];
+        const int s = lane;
+        const size_t row = (size_t)(s0 + s) * a.nt + t;
+        const float hp = a.Hp[row * U + k], ar = a.A[row * 2 * U + U + k];
+        dgp[s][U + k] = drh * hp * hsig_d(ar);
+        dh[s][k] += drh * hsig(ar);
+      } else if (lane < SB) {
+        dgp[lane][U + k] = 0.f;
+      }
+    }
+    __syncthreads();
+    for (int i = tid; i < nv * 2 * U; i += NTH) {
+      const int s = i / (2 * U), j = i % (2 * U);
+      a.dZR[((size_t)(s0 + s) * a.nt + t) * 2 * U + j] = dgp[s][j];
+    }
+    // dh += d([z | r]) rk_zr^T
+    for (int k = warp; k < U; k += NTH / 32) {
+      float p[SB];
+#pragma unroll
+      for (int s = 0; s < SB; ++s) p[s] = 0.f;
+      for (int j = lane; j < 2 * U; j += 32) {
+        const float w = __ldg(a.rk + (size_t)k * NG3 + j);
+#pragma unroll
+        for (int s = 0; s < SB; ++s) p[s] = fmaf(dgp[s][j], w, p[s]);
+      }
+#pragma unroll
+      for (int s = 0; s < SB; ++s) p[s] = r4ppo::warp_sum(p[s]);
+      if (lane < SB) {
+        float v = 0.f;
+#pragma unroll
+        for (int s = 0; s < SB; ++s) if (s == lane) v = p[s];
+        dh[lane][k] += v;
+      }
+    }
+    __syncthreads();
+  }
+}
+
+// The weight-gradient jobs write each GRU's [z | r] columns ([GROWS][2U]) and h columns ([GROWS][U]) apart, since a job's
+// output rows are dense; this copies them into the fused [GROWS][3U] block (kernel, recurrent_kernel, bias) of each GRU.
+__global__ void k_st_kgru_merge(const float* __restrict__ tmp, float* __restrict__ grad, int64_t g0, int64_t g1, int64_t g2) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 3 * GROWS * NG3) return;
+  const int g = i / (GROWS * NG3), e = i % (GROWS * NG3), r = e / NG3, c = e % NG3;
+  const float* zr = tmp + (size_t)g * GROWS * NG3;
+  const float* hc = zr + (size_t)GROWS * 2 * U;
+  grad[(g == 0 ? g0 : g == 1 ? g1 : g2) + e] = c < 2 * U ? zr[r * 2 * U + c] : hc[r * U + c - 2 * U];
+}
+
+// ------------------------------------------------------------------------------------------------
+// The embedding gradients of a backbone: entry e = s * nslot + k; k < ncp the emb_cat slot k (source dEcat[s][k]), else
+// emb_seq for sequence (k - ncp) / 64, step (k - ncp) % 64 (source dX[i][s][t]).  Keys, the stable radix sort and the
+// ordered per-run sums as k_st_embkeys / k_st_embsum.
+// ------------------------------------------------------------------------------------------------
+__global__ void k_st_nembkeys(int64_t H, Data D, const int64_t* __restrict__ idx, int n, int slate, int ncp, int nslot,
+                              const int32_t* __restrict__ cat, uint32_t* __restrict__ keys, int32_t* __restrict__ vals) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n * nslot) return;
+  const int s = e / nslot, k = e % nslot;
+  uint32_t key;
+  if (k < ncp) {
+    key = (uint32_t)cat[s * NC + k];
+  } else {
+    const int i = (k - ncp) / T, t = (k - ncp) % T;
+    const int64_t rec = slate ? idx[s] : idx[s] / 9;
+    key = (uint32_t)(H + clampid(D.seq[(rec * 2 + i) * T + t], H));
+  }
+  keys[e] = key;
+  vals[e] = e;
+}
+__global__ void __launch_bounds__(EST) k_st_nembsum(int64_t H, int64_t emb_cat, int64_t emb_seq, int ncp, int nslot,
+                                                    const uint32_t* __restrict__ keys, const int32_t* __restrict__ vals, int total,
+                                                    const float* __restrict__ dEcat, const float* __restrict__ dX0,
+                                                    const float* __restrict__ dX1, float* __restrict__ grad) {
+  __shared__ float part[ESG][E];
+  const int i0 = blockIdx.x;
+  const uint32_t key = keys[i0];
+  if (i0 > 0 && keys[i0 - 1] == key) return;
+  const int c = threadIdx.x % E, grp = threadIdx.x / E;
+  float acc = 0.f;
+  for (int i = i0 + grp; i < total && keys[i] == key; i += ESG) {
+    const int e = vals[i], s = e / nslot, k = e % nslot;
+    const float* src = k < ncp ? dEcat + ((size_t)s * NC + k) * E
+                               : ((k - ncp) / T ? dX1 : dX0) + ((size_t)s * T + (k - ncp) % T) * E;
+    acc += src[c];
+  }
+  part[grp][c] = acc;
+  __syncthreads();
+  if (grp == 0) {
+    float v = part[0][c];
+    for (int g = 1; g < ESG; ++g) v += part[g][c];
+    const int64_t base = key < (uint32_t)H ? emb_cat + (int64_t)key * E : emb_seq + (int64_t)(key - H) * E;
+    grad[base + c] = v;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// k_st_loss_adv (one CTA): adversarial_slate.py's loss on record samples with clicks y[9].  p = sigmoid(z) (9 columns),
+// q = softmax(p) (over the sigmoid outputs, not the logits); per sample
+//   l = 0.1 mean_j [max(z, 0) - z y + log(1 + exp(-|z|))] + sum_j q_j (1 - y_j),
+// averaged over the batch; dz_j = [0.1 (p_j - y_j) / 9 + q_j ((1 - y_j) - sum_k q_k (1 - y_k)) p_j (1 - p_j)] / n.
+// acc / stats / probs as k_st_loss_slate<9> (AUC, Precision and Recall on p).
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(NTH) k_st_loss_adv(Data D, const int64_t* __restrict__ idx, int n, const float* __restrict__ Z,
+                                                     float* __restrict__ dZ, float* __restrict__ srow, float* __restrict__ stats,
+                                                     double* __restrict__ acc, float* __restrict__ probs) {
+  __shared__ unsigned int hist[2][NBIN];
+  __shared__ unsigned int cnt[3];
+  const int tid = threadIdx.x;
+  for (int i = tid; i < 2 * NBIN; i += NTH) hist[i / NBIN][i % NBIN] = 0u;
+  if (tid < 3) cnt[tid] = 0u;
+  __syncthreads();
+  const float inv = 1.f / (float)n;
+  for (int s = tid; s < n; s += NTH) {
+    const uint8_t* y = D.label + idx[s] * 9;
+    const float* z = Z + (size_t)s * NS;
+    float p[NS], q[NS], bce = 0.f, hit = 0.f, pm = -INFINITY, den = 0.f;
+#pragma unroll
+    for (int j = 0; j < NS; ++j) {
+      const bool yj = y[j] != 0;
+      const float zj = z[j], e = expf(-fabsf(zj));
+      p[j] = zj >= 0.f ? 1.f / (1.f + e) : e / (1.f + e);
+      bce += fmaxf(zj, 0.f) - (yj ? zj : 0.f) + log1pf(e);
+      pm = fmaxf(pm, p[j]);
+      const bool pos = p[j] > 0.5f;
+      hit += pos == yj ? 1.f : 0.f;
+      if (acc) {
+        atomicAdd(&hist[yj ? 0 : 1][auc_bin(p[j])], 1u);
+        if (pos || yj) atomicAdd(&cnt[pos ? (yj ? 0 : 1) : 2], 1u);
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < NS; ++j) { q[j] = expf(p[j] - pm); den += q[j]; }
+    float l2 = 0.f;
+#pragma unroll
+    for (int j = 0; j < NS; ++j) { q[j] /= den; l2 += y[j] != 0 ? 0.f : q[j]; }
+#pragma unroll
+    for (int j = 0; j < NS; ++j) {
+      const float nc = y[j] != 0 ? 0.f : 1.f;
+      const float d = 0.1f * (p[j] - (1.f - nc)) / (float)NS + q[j] * (nc - l2) * p[j] * (1.f - p[j]);
+      if (dZ) dZ[(size_t)s * NS + j] = d * inv;
+      if (probs) probs[(size_t)s * NS + j] = p[j];
+    }
+    srow[2 * s] = 0.1f * bce / (float)NS + l2;
+    srow[2 * s + 1] = hit / (float)NS;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    double l = 0.0, h = 0.0;
+    for (int s = 0; s < n; ++s) { l += srow[2 * s]; h += srow[2 * s + 1]; }
+    if (stats) { stats[0] = (float)(l / n); stats[1] = (float)(h / n); }
+    if (acc) { acc[0] += l; acc[1] += h; acc[2] += n; }
+  }
+  if (acc) {
+    for (int i = tid; i < 2 * NBIN; i += NTH) acc[3 + i] += (double)hist[i / NBIN][i % NBIN];
+    if (tid < 3) acc[NACC + tid] += (double)cnt[tid];
+  }
+}
+
 }  // namespace r4st

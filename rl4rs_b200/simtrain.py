@@ -1,11 +1,12 @@
 """Training the DIEN user simulator on the logged data: ``script/supervised_train.py <train> <test> <model_file> dien 0`` without
-TensorFlow, from log text to the Saver checkpoint ``SlateRecEnv`` restores through ``config['model_file']``; and the
-slate-label nets on the same backbone, ``supervised_train.py ... dien_slate 1`` / ``dien_slate_multiclass 1``.
+TensorFlow, from log text to the Saver checkpoint ``SlateRecEnv`` restores through ``config['model_file']``; the
+slate-label nets on the same backbone, ``supervised_train.py ... dien_slate 1`` / ``dien_slate_multiclass 1``; and the
+slate-label nets on the dnn / widedeep / lstm backbones and adversarial_slate (SLATE_NETS, ``... lstm_slate 1`` etc.).
 
   item_samples(lines_or_path, config) -> ItemSamples   the samples of ``data_preprocess.py tfrecord_item`` (:91-131 with
                                                       ``FeatureUtil.feature_extraction``, datautil.py:34-69), kept per record
   slate_samples(lines_or_path, config) -> SlateSamples the samples of ``tfrecord_slate``: one per record, the same store
-  get_model(config, 'dien' | 'dien_slate' | 'dien_slate_multiclass') -> SimulatorTrainer: fit / evaluate / weights / save /
+  get_model(config, 'dien' | 'dien_slate' | 'dien_slate_multiclass' | SLATE_NETS) -> SimulatorTrainer: fit / evaluate / weights / save /
                                                       save_state / load_state
   supervised_train(train, test, model_file, model_type, is_slate_label)   the script, in its argument order
 
@@ -26,13 +27,20 @@ from .utils import tf_checkpoint
 from .utils.datautil import FeatureUtil
 
 NOT_BUILT = {"dnn": "the dnn simulator", "widedeep": "the widedeep simulator", "lstm": "the lstm simulator"}
-# the nets get_model trains -> the library's head (R4_SIMHEAD_*): nets/dien.py, dien_slate.py, dien_slate_multiclass.py
+# the DIEN nets get_model trains -> the library's head (R4_SIMHEAD_*): nets/dien.py, dien_slate.py, dien_slate_multiclass.py
 HEADS = {"dien": 0, "dien_slate": 1, "dien_slate_multiclass": 2}
-CLASSES = (2, 9, 22)                       # simulator_reward's width per head
-HISTORY = (("loss", "auc", "acc"), ("loss", "auc", "precision", "recall"), ("loss", "acc"))
-# the slate-label nets whose backbones (dnn, widedeep, lstm) or training (adversarial) are not built
-NOT_BUILT_SLATE = ("dnn_slate", "dnn_slate_multiclass", "widedeep_slate", "widedeep_slate_multiclass", "lstm_slate",
-                   "lstm_slate_multiclass", "adversarial_slate")
+# the backbones (R4_SIM_*, R4_SIMNET_ADVERSARIAL_SLATE) and head 3 (R4_SIMHEAD_ADVERSARIAL): adversarial_slate's loss
+NET_DIEN, NET_DNN, NET_WIDEDEEP, NET_LSTM, NET_ADV = range(5)
+HEAD_ADV = 3
+NET_NAMES = ("dien", "dnn", "widedeep", "lstm", "adversarial_slate")
+# the slate-label nets on the other backbones -> (net, head): nets/{dnn,widedeep,lstm}_slate[_multiclass].py, adversarial_slate.py
+SLATE_NETS = {"dnn_slate": (1, 1), "dnn_slate_multiclass": (1, 2), "widedeep_slate": (2, 1), "widedeep_slate_multiclass": (2, 2),
+              "lstm_slate": (3, 1), "lstm_slate_multiclass": (3, 2), "adversarial_slate": (4, 3)}
+CLASSES = (2, 9, 22, 9)                    # simulator_reward's width per head (adversarial_slate: dense_2's 9 columns)
+HISTORY = (("loss", "auc", "acc"), ("loss", "auc", "precision", "recall"), ("loss", "acc"),
+           ("loss", "auc", "precision", "recall"))
+# the slate-label nets not built (all of them are)
+NOT_BUILT_SLATE = ()
 # dien_slate_multiclass.py:8-11: the class of a page's click pattern y[9] is y . SLATE2LABEL (0..21)
 SLATE2LABEL = np.array([1, 2, 4, 1, 2, 4, 1, 2, 4], np.int64)
 # the fit schedule of supervised_train.py:38-42 and the Keras defaults it leaves (INTEGRATION.md section 8)
@@ -212,18 +220,26 @@ def _load_samples(src, config, head=0):
 
 
 # ---- the torch twin -------------------------------------------------------------------------------------------------
-def layer_plan(config):
-    """[(W-table name, shape)] in the flat parameter order (tf_checkpoint.dien_layer_plan, the C-ABI's layout)."""
-    return [(name, tuple(shape)) for name, _, shape in tf_checkpoint.dien_layer_plan(config)]
+PLANS = (tf_checkpoint.dien_layer_plan, tf_checkpoint.dnn_layer_plan, tf_checkpoint.widedeep_layer_plan,
+         tf_checkpoint.lstm_layer_plan, tf_checkpoint.adversarial_slate_layer_plan)
+SAVERS = (tf_checkpoint.save_dien_checkpoint, tf_checkpoint.save_dnn_checkpoint, tf_checkpoint.save_widedeep_checkpoint,
+          tf_checkpoint.save_lstm_checkpoint, tf_checkpoint.save_adversarial_slate_checkpoint)
+LOADERS = (tf_checkpoint.load_dien_checkpoint, tf_checkpoint.load_dnn_checkpoint, tf_checkpoint.load_widedeep_checkpoint,
+           tf_checkpoint.load_lstm_checkpoint, tf_checkpoint.load_adversarial_slate_checkpoint)
 
 
-def flatten(weights, config):
-    return np.concatenate([np.asarray(weights[k], np.float32).reshape(-1) for k, _ in layer_plan(config)])
+def layer_plan(config, net=NET_DIEN):
+    """[(W-table name, shape)] in the flat parameter order (tf_checkpoint.<net>_layer_plan, the C-ABI's layout)."""
+    return [(name, tuple(shape)) for name, _, shape in PLANS[net](config)]
 
 
-def unflatten(flat, config):
+def flatten(weights, config, net=NET_DIEN):
+    return np.concatenate([np.asarray(weights[k], np.float32).reshape(-1) for k, _ in layer_plan(config, net)])
+
+
+def unflatten(flat, config, net=NET_DIEN):
     out, o = {}, 0
-    for k, shape in layer_plan(config):
+    for k, shape in layer_plan(config, net):
         n = int(np.prod(shape))
         out[k] = flat[o:o + n].reshape(shape)
         o += n
@@ -323,6 +339,109 @@ class SimulatorNet(torch.nn.Module):
         return obs @ w["rew_w"] + w["rew_b"], obs
 
 
+def net_weights(config, net, head=0, seed=synth.WEIGHT_SEED, stress=1.0, bias_noise=0.0, **kw):
+    """A backbone's W-table with Keras default initialisers and the head's width: head_weights for dien,
+    synth.make_{dnn,widedeep,lstm}_weights (kw: make_lstm_weights' gru_stress / gru_bias_noise), adversarial_slate's plan
+    drawn as synth draws the plain nets."""
+    c = dict(config, class_num=CLASSES[head])
+    if net == NET_DIEN:
+        return head_weights(c, head, seed=seed, stress=stress, bias_noise=bias_noise, **kw)
+    if net == NET_DNN:
+        return synth.make_dnn_weights(c, seed, stress, bias_noise)
+    if net == NET_WIDEDEEP:
+        return synth.make_widedeep_weights(c, seed, stress, bias_noise)
+    if net == NET_LSTM:
+        return synth.make_lstm_weights(c, seed, stress, bias_noise, **kw)
+    return synth._make_plain(layer_plan(c, NET_ADV), seed, stress, bias_noise)
+
+
+def keras_gru(x, k, rk, b, margins=None):
+    """The last state of a Keras-v1 GRU (TF 1.15 recurrent.GRU: tanh, hard sigmoid clip(0.2 a + 0.5, 0, 1), reset_after
+    = False, one bias, gates [z | r | h], h0 = 0, no masking) over x [n, T, E].  torch's clamp passes the gradient at both
+    kinks, as TF's minimum / maximum do (INTEGRATION.md section 8).  margins (a list, may be None) receives per step the
+    smallest distance of a hard-sigmoid argument from 0 or 1."""
+    n, T, _ = x.shape
+    U = rk.shape[0]
+    h = x.new_zeros(n, U)
+    xp = x @ k + b
+    for t in range(T):
+        a = 0.2 * (xp[:, t, :2 * U] + h @ rk[:, :2 * U]) + 0.5
+        if margins is not None:
+            margins.append(float(torch.minimum(a.detach().abs(), (a.detach() - 1.0).abs()).min()))
+        zr = a.clamp(0.0, 1.0)
+        z, r = zr[:, :U], zr[:, U:]
+        hh = torch.tanh(xp[:, t, 2 * U:] + (r * h) @ rk[:, 2 * U:])
+        h = z * h + (1.0 - z) * hh
+    return h
+
+
+class BackboneNet(torch.nn.Module):
+    """nets/{dnn,widedeep,lstm}*.py and adversarial_slate.py in training mode over a flat parameter vector (the net's
+    layer plan): the CPU path of the trainer and, in float64, the kernels' reference.  logits(cat, dense, seq, keep, rate)
+    -> (z [n, C], obs): obs is the head's input (dnn / lstm: simulator_obs; widedeep: the 3072-wide simulator_obs
+    Concatenate; adversarial_slate: the 512-wide concatenation).  forward applies the head's activation (softmax for heads
+    0 and 2, sigmoid for 1 and 3).  After a forward of the lstm net, margin is the smallest distance of any hard-sigmoid
+    argument from its kinks at 0 and 1."""
+
+    def __init__(self, config, net, flat=None, dtype=torch.float32, seed=synth.WEIGHT_SEED, head=0):
+        super().__init__()
+        self.net, self.head = int(net), int(head)
+        self.config = dict(config, class_num=CLASSES[head])
+        if flat is None:
+            flat = flatten(net_weights(self.config, self.net, self.head, seed=seed), self.config, self.net)
+        self.flat = torch.nn.Parameter(torch.as_tensor(np.asarray(flat)).to(dtype).clone())
+        self.margin = math.inf
+
+    def tensors(self):
+        return unflatten(self.flat, self.config, self.net)
+
+    def forward(self, cat, dense, seq, keep=None, rate=DROPOUT):
+        z, obs = self.logits(cat, dense, seq, keep, rate)
+        return (torch.sigmoid(z) if self.head in (1, HEAD_ADV) else torch.softmax(z, -1)), obs
+
+    def logits(self, cat, dense, seq, keep=None, rate=DROPOUT):
+        w = self.tensors()
+        dt, dev = self.flat.dtype, self.flat.device
+        elu = torch.nn.functional.elu
+
+        def t(x, dtype):
+            return (x if torch.is_tensor(x) else torch.as_tensor(np.asarray(x))).to(dev, dtype)
+        cat, seq, dense = t(cat, torch.int64), t(seq, torch.int64), t(dense, dt)
+        n = cat.shape[0]
+        ec = w["emb_cat"][cat]
+        x = elu(dense @ w["dense_w1"] + w["dense_b1"])
+        if keep is not None:
+            k0, k1 = keep_scale(t(keep, torch.uint8), rate)
+            x = x * k0.to(dt)
+        x = elu(x @ w["dense_w2"] + w["dense_b2"])
+        if keep is not None:
+            x = x * k1.to(dt)
+        if self.net == NET_DNN:
+            f = elu(torch.cat([ec.mean(1), x], -1) @ w["fc_w"] + w["fc_b"])
+            obs = elu(f @ w["obs_w"] + w["obs_b"])
+        elif self.net == NET_WIDEDEEP:
+            sp = torch.cat([w["emb_seq"][seq[:, i]].mean(1) for i in range(SEQ_NUM)], -1)
+            obs = torch.cat([elu(sp @ w["fc_w"] + w["fc_b"]), x, ec.reshape(n, -1)], -1)
+        elif self.net == NET_LSTM:
+            margins = []
+            sg = [keras_gru(w["emb_seq"][seq[:, i]], w["sgru%d_k" % i], w["sgru%d_rk" % i], w["sgru%d_b" % i], margins)
+                  for i in range(SEQ_NUM)]
+            cg = keras_gru(ec, w["cgru_k"], w["cgru_rk"], w["cgru_b"], margins)
+            self.margin = min(margins)
+            obs = elu(torch.cat(sg + [x, cg, ec.reshape(n, -1)], -1) @ w["obs_w"] + w["obs_b"])
+        else:
+            sp = [w["emb_seq"][seq[:, i]].mean(1) for i in range(SEQ_NUM)]
+            obs = torch.cat(sp + [x, ec[:, :NCAT - 1].mean(1)], -1)
+        return obs @ w["rew_w"] + w["rew_b"], obs
+
+
+def twin(config, net, flat=None, dtype=torch.float32, head=0, seed=synth.WEIGHT_SEED):
+    """The torch twin of (net, head): SimulatorNet for dien, BackboneNet for the others."""
+    if net == NET_DIEN:
+        return SimulatorNet(config, flat, dtype, seed=seed, head=head)
+    return BackboneNet(config, net, flat, dtype, seed=seed, head=head)
+
+
 def keras_bce(probs, labels):
     """Keras binary_crossentropy of softmax probabilities against one_hot(labels, 2): p clipped to [1e-7, 1 - 1e-7] (zero
     gradient where clipped), the mean over both columns and the batch."""
@@ -350,8 +469,18 @@ def slate_cce_rows(logits, labels):
     return torch.nn.functional.cross_entropy(logits, cls, reduction="none")
 
 
+def adversarial_rows(logits, labels):
+    """adversarial_slate's loss per sample: 0.1 binary_crossentropy of its Sigmoid output from the logits (no clip, the
+    mean over the 9 columns) plus sum_j softmax(p)_j (1 - y_j), the softmax taken over p = sigmoid(z)."""
+    y = torch.as_tensor(np.asarray(labels), device=logits.device).to(logits.dtype)
+    q = torch.softmax(torch.sigmoid(logits), -1)
+    return 0.1 * slate_bce_rows(logits, labels) + (q * (1.0 - y)).sum(1)
+
+
 def loss_rows(head, logits, labels):
-    """The per-sample loss of a slate head (1, 2) from its logits; the batch loss is their mean."""
+    """The per-sample loss of a slate head (1, 2, 3) from its logits; the batch loss is their mean."""
+    if head == HEAD_ADV:
+        return adversarial_rows(logits, labels)
     return slate_bce_rows(logits, labels) if head == 1 else slate_cce_rows(logits, labels)
 
 
@@ -456,7 +585,7 @@ class MulticlassMetrics(object):
         return {"loss": self.acc[0] / n, "acc": self.acc[1] / n}
 
 
-METRICS = (Metrics, SlateMetrics, MulticlassMetrics)
+METRICS = (Metrics, SlateMetrics, MulticlassMetrics, SlateMetrics)
 
 
 # ---- the trainer ----------------------------------------------------------------------------------------------------
@@ -481,20 +610,26 @@ class SimulatorTrainer(object):
     """The compiled `dien` simulator of supervised_train.py: Keras Adam (lr 1e-3), binary_crossentropy, dropout 0.2 in the
     dense tower, metrics AUC and acc.  device 'cuda[:k]' runs the kernels, 'cpu' the torch twin.  head 1 / 2 (HEADS) is the
     compiled dien_slate / dien_slate_multiclass on SlateSamples: the same backbone and Adam, their own head, loss and
-    metrics (HISTORY)."""
+    metrics (HISTORY).  net (NET_NAMES) picks the backbone: 1..3 the dnn / widedeep / lstm graphs with heads 0..2, 4
+    adversarial_slate with head 3 (SLATE_NETS)."""
 
-    def __init__(self, config, device=None, seed=synth.WEIGHT_SEED, data_seed=0, weights=None, head=0):
-        if head not in (0, 1, 2):
-            raise ValueError("head must be 0 (dien), 1 (dien_slate) or 2 (dien_slate_multiclass), not %r" % (head,))
-        self.head = int(head)
+    def __init__(self, config, device=None, seed=synth.WEIGHT_SEED, data_seed=0, weights=None, head=0, net=NET_DIEN):
+        if net == NET_ADV and head != HEAD_ADV or net != NET_ADV and head not in (0, 1, 2) or net not in range(5):
+            raise ValueError("(net, head) must be a dien / dnn / widedeep / lstm net (0..3) with head 0 (item), 1 (slate) or "
+                             "2 (slate_multiclass), or adversarial_slate (4) with head 3, not (%r, %r)" % (net, head))
+        self.head, self.net = int(head), int(net)
         self.config = dict(config, class_num=CLASSES[head]) if head else dict(config)
         self.H = _check_config(self.config, self.head)
         self.config["category_hash_size"] = self.H
         self.device = torch.device(device or ("cuda" if torch.cuda.is_available() else "cpu"))
         self.data_seed = int(data_seed)
-        w = weights if weights is not None else head_weights(self.config, self.head, seed=seed)
-        flat = torch.from_numpy(flatten(w, self.config)).to(self.device)
-        if self.head and flat.numel() != sum(int(np.prod(s)) for _, s in layer_plan(self.config)):
+        if weights is not None:
+            w = weights
+        else:
+            w = head_weights(self.config, self.head, seed=seed) if self.net == NET_DIEN else net_weights(self.config, self.net,
+                                                                                                          self.head, seed=seed)
+        flat = torch.from_numpy(flatten(w, self.config, self.net)).to(self.device)
+        if self.head and flat.numel() != sum(int(np.prod(s)) for _, s in layer_plan(self.config, self.net)):
             raise ValueError("the weights do not fit the %d-wide head" % CLASSES[head])
         self.step = 0
         self.m = torch.zeros_like(flat)
@@ -502,7 +637,7 @@ class SimulatorTrainer(object):
         self._uploaded = {}
         if self.device.type == "cuda":
             self.lib = _capi.load_library()
-            if self.lib.r4_simtrain_head_num_params(self.head, self.H) != flat.numel():
+            if self.lib.r4_simtrain_net_num_params(self.net, self.head, self.H) != flat.numel():
                 raise ValueError("category_hash_size %d is outside the library's range" % self.H)
             self.params = flat
             self.grad = torch.zeros_like(flat)
@@ -511,24 +646,26 @@ class SimulatorTrainer(object):
                                    device=self.device)
             self.stats = torch.zeros(2, dtype=torch.float32, device=self.device)
         else:
-            self.net = SimulatorNet(self.config, flat.numpy(), torch.float32, head=self.head)
+            self.twin = twin(self.config, self.net, flat.numpy(), torch.float32, head=self.head)
 
     # -- parameters --
     def flat_params(self):
-        return (self.params if self.device.type == "cuda" else self.net.flat.data).detach()
+        return (self.params if self.device.type == "cuda" else self.twin.flat.data).detach()
 
     def weights(self):
-        """The W-table {name: float32 array} (what save_dien_checkpoint writes and the env loads)."""
+        """The W-table {name: float32 array} (what save_<net>_checkpoint writes and the env loads)."""
         flat = self.flat_params().cpu().numpy()
-        return {k: np.array(v) for k, v in unflatten(flat, self.config).items()}
+        return {k: np.array(v) for k, v in unflatten(flat, self.config, self.net).items()}
 
     def save(self, model_file):
-        """A TF1 Saver-format checkpoint at the prefix model_file (SlateRecEnv's config['model_file'])."""
-        return tf_checkpoint.save_dien_checkpoint(model_file, self.weights(), self.config)
+        """A TF1 Saver-format checkpoint at the prefix model_file (SlateRecEnv's config['model_file']) through the net's
+        layer plan."""
+        return SAVERS[self.net](model_file, self.weights(), self.config)
 
     def save_state(self, path):
         np.savez(path, params=self.flat_params().cpu().numpy(), m=self.m.cpu().numpy(), v=self.v.cpu().numpy(),
-                 step=np.int64(self.step), hash_size=np.int64(self.H), **({"head": np.int64(self.head)} if self.head else {}))
+                 step=np.int64(self.step), hash_size=np.int64(self.H), **({"head": np.int64(self.head)} if self.head else {}),
+                 **({"net": np.int64(self.net)} if self.net else {}))
 
     def load_state(self, path):
         z = np.load(path)
@@ -537,6 +674,9 @@ class SimulatorTrainer(object):
         head = int(z["head"]) if "head" in z else 0
         if head != self.head:
             raise ValueError("state was saved for head %d, not %d" % (head, self.head))
+        net = int(z["net"]) if "net" in z else NET_DIEN
+        if net != self.net:
+            raise ValueError("state was saved for net %s, not %s" % (NET_NAMES[net], NET_NAMES[self.net]))
         self.flat_params().copy_(torch.from_numpy(z["params"]))
         self.m.copy_(torch.from_numpy(z["m"]))
         self.v.copy_(torch.from_numpy(z["v"]))
@@ -554,7 +694,7 @@ class SimulatorTrainer(object):
 
     def _scratch(self, n):
         if self.scratch is None or self.scratch_n < n:
-            size = self.lib.r4_simtrain_head_scratch_size(self.head, n)
+            size = self.lib.r4_simtrain_net_scratch_size(self.net, self.head, n)
             if size < 0:
                 raise ValueError("batch size %d is outside 1..4096" % n)
             self.scratch = torch.empty(size, dtype=torch.uint8, device=self.device)
@@ -573,7 +713,7 @@ class SimulatorTrainer(object):
         n = int(idx.numel())
         if self.device.type == "cuda":
             d = self._data(samples)
-            rc = self.lib.r4_simtrain_head_step(self.head, self.H, ptr(self.params), ptr(self.grad), ptr(self.m), ptr(self.v),
+            rc = self.lib.r4_simtrain_net_step(self.net, self.head, self.H, ptr(self.params), ptr(self.grad), ptr(self.m), ptr(self.v),
                                                 C.byref(d), ptr(idx), n, self.data_seed, counter, rate, self.step, ADAM["lr"],
                                                 ADAM["beta1"], ADAM["beta2"], ADAM["eps"], ptr(self._scratch(n)), ptr(self.stats),
                                                 ptr(self.acc), _capi.stream(self.device))
@@ -583,25 +723,25 @@ class SimulatorTrainer(object):
         gen = torch.Generator().manual_seed(self.data_seed * 1000003 + counter)
         keep = (torch.rand(n, 256, generator=gen) >= rate).to(torch.uint8) if rate > 0 else None
         if self.head:
-            z, _ = self.net.logits(cat, dense, seq, keep, rate)
+            z, _ = self.twin.logits(cat, dense, seq, keep, rate)
             rows = loss_rows(self.head, z, y)
-            self.net.flat.grad = None
+            self.twin.flat.grad = None
             rows.mean().backward()
-            keras_adam_(self.net.flat.data, self.net.flat.grad, self.m, self.v, self.step)
+            keras_adam_(self.twin.flat.data, self.twin.flat.grad, self.m, self.v, self.step)
             if metrics is not None:
                 metrics.add(self._activate(z).detach().numpy(), y, rows.detach().numpy())
             return
-        probs, _ = self.net(cat, dense, seq, keep, rate)
+        probs, _ = self.twin(cat, dense, seq, keep, rate)
         loss = keras_bce(probs, y)
-        self.net.flat.grad = None
+        self.twin.flat.grad = None
         loss.backward()
-        keras_adam_(self.net.flat.data, self.net.flat.grad, self.m, self.v, self.step)
+        keras_adam_(self.twin.flat.data, self.twin.flat.grad, self.m, self.v, self.step)
         if metrics is not None:
             p = probs.detach().numpy()
             metrics.add(p, y, _bce_rows(p, y))
 
     def _activate(self, z):
-        return torch.sigmoid(z) if self.head == 1 else torch.softmax(z, -1)
+        return torch.sigmoid(z) if self.head in (1, HEAD_ADV) else torch.softmax(z, -1)
 
     def eval_batch(self, samples, idx, metrics=None):
         """probs f32[n, C] of the samples idx without dropout (accumulating the metrics on the CUDA path into self.acc)."""
@@ -609,20 +749,20 @@ class SimulatorTrainer(object):
         if self.device.type == "cuda":
             d = self._data(samples)
             probs = torch.empty(n, CLASSES[self.head], dtype=torch.float32, device=self.device)
-            rc = self.lib.r4_simtrain_head_eval(self.head, self.H, ptr(self.params), C.byref(d), ptr(idx), n, ptr(self._scratch(n)),
+            rc = self.lib.r4_simtrain_net_eval(self.net, self.head, self.H, ptr(self.params), C.byref(d), ptr(idx), n, ptr(self._scratch(n)),
                                                 ptr(probs), ptr(self.acc), _capi.stream(self.device))
             self._check(rc, "r4_simtrain_eval")
             return probs
         cat, dense, seq, y = samples.features(idx.numpy())
         if self.head:
             with torch.no_grad():
-                z, _ = self.net.logits(cat, dense, seq, None)
+                z, _ = self.twin.logits(cat, dense, seq, None)
                 probs = self._activate(z)
             if metrics is not None:
                 metrics.add(probs.numpy(), y, loss_rows(self.head, z, y).numpy())
             return probs
         with torch.no_grad():
-            probs, _ = self.net(cat, dense, seq, None)
+            probs, _ = self.twin(cat, dense, seq, None)
         p = probs.numpy()
         if metrics is not None:
             metrics.add(p, y, _bce_rows(p, y))
@@ -698,14 +838,19 @@ def _bce_rows(p, y):
 
 
 def get_model(config, model_type="dien", **kw):
-    """rl4rs.nets.<model_type>.get_model for training: 'dien', 'dien_slate' and 'dien_slate_multiclass' are built."""
+    """rl4rs.nets.<model_type>.get_model for training: 'dien', the slate-label nets 'dien_slate' and
+    'dien_slate_multiclass', and the SLATE_NETS on the other backbones ('{dnn,widedeep,lstm}_slate[_multiclass]',
+    'adversarial_slate') are built."""
+    if model_type in SLATE_NETS:
+        net, head = SLATE_NETS[model_type]
+        return SimulatorTrainer(config, head=head, net=net, **kw)
     if model_type in NOT_BUILT:
         raise NotImplementedError("%s: training %s is not built in this project" % (model_type, NOT_BUILT[model_type]))
     if model_type in NOT_BUILT_SLATE:
         raise NotImplementedError("%s: training this slate-label net is not built in this project (only dien_slate and "
                                   "dien_slate_multiclass are)" % model_type)
     if model_type not in HEADS:
-        raise NotImplementedError("%s: training the slate-label and other nets is not built in this project" % model_type)
+        raise NotImplementedError("%s: training this net is not built in this project" % model_type)
     return SimulatorTrainer(config, head=HEADS[model_type], **kw)
 
 
@@ -713,14 +858,14 @@ def supervised_train(train_file, test_file, model_file, model_type="dien", is_sl
                      verbose=2, **fit_kw):
     """script/supervised_train.py in its argument order.  train_file / test_file: log text (path or lines) or an ItemSamples
     .npz, where the script took TFRecords.  Trains, saves the Saver checkpoint at model_file and returns (trainer, history).
-    is_slate_label = 1 reads slate samples and trains dien_slate / dien_slate_multiclass; those nets need it (in the
-    reference the item samples' labels do not fit their heads)."""
-    slate_net = model_type in HEADS and HEADS[model_type] != 0
+    is_slate_label = 1 reads slate samples and trains the slate-label nets (dien_slate[_multiclass] and SLATE_NETS); those
+    nets need it (in the reference the item samples' labels do not fit their heads)."""
+    slate_net = model_type in HEADS and HEADS[model_type] != 0 or model_type in SLATE_NETS
     if int(is_slate_label) and not slate_net:
         if model_type in NOT_BUILT_SLATE:
             get_model({}, model_type)
-        raise NotImplementedError("is_slate_label = 1 with %s: only dien_slate and dien_slate_multiclass train on slate "
-                                  "labels in this project" % model_type)
+        raise NotImplementedError("is_slate_label = 1 with %s: only the slate-label nets train on slate labels in this "
+                                  "project" % model_type)
     if slate_net and not int(is_slate_label):
         raise ValueError("%s trains on slate labels: is_slate_label must be 1, not %r" % (model_type, is_slate_label))
     cfg = {"epoch": EPOCHS, "maxlen": 64, "batch_size": BATCH_SIZE, "class_num": 2, "dense_feature_num": 432,

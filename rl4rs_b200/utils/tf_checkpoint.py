@@ -528,6 +528,32 @@ def save_dnn_checkpoint(prefix, weights, config=None):
     return write_bundle(prefix, {names[k]: np.asarray(v, dtype=np.float32) for k, v in weights.items() if k in names})
 
 
+def adversarial_slate_layer_plan(config=None):
+    """nets/adversarial_slate.py in creation order: id_input_processing over the first 20 cat slots -> Embedding #0; dense
+    tower -> Dense #0, #1; sequence_input_concat -> Embedding #1; the unnamed Dense(9, sigmoid) -> Dense #2."""
+    cfg = config or {}
+    H, E, U = cfg.get("category_hash_size", 100000), cfg.get("emb_size", 128), cfg.get("hidden_units", 128)
+    D, S = cfg.get("dense_feature_num", 432), cfg.get("seq_num", 2)
+    return [("emb_cat", "embedding", (H, E)), ("dense_w1", "dense", (D, U)), ("dense_b1", "dense", (U,)),
+            ("dense_w2", "dense_1", (U, U)), ("dense_b2", "dense_1", (U,)), ("emb_seq", "embedding_1", (H, E)),
+            ("rew_w", "dense_2", (S * E + U + E, 9)), ("rew_b", "dense_2", (9,))]
+
+
+def adversarial_slate_variable_names(config=None):
+    inner = {"emb_cat": "embeddings", "emb_seq": "embeddings"}
+    return {name: scope + "/" + inner.get(name, "kernel" if name.endswith(("_w", "_w1", "_w2")) else "bias")
+            for name, scope, _ in adversarial_slate_layer_plan(config)}
+
+
+def load_adversarial_slate_checkpoint(prefix, config=None, name_map=None):
+    return _load_by_plan(prefix, adversarial_slate_layer_plan(config), adversarial_slate_variable_names(config), name_map)
+
+
+def save_adversarial_slate_checkpoint(prefix, weights, config=None):
+    names = adversarial_slate_variable_names(config)
+    return write_bundle(prefix, {names[k]: np.asarray(v, dtype=np.float32) for k, v in weights.items() if k in names})
+
+
 def save_dien_checkpoint(prefix, weights, config=None):
     """W-table -> Saver-style checkpoint under the expected TF1 variable names (inverse of load_dien_checkpoint)."""
     names = dien_variable_names(config)

@@ -2,7 +2,8 @@
 ms per optimiser step at batch 256 and 1024 over back-to-back steps, with the launches per step (counted by the library)
 and samples/s; one steps_per_epoch epoch (2343 steps of 256) plus its validation (1562 batches); the torch twin's step on
 the same card; and peak device memory.  Prints the card name and power limit read in the same run.  --model dien_slate /
-dien_slate_multiclass times the slate-label nets instead (one sample per record, so samples/s reads records/s; no twin).
+dien_slate_multiclass, {dnn,widedeep,lstm}_slate[_multiclass] or adversarial_slate times a slate-label net instead (one
+sample per record, so samples/s reads records/s; no twin).  --skip-epoch leaves out the epoch run.
 
     python tools/simtrain_time.py [--model dien] [--steps 50] [--epoch-steps 2343] [--val-steps 1562] [--records 20000]
 """
@@ -15,6 +16,7 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
+from rl4rs_b200.simtrain import SLATE_NETS  # noqa: E402
 
 
 def card():
@@ -27,12 +29,13 @@ def card():
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", default="dien", choices=["dien", "dien_slate", "dien_slate_multiclass"])
+    ap.add_argument("--model", default="dien", choices=["dien", "dien_slate", "dien_slate_multiclass"] + sorted(SLATE_NETS))
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--epoch-steps", type=int, default=600000 // 256)
     ap.add_argument("--val-steps", type=int, default=400000 // 256)
     ap.add_argument("--records", type=int, default=20000)
     ap.add_argument("--twin-steps", type=int, default=2)
+    ap.add_argument("--skip-epoch", action="store_true")
     a = ap.parse_args()
     import numpy as np
     import torch
@@ -64,6 +67,9 @@ def main():
         launches = (lib.r4_simtrain_launch_count() - l0) / a.steps
         print("batch %d: %.2f ms/step, %.0f launches/step, %.0f %s/s" % (B, dt * 1e3, launches, B / dt, unit))
         del tr
+    if a.skip_epoch:
+        print("peak device memory: %.2f GB" % (torch.cuda.max_memory_allocated() / 1e9))
+        return
     torch.cuda.reset_peak_memory_stats()
     tr = simtrain.get_model(cfg, a.model, device="cuda")
     test = R.make_samples(max(a.records // 4, 100), 100000, seed=1)
