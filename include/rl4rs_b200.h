@@ -572,7 +572,7 @@ int r4_simtrain_eval(int hash_size, const float* params, const r4_simtrain_data*
                      float* probs, double* acc, void* stream);
 /* ---- the slate-label heads on the same backbone (nets/dien_slate.py, nets/dien_slate_multiclass.py; supervised_train.py
  * <train> <test> <model> dien_slate[_multiclass] 1).  head selects simulator_reward's width C and the loss:
- *   R4_SIMHEAD_ITEM (C = 2): the r4_simtrain_* entry points above, exactly (they forward here).
+ *   R4_SIMHEAD_ITEM (C = 2): the r4_simtrain_* entry points above.
  *   R4_SIMHEAD_SLATE (C = 9): sigmoid output against the page's 9 clicks; binary cross-entropy from the logits (no clip),
  *     mean over the 9 columns and the n samples.  acc f64[408] = the 405 of the item head (accuracy: binary accuracy at
  *     0.5 per column; histograms over all 9 columns) then {TP, FP, FN} at p > 0.5.
@@ -581,7 +581,9 @@ int r4_simtrain_eval(int hash_size, const float* params, const r4_simtrain_data*
  * For the slate heads idx holds RECORD indices: sample s is record idx[s] (data_preprocess.py tfrecord_slate): cat = portrait
  * ids + [sequence_id] + the 9 items + the pad id 0, dense = portrait dense + item features + 40 zeros.  The flat layout is the
  * item head's with rew_w [256, C], rew_b [C]; scratch_size depends on the head.  Each entry point has the signature of its
- * r4_simtrain_* namesake with head first; probs is f32[n, C].  Bad head, hash_size or n: -1 or R4_ERR_ARG, nothing written. */
+ * r4_simtrain_* namesake with head first; probs is f32[n, C].  Bad head, hash_size or n: -1 or R4_ERR_ARG, nothing written.
+ * Each r4_simtrain_head_* is r4_simtrain_net_* below with net R4_SIM_DIEN, and each r4_simtrain_* is r4_simtrain_head_*
+ * with head R4_SIMHEAD_ITEM: one implementation, one argument check and the same results, launches and scratch layout. */
 enum { R4_SIMHEAD_ITEM = 0, R4_SIMHEAD_SLATE = 1, R4_SIMHEAD_SLATE_MULTICLASS = 2 };
 int64_t r4_simtrain_head_num_params(int head, int hash_size);
 int64_t r4_simtrain_head_scratch_size(int head, int n);
@@ -597,8 +599,8 @@ int r4_simtrain_head_eval(int head, int hash_size, const float* params, const r4
                           void* scratch, float* probs, double* acc, void* stream);
 /* ---- the other backbones and adversarial_slate (nets/dnn*.py, widedeep*.py, lstm*.py, adversarial_slate.py).  net is
  * an R4_SIM_* value or R4_SIMNET_ADVERSARIAL_SLATE; nets 0..3 take heads 0..2, net 4 only R4_SIMHEAD_ADVERSARIAL.  Each entry
- * point takes the arguments of its r4_simtrain_head_* namesake after net; net R4_SIM_DIEN forwards to it unchanged.  A bad
- * pair, hash_size or n: -1 or R4_ERR_ARG, nothing written.  The samples, keep bits, dropout, heads, acc layouts and Adam are
+ * point takes the arguments of its r4_simtrain_head_* namesake after net; net R4_SIM_DIEN is the DIEN net above.  A bad
+ * pair, hash_size, n, drop_rate or step, or a NULL pointer: -1 or R4_ERR_ARG ("bad argument"), nothing written.  The samples, keep bits, dropout, heads, acc layouts and Adam are
  * the DIEN heads' (R4_SIMHEAD_ADVERSARIAL: the R4_SIMHEAD_SLATE acc layout, f64[408]).  The flat layouts, with H =
  * hash_size, E = U = 128 and C the head's width (2, 9, 22; adversarial 9), in tf_checkpoint.*_layer_plan order:
  *   dnn       emb_cat[H,E] dense_w1[432,128] dense_b1 dense_w2[128,128] dense_b2 fc_w[256,256] fc_b obs_w[256,256] obs_b

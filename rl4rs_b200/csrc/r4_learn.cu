@@ -14,6 +14,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <initializer_list>
 #include <string>
 #include <vector>
 
@@ -784,21 +785,9 @@ int r4_batchrl_act(int algo, int obs_dim, int action_size, const float* params, 
 
 }  // extern "C"
 
-// ---- training the DIEN simulator (r4_simtrain.cuh) -------------------------------------------------------------------
+// ---- training the simulators (r4_simtrain.cuh): DIEN, the dnn / widedeep / lstm backbones and adversarial_slate --------
 // kernels launched by the r4_simtrain_* entry points in this process (the radix sort counted once)
 int64_t r4_simtrain_launch_count(void) { return g_launches[FAM_SIMTRAIN].load(std::memory_order_relaxed); }
-
-static bool st_hash_ok(int H) { return H >= 1 && H <= r4st::MAXH; }
-static bool st_head_ok(int head) { return head >= 0 && head < r4st::NHEAD; }
-
-int64_t r4_simtrain_head_num_params(int head, int hash_size) {
-  return st_head_ok(head) && st_hash_ok(hash_size) ? r4st::make_layout(hash_size, r4st::head_classes(head)).n : -1;
-}
-int64_t r4_simtrain_head_scratch_size(int head, int n) {
-  return (!st_head_ok(head) || n < 1 || n > r4st::MAXN) ? -1 : (int64_t)r4st::scratch_bytes(n, r4st::head_classes(head));
-}
-int64_t r4_simtrain_num_params(int hash_size) { return r4_simtrain_head_num_params(R4_SIMHEAD_ITEM, hash_size); }
-int64_t r4_simtrain_scratch_size(int n) { return r4_simtrain_head_scratch_size(R4_SIMHEAD_ITEM, n); }
 
 template <typename... P, typename... A>
 static int st_launch(const char* name, void (*kernel)(P...), dim3 grid, int threads, cudaStream_t st, A&&... args) {
@@ -820,20 +809,93 @@ static int st_gemm(bool tb, const float* A, int lda, const float* B, int ldb, co
   return st_launch("k_st_gemm", tb ? r4st::k_st_gemm<true> : r4st::k_st_gemm<false>, grid, r4st::NTH, st, g);
 }
 
-// The forward with saved activations: gather, towers, both sequences (GRU-1, attention, AUGRU), the head and the loss.
+// The pieces every net shares.  Lay / Pl are a net's layout and planes (Layout / Planes for DIEN, NLayout / NPlanes for the
+// others), which name the dense tower's weights and planes alike.
+// The dense tower with dropout: T1d = ELU(dense dw1 + db1) keep0 (T1 before the keep), out (ld ldo) = ELU(T1d dw2 + db2) keep1.
+template <class Lay, class Pl>
+static int st_tower(const Lay& L, const float* prm, const Pl& P, int n, float* out, int ldo, cudaStream_t st) {
+  using namespace r4st;
+  const int rc = st_gemm(false, P.dense, ND, prm + L.dw1, U, prm + L.db1, P.T1d, U, n, U, ND, EP_ELU, st, nullptr, P.keep, P.T1);
+  return rc ? rc : st_gemm(false, P.T1d, U, prm + L.dw2, U, prm + L.db2, out, ldo, n, U, U, EP_ELU, st, nullptr, P.keep + (size_t)n * U, P.T2);
+}
+// Its backward from the layer above: dT2 = (dtop W^T) elu'(T2) keep1, with W the rows of that layer's weight (ld wide) the
+// tower feeds, then dT1 = (dT2 dw2^T) elu'(T1) keep0.
+template <class Lay, class Pl>
+static int st_tower_bwd(const Lay& L, const float* prm, const Pl& P, int n, const float* dtop, const float* W, int ld, cudaStream_t st) {
+  using namespace r4st;
+  const int rc = st_gemm(true, dtop, ld, W, ld, nullptr, P.dT2, U, n, U, ld, EP_DELU, st, P.T2, P.keep + (size_t)n * U);
+  return rc ? rc : st_gemm(true, P.dT2, U, prm + L.dw2, U, nullptr, P.dT1, U, n, U, U, EP_DELU, st, P.T1, P.keep);
+}
+
+static r4ddpg::Job st_job(const float* X, int ldx, const float* Z, int M, int N, int64_t off) {
+  return r4ddpg::Job{X, Z, ldx, M, N, (int)off, 0};
+}
+// the tower's four weight-gradient jobs, the first of a net's n-row jobs; returns the job count
+template <class Lay, class Pl>
+static int st_tower_jobs(r4ddpg::Jobs& J, const Lay& L, const Pl& P) {
+  using namespace r4st;
+  int k = 0;
+  J.j[k++] = st_job(P.dense, ND, P.dT1, ND, U, L.dw1);  J.j[k++] = st_job(nullptr, 1, P.dT1, 1, U, L.db1);
+  J.j[k++] = st_job(P.T1d, U, P.dT2, U, U, L.dw2);      J.j[k++] = st_job(nullptr, 1, P.dT2, 1, U, L.db2);
+  return k;
+}
+static int st_wgrad(r4ddpg::Jobs J, int njob, int rows, float* grad, cudaStream_t st) {
+  J.njob = njob;
+  int t = 0;
+  for (int i = 0; i < njob; ++i) {
+    J.j[i].tile0 = t;
+    t += ((J.j[i].M + r4ddpg::WT - 1) / r4ddpg::WT) * ((J.j[i].N + r4ddpg::WT - 1) / r4ddpg::WT);
+  }
+  J.ntiles = t;
+  return st_launch("k_ddpg_wgrad", r4ddpg::k_ddpg_wgrad, t, r4ddpg::NT, st, J, rows, grad, nullptr, nullptr, 0.f);
+}
+
+// The head's loss: logits Z [n][C] -> dZ (may be NULL), the per-sample rows srow, stats, acc and probs.
+static int st_loss(int head, const r4st::Data& D, const int64_t* idx, int n, const float* Z, float* dZ, float* srow, float* stats,
+                   double* acc, float* probs, cudaStream_t st) {
+  using namespace r4st;
+  if (head == HEAD_ADV) return st_launch("k_st_loss_adv", k_st_loss_adv, 1, NTH, st, D, idx, n, Z, dZ, srow, stats, acc, probs);
+  if (head == HEAD_SLATE)
+    return st_launch("k_st_loss_slate<9>", k_st_loss_slate<NS>, 1, NTH, st, D, idx, n, Z, dZ, srow, stats, acc, probs);
+  if (head == HEAD_SLATE_MULTICLASS)
+    return st_launch("k_st_loss_slate<22>", k_st_loss_slate<NMC>, 1, NTH, st, D, idx, n, Z, dZ, srow, stats, acc, probs);
+  return st_launch("k_st_loss", k_st_loss, 1, NTH, st, D, idx, n, Z, dZ, srow, stats, acc, probs);
+}
+
+// The embedding gradients: keys of every (sample, slot), a stable radix sort by (table, id), one ordered sum per run.
+template <int NQ>
+static int st_embgrad(const r4st::Slots& sl, const r4st::Data& D, const int64_t* idx, int n, int slate, const int32_t* cat,
+                      const r4st::SortPlanes& sb, const float* dEcat, const float* dX0, const float* dX1, const float* dqs,
+                      float* grad, cudaStream_t st) {
+  const int total = n * r4st::slot_count<NQ>(sl);
+  int rc;
+  if ((rc = st_launch("k_st_embkeys", r4st::k_st_embkeys<NQ>, (total + 255) / 256, 256, st, sl, D, idx, n, slate, cat, sb.keys, sb.vals)))
+    return rc;
+  int bits = 1;
+  while (bits < 32 && ((uint64_t)1 << bits) < (uint64_t)(2 * sl.H)) ++bits;
+  cub::DoubleBuffer<uint32_t> kb(sb.keys, sb.keys2);
+  cub::DoubleBuffer<int32_t> vb(sb.vals, sb.vals2);
+  size_t need = 0;
+  if (cub::DeviceRadixSort::SortPairs(nullptr, need, kb, vb, total, 0, bits, st) != cudaSuccess || need > sb.cub_bytes)
+    return fail(R4_ERR_NOMEM, "r4_simtrain: radix sort temporary storage exceeds the scratch reserve");
+  size_t have = sb.cub_bytes;
+  if (cub::DeviceRadixSort::SortPairs(sb.cub_tmp, have, kb, vb, total, 0, bits, st) != cudaSuccess)
+    return fail(R4_ERR_CUDA, std::string("cub::DeviceRadixSort: ") + cudaGetErrorString(cudaGetLastError()));
+  count_launch(FAM_SIMTRAIN);      // the sort's own launches count as one
+  return st_launch("k_st_embsum", r4st::k_st_embsum<NQ>, total, r4st::EST, st, sl, kb.Current(), vb.Current(), total, dEcat, dX0, dX1,
+                   dqs, grad);
+}
+
+// DIEN's forward with saved activations: gather, towers, both sequences (GRU-1, attention, AUGRU), the head and the loss.
 static int st_forward(int head, const r4st::Layout& L, const float* prm, const r4st::Data& D, const int64_t* idx, int n,
                       uint64_t seed, uint64_t counter, float rate, const uint8_t* keep_in, uint8_t* keep_out, const r4st::Planes& P,
                       bool with_grad, float* stats, double* acc, float* probs, cudaStream_t st) {
   using namespace r4st;
   const int R = n * T, C = head_classes(head);
-  const GatherArgs ga{L, D, idx, n, seed, counter, rate, keep_in, keep_out, head != HEAD_ITEM};
+  const GatherArgs ga{L.H, D, idx, n, seed, counter, rate, keep_in, keep_out, head != HEAD_ITEM};
   int rc;
-  if ((rc = st_launch("k_st_gather", k_st_gather, n, E, st, ga, prm, P))) return rc;
-  const float* keep0 = P.keep;
-  const float* keep1 = P.keep + (size_t)n * U;
-  if ((rc = st_gemm(false, P.dense, ND, prm + L.dw1, U, prm + L.db1, P.T1d, U, n, U, ND, EP_ELU, st, nullptr, keep0, P.T1))) return rc;
-  if ((rc = st_gemm(false, P.T1d, U, prm + L.dw2, U, prm + L.db2, P.allf + F_DENSE, FEAT, n, U, U, EP_ELU, st, nullptr, keep1, P.T2)))
-    return rc;
+  if ((rc = st_launch("k_st_gather", k_st_gather, n, E, st, ga, L.emb_cat, L.emb_seq, prm, P))) return rc;
+  if ((rc = st_tower(L, prm, P, n, P.allf + F_DENSE, FEAT, st))) return rc;
   for (int i = 0; i < 2; ++i) {
     const Seq& w = L.s[i];
     const SeqPlanes& s = P.sp[i];
@@ -853,26 +915,7 @@ static int st_forward(int head, const r4st::Layout& L, const float* prm, const r
   }
   if ((rc = st_gemm(false, P.allf, FEAT, prm + L.ow, OBS, prm + L.ob, P.O, OBS, n, OBS, FEAT, EP_ELU, st))) return rc;
   if ((rc = st_gemm(false, P.O, OBS, prm + L.rw, C, prm + L.rb, P.Z, C, n, C, OBS, EP_LIN, st))) return rc;
-  float* dZ = with_grad ? P.dZ : nullptr;
-  if (head == HEAD_SLATE)
-    return st_launch("k_st_loss_slate<9>", k_st_loss_slate<NS>, 1, NTH, st, D, idx, n, P.Z, dZ, P.stats, stats, acc, probs);
-  if (head == HEAD_SLATE_MULTICLASS)
-    return st_launch("k_st_loss_slate<22>", k_st_loss_slate<NMC>, 1, NTH, st, D, idx, n, P.Z, dZ, P.stats, stats, acc, probs);
-  return st_launch("k_st_loss", k_st_loss, 1, NTH, st, D, idx, n, P.Z, dZ, P.stats, stats, acc, probs);
-}
-
-static r4ddpg::Job st_job(const float* X, int ldx, const float* Z, int M, int N, int64_t off) {
-  return r4ddpg::Job{X, Z, ldx, M, N, (int)off, 0};
-}
-static int st_wgrad(r4ddpg::Jobs J, int njob, int rows, float* grad, cudaStream_t st) {
-  J.njob = njob;
-  int t = 0;
-  for (int i = 0; i < njob; ++i) {
-    J.j[i].tile0 = t;
-    t += ((J.j[i].M + r4ddpg::WT - 1) / r4ddpg::WT) * ((J.j[i].N + r4ddpg::WT - 1) / r4ddpg::WT);
-  }
-  J.ntiles = t;
-  return st_launch("k_ddpg_wgrad", r4ddpg::k_ddpg_wgrad, t, r4ddpg::NT, st, J, rows, grad, nullptr, nullptr, 0.f);
+  return st_loss(head, D, idx, n, P.Z, with_grad ? P.dZ : nullptr, P.stats, stats, acc, probs, st);
 }
 
 static int st_backward(int head, const r4st::Layout& L, const float* prm, const r4st::Data& D, const int64_t* idx, int n,
@@ -883,10 +926,7 @@ static int st_backward(int head, const r4st::Layout& L, const float* prm, const 
   // head: dO = dZ rew_w^T elu'(O); dAllf = dO obs_w^T; the dense tower's columns again with its activation and dropout
   if ((rc = st_gemm(true, P.dZ, C, prm + L.rw, C, nullptr, P.dO, OBS, n, OBS, C, EP_DELU, st, P.O))) return rc;
   if ((rc = st_gemm(true, P.dO, OBS, prm + L.ow, OBS, nullptr, P.dAllf, FEAT, n, FEAT, OBS, EP_LIN, st))) return rc;
-  if ((rc = st_gemm(true, P.dO, OBS, prm + L.ow + (int64_t)F_DENSE * OBS, OBS, nullptr, P.dT2, U, n, U, OBS, EP_DELU, st, P.T2,
-                    P.keep + (size_t)n * U)))
-    return rc;
-  if ((rc = st_gemm(true, P.dT2, U, prm + L.dw2, U, nullptr, P.dT1, U, n, U, U, EP_DELU, st, P.T1, P.keep))) return rc;
+  if ((rc = st_tower_bwd(L, prm, P, n, P.dO, prm + L.ow + (int64_t)F_DENSE * OBS, OBS, st))) return rc;
   if ((rc = st_launch("k_st_cat_bwd", k_st_cat_bwd, n, E, st, P.allf, P.P, P.dAllf, P.dEcat))) return rc;
   for (int i = 0; i < 2; ++i) {
     const Seq& w = L.s[i];
@@ -911,9 +951,7 @@ static int st_backward(int head, const r4st::Layout& L, const float* prm, const 
   }
   // dense weight gradients: one launch over the n-row jobs, one per sequence over its 64 n-row jobs
   r4ddpg::Jobs J;
-  int k = 0;
-  J.j[k++] = st_job(P.dense, ND, P.dT1, ND, U, L.dw1);  J.j[k++] = st_job(nullptr, 1, P.dT1, 1, U, L.db1);
-  J.j[k++] = st_job(P.T1d, U, P.dT2, U, U, L.dw2);      J.j[k++] = st_job(nullptr, 1, P.dT2, 1, U, L.db2);
+  int k = st_tower_jobs(J, L, P);
   J.j[k++] = st_job(P.allf, FEAT, P.dO, FEAT, OBS, L.ow); J.j[k++] = st_job(nullptr, 1, P.dO, 1, OBS, L.ob);
   J.j[k++] = st_job(P.O, OBS, P.dZ, OBS, C, L.rw);      J.j[k++] = st_job(nullptr, 1, P.dZ, 1, C, L.rb);
   if ((rc = st_wgrad(J, k, n, grad, st))) return rc;
@@ -934,127 +972,19 @@ static int st_backward(int head, const r4st::Layout& L, const float* prm, const 
     J.j[k++] = st_job(nullptr, 1, s.XC2, 1, 2 * E, w.ubc);
     if ((rc = st_wgrad(J, k, R, grad, st))) return rc;
   }
-  // embedding gradients: keys, a stable radix sort by (table, id), one ordered sum per run
-  const int total = n * NSLOT;
+  // embedding gradients: the 21 cat slots, both sequences and the query's 10 emb_seq slots (dqs)
   if ((rc = st_launch("k_st_dq", k_st_dq, (n * E + 255) / 256, 256, st, P.sp[0].dq, P.sp[1].dq, P.dqs, n))) return rc;
-  if ((rc = st_launch("k_st_embkeys", k_st_embkeys, (total + 255) / 256, 256, st, L, D, idx, n, (int)(head != HEAD_ITEM), P.cat, P.keys,
-                       P.vals))) return rc;
-  int bits = 1;
-  while (bits < 32 && ((uint64_t)1 << bits) < (uint64_t)(2 * L.H)) ++bits;
-  cub::DoubleBuffer<uint32_t> kb(P.keys, P.keys2);
-  cub::DoubleBuffer<int32_t> vb(P.vals, P.vals2);
-  size_t need = 0;
-  if (cub::DeviceRadixSort::SortPairs(nullptr, need, kb, vb, total, 0, bits, st) != cudaSuccess || need > P.cub_bytes)
-    return fail(R4_ERR_NOMEM, "r4_simtrain: radix sort temporary storage exceeds the scratch reserve");
-  size_t have = P.cub_bytes;
-  if (cub::DeviceRadixSort::SortPairs(P.cub_tmp, have, kb, vb, total, 0, bits, st) != cudaSuccess)
-    return fail(R4_ERR_CUDA, std::string("cub::DeviceRadixSort: ") + cudaGetErrorString(cudaGetLastError()));
-  count_launch(FAM_SIMTRAIN);      // the sort's own launches count as one
-  return st_launch("k_st_embsum", k_st_embsum, total, EST, st, L, kb.Current(), vb.Current(), total, P.dEcat, P.sp[0].dX,
-                   P.sp[1].dX, P.dqs, grad);
+  const Slots sl{L.H, L.emb_cat, L.emb_seq, NC, 2 * T};
+  return st_embgrad<10>(sl, D, idx, n, head != HEAD_ITEM, P.cat, P.sort, P.dEcat, P.sp[0].dX, P.sp[1].dX, P.dqs, grad, st);
 }
 
-static int st_apply(int head, int H, float* params, float* grad, float* m, float* v, int step, float lr, float b1, float b2,
-                    float eps, cudaStream_t st) {
-  const r4st::Layout L = r4st::make_layout(H, r4st::head_classes(head));
-  const double alpha = (double)lr * std::sqrt(1.0 - std::pow((double)b2, step)) / (1.0 - std::pow((double)b1, step));
-  return st_launch("k_st_apply", r4st::k_st_apply, (unsigned)((L.n + 255) / 256), 256, st, L, params, grad, m, v, (float)alpha,
-                   b1, b2, eps);
-}
-
-int r4_simtrain_head_grad(int head, int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n,
-                          uint64_t seed, uint64_t counter, float drop_rate, const uint8_t* keep_in, uint8_t* keep_out,
-                          void* scratch, float* grad, float* stats, double* acc, void* stream) {
-  if (!st_head_ok(head) || !st_hash_ok(hash_size) || !params || !st_data_ok(data) || !idx || n < 1 || n > r4st::MAXN ||
-      !(drop_rate >= 0.f) || !(drop_rate < 1.f) || !scratch || !grad)
-    return fail(R4_ERR_ARG, "r4_simtrain_grad: bad argument (head 0..2, hash_size 1..4000000, n 1..4096, drop_rate in [0, 1))");
-  const int C = r4st::head_classes(head);
-  const r4st::Layout L = r4st::make_layout(hash_size, C);
-  const r4st::Planes P = r4st::make_planes(scratch, n, C);
-  const r4st::Data D = st_data(data);
-  cudaStream_t st = S(stream);
-  int rc = st_forward(head, L, params, D, idx, n, seed, counter, drop_rate, keep_in, keep_out, P, true, stats, acc, nullptr, st);
-  return rc ? rc : st_backward(head, L, params, D, idx, n, P, grad, st);
-}
-
-int r4_simtrain_head_apply(int head, int hash_size, float* params, float* grad, float* m, float* v, int step, float lr,
-                           float beta1, float beta2, float eps, void* stream) {
-  if (!st_head_ok(head) || !st_hash_ok(hash_size) || !params || !grad || !m || !v || step < 1)
-    return fail(R4_ERR_ARG, "r4_simtrain_apply: bad argument");
-  return st_apply(head, hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, S(stream));
-}
-
-int r4_simtrain_head_step(int head, int hash_size, float* params, float* grad, float* m, float* v, const r4_simtrain_data* data,
-                          const int64_t* idx, int n, uint64_t seed, uint64_t counter, float drop_rate, int step, float lr,
-                          float beta1, float beta2, float eps, void* scratch, float* stats, double* acc, void* stream) {
-  if (!m || !v || step < 1) return fail(R4_ERR_ARG, "r4_simtrain_step: bad argument");
-  int rc = r4_simtrain_head_grad(head, hash_size, params, data, idx, n, seed, counter, drop_rate, nullptr, nullptr, scratch, grad,
-                                 stats, acc, stream);
-  return rc ? rc : st_apply(head, hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, S(stream));
-}
-
-int r4_simtrain_head_eval(int head, int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n,
-                          void* scratch, float* probs, double* acc, void* stream) {
-  if (!st_head_ok(head) || !st_hash_ok(hash_size) || !params || !st_data_ok(data) || !idx || n < 1 || n > r4st::MAXN || !scratch)
-    return fail(R4_ERR_ARG, "r4_simtrain_eval: bad argument");
-  const int C = r4st::head_classes(head);
-  const r4st::Layout L = r4st::make_layout(hash_size, C);
-  const r4st::Planes P = r4st::make_planes(scratch, n, C);
-  return st_forward(head, L, params, st_data(data), idx, n, 0, 0, 0.f, nullptr, nullptr, P, false, nullptr, acc, probs, S(stream));
-}
-
-// the item head's entry points
-int r4_simtrain_grad(int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n, uint64_t seed,
-                     uint64_t counter, float drop_rate, const uint8_t* keep_in, uint8_t* keep_out, void* scratch, float* grad,
-                     float* stats, double* acc, void* stream) {
-  return r4_simtrain_head_grad(R4_SIMHEAD_ITEM, hash_size, params, data, idx, n, seed, counter, drop_rate, keep_in, keep_out,
-                               scratch, grad, stats, acc, stream);
-}
-
-int r4_simtrain_apply(int hash_size, float* params, float* grad, float* m, float* v, int step, float lr, float beta1, float beta2,
-                      float eps, void* stream) {
-  return r4_simtrain_head_apply(R4_SIMHEAD_ITEM, hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, stream);
-}
-
-int r4_simtrain_step(int hash_size, float* params, float* grad, float* m, float* v, const r4_simtrain_data* data,
-                     const int64_t* idx, int n, uint64_t seed, uint64_t counter, float drop_rate, int step, float lr, float beta1,
-                     float beta2, float eps, void* scratch, float* stats, double* acc, void* stream) {
-  return r4_simtrain_head_step(R4_SIMHEAD_ITEM, hash_size, params, grad, m, v, data, idx, n, seed, counter, drop_rate, step, lr,
-                               beta1, beta2, eps, scratch, stats, acc, stream);
-}
-
-int r4_simtrain_eval(int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n, void* scratch,
-                     float* probs, double* acc, void* stream) {
-  return r4_simtrain_head_eval(R4_SIMHEAD_ITEM, hash_size, params, data, idx, n, scratch, probs, acc, stream);
-}
-
-// ---- the other simulator backbones (dnn, widedeep, lstm) and adversarial_slate (r4_simtrain.cuh) -----------------------
-static bool st_pair_ok(int net, int head) {
-  if (net == r4st::NET_ADV) return head == r4st::HEAD_ADV;
-  return net >= 0 && net < r4st::NET_ADV && st_head_ok(head);
-}
-static int st_net_classes(int head) { return head == r4st::HEAD_ADV ? r4st::NS : r4st::head_classes(head); }
-
-int64_t r4_simtrain_net_num_params(int net, int head, int hash_size) {
-  if (!st_pair_ok(net, head) || !st_hash_ok(hash_size)) return -1;
-  if (net == r4st::NET_DIEN) return r4_simtrain_head_num_params(head, hash_size);
-  return r4st::make_nlayout(net, hash_size, st_net_classes(head)).n;
-}
-int64_t r4_simtrain_net_scratch_size(int net, int head, int n) {
-  if (!st_pair_ok(net, head) || n < 1 || n > r4st::MAXN) return -1;
-  if (net == r4st::NET_DIEN) return r4_simtrain_head_scratch_size(head, n);
-  return (int64_t)r4st::make_nplanes(nullptr, r4st::make_nlayout(net, 1, st_net_classes(head)), n).bytes;
-}
-
-// The forward with saved activations: the embedding front, the dense tower, lstm's three GRUs, the net's dense layers,
-// the head and the loss.
+// A backbone's forward with saved activations: the embedding front, the dense tower, lstm's three GRUs, the net's dense
+// layers, the head and the loss.
 static int sn_forward(int head, const r4st::NLayout& L, const float* prm, const r4st::Data& D, const int64_t* idx, int n,
                       uint64_t seed, uint64_t counter, float rate, const uint8_t* keep_in, uint8_t* keep_out,
                       const r4st::NPlanes& P, bool with_grad, float* stats, double* acc, float* probs, cudaStream_t st) {
   using namespace r4st;
-  Layout LH{};
-  LH.H = L.H;
-  const GatherArgs ga{LH, D, idx, n, seed, counter, rate, keep_in, keep_out, head != HEAD_ITEM};
+  const GatherArgs ga{L.H, D, idx, n, seed, counter, rate, keep_in, keep_out, head != HEAD_ITEM};
   Front f{};
   f.ncp = L.ncp;
   if (L.net == NET_DNN) { f.cpool = P.A; f.ldc = L.FA; }
@@ -1066,10 +996,7 @@ static int sn_forward(int head, const r4st::NLayout& L, const float* prm, const 
   if ((rc = st_launch("k_st_front", k_st_front, n, E, st, ga, L.emb_cat, L.emb_seq, prm, P.cat, P.dense, P.keep, f))) return rc;
   float* tower = L.A_tower >= 0 ? P.A + L.A_tower : P.O + L.O_tower;
   const int ldt = L.A_tower >= 0 ? L.FA : L.FO;
-  if ((rc = st_gemm(false, P.dense, ND, prm + L.dw1, U, prm + L.db1, P.T1d, U, n, U, ND, EP_ELU, st, nullptr, P.keep, P.T1))) return rc;
-  if ((rc = st_gemm(false, P.T1d, U, prm + L.dw2, U, prm + L.db2, tower, ldt, n, U, U, EP_ELU, st, nullptr, P.keep + (size_t)n * U,
-                    P.T2)))
-    return rc;
+  if ((rc = st_tower(L, prm, P, n, tower, ldt, st))) return rc;
   if (L.net == NET_LSTM) {
     const int col[3] = {3 * U, 0, U};             // the category GRU's state after the tower; the sequence GRUs first
     for (int i = 0; i < 3; ++i) {
@@ -1091,21 +1018,13 @@ static int sn_forward(int head, const r4st::NLayout& L, const float* prm, const 
   }
   const float* hin = L.FO ? P.O : P.A;
   if ((rc = st_gemm(false, hin, L.FH, prm + L.rw, L.C, prm + L.rb, P.Z, L.C, n, L.C, L.FH, EP_LIN, st))) return rc;
-  float* dZ = with_grad ? P.dZ : nullptr;
-  if (head == HEAD_ADV) return st_launch("k_st_loss_adv", k_st_loss_adv, 1, NTH, st, D, idx, n, P.Z, dZ, P.srow, stats, acc, probs);
-  if (head == HEAD_SLATE)
-    return st_launch("k_st_loss_slate<9>", k_st_loss_slate<NS>, 1, NTH, st, D, idx, n, P.Z, dZ, P.srow, stats, acc, probs);
-  if (head == HEAD_SLATE_MULTICLASS)
-    return st_launch("k_st_loss_slate<22>", k_st_loss_slate<NMC>, 1, NTH, st, D, idx, n, P.Z, dZ, P.srow, stats, acc, probs);
-  return st_launch("k_st_loss", k_st_loss, 1, NTH, st, D, idx, n, P.Z, dZ, P.srow, stats, acc, probs);
+  return st_loss(head, D, idx, n, P.Z, with_grad ? P.dZ : nullptr, P.srow, stats, acc, probs, st);
 }
 
 static int sn_backward(int head, const r4st::NLayout& L, const float* prm, const r4st::Data& D, const int64_t* idx, int n,
                        const r4st::NPlanes& P, float* grad, cudaStream_t st) {
   using namespace r4st;
   const int C = L.C;
-  const float* keep0 = P.keep;
-  const float* keep1 = P.keep + (size_t)n * U;
   int rc;
   // the head and dense layers down to dA (the front's and GRUs' columns) and dT2 (the tower's output, with its activation
   // and dropout); Wt(w, r0) is the weight w from its row r0 on, read transposed
@@ -1131,10 +1050,7 @@ static int sn_backward(int head, const r4st::NLayout& L, const float* prm, const
     dtop = P.dZ; tower_r0 = L.A_tower; tower_ld = C;
   }
   const int64_t tw = L.net == NET_DNN ? L.fcw : L.net == NET_LSTM ? L.ow : L.rw;
-  if ((rc = st_gemm(true, dtop, tower_ld, Wt(tw, tower_r0, tower_ld), tower_ld, nullptr, P.dT2, U, n, U, tower_ld, EP_DELU, st, P.T2,
-                    keep1)))
-    return rc;
-  if ((rc = st_gemm(true, P.dT2, U, prm + L.dw2, U, nullptr, P.dT1, U, n, U, U, EP_DELU, st, P.T1, keep0))) return rc;
+  if ((rc = st_tower_bwd(L, prm, P, n, dtop, Wt(tw, tower_r0, tower_ld), tower_ld, st))) return rc;
   // the embedding front: pools and Flatten; lstm's GRUs (BPTT) and their input gradients
   FrontBack fb{};
   fb.ncp = L.ncp;
@@ -1161,9 +1077,7 @@ static int sn_backward(int head, const r4st::NLayout& L, const float* prm, const
   }
   // dense weight gradients over the n-row jobs
   r4ddpg::Jobs J;
-  int k = 0;
-  J.j[k++] = st_job(P.dense, ND, P.dT1, ND, U, L.dw1);  J.j[k++] = st_job(nullptr, 1, P.dT1, 1, U, L.db1);
-  J.j[k++] = st_job(P.T1d, U, P.dT2, U, U, L.dw2);      J.j[k++] = st_job(nullptr, 1, P.dT2, 1, U, L.db2);
+  int k = st_tower_jobs(J, L, P);
   if (L.net == NET_DNN) {
     J.j[k++] = st_job(P.A, L.FA, P.dF, L.FA, OBS, L.fcw); J.j[k++] = st_job(nullptr, 1, P.dF, 1, OBS, L.fcb);
     J.j[k++] = st_job(P.F, OBS, P.dO, OBS, OBS, L.ow);    J.j[k++] = st_job(nullptr, 1, P.dO, 1, OBS, L.ob);
@@ -1196,82 +1110,160 @@ static int sn_backward(int head, const r4st::NLayout& L, const float* prm, const
                         L.g[0].k, L.g[1].k, L.g[2].k)))
       return rc;
   }
-  // embedding gradients: keys, a stable radix sort by (table, id), one ordered sum per run
-  const int ns = nslots(L), total = n * ns;
-  if ((rc = st_launch("k_st_nembkeys", k_st_nembkeys, (total + 255) / 256, 256, st, L.H, D, idx, n, (int)(head != HEAD_ITEM), L.ncp,
-                       ns, P.cat, P.keys, P.vals)))
-    return rc;
-  int bits = 1;
-  while (bits < 32 && ((uint64_t)1 << bits) < (uint64_t)(2 * L.H)) ++bits;
-  cub::DoubleBuffer<uint32_t> kb(P.keys, P.keys2);
-  cub::DoubleBuffer<int32_t> vb(P.vals, P.vals2);
-  size_t need = 0;
-  if (cub::DeviceRadixSort::SortPairs(nullptr, need, kb, vb, total, 0, bits, st) != cudaSuccess || need > P.cub_bytes)
-    return fail(R4_ERR_NOMEM, "r4_simtrain: radix sort temporary storage exceeds the scratch reserve");
-  size_t have = P.cub_bytes;
-  if (cub::DeviceRadixSort::SortPairs(P.cub_tmp, have, kb, vb, total, 0, bits, st) != cudaSuccess)
-    return fail(R4_ERR_CUDA, std::string("cub::DeviceRadixSort: ") + cudaGetErrorString(cudaGetLastError()));
-  count_launch(FAM_SIMTRAIN);
-  return st_launch("k_st_nembsum", k_st_nembsum, total, EST, st, L.H, L.emb_cat, L.emb_seq, L.ncp, ns, kb.Current(), vb.Current(),
-                   total, (const float*)P.dEcat, (const float*)P.dX[0], (const float*)P.dX[1], grad);
+  // embedding gradients: the net's pooled / Flattened cat slots and, but for dnn, both sequences
+  const Slots sl{L.H, L.emb_cat, L.emb_seq, L.ncp, L.nseq};
+  return st_embgrad<0>(sl, D, idx, n, head != HEAD_ITEM, P.cat, P.sort, P.dEcat, P.dX[0], P.dX[1], nullptr, grad, st);
+}
+
+// One pass of (net, head) over n samples: the forward with saved activations, then, with grad, the backward into grad.
+static int st_pass(int net, int head, int H, const float* prm, const r4_simtrain_data* data, const int64_t* idx, int n,
+                   uint64_t seed, uint64_t counter, float rate, const uint8_t* keep_in, uint8_t* keep_out, void* scratch,
+                   float* grad, float* stats, double* acc, float* probs, cudaStream_t st) {
+  using namespace r4st;
+  const int C = head_classes(head);
+  const Data D = st_data(data);
+  int rc;
+  if (net == NET_DIEN) {
+    const Layout L = make_layout(H, C);
+    const Planes P = make_planes(scratch, n, C);
+    rc = st_forward(head, L, prm, D, idx, n, seed, counter, rate, keep_in, keep_out, P, grad != nullptr, stats, acc, probs, st);
+    return rc || !grad ? rc : st_backward(head, L, prm, D, idx, n, P, grad, st);
+  }
+  const NLayout L = make_nlayout(net, H, C);
+  const NPlanes P = make_nplanes(scratch, L, n);
+  rc = sn_forward(head, L, prm, D, idx, n, seed, counter, rate, keep_in, keep_out, P, grad != nullptr, stats, acc, probs, st);
+  return rc || !grad ? rc : sn_backward(head, L, prm, D, idx, n, P, grad, st);
+}
+
+// Keras Adam over every parameter of (net, head), clearing the embedding tables' gradient rows.
+static int st_apply(int net, int head, int H, float* params, float* grad, float* m, float* v, int step, float lr, float b1, float b2,
+                    float eps, cudaStream_t st) {
+  using namespace r4st;
+  const int C = head_classes(head);
+  int64_t np, emb_cat, emb_seq;
+  if (net == NET_DIEN) {
+    const Layout L = make_layout(H, C);
+    np = L.n; emb_cat = L.emb_cat; emb_seq = L.emb_seq;
+  } else {
+    const NLayout L = make_nlayout(net, H, C);
+    np = L.n; emb_cat = L.emb_cat; emb_seq = L.emb_seq >= 0 ? L.emb_seq : L.emb_cat;
+  }
+  const double alpha = (double)lr * std::sqrt(1.0 - std::pow((double)b2, step)) / (1.0 - std::pow((double)b1, step));
+  return st_launch("k_st_apply", k_st_apply, (unsigned)((np + 255) / 256), 256, st, np, (int64_t)H, emb_cat, emb_seq, params, grad,
+                   m, v, (float)alpha, b1, b2, eps);
+}
+
+// The one argument check of every entry point: the (net, head) pair, the hash size, n, the drop rate, the Adam step and the
+// pointers.  An entry point passes a valid value for what it does not take.
+static bool st_args_ok(int net, int head, int H, int n, float rate, int step, std::initializer_list<const void*> ptrs) {
+  using namespace r4st;
+  for (const void* p : ptrs)
+    if (!p) return false;
+  const bool pair = net == NET_ADV ? head == HEAD_ADV : net >= 0 && net < NET_ADV && head >= 0 && head < HEAD_ADV;
+  return pair && H >= 1 && H <= MAXH && n >= 1 && n <= MAXN && rate >= 0.f && rate < 1.f && step >= 1;
+}
+static int st_reject(const char* fn) {
+  return fail(R4_ERR_ARG, std::string(fn) + ": bad argument (nets 0..3 take heads 0..2, net 4 head 3; hash_size 1..4000000, "
+                                            "n 1..4096, drop_rate in [0, 1), step >= 1, no NULL pointer)");
+}
+
+int64_t r4_simtrain_net_num_params(int net, int head, int hash_size) {
+  if (!st_args_ok(net, head, hash_size, 1, 0.f, 1, {})) return -1;
+  const int C = r4st::head_classes(head);
+  return net == r4st::NET_DIEN ? r4st::make_layout(hash_size, C).n : r4st::make_nlayout(net, hash_size, C).n;
+}
+int64_t r4_simtrain_net_scratch_size(int net, int head, int n) {
+  if (!st_args_ok(net, head, 1, n, 0.f, 1, {})) return -1;
+  const int C = r4st::head_classes(head);
+  return (int64_t)(net == r4st::NET_DIEN ? r4st::scratch_bytes(n, C) : r4st::make_nplanes(nullptr, r4st::make_nlayout(net, 1, C), n).bytes);
 }
 
 int r4_simtrain_net_grad(int net, int head, int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx,
                          int n, uint64_t seed, uint64_t counter, float drop_rate, const uint8_t* keep_in, uint8_t* keep_out,
                          void* scratch, float* grad, float* stats, double* acc, void* stream) {
-  if (!st_pair_ok(net, head))
-    return fail(R4_ERR_ARG, "r4_simtrain_net_grad: bad (net, head): nets 0..3 take heads 0..2, net 4 head 3");
-  if (net == r4st::NET_DIEN)
-    return r4_simtrain_head_grad(head, hash_size, params, data, idx, n, seed, counter, drop_rate, keep_in, keep_out, scratch, grad,
-                                 stats, acc, stream);
-  if (!st_hash_ok(hash_size) || !params || !st_data_ok(data) || !idx || n < 1 || n > r4st::MAXN || !(drop_rate >= 0.f) ||
-      !(drop_rate < 1.f) || !scratch || !grad)
-    return fail(R4_ERR_ARG, "r4_simtrain_net_grad: bad argument (hash_size 1..4000000, n 1..4096, drop_rate in [0, 1))");
-  const r4st::NLayout L = r4st::make_nlayout(net, hash_size, st_net_classes(head));
-  const r4st::NPlanes P = r4st::make_nplanes(scratch, L, n);
-  const r4st::Data D = st_data(data);
-  cudaStream_t st = S(stream);
-  int rc = sn_forward(head, L, params, D, idx, n, seed, counter, drop_rate, keep_in, keep_out, P, true, stats, acc, nullptr, st);
-  return rc ? rc : sn_backward(head, L, params, D, idx, n, P, grad, st);
-}
-
-static int sn_apply(int net, int head, int H, float* params, float* grad, float* m, float* v, int step, float lr, float b1, float b2,
-                    float eps, cudaStream_t st) {
-  const r4st::Layout L = r4st::apply_layout(r4st::make_nlayout(net, H, st_net_classes(head)));
-  const double alpha = (double)lr * std::sqrt(1.0 - std::pow((double)b2, step)) / (1.0 - std::pow((double)b1, step));
-  return st_launch("k_st_apply", r4st::k_st_apply, (unsigned)((L.n + 255) / 256), 256, st, L, params, grad, m, v, (float)alpha,
-                   b1, b2, eps);
+  if (!st_args_ok(net, head, hash_size, n, drop_rate, 1, {params, idx, scratch, grad}) || !st_data_ok(data))
+    return st_reject("r4_simtrain_net_grad");
+  return st_pass(net, head, hash_size, params, data, idx, n, seed, counter, drop_rate, keep_in, keep_out, scratch, grad, stats, acc,
+                 nullptr, S(stream));
 }
 
 int r4_simtrain_net_apply(int net, int head, int hash_size, float* params, float* grad, float* m, float* v, int step, float lr,
                           float beta1, float beta2, float eps, void* stream) {
-  if (!st_pair_ok(net, head)) return fail(R4_ERR_ARG, "r4_simtrain_net_apply: bad (net, head)");
-  if (net == r4st::NET_DIEN) return r4_simtrain_head_apply(head, hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, stream);
-  if (!st_hash_ok(hash_size) || !params || !grad || !m || !v || step < 1) return fail(R4_ERR_ARG, "r4_simtrain_net_apply: bad argument");
-  return sn_apply(net, head, hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, S(stream));
+  if (!st_args_ok(net, head, hash_size, 1, 0.f, step, {params, grad, m, v})) return st_reject("r4_simtrain_net_apply");
+  return st_apply(net, head, hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, S(stream));
 }
 
 int r4_simtrain_net_step(int net, int head, int hash_size, float* params, float* grad, float* m, float* v,
                          const r4_simtrain_data* data, const int64_t* idx, int n, uint64_t seed, uint64_t counter, float drop_rate,
                          int step, float lr, float beta1, float beta2, float eps, void* scratch, float* stats, double* acc,
                          void* stream) {
-  if (!st_pair_ok(net, head)) return fail(R4_ERR_ARG, "r4_simtrain_net_step: bad (net, head)");
-  if (net == r4st::NET_DIEN)
-    return r4_simtrain_head_step(head, hash_size, params, grad, m, v, data, idx, n, seed, counter, drop_rate, step, lr, beta1, beta2,
-                                 eps, scratch, stats, acc, stream);
-  if (!m || !v || step < 1) return fail(R4_ERR_ARG, "r4_simtrain_net_step: bad argument");
-  int rc = r4_simtrain_net_grad(net, head, hash_size, params, data, idx, n, seed, counter, drop_rate, nullptr, nullptr, scratch, grad,
-                                stats, acc, stream);
-  return rc ? rc : sn_apply(net, head, hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, S(stream));
+  if (!st_args_ok(net, head, hash_size, n, drop_rate, step, {params, grad, m, v, idx, scratch}) || !st_data_ok(data))
+    return st_reject("r4_simtrain_net_step");
+  const int rc = st_pass(net, head, hash_size, params, data, idx, n, seed, counter, drop_rate, nullptr, nullptr, scratch, grad, stats,
+                         acc, nullptr, S(stream));
+  return rc ? rc : st_apply(net, head, hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, S(stream));
 }
 
 int r4_simtrain_net_eval(int net, int head, int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx,
                          int n, void* scratch, float* probs, double* acc, void* stream) {
-  if (!st_pair_ok(net, head)) return fail(R4_ERR_ARG, "r4_simtrain_net_eval: bad (net, head)");
-  if (net == r4st::NET_DIEN) return r4_simtrain_head_eval(head, hash_size, params, data, idx, n, scratch, probs, acc, stream);
-  if (!st_hash_ok(hash_size) || !params || !st_data_ok(data) || !idx || n < 1 || n > r4st::MAXN || !scratch)
-    return fail(R4_ERR_ARG, "r4_simtrain_net_eval: bad argument");
-  const r4st::NLayout L = r4st::make_nlayout(net, hash_size, st_net_classes(head));
-  const r4st::NPlanes P = r4st::make_nplanes(scratch, L, n);
-  return sn_forward(head, L, params, st_data(data), idx, n, 0, 0, 0.f, nullptr, nullptr, P, false, nullptr, acc, probs, S(stream));
+  if (!st_args_ok(net, head, hash_size, n, 0.f, 1, {params, idx, scratch}) || !st_data_ok(data))
+    return st_reject("r4_simtrain_net_eval");
+  return st_pass(net, head, hash_size, params, data, idx, n, 0, 0, 0.f, nullptr, nullptr, scratch, nullptr, nullptr, acc, probs,
+                 S(stream));
+}
+
+// DIEN's heads: net 0
+int64_t r4_simtrain_head_num_params(int head, int hash_size) { return r4_simtrain_net_num_params(R4_SIM_DIEN, head, hash_size); }
+int64_t r4_simtrain_head_scratch_size(int head, int n) { return r4_simtrain_net_scratch_size(R4_SIM_DIEN, head, n); }
+
+int r4_simtrain_head_grad(int head, int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n,
+                          uint64_t seed, uint64_t counter, float drop_rate, const uint8_t* keep_in, uint8_t* keep_out,
+                          void* scratch, float* grad, float* stats, double* acc, void* stream) {
+  return r4_simtrain_net_grad(R4_SIM_DIEN, head, hash_size, params, data, idx, n, seed, counter, drop_rate, keep_in, keep_out,
+                              scratch, grad, stats, acc, stream);
+}
+
+int r4_simtrain_head_apply(int head, int hash_size, float* params, float* grad, float* m, float* v, int step, float lr,
+                           float beta1, float beta2, float eps, void* stream) {
+  return r4_simtrain_net_apply(R4_SIM_DIEN, head, hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, stream);
+}
+
+int r4_simtrain_head_step(int head, int hash_size, float* params, float* grad, float* m, float* v, const r4_simtrain_data* data,
+                          const int64_t* idx, int n, uint64_t seed, uint64_t counter, float drop_rate, int step, float lr,
+                          float beta1, float beta2, float eps, void* scratch, float* stats, double* acc, void* stream) {
+  return r4_simtrain_net_step(R4_SIM_DIEN, head, hash_size, params, grad, m, v, data, idx, n, seed, counter, drop_rate, step, lr,
+                              beta1, beta2, eps, scratch, stats, acc, stream);
+}
+
+int r4_simtrain_head_eval(int head, int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n,
+                          void* scratch, float* probs, double* acc, void* stream) {
+  return r4_simtrain_net_eval(R4_SIM_DIEN, head, hash_size, params, data, idx, n, scratch, probs, acc, stream);
+}
+
+// DIEN's item head: net 0, head 0
+int64_t r4_simtrain_num_params(int hash_size) { return r4_simtrain_head_num_params(R4_SIMHEAD_ITEM, hash_size); }
+int64_t r4_simtrain_scratch_size(int n) { return r4_simtrain_head_scratch_size(R4_SIMHEAD_ITEM, n); }
+
+int r4_simtrain_grad(int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n, uint64_t seed,
+                     uint64_t counter, float drop_rate, const uint8_t* keep_in, uint8_t* keep_out, void* scratch, float* grad,
+                     float* stats, double* acc, void* stream) {
+  return r4_simtrain_head_grad(R4_SIMHEAD_ITEM, hash_size, params, data, idx, n, seed, counter, drop_rate, keep_in, keep_out,
+                               scratch, grad, stats, acc, stream);
+}
+
+int r4_simtrain_apply(int hash_size, float* params, float* grad, float* m, float* v, int step, float lr, float beta1, float beta2,
+                      float eps, void* stream) {
+  return r4_simtrain_head_apply(R4_SIMHEAD_ITEM, hash_size, params, grad, m, v, step, lr, beta1, beta2, eps, stream);
+}
+
+int r4_simtrain_step(int hash_size, float* params, float* grad, float* m, float* v, const r4_simtrain_data* data,
+                     const int64_t* idx, int n, uint64_t seed, uint64_t counter, float drop_rate, int step, float lr, float beta1,
+                     float beta2, float eps, void* scratch, float* stats, double* acc, void* stream) {
+  return r4_simtrain_head_step(R4_SIMHEAD_ITEM, hash_size, params, grad, m, v, data, idx, n, seed, counter, drop_rate, step, lr,
+                               beta1, beta2, eps, scratch, stats, acc, stream);
+}
+
+int r4_simtrain_eval(int hash_size, const float* params, const r4_simtrain_data* data, const int64_t* idx, int n, void* scratch,
+                     float* probs, double* acc, void* stream) {
+  return r4_simtrain_head_eval(R4_SIMHEAD_ITEM, hash_size, params, data, idx, n, scratch, probs, acc, stream);
 }

@@ -49,13 +49,16 @@ constexpr int MAXN = 4096;                      // samples per pass
 constexpr int MAXH = 4000000;                   // category_hash_size
 constexpr int NTH = 256;
 
-// ---- the heads: the item head of nets/dien.py and the two slate-label heads ----
-// A head sets the width C of simulator_reward ([OBS, C] + [C]) and whether a sample is (record idx / 9, item idx % 9) or the
-// record idx itself (the slate samples of data_preprocess.py tfrecord_slate: cat slot 20 and dense 392..431 are padding).
-enum { HEAD_ITEM = 0, HEAD_SLATE = 1, HEAD_SLATE_MULTICLASS = 2, NHEAD = 3 };
+// ---- the heads: the item head of nets/dien.py, the two slate-label heads and adversarial_slate's ----
+// A head sets the width C of simulator_reward ([OBS, C] + [C]), the loss, and whether a sample is (record idx / 9, item
+// idx % 9) or the record idx itself (the slate samples of data_preprocess.py tfrecord_slate: cat slot 20 and dense
+// 392..431 are padding).
+enum { HEAD_ITEM = 0, HEAD_SLATE = 1, HEAD_SLATE_MULTICLASS = 2, HEAD_ADV = 3 };
 constexpr int NS = 9;            // slate columns: one per exposed item
 constexpr int NMC = 22;          // click-pattern classes: sum_j y_j [1, 2, 4, 1, 2, 4, 1, 2, 4]_j in 0..21
-__host__ __device__ constexpr int head_classes(int head) { return head == HEAD_SLATE ? NS : head == HEAD_SLATE_MULTICLASS ? NMC : 2; }
+__host__ __device__ constexpr int head_classes(int head) {
+  return head == HEAD_SLATE || head == HEAD_ADV ? NS : head == HEAD_SLATE_MULTICLASS ? NMC : 2;
+}
 
 // ---- the flat parameter layout: tf_checkpoint.dien_layer_plan order ----
 struct Seq {
@@ -109,17 +112,30 @@ struct SeqPlanes {                       // R = 64 n rows each
   float *XG2, *XC2, *Hp2, *G2, *C2, *RH2;                // AUGRU (XG2 / XC2 hold dG2 / dC2 in the backward)
   float *dS, *dH1, *dA2, *dA1, *dAin, *dX, *dq;          // dq [n][E]
 };
+struct SortPlanes {                      // the embedding-gradient key sort over n * nslot entries
+  uint32_t *keys, *keys2;
+  int32_t *vals, *vals2;
+  void* cub_tmp;
+  size_t cub_bytes;
+};
+// The sort's four planes, cut last by a planes maker's take, then the radix sort's reserve at the end of the scratch.
+template <class Take>
+__host__ inline SortPlanes take_sort(Take& take, int n, int nslot) {
+  const size_t m = (size_t)n * nslot;
+  SortPlanes S;
+  S.keys = reinterpret_cast<uint32_t*>(take(m)); S.keys2 = reinterpret_cast<uint32_t*>(take(m));
+  S.vals = reinterpret_cast<int32_t*>(take(m)); S.vals2 = reinterpret_cast<int32_t*>(take(m));
+  S.cub_tmp = take(0);
+  S.cub_bytes = ((size_t)4 << 20) + (size_t)16 * m;
+  return S;
+}
 struct Planes {
   int32_t* cat;                          // [n][21]
   float *dense, *keep /* [2][n][U] keep scales */, *T1, *T1d, *T2, *allf, *P, *q, *O, *Z, *dZ, *dO, *dAllf, *dT1, *dT2, *dEcat, *dqs, *stats;
   SeqPlanes sp[2];
-  uint32_t *keys, *keys2;                // [n * NSLOT]
-  int32_t *vals, *vals2;
-  void* cub_tmp;
-  size_t cub_bytes;
+  SortPlanes sort;                       // n * NSLOT entries
   size_t bytes;                          // the end of the radix sort's reserve: the scratch size the layout needs
 };
-__host__ inline size_t cub_reserve(int n) { return ((size_t)4 << 20) + (size_t)16 * n * NSLOT; }
 
 // The planes are cut from the scratch in this order, each rounded up to 256 bytes, and the radix sort's reserve follows.
 // With base = nullptr only the offsets are formed: scratch_bytes is the end of the same cuts, so the size a caller
@@ -147,11 +163,8 @@ __host__ inline Planes make_planes(void* base, int n, int C = 2) {
     s.dS = take(R); s.dH1 = take(R * E); s.dA2 = take(R * A2); s.dA1 = take(R * A1); s.dAin = take(R * 4 * E);
     s.dX = take(R * E); s.dq = take((size_t)n * E);
   }
-  P.keys = reinterpret_cast<uint32_t*>(take((size_t)n * NSLOT)); P.keys2 = reinterpret_cast<uint32_t*>(take((size_t)n * NSLOT));
-  P.vals = reinterpret_cast<int32_t*>(take((size_t)n * NSLOT)); P.vals2 = reinterpret_cast<int32_t*>(take((size_t)n * NSLOT));
-  P.cub_tmp = reinterpret_cast<void*>(b + o);
-  P.cub_bytes = cub_reserve(n);
-  P.bytes = o + P.cub_bytes;
+  P.sort = take_sort(take, n, NSLOT);
+  P.bytes = o + P.sort.cub_bytes;
   return P;
 }
 __host__ inline size_t scratch_bytes(int n, int C = 2) { return make_planes(nullptr, n, C).bytes; }
@@ -173,7 +186,7 @@ __device__ __forceinline__ float drop_u(uint64_t seed, uint64_t counter, int s, 
 // scale is 1 / (1 - rate) (inverted dropout); rate 0 keeps every unit at scale 1.  keep_out (may be NULL) receives the bits.
 // ------------------------------------------------------------------------------------------------
 struct GatherArgs {
-  Layout L;
+  int64_t H;
   Data D;
   const int64_t* idx;
   int n;
@@ -183,37 +196,44 @@ struct GatherArgs {
   uint8_t* keep_out;
   int slate;
 };
-__global__ void __launch_bounds__(E) k_st_gather(GatherArgs g, const float* __restrict__ prm, Planes P) {
-  __shared__ float Es[NC][E + 1];
-  __shared__ float Ps[NC][NC];
-  __shared__ int ids[NC];
-  __shared__ float w[NC];
-  const int s = blockIdx.x, c = threadIdx.x;
+// The part every front shares, for sample s at thread c: the cat ids (into ids and cat), the dense features and the keep
+// scales ([layer][n][U]).  Returns the sample's record; ids is complete after the caller's next barrier.
+__device__ __forceinline__ int64_t gather_sample(const GatherArgs& g, int s, int c, int* ids, int32_t* cat,
+                                                 float* dense, float* keep) {
   const int64_t smp = g.idx[s], rec = g.slate ? smp : smp / 9;
   const int j = g.slate ? -1 : (int)(smp % 9);
   const Data& D = g.D;
-  const Layout& L = g.L;
   if (c < NC) {
     int id = c < 10 ? D.ucat[rec * 10 + c] : c == 10 ? D.seqid[rec] : c < 20 ? D.items[rec * 9 + c - 11] : j < 0 ? 0 : D.items[rec * 9 + j];
-    id = clampid(id, L.H);
+    id = clampid(id, g.H);
     ids[c] = id;
-    P.cat[(size_t)s * NC + c] = id;
+    cat[(size_t)s * NC + c] = id;
   }
   for (int k = c; k < ND; k += E) {
     const float v = k < 32 ? D.udense[rec * 32 + k] : k < 392 ? D.ifeat[rec * 360 + k - 32] : j < 0 ? 0.f : D.ifeat[rec * 360 + j * 40 + k - 392];
-    P.dense[(size_t)s * ND + k] = v;
+    dense[(size_t)s * ND + k] = v;
   }
   for (int u = c; u < 2 * U; u += E) {
     bool kept;
     if (g.keep_in) kept = g.keep_in[(size_t)s * 2 * U + u] != 0;
     else kept = g.rate <= 0.f || drop_u(g.seed, g.counter, s, u) >= g.rate;
     if (g.keep_out) g.keep_out[(size_t)s * 2 * U + u] = kept ? 1 : 0;
-    P.keep[((size_t)(u / U) * g.n + s) * U + u % U] = kept ? 1.f / (1.f - g.rate) : 0.f;   // [layer][n][U]
+    keep[((size_t)(u / U) * g.n + s) * U + u % U] = kept ? 1.f / (1.f - g.rate) : 0.f;
   }
+  return rec;
+}
+__global__ void __launch_bounds__(E) k_st_gather(GatherArgs g, int64_t emb_cat, int64_t emb_seq, const float* __restrict__ prm,
+                                                 Planes P) {
+  __shared__ float Es[NC][E + 1];
+  __shared__ float Ps[NC][NC];
+  __shared__ int ids[NC];
+  __shared__ float w[NC];
+  const int s = blockIdx.x, c = threadIdx.x;
+  const int64_t rec = gather_sample(g, s, c, ids, P.cat, P.dense, P.keep);
   __syncthreads();
   float* allf = P.allf + (size_t)s * FEAT;
   for (int r = 0; r < NC; ++r) {
-    const float v = __ldg(prm + L.emb_cat + (int64_t)ids[r] * E + c);
+    const float v = __ldg(prm + emb_cat + (int64_t)ids[r] * E + c);
     Es[r][c] = v;
     allf[F_FLAT + r * E + c] = v;
   }
@@ -245,13 +265,13 @@ __global__ void __launch_bounds__(E) k_st_gather(GatherArgs g, const float* __re
     for (int b = 0; b < NC; ++b) a = fmaf(w[b], Es[b][c], a);
     allf[F_CATT + c] = a / (float)NC;
     float q = 0.f;
-    for (int r = NC - 10; r < NC; ++r) q += __ldg(prm + L.emb_seq + (int64_t)ids[r] * E + c);
+    for (int r = NC - 10; r < NC; ++r) q += __ldg(prm + emb_seq + (int64_t)ids[r] * E + c);
     P.q[(size_t)s * E + c] = q / 10.f;
   }
   for (int i = 0; i < 2; ++i)
     for (int t = 0; t < T; ++t) {
-      const int id = clampid(D.seq[(rec * 2 + i) * T + t], L.H);
-      P.sp[i].X[((size_t)s * T + t) * E + c] = __ldg(prm + L.emb_seq + (int64_t)id * E + c);
+      const int id = clampid(g.D.seq[(rec * 2 + i) * T + t], g.H);
+      P.sp[i].X[((size_t)s * T + t) * E + c] = __ldg(prm + emb_seq + (int64_t)id * E + c);
     }
 }
 
@@ -745,31 +765,43 @@ __global__ void k_st_dq(const float* __restrict__ dq0, const float* __restrict__
 }
 
 // ------------------------------------------------------------------------------------------------
-// The embedding gradients.  Entry e = s * NSLOT + k of sample s: k < 21 the emb_cat slot k (source row dEcat[s][k]);
-// 21 <= k < 149 emb_seq for sequence (k - 21) / 64, step (k - 21) % 64 (source dX); k >= 149 emb_seq of cat slot 11 + (k - 149)
-// (the query, source dqs[s]).  key = table * H + id; a stable radix sort keeps equal keys in (s, k) order.  slate: the
-// sequences are record idx[s]'s, and the pad id 0 of cat slot 20 (in the query too) keys row 0 like any other id.
+// The embedding gradients of every net.  A sample has ncp emb_cat slots, nseq emb_seq sequence slots and NQ emb_seq query
+// slots (DIEN: 21, 128, 10; the backbones: 21 or 20, 128 or 0, 0).  Entry e = s * nslot + k of sample s: k < ncp the
+// emb_cat slot k (source row dEcat[s][k]); then emb_seq for sequence i = (k - ncp) / 64, step (k - ncp) % 64 (source
+// dX_i[s][t]); then emb_seq of cat slot 11 + the query slot (source dqs[s]).  key = table * H + id; a stable radix sort
+// keeps equal keys in (s, k) order.  slate: the sequences are record idx[s]'s, and the pad id 0 of cat slot 20 (in the
+// query too) keys row 0 like any other id.  NQ is the query slot count: 10 only in DIEN, whose slot count is then the
+// constant NSLOT (the one-CTA sum of a long run divides by it once per entry).
 // ------------------------------------------------------------------------------------------------
-__global__ void k_st_embkeys(Layout L, Data D, const int64_t* __restrict__ idx, int n, int slate, const int32_t* __restrict__ cat,
+struct Slots {
+  int64_t H, emb_cat, emb_seq;
+  int ncp, nseq;
+};
+template <int NQ>
+__host__ __device__ inline int slot_count(const Slots& sl) { return NQ ? NSLOT : sl.ncp + sl.nseq; }
+template <int NQ>
+__global__ void k_st_embkeys(Slots sl, Data D, const int64_t* __restrict__ idx, int n, int slate, const int32_t* __restrict__ cat,
                              uint32_t* __restrict__ keys, int32_t* __restrict__ vals) {
+  const int nslot = slot_count<NQ>(sl);
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= n * NSLOT) return;
-  const int s = e / NSLOT, k = e % NSLOT;
+  if (e >= n * nslot) return;
+  const int s = e / nslot, k = e % nslot;
   uint32_t key;
-  if (k < NC) {
+  if (k < sl.ncp) {
     key = (uint32_t)cat[s * NC + k];
-  } else if (k < NC + 2 * T) {
-    const int i = (k - NC) / T, t = (k - NC) % T;
+  } else if (!NQ || k < sl.ncp + sl.nseq) {
+    const int i = (k - sl.ncp) / T, t = (k - sl.ncp) % T;
     const int64_t rec = slate ? idx[s] : idx[s] / 9;
-    key = (uint32_t)(L.H + clampid(D.seq[(rec * 2 + i) * T + t], L.H));
+    key = (uint32_t)(sl.H + clampid(D.seq[(rec * 2 + i) * T + t], sl.H));
   } else {
-    key = (uint32_t)(L.H + cat[s * NC + NC - 10 + (k - NC - 2 * T)]);
+    key = (uint32_t)(sl.H + cat[s * NC + NC - 10 + (k - sl.ncp - sl.nseq)]);
   }
   keys[e] = key;
   vals[e] = e;
 }
 constexpr int EST = 512, ESG = EST / E;        // 4 row groups x 128 columns
-__global__ void __launch_bounds__(EST) k_st_embsum(Layout L, const uint32_t* __restrict__ keys, const int32_t* __restrict__ vals,
+template <int NQ>
+__global__ void __launch_bounds__(EST) k_st_embsum(Slots sl, const uint32_t* __restrict__ keys, const int32_t* __restrict__ vals,
                                                    int total, const float* __restrict__ dEcat, const float* __restrict__ dX0,
                                                    const float* __restrict__ dX1, const float* __restrict__ dqs,
                                                    float* __restrict__ grad) {
@@ -777,13 +809,13 @@ __global__ void __launch_bounds__(EST) k_st_embsum(Layout L, const uint32_t* __r
   const int i0 = blockIdx.x;
   const uint32_t key = keys[i0];
   if (i0 > 0 && keys[i0 - 1] == key) return;           // one CTA per run: the one at its first entry
-  const int c = threadIdx.x % E, grp = threadIdx.x / E;
+  const int c = threadIdx.x % E, grp = threadIdx.x / E, nslot = slot_count<NQ>(sl);
   float acc = 0.f;
   for (int i = i0 + grp; i < total && keys[i] == key; i += ESG) {
-    const int e = vals[i], s = e / NSLOT, k = e % NSLOT;
+    const int e = vals[i], s = e / nslot, k = e % nslot;
     const float* src;
-    if (k < NC) src = dEcat + ((size_t)s * NC + k) * E;
-    else if (k < NC + 2 * T) src = ((k - NC) / T ? dX1 : dX0) + ((size_t)s * T + (k - NC) % T) * E;
+    if (k < sl.ncp) src = dEcat + ((size_t)s * NC + k) * E;
+    else if (!NQ || k < sl.ncp + sl.nseq) src = ((k - sl.ncp) / T ? dX1 : dX0) + ((size_t)s * T + (k - sl.ncp) % T) * E;
     else src = dqs + (size_t)s * E;
     acc += src[c];
   }
@@ -792,7 +824,7 @@ __global__ void __launch_bounds__(EST) k_st_embsum(Layout L, const uint32_t* __r
   if (grp == 0) {
     float v = part[0][c];
     for (int g = 1; g < ESG; ++g) v += part[g][c];
-    const int64_t base = key < (uint32_t)L.H ? L.emb_cat + (int64_t)key * E : L.emb_seq + (int64_t)(key - L.H) * E;
+    const int64_t base = key < (uint32_t)sl.H ? sl.emb_cat + (int64_t)key * E : sl.emb_seq + (int64_t)(key - sl.H) * E;
     grad[base + c] = v;
   }
 }
@@ -801,19 +833,21 @@ __global__ void __launch_bounds__(EST) k_st_embsum(Layout L, const uint32_t* __r
 // Keras Adam (OptimizerV2 / ResourceApplyAdam): m += (g - m)(1 - b1), v += (g^2 - v)(1 - b2),
 // p -= alpha m / (sqrt(v) + eps) with alpha = lr sqrt(1 - b2^t) / (1 - b1^t).  Dense over every parameter (the sparse
 // embedding apply of OptimizerV2 decays m and v on every row too).  Clears the nonzero embedding gradient entries, so the
-// embedding part of grad is zero again for the next r4_simtrain_grad.
+// embedding part of grad is zero again for the next r4_simtrain_grad.  np parameters; the two H-row tables at emb_cat and
+// emb_seq (a net without a sequence table names its category table twice).
 // ------------------------------------------------------------------------------------------------
-__global__ void k_st_apply(Layout L, float* __restrict__ prm, float* __restrict__ grad, float* __restrict__ m,
-                           float* __restrict__ v, float alpha, float b1, float b2, float eps) {
+__global__ void k_st_apply(int64_t np, int64_t H, int64_t emb_cat, int64_t emb_seq, float* __restrict__ prm,
+                           float* __restrict__ grad, float* __restrict__ m, float* __restrict__ v, float alpha, float b1, float b2,
+                           float eps) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= L.n) return;
+  if (i >= np) return;
   const float g = grad[i];
   float mi = m[i], vi = v[i];
   mi += (g - mi) * (1.f - b1);
   vi += (g * g - vi) * (1.f - b2);
   prm[i] -= alpha * mi / (sqrtf(vi) + eps);
   m[i] = mi; v[i] = vi;
-  const bool emb = (i >= L.emb_cat && i < L.emb_cat + L.H * E) || (i >= L.emb_seq && i < L.emb_seq + L.H * E);
+  const bool emb = (i >= emb_cat && i < emb_cat + H * E) || (i >= emb_seq && i < emb_seq + H * E);
   if (emb && g != 0.f) grad[i] = 0.f;
 }
 
@@ -829,7 +863,6 @@ __global__ void k_st_apply(Layout L, float* __restrict__ prm, float* __restrict_
 //   adversarial  A = [mean E_s[seq0] | mean E_s[seq1] | tower | mean_20 E_c[cat[:20]]] (512); p = sigmoid(A W + b) (9)
 // ================================================================================================
 enum { NET_DIEN = 0, NET_DNN = 1, NET_WIDEDEEP = 2, NET_LSTM = 3, NET_ADV = 4, NNET = 5 };
-enum { HEAD_ADV = 3 };
 constexpr int NG3 = 3 * U;                       // a Keras GRU's fused gate width [z | r | h]
 constexpr int GROWS = E + U + 1;                 // a GRU's parameter rows: kernel [E], recurrent_kernel [U], bias [1]
 constexpr int ADV_NCAT = NC - 1;                 // adversarial_slate pools the first 20 cat slots
@@ -887,14 +920,6 @@ __host__ __device__ inline NLayout make_nlayout(int net, int64_t H, int C) {
   L.n = o;
   return L;
 }
-__host__ __device__ inline int nslots(const NLayout& L) { return L.ncp + L.nseq; }
-// the DIEN Layout k_st_apply reads: the parameter count and the tables whose gradient rows it clears (a net without a
-// sequence table names its category table twice)
-__host__ inline Layout apply_layout(const NLayout& N) {
-  Layout L{};
-  L.H = N.H; L.emb_cat = N.emb_cat; L.emb_seq = N.emb_seq >= 0 ? N.emb_seq : N.emb_cat; L.n = N.n;
-  return L;
-}
 
 struct GruPlanes { float *X, *XG, *Hp, *A, *HH, *RH, *dZR, *dHH; };   // R = T n rows ([R][E], [R][3U], [R][U], [R][2U] ...)
 struct NPlanes {
@@ -903,12 +928,9 @@ struct NPlanes {
   float* dX[2];                                  // [n][T][E] the sequence slots' gradient rows
   GruPlanes g[3];                                // lstm: the category GRU (21 steps, X = E_c[cat]), the two sequence GRUs
   float* gtmp;                                   // [3][GROWS][3U]: each GRU's [z|r] and h weight gradients before the merge
-  uint32_t *keys, *keys2;
-  int32_t *vals, *vals2;
-  void* cub_tmp;
-  size_t cub_bytes, bytes;
+  SortPlanes sort;                               // n * (ncp + nseq) entries
+  size_t bytes;
 };
-__host__ inline size_t ncub_reserve(int n, int nslot) { return ((size_t)4 << 20) + (size_t)16 * n * nslot; }
 __host__ inline NPlanes make_nplanes(void* base, const NLayout& L, int n) {
   NPlanes P{};
   const uintptr_t b = reinterpret_cast<uintptr_t>(base);
@@ -935,12 +957,8 @@ __host__ inline NPlanes make_nplanes(void* base, const NLayout& L, int n) {
     }
     P.gtmp = take((size_t)3 * GROWS * NG3);
   }
-  const int ns = nslots(L);
-  P.keys = reinterpret_cast<uint32_t*>(take(N * ns)); P.keys2 = reinterpret_cast<uint32_t*>(take(N * ns));
-  P.vals = reinterpret_cast<int32_t*>(take(N * ns)); P.vals2 = reinterpret_cast<int32_t*>(take(N * ns));
-  P.cub_tmp = reinterpret_cast<void*>(b + o);
-  P.cub_bytes = ncub_reserve(n, ns);
-  P.bytes = o + P.cub_bytes;
+  P.sort = take_sort(take, n, L.ncp + L.nseq);
+  P.bytes = o + P.sort.cub_bytes;
   return P;
 }
 
@@ -962,26 +980,7 @@ __global__ void __launch_bounds__(E) k_st_front(GatherArgs g, int64_t emb_cat, i
                                                 Front f) {
   __shared__ int ids[NC];
   const int s = blockIdx.x, c = threadIdx.x;
-  const int64_t smp = g.idx[s], rec = g.slate ? smp : smp / 9;
-  const int j = g.slate ? -1 : (int)(smp % 9);
-  const Data& D = g.D;
-  if (c < NC) {
-    int id = c < 10 ? D.ucat[rec * 10 + c] : c == 10 ? D.seqid[rec] : c < 20 ? D.items[rec * 9 + c - 11] : j < 0 ? 0 : D.items[rec * 9 + j];
-    id = clampid(id, g.L.H);
-    ids[c] = id;
-    catp[(size_t)s * NC + c] = id;
-  }
-  for (int k = c; k < ND; k += E) {
-    const float v = k < 32 ? D.udense[rec * 32 + k] : k < 392 ? D.ifeat[rec * 360 + k - 32] : j < 0 ? 0.f : D.ifeat[rec * 360 + j * 40 + k - 392];
-    densep[(size_t)s * ND + k] = v;
-  }
-  for (int u = c; u < 2 * U; u += E) {
-    bool kept;
-    if (g.keep_in) kept = g.keep_in[(size_t)s * 2 * U + u] != 0;
-    else kept = g.rate <= 0.f || drop_u(g.seed, g.counter, s, u) >= g.rate;
-    if (g.keep_out) g.keep_out[(size_t)s * 2 * U + u] = kept ? 1 : 0;
-    keepp[((size_t)(u / U) * g.n + s) * U + u % U] = kept ? 1.f / (1.f - g.rate) : 0.f;
-  }
+  const int64_t rec = gather_sample(g, s, c, ids, catp, densep, keepp);
   __syncthreads();
   float pool = 0.f;
   for (int r = 0; r < NC; ++r) {
@@ -996,7 +995,7 @@ __global__ void __launch_bounds__(E) k_st_front(GatherArgs g, int64_t emb_cat, i
     float* xs = i ? f.xs1 : f.xs0;
     float sum = 0.f;
     for (int t = 0; t < T; ++t) {
-      const int id = clampid(D.seq[(rec * 2 + i) * T + t], g.L.H);
+      const int id = clampid(g.D.seq[(rec * 2 + i) * T + t], g.H);
       const float v = __ldg(prm + emb_seq + (int64_t)id * E + c);
       sum += v;
       if (xs) xs[((size_t)s * T + t) * E + c] = v;
@@ -1215,53 +1214,6 @@ __global__ void k_st_kgru_merge(const float* __restrict__ tmp, float* __restrict
   const float* zr = tmp + (size_t)g * GROWS * NG3;
   const float* hc = zr + (size_t)GROWS * 2 * U;
   grad[(g == 0 ? g0 : g == 1 ? g1 : g2) + e] = c < 2 * U ? zr[r * 2 * U + c] : hc[r * U + c - 2 * U];
-}
-
-// ------------------------------------------------------------------------------------------------
-// The embedding gradients of a backbone: entry e = s * nslot + k; k < ncp the emb_cat slot k (source dEcat[s][k]), else
-// emb_seq for sequence (k - ncp) / 64, step (k - ncp) % 64 (source dX[i][s][t]).  Keys, the stable radix sort and the
-// ordered per-run sums as k_st_embkeys / k_st_embsum.
-// ------------------------------------------------------------------------------------------------
-__global__ void k_st_nembkeys(int64_t H, Data D, const int64_t* __restrict__ idx, int n, int slate, int ncp, int nslot,
-                              const int32_t* __restrict__ cat, uint32_t* __restrict__ keys, int32_t* __restrict__ vals) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= n * nslot) return;
-  const int s = e / nslot, k = e % nslot;
-  uint32_t key;
-  if (k < ncp) {
-    key = (uint32_t)cat[s * NC + k];
-  } else {
-    const int i = (k - ncp) / T, t = (k - ncp) % T;
-    const int64_t rec = slate ? idx[s] : idx[s] / 9;
-    key = (uint32_t)(H + clampid(D.seq[(rec * 2 + i) * T + t], H));
-  }
-  keys[e] = key;
-  vals[e] = e;
-}
-__global__ void __launch_bounds__(EST) k_st_nembsum(int64_t H, int64_t emb_cat, int64_t emb_seq, int ncp, int nslot,
-                                                    const uint32_t* __restrict__ keys, const int32_t* __restrict__ vals, int total,
-                                                    const float* __restrict__ dEcat, const float* __restrict__ dX0,
-                                                    const float* __restrict__ dX1, float* __restrict__ grad) {
-  __shared__ float part[ESG][E];
-  const int i0 = blockIdx.x;
-  const uint32_t key = keys[i0];
-  if (i0 > 0 && keys[i0 - 1] == key) return;
-  const int c = threadIdx.x % E, grp = threadIdx.x / E;
-  float acc = 0.f;
-  for (int i = i0 + grp; i < total && keys[i] == key; i += ESG) {
-    const int e = vals[i], s = e / nslot, k = e % nslot;
-    const float* src = k < ncp ? dEcat + ((size_t)s * NC + k) * E
-                               : ((k - ncp) / T ? dX1 : dX0) + ((size_t)s * T + (k - ncp) % T) * E;
-    acc += src[c];
-  }
-  part[grp][c] = acc;
-  __syncthreads();
-  if (grp == 0) {
-    float v = part[0][c];
-    for (int g = 1; g < ESG; ++g) v += part[g][c];
-    const int64_t base = key < (uint32_t)H ? emb_cat + (int64_t)key * E : emb_seq + (int64_t)(key - H) * E;
-    grad[base + c] = v;
-  }
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -265,6 +265,27 @@ def keep_scale(keep, rate):
     return k[:, :128], k[:, 128:]
 
 
+def twin_front(twin, cat, dense, seq, keep, rate):
+    """What every twin's forward opens with: its tensors w, cat / seq (int64) and dense on the parameters' device and dtype,
+    the emb_cat rows ec [n, 21, E] and the dense tower x [n, 128] with dropout (keep as in SimulatorNet.forward)."""
+    w = twin.tensors()
+    dt, dev = twin.flat.dtype, twin.flat.device
+    elu = torch.nn.functional.elu
+
+    def t(x, dtype):
+        return (x if torch.is_tensor(x) else torch.as_tensor(np.asarray(x))).to(dev, dtype)
+    cat, seq, dense = t(cat, torch.int64), t(seq, torch.int64), t(dense, dt)
+    ec = w["emb_cat"][cat]
+    x = elu(dense @ w["dense_w1"] + w["dense_b1"])
+    if keep is not None:
+        k0, k1 = keep_scale(t(keep, torch.uint8), rate)
+        x = x * k0.to(dt)
+    x = elu(x @ w["dense_w2"] + w["dense_b2"])
+    if keep is not None:
+        x = x * k1.to(dt)
+    return w, cat, seq, ec, x
+
+
 class SimulatorNet(torch.nn.Module):
     """nets/dien.py in training mode over a flat parameter vector: the CPU path of the trainer and the autograd reference of
     the kernels.  forward(cat, dense, seq, keep, rate) -> (probs [n, C], obs [n, 256]); keep (u8 [n, 256] or None: no dropout).
@@ -304,24 +325,10 @@ class SimulatorNet(torch.nn.Module):
         return (torch.sigmoid(z) if self.head == 1 else torch.softmax(z, -1)), obs
 
     def logits(self, cat, dense, seq, keep=None, rate=DROPOUT):
-        w = self.tensors()
-        dt, dev = self.flat.dtype, self.flat.device
-
-        def t(x, dtype):
-            return (x if torch.is_tensor(x) else torch.as_tensor(np.asarray(x))).to(dev, dtype)
-        cat, seq, dense = t(cat, torch.int64), t(seq, torch.int64), t(dense, dt)
+        w, cat, seq, ec, x = twin_front(self, cat, dense, seq, keep, rate)
         n = cat.shape[0]
-        ec = w["emb_cat"][cat]
         p = torch.softmax(ec @ ec.transpose(1, 2), -1)
         c1 = (p @ ec).mean(1)
-        x = torch.nn.functional.elu(dense @ w["dense_w1"] + w["dense_b1"])
-        k0 = k1 = None
-        if keep is not None:
-            k0, k1 = keep_scale(t(keep, torch.uint8), rate)
-            x = x * k0.to(dt)
-        x = torch.nn.functional.elu(x @ w["dense_w2"] + w["dense_b2"])
-        if keep is not None:
-            x = x * k1.to(dt)
         q = w["emb_seq"][cat[:, -10:]].mean(1)
         hs = []
         for i in range(SEQ_NUM):
@@ -400,22 +407,9 @@ class BackboneNet(torch.nn.Module):
         return (torch.sigmoid(z) if self.head in (1, HEAD_ADV) else torch.softmax(z, -1)), obs
 
     def logits(self, cat, dense, seq, keep=None, rate=DROPOUT):
-        w = self.tensors()
-        dt, dev = self.flat.dtype, self.flat.device
-        elu = torch.nn.functional.elu
-
-        def t(x, dtype):
-            return (x if torch.is_tensor(x) else torch.as_tensor(np.asarray(x))).to(dev, dtype)
-        cat, seq, dense = t(cat, torch.int64), t(seq, torch.int64), t(dense, dt)
+        w, cat, seq, ec, x = twin_front(self, cat, dense, seq, keep, rate)
         n = cat.shape[0]
-        ec = w["emb_cat"][cat]
-        x = elu(dense @ w["dense_w1"] + w["dense_b1"])
-        if keep is not None:
-            k0, k1 = keep_scale(t(keep, torch.uint8), rate)
-            x = x * k0.to(dt)
-        x = elu(x @ w["dense_w2"] + w["dense_b2"])
-        if keep is not None:
-            x = x * k1.to(dt)
+        elu = torch.nn.functional.elu
         if self.net == NET_DNN:
             f = elu(torch.cat([ec.mean(1), x], -1) @ w["fc_w"] + w["fc_b"])
             obs = elu(f @ w["obs_w"] + w["obs_b"])
