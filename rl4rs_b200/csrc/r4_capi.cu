@@ -184,6 +184,9 @@ int gemm(r4_env* e, int slot, int act, int M, int N, int K, const float* A, int 
          int ksplit_max = 1) {
   if (M <= 0) return R4_OK;
   if ((N & 15) || (K & 7) || (lda & 3) || (ldc & 3)) return fail(e, R4_ERR_ARG, "gemm: unaligned shape");
+  // the epilogue writes 16-byte column quads
+  if ((C && (reinterpret_cast<uintptr_t>(C) & 15)) || (tm_ns > 0 && (ldT & 3)))
+    return fail(e, R4_ERR_ARG, "gemm: output not 16-byte aligned");
   ProfScope ps(e, slot, st, 2.0 * M * N * K);
   r4tc::GemmTcParams p{A, lda, gather, Wimg, bias, C, ldc, M, N, K, act, tm_ns, cr_base, ldT, outT, outK};
   p.A2 = A2; p.gather2 = gather2; p.k2_start = k2_start; p.g2_n = g2_n;

@@ -23,6 +23,8 @@ constexpr int G_SMEM_BYTES = G_NST * G_STAGE_BYTES + G_RAW * G_RAW_BYTES;
 constexpr int G_THREADS = 256;                             // two warpgroups
 constexpr int G_A_SBO = (G_BK / 8) * 128;                  // 512
 constexpr int G_B_SBO = (G_BK / 8) * 128;                  // 512
+constexpr int G_CT_LD = G_BNMAX + 4;                       // output tile row stride in floats (rows 4 banks apart)
+static_assert(G_BM * G_CT_LD * 4 <= G_NST * G_STAGE_BYTES, "the output tile lives in the operand stages");
 
 // host-side description of a pre-tiled weight
 struct GemmImage {
@@ -299,39 +301,56 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_gemm_tc(GemmTcParams p) {
       wgmma_commit();
     }
     wgmma_wait<0>();
-    // ===== epilogue from the accumulator registers: a thread holds rows rl, rl + 8 and column pairs (2 tq, 2 tq + 1) =====
+    __syncthreads();                    // both warpgroups' wgmmas are done: the operand stages are free for the output tile
+    // ===== epilogue, through shared memory.  The accumulators are parked in the output tile ct (a thread holds rows
+    // rl, rl + 8 and column pairs (2 tq, 2 tq + 1)); then a rolled loop writes 4-column quads with 16-byte stores.  The loop
+    // is rolled on purpose: unrolled over the 128 registers, with the store layouts and ELU inlined at every site, the
+    // epilogue is ~15 k instructions run once per tile, and fetching them sets the time of a short-K tile. =====
+    float* ct = reinterpret_cast<float*>(smem);
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
       if (c >= nch) continue;
 #pragma unroll
-      for (int jj = 0; jj < 8; ++jj) {
-        const int cl = c * 64 + jj * 8 + 2 * tq;
-        if (cl >= bn) continue;
-        const int col = n0 + cl;
-        float2 bv = make_float2(0.f, 0.f);
-        if (ksp == 1 && p.bias) bv = make_float2(__ldg(p.bias + col), __ldg(p.bias + col + 1));
+      for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const int m = m0 + wg * 64 + wq * 16 + g + 8 * h;
-          if (m >= p.M) continue;
-          float2 v = make_float2(acc[c][jj * 4 + 2 * h], acc[c][jj * 4 + 2 * h + 1]);
-          if (ksp > 1) {            // split-K: raw partial sums, bias + activation in k_splitk_finish
-            *reinterpret_cast<float2*>(p.part + ((size_t)ks * p.M + m) * p.N + col) = v;
-            continue;
-          }
-          v.x += bv.x; v.y += bv.y;
-          if (p.act == 1) { v.x = v.x > 0.f ? v.x : expm1f(v.x); v.y = v.y > 0.f ? v.y : expm1f(v.y); }
-          if (p.tm_ns > 0) {
-            const int t = m / p.tm_ns, nabs = p.cr_base + m % p.tm_ns;
-            if (col >= p.ldT)       // ldT is even: a column pair lies on one side.  outK in the quad layout (kq_index)
-              *reinterpret_cast<float2*>(p.outK + kq_index(nabs, (p.N - p.ldT) / 4, (col - p.ldT) / 4, p.tm_steps, t) + ((col - p.ldT) & 3)) = v;
-            else
-              *reinterpret_cast<float2*>(p.outT + xt_index((size_t)(nabs / TM) * p.tm_steps + t, p.ldT, col, nabs % TM)) = v;
-          } else {
-            *reinterpret_cast<float2*>(p.C + (size_t)m * p.ldc + col) = v;
-          }
+          const int r = wg * 64 + wq * 16 + g + 8 * h;
+          *reinterpret_cast<float2*>(ct + r * G_CT_LD + c * 64 + jj * 8 + 2 * tq) =
+              make_float2(acc[c][jj * 4 + 2 * h], acc[c][jj * 4 + 2 * h + 1]);
         }
+    }
+    __syncthreads();
+    // sequence mode: consecutive threads take consecutive rows (= lanes of the lane-major layouts, 16 B apart);
+    // row-major outputs: consecutive quads of one row
+    const int nq = bn >> 2;
+    const bool seq = p.tm_ns > 0;
+    for (int i = tid; i < G_BM * nq; i += G_THREADS) {
+      const int r = seq ? i % G_BM : i / nq, q = seq ? i / G_BM : i % nq;
+      const int m = m0 + r;
+      if (m >= p.M) continue;
+      const int col = n0 + 4 * q;
+      float4 v = *reinterpret_cast<const float4*>(ct + r * G_CT_LD + 4 * q);
+      if (ksp > 1) {                    // split-K: raw partial sums, bias + activation in k_splitk_finish
+        *reinterpret_cast<float4*>(p.part + ((size_t)ks * p.M + m) * p.N + col) = v;
+        continue;
       }
+      float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (p.bias) bv = make_float4(__ldg(p.bias + col), __ldg(p.bias + col + 1), __ldg(p.bias + col + 2), __ldg(p.bias + col + 3));
+      v.x += bv.x; v.y += bv.y; v.z += bv.z; v.w += bv.w;
+      if (p.act == 1) {
+        v.x = v.x > 0.f ? v.x : expm1f(v.x); v.y = v.y > 0.f ? v.y : expm1f(v.y);
+        v.z = v.z > 0.f ? v.z : expm1f(v.z); v.w = v.w > 0.f ? v.w : expm1f(v.w);
+      }
+      float* dst;
+      if (seq) {
+        const int t = m / p.tm_ns, nabs = p.cr_base + m % p.tm_ns;
+        dst = col >= p.ldT       // ldT % 4 == 0: a quad lies on one side.  outK in the quad layout (kq_index)
+                  ? p.outK + kq_index(nabs, (p.N - p.ldT) / 4, (col - p.ldT) / 4, p.tm_steps, t)
+                  : p.outT + xt_index((size_t)(nabs / TM) * p.tm_steps + t, p.ldT, col, nabs % TM);
+      } else {
+        dst = p.C + (size_t)m * p.ldc + col;
+      }
+      *reinterpret_cast<float4*>(dst) = v;
     }
   }
   cp_async_wait<0>();
