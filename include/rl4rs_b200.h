@@ -630,9 +630,61 @@ int r4_simtrain_net_eval(int net, int head, int hash_size, const float* params, 
                          int n, void* scratch, float* probs, double* acc, void* stream);
 /* kernels launched so far by the r4_simtrain_* entry points in this process (the radix sort counted once) */
 int64_t r4_simtrain_launch_count(void);
+/* ---- Exact-K (nets/exact_k/model.py, script/exact_k_train.py): the pointer-network slate generator and its reward
+ * critic.  Every pointer is device memory; the work runs on stream.  fp32 row-major; one writer per output element, so
+ * results are deterministic.
+ *
+ * Generator (R4_EXACTK_GENERATOR), hidden_units 64 (D = 128), 4 heads, 2 blocks, one glimpse, one LSTM layer, res_length 9.
+ * Flat parameters, in this order (kernels [in, out]):
+ *   u_w[256,64] u_b[64] emb[500,64]
+ *   per block 0, 1: qkv_w[128,384] (Q | K | V columns) qkv_b[384] ln1_beta[128] ln1_gamma[128] ff1_w[128,256] ff1_b[256]
+ *                   ff2_w[256,128] ff2_b[128] ln2_beta[128] ln2_gamma[128]
+ *   lstm_w[256,512] (rows: input | h; columns: gates i | j | f | o) lstm_b[512] c0[128] x0[128] (first input) h0[128]
+ *   intra: W_b[128,128] v_dec[128] W_bef[128,128] bias_dec[128]
+ *   glimpse_0, then attention (the pointer), each: W_q[128,128] W_dec[128,128] v[128] bias[128] W_ref[128,128]
+ * Critic (R4_EXACTK_CRITIC): w1[256,128] b1 w2[128,128] b2 w3[128,128] b3 w4[128,1] b4[1]; relu on the three hidden layers.
+ *
+ * user: f32[n, 256]; n in 1..4096; seq_length T in 9..500 (the candidates are the item ids 0..T-1).  masks: u8[4, T], rows
+ * the location masks of positions 0-2, 3-5 and 6-8 and the special items; the point mask of position t is its location
+ * mask, minus the items already chosen, minus every special item once one is chosen (position 0: its location mask).
+ * Masked logits are -2^32 + 1.  dropout (the rate, in [0, 1)) is live on the encoder input and both blocks' attention
+ * probabilities; keep draws and the SAMPLE draws are U[0, 1) = (top 24 bits of a splitmix64 hash of (seed, call, stream,
+ * element)) / 2^24 (see r4_exactk.cuh: draw24), kept when U >= dropout.  SAMPLE picks the first candidate whose running
+ * sum of exp(logit / temperature - max) reaches (U + 2^-25) times their total. */
+enum { R4_EXACTK_GENERATOR = 0, R4_EXACTK_CRITIC = 1 };
+enum { R4_EXACTK_SAMPLE = 0, R4_EXACTK_GREEDY = 1, R4_EXACTK_TRAIN = 2 };
+/* parameter count of net; -1 for another net */
+int64_t r4_exactk_num_params(int net);
+/* BYTES of scratch the generator (net 0) or the critic (net 1, seq_length ignored) needs for n rows; -1 out of range */
+int64_t r4_exactk_scratch_size(int net, int n, int seq_length);
+/* The encoder and the nine decode steps: path i32[n, 9] (TRAIN: the teacher path on entry) and logits f32[n, 9, T] (may be
+ * NULL).  122 launches. */
+int r4_exactk_decode(const float* params, const float* user, int n, int seq_length, const uint8_t* masks, int mode,
+                     float temperature, uint64_t seed, uint64_t call, float dropout, int32_t* path, float* logits, void* scratch,
+                     void* stream);
+/* The teacher-forced forward on target i32[n, 9] and the gradient of mean_b(sum_t CE(logits[b, t], target[b, t]) reward[b])
+ * into grad f32[num_params] (overwritten); loss f32[1] (may be NULL).  349 launches (348 without loss).
+ * Targets (and the TRAIN path of r4_exactk_decode) are candidate indices in [0, T); an entry outside is clamped into it.
+ * After r4_exactk_decode or r4_exactk_grad the scratch begins with the encoder's activations, f32 planes in this order,
+ * each starting at a multiple of 64 floats: relu(user W_u + b_u) [n,64], X0 [n,T,128], then per block 0, 1: the key /
+ * query mask [n,T], relu(X W_qkv + b_qkv) [n,T,384], softmax [n,4,T,T], dropped probabilities [n,4,T,T], attention output
+ * [n,T,128], Y1 [n,T,128], its normalised input [n,T,128], 1 / std [n,T], relu(Y1 W_1 + b_1) [n,T,256], Y2 [n,T,128], its
+ * normalised input [n,T,128], 1 / std [n,T]. */
+int r4_exactk_grad(const float* params, const float* user, int n, int seq_length, const uint8_t* masks, const int32_t* target,
+                   const float* reward, uint64_t seed, uint64_t call, float dropout, float* grad, float* loss, void* scratch,
+                   void* stream);
+/* The critic: pred f32[n] (may be NULL); with target f32[n], also loss = sum_b (target - pred)^2 (f32[1], may be NULL) and
+ * its gradient into grad (overwritten).  5 launches without target, 27 with. */
+int r4_exactk_critic(const float* params, const float* user, int n, const float* target, float* pred, float* grad, float* loss,
+                     void* scratch, void* stream);
+/* TF1 AdamOptimizer step `step` (1-based) of net: m, v, params updated in place.  1 launch. */
+int r4_exactk_adam(int net, float* params, float* grad, float* m, float* v, int step, float lr, float beta1, float beta2,
+                   float eps, void* stream);
+/* kernels launched so far by the r4_exactk_* entry points in this process */
+int64_t r4_exactk_launch_count(void);
 /* kernels launched so far by every learner entry point in this process (r4_policy_*, r4_gae, r4_adam_step, r4_ppo_epoch*,
- * r4_grad_exchange*, r4_gauss_*, r4_vtrace, r4_impala_step, r4_ddpg_*, r4_replay_*, r4_rainbow_*, r4_batchrl_*, r4_simtrain_*): the sum of the batch
- * RL and simulator-trainer counts above and the online learners'. */
+ * r4_grad_exchange*, r4_gauss_*, r4_vtrace, r4_impala_step, r4_ddpg_*, r4_replay_*, r4_rainbow_*, r4_batchrl_*, r4_simtrain_*, r4_exactk_*): the
+ * sum of the batch RL, simulator-trainer and Exact-K counts above and the online learners'. */
 int64_t r4_learner_launch_count(void);
 
 #ifdef __cplusplus

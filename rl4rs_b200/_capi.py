@@ -175,6 +175,15 @@ EXPORTS = {
                              [C.c_void_p] * 4),
     "r4_simtrain_launch_count": (C.c_int64, []),
     "r4_learner_launch_count": (C.c_int64, []),
+    "r4_exactk_num_params": (C.c_int64, [C.c_int]),
+    "r4_exactk_scratch_size": (C.c_int64, [C.c_int, C.c_int, C.c_int]),
+    "r4_exactk_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_uint64,
+                                   C.c_uint64, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "r4_exactk_grad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
+                                 C.c_uint64, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "r4_exactk_critic": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 6),
+    "r4_exactk_adam": (C.c_int, [C.c_int] + [C.c_void_p] * 4 + [C.c_int] + [C.c_float] * 4 + [C.c_void_p]),
+    "r4_exactk_launch_count": (C.c_int64, []),
 }
 
 _lib = None

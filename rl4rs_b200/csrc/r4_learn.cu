@@ -1267,3 +1267,445 @@ int r4_simtrain_eval(int hash_size, const float* params, const r4_simtrain_data*
                      float* probs, double* acc, void* stream) {
   return r4_simtrain_head_eval(R4_SIMHEAD_ITEM, hash_size, params, data, idx, n, scratch, probs, acc, stream);
 }
+
+// ---- Exact-K (r4_exactk.cuh): the pointer-network generator and its reward critic ----------------------------------------
+int64_t r4_exactk_launch_count(void) { return g_launches[FAM_EXACTK].load(std::memory_order_relaxed); }
+
+namespace {
+
+template <typename... P, typename... A>
+int ek_launch(const char* name, void (*kernel)(P...), dim3 grid, int threads, size_t smem, cudaStream_t st, A&&... args) {
+  return launch(FAM_EXACTK, name, kernel, grid, threads, smem, st, false, std::forward<A>(args)...);
+}
+
+unsigned blocks(int64_t n, int per) { return (unsigned)((n + per - 1) / per); }
+
+using r4ek::Op;
+constexpr int EK_SPLITS = 128;                 // split-K partials of a weight gradient at most
+constexpr int64_t EK_KC = 1024;                // rows per split-K partial at least
+
+// a [rows, cols] row-major matrix at leading dimension ld as a GEMM operand, or its transpose
+Op rm(const float* p, int64_t ld) { return Op{p, 0, 0, ld, 1}; }
+Op tr(const float* p, int64_t ld) { return Op{p, 0, 0, 1, ld}; }
+
+// C[M, N] (ldc) = alpha A B (+ C if beta) (+ bias) (relu), one batch
+int ek_mm(cudaStream_t st, Op A, Op B, float* C, int64_t ldc, int M, int N, int K, const float* bias = nullptr,
+          int relu = 0, int beta = 0, float alpha = 1.f) {
+  r4ek::Gemm g{A, B, C, 0, 0, ldc, 1, bias, M, N, K, 1, 0, alpha, beta, relu};
+  return ek_launch("k_ek_gemm", r4ek::k_ek_gemm, dim3(blocks(N, r4ek::GT), blocks(M, r4ek::GT), 1), r4ek::GNT, 0, st, g);
+}
+
+// the per-(row, head) attention products: batch z = 4 b + h
+int ek_bmm(cudaStream_t st, Op A, Op B, float* C, int64_t cso, int64_t csi, int64_t cs0, int64_t cs1, int M, int N, int K,
+           int n, float alpha, int beta = 0) {
+  r4ek::Gemm g{A, B, C, cso, csi, cs0, cs1, nullptr, M, N, K, r4ek::NH, 0, alpha, beta, 0};
+  return ek_launch("k_ek_gemm", r4ek::k_ek_gemm, dim3(blocks(N, r4ek::GT), blocks(M, r4ek::GT), n * r4ek::NH), r4ek::GNT, 0,
+                   st, g);
+}
+
+// out[N] (+)= sum over R rows (stride rs) of in[r, (i / w) ls + i % w]: chunks of rows into partials, then their sum
+// (two launches at every size, so a pass launches the same number of kernels for every n)
+int ek_colsum(cudaStream_t st, const float* in, int64_t R, int64_t rs, int w, int64_t ls, int N, float* out, int accumulate,
+              float* part, float scale = 1.f) {
+  const int64_t S = std::max<int64_t>(1, std::min<int64_t>(EK_SPLITS, (R + EK_KC - 1) / EK_KC));
+  const int64_t rc = (R + S - 1) / S;
+  if (int rc2 = ek_launch("k_ek_colsum", r4ek::k_ek_colsum, dim3(blocks(N, 128), (unsigned)S), 128, 0, st, in, R, rs, w, ls, N,
+                          rc, part, (int64_t)N, 1.f, 0))
+    return rc2;
+  return ek_launch("k_ek_colsum", r4ek::k_ek_colsum, dim3(blocks(N, 128), 1), 128, 0, st, (const float*)part, S, (int64_t)N, N,
+                   (int64_t)0, N, S, out, (int64_t)0, scale, accumulate);
+}
+
+// dW[K, N] += X^T dY over R rows (X at ldx, dY at ldy): split-K partials, then their sum in order
+int ek_wgrad(cudaStream_t st, const float* X, int64_t ldx, const float* dY, int64_t ldy, int64_t R, int K, int N, float* dW,
+             float* part) {
+  const int64_t S = std::min<int64_t>(EK_SPLITS, (R + EK_KC - 1) / EK_KC);
+  const int64_t kc = (R + S - 1) / S;
+  r4ek::Gemm g{tr(X, ldx), rm(dY, ldy), part, (int64_t)K * N, 0, N, 1, nullptr, K, N, (int)kc, 1, R, 1.f, 0, 0};
+  if (int rc = ek_launch("k_ek_gemm", r4ek::k_ek_gemm, dim3(blocks(N, r4ek::GT), blocks(K, r4ek::GT), (unsigned)S), r4ek::GNT,
+                         0, st, g))
+    return rc;
+  return ek_launch("k_ek_colsum", r4ek::k_ek_colsum, dim3(blocks((int64_t)K * N, 128), 1), 128, 0, st, (const float*)part, S,
+                   (int64_t)K * N, K * N, (int64_t)0, K * N, S, dW, (int64_t)0, 1.f, 1);
+}
+
+// a linear layer's gradients: dW += X^T dY, db += colsum dY
+int ek_lin_grad(cudaStream_t st, const float* X, int64_t ldx, const float* dY, int64_t ldy, int64_t R, int K, int N, float* dW,
+                float* db, float* part) {
+  if (int rc = ek_wgrad(st, X, ldx, dY, ldy, R, K, N, dW, part)) return rc;
+  return ek_colsum(st, dY, R, ldy, N, 0, N, db, 1, part);
+}
+
+// Scratch planes of the generator for n rows over T candidates (offsets in floats; path in int32 slots)
+struct EkPlanes {
+  int64_t uenc, X0, m[2], QKV[2], A[2], P[2], O[2], Y1[2], xh1[2], rs1[2], F1[2], Y2[2], xh2[2], rs2[2], eref[2];
+  int64_t XH, G, C, H, IN, PI, HB, QB, A1, A2, P1, GL, logits, path, ce;
+  int64_t dlog, deref[2], denc, dA1, dA2, dGL, dIN, dHs, dC, dHB, dQB, dG, dXH, rv;
+  int64_t dY, dZ, dF1, dQKV, dP, gx, dU, part, n;
+};
+EkPlanes ek_planes(int64_t n, int64_t T) {
+  using namespace r4ek;
+  EkPlanes p;
+  int64_t o = 0;
+  auto take = [&](int64_t k) { int64_t r = o; o += (k + 63) / 64 * 64; return r; };
+  const int64_t nT = n * T, S4 = n * NH * T * T;
+  p.uenc = take(n * HU); p.X0 = take(nT * D);
+  for (int l = 0; l < NBLK; ++l) {
+    p.m[l] = take(nT); p.QKV[l] = take(nT * 3 * D); p.A[l] = take(S4); p.P[l] = take(S4); p.O[l] = take(nT * D);
+    p.Y1[l] = take(nT * D); p.xh1[l] = take(nT * D); p.rs1[l] = take(nT); p.F1[l] = take(nT * FF); p.Y2[l] = take(nT * D);
+    p.xh2[l] = take(nT * D); p.rs2[l] = take(nT);
+  }
+  p.eref[0] = take(nT * D); p.eref[1] = take(nT * D);
+  p.XH = take(RES * n * 2 * D); p.G = take(RES * n * 4 * D); p.C = take(RES * n * D); p.H = take(RES * n * D);
+  p.IN = take(RES * n * D); p.PI = take(RES * n * RES); p.HB = take(RES * n * D); p.QB = take(RES * n * D);
+  p.A1 = take(RES * n * D); p.A2 = take(RES * n * D); p.P1 = take(RES * nT); p.GL = take(RES * n * D);
+  p.logits = take(n * RES * T); p.path = take(n * RES); p.ce = take(n);
+  p.dlog = take(nT); p.deref[0] = take(nT * D); p.deref[1] = take(nT * D); p.denc = take(nT * D);
+  p.dA1 = take(RES * n * D); p.dA2 = take(RES * n * D); p.dGL = take(n * D); p.dIN = take(n * D); p.dHs = take(RES * n * D);
+  p.dC = take(n * D); p.dHB = take(RES * n * D); p.dQB = take(RES * n * D); p.dG = take(RES * n * 4 * D);
+  p.dXH = take(RES * n * 2 * D); p.rv = take(n * RV_N * D);
+  p.dY = take(nT * D); p.dZ = take(nT * D); p.dF1 = take(nT * FF); p.dQKV = take(nT * 3 * D); p.dP = take(S4);
+  p.gx = take(nT * D); p.dU = take(n * HU);
+  p.part = take((int64_t)EK_SPLITS * 2 * D * 4 * D);
+  p.n = o;
+  return p;
+}
+
+bool ek_shape_ok(int n, int T) { return n >= 1 && n <= r4ek::MAXN && T >= r4ek::TMIN && T <= r4ek::TMAX; }
+
+struct EkRun {
+  const float* prm;
+  r4ek::Layout L;
+  int n, T;
+  uint64_t seed, call;
+  float rate;
+  float* s;
+  EkPlanes p;
+  cudaStream_t st;
+  float* f(int64_t off) const { return s + off; }
+};
+
+// the encoder forward: enc = Y2 of block 1; eref[a] = enc W_ref[a]
+int ek_encoder(const EkRun& r, const float* user) {
+  using namespace r4ek;
+  const int n = r.n, T = r.T;
+  const int64_t nT = (int64_t)n * T;
+  const float* prm = r.prm;
+  const Layout& L = r.L;
+  cudaStream_t st = r.st;
+  int rc;
+  if ((rc = ek_mm(st, rm(user, UIN), rm(prm + L.u_w, HU), r.f(r.p.uenc), HU, n, HU, UIN, prm + L.u_b, 1))) return rc;
+  if ((rc = ek_launch("k_ek_input", k_ek_input, blocks(nT * D, 256), 256, 0, st, (const float*)r.f(r.p.uenc), prm + L.emb, n,
+                      T, r.seed, r.call, r.rate, r.f(r.p.X0))))
+    return rc;
+  const float inv = 1.0f / sqrtf((float)DH);
+  for (int l = 0; l < NBLK; ++l) {
+    const Block& B = L.blk[l];
+    const float* X = l == 0 ? r.f(r.p.X0) : r.f(r.p.Y2[0]);
+    float* QKV = r.f(r.p.QKV[l]);
+    float* S = r.f(r.p.dP);
+    if ((rc = ek_launch("k_ek_rowmask", k_ek_rowmask, blocks(nT * 32, 256), 256, 0, st, X, nT, r.f(r.p.m[l])))) return rc;
+    if ((rc = ek_mm(st, rm(X, D), rm(prm + B.qkv_w, 3 * D), QKV, 3 * D, (int)nT, 3 * D, D, prm + B.qkv_b, 1))) return rc;
+    if ((rc = ek_bmm(st, Op{QKV, T * 3 * D, DH, 3 * D, 1}, Op{QKV + D, T * 3 * D, DH, 1, 3 * D}, S, (int64_t)NH * T * T,
+                     (int64_t)T * T, T, 1, T, T, DH, n, inv)))
+      return rc;
+    if ((rc = ek_launch("k_ek_softmax", k_ek_softmax, blocks((int64_t)n * NH * T * 32, 256), 256, 0, st, (const float*)S,
+                        (const float*)r.f(r.p.m[l]), n, T, r.seed, r.call, l == 0 ? ST_ATT0 : ST_ATT1, r.rate, r.f(r.p.A[l]),
+                        r.f(r.p.P[l]))))
+      return rc;
+    if ((rc = ek_bmm(st, Op{r.f(r.p.P[l]), (int64_t)NH * T * T, (int64_t)T * T, T, 1}, Op{QKV + 2 * D, T * 3 * D, DH, 3 * D, 1},
+                     r.f(r.p.O[l]), (int64_t)T * D, DH, D, 1, T, DH, T, n, 1.f)))
+      return rc;
+    if ((rc = ek_launch("k_ek_ln", k_ek_ln, blocks(nT * 32, 256), 256, 0, st, (const float*)r.f(r.p.O[l]), X, nT,
+                        prm + B.ln1_b, prm + B.ln1_g, r.f(r.p.Y1[l]), r.f(r.p.xh1[l]), r.f(r.p.rs1[l]))))
+      return rc;
+    if ((rc = ek_mm(st, rm(r.f(r.p.Y1[l]), D), rm(prm + B.f1_w, FF), r.f(r.p.F1[l]), FF, (int)nT, FF, D, prm + B.f1_b, 1)))
+      return rc;
+    if ((rc = ek_mm(st, rm(r.f(r.p.F1[l]), FF), rm(prm + B.f2_w, D), r.f(r.p.dY), D, (int)nT, D, FF, prm + B.f2_b))) return rc;
+    if ((rc = ek_launch("k_ek_ln", k_ek_ln, blocks(nT * 32, 256), 256, 0, st, (const float*)r.f(r.p.dY),
+                        (const float*)r.f(r.p.Y1[l]), nT, prm + B.ln2_b, prm + B.ln2_g, r.f(r.p.Y2[l]), r.f(r.p.xh2[l]),
+                        r.f(r.p.rs2[l]))))
+      return rc;
+  }
+  for (int a = 0; a < 2; ++a)
+    if ((rc = ek_mm(st, rm(r.f(r.p.Y2[1]), D), rm(prm + L.att[a].w_ref, D), r.f(r.p.eref[a]), D, (int)nT, D, D))) return rc;
+  return R4_OK;
+}
+
+r4ek::Dec ek_dec(const EkRun& r, const uint8_t* masks, int32_t* path, float* logits) {
+  r4ek::Dec d;
+  d.n = r.n; d.T = r.T;
+  d.enc = r.f(r.p.Y2[1]);
+  d.eref[0] = r.f(r.p.eref[0]); d.eref[1] = r.f(r.p.eref[1]);
+  d.XH = r.f(r.p.XH); d.G = r.f(r.p.G); d.C = r.f(r.p.C); d.H = r.f(r.p.H); d.IN = r.f(r.p.IN); d.PI = r.f(r.p.PI);
+  d.HB = r.f(r.p.HB); d.QB = r.f(r.p.QB); d.A1 = r.f(r.p.A1); d.A2 = r.f(r.p.A2); d.P1 = r.f(r.p.P1); d.GL = r.f(r.p.GL);
+  d.logits = logits; d.path = path; d.masks = masks;
+  return d;
+}
+
+// the nine decode steps (mode 0 SAMPLE, 1 GREEDY, 2 TRAIN on the path already in d.path)
+int ek_decoder(const EkRun& r, const r4ek::Dec& d, int mode, float temperature) {
+  using namespace r4ek;
+  const int n = r.n, T = r.T;
+  const float* prm = r.prm;
+  const Layout& L = r.L;
+  cudaStream_t st = r.st;
+  const size_t smT = (size_t)T * sizeof(float);
+  int rc;
+  // XH[0] = [first input | initial h] in every row: a K = 0 product with that row as its bias
+  if ((rc = ek_mm(st, Op{nullptr, 0, 0, 0, 0}, Op{prm + L.x0, 0, 0, 0, 1}, d.XH, 2 * D, n, 2 * D, 0, prm + L.x0))) return rc;
+  for (int t = 0; t < RES; ++t) {
+    float* H = d.H + plane(n, t, D);
+    float* IN = d.IN + plane(n, t, D);
+    if ((rc = ek_mm(st, rm(d.XH + plane(n, t, 2 * D), 2 * D), rm(prm + L.lstm_w, 4 * D), d.G + plane(n, t, 4 * D), 4 * D, n,
+                    4 * D, 2 * D, prm + L.lstm_b)))
+      return rc;
+    if ((rc = ek_launch("k_ek_cell", k_ek_cell, blocks((int64_t)n * D, 256), 256, 0, st, d, t, prm + L.c0))) return rc;
+    if ((rc = ek_mm(st, rm(H, D), rm(prm + L.w_bef, D), d.HB + plane(n, t, D), D, n, D, D))) return rc;
+    if ((rc = ek_mm(st, rm(H, D), rm(prm + L.w_b, D), d.QB + plane(n, t, D), D, n, D, D))) return rc;
+    if ((rc = ek_mm(st, rm(H, D), rm(prm + L.att[0].w_q, D), d.A1 + plane(n, t, D), D, n, D, D))) return rc;
+    if ((rc = ek_launch("k_ek_intra", k_ek_intra, n, D, 0, st, d, t, prm, L))) return rc;
+    if ((rc = ek_mm(st, rm(IN, D), rm(prm + L.att[0].w_dec, D), d.A1 + plane(n, t, D), D, n, D, D, nullptr, 0, 1))) return rc;
+    if ((rc = ek_mm(st, rm(IN, D), rm(prm + L.att[1].w_dec, D), d.A2 + plane(n, t, D), D, n, D, D))) return rc;
+    if ((rc = ek_launch("k_ek_glimpse", k_ek_glimpse, n, RNT, smT, st, d, t, prm, L))) return rc;
+    if ((rc = ek_mm(st, rm(d.GL + plane(n, t, D), D), rm(prm + L.att[1].w_q, D), d.A2 + plane(n, t, D), D, n, D, D, nullptr, 0,
+                    1)))
+      return rc;
+    if ((rc = ek_launch("k_ek_point", k_ek_point, n, RNT, smT, st, d, t, mode, temperature, r.seed, r.call, prm, L))) return rc;
+  }
+  return R4_OK;
+}
+
+// the backward of the policy loss mean_b(sum_t CE(logits[b, t], path[b, t]) reward[b]) into grad (zeroed here)
+int ek_backward(const EkRun& r, const r4ek::Dec& d, const float* user, const float* reward, float* grad, float* loss) {
+  using namespace r4ek;
+  const int n = r.n, T = r.T;
+  const int64_t nT = (int64_t)n * T;
+  const float* prm = r.prm;
+  const Layout& L = r.L;
+  cudaStream_t st = r.st;
+  const size_t smT = (size_t)T * sizeof(float);
+  float* part = r.f(r.p.part);
+  int rc;
+  cudaError_t ce = cudaSuccess;
+  auto zero = [&](int64_t off, int64_t k) { if (ce == cudaSuccess) ce = cudaMemsetAsync(r.f(off), 0, k * sizeof(float), st); };
+  if (cudaMemsetAsync(grad, 0, L.n * sizeof(float), st) != cudaSuccess) return fail(R4_ERR_CUDA, "r4_exactk_grad: memset");
+  zero(r.p.deref[0], nT * D); zero(r.p.deref[1], nT * D); zero(r.p.denc, nT * D); zero(r.p.dHs, RES * n * D);
+  zero(r.p.dHB, RES * n * D); zero(r.p.dQB, RES * n * D); zero(r.p.rv, n * RV_N * D);
+  if (ce != cudaSuccess) return fail(R4_ERR_CUDA, "r4_exactk_grad: memset");
+  DecBack g;
+  g.dlog = r.f(r.p.dlog); g.deref[0] = r.f(r.p.deref[0]); g.deref[1] = r.f(r.p.deref[1]); g.denc = r.f(r.p.denc);
+  g.dGL = r.f(r.p.dGL); g.dIN = r.f(r.p.dIN); g.dC = r.f(r.p.dC); g.dHB = r.f(r.p.dHB); g.rv = r.f(r.p.rv);
+  float* ceb = r.f(r.p.ce);
+  for (int t = RES - 1; t >= 0; --t) {
+    g.dA1 = r.f(r.p.dA1) + plane(n, t, D); g.dA2 = r.f(r.p.dA2) + plane(n, t, D);
+    g.dH = r.f(r.p.dHs) + plane(n, t, D); g.dQB = r.f(r.p.dQB) + plane(n, t, D);
+    g.dG = r.f(r.p.dG); g.dXH = r.f(r.p.dXH) + plane(n, t, 2 * D);
+    float* dHt = g.dH;
+    if ((rc = ek_launch("k_ek_loss_bwd", k_ek_loss_bwd, n, RNT, 0, st, d, g, t, reward, ceb))) return rc;
+    if ((rc = ek_launch("k_ek_point_bwd", k_ek_point_bwd, n, RNT, smT, st, d, g, t, prm, L))) return rc;
+    if ((rc = ek_mm(st, rm(g.dA2, D), tr(prm + L.att[1].w_q, D), g.dGL, D, n, D, D))) return rc;
+    if ((rc = ek_mm(st, rm(g.dA2, D), tr(prm + L.att[1].w_dec, D), g.dIN, D, n, D, D))) return rc;
+    if ((rc = ek_launch("k_ek_glimpse_bwd", k_ek_glimpse_bwd, n, RNT, smT, st, d, g, t, prm, L))) return rc;
+    if ((rc = ek_mm(st, rm(g.dA1, D), tr(prm + L.att[0].w_dec, D), g.dIN, D, n, D, D, nullptr, 0, 1))) return rc;
+    if ((rc = ek_launch("k_ek_intra_bwd", k_ek_intra_bwd, n, D, 0, st, d, g, t, r.f(r.p.dHs), prm, L))) return rc;
+    // dh_t: the later steps' direct terms (in dHs[t]) + the glimpse query + the intra-attention query and keys
+    if ((rc = ek_mm(st, rm(g.dA1, D), tr(prm + L.att[0].w_q, D), dHt, D, n, D, D, nullptr, 0, 1))) return rc;
+    if ((rc = ek_mm(st, rm(g.dQB, D), tr(prm + L.w_b, D), dHt, D, n, D, D, nullptr, 0, 1))) return rc;
+    if ((rc = ek_mm(st, rm(r.f(r.p.dHB) + plane(n, t, D), D), tr(prm + L.w_bef, D), dHt, D, n, D, D, nullptr, 0, 1))) return rc;
+    if ((rc = ek_launch("k_ek_cell_bwd", k_ek_cell_bwd, blocks((int64_t)n * D, 256), 256, 0, st, d, g, t, prm + L.c0,
+                        t + 1 < RES ? (const float*)(r.f(r.p.dXH) + plane(n, t + 1, 2 * D)) : (const float*)nullptr)))
+      return rc;
+    if ((rc = ek_mm(st, rm(g.dG + plane(n, t, 4 * D), 4 * D), tr(prm + L.lstm_w, 4 * D), g.dXH, 2 * D, n, 2 * D, 4 * D))) return rc;
+    if (t > 0 && (rc = ek_launch("k_ek_input_bwd", k_ek_input_bwd, blocks((int64_t)n * D, 256), 256, 0, st, d, g, t))) return rc;
+  }
+  if (loss && (rc = ek_launch("k_ek_gloss", k_ek_gloss, 1, 1, 0, st, (const float*)ceb, reward, n, 1.0f / n, loss))) return rc;
+  // decoder weights: stacked over the nine steps
+  const int64_t R9 = (int64_t)RES * n;
+  float* dgr = grad;
+  if ((rc = ek_lin_grad(st, r.f(r.p.XH), 2 * D, r.f(r.p.dG), 4 * D, R9, 2 * D, 4 * D, dgr + L.lstm_w, dgr + L.lstm_b, part)))
+    return rc;
+  if ((rc = ek_colsum(st, r.f(r.p.dC), n, D, D, 0, D, dgr + L.c0, 1, part))) return rc;
+  if ((rc = ek_colsum(st, r.f(r.p.dXH), n, 2 * D, D, 0, D, dgr + L.x0, 1, part))) return rc;
+  if ((rc = ek_colsum(st, r.f(r.p.dXH) + D, n, 2 * D, D, 0, D, dgr + L.h0, 1, part))) return rc;
+  if ((rc = ek_wgrad(st, r.f(r.p.H), D, r.f(r.p.dHB), D, R9, D, D, dgr + L.w_bef, part))) return rc;
+  if ((rc = ek_wgrad(st, r.f(r.p.H), D, r.f(r.p.dQB), D, R9, D, D, dgr + L.w_b, part))) return rc;
+  if ((rc = ek_wgrad(st, r.f(r.p.H), D, r.f(r.p.dA1), D, R9, D, D, dgr + L.att[0].w_q, part))) return rc;
+  if ((rc = ek_wgrad(st, r.f(r.p.IN), D, r.f(r.p.dA1), D, R9, D, D, dgr + L.att[0].w_dec, part))) return rc;
+  if ((rc = ek_wgrad(st, r.f(r.p.GL), D, r.f(r.p.dA2), D, R9, D, D, dgr + L.att[1].w_q, part))) return rc;
+  if ((rc = ek_wgrad(st, r.f(r.p.IN), D, r.f(r.p.dA2), D, R9, D, D, dgr + L.att[1].w_dec, part))) return rc;
+  const int64_t rvo[RV_N] = {L.att[0].v, L.att[0].bias, L.att[1].v, L.att[1].bias, L.v_dec, L.bias_dec};
+  for (int k = 0; k < RV_N; ++k)
+    if ((rc = ek_colsum(st, r.f(r.p.rv) + k * D, n, RV_N * D, D, 0, D, dgr + rvo[k], 1, part))) return rc;
+  // the encoder outputs: the W_ref projections, then the blocks in reverse
+  const float* enc = r.f(r.p.Y2[1]);
+  float* dY = r.f(r.p.denc);
+  for (int a = 0; a < 2; ++a) {
+    if ((rc = ek_wgrad(st, enc, D, r.f(r.p.deref[a]), D, nT, D, D, dgr + L.att[a].w_ref, part))) return rc;
+    if ((rc = ek_mm(st, rm(r.f(r.p.deref[a]), D), tr(prm + L.att[a].w_ref, D), dY, D, (int)nT, D, D, nullptr, 0, 1))) return rc;
+  }
+  const float inv = 1.0f / sqrtf((float)DH);
+  for (int l = NBLK - 1; l >= 0; --l) {
+    const Block& B = L.blk[l];
+    const float* X = l == 0 ? r.f(r.p.X0) : r.f(r.p.Y2[0]);
+    const float* QKV = r.f(r.p.QKV[l]);
+    float* gx = r.f(r.p.gx);
+    float* dZ = r.f(r.p.dZ);
+    float* dF1 = r.f(r.p.dF1);
+    float* dQKV = r.f(r.p.dQKV);
+    float* dP = r.f(r.p.dP);
+    // Y2 = LN(F1 W2 + b2 + Y1): beta's gradient from dY, then dY (in place) -> d(sum)
+    if ((rc = ek_colsum(st, dY, nT, D, D, 0, D, dgr + B.ln2_b, 1, part))) return rc;
+    if ((rc = ek_launch("k_ek_ln_bwd", k_ek_ln_bwd, blocks(nT * 32, 256), 256, 0, st, (const float*)r.f(r.p.xh2[l]),
+                        (const float*)r.f(r.p.rs2[l]), nT, prm + B.ln2_g, dY, gx)))
+      return rc;
+    if ((rc = ek_colsum(st, gx, nT, D, D, 0, D, dgr + B.ln2_g, 1, part))) return rc;
+    if ((rc = ek_lin_grad(st, r.f(r.p.F1[l]), FF, dY, D, nT, FF, D, dgr + B.f2_w, dgr + B.f2_b, part))) return rc;
+    if ((rc = ek_mm(st, rm(dY, D), tr(prm + B.f2_w, D), dF1, FF, (int)nT, FF, D))) return rc;
+    if ((rc = ek_launch("k_ek_relu_bwd", k_ek_relu_bwd, blocks(nT * FF, 256), 256, 0, st, (const float*)r.f(r.p.F1[l]),
+                        (int64_t)FF, dF1, (int64_t)FF, nT, FF)))
+      return rc;
+    if ((rc = ek_lin_grad(st, r.f(r.p.Y1[l]), D, dF1, FF, nT, D, FF, dgr + B.f1_w, dgr + B.f1_b, part))) return rc;
+    if ((rc = ek_mm(st, rm(dF1, FF), tr(prm + B.f1_w, FF), dY, D, (int)nT, D, FF, nullptr, 0, 1))) return rc;   // dY1
+    // Y1 = LN(O + X)
+    if ((rc = ek_colsum(st, dY, nT, D, D, 0, D, dgr + B.ln1_b, 1, part))) return rc;
+    if ((rc = ek_launch("k_ek_ln_bwd", k_ek_ln_bwd, blocks(nT * 32, 256), 256, 0, st, (const float*)r.f(r.p.xh1[l]),
+                        (const float*)r.f(r.p.rs1[l]), nT, prm + B.ln1_g, dY, gx)))
+      return rc;
+    if ((rc = ek_colsum(st, gx, nT, D, D, 0, D, dgr + B.ln1_g, 1, part))) return rc;
+    // O_h = P V_h: dP = dO_h V_h^T, dV_h = P^T dO_h
+    if ((rc = ek_bmm(st, Op{dY, (int64_t)T * D, DH, D, 1}, Op{QKV + 2 * D, (int64_t)T * 3 * D, DH, 1, 3 * D}, dP,
+                     (int64_t)NH * T * T, (int64_t)T * T, T, 1, T, T, DH, n, 1.f)))
+      return rc;
+    if ((rc = ek_bmm(st, Op{r.f(r.p.P[l]), (int64_t)NH * T * T, (int64_t)T * T, 1, T}, Op{dY, (int64_t)T * D, DH, D, 1},
+                     dQKV + 2 * D, (int64_t)T * 3 * D, DH, 3 * D, 1, T, DH, T, n, 1.f)))
+      return rc;
+    if ((rc = ek_launch("k_ek_softmax_bwd", k_ek_softmax_bwd, blocks((int64_t)n * NH * T * 32, 256), 256, 0, st,
+                        (const float*)r.f(r.p.A[l]), (const float*)r.f(r.p.m[l]), n, T, r.seed, r.call,
+                        l == 0 ? ST_ATT0 : ST_ATT1, r.rate, dP)))
+      return rc;
+    // S = Q K^T / sqrt(32): dQ_h = dS K_h / sqrt(32), dK_h = dS^T Q_h / sqrt(32)
+    if ((rc = ek_bmm(st, Op{dP, (int64_t)NH * T * T, (int64_t)T * T, T, 1}, Op{QKV + D, (int64_t)T * 3 * D, DH, 3 * D, 1},
+                     dQKV, (int64_t)T * 3 * D, DH, 3 * D, 1, T, DH, T, n, inv)))
+      return rc;
+    if ((rc = ek_bmm(st, Op{dP, (int64_t)NH * T * T, (int64_t)T * T, 1, T}, Op{QKV, (int64_t)T * 3 * D, DH, 3 * D, 1},
+                     dQKV + D, (int64_t)T * 3 * D, DH, 3 * D, 1, T, DH, T, n, inv)))
+      return rc;
+    if ((rc = ek_launch("k_ek_relu_bwd", k_ek_relu_bwd, blocks(nT * 3 * D, 256), 256, 0, st, QKV, (int64_t)3 * D, dQKV,
+                        (int64_t)3 * D, nT, 3 * D)))
+      return rc;
+    if ((rc = ek_lin_grad(st, X, D, dQKV, 3 * D, nT, D, 3 * D, dgr + B.qkv_w, dgr + B.qkv_b, part))) return rc;
+    // dX = d(sum) (the residual) + dQKV W_qkv^T: the block input's gradient, kept in dY
+    if ((rc = ek_mm(st, rm(dQKV, 3 * D), tr(prm + B.qkv_w, 3 * D), dY, D, (int)nT, D, 3 * D, nullptr, 0, 1))) return rc;
+  }
+  // X0 = dropout([relu(user W_u + b_u) | emb * 8])
+  float* dU = r.f(r.p.dU);
+  if ((rc = ek_launch("k_ek_emb_bwd", k_ek_emb_bwd, blocks((int64_t)(n + T) * HU, 128), 128, 0, st, (const float*)dY, n, T,
+                      r.seed, r.call, r.rate, dU, dgr + L.emb)))
+    return rc;
+  if ((rc = ek_launch("k_ek_relu_bwd", k_ek_relu_bwd, blocks((int64_t)n * HU, 256), 256, 0, st, (const float*)r.f(r.p.uenc),
+                      (int64_t)HU, dU, (int64_t)HU, (int64_t)n, HU)))
+    return rc;
+  return ek_lin_grad(st, user, UIN, dU, HU, n, UIN, HU, dgr + L.u_w, dgr + L.u_b, part);
+}
+
+struct CPlanes { int64_t Z[4], dZ[4], part, n; };
+CPlanes ek_cplanes(int64_t n) {
+  CPlanes p;
+  int64_t o = 0;
+  auto take = [&](int64_t k) { int64_t r = o; o += (k + 63) / 64 * 64; return r; };
+  for (int i = 0; i < 4; ++i) { p.Z[i] = take(n * r4ek::CH); p.dZ[i] = take(n * r4ek::CH); }
+  p.part = take((int64_t)EK_SPLITS * r4ek::UIN * r4ek::CH);
+  p.n = o;
+  return p;
+}
+
+}  // namespace
+
+int64_t r4_exactk_num_params(int net) {
+  return net == R4_EXACTK_GENERATOR ? r4ek::make_layout().n : net == R4_EXACTK_CRITIC ? r4ek::make_clayout().n : -1;
+}
+
+int64_t r4_exactk_scratch_size(int net, int n, int seq_length) {
+  if (n < 1 || n > r4ek::MAXN) return -1;
+  if (net == R4_EXACTK_CRITIC) return ek_cplanes(n).n * (int64_t)sizeof(float);
+  if (net != R4_EXACTK_GENERATOR || !ek_shape_ok(n, seq_length)) return -1;
+  return ek_planes(n, seq_length).n * (int64_t)sizeof(float);
+}
+
+static int ek_run(const float* params, int n, int T, uint64_t seed, uint64_t call, float dropout, void* scratch, void* stream,
+                  EkRun* r) {
+  if (!params || !scratch || !ek_shape_ok(n, T) || !(dropout >= 0.f && dropout < 1.f)) return fail(R4_ERR_ARG, "bad argument");
+  r->prm = params; r->L = r4ek::make_layout(); r->n = n; r->T = T; r->seed = seed; r->call = call; r->rate = dropout;
+  r->s = static_cast<float*>(scratch); r->p = ek_planes(n, T); r->st = S(stream);
+  return R4_OK;
+}
+
+int r4_exactk_decode(const float* params, const float* user, int n, int seq_length, const uint8_t* masks, int mode,
+                     float temperature, uint64_t seed, uint64_t call, float dropout, int32_t* path, float* logits, void* scratch,
+                     void* stream) {
+  EkRun r;
+  if (int rc = ek_run(params, n, seq_length, seed, call, dropout, scratch, stream, &r)) return rc;
+  if (!user || !masks || !path || mode < R4_EXACTK_SAMPLE || mode > R4_EXACTK_TRAIN || !(temperature > 0.f))
+    return fail(R4_ERR_ARG, "bad argument");
+  if (int rc = ek_encoder(r, user)) return rc;
+  return ek_decoder(r, ek_dec(r, masks, path, logits ? logits : r.f(r.p.logits)), mode, temperature);
+}
+
+int r4_exactk_grad(const float* params, const float* user, int n, int seq_length, const uint8_t* masks, const int32_t* target,
+                   const float* reward, uint64_t seed, uint64_t call, float dropout, float* grad, float* loss, void* scratch,
+                   void* stream) {
+  EkRun r;
+  if (int rc = ek_run(params, n, seq_length, seed, call, dropout, scratch, stream, &r)) return rc;
+  if (!user || !masks || !target || !reward || !grad) return fail(R4_ERR_ARG, "bad argument");
+  int32_t* path = reinterpret_cast<int32_t*>(r.f(r.p.path));
+  if (cudaMemcpyAsync(path, target, (size_t)n * r4ek::RES * sizeof(int32_t), cudaMemcpyDeviceToDevice, r.st) != cudaSuccess)
+    return fail(R4_ERR_CUDA, "r4_exactk_grad: copy");
+  if (int rc = ek_encoder(r, user)) return rc;
+  const r4ek::Dec d = ek_dec(r, masks, path, r.f(r.p.logits));
+  if (int rc = ek_decoder(r, d, R4_EXACTK_TRAIN, 1.f)) return rc;
+  return ek_backward(r, d, user, reward, grad, loss);
+}
+
+int r4_exactk_critic(const float* params, const float* user, int n, const float* target, float* pred, float* grad, float* loss,
+                     void* scratch, void* stream) {
+  using namespace r4ek;
+  if (!params || !user || !scratch || n < 1 || n > MAXN || (target && !grad)) return fail(R4_ERR_ARG, "bad argument");
+  const CLayout L = make_clayout();
+  const CPlanes p = ek_cplanes(n);
+  float* s = static_cast<float*>(scratch);
+  cudaStream_t st = S(stream);
+  const int in[4] = {UIN, CH, CH, CH}, out[4] = {CH, CH, CH, 1};
+  int rc;
+  const float* X = user;
+  for (int i = 0; i < 4; ++i) {
+    if ((rc = ek_mm(st, rm(X, in[i]), rm(params + L.w[i], out[i]), s + p.Z[i], out[i], n, out[i], in[i], params + L.b[i],
+                    i < 3)))
+      return rc;
+    X = s + p.Z[i];
+  }
+  if ((rc = ek_launch("k_ek_closs", k_ek_closs, 1, 256, 0, st, (const float*)(s + p.Z[3]), target, n, pred, s + p.dZ[3], loss)))
+    return rc;
+  if (!target) return R4_OK;
+  if (cudaMemsetAsync(grad, 0, L.n * sizeof(float), st) != cudaSuccess) return fail(R4_ERR_CUDA, "r4_exactk_critic: memset");
+  for (int i = 3; i >= 0; --i) {
+    const float* Xi = i == 0 ? user : s + p.Z[i - 1];
+    if ((rc = ek_lin_grad(st, Xi, in[i], s + p.dZ[i], out[i], n, in[i], out[i], grad + L.w[i], grad + L.b[i], s + p.part)))
+      return rc;
+    if (i == 0) break;
+    if ((rc = ek_mm(st, rm(s + p.dZ[i], out[i]), tr(params + L.w[i], out[i]), s + p.dZ[i - 1], CH, n, CH, out[i]))) return rc;
+    if ((rc = ek_launch("k_ek_relu_bwd", k_ek_relu_bwd, blocks((int64_t)n * CH, 256), 256, 0, st, (const float*)(s + p.Z[i - 1]),
+                        (int64_t)CH, s + p.dZ[i - 1], (int64_t)CH, (int64_t)n, CH)))
+      return rc;
+  }
+  return R4_OK;
+}
+
+int r4_exactk_adam(int net, float* params, float* grad, float* m, float* v, int step, float lr, float beta1, float beta2,
+                   float eps, void* stream) {
+  const int64_t np = r4_exactk_num_params(net);
+  if (np < 0 || !params || !grad || !m || !v || step < 1) return fail(R4_ERR_ARG, "bad argument");
+  const float alpha = lr * sqrtf(1.f - powf(beta2, (float)step)) / (1.f - powf(beta1, (float)step));
+  return ek_launch("k_st_apply", r4ek::k_ek_adam, blocks(np, 256), 256, 0, S(stream), np, (int64_t)0, np, np, params, grad, m, v,
+                   alpha, beta1, beta2, eps);
+}

@@ -1280,3 +1280,7 @@ __global__ void __launch_bounds__(NTH) k_st_loss_adv(Data D, const int64_t* __re
 }
 
 }  // namespace r4st
+
+// Exact-K's kernels reach r4_learn.cu through this header: they run on the same Adam (k_st_apply), and the learner
+// translation unit keeps one include per learner family.
+#include "r4_exactk.cuh"
