@@ -18,7 +18,7 @@
 //   BC: M (imitator) ; BCQ: M (Q) | M (imitator) ; CQL: C.   The target holds the Q part only (BCQ: the first M; CQL: C).
 //
 // One SGD step is four launches: k_bq_rows (one CTA per TS samples: the forwards on s' and s, the loss rows and the
-// backward rows, written to the scratch planes), r4ddpg::k_ddpg_wgrad over the dense layers (dW = X^T dZ, one CTA per
+// backward rows, written to the scratch planes), r4dense::k_dense_wgrad over the dense layers (dW = X^T dZ, one CTA per
 // 64 x 64 tile, samples walked in order), k_bq_embgrad (the embedding scatter, one thread per table element walking the
 // samples and slots in order: deterministic, no atomics) and k_bq_apply (Adam, then the hard target copy when due).
 #pragma once
@@ -369,8 +369,8 @@ __global__ void __launch_bounds__(NT) k_bq_rows(Layout L, Hyper hp, const float*
   }
 }
 
-inline r4ddpg::Jobs make_jobs(const Layout& L, const Planes& P) {
-  r4ddpg::Jobs J;
+inline r4dense::Jobs make_jobs(const Layout& L, const Planes& P) {
+  r4dense::Jobs J;
   int k = 0;
   auto layer = [&](const float* X, int ldx, const float* dZ, int M, int N, int w, int b) {
     J.j[k++] = {X, dZ, ldx, M, N, w, 0};
@@ -388,13 +388,7 @@ inline r4ddpg::Jobs make_jobs(const Layout& L, const Planes& P) {
     layer(P.h1, H, P.c2, H, H, L.c.w2, L.c.b2);
     layer(P.h2, H, P.c3, H, L.A, L.c.w3, L.c.b3);
   }
-  J.njob = k;
-  int t = 0;
-  for (int i = 0; i < k; ++i) {
-    J.j[i].tile0 = t;
-    t += ((J.j[i].M + r4ddpg::WT - 1) / r4ddpg::WT) * ((J.j[i].N + r4ddpg::WT - 1) / r4ddpg::WT);
-  }
-  J.ntiles = t;
+  r4dense::tile_jobs(J, k);
   return J;
 }
 

@@ -17,13 +17,14 @@
 //   k_ddpg_rows   one CTA per TS samples: target actor (+ smoothing) and target critic(s) on s', the critic(s) on (s, a),
 //                 the TD errors, Q1(s, pi(s)), and the backward rows of both losses; writes every layer's input rows X and
 //                 output-gradient rows dZ to the scratch planes.
-//   k_ddpg_wgrad  one CTA per 64 x 64 tile of one dW = X^T dZ (or a bias), walking the samples in order (the pattern of
-//                 k_gauss_wgrad): deterministic, every element has one writer.  One extra CTA sums the loss statistics.
+//   r4dense::k_dense_wgrad  one CTA per 64 x 64 tile of one dW = X^T dZ (or a bias), walking the samples in order:
+//                 deterministic, every element has one writer.  One extra CTA sums the loss statistics.
 // k_ddpg_apply then adds the l2 terms, runs both Adams (the actor's skipped on delayed steps) and the soft target update.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "r4_dense.cuh"
 #include "r4_ppo.cuh"
 
 namespace r4ddpg {
@@ -447,78 +448,10 @@ __global__ void __launch_bounds__(NT) k_ddpg_rows(Layout L, Hyper hp, const floa
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// learner, part 2: weight gradients, as k_gauss_wgrad with a row stride for X (the actor reads the s columns of [s | a]).
-// ------------------------------------------------------------------------------------------------
-constexpr int NJOB = 18, WT = 64, WK = 32;
-struct Job {
-  const float* X;
-  const float* Z;
-  int ldx, M, N, off, tile0;
-};
-struct Jobs {
-  Job j[NJOB];
-  int njob, ntiles;
-};
-
-__global__ void __launch_bounds__(NT) k_ddpg_wgrad(Jobs jobs, int n, float* __restrict__ grad, const float* __restrict__ stats,
-                                                   float* __restrict__ stats_out, float inv_n) {
-  __shared__ float xs[WK][WT];
-  __shared__ float zs[WK][WT];
-  const int tid = threadIdx.x;
-  if ((int)blockIdx.x == jobs.ntiles) {                    // the loss statistics, summed in sample order
-    if (tid < 3 && stats_out) {
-      float a = 0.f;
-      for (int q = 0; q < n; ++q) a += stats[q * 3 + tid];
-      stats_out[tid] = a * inv_n;
-    }
-    return;
-  }
-  int jb = 0;
-  while (jb + 1 < jobs.njob && (int)blockIdx.x >= jobs.j[jb + 1].tile0) ++jb;
-  const Job J = jobs.j[jb];
-  const int t = blockIdx.x - J.tile0, tn = (J.N + WT - 1) / WT;
-  const int i0 = (t / tn) * WT, c0 = (t % tn) * WT;
-  const int ty = tid / 16, tx = tid % 16;
-  float acc[4][4];
-#pragma unroll
-  for (int a = 0; a < 4; ++a)
-#pragma unroll
-    for (int b = 0; b < 4; ++b) acc[a][b] = 0.f;
-  for (int k0 = 0; k0 < n; k0 += WK) {
-    __syncthreads();
-    for (int e = tid; e < WK * WT; e += NT) {
-      const int k = e / WT, c = e % WT, q = k0 + k;
-      const bool ok = q < n;
-      xs[k][c] = (ok && i0 + c < J.M) ? (J.X ? J.X[(size_t)q * J.ldx + i0 + c] : 1.f) : 0.f;
-      zs[k][c] = (ok && c0 + c < J.N) ? J.Z[(size_t)q * J.N + c0 + c] : 0.f;
-    }
-    __syncthreads();
-#pragma unroll 4
-    for (int k = 0; k < WK; ++k) {
-      float xv[4], zv[4];
-#pragma unroll
-      for (int a = 0; a < 4; ++a) { xv[a] = xs[k][4 * ty + a]; zv[a] = zs[k][4 * tx + a]; }
-#pragma unroll
-      for (int a = 0; a < 4; ++a)
-#pragma unroll
-        for (int b = 0; b < 4; ++b) acc[a][b] = fmaf(xv[a], zv[b], acc[a][b]);
-    }
-  }
-#pragma unroll
-  for (int a = 0; a < 4; ++a) {
-    const int i = i0 + 4 * ty + a;
-    if (i >= J.M) continue;
-#pragma unroll
-    for (int b = 0; b < 4; ++b) {
-      const int c = c0 + 4 * tx + b;
-      if (c < J.N) grad[J.off + (size_t)i * J.N + c] = acc[a][b];
-    }
-  }
-}
-
-inline Jobs make_jobs(const Layout& L, const Planes& P) {
-  Jobs J;
+// The weight-gradient jobs (r4dense::k_dense_wgrad), six per net; the first layers read the [s | a] plane at its row stride
+// (the actor only its s columns).
+inline r4dense::Jobs make_jobs(const Layout& L, const Planes& P) {
+  r4dense::Jobs J;
   int k = 0;
   auto net = [&](const Net& q, const float* X, int ldx, const float* h1, const float* h2, const float* d1, const float* d2,
                  const float* d3) {
@@ -529,13 +462,7 @@ inline Jobs make_jobs(const Layout& L, const Planes& P) {
   net(L.actor, P.x, XIN, P.ah1, P.ah2, P.ad1, P.ad2, P.ad3);
   net(L.q1, P.x, XIN, P.ch1[0], P.ch2[0], P.cd1[0], P.cd2[0], P.cd3[0]);
   if (L.twin) net(L.q2, P.x, XIN, P.ch1[1], P.ch2[1], P.cd1[1], P.cd2[1], P.cd3[1]);
-  J.njob = k;
-  int t = 0;
-  for (int i = 0; i < k; ++i) {
-    J.j[i].tile0 = t;
-    t += ((J.j[i].M + WT - 1) / WT) * ((J.j[i].N + WT - 1) / WT);
-  }
-  J.ntiles = t;
+  r4dense::tile_jobs(J, k);
   return J;
 }
 

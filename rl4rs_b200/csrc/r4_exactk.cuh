@@ -9,7 +9,8 @@
 //   decoder  nine steps of an LSTM (128), the intra-attention over its earlier outputs, one glimpse and the pointer
 //            attention over the encoder outputs, the point mask, and the SAMPLE / GREEDY / TRAIN choice of the next index
 // Kernels (host sequence in r4_learn.cu):
-//   k_ek_gemm        C = epilogue(alpha A B [+ C] [+ bias]) over strided, two-level batched operands; split-K partials
+//   r4dense::k_dense_gemm  C = epilogue(alpha A B [+ C] [+ bias]) over strided, two-level batched operands; split-K
+//                    partials
 //   k_ek_colsum      out (+)= sum over rows of a strided plane (bias, LayerNorm and split-K reductions), rows in order
 //   k_ek_input       X0 and its dropout; k_ek_rowmask the key / query masks sign(|sum_c X|)
 //   k_ek_softmax     the masked attention softmax and its dropout; k_ek_softmax_bwd its backward
@@ -18,7 +19,7 @@
 //   k_ek_intra / _bwd, k_ek_glimpse / _bwd, k_ek_point / _bwd   the decoder attentions, one CTA per row
 //   k_ek_loss_bwd    d(logits) of the policy loss; k_ek_gloss the loss; k_ek_closs the critic's summed squared error
 //   k_ek_cell_bwd, k_ek_input_bwd, k_ek_relu_bwd, k_ek_emb_bwd   the element-wise backward pieces
-// Adam is r4st::k_st_apply (k_ek_adam; TF1 AdamOptimizer and Keras Adam are the same ResourceApplyAdam update).
+// Adam is r4dense::k_keras_adam (TF1 AdamOptimizer and Keras Adam are the same ResourceApplyAdam update).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -91,82 +92,6 @@ __host__ __device__ inline uint32_t draw24(uint64_t seed, uint64_t call, int str
 // dropout keep of one element: kept when U >= rate (TF's floor(keep_prob + U) == 1)
 __device__ __forceinline__ bool kept(uint64_t seed, uint64_t call, int stream, uint64_t elem, float rate) {
   return rate <= 0.f || (float)draw24(seed, call, stream, elem) * (1.0f / 16777216.0f) >= rate;
-}
-
-// ------------------------------------------------------------------------------------------------
-// k_ek_gemm: C[z](m, n) = alpha sum_k A[z](m, k) B[z](k, n) (+ C if beta) (+ bias[n]) (relu).  Operand X's element (i, j) of
-// batch z sits at X + (z / zdiv) so + (z % zdiv) si + i s0 + j s1.  ktot > 0: split-K, batch z covers k in
-// [z K, min((z + 1) K, ktot)) and A / B advance by z K along k (their batch strides are then ignored).
-// 64 x 64 tile, 256 threads of 4 x 4 outputs, K in steps of 16 through shared memory.
-// ------------------------------------------------------------------------------------------------
-struct Op { const float* p; int64_t so, si, s0, s1; };
-struct Gemm {
-  Op A, B;
-  float* C; int64_t cso, csi, cs0, cs1;
-  const float* bias;
-  int M, N, K, zdiv;
-  int64_t ktot;
-  float alpha;
-  int beta, relu;
-};
-constexpr int GT = 64, GK = 16, GNT = 256;
-__global__ void __launch_bounds__(GNT) k_ek_gemm(Gemm g) {
-  __shared__ float As[GK][GT + 4], Bs[GK][GT + 4];
-  const int z = blockIdx.z, zo = z / g.zdiv, zi = z % g.zdiv;
-  const int m0 = blockIdx.y * GT, n0 = blockIdx.x * GT;
-  const float* A = g.A.p;
-  const float* B = g.B.p;
-  int K = g.K;
-  if (g.ktot > 0) {
-    const int64_t k0 = (int64_t)z * g.K;
-    A += k0 * g.A.s1; B += k0 * g.B.s0;
-    K = (int)min((int64_t)g.K, g.ktot - k0);
-  } else {
-    A += zo * g.A.so + zi * g.A.si; B += zo * g.B.so + zi * g.B.si;
-  }
-  const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
-  float acc[4][4] = {};
-  for (int k0 = 0; k0 < K; k0 += GK) {
-    for (int e = tid; e < GT * GK; e += GNT) {
-      // A: e -> (m, k) with k fastest when A is k-contiguous, else m fastest; B likewise with n
-      int am, ak, bk, bn;
-      if (g.A.s1 == 1) { am = e / GK; ak = e % GK; } else { am = e % GT; ak = e / GT; }
-      if (g.B.s1 == 1) { bk = e / GT; bn = e % GT; } else { bk = e % GK; bn = e / GK; }
-      const int gm = m0 + am, gk = k0 + ak;
-      As[ak][am] = (gm < g.M && gk < K) ? A[gm * g.A.s0 + (int64_t)gk * g.A.s1] : 0.f;
-      const int gk2 = k0 + bk, gn = n0 + bn;
-      Bs[bk][bn] = (gn < g.N && gk2 < K) ? B[(int64_t)gk2 * g.B.s0 + gn * g.B.s1] : 0.f;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int kk = 0; kk < GK; ++kk) {
-      float a[4], b[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) { a[i] = As[kk][ty + 16 * i]; b[i] = Bs[kk][tx + 16 * i]; }
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-  float* C = g.C + (g.ktot > 0 ? (int64_t)z * g.cso : zo * g.cso + zi * g.csi);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int m = m0 + ty + 16 * i;
-    if (m >= g.M) continue;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int n = n0 + tx + 16 * j;
-      if (n >= g.N) continue;
-      float* c = C + m * g.cs0 + n * g.cs1;
-      float r = g.alpha * acc[i][j];
-      if (g.beta) r += *c;
-      if (g.bias) r += g.bias[n];
-      if (g.relu) r = fmaxf(r, 0.f);
-      *c = r;
-    }
-  }
 }
 
 // k_ek_colsum: out[i] (+)= scale sum_{r < R} in[r rs + (i / w) ls + i % w], rows in order, for i < N.  blockIdx.y = chunk of
@@ -737,9 +662,5 @@ __global__ void k_ek_gloss(const float* __restrict__ ce, const float* __restrict
   for (int b = 0; b < n; ++b) s += ce[b] * reward[b];
   *loss = s * scale;
 }
-
-// Adam: TF1's AdamOptimizer is the simulator trainer's ResourceApplyAdam update, so both run the one kernel
-// (an empty embedding range: H = 0)
-inline constexpr auto k_ek_adam = r4st::k_st_apply;
 
 }  // namespace r4ek

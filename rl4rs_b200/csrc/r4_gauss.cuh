@@ -13,13 +13,13 @@
 // The gradient runs in two launches per chunk of at most CH samples:
 //   k_gauss_rows   one CTA per TS samples: forward of both branches, loss derivatives, backward through the activations;
 //                  writes every layer's input rows X and output-gradient rows dZ (no weight gradients).
-//   k_gauss_wgrad  one CTA owns one 64 x 64 tile of one dW = X^T dZ (or a bias = column sum of dZ) and walks the samples
-//                  in order: every gradient element has exactly one writer and a fixed summation order, so the result is
-//                  deterministic without per-CTA partial gradients.  One extra CTA sums the per-sample loss statistics.
+//   r4dense::k_dense_wgrad  one CTA per 64 x 64 tile of one dW = X^T dZ (or a bias = column sum of dZ), walking the
+//                  samples in order; later chunks add.  One extra CTA sums the per-sample loss statistics.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "r4_dense.cuh"
 #include "r4_ppo.cuh"
 
 namespace r4gauss {
@@ -297,99 +297,21 @@ __global__ void __launch_bounds__(NT) k_gauss_rows(Layout L, r4ppo::LossHyper hp
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// gradient, part 2: weight gradients.  Job j: out[i][c] (+)= sum_q X[q][i] dZ[q][c] over the cn rows (X == nullptr: a
-// bias, X = 1 and M = 1).  64 x 64 output tile per CTA, 4 x 4 per thread; first chunk stores, later chunks add.
-// ------------------------------------------------------------------------------------------------
-constexpr int NJOB = 12, WT = 64, WK = 32;
-struct Job {
-  const float* X;
-  const float* Z;
-  int M, N, off, tile0;
-};
-struct Jobs {
-  Job j[NJOB];
-  int ntiles;
-};
-
-__global__ void __launch_bounds__(NT) k_gauss_wgrad(Jobs jobs, int cn, int first, float* __restrict__ grad,
-                                                    const float* __restrict__ stats, float* __restrict__ stat_sum,
-                                                    float* __restrict__ stats_accum, float stat_scale) {
-  __shared__ float xs[WK][WT];
-  __shared__ float zs[WK][WT];
-  const int tid = threadIdx.x;
-  if ((int)blockIdx.x == jobs.ntiles) {                    // the loss statistics, summed in sample order
-    if (tid < 5) {
-      float a = first ? 0.f : stat_sum[tid];
-      for (int q = 0; q < cn; ++q) a += stats[q * 5 + tid];
-      stat_sum[tid] = a;
-      if (stats_accum) stats_accum[tid] += a * stat_scale;
-    }
-    return;
-  }
-  int jb = 0;
-  while (jb + 1 < NJOB && (int)blockIdx.x >= jobs.j[jb + 1].tile0) ++jb;
-  const Job J = jobs.j[jb];
-  const int t = blockIdx.x - J.tile0, tn = (J.N + WT - 1) / WT;
-  const int i0 = (t / tn) * WT, c0 = (t % tn) * WT;
-  const int ty = tid / 16, tx = tid % 16;                  // rows i0 + 4 ty .. +3, columns c0 + 4 tx .. +3
-  float acc[4][4];
-#pragma unroll
-  for (int a = 0; a < 4; ++a)
-#pragma unroll
-    for (int b = 0; b < 4; ++b) acc[a][b] = 0.f;
-  for (int k0 = 0; k0 < cn; k0 += WK) {
-    __syncthreads();
-    for (int e = tid; e < WK * WT; e += NT) {
-      const int k = e / WT, c = e % WT, q = k0 + k;
-      const bool ok = q < cn;
-      xs[k][c] = (ok && i0 + c < J.M) ? (J.X ? J.X[(size_t)q * J.M + i0 + c] : 1.f) : 0.f;
-      zs[k][c] = (ok && c0 + c < J.N) ? J.Z[(size_t)q * J.N + c0 + c] : 0.f;
-    }
-    __syncthreads();
-#pragma unroll 4
-    for (int k = 0; k < WK; ++k) {
-      float xv[4], zv[4];
-#pragma unroll
-      for (int a = 0; a < 4; ++a) { xv[a] = xs[k][4 * ty + a]; zv[a] = zs[k][4 * tx + a]; }
-#pragma unroll
-      for (int a = 0; a < 4; ++a)
-#pragma unroll
-        for (int b = 0; b < 4; ++b) acc[a][b] = fmaf(xv[a], zv[b], acc[a][b]);
-    }
-  }
-#pragma unroll
-  for (int a = 0; a < 4; ++a) {
-    const int i = i0 + 4 * ty + a;
-    if (i >= J.M) continue;
-#pragma unroll
-    for (int b = 0; b < 4; ++b) {
-      const int c = c0 + 4 * tx + b;
-      if (c >= J.N) continue;
-      float* g = grad + J.off + (size_t)i * J.N + c;
-      *g = first ? acc[a][b] : *g + acc[a][b];
-    }
-  }
-}
-
-// The twelve jobs of one chunk, in parameter order.
-inline Jobs make_jobs(const Layout& L, const Planes& P) {
-  Jobs J;
-  const int D2 = 2 * L.D;
-  const Job list[NJOB] = {
-      {P.x, P.d1, OBS, H, L.p_w1, 0},     {nullptr, P.d1, 1, H, L.p_b1, 0},
-      {P.h1, P.d2, H, H, L.p_w2, 0},      {nullptr, P.d2, 1, H, L.p_b2, 0},
-      {P.h2, P.dout, H, D2, L.p_wo, 0},   {nullptr, P.dout, 1, D2, L.p_bo, 0},
-      {P.x, P.e1, OBS, H, L.v_w1, 0},     {nullptr, P.e1, 1, H, L.v_b1, 0},
-      {P.g1, P.e2, H, H, L.v_w2, 0},      {nullptr, P.e2, 1, H, L.v_b2, 0},
-      {P.g2, P.dv, H, 1, L.v_wo, 0},      {nullptr, P.dv, 1, 1, L.v_bo, 0}};
-  int t = 0;
-  for (int k = 0; k < NJOB; ++k) {
-    J.j[k] = list[k];
-    J.j[k].tile0 = t;
-    t += ((list[k].M + WT - 1) / WT) * ((list[k].N + WT - 1) / WT);
-  }
-  J.ntiles = t;
+// The twelve weight-gradient jobs of one chunk (r4dense::k_dense_wgrad), in parameter order.
+inline r4dense::Jobs make_jobs(const Layout& L, const Planes& P) {
+  r4dense::Jobs J;
+  int k = 0;
+  auto layer = [&](const float* X, const float* dZ, int M, int N, int w, int b) {
+    J.j[k++] = {X, dZ, M, M, N, w, 0};
+    J.j[k++] = {nullptr, dZ, 1, 1, N, b, 0};
+  };
+  layer(P.x, P.d1, OBS, H, L.p_w1, L.p_b1);
+  layer(P.h1, P.d2, H, H, L.p_w2, L.p_b2);
+  layer(P.h2, P.dout, H, 2 * L.D, L.p_wo, L.p_bo);
+  layer(P.x, P.e1, OBS, H, L.v_w1, L.v_b1);
+  layer(P.g1, P.e2, H, H, L.v_w2, L.v_b2);
+  layer(P.g2, P.dv, H, 1, L.v_wo, L.v_bo);
+  r4dense::tile_jobs(J, k);
   return J;
 }
 

@@ -10,6 +10,8 @@
 #include "r4_rainbow.cuh"
 #include "r4_batchrl.cuh"
 #include "r4_simtrain.cuh"
+#include "r4_dense.cuh"
+#include "r4_exactk.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -19,6 +21,7 @@
 #include <vector>
 
 using namespace r4h;
+using namespace r4dense;
 
 // Dynamic shared memory starts at one offset for every kernel of a module, aligned for the module's most-aligned
 // extern __shared__ array.  The env module's tensor-core kernels align theirs to 1024 bytes; the learner kernels were
@@ -293,7 +296,7 @@ static int gauss_grad_impl(int mode, const float* params, const float* obs, cons
   const r4gauss::Layout L = r4gauss::make_layout(D);
   const r4ppo::LossHyper hp{mode, clip, vf_clip, vf_coeff, kl_coeff, ent_coeff, inv_n};
   const r4gauss::Planes P = r4gauss::make_planes(scratch, D);
-  const r4gauss::Jobs J = r4gauss::make_jobs(L, P);
+  const Jobs J = r4gauss::make_jobs(L, P);
   for (int c0 = 0; c0 < n; c0 += r4gauss::CH) {
     const int cn = std::min(r4gauss::CH, n - c0);
     const bool last = c0 + cn >= n;
@@ -301,8 +304,8 @@ static int gauss_grad_impl(int mode, const float* params, const float* obs, cons
                     r4gauss::ROWS_SMEM, S(stream), false, L, hp, params, obs, action, old_logp, old_dist, old_value, adv, target,
                     idx, c0, cn, P);
     if (!rc)
-      rc = launch(FAM_ONLINE, "k_gauss_wgrad", r4gauss::k_gauss_wgrad, J.ntiles + 1, r4gauss::NT, 0, S(stream), false, J, cn,
-                  c0 == 0, grad_out, P.stats, stat_sum, last ? stats_accum : nullptr, stat_scale);
+      rc = launch(FAM_ONLINE, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, S(stream), false, J, cn, c0 == 0, grad_out,
+                  Stats{P.stats, 5, stat_sum, last ? stats_accum : nullptr, stat_scale, 1});
     if (rc) return rc;
   }
   return R4_OK;
@@ -528,14 +531,14 @@ int r4_ddpg_grad(const float* params, const float* target, int action_dim, int t
   const r4ddpg::Layout L = r4ddpg::make_layout(action_dim, twin != 0);
   r4ddpg::Planes P = r4ddpg::make_planes(scratch, action_dim, twin != 0, n);
   if (td) P.td = td;
-  const r4ddpg::Jobs J = r4ddpg::make_jobs(L, P);
+  const Jobs J = r4ddpg::make_jobs(L, P);
   const r4ddpg::Replay R{r_obs, r_action, r_reward, r_new_obs, r_done};
   const r4ddpg::Hyper hp{gamma, target_noise, noise_clip, inv_n};
   if (int rc = launch(FAM_ONLINE, "k_ddpg_rows", r4ddpg::k_ddpg_rows, (n + r4ddpg::TS - 1) / r4ddpg::TS, r4ddpg::NT,
                       r4ddpg::ROWS_SMEM, S(stream), false, L, hp, params, target, R, idx, weights, smooth_noise, n, P))
     return rc;
-  return launch(FAM_ONLINE, "k_ddpg_wgrad", r4ddpg::k_ddpg_wgrad, J.ntiles + 1, r4ddpg::NT, 0, S(stream), false, J, n, grad,
-                P.stats, stats, inv_n);
+  return launch(FAM_ONLINE, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, S(stream), false, J, n, 1, grad,
+                Stats{P.stats, 3, nullptr, stats, inv_n, 0});
 }
 
 int r4_ddpg_apply(float* params, float* target, const float* grad, float* m, float* v, int action_dim, int twin, int actor_step,
@@ -624,14 +627,14 @@ int r4_rainbow_grad(const float* params, const float* target, int num_actions, i
   const r4rb::Layout L = r4rb::make_layout(num_actions, num_atoms);
   r4rb::Planes P = r4rb::make_planes(scratch, L, n);
   if (td) P.td = td;
-  const r4ddpg::Jobs J = r4rb::make_jobs(L, P);
+  const Jobs J = r4rb::make_jobs(L, P);
   const r4rb::Replay R{r_obs, r_action, r_reward, r_new_obs, r_done};
   const r4rb::Hyper hp{v_min, v_max, (v_max - v_min) / (float)(num_atoms - 1), gamma_n, inv_n};
   if (int rc = launch(FAM_ONLINE, "k_rainbow_rows", r4rb::k_rainbow_rows, (n + r4rb::TS - 1) / r4rb::TS, r4rb::NT,
                       r4rb::rows_smem(L.A, L.AZ), S(stream), false, L, hp, params, target, R, idx, weights, n, P))
     return rc;
-  return launch(FAM_ONLINE, "k_ddpg_wgrad", r4ddpg::k_ddpg_wgrad, J.ntiles + 1, r4ddpg::NT, 0, S(stream), false, J, n, grad,
-                P.stats, stats, inv_n);
+  return launch(FAM_ONLINE, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, S(stream), false, J, n, 1, grad,
+                Stats{P.stats, 3, nullptr, stats, inv_n, 0});
 }
 
 int r4_rainbow_apply(float* params, float* target, const float* grad, float* m, float* v, int num_actions, int num_atoms,
@@ -710,9 +713,9 @@ static int bq_grad(int algo, int K, int A, const float* params, const float* tar
   int rc = launch(FAM_BATCHRL, "k_bq_rows", rows[algo], (n + r4bq::TS - 1) / r4bq::TS, r4bq::NT, r4bq::rows_smem(K, A), st, pdl,
                   L, hp, params, target, bq_data(data), idx, n, P);
   if (rc) return rc;
-  const r4ddpg::Jobs J = r4bq::make_jobs(L, P);
-  if ((rc = launch(FAM_BATCHRL, "k_ddpg_wgrad", r4ddpg::k_ddpg_wgrad, J.ntiles + 1, r4ddpg::NT, 0, st, false, J, n, grad, P.stats,
-                   stats, 1.0f / (float)n)))
+  const Jobs J = r4bq::make_jobs(L, P);
+  if ((rc = launch(FAM_BATCHRL, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, st, false, J, n, 1, grad,
+                   Stats{P.stats, 3, nullptr, stats, 1.0f / (float)n, 0})))
     return rc;
   const int nets = r4bq::n_mnets(algo);
   if (!nets) return R4_OK;
@@ -804,9 +807,9 @@ static bool st_data_ok(const r4_simtrain_data* d) {
 static int st_gemm(bool tb, const float* A, int lda, const float* B, int ldb, const float* bias, float* C, int ldc, int M, int N,
                    int K, int epi, cudaStream_t st, const float* aux = nullptr, const float* mul = nullptr, float* pre = nullptr,
                    int accum = 0) {
-  const r4st::Gemm g{A, lda, B, ldb, bias, C, ldc, M, N, K, epi, accum, aux, mul, pre};
-  const dim3 grid((N + r4st::GT - 1) / r4st::GT, (M + r4st::GT - 1) / r4st::GT);
-  return st_launch("k_st_gemm", tb ? r4st::k_st_gemm<true> : r4st::k_st_gemm<false>, grid, r4st::NTH, st, g);
+  const Op b = tb ? Op{B, 0, 0, 1, ldb} : Op{B, 0, 0, ldb, 1};
+  const Gemm g{Op{A, 0, 0, lda, 1}, b, C, 0, 0, ldc, 1, bias, aux, mul, pre, M, N, K, 1, 0, 1.f, epi, accum};
+  return st_launch("k_dense_gemm", gemm_kernel(g), dim3((N + GT - 1) / GT, (M + GT - 1) / GT), NT, st, g);
 }
 
 // The pieces every net shares.  Lay / Pl are a net's layout and planes (Layout / Planes for DIEN, NLayout / NPlanes for the
@@ -827,27 +830,21 @@ static int st_tower_bwd(const Lay& L, const float* prm, const Pl& P, int n, cons
   return rc ? rc : st_gemm(true, P.dT2, U, prm + L.dw2, U, nullptr, P.dT1, U, n, U, U, EP_DELU, st, P.T1, P.keep);
 }
 
-static r4ddpg::Job st_job(const float* X, int ldx, const float* Z, int M, int N, int64_t off) {
-  return r4ddpg::Job{X, Z, ldx, M, N, (int)off, 0};
+static Job st_job(const float* X, int ldx, const float* Z, int M, int N, int64_t off) {
+  return Job{X, Z, ldx, M, N, (int)off, 0};
 }
 // the tower's four weight-gradient jobs, the first of a net's n-row jobs; returns the job count
 template <class Lay, class Pl>
-static int st_tower_jobs(r4ddpg::Jobs& J, const Lay& L, const Pl& P) {
+static int st_tower_jobs(Jobs& J, const Lay& L, const Pl& P) {
   using namespace r4st;
   int k = 0;
   J.j[k++] = st_job(P.dense, ND, P.dT1, ND, U, L.dw1);  J.j[k++] = st_job(nullptr, 1, P.dT1, 1, U, L.db1);
   J.j[k++] = st_job(P.T1d, U, P.dT2, U, U, L.dw2);      J.j[k++] = st_job(nullptr, 1, P.dT2, 1, U, L.db2);
   return k;
 }
-static int st_wgrad(r4ddpg::Jobs J, int njob, int rows, float* grad, cudaStream_t st) {
-  J.njob = njob;
-  int t = 0;
-  for (int i = 0; i < njob; ++i) {
-    J.j[i].tile0 = t;
-    t += ((J.j[i].M + r4ddpg::WT - 1) / r4ddpg::WT) * ((J.j[i].N + r4ddpg::WT - 1) / r4ddpg::WT);
-  }
-  J.ntiles = t;
-  return st_launch("k_ddpg_wgrad", r4ddpg::k_ddpg_wgrad, t, r4ddpg::NT, st, J, rows, grad, nullptr, nullptr, 0.f);
+static int st_wgrad(Jobs J, int njob, int rows, float* grad, cudaStream_t st) {
+  tile_jobs(J, njob);
+  return st_launch("k_dense_wgrad", k_dense_wgrad, J.ntiles, NT, st, J, rows, 1, grad, Stats{});
 }
 
 // The head's loss: logits Z [n][C] -> dZ (may be NULL), the per-sample rows srow, stats, acc and probs.
@@ -950,7 +947,7 @@ static int st_backward(int head, const r4st::Layout& L, const float* prm, const 
       return rc;
   }
   // dense weight gradients: one launch over the n-row jobs, one per sequence over its 64 n-row jobs
-  r4ddpg::Jobs J;
+  Jobs J;
   int k = st_tower_jobs(J, L, P);
   J.j[k++] = st_job(P.allf, FEAT, P.dO, FEAT, OBS, L.ow); J.j[k++] = st_job(nullptr, 1, P.dO, 1, OBS, L.ob);
   J.j[k++] = st_job(P.O, OBS, P.dZ, OBS, C, L.rw);      J.j[k++] = st_job(nullptr, 1, P.dZ, 1, C, L.rb);
@@ -1076,7 +1073,7 @@ static int sn_backward(int head, const r4st::NLayout& L, const float* prm, const
     }
   }
   // dense weight gradients over the n-row jobs
-  r4ddpg::Jobs J;
+  Jobs J;
   int k = st_tower_jobs(J, L, P);
   if (L.net == NET_DNN) {
     J.j[k++] = st_job(P.A, L.FA, P.dF, L.FA, OBS, L.fcw); J.j[k++] = st_job(nullptr, 1, P.dF, 1, OBS, L.fcb);
@@ -1149,8 +1146,8 @@ static int st_apply(int net, int head, int H, float* params, float* grad, float*
     np = L.n; emb_cat = L.emb_cat; emb_seq = L.emb_seq >= 0 ? L.emb_seq : L.emb_cat;
   }
   const double alpha = (double)lr * std::sqrt(1.0 - std::pow((double)b2, step)) / (1.0 - std::pow((double)b1, step));
-  return st_launch("k_st_apply", k_st_apply, (unsigned)((np + 255) / 256), 256, st, np, (int64_t)H, emb_cat, emb_seq, params, grad,
-                   m, v, (float)alpha, b1, b2, eps);
+  return st_launch("k_keras_adam", k_keras_adam, (unsigned)((np + 255) / 256), 256, st, np, (int64_t)H * E, emb_cat, emb_seq, params,
+                   grad, m, v, (float)alpha, b1, b2, eps);
 }
 
 // The one argument check of every entry point: the (net, head) pair, the hash size, n, the drop rate, the Adam step and the
@@ -1280,7 +1277,6 @@ int ek_launch(const char* name, void (*kernel)(P...), dim3 grid, int threads, si
 
 unsigned blocks(int64_t n, int per) { return (unsigned)((n + per - 1) / per); }
 
-using r4ek::Op;
 constexpr int EK_SPLITS = 128;                 // split-K partials of a weight gradient at most
 constexpr int64_t EK_KC = 1024;                // rows per split-K partial at least
 
@@ -1291,16 +1287,15 @@ Op tr(const float* p, int64_t ld) { return Op{p, 0, 0, 1, ld}; }
 // C[M, N] (ldc) = alpha A B (+ C if beta) (+ bias) (relu), one batch
 int ek_mm(cudaStream_t st, Op A, Op B, float* C, int64_t ldc, int M, int N, int K, const float* bias = nullptr,
           int relu = 0, int beta = 0, float alpha = 1.f) {
-  r4ek::Gemm g{A, B, C, 0, 0, ldc, 1, bias, M, N, K, 1, 0, alpha, beta, relu};
-  return ek_launch("k_ek_gemm", r4ek::k_ek_gemm, dim3(blocks(N, r4ek::GT), blocks(M, r4ek::GT), 1), r4ek::GNT, 0, st, g);
+  const Gemm g{A, B, C, 0, 0, ldc, 1, bias, nullptr, nullptr, nullptr, M, N, K, 1, 0, alpha, relu ? EP_RELU : EP_LIN, beta};
+  return ek_launch("k_dense_gemm", gemm_kernel(g), dim3(blocks(N, GT), blocks(M, GT), 1), NT, 0, st, g);
 }
 
 // the per-(row, head) attention products: batch z = 4 b + h
 int ek_bmm(cudaStream_t st, Op A, Op B, float* C, int64_t cso, int64_t csi, int64_t cs0, int64_t cs1, int M, int N, int K,
            int n, float alpha, int beta = 0) {
-  r4ek::Gemm g{A, B, C, cso, csi, cs0, cs1, nullptr, M, N, K, r4ek::NH, 0, alpha, beta, 0};
-  return ek_launch("k_ek_gemm", r4ek::k_ek_gemm, dim3(blocks(N, r4ek::GT), blocks(M, r4ek::GT), n * r4ek::NH), r4ek::GNT, 0,
-                   st, g);
+  const Gemm g{A, B, C, cso, csi, cs0, cs1, nullptr, nullptr, nullptr, nullptr, M, N, K, r4ek::NH, 0, alpha, EP_LIN, beta};
+  return ek_launch("k_dense_gemm", gemm_kernel(g), dim3(blocks(N, GT), blocks(M, GT), n * r4ek::NH), NT, 0, st, g);
 }
 
 // out[N] (+)= sum over R rows (stride rs) of in[r, (i / w) ls + i % w]: chunks of rows into partials, then their sum
@@ -1321,9 +1316,9 @@ int ek_wgrad(cudaStream_t st, const float* X, int64_t ldx, const float* dY, int6
              float* part) {
   const int64_t S = std::min<int64_t>(EK_SPLITS, (R + EK_KC - 1) / EK_KC);
   const int64_t kc = (R + S - 1) / S;
-  r4ek::Gemm g{tr(X, ldx), rm(dY, ldy), part, (int64_t)K * N, 0, N, 1, nullptr, K, N, (int)kc, 1, R, 1.f, 0, 0};
-  if (int rc = ek_launch("k_ek_gemm", r4ek::k_ek_gemm, dim3(blocks(N, r4ek::GT), blocks(K, r4ek::GT), (unsigned)S), r4ek::GNT,
-                         0, st, g))
+  const Gemm g{tr(X, ldx), rm(dY, ldy), part, (int64_t)K * N, 0, N, 1, nullptr, nullptr, nullptr, nullptr, K, N, (int)kc, 1, R,
+               1.f, EP_LIN, 0};
+  if (int rc = ek_launch("k_dense_gemm", gemm_kernel(g), dim3(blocks(N, GT), blocks(K, GT), (unsigned)S), NT, 0, st, g))
     return rc;
   return ek_launch("k_ek_colsum", r4ek::k_ek_colsum, dim3(blocks((int64_t)K * N, 128), 1), 128, 0, st, (const float*)part, S,
                    (int64_t)K * N, K * N, (int64_t)0, K * N, S, dW, (int64_t)0, 1.f, 1);
@@ -1706,6 +1701,6 @@ int r4_exactk_adam(int net, float* params, float* grad, float* m, float* v, int 
   const int64_t np = r4_exactk_num_params(net);
   if (np < 0 || !params || !grad || !m || !v || step < 1) return fail(R4_ERR_ARG, "bad argument");
   const float alpha = lr * sqrtf(1.f - powf(beta2, (float)step)) / (1.f - powf(beta1, (float)step));
-  return ek_launch("k_st_apply", r4ek::k_ek_adam, blocks(np, 256), 256, 0, S(stream), np, (int64_t)0, np, np, params, grad, m, v,
-                   alpha, beta1, beta2, eps);
+  return ek_launch("k_keras_adam", k_keras_adam, blocks(np, 256), 256, 0, S(stream), np, (int64_t)0, np, np, params, grad, m,
+                   v, alpha, beta1, beta2, eps);
 }

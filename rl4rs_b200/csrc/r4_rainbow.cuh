@@ -14,7 +14,7 @@
 //                        sw1[256,128] sb1[128] sw2[128,atoms] sb2[atoms]      (12 tensors; the target has the same layout)
 //
 // The gradient runs in two launches: k_rainbow_rows (one CTA per TS samples: both nets on s', the projection, the online
-// net on s, the loss and the backward rows, written to the scratch planes), then r4ddpg::k_ddpg_wgrad over this net's 12
+// net on s, the loss and the backward rows, written to the scratch planes), then r4dense::k_dense_wgrad over this net's 12
 // jobs (one CTA per 64 x 64 tile of dW = X^T dZ, samples walked in order: deterministic).  k_rainbow_apply clips every
 // tensor's gradient to norm <= clip on its own (RLlib's minimize_and_clip), runs Adam and, when flagged, copies the
 // parameters into the target.
@@ -349,10 +349,10 @@ __global__ void __launch_bounds__(NT) k_rainbow_rows(Layout L, Hyper hp, const f
 }
 
 // ------------------------------------------------------------------------------------------------
-// learner, part 2: the weight gradients of the 12 tensors, as jobs of r4ddpg::k_ddpg_wgrad
+// learner, part 2: the weight gradients of the 12 tensors, as jobs of r4dense::k_dense_wgrad
 // ------------------------------------------------------------------------------------------------
-inline r4ddpg::Jobs make_jobs(const Layout& L, const Planes& P) {
-  r4ddpg::Jobs J;
+inline r4dense::Jobs make_jobs(const Layout& L, const Planes& P) {
+  r4dense::Jobs J;
   int k = 0;
   auto layer = [&](const float* X, const float* dZ, int M, int N, int w, int b) {
     J.j[k++] = {X, dZ, M, M, N, w, 0};
@@ -364,13 +364,7 @@ inline r4ddpg::Jobs make_jobs(const Layout& L, const Planes& P) {
   layer(P.ha, P.da2, HQ, L.AZ, L.aw2, L.ab2);
   layer(P.h2, P.ds1, HT, HQ, L.sw1, L.sb1);
   layer(P.hs, P.ds2, HQ, L.Z, L.sw2, L.sb2);
-  J.njob = k;
-  int t = 0;
-  for (int i = 0; i < k; ++i) {
-    J.j[i].tile0 = t;
-    t += ((J.j[i].M + r4ddpg::WT - 1) / r4ddpg::WT) * ((J.j[i].N + r4ddpg::WT - 1) / r4ddpg::WT);
-  }
-  J.ntiles = t;
+  r4dense::tile_jobs(J, k);
   return J;
 }
 

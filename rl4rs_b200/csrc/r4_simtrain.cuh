@@ -8,8 +8,8 @@
 //   k_st_gather      per sample: the sample's cat / dense / seq features from the per-record store, the dropout keep scales,
 //                    the category self-attention (softmax(E E^T) E, mean over the 21 slots | flatten E), the query q (mean of
 //                    emb_seq over the last 10 cat ids) and the emb_seq rows of both sequences
-//   k_st_gemm        C = epilogue(A B [+ bias]) for every batched dense product (towers, input projections, attention MLP,
-//                    head, and their transposed products in the backward)
+//   r4dense::k_dense_gemm  C = epilogue(A B [+ bias]) for every batched dense product (towers, input projections,
+//                    attention MLP, head, and their transposed products in the backward)
 //   k_st_gru_fwd     GRU-1 (hidden 128) and the AUGRU (hidden 256) over 64 steps, 8 samples per CTA, the hidden state in
 //                    shared memory and the recurrent weights streamed from L2; stores h_{t-1}, r, u, c~ and r h_{t-1}
 //   k_st_gru_bwd     the same recurrences in reverse (BPTT), dh kept in shared memory; writes the pre-activation gradients
@@ -20,17 +20,18 @@
 //   k_st_loss_slate  the slate-label heads (nets/dien_slate.py, dien_slate_multiclass.py): 9 sigmoid columns against the
 //                    page's clicks, or a 22-way softmax against the click pattern's class; same one-CTA ordered sums
 //   k_st_cat_bwd     the category self-attention backward
-//   r4ddpg::k_ddpg_wgrad  every dW = X^T dZ and bias, one CTA per 64 x 64 tile walking the rows in order
+//   r4dense::k_dense_wgrad  every dW = X^T dZ and bias, one CTA per 64 x 64 tile walking the rows in order
 //   k_st_embkeys + a stable CUB radix sort + k_st_embsum   the two embedding tables' gradients: (table, id) keys of every
 //                    (sample, slot) sorted stably, each run summed in order into the dense gradient buffer
-//   k_st_apply       Keras Adam over every parameter; clears the embedding gradient rows the step wrote
+//   r4dense::k_keras_adam  Keras Adam over every parameter; clears the embedding gradient rows the step wrote
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <cub/device/device_radix_sort.cuh>
 
-#include "r4_ddpg.cuh"
+#include "r4_dense.cuh"
+#include "r4_ppo.cuh"
 
 namespace r4st {
 
@@ -169,8 +170,8 @@ __host__ inline Planes make_planes(void* base, int n, int C = 2) {
 }
 __host__ inline size_t scratch_bytes(int n, int C = 2) { return make_planes(nullptr, n, C).bytes; }
 
-__device__ __forceinline__ float sigm(float x) { return 1.f / (1.f + expf(-x)); }
-__device__ __forceinline__ float elu(float x) { return x > 0.f ? x : expm1f(x); }
+using r4dense::elu;
+using r4dense::sigm;
 __device__ __forceinline__ int clampid(int id, int64_t H) { return id < 0 ? 0 : (id >= H ? (int)(H - 1) : id); }
 
 // the dropout draw of (seed, counter, sample, unit): U[0, 1) from the top 24 bits of a counter-based hash
@@ -273,88 +274,6 @@ __global__ void __launch_bounds__(E) k_st_gather(GatherArgs g, int64_t emb_cat, 
       const int id = clampid(g.D.seq[(rec * 2 + i) * T + t], g.H);
       P.sp[i].X[((size_t)s * T + t) * E + c] = __ldg(prm + emb_seq + (int64_t)id * E + c);
     }
-}
-
-// ------------------------------------------------------------------------------------------------
-// k_st_gemm: C[M][N] (ldc) = epi(sum_k A[m][k] B[k][n] (+ bias[n])), B = W[k][n] (ldb) or, TB, W[n][k] (ldb).
-//   EP_LIN   v = acc + bias         EP_SIG  v = sigmoid(acc + bias)     EP_ELU  v = elu(acc + bias)
-//   EP_DSIG  v = acc y (1 - y)      EP_DELU v = acc (y > 0 ? 1 : y + 1)   (y = aux[m][n], ld N: the forward activation)
-// then pre (may be NULL, ld N) receives v, v *= mul[m][n] (may be NULL, ld N), and C = v or C += v (accum).
-// 64 x 64 tiles, 16-deep k-slices, 4 x 4 outputs per thread, each output summed over k in order.
-// ------------------------------------------------------------------------------------------------
-enum { EP_LIN = 0, EP_SIG = 1, EP_ELU = 2, EP_DSIG = 3, EP_DELU = 4 };
-struct Gemm {
-  const float* A; int lda;
-  const float* B; int ldb;
-  const float* bias;
-  float* C; int ldc;
-  int M, N, K, epi, accum;
-  const float* aux;
-  const float* mul;
-  float* pre;
-};
-constexpr int GT = 64, GK = 16;
-template <bool TB>
-__global__ void __launch_bounds__(NTH) k_st_gemm(Gemm g) {
-  __shared__ float as[GK][GT + 4];
-  __shared__ float bs[GK][GT + 4];
-  const int tid = threadIdx.x, ty = tid / 16, tx = tid % 16;
-  const int m0 = blockIdx.y * GT, n0 = blockIdx.x * GT;
-  float acc[4][4];
-#pragma unroll
-  for (int a = 0; a < 4; ++a)
-#pragma unroll
-    for (int b = 0; b < 4; ++b) acc[a][b] = 0.f;
-  for (int k0 = 0; k0 < g.K; k0 += GK) {
-    for (int e = tid; e < GK * GT; e += NTH) {
-      const int r = e / GK, k = e % GK;           // A: rows m0 + r, k contiguous
-      const int m = m0 + r, kk = k0 + k;
-      as[k][r] = (m < g.M && kk < g.K) ? g.A[(size_t)m * g.lda + kk] : 0.f;
-    }
-    for (int e = tid; e < GK * GT; e += NTH) {
-      int k, c;
-      if (TB) { c = e / GK; k = e % GK; } else { k = e / GT; c = e % GT; }
-      const int nn = n0 + c, kk = k0 + k;
-      float v = 0.f;
-      if (nn < g.N && kk < g.K) v = TB ? g.B[(size_t)nn * g.ldb + kk] : g.B[(size_t)kk * g.ldb + nn];
-      bs[k][c] = v;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < GK; ++k) {
-      float av[4], bv[4];
-#pragma unroll
-      for (int a = 0; a < 4; ++a) { av[a] = as[k][ty + 16 * a]; bv[a] = bs[k][tx + 16 * a]; }
-#pragma unroll
-      for (int a = 0; a < 4; ++a)
-#pragma unroll
-        for (int b = 0; b < 4; ++b) acc[a][b] = fmaf(av[a], bv[b], acc[a][b]);
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int a = 0; a < 4; ++a) {
-    const int m = m0 + ty + 16 * a;
-    if (m >= g.M) continue;
-#pragma unroll
-    for (int b = 0; b < 4; ++b) {
-      const int n = n0 + tx + 16 * b;
-      if (n >= g.N) continue;
-      const size_t o = (size_t)m * g.N + n;
-      float v = acc[a][b];
-      if (g.epi <= EP_ELU) {
-        if (g.bias) v += g.bias[n];
-        v = g.epi == EP_SIG ? sigm(v) : g.epi == EP_ELU ? elu(v) : v;
-      } else {
-        const float y = g.aux[o];
-        v = g.epi == EP_DSIG ? v * (y * (1.f - y)) : v * (y > 0.f ? 1.f : y + 1.f);
-      }
-      if (g.pre) g.pre[o] = v;
-      if (g.mul) v *= g.mul[o];
-      float* cp = g.C + (size_t)m * g.ldc + n;
-      *cp = g.accum ? *cp + v : v;
-    }
-  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -829,28 +748,6 @@ __global__ void __launch_bounds__(EST) k_st_embsum(Slots sl, const uint32_t* __r
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// Keras Adam (OptimizerV2 / ResourceApplyAdam): m += (g - m)(1 - b1), v += (g^2 - v)(1 - b2),
-// p -= alpha m / (sqrt(v) + eps) with alpha = lr sqrt(1 - b2^t) / (1 - b1^t).  Dense over every parameter (the sparse
-// embedding apply of OptimizerV2 decays m and v on every row too).  Clears the nonzero embedding gradient entries, so the
-// embedding part of grad is zero again for the next r4_simtrain_grad.  np parameters; the two H-row tables at emb_cat and
-// emb_seq (a net without a sequence table names its category table twice).
-// ------------------------------------------------------------------------------------------------
-__global__ void k_st_apply(int64_t np, int64_t H, int64_t emb_cat, int64_t emb_seq, float* __restrict__ prm,
-                           float* __restrict__ grad, float* __restrict__ m, float* __restrict__ v, float alpha, float b1, float b2,
-                           float eps) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= np) return;
-  const float g = grad[i];
-  float mi = m[i], vi = v[i];
-  mi += (g - mi) * (1.f - b1);
-  vi += (g * g - vi) * (1.f - b2);
-  prm[i] -= alpha * mi / (sqrtf(vi) + eps);
-  m[i] = mi; v[i] = vi;
-  const bool emb = (i >= emb_cat && i < emb_cat + H * E) || (i >= emb_seq && i < emb_seq + H * E);
-  if (emb && g != 0.f) grad[i] = 0.f;
-}
-
 // ================================================================================================
 // The other backbones: nets/dnn*.py, widedeep*.py, lstm*.py and adversarial_slate.py on the same samples, dense tower,
 // heads, GEMM, weight-gradient jobs, embedding key sort and Adam.  What a backbone adds is its embedding front (mean
@@ -1281,6 +1178,3 @@ __global__ void __launch_bounds__(NTH) k_st_loss_adv(Data D, const int64_t* __re
 
 }  // namespace r4st
 
-// Exact-K's kernels reach r4_learn.cu through this header: they run on the same Adam (k_st_apply), and the learner
-// translation unit keeps one include per learner family.
-#include "r4_exactk.cuh"

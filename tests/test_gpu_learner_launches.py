@@ -81,7 +81,7 @@ def test_gauss_ppo_launches_per_chunk():
     dev = torch.device("cuda")
     pol = _policy(dev)
     ops = GaussKernelOps(D, dev, pol.n_params)
-    n = 2500                      # one minibatch of 2500 samples: two chunks of k_gauss_rows + k_gauss_wgrad (CH = 2048)
+    n = 2500                      # one minibatch of 2500 samples: two chunks of k_gauss_rows + k_dense_wgrad (CH = 2048)
     data = _batch(pol, n, dev)
     perm = torch.randperm(n, generator=torch.Generator().manual_seed(2)).to(dev)
     chunks = lambda k: 2 * -(-k // 2048)

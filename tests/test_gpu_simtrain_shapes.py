@@ -337,7 +337,7 @@ def test_step_equals_grad_then_apply():
 def test_next_gradient_after_a_step_holds_no_stale_rows():
     """A step on a batch whose ids all lie in [1, H/2), then the gradient of a batch whose ids lie in [H/2, H) into the
     same buffer: it matches the reference at the stepped parameters, and the rows of the first batch are exactly zero
-    (k_st_apply cleared what the step wrote; the second pass writes only its own rows)."""
+    (k_keras_adam cleared what the step wrote; the second pass writes only its own rows)."""
     lib = _lib()
     H = 3000
     lo, hi = R.make_range_samples(40, H, 1, H // 2, seed=6), R.make_range_samples(40, H, H // 2, H, seed=7)

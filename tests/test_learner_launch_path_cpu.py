@@ -47,16 +47,16 @@ def test_learner_kernels_launch_only_through_the_launcher():
 
 def test_env_translation_unit_names_no_learner():
     capi = _src(os.path.join(CSRC, "r4_capi.cu"))
-    for ns in ("r4ppo::", "r4gauss::", "r4ddpg::", "r4rb::", "r4bq::", "r4st::", "r4comm::"):
+    for ns in ("r4ppo::", "r4gauss::", "r4ddpg::", "r4rb::", "r4bq::", "r4st::", "r4comm::", "r4dense::"):
         assert ns not in capi, ns
 
 
-def test_each_kernel_header_is_included_by_one_translation_unit():
+def test_each_kernel_header_including_the_shared_dense_one_is_included_by_one_translation_unit():
     sources = [f for f in os.listdir(CSRC) if f.endswith(".cu")]
     assert sorted(sources) == ["r4_capi.cu", "r4_learn.cu"]
     includes = {f: set(re.findall(r'#include "(r4_\w+\.cuh)"', _src(os.path.join(CSRC, f)))) for f in sources}
     assert includes["r4_learn.cu"] == {"r4_ppo.cuh", "r4_comm.cuh", "r4_gauss.cuh", "r4_ddpg.cuh", "r4_rainbow.cuh",
-                                       "r4_batchrl.cuh", "r4_simtrain.cuh"}
+                                       "r4_batchrl.cuh", "r4_simtrain.cuh", "r4_dense.cuh", "r4_exactk.cuh"}
     assert not includes["r4_capi.cu"] & includes["r4_learn.cu"]
 
 
