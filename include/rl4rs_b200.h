@@ -520,6 +520,101 @@ int r4_batchrl_act(int algo, int obs_dim, int action_size, const float* params, 
                    const r4_batchrl_data* data, int mode, float log_flex, int32_t* action, float* probs, float* values,
                    void* stream);
 
+/* ---- continuous-action CQL on the logged dataset (batchrl_trainer.py:61-73, 91-107 'CQL-conti'; d3rlpy 0.91 CQL as the
+ * script configures it, INTEGRATION.md section 3).  obs_dim K in 1..4096, action_dim D in 1..512, minibatch n in 1..4096,
+ * n_action_samples S in 1..64.  Flat parameter layout (H = 256):
+ * actor     w1[K,H] b1[H] w2[H,H] b2[H] w3[H,2D] b3[2D]   (output [mu | logstd], logstd clamped to [-20, 2], tanh squash)
+ * critic k  w1[K+D,H] b1[H] w2[H,H] b2[H] w3[H,1] b3[1]   (k = 0, 1; input [obs | action])
+ * then log_temp, log_alpha.  The target (r4_cqlc_target_size floats) is [critic 0 | critic 1].  The noise of a step is
+ * counter-based, keyed by (seed, step, stream, row, sample, dim) (csrc/r4_cqlconti.cuh); every pointer is caller-owned
+ * DEVICE memory.  The kernels count in r4_batchrl_launch_count. */
+typedef struct {
+  const float* obs;            /* f32[N, K] */
+  const float* action;         /* f32[N, D] */
+  const float* reward;         /* f32[N] */
+  const uint8_t* terminal;     /* u8[N] */
+  const int64_t* transitions;  /* i64[T] from r4_batchrl_transitions */
+} r4_cqlc_data;
+typedef struct {
+  float gamma, tau;            /* discount, soft target update rate */
+  float lr_actor, lr_critic, lr_temp, lr_alpha, adam_eps;   /* torch.optim.Adam per group, betas 0.9 / 0.999 */
+  float alpha_threshold, conservative_weight;
+  float reward_mean, reward_den;   /* the reward scaler r' = (r - mean) / den (0, 1: off) */
+  int n_action_samples;        /* S */
+  uint64_t seed;               /* the noise seed */
+} r4_cqlc_hyper;
+int r4_cqlc_num_params(int obs_dim, int action_dim);
+int r4_cqlc_target_size(int obs_dim, int action_dim);
+/* floats of the scratch r4_cqlc_grad / r4_cqlc_epoch need for minibatches of up to n; -1 for bad arguments */
+int64_t r4_cqlc_scratch_size(int obs_dim, int action_dim, int n_action_samples, int n);
+/* floats of the scratch r4_cqlc_act needs for n rows; -1 for bad arguments */
+int64_t r4_cqlc_act_scratch_size(int obs_dim, int action_dim, int n);
+/* The gradients of the four losses of one step (temperature, alpha, critic, actor) at the given parameters, with the noise
+ * of step `step` (>= 1), over the transitions data->transitions[idx[0..n)] -> grad f32[num_params] (each group's part from
+ * its own loss; deterministic) and stats f32[5] (may be NULL): {critic loss, actor loss, temperature loss, alpha loss,
+ * mean Q_0(s, a)}.  Nothing is updated.  54 launches. */
+int r4_cqlc_grad(int obs_dim, int action_dim, const float* params, const float* target, const r4_cqlc_data* data,
+                 const r4_cqlc_hyper* hp, const int64_t* idx, int n, int step, float* scratch, float* grad, float* stats,
+                 void* stream);
+/* One epoch of d3rlpy's RoundIterator with no host round trip: minibatch k is perm[k mb .. (k + 1) mb) for k < n_perm / mb;
+ * each is one SGD step at step step0 + k + 1: temperature, alpha, critic and actor updates in that order (each phase sees
+ * the parameters the earlier ones left), Adam per group, the soft target update after the critic's Adam.  stats (may be
+ * NULL) receives f32[steps, 5].  56 launches per step.  Returns the number of steps, or an r4_status. */
+int r4_cqlc_epoch(int obs_dim, int action_dim, float* params, float* target, float* m, float* v, const r4_cqlc_data* data,
+                  const r4_cqlc_hyper* hp, const int64_t* perm, int64_t n_perm, int mb, int step0, float* scratch,
+                  float* stats, void* stream);
+/* predict on n observations (n <= 2^20; obs_f64 != 0: f64[n, K], as the env's 'torch' output; else f32[n, K]): action f32[n, D]
+ * (may be NULL) = tanh(mu); q f32[n] (may be NULL) = the mean of the two critics at (obs, action_in) (action_in f32[n, D],
+ * or NULL for the predicted action).  At least one of action, q.  5 launches (12 with q). */
+int r4_cqlc_act(int obs_dim, int action_dim, const float* params, const void* obs, int obs_f64, int n,
+                const float* action_in, float* action, float* q, float* scratch, void* stream);
+
+/* ---- continuous-action BCQ on the logged dataset (batchrl_trainer.py:61-73, 91-107 'BCQ-conti'; d3rlpy 0.91 BCQ as the
+ * script configures it, INTEGRATION.md section 3).  obs_dim K in 1..4096, action_dim D in 1..512, latent_size L in 1..512,
+ * minibatch n in 1..4096, n_action_samples S in 1..256 (n S <= 2^20 for r4_bcqc_act).  Flat parameter layout (H = 256;
+ * each net w1[in,H] b1[H] w2[H,H] b2[H] w3[H,out] b3[out]): actor (K+D -> D; pi = clamp(a + flex tanh(f), -1, 1)) |
+ * critic 0 (K+D -> 1) | critic 1 | VAE encoder (K+D -> [mu | logstd] 2L, logstd clamped to [-20, 2]) | VAE decoder
+ * (K+L -> D, tanh).  The target (r4_bcqc_target_size floats) is [actor | critic 0 | critic 1], the first floats of the
+ * layout.  The data is r4_cqlc_data; the kernels count in r4_batchrl_launch_count. */
+typedef struct {
+  float gamma, tau;            /* discount, soft target update rate */
+  float lr_actor, lr_critic, lr_imitator, adam_eps;   /* torch.optim.Adam per group, betas 0.9 / 0.999 */
+  float lam;                   /* the target's mix lam min_k + (1 - lam) max_k */
+  float beta;                  /* the VAE's KL weight */
+  float action_flexibility;    /* the actor's residual scale */
+  float reward_mean, reward_den;   /* the reward scaler r' = (r - mean) / den (0, 1: off) */
+  int n_action_samples;        /* S */
+  int latent_size;             /* L */
+  uint64_t seed;               /* the noise seed */
+} r4_bcqc_hyper;
+int r4_bcqc_num_params(int obs_dim, int action_dim, int latent_size);
+int r4_bcqc_target_size(int obs_dim, int action_dim, int latent_size);
+/* floats of the scratch r4_bcqc_grad / r4_bcqc_epoch need for minibatches of up to n; -1 for bad arguments */
+int64_t r4_bcqc_scratch_size(int obs_dim, int action_dim, int latent_size, int n_action_samples, int n);
+/* floats of the scratch r4_bcqc_act needs for n rows; -1 for bad arguments */
+int64_t r4_bcqc_act_scratch_size(int obs_dim, int action_dim, int latent_size, int n_action_samples, int n);
+/* The gradients of the three losses of one step (imitator, critic, actor) at the given parameters, with the noise of step
+ * `step` (>= 1), over data->transitions[idx[0..n)] -> grad f32[num_params] (each group's part from its own loss) and stats
+ * f32[5] (may be NULL): {imitator loss, critic loss, actor loss, mean Q_0(s, a), VAE reconstruction mse}.  Nothing is
+ * updated.  66 launches. */
+int r4_bcqc_grad(int obs_dim, int action_dim, const float* params, const float* target, const r4_cqlc_data* data,
+                 const r4_bcqc_hyper* hp, const int64_t* idx, int n, int step, float* scratch, float* grad, float* stats,
+                 void* stream);
+/* One epoch of d3rlpy's RoundIterator with no host round trip (as r4_cqlc_epoch): each minibatch is one SGD step at step
+ * step0 + k + 1: imitator, critic and actor updates in that order, Adam per group, the soft target update of the critics
+ * after their Adam and of the actor after its Adam.  stats (may be NULL) receives f32[steps, 5].  69 launches per step.
+ * Returns the number of steps, or an r4_status. */
+int r4_bcqc_epoch(int obs_dim, int action_dim, float* params, float* target, float* m, float* v, const r4_cqlc_data* data,
+                  const r4_bcqc_hyper* hp, const int64_t* perm, int64_t n_perm, int mb, int step0, float* scratch,
+                  float* stats, void* stream);
+/* predict on n observations (obs_f64 != 0: f64[n, K], else f32[n, K]): action f32[n, D] (may be NULL) = the candidate with
+ * the largest Q_0 among S decoded, perturbed actions (latent draws keyed by (hp->seed, counter)); q f32[n] (may be NULL)
+ * = the mean of the two critics at (obs, action_in), or at the predicted action when action_in is NULL.  Needs action, or
+ * q with action_in.  13 launches for the action, 8 for q. */
+int r4_bcqc_act(int obs_dim, int action_dim, const float* params, const void* obs, int obs_f64, int n,
+                const r4_bcqc_hyper* hp, uint64_t counter, const float* action_in, float* action, float* q, float* scratch,
+                void* stream);
+
 /* ---- the simulator alone (nets/dien.py:8-45), for parity tests and kernel benchmarks ------- */
 /* seq i32[R,2,64], dense f32[R,432], cat i32[R,21] (device) -> obs f32[R,256], probs f32[R,2]
  * (either may be NULL).  Runs the uncached path: GRU-1 is recomputed for every row. */

@@ -42,6 +42,22 @@ class BatchRLHyper(C.Structure):
     _fields_ = [(n, C.c_float) for n in ("gamma", "beta", "alpha", "log_flex", "reward_mean", "reward_den")]
 
 
+class CQLContiData(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("obs", "action", "reward", "terminal", "transitions")]
+
+
+class CQLContiHyper(C.Structure):
+    _fields_ = [(n, C.c_float) for n in ("gamma", "tau", "lr_actor", "lr_critic", "lr_temp", "lr_alpha", "adam_eps",
+                                         "alpha_threshold", "conservative_weight", "reward_mean", "reward_den")] + \
+        [("n_action_samples", C.c_int), ("seed", C.c_uint64)]
+
+
+class BCQContiHyper(C.Structure):
+    _fields_ = [(n, C.c_float) for n in ("gamma", "tau", "lr_actor", "lr_critic", "lr_imitator", "adam_eps", "lam", "beta",
+                                         "action_flexibility", "reward_mean", "reward_den")] + \
+        [("n_action_samples", C.c_int), ("latent_size", C.c_int), ("seed", C.c_uint64)]
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     "r4_create": (C.c_int, [C.POINTER(R4Config), C.c_int, C.POINTER(C.c_void_p)]),
@@ -141,6 +157,25 @@ EXPORTS = {
     "r4_batchrl_launch_count": (C.c_int64, []),
     "r4_batchrl_act": (C.c_int, [C.c_int] * 3 + [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(BatchRLData), C.c_int,
                                                   C.c_float] + [C.c_void_p] * 4),
+    "r4_cqlc_num_params": (C.c_int, [C.c_int] * 2),
+    "r4_cqlc_target_size": (C.c_int, [C.c_int] * 2),
+    "r4_cqlc_scratch_size": (C.c_int64, [C.c_int] * 4),
+    "r4_cqlc_act_scratch_size": (C.c_int64, [C.c_int] * 3),
+    "r4_cqlc_grad": (C.c_int, [C.c_int] * 2 + [C.c_void_p] * 2 + [C.POINTER(CQLContiData), C.POINTER(CQLContiHyper),
+                                                                C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 4),
+    "r4_cqlc_epoch": (C.c_int, [C.c_int] * 2 + [C.c_void_p] * 4 + [C.POINTER(CQLContiData), C.POINTER(CQLContiHyper),
+                                                                 C.c_void_p, C.c_int64, C.c_int, C.c_int] + [C.c_void_p] * 3),
+    "r4_cqlc_act": (C.c_int, [C.c_int] * 2 + [C.c_void_p] * 2 + [C.c_int, C.c_int] + [C.c_void_p] * 5),
+    "r4_bcqc_num_params": (C.c_int, [C.c_int] * 3),
+    "r4_bcqc_target_size": (C.c_int, [C.c_int] * 3),
+    "r4_bcqc_scratch_size": (C.c_int64, [C.c_int] * 5),
+    "r4_bcqc_act_scratch_size": (C.c_int64, [C.c_int] * 5),
+    "r4_bcqc_grad": (C.c_int, [C.c_int] * 2 + [C.c_void_p] * 2 + [C.POINTER(CQLContiData), C.POINTER(BCQContiHyper),
+                                                                C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 4),
+    "r4_bcqc_epoch": (C.c_int, [C.c_int] * 2 + [C.c_void_p] * 4 + [C.POINTER(CQLContiData), C.POINTER(BCQContiHyper),
+                                                                 C.c_void_p, C.c_int64, C.c_int, C.c_int] + [C.c_void_p] * 3),
+    "r4_bcqc_act": (C.c_int, [C.c_int] * 2 + [C.c_void_p] * 2 + [C.c_int, C.c_int, C.POINTER(BCQContiHyper), C.c_uint64] +
+                    [C.c_void_p] * 5),
     "r4_adam_step": (C.c_int,[C.c_void_p] * 4 + [C.c_int, C.c_int] + [C.c_float] * 6 + [C.c_void_p, C.c_void_p]),
     "r4_dien_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "r4_simtrain_num_params": (C.c_int64, [C.c_int]),

@@ -15,6 +15,10 @@ On a CUDA device the dataset is uploaded once and stays there; an epoch is one d
 r4_batchrl_act.  On the CPU the torch twin (policy.BatchRLNet) runs the same algorithm.  The d3rlpy 0.91 semantics
 restated here are listed in INTEGRATION.md section 3 as not verified (d3rlpy is not in this
 project's environment).
+
+'BCQ-conti' (ContinuousBCQ) and 'CQL-conti' (ContinuousCQL) train on the continuous dataset (data_generate_rl4rs_a_conti /
+_b_conti) for a config with support_conti_env: r4_bcqc_epoch / r4_cqlc_epoch on CUDA (csrc/r4_bcqconti.cuh,
+csrc/r4_cqlconti.cuh), policy.BatchRLContiBCQNet / BatchRLContiNet on the CPU, r4_bcqc_act / r4_cqlc_act to act.
 """
 import ctypes as C
 import math
@@ -24,16 +28,16 @@ import torch
 
 from . import _capi
 from ._capi import ptr
-from .policy import BatchRLNet
+from .policy import BatchRLContiBCQNet, BatchRLContiNet, BatchRLNet
 
 ALGOS = {"BC": 0, "BCQ": 1, "CQL": 2}
 NOT_BUILT = {
     "dynamics": "the ProbabilisticEnsembleDynamics model",
-    "BCQ-conti": "continuous-action BCQ",
-    "CQL-conti": "continuous-action CQL",
     "MOPO": "MOPO (needs the dynamics model)",
     "COMBO": "COMBO (needs the dynamics model)",
 }
+# the continuous learners exist for the continuous dataset only: the script sets support_conti_env for them
+CONTI_ONLY = {"BCQ-conti": "continuous-action BCQ", "CQL-conti": "continuous-action CQL"}
 # d3rlpy 0.91 defaults as batchrl_trainer.py:34-90 leaves or sets them (INTEGRATION.md section 3, not verified)
 DEFAULTS = {
     "BC": {"batch_size": 256, "learning_rate": 1e-3, "eps": 1e-8, "beta": 0.0},
@@ -41,14 +45,31 @@ DEFAULTS = {
             "action_flexibility": 0.3, "target_update_interval": 8000},
     "CQL": {"batch_size": 256, "learning_rate": 6.25e-5, "eps": 1e-8, "gamma": 1.0, "alpha": 1.0,
             "target_update_interval": 8000, "reward_scaler": "standard"},
+    # d3rlpy 0.91 BCQ (continuous) with batchrl_trainer.py:61-73's batch size (INTEGRATION.md section 3, not verified)
+    "BCQ-conti": {"batch_size": 256, "actor_learning_rate": 1e-3, "critic_learning_rate": 1e-3,
+                  "imitator_learning_rate": 1e-3, "eps": 1e-8, "gamma": 0.99, "tau": 0.005, "lam": 0.75,
+                  "n_action_samples": 100, "action_flexibility": 0.05, "latent_size": 32, "beta": 0.5,
+                  "update_actor_interval": 1, "rl_start_epoch": 0, "reward_scaler": None},
+    # d3rlpy 0.91 CQL (continuous) with batchrl_trainer.py:61-73's batch size, gamma and reward scaler
+    "CQL-conti": {"batch_size": 256, "actor_learning_rate": 1e-4, "critic_learning_rate": 3e-4,
+                  "temp_learning_rate": 1e-4, "alpha_learning_rate": 1e-4, "eps": 1e-8, "gamma": 1.0, "tau": 0.005,
+                  "initial_temperature": 1.0, "initial_alpha": 1.0, "alpha_threshold": 10.0, "conservative_weight": 5.0,
+                  "n_action_samples": 10, "soft_q_backup": False, "reward_scaler": "standard"},
 }
 
 
 def get_model(config, algo, dynamics=None):
-    """batchrl_trainer.get_model: 'BC', 'BCQ' or 'CQL' (alpha = config['CQL_alpha']).  The other names of the reference raise
-    NotImplementedError; any other name fails its assert."""
+    """batchrl_trainer.get_model: 'BC', 'BCQ' or 'CQL' (alpha = config['CQL_alpha']), and 'CQL-conti' for a config with
+    support_conti_env (the script sets it for the conti names).  CQL-conti ignores CQL_alpha, as d3rlpy 0.91's continuous
+    CQL drops the unknown `alpha` argument: its initial alpha is 1.0 (INTEGRATION.md section 3).  The other names of the
+    reference raise NotImplementedError; any other name fails its assert."""
     if algo in NOT_BUILT:
         raise NotImplementedError("%s: %s is not built in this project" % (algo, NOT_BUILT[algo]))
+    if algo in CONTI_ONLY:
+        if not config.get("support_conti_env", False):
+            raise NotImplementedError("%s: %s is built for a support_conti_env config only (the continuous dataset of "
+                                      "data_generate_rl4rs_a_conti / _b_conti)" % (algo, CONTI_ONLY[algo]))
+        return {"BCQ-conti": ContinuousBCQ, "CQL-conti": ContinuousCQL}[algo](config)
     assert algo in ("BC", "BCQ", "CQL", "MOPO", "COMBO")
     cls = {"BC": DiscreteBC, "BCQ": DiscreteBCQ, "CQL": DiscreteCQL}[algo]
     extra = {"alpha": float(config["CQL_alpha"])} if algo == "CQL" and "CQL_alpha" in config else {}
@@ -362,6 +383,347 @@ class DiscreteCQL(BatchRLModel):
     algo = "CQL"
 
 
+class ContiDeviceDataset(object):
+    """The continuous dataset where the learner runs: obs f32 [N, K], action f32 [N, D] (the logged items' embeddings,
+    not clipped), reward f32 [N], terminal u8 [N] and the transition entries i64 [T] (r4_batchrl_transitions).  On CUDA
+    it is uploaded once; a dataset that does not fit raises MemoryError."""
+
+    def __init__(self, dataset, device):
+        obs = np.asarray(dataset["observations"], dtype=np.float32)
+        N = obs.shape[0]
+        act = np.asarray(dataset["actions"], dtype=np.float32)
+        discrete = np.asarray(dataset.get("discrete_action", act.ndim < 2 or act.shape[1] == 1)).item()
+        if discrete or act.ndim != 2 or act.shape[0] != N:
+            raise ValueError("continuous batch RL needs the continuous dataset (actions f32 [N, D], discrete_action "
+                             "False): data_generate_rl4rs_a_conti / _b_conti")
+        self.device, self.N, self.K, self.D = torch.device(device), N, obs.shape[1], act.shape[1]
+        need = N * (self.K * 4 + self.D * 4 + 4 + 1 + 8)
+        if self.device.type == "cuda":
+            free = torch.cuda.mem_get_info(self.device)[0]
+            if need > free:
+                raise MemoryError("the dataset needs %d bytes on %s, %d are free" % (need, self.device, free))
+        try:
+            self.obs = torch.from_numpy(obs).to(self.device)
+            self.action = torch.from_numpy(act).to(self.device)
+            self.reward = torch.from_numpy(np.asarray(dataset["rewards"], dtype=np.float32).reshape(N)).to(self.device)
+            self.terminal = torch.from_numpy((np.asarray(dataset["terminals"]).reshape(N) != 0).astype(np.uint8)).to(self.device)
+            if self.device.type == "cuda":
+                lib = _capi.load_library()
+                index = torch.empty(N, dtype=torch.int64, device=self.device)
+                count = torch.zeros(1, dtype=torch.int64, device=self.device)
+                rc = lib.r4_batchrl_transitions(ptr(self.terminal), N, ptr(index), ptr(count), _capi.stream(self.device))
+                _capi.check(lib, None, rc, "r4_batchrl_transitions")
+                self.transitions = index[:int(count)]
+            else:
+                self.transitions = transitions_host(self.terminal)
+        except torch.OutOfMemoryError as exc:
+            raise MemoryError("the dataset needs %d bytes on %s: %s" % (need, self.device, exc)) from exc
+        self.n = int(self.transitions.numel())
+
+    batch = DeviceDataset.batch
+
+    def c_data(self):
+        return _capi.CQLContiData(self.obs.data_ptr(), self.action.data_ptr(), self.reward.data_ptr(),
+                                  self.terminal.data_ptr(), self.transitions.data_ptr())
+
+
+class ContinuousCQL(object):
+    """d3rlpy 0.91 CQL (continuous actions) as batchrl_trainer.py:61-73 configures 'CQL-conti', with d3rlpy AlgoBase's
+    surface the scripts call, over policy.BatchRLContiNet (CPU) or the r4_cqlc_* kernels (CUDA).  One SGD step updates the
+    temperature, alpha, the critics and the actor in that order, each with its own Adam, then the critics' soft target.
+    The noise of step t is keyed by (seed, t) (policy.cqlc_draws), so the CPU and CUDA paths draw the same numbers."""
+
+    algo = "CQL-conti"
+    PREFIX = "r4_cqlc"
+    STAT_NAMES = ("critic_loss", "actor_loss", "temp_loss", "alpha_loss", "q")
+    # (loss, learning-rate key, its stats slots), in update order; the soft target update follows SOFT_AFTER's update
+    PHASES = (("temp", "temp_learning_rate", (2,)), ("alpha", "alpha_learning_rate", (3,)),
+              ("critic", "critic_learning_rate", (0, 4)), ("actor", "actor_learning_rate", (1,)))
+    SOFT_AFTER = "critic"
+
+    def __init__(self, config, device=None, seed=0, use_kernels=None, **overrides):
+        self.config = dict(config)
+        self.hp = dict(DEFAULTS[self.algo], **overrides)
+        if self.hp.get("soft_q_backup"):
+            raise NotImplementedError("CQL-conti: soft_q_backup is not built (the script leaves it False)")
+        self.batch_size = int(self.hp["batch_size"])
+        if device is None:
+            device = "cuda" if torch.cuda.is_available() and config.get("gpu", True) else "cpu"
+        self.device = torch.device(device)
+        self.use_kernels = (self.device.type == "cuda") if use_kernels is None else bool(use_kernels)
+        onehot = config.get("support_onehot_action", False)
+        self.D = int(config.get("action_size", 284)) if onehot else int(config.get("action_emb_size", 32))
+        self.seed = seed
+        self.net = None
+        self.reward_mean, self.reward_std = 0.0, 1.0
+        self.reward_scaler = None
+        self._data, self._data_src = None, None
+        self.step = 0
+        self.act_counter = 0
+
+    fit_reward_scaler = BatchRLModel.fit_reward_scaler
+
+    def _new_net(self, obs_dim):
+        hp = self.hp
+        return BatchRLContiNet(obs_dim, self.D, self.device, self.seed, hp["initial_temperature"], hp["initial_alpha"])
+
+    def _dims(self, K):
+        """The leading shape arguments of the r4_*_num_params / _target_size / _scratch_size calls."""
+        return (K, self.D)
+
+    def create_impl(self, obs_dim):
+        hp = self.hp
+        self.net = self._new_net(obs_dim)
+        z = lambda: torch.zeros(self.net.n_params, dtype=torch.float32, device=self.device)
+        self.m, self.v = z(), z()
+        self.step = 0
+        self._gen = torch.Generator(device=self.device).manual_seed(self.seed)
+        if self.use_kernels:
+            self.lib = _capi.load_library()
+            K, D, dims = obs_dim, self.D, self._dims(obs_dim)
+            if getattr(self.lib, self.PREFIX + "_num_params")(*dims) != self.net.n_params:
+                raise ValueError("obs_dim %d / action_dim %d is outside the kernels' range" % (K, D))
+            assert getattr(self.lib, self.PREFIX + "_target_size")(*dims) == self.net.n_target
+            self.grad = z()
+            self.stats = torch.zeros(5, dtype=torch.float32, device=self.device)
+            n = getattr(self.lib, self.PREFIX + "_scratch_size")(*dims, int(hp["n_action_samples"]), self.batch_size)
+            if n < 0:
+                raise ValueError("batch_size %d / n_action_samples %d is outside the kernels' range"
+                                 % (self.batch_size, hp["n_action_samples"]))
+            self.scratch = torch.zeros(n, dtype=torch.float32, device=self.device)
+
+    def build_with_dataset(self, dataset):
+        obs, act = dataset["observations"], np.asarray(dataset["actions"])
+        if act.ndim != 2 or act.shape[1] != self.D:
+            raise ValueError("the dataset's actions have shape %s, the model takes [N, %d] (action_emb_size, or "
+                             "action_size with support_onehot_action)" % (act.shape, self.D))
+        if self.net is None or self.net.K != obs.shape[1]:
+            self.create_impl(obs.shape[1])
+        if self.hp.get("reward_scaler") == "standard":
+            self.fit_reward_scaler(dataset)
+
+    def _hyper(self):
+        hp = self.hp
+        return {"gamma": float(hp["gamma"]), "tau": float(hp["tau"]), "alpha_threshold": float(hp["alpha_threshold"]),
+                "conservative_weight": float(hp["conservative_weight"]),
+                "reward_mean": self.reward_mean if self.reward_scaler else 0.0,
+                "reward_den": (self.reward_std + 1e-3) if self.reward_scaler else 1.0}
+
+    def _hyper_c(self):
+        h, hp = self._hyper(), self.hp
+        return _capi.CQLContiHyper(h["gamma"], h["tau"], hp["actor_learning_rate"], hp["critic_learning_rate"],
+                                   hp["temp_learning_rate"], hp["alpha_learning_rate"], hp["eps"], h["alpha_threshold"],
+                                   h["conservative_weight"], h["reward_mean"], h["reward_den"], int(hp["n_action_samples"]),
+                                   self.seed)
+
+    # ---- training ------------------------------------------------------------------------------------
+    def _device_data(self, dataset):
+        if self._data_src is not dataset:
+            self._data = None
+            self._data = ContiDeviceDataset(dataset, self.device)
+            self._data_src = dataset
+        return self._data
+
+    def fit(self, dataset, n_epochs=1, eval_episodes=None, show_progress=False, **kwargs):
+        """d3rlpy fit with its RoundIterator (one device permutation per epoch, floor(n / batch_size) minibatches).
+        eval_episodes is accepted and not scored.  The reward scaler as in the discrete models.  Returns
+        [(epoch, {STAT_NAMES: the epoch's means})]."""
+        data = self._device_data(dataset)
+        if data.D != self.D:
+            raise ValueError("the dataset's actions have %d dims, the model %d" % (data.D, self.D))
+        if self.net is None or self.net.K != data.K:
+            self.build_with_dataset(dataset)
+        elif self.hp.get("reward_scaler") == "standard" and self.reward_scaler is None:
+            self.fit_reward_scaler(dataset)
+        mb = self.batch_size
+        if data.n < mb:
+            raise ValueError("the dataset has %d transitions, fewer than one minibatch of %d" % (data.n, mb))
+        names = self.STAT_NAMES
+        out = []
+        for epoch in range(1, int(n_epochs) + 1):
+            perm = torch.randperm(data.n, generator=self._gen, device=self.device)
+            st = self._epoch_kernels(data, perm) if self.use_kernels else self._epoch_twin(data, perm)
+            out.append((epoch, dict(zip(names, st))))
+            if show_progress:
+                print("epoch %d %s" % (epoch, out[-1][1]))
+        return out
+
+    def _epoch_twin(self, data, perm):
+        mb, steps = self.batch_size, data.n // self.batch_size
+        acc = torch.zeros(5, dtype=torch.float64)
+        for k in range(steps):
+            acc += self.train_step_twin(data.batch(perm[k * mb:(k + 1) * mb])).double().cpu()
+        return [float(v) for v in acc / max(steps, 1)]
+
+    def train_step_twin(self, batch):
+        """One SGD step of the twin with the kernels' noise: the PHASES' updates in order (each loss at the parameters the
+        earlier updates left), the soft target update after SOFT_AFTER's.  -> stats [5]."""
+        net, hp, h = self.net, self.hp, self._hyper()
+        self.step += 1
+        noise = net.noise(self.seed, self.step, batch[0].shape[0], int(hp["n_action_samples"]))
+        st = torch.zeros(5, dtype=torch.float32, device=self.device)
+        for name, lr, slots in self.PHASES:
+            losses, s = net.losses(batch, noise, h)
+            g = torch.autograd.grad(losses[name], net.flat)[0]
+            sl = net.group(name)
+            for k in slots:
+                st[k] = s[k]
+            adam_(net.flat.data[sl], g[sl], self.m[sl], self.v[sl], self.step, hp[lr], hp["eps"])
+            if name == self.SOFT_AFTER:
+                net.soft_update(hp["tau"])
+        self._last_stats = st
+        return st
+
+    def _epoch_kernels(self, data, perm):
+        mb = self.batch_size
+        steps = data.n // mb
+        stats = torch.zeros(steps * 5, dtype=torch.float32, device=self.device)
+        rc = getattr(self.lib, self.PREFIX + "_epoch")(self.net.K, self.D, ptr(self.net.flat), ptr(self.net.target), ptr(self.m),
+                                    ptr(self.v), C.byref(data.c_data()), C.byref(self._hyper_c()), ptr(perm),
+                                    perm.numel(), mb, self.step, ptr(self.scratch), ptr(stats), _capi.stream(self.device))
+        if rc < 0:
+            _capi.check(self.lib, None, rc, self.PREFIX + "_epoch")
+        self.step += rc
+        return [float(v) for v in stats.view(steps, 5).double().mean(0)]
+
+    def grad_kernels(self, data, pos, step=None):
+        """r4_cqlc_grad / r4_bcqc_grad over the transitions at positions pos (i64, device) with the noise of `step`
+        (default: the next step) -> self.grad, self.stats."""
+        rc = getattr(self.lib, self.PREFIX + "_grad")(self.net.K, self.D, ptr(self.net.flat), ptr(self.net.target), C.byref(data.c_data()),
+                                   C.byref(self._hyper_c()), ptr(pos), pos.numel(), self.step + 1 if step is None else step,
+                                   ptr(self.scratch), ptr(self.grad), ptr(self.stats), _capi.stream(self.device))
+        _capi.check(self.lib, None, rc, self.PREFIX + "_grad")
+
+    # ---- acting --------------------------------------------------------------------------------------
+    def _act_inputs(self, obs, action):
+        x = torch.as_tensor(obs, device=self.device)
+        if x.dtype not in (torch.float32, torch.float64):
+            x = x.to(torch.float32)
+        x = x.reshape(-1, self.net.K).contiguous()
+        a_in = None if action is None else torch.as_tensor(np.asarray(action) if not torch.is_tensor(action) else action,
+                                                             device=self.device, dtype=torch.float32).reshape(-1, self.D)
+        return x, None if a_in is None else a_in.contiguous()
+
+    def act(self, obs, action=None, want_q=False):
+        """tanh(mu) [n, D] and (want_q) the critics' mean at (obs, action or tanh mu) [n], as device tensors; obs numpy
+        or torch, f32 or f64 [n, K]."""
+        x, a_in = self._act_inputs(obs, action)
+        if not self.use_kernels:
+            with torch.no_grad():
+                a = self.net.predict(x.to(torch.float32))
+                q = self.net.predict_value(x.to(torch.float32), a if a_in is None else a_in) if want_q else None
+            return a, q
+        n = x.shape[0]
+        a = torch.empty(n, self.D, dtype=torch.float32, device=self.device)
+        q = torch.empty(n, dtype=torch.float32, device=self.device) if want_q else None
+        scratch = torch.empty(self.lib.r4_cqlc_act_scratch_size(self.net.K, self.D, n), dtype=torch.float32,
+                              device=self.device)
+        rc = self.lib.r4_cqlc_act(self.net.K, self.D, ptr(self.net.flat), ptr(x), int(x.dtype == torch.float64), n,
+                                  ptr(a_in), ptr(a), ptr(q), ptr(scratch), _capi.stream(self.device))
+        _capi.check(self.lib, None, rc, "r4_cqlc_act")
+        return a, q
+
+    def predict(self, x):
+        """d3rlpy predict: tanh(mu) -> f32 numpy [n, D]."""
+        return self.act(x)[0].cpu().numpy()
+
+    def predict_value(self, x, action):
+        """d3rlpy predict_value: the mean of the two critics' Q(s, a), in the scaled reward units -> numpy [n]."""
+        return self.act(x, action, want_q=True)[1].cpu().numpy()
+
+    # ---- checkpoints ---------------------------------------------------------------------------------
+    def save_model(self, fname):
+        """torch.save of every network (the flat vector: CQL's actor, critics, log_temp and log_alpha; BCQ's actor, critics
+        and VAE), the targets, the Adam moments, the step and act counters, the epoch-permutation generator's state and
+        the reward scaler, so a loaded model predicts and continues fit as the saved one would."""
+        torch.save({"algo": self.algo, "obs_dim": self.net.K, "action_dim": self.D, "params": self.net.flat.detach().cpu(),
+                    "target": self.net.target.cpu(), "m": self.m.cpu(), "v": self.v.cpu(), "step": self.step,
+                    "act_counter": self.act_counter, "gen": self._gen.get_state(),
+                    "reward_scaler": self.reward_scaler, "reward_mean": self.reward_mean, "reward_std": self.reward_std},
+                   fname)
+
+    def load_model(self, fname):
+        ck = torch.load(fname, map_location="cpu")
+        if ck["algo"] != self.algo or ck["action_dim"] != self.D:
+            raise ValueError("%s holds a %s model for %d action dims" % (fname, ck["algo"], ck.get("action_dim", -1)))
+        if self.net is None or self.net.K != ck["obs_dim"]:
+            self.create_impl(ck["obs_dim"])
+        with torch.no_grad():
+            for dst, key in ((self.net.flat, "params"), (self.net.target, "target"), (self.m, "m"), (self.v, "v")):
+                dst.copy_(ck[key].to(self.device))
+        self.step, self.act_counter = int(ck["step"]), int(ck["act_counter"])
+        self._gen.set_state(ck["gen"])
+        self.reward_scaler, self.reward_mean, self.reward_std = ck["reward_scaler"], ck["reward_mean"], ck["reward_std"]
+
+
+class ContinuousBCQ(ContinuousCQL):
+    """d3rlpy 0.91 BCQ (continuous actions) as batchrl_trainer.py:61-73 configures 'BCQ-conti', over
+    policy.BatchRLContiBCQNet (CPU) or the r4_bcqc_* kernels (CUDA).  One SGD step updates the VAE imitator, the critics
+    and the actor in that order, each with its own Adam, then the soft update of the actor and critic targets.  predict is
+    stochastic: each call draws its latents from (seed, the call counter)."""
+
+    algo = "BCQ-conti"
+    PREFIX = "r4_bcqc"
+    STAT_NAMES = ("imitator_loss", "critic_loss", "actor_loss", "q", "reconstruction")
+    PHASES = (("imitator", "imitator_learning_rate", (0, 4)), ("critic", "critic_learning_rate", (1, 3)),
+              ("actor", "actor_learning_rate", (2,)))
+    SOFT_AFTER = "actor"
+
+    def __init__(self, config, **kw):
+        super(ContinuousBCQ, self).__init__(config, **kw)
+        if int(self.hp["update_actor_interval"]) != 1 or int(self.hp["rl_start_epoch"]) != 0:
+            raise NotImplementedError("BCQ-conti: update_actor_interval != 1 and rl_start_epoch != 0 are not built (the "
+                                      "script leaves them at 1 and 0)")
+
+    def _new_net(self, obs_dim):
+        return BatchRLContiBCQNet(obs_dim, self.D, self.device, self.seed, int(self.hp["latent_size"]))
+
+    def _dims(self, K):
+        return (K, self.D, int(self.hp["latent_size"]))
+
+    def _hyper(self):
+        hp = self.hp
+        return {"gamma": float(hp["gamma"]), "tau": float(hp["tau"]), "lam": float(hp["lam"]), "beta": float(hp["beta"]),
+                "action_flexibility": float(hp["action_flexibility"]),
+                "reward_mean": self.reward_mean if self.reward_scaler else 0.0,
+                "reward_den": (self.reward_std + 1e-3) if self.reward_scaler else 1.0}
+
+    def _hyper_c(self):
+        h, hp = self._hyper(), self.hp
+        return _capi.BCQContiHyper(h["gamma"], h["tau"], hp["actor_learning_rate"], hp["critic_learning_rate"],
+                                   hp["imitator_learning_rate"], hp["eps"], h["lam"], h["beta"], h["action_flexibility"],
+                                   h["reward_mean"], h["reward_den"], int(hp["n_action_samples"]), int(hp["latent_size"]),
+                                   self.seed)
+
+    def act(self, obs, action=None, want_q=False):
+        """The best of n_action_samples decoded, perturbed candidates by Q_0 [n, D] (when action is None) and (want_q)
+        the critics' mean at (obs, action or that prediction) [n], as device tensors."""
+        x, a_in = self._act_inputs(obs, action)
+        n, S = x.shape[0], int(self.hp["n_action_samples"])
+        a = None
+        if a_in is None:
+            self.act_counter += 1
+        if not self.use_kernels:
+            with torch.no_grad():
+                x32 = x.to(torch.float32)
+                if a_in is None:
+                    z = self.net.predict_noise(self.seed, self.act_counter, n, S)
+                    a = self.net.predict(x32, z, self._hyper())
+                q = self.net.predict_value(x32, a if a_in is None else a_in) if want_q else None
+            return a, q
+        a = torch.empty(n, self.D, dtype=torch.float32, device=self.device) if a_in is None else None
+        q = torch.empty(n, dtype=torch.float32, device=self.device) if want_q else None
+        size = self.lib.r4_bcqc_act_scratch_size(self.net.K, self.D, int(self.hp["latent_size"]), S, n)
+        if size < 0:
+            raise ValueError("predict on %d rows x %d samples is outside the kernels' range" % (n, S))
+        scratch = torch.empty(size, dtype=torch.float32, device=self.device)
+        rc = self.lib.r4_bcqc_act(self.net.K, self.D, ptr(self.net.flat), ptr(x), int(x.dtype == torch.float64), n,
+                                  C.byref(self._hyper_c()), self.act_counter, ptr(a_in), ptr(a), ptr(q), ptr(scratch),
+                                  _capi.stream(self.device))
+        _capi.check(self.lib, None, rc, "r4_bcqc_act")
+        return a, q
+
+
 class BatchRLDataPtrs(object):
     """The r4_batchrl_data structure: the device dataset's planes and the net's masking tables."""
 
@@ -403,8 +765,12 @@ class policy_model(object):
 
     def predict_with_mask(self, obs):
         """policy_model.py:17-36: action_probs, -2^15 where the location layer, the prev actions or the special-item rule
-        exclude an item, the first argmax.  A device tensor in gives a device tensor out, else a numpy array."""
+        exclude an item, the first argmax.  A device tensor in gives a device tensor out, else a numpy array.  Under
+        support_conti_env it is predict (policy_model.py:18-19); a continuous model then returns device actions
+        f32 [n, D] for a device tensor."""
         if self.config.get("support_conti_env", False):
+            if hasattr(obs, "is_cuda") and isinstance(self.policy, ContinuousCQL):     # ContinuousBCQ too
+                return self.policy.act(obs)[0]
             return self.predict(obs)
         a = self.policy.act(obs, 0)[0]
         return a if hasattr(obs, "is_cuda") else a.long().cpu().numpy()

@@ -533,3 +533,6 @@ __global__ void __launch_bounds__(TRT) k_bq_transitions(const uint8_t* __restric
 }
 
 }  // namespace r4bq
+
+#include "r4_cqlconti.cuh"   // continuous-action CQL, on the same dataset planes and launch family
+#include "r4_bcqconti.cuh"   // continuous-action BCQ, likewise

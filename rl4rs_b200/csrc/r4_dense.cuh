@@ -19,14 +19,15 @@ __device__ __forceinline__ float elu(float x) { return x > 0.f ? x : expm1f(x); 
 // C by z cso.  The epilogue, in this order:
 //   v = alpha acc;  v += bias[n] (bias may be NULL);  then by epi
 //     EP_LIN  v        EP_RELU  max(v, 0)     EP_SIG  sigmoid(v)     EP_ELU  elu(v)
-//     EP_DSIG v y (1 - y)      EP_DELU  v (y > 0 ? 1 : y + 1)        (y = aux[m][n], the forward activation);
+//     EP_DSIG v y (1 - y)      EP_DELU  v (y > 0 ? 1 : y + 1)        EP_DRELU  y > 0 ? v : 0
+//     (y = aux[m][n], the forward activation);
 //   pre[m][n] = v (pre may be NULL);  v *= mul[m][n] (mul may be NULL);  C = accum ? C + v : v.
 // aux, mul and pre have leading dimension N and serve unbatched products only.
 // 64 x 64 tile, 256 threads of 4 x 4 outputs, K in 16-deep slices through shared memory, each output summed over k in order.
 // AT: A is m-contiguous (s0 == 1), else k-contiguous (s1 == 1); BT: B is k-contiguous (s0 == 1), else n-contiguous
 // (s1 == 1).  The layouts are template parameters so the loaders index with a known unit stride (gemm_kernel picks one).
 // ------------------------------------------------------------------------------------------------
-enum { EP_LIN = 0, EP_RELU, EP_SIG, EP_ELU, EP_DSIG, EP_DELU };
+enum { EP_LIN = 0, EP_RELU, EP_SIG, EP_ELU, EP_DSIG, EP_DELU, EP_DRELU };
 struct Op { const float* p; int64_t so, si, s0, s1; };
 struct Gemm {
   Op A, B;
@@ -47,6 +48,7 @@ __device__ __noinline__ float activate(float v, int epi, float y) {
   if (epi == EP_SIG) return sigm(v);
   if (epi == EP_ELU) return elu(v);
   if (epi == EP_DSIG) return v * (y * (1.f - y));
+  if (epi == EP_DRELU) return y > 0.f ? v : 0.f;
   return v * (y > 0.f ? 1.f : y + 1.f);
 }
 // At most 48 registers (5 CTAs per SM): ptxas would take 64, and fits 48 without spills.

@@ -788,6 +788,212 @@ int r4_batchrl_act(int algo, int obs_dim, int action_size, const float* params, 
 
 }  // extern "C"
 
+// ---- batch RL: continuous-action CQL (r4_cqlconti.cuh), counted with the discrete learners ------------------------
+namespace {
+using r4cqlc::H;
+
+// C = epi(A B + bias): A row-major [M][K] at row stride lda, B = W [K][N] row-major, or its transpose (bt: W [N][K]).
+int cq_gemm(cudaStream_t st, const float* A, int lda, const float* W, int ldw, bool bt, float* C, int M, int N, int K,
+            const float* bias, int epi, const float* aux, int accum) {
+  const Op b = bt ? Op{W, 0, 0, 1, ldw} : Op{W, 0, 0, ldw, 1};
+  const Gemm g{Op{A, 0, 0, lda, 1}, b, C, 0, 0, N, 1, bias, aux, nullptr, nullptr, M, N, K, 1, 0, 1.f, epi, accum};
+  return launch(FAM_BATCHRL, "k_dense_gemm", gemm_kernel(g), dim3((N + GT - 1) / GT, (M + GT - 1) / GT), NT, 0, st, false, g);
+}
+// the relu MLP of net m on rows x [M][m.in] -> h1, h2 [M][H], out [M][m.out]
+int cq_forward(cudaStream_t st, const float* prm, const r4cqlc::Net& m, const float* x, int M, float* h1, float* h2,
+               float* out) {
+  int rc;
+  if ((rc = cq_gemm(st, x, m.in, prm + m.w1, H, false, h1, M, H, m.in, prm + m.b1, EP_RELU, nullptr, 0))) return rc;
+  if ((rc = cq_gemm(st, h1, H, prm + m.w2, H, false, h2, M, H, H, prm + m.b2, EP_RELU, nullptr, 0))) return rc;
+  return cq_gemm(st, h2, H, prm + m.w3, m.out, false, out, M, m.out, H, prm + m.b3, EP_LIN, nullptr, 0);
+}
+// dout [M][m.out] -> dz2 = dout W3^T [h2 > 0], dz1 = dz2 W2^T [h1 > 0]
+int cq_backward(cudaStream_t st, const float* prm, const r4cqlc::Net& m, const float* dout, int M, const float* h1,
+                const float* h2, float* dz2, float* dz1) {
+  int rc;
+  if ((rc = cq_gemm(st, dout, m.out, prm + m.w3, m.out, true, dz2, M, H, m.out, nullptr, EP_DRELU, h2, 0))) return rc;
+  return cq_gemm(st, dz2, H, prm + m.w2, H, true, dz1, M, H, H, nullptr, EP_DRELU, h1, 0);
+}
+// the six weight-gradient jobs of net m over rows x, h1, h2 and their output gradients dz1, dz2, dout
+void cq_jobs(Jobs& J, int& k, const r4cqlc::Net& m, const float* x, const float* h1, const float* h2, const float* dz1,
+             const float* dz2, const float* dout) {
+  J.j[k++] = {x, dz1, m.in, m.in, H, m.w1, 0};
+  J.j[k++] = {nullptr, dz1, 1, 1, H, m.b1, 0};
+  J.j[k++] = {h1, dz2, H, H, H, m.w2, 0};
+  J.j[k++] = {nullptr, dz2, 1, 1, H, m.b2, 0};
+  J.j[k++] = {h2, dout, H, H, m.out, m.w3, 0};
+  J.j[k++] = {nullptr, dout, 1, 1, m.out, m.b3, 0};
+}
+template <typename... P, typename... A>
+int cq_launch(const char* name, void (*kernel)(P...), unsigned grid, cudaStream_t st, bool pdl, A&&... args) {
+  return launch(FAM_BATCHRL, name, kernel, grid, r4cqlc::NT, 0, st, pdl, std::forward<A>(args)...);
+}
+unsigned cq_blocks(int64_t n, int per) { return (unsigned)((n + per - 1) / per); }
+
+// One SGD step at 1-based step `step` (the noise counter): temperature, alpha, critic, actor.  apply: each phase's Adam
+// (the critic's with the soft target update) runs before the next phase; else the phases' gradients at the given
+// parameters go to P.grad and nothing is updated.  pdl: the r4cqlc kernels of the chain wait on griddepcontrol.
+int cq_step(const r4cqlc::Layout& L, const r4cqlc::Hyper& hp, float* prm, float* tgt, float* m, float* v,
+            const r4cqlc::Data& D, const int64_t* idx, int n, int step, int apply, const r4cqlc::Planes& P, float* stats,
+            cudaStream_t st, bool pdl) {
+  using namespace r4cqlc;
+  const int S = hp.S, R = (1 + 2 * S) * n;
+  const int ap = apply ? step : 1;
+  int rc;
+  if ((rc = cq_launch("k_cqlc_gather", k_cqlc_gather, 2 * sm_count(), st, pdl, L, hp, D, idx, n, (uint64_t)step, P))) return rc;
+  if ((rc = cq_forward(st, prm, L.actor, P.xs, n, P.ah1, P.ah2, P.ao))) return rc;
+  if ((rc = cq_launch("k_cqlc_temp", k_cqlc_temp, 1, st, pdl, L, hp, n, P, prm, m, v, ap, apply, stats))) return rc;
+  // alpha
+  if ((rc = cq_launch("k_cqlc_pack", k_cqlc_pack, cq_blocks(R, NT / 32), st, pdl, L, S, n, (int)PK_ALPHA, P))) return rc;
+  for (int k = 0; k < 2; ++k)
+    if ((rc = cq_forward(st, prm, L.c[k], P.x, R, P.c[k].h1, P.c[k].h2, P.c[k].q))) return rc;
+  if ((rc = cq_launch("k_cqlc_loss", k_cqlc_loss, 1, st, pdl, L, hp, n, (int)PH_ALPHA, P, prm, m, v, ap, apply, stats))) return rc;
+  // critic: the target on s', then the critic rows
+  if ((rc = cq_forward(st, prm, L.actor, P.xn, n, P.nh1, P.nh2, P.no))) return rc;
+  if ((rc = cq_launch("k_cqlc_pack", k_cqlc_pack, cq_blocks(n, NT / 32), st, pdl, L, S, n, (int)PK_TARGET, P))) return rc;
+  for (int k = 0; k < 2; ++k)
+    if ((rc = cq_forward(st, tgt, r4cqlc::make_net(L.c[k].w1 - L.t0, L.c[k].in, L.c[k].out), P.x, n, P.c[k].h1, P.c[k].h2,
+                         P.qt + (size_t)k * n)))
+      return rc;
+  if ((rc = cq_launch("k_cqlc_pack", k_cqlc_pack, cq_blocks(R, NT / 32), st, pdl, L, S, n, (int)PK_CRITIC, P))) return rc;
+  for (int k = 0; k < 2; ++k)
+    if ((rc = cq_forward(st, prm, L.c[k], P.x, R, P.c[k].h1, P.c[k].h2, P.c[k].q))) return rc;
+  if ((rc = cq_launch("k_cqlc_loss", k_cqlc_loss, 1, st, pdl, L, hp, n, (int)PH_CRITIC, P, prm, m, v, ap, apply, stats))) return rc;
+  Jobs J;
+  int nj = 0;
+  for (int k = 0; k < 2; ++k) {
+    const CPlanes& c = P.c[k];
+    if ((rc = cq_backward(st, prm, L.c[k], c.dq, R, c.h1, c.h2, c.dz2, c.dz1))) return rc;
+    cq_jobs(J, nj, L.c[k], P.x, c.h1, c.h2, c.dz1, c.dz2, c.dq);
+  }
+  tile_jobs(J, nj);
+  const Stats none{nullptr, 0, nullptr, nullptr, 0.f, 0};
+  if ((rc = launch(FAM_BATCHRL, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, st, false, J, R, 1, P.grad, none))) return rc;
+  if (apply && (rc = cq_launch("k_cqlc_adam", k_cqlc_adam, cq_blocks(L.ntgt, NT), st, pdl, L.t0, L.ntgt, prm,
+                               (const float*)P.grad, m, v, step, hp.lr_critic, hp.eps, tgt, hp.tau)))
+    return rc;
+  // actor: d(-min_k Q_k)/da through the critics, then the squashed head and the actor's layers
+  if ((rc = cq_launch("k_cqlc_pack", k_cqlc_pack, cq_blocks(n, NT / 32), st, pdl, L, S, n, (int)PK_ACTOR, P))) return rc;
+  for (int k = 0; k < 2; ++k)
+    if ((rc = cq_forward(st, prm, L.c[k], P.x, n, P.c[k].h1, P.c[k].h2, P.c[k].q))) return rc;
+  if ((rc = cq_launch("k_cqlc_loss", k_cqlc_loss, 1, st, pdl, L, hp, n, (int)PH_ACTOR, P, prm, m, v, ap, apply, stats))) return rc;
+  for (int k = 0; k < 2; ++k) {
+    const CPlanes& c = P.c[k];
+    if ((rc = cq_backward(st, prm, L.c[k], c.dq, n, c.h1, c.h2, c.dz2, c.dz1))) return rc;
+    if ((rc = cq_gemm(st, c.dz1, H, prm + L.c[k].w1 + (size_t)L.K * H, H, true, P.da, n, L.D, H, nullptr, EP_LIN, nullptr, k)))
+      return rc;
+  }
+  if ((rc = cq_launch("k_cqlc_head", k_cqlc_head, cq_blocks((int64_t)n * L.D, NT), st, pdl, L, hp, n, P, (const float*)prm)))
+    return rc;
+  if ((rc = cq_backward(st, prm, L.actor, P.dout, n, P.ah1, P.ah2, P.adz2, P.adz1))) return rc;
+  nj = 0;
+  cq_jobs(J, nj, L.actor, P.xs, P.ah1, P.ah2, P.adz1, P.adz2, P.dout);
+  tile_jobs(J, nj);
+  if ((rc = launch(FAM_BATCHRL, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, st, false, J, n, 1, P.grad, none))) return rc;
+  if (apply && (rc = cq_launch("k_cqlc_adam", k_cqlc_adam, cq_blocks(L.actor.end, NT), st, pdl, 0, L.actor.end, prm,
+                               (const float*)P.grad, m, v, step, hp.lr_actor, hp.eps, (float*)nullptr, 0.f)))
+    return rc;
+  return R4_OK;
+}
+
+r4cqlc::Hyper cq_hyper(const r4_cqlc_hyper* h, int D) {
+  return r4cqlc::Hyper{h->gamma, h->tau, h->adam_eps, h->alpha_threshold, h->conservative_weight, h->reward_mean,
+                       h->reward_den, (float)((double)D * std::log(0.5)), h->lr_actor, h->lr_critic, h->lr_temp,
+                       h->lr_alpha, h->n_action_samples, h->seed};
+}
+bool cq_args_ok(int K, int D, const r4_cqlc_data* d, const r4_cqlc_hyper* h, int n) {
+  return r4cqlc::dims_ok(K, D) && d && d->obs && d->action && d->reward && d->terminal && d->transitions && h &&
+         h->n_action_samples >= 1 && h->n_action_samples <= r4cqlc::MAXS && n >= 1 && n <= r4cqlc::MAXN;
+}
+}  // namespace
+
+extern "C" {
+
+int r4_cqlc_num_params(int obs_dim, int action_dim) {
+  return r4cqlc::dims_ok(obs_dim, action_dim) ? r4cqlc::make_layout(obs_dim, action_dim).n : -1;
+}
+
+int r4_cqlc_target_size(int obs_dim, int action_dim) {
+  return r4cqlc::dims_ok(obs_dim, action_dim) ? r4cqlc::make_layout(obs_dim, action_dim).ntgt : -1;
+}
+
+int64_t r4_cqlc_scratch_size(int obs_dim, int action_dim, int n_action_samples, int n) {
+  if (!r4cqlc::dims_ok(obs_dim, action_dim) || n_action_samples < 1 || n_action_samples > r4cqlc::MAXS || n < 1 ||
+      n > r4cqlc::MAXN)
+    return -1;
+  return (int64_t)r4cqlc::scratch_floats(r4cqlc::make_layout(obs_dim, action_dim), n_action_samples, n);
+}
+
+int64_t r4_cqlc_act_scratch_size(int obs_dim, int action_dim, int n) {
+  if (!r4cqlc::dims_ok(obs_dim, action_dim) || n < 1 || n > r4cqlc::MAXACT) return -1;
+  return (int64_t)r4cqlc::act_scratch_floats(r4cqlc::make_layout(obs_dim, action_dim), n);
+}
+
+int r4_cqlc_grad(int obs_dim, int action_dim, const float* params, const float* target, const r4_cqlc_data* data,
+                 const r4_cqlc_hyper* hp, const int64_t* idx, int n, int step, float* scratch, float* grad, float* stats,
+                 void* stream) {
+  if (!cq_args_ok(obs_dim, action_dim, data, hp, n) || !params || !target || !idx || step < 1 || !scratch || !grad)
+    return fail(R4_ERR_ARG, "r4_cqlc_grad: bad argument (obs_dim 1..4096, action_dim 1..512, n 1..4096, samples 1..64)");
+  const r4cqlc::Layout L = r4cqlc::make_layout(obs_dim, action_dim);
+  r4cqlc::Planes P = r4cqlc::make_planes(scratch, L, hp->n_action_samples, n);
+  P.grad = grad;
+  const r4cqlc::Data D{data->obs, data->action, data->reward, data->terminal, data->transitions};
+  return cq_step(L, cq_hyper(hp, action_dim), const_cast<float*>(params), const_cast<float*>(target), nullptr, nullptr, D,
+                 idx, n, step, 0, P, stats, S(stream), false);
+}
+
+int r4_cqlc_epoch(int obs_dim, int action_dim, float* params, float* target, float* m, float* v, const r4_cqlc_data* data,
+                  const r4_cqlc_hyper* hp, const int64_t* perm, int64_t n_perm, int mb, int step0, float* scratch,
+                  float* stats, void* stream) {
+  if (!cq_args_ok(obs_dim, action_dim, data, hp, mb) || !params || !target || !m || !v || !perm || n_perm < 1 ||
+      step0 < 0 || !scratch)
+    return fail(R4_ERR_ARG, "r4_cqlc_epoch: bad argument");
+  const int64_t steps = n_perm / mb;
+  if (steps > (int64_t)0x7fffffff - step0) return fail(R4_ERR_ARG, "r4_cqlc_epoch: too many steps");
+  const r4cqlc::Layout L = r4cqlc::make_layout(obs_dim, action_dim);
+  const r4cqlc::Planes P = r4cqlc::make_planes(scratch, L, hp->n_action_samples, mb);
+  const r4cqlc::Data D{data->obs, data->action, data->reward, data->terminal, data->transitions};
+  const r4cqlc::Hyper h = cq_hyper(hp, action_dim);
+  for (int64_t k = 0; k < steps; ++k) {
+    const int rc = cq_step(L, h, params, target, m, v, D, perm + k * mb, mb, step0 + (int)k + 1, 1, P,
+                           stats ? stats + r4cqlc::NSTAT * k : nullptr, S(stream), true);
+    if (rc) return rc;
+  }
+  return (int)steps;
+}
+
+int r4_cqlc_act(int obs_dim, int action_dim, const float* params, const void* obs, int obs_f64, int n,
+                const float* action_in, float* action, float* q, float* scratch, void* stream) {
+  if (!r4cqlc::dims_ok(obs_dim, action_dim) || !params || !obs || n < 1 || n > r4cqlc::MAXACT || !scratch || (!action && !q))
+    return fail(R4_ERR_ARG, "r4_cqlc_act: bad argument");
+  using namespace r4cqlc;
+  const Layout L = make_layout(obs_dim, action_dim);
+  const int K = obs_dim, D = action_dim;
+  cudaStream_t st = S(stream);
+  float* p = scratch;
+  float *x = p, *h1 = x + (size_t)n * K, *h2 = h1 + (size_t)n * H, *o = h2 + (size_t)n * H, *xa = o + (size_t)n * 2 * D;
+  float* ch = xa + (size_t)n * (K + D);          // per critic: h1, h2 [n][H], q [n]
+  const int64_t total = (int64_t)n * K;
+  int rc;
+  if ((rc = cq_launch("k_cqlc_obs", k_cqlc_obs, cq_blocks(total, NT), st, false, obs_f64 ? nullptr : (const float*)obs,
+                      obs_f64 ? (const double*)obs : nullptr, total, x)))
+    return rc;
+  if ((rc = cq_forward(st, params, L.actor, x, n, h1, h2, o))) return rc;
+  if ((rc = cq_launch("k_cqlc_predict", k_cqlc_predict, cq_blocks((int64_t)n * (K + D), NT), st, false, K, D, n,
+                      (const float*)x, (const float*)o, action_in, action, q ? xa : nullptr)))
+    return rc;
+  if (!q) return R4_OK;
+  float* qk[2];
+  for (int k = 0; k < 2; ++k) {
+    float* c = ch + (size_t)k * n * (2 * H + 1);
+    qk[k] = c + (size_t)n * 2 * H;
+    if ((rc = cq_forward(st, params, L.c[k], xa, n, c, c + (size_t)n * H, qk[k]))) return rc;
+  }
+  return cq_launch("k_cqlc_qmean", k_cqlc_qmean, cq_blocks(n, NT), st, false, n, (const float*)qk[0], (const float*)qk[1], q);
+}
+
+}  // extern "C"
+
 // ---- training the simulators (r4_simtrain.cuh): DIEN, the dnn / widedeep / lstm backbones and adversarial_slate --------
 // kernels launched by the r4_simtrain_* entry points in this process (the radix sort counted once)
 int64_t r4_simtrain_launch_count(void) { return g_launches[FAM_SIMTRAIN].load(std::memory_order_relaxed); }
@@ -1704,3 +1910,209 @@ int r4_exactk_adam(int net, float* params, float* grad, float* m, float* v, int 
   return ek_launch("k_keras_adam", k_keras_adam, blocks(np, 256), 256, 0, S(stream), np, (int64_t)0, np, np, params, grad, m,
                    v, alpha, beta1, beta2, eps);
 }
+
+// ---- batch RL: continuous-action BCQ (r4_bcqconti.cuh), counted with the discrete learners ------------------------
+namespace {
+
+int bc_pack(cudaStream_t st, bool pdl, const float* obs, int K, int rep, const float* A, int lda, const float* B, int W,
+            int mode, float flex, int R, float* x, float* out) {
+  return cq_launch("k_bcqc_pack", r4bcqc::k_bcqc_pack, cq_blocks(R, NT / 32), st, pdl, obs, K, rep, A, lda, B, W, mode, flex, R,
+                   x, out);
+}
+
+// One SGD step at 1-based step `step`: imitator, critic, actor (each phase's Adam before the next when apply; the
+// critic's and the actor's Adam with the soft update of their targets), else every group's gradient at the given
+// parameters into P.grad.
+int bc_step(const r4bcqc::Layout& L, const r4bcqc::Hyper& hp, float* prm, float* tgt, float* m, float* v,
+            const r4cqlc::Data& Dt, const int64_t* idx, int n, int step, int apply, const r4bcqc::Planes& P, float* stats,
+            cudaStream_t st, bool pdl) {
+  using namespace r4bcqc;
+  const int K = L.K, D = L.D, La = L.L, S = hp.S, R = n * S;
+  const Stats none{nullptr, 0, nullptr, nullptr, 0.f, 0};
+  int rc;
+  if ((rc = cq_launch("k_bcqc_gather", k_bcqc_gather, 2 * sm_count(), st, pdl, K, D, Dt, idx, n, P))) return rc;
+  if ((rc = cq_launch("k_bcqc_noise", k_bcqc_noise, 2 * sm_count(), st, pdl, L, hp, n, (uint64_t)step, P))) return rc;
+  // imitator: the conditional VAE
+  if ((rc = bc_pack(st, pdl, P.xs, K, 1, P.act, D, nullptr, D, PK_PLAIN, 0.f, n, P.ex, nullptr))) return rc;
+  if ((rc = cq_forward(st, prm, L.enc, P.ex, n, P.eh1, P.eh2, P.eo))) return rc;
+  if ((rc = bc_pack(st, pdl, P.xs, K, 1, P.eo, 2 * La, P.eps, La, PK_REPARAM, 0.f, n, P.dx, nullptr))) return rc;
+  if ((rc = cq_forward(st, prm, L.dec, P.dx, n, P.dh1, P.dh2, P.o))) return rc;
+  if ((rc = cq_launch("k_bcqc_vae", k_bcqc_vae, 1, st, pdl, L, hp, n, P, (const float*)P.o, stats))) return rc;
+  if ((rc = cq_backward(st, prm, L.dec, P.dout, n, P.dh1, P.dh2, P.ddz2, P.ddz1))) return rc;
+  if ((rc = cq_gemm(st, P.ddz1, H, prm + L.dec.w1 + (size_t)K * H, H, true, P.dlat, n, La, H, nullptr, EP_LIN, nullptr, 0)))
+    return rc;
+  if ((rc = cq_launch("k_bcqc_vae_head", k_bcqc_vae_head, cq_blocks((int64_t)n * La, NT), st, pdl, L, hp, n, P))) return rc;
+  if ((rc = cq_backward(st, prm, L.enc, P.deo, n, P.eh1, P.eh2, P.edz2, P.edz1))) return rc;
+  Jobs J;
+  int nj = 0;
+  cq_jobs(J, nj, L.dec, P.dx, P.dh1, P.dh2, P.ddz1, P.ddz2, P.dout);
+  cq_jobs(J, nj, L.enc, P.ex, P.eh1, P.eh2, P.edz1, P.edz2, P.deo);
+  tile_jobs(J, nj);
+  if ((rc = launch(FAM_BATCHRL, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, st, false, J, n, 1, P.grad, none))) return rc;
+  if (apply && (rc = cq_launch("k_cqlc_adam", r4cqlc::k_cqlc_adam, cq_blocks(L.dec.end - L.enc.w1, NT), st, pdl, L.enc.w1,
+                               L.dec.end - L.enc.w1, prm, (const float*)P.grad, m, v, step, hp.lr_imitator, hp.eps,
+                               (float*)nullptr, 0.f)))
+    return rc;
+  // critic: the target over S decoded, perturbed actions per s'
+  if ((rc = bc_pack(st, pdl, P.xn, K, S, P.zt, La, nullptr, La, PK_LATENT, 0.f, R, P.x, nullptr))) return rc;
+  if ((rc = cq_forward(st, prm, L.dec, P.x, R, P.h1, P.h2, P.o))) return rc;
+  if ((rc = bc_pack(st, pdl, P.xn, K, S, P.o, D, nullptr, D, PK_TANH, 0.f, R, P.x, P.base))) return rc;
+  if ((rc = cq_forward(st, tgt, L.actor, P.x, R, P.h1, P.h2, P.o))) return rc;
+  if ((rc = bc_pack(st, pdl, P.xn, K, S, P.o, D, P.base, D, PK_PERTURB, hp.flex, R, P.x, nullptr))) return rc;
+  for (int k = 0; k < 2; ++k)
+    if ((rc = cq_forward(st, tgt, L.c[k], P.x, R, P.h1, P.h2, k ? P.qb : P.qa))) return rc;
+  if ((rc = bc_pack(st, pdl, P.xs, K, 1, P.act, D, nullptr, D, PK_PLAIN, 0.f, n, P.cx, nullptr))) return rc;
+  for (int k = 0; k < 2; ++k)
+    if ((rc = cq_forward(st, prm, L.c[k], P.cx, n, P.ch1[k], P.ch2[k], P.cq[k]))) return rc;
+  if ((rc = cq_launch("k_bcqc_critic", k_bcqc_critic, 1, st, pdl, hp, n, P, stats))) return rc;
+  nj = 0;
+  for (int k = 0; k < 2; ++k) {
+    if ((rc = cq_backward(st, prm, L.c[k], P.dq[k], n, P.ch1[k], P.ch2[k], P.dz2[k], P.dz1[k]))) return rc;
+    cq_jobs(J, nj, L.c[k], P.cx, P.ch1[k], P.ch2[k], P.dz1[k], P.dz2[k], P.dq[k]);
+  }
+  tile_jobs(J, nj);
+  if ((rc = launch(FAM_BATCHRL, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, st, false, J, n, 1, P.grad, none))) return rc;
+  const int c0 = L.c[0].w1, nc = L.c[1].end - c0;
+  if (apply && (rc = cq_launch("k_cqlc_adam", r4cqlc::k_cqlc_adam, cq_blocks(nc, NT), st, pdl, c0, nc, prm,
+                               (const float*)P.grad, m, v, step, hp.lr_critic, hp.eps, tgt + c0, hp.tau)))
+    return rc;
+  // actor: -Q_0(s, pi(s, dec(s, clamp(z))))
+  if ((rc = bc_pack(st, pdl, P.xs, K, 1, P.za, La, nullptr, La, PK_LATENT, 0.f, n, P.x, nullptr))) return rc;
+  if ((rc = cq_forward(st, prm, L.dec, P.x, n, P.h1, P.h2, P.o))) return rc;
+  if ((rc = bc_pack(st, pdl, P.xs, K, 1, P.o, D, nullptr, D, PK_TANH, 0.f, n, P.ax, P.abase))) return rc;
+  if ((rc = cq_forward(st, prm, L.actor, P.ax, n, P.ah1, P.ah2, P.ao))) return rc;
+  if ((rc = bc_pack(st, pdl, P.xs, K, 1, P.ao, D, P.abase, D, PK_PERTURB, hp.flex, n, P.cx, nullptr))) return rc;
+  if ((rc = cq_forward(st, prm, L.c[0], P.cx, n, P.ch1[0], P.ch2[0], P.cq[0]))) return rc;
+  if ((rc = cq_launch("k_bcqc_actor_loss", k_bcqc_actor_loss, 1, st, pdl, n, P, stats))) return rc;
+  if ((rc = cq_backward(st, prm, L.c[0], P.dq[0], n, P.ch1[0], P.ch2[0], P.dz2[0], P.dz1[0]))) return rc;
+  if ((rc = cq_gemm(st, P.dz1[0], H, prm + L.c[0].w1 + (size_t)K * H, H, true, P.da, n, D, H, nullptr, EP_LIN, nullptr, 0)))
+    return rc;
+  if ((rc = cq_launch("k_bcqc_actor_head", k_bcqc_actor_head, cq_blocks((int64_t)n * D, NT), st, pdl, D, hp.flex, n, P)))
+    return rc;
+  if ((rc = cq_backward(st, prm, L.actor, P.dout, n, P.ah1, P.ah2, P.adz2, P.adz1))) return rc;
+  nj = 0;
+  cq_jobs(J, nj, L.actor, P.ax, P.ah1, P.ah2, P.adz1, P.adz2, P.dout);
+  tile_jobs(J, nj);
+  if ((rc = launch(FAM_BATCHRL, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, st, false, J, n, 1, P.grad, none))) return rc;
+  if (apply && (rc = cq_launch("k_cqlc_adam", r4cqlc::k_cqlc_adam, cq_blocks(L.actor.end, NT), st, pdl, 0, L.actor.end, prm,
+                               (const float*)P.grad, m, v, step, hp.lr_actor, hp.eps, tgt, hp.tau)))
+    return rc;
+  return R4_OK;
+}
+
+r4bcqc::Hyper bc_hyper(const r4_bcqc_hyper* h) {
+  return r4bcqc::Hyper{h->gamma, h->tau, h->lam, h->beta, h->action_flexibility, h->adam_eps, h->reward_mean, h->reward_den,
+                       h->lr_actor, h->lr_critic, h->lr_imitator, h->n_action_samples, h->seed};
+}
+bool bc_args_ok(int K, int D, const r4_cqlc_data* d, const r4_bcqc_hyper* h, int n) {
+  return h && r4bcqc::dims_ok(K, D, h->latent_size) && d && d->obs && d->action && d->reward && d->terminal &&
+         d->transitions && h->n_action_samples >= 1 && h->n_action_samples <= r4bcqc::MAXS && n >= 1 && n <= r4bcqc::MAXN;
+}
+}  // namespace
+
+extern "C" {
+
+int r4_bcqc_num_params(int obs_dim, int action_dim, int latent_size) {
+  return r4bcqc::dims_ok(obs_dim, action_dim, latent_size) ? r4bcqc::make_layout(obs_dim, action_dim, latent_size).n : -1;
+}
+
+int r4_bcqc_target_size(int obs_dim, int action_dim, int latent_size) {
+  return r4bcqc::dims_ok(obs_dim, action_dim, latent_size) ? r4bcqc::make_layout(obs_dim, action_dim, latent_size).ntgt : -1;
+}
+
+int64_t r4_bcqc_scratch_size(int obs_dim, int action_dim, int latent_size, int n_action_samples, int n) {
+  if (!r4bcqc::dims_ok(obs_dim, action_dim, latent_size) || n_action_samples < 1 || n_action_samples > r4bcqc::MAXS ||
+      n < 1 || n > r4bcqc::MAXN)
+    return -1;
+  return (int64_t)r4bcqc::scratch_floats(r4bcqc::make_layout(obs_dim, action_dim, latent_size), n_action_samples, n);
+}
+
+int64_t r4_bcqc_act_scratch_size(int obs_dim, int action_dim, int latent_size, int n_action_samples, int n) {
+  if (!r4bcqc::dims_ok(obs_dim, action_dim, latent_size) || n_action_samples < 1 || n_action_samples > r4bcqc::MAXS ||
+      n < 1 || (int64_t)n * n_action_samples > r4cqlc::MAXACT)
+    return -1;
+  return (int64_t)r4bcqc::act_scratch_floats(r4bcqc::make_layout(obs_dim, action_dim, latent_size), n_action_samples, n);
+}
+
+int r4_bcqc_grad(int obs_dim, int action_dim, const float* params, const float* target, const r4_cqlc_data* data,
+                 const r4_bcqc_hyper* hp, const int64_t* idx, int n, int step, float* scratch, float* grad, float* stats,
+                 void* stream) {
+  if (!bc_args_ok(obs_dim, action_dim, data, hp, n) || !params || !target || !idx || step < 1 || !scratch || !grad)
+    return fail(R4_ERR_ARG, "r4_bcqc_grad: bad argument (obs_dim 1..4096, action_dim 1..512, latent 1..512, n 1..4096, "
+                            "samples 1..256)");
+  const r4bcqc::Layout L = r4bcqc::make_layout(obs_dim, action_dim, hp->latent_size);
+  r4bcqc::Planes P = r4bcqc::make_planes(scratch, L, hp->n_action_samples, n);
+  P.grad = grad;
+  const r4cqlc::Data D{data->obs, data->action, data->reward, data->terminal, data->transitions};
+  return bc_step(L, bc_hyper(hp), const_cast<float*>(params), const_cast<float*>(target), nullptr, nullptr, D, idx, n, step,
+                 0, P, stats, S(stream), false);
+}
+
+int r4_bcqc_epoch(int obs_dim, int action_dim, float* params, float* target, float* m, float* v, const r4_cqlc_data* data,
+                  const r4_bcqc_hyper* hp, const int64_t* perm, int64_t n_perm, int mb, int step0, float* scratch,
+                  float* stats, void* stream) {
+  if (!bc_args_ok(obs_dim, action_dim, data, hp, mb) || !params || !target || !m || !v || !perm || n_perm < 1 ||
+      step0 < 0 || !scratch)
+    return fail(R4_ERR_ARG, "r4_bcqc_epoch: bad argument");
+  const int64_t steps = n_perm / mb;
+  if (steps > (int64_t)0x7fffffff - step0) return fail(R4_ERR_ARG, "r4_bcqc_epoch: too many steps");
+  const r4bcqc::Layout L = r4bcqc::make_layout(obs_dim, action_dim, hp->latent_size);
+  const r4bcqc::Planes P = r4bcqc::make_planes(scratch, L, hp->n_action_samples, mb);
+  const r4cqlc::Data D{data->obs, data->action, data->reward, data->terminal, data->transitions};
+  const r4bcqc::Hyper h = bc_hyper(hp);
+  for (int64_t k = 0; k < steps; ++k) {
+    const int rc = bc_step(L, h, params, target, m, v, D, perm + k * mb, mb, step0 + (int)k + 1, 1, P,
+                           stats ? stats + r4bcqc::NSTAT * k : nullptr, S(stream), true);
+    if (rc) return rc;
+  }
+  return (int)steps;
+}
+
+int r4_bcqc_act(int obs_dim, int action_dim, const float* params, const void* obs, int obs_f64, int n,
+                const r4_bcqc_hyper* hp, uint64_t counter, const float* action_in, float* action, float* q, float* scratch,
+                void* stream) {
+  if (!hp || !r4bcqc::dims_ok(obs_dim, action_dim, hp->latent_size) || hp->n_action_samples < 1 ||
+      hp->n_action_samples > r4bcqc::MAXS || !params || !obs || n < 1 ||
+      (int64_t)n * hp->n_action_samples > r4cqlc::MAXACT || !scratch || (!action && !(q && action_in)))
+    return fail(R4_ERR_ARG, "r4_bcqc_act: bad argument");
+  using namespace r4bcqc;
+  const Layout L = make_layout(obs_dim, action_dim, hp->latent_size);
+  const int K = obs_dim, D = action_dim, La = hp->latent_size, NS = hp->n_action_samples, R = n * NS;
+  const int W = D > La ? D : La;
+  cudaStream_t st = r4h::S(stream);
+  float *x = scratch, *xin = x + (size_t)n * K, *h1 = xin + (size_t)R * (K + W), *h2 = h1 + (size_t)R * H;
+  float *o = h2 + (size_t)R * H, *base = o + (size_t)R * D, *cq = base + (size_t)R * D, *z = cq + R;
+  float *xa = z + (size_t)R * La, *ch = xa + (size_t)n * (K + D);
+  const int64_t total = (int64_t)n * K;
+  int rc;
+  if ((rc = cq_launch("k_cqlc_obs", r4cqlc::k_cqlc_obs, cq_blocks(total, NT), st, false,
+                      obs_f64 ? nullptr : (const float*)obs, obs_f64 ? (const double*)obs : nullptr, total, x)))
+    return rc;
+  if (action) {
+    if ((rc = cq_launch("k_bcqc_predict_noise", k_bcqc_predict_noise, cq_blocks((int64_t)R * La, NT), st, false, La, NS, n,
+                        hp->seed, counter, z)))
+      return rc;
+    if ((rc = bc_pack(st, false, x, K, NS, z, La, nullptr, La, PK_LATENT, 0.f, R, xin, nullptr))) return rc;
+    if ((rc = cq_forward(st, params, L.dec, xin, R, h1, h2, o))) return rc;
+    if ((rc = bc_pack(st, false, x, K, NS, o, D, nullptr, D, PK_TANH, 0.f, R, xin, base))) return rc;
+    if ((rc = cq_forward(st, params, L.actor, xin, R, h1, h2, o))) return rc;
+    if ((rc = bc_pack(st, false, x, K, NS, o, D, base, D, PK_PERTURB, hp->action_flexibility, R, xin, base))) return rc;
+    if ((rc = cq_forward(st, params, L.c[0], xin, R, h1, h2, cq))) return rc;
+    if ((rc = cq_launch("k_bcqc_argmax", k_bcqc_argmax, cq_blocks(n, NT / 32), st, false, D, NS, n, (const float*)cq,
+                        (const float*)base, action)))
+      return rc;
+  }
+  if (!q) return R4_OK;
+  if ((rc = bc_pack(st, false, x, K, 1, action_in ? action_in : action, D, nullptr, D, PK_PLAIN, 0.f, n, xa, nullptr)))
+    return rc;
+  float* qk[2];
+  for (int k = 0; k < 2; ++k) {
+    float* c = ch + (size_t)k * n * (2 * H + 1);
+    qk[k] = c + (size_t)n * 2 * H;
+    if ((rc = cq_forward(st, params, L.c[k], xa, n, c, c + (size_t)n * H, qk[k]))) return rc;
+  }
+  return cq_launch("k_cqlc_qmean", r4cqlc::k_cqlc_qmean, cq_blocks(n, NT), st, false, n, (const float*)qk[0],
+                   (const float*)qk[1], q);
+}
+
+}  // extern "C"

@@ -620,3 +620,316 @@ class BatchRLNet(object):
         else:
             pick = probs
         return pick.argmax(1).to(torch.int32), probs, raw
+
+
+def cqlc_draws(seed, counter, stream, rows, samples, dims, uniform=None):
+    """The noise of csrc/r4_cqlconti.cuh for one stream of one step: splitmix64(splitmix64(seed ^ splitmix64(counter << 3 |
+    stream)) ^ (row << 24 | sample << 12 | dim)) -> float64 [rows, samples, dims]: uniform in [-1, 1) for the uniform
+    streams (2 and 4), else standard normal (Box-Muller on (2 hi + 1) / 2^25, hi the top 24 bits, and bits 16..39)."""
+    import numpy as np
+    assert samples <= 4096 and dims <= 4096
+    with np.errstate(over="ignore"):
+        base = _splitmix64(np.uint64(seed) ^ _splitmix64(np.uint64((int(counter) << 3) | int(stream))))
+        r = np.arange(rows, dtype=np.uint64)[:, None, None] << np.uint64(24)
+        s = np.arange(samples, dtype=np.uint64)[None, :, None] << np.uint64(12)
+        d = np.arange(dims, dtype=np.uint64)[None, None, :]
+        x = _splitmix64(base ^ (r | s | d))
+    hi = (x >> np.uint64(40)).astype(np.float64)
+    if (stream in (2, 4)) if uniform is None else uniform:
+        return hi * (2.0 / 16777216.0) - 1.0
+    u1 = (2.0 * hi + 1.0) / 33554432.0
+    u2 = ((x >> np.uint64(16)) & np.uint64(0xFFFFFF)).astype(np.float64) / 16777216.0
+    return np.sqrt(-2.0 * np.log(u1)) * np.cos(2.0 * np.pi * u2)
+
+
+class BatchRLContiNet(object):
+    """The networks of continuous-action CQL (script/batchrl_trainer.py:61-73 'CQL-conti', d3rlpy 0.91 CQL with its default
+    VectorEncoderFactory), in csrc/r4_cqlconti.cuh's flat layout:
+        actor     obs [K] -> 256 relu -> 256 relu -> [mu | logstd] [2D]   (SquashedNormalPolicy; logstd clamped to [-20, 2])
+        critic k  [obs | action] [K + D] -> 256 relu -> 256 relu -> Q [1]   (k = 0, 1)
+        log_temp, log_alpha   (initial temperature and alpha 1.0)
+    Init is torch's default (Linear: U(+-1/sqrt(fan_in)) for weight and bias).  The target is a copy of both critics.
+    The noise enters explicitly (cqlc_draws), so the same draws drive this twin and the kernels.  This twin is the CPU
+    path of rl4rs_b200.batchrl.ContinuousCQL and the autograd cross-check of the kernels (tests/test_gpu_batchrl_conti.py)."""
+
+    H = 256
+    STREAMS = ("temp", "alpha_policy", "alpha_uniform", "critic_policy", "critic_uniform", "actor")
+
+    def __init__(self, obs_dim, action_dim, device="cuda", seed=0, initial_temperature=1.0, initial_alpha=1.0):
+        self.K, self.D = int(obs_dim), int(action_dim)
+        self.device = torch.device(device)
+        K, D, H = self.K, self.D, self.H
+
+        def net(p, n_in, n_out):
+            return [(p + "w1", (n_in, H)), (p + "b1", (H,)), (p + "w2", (H, H)), (p + "b2", (H,)), (p + "w3", (H, n_out)),
+                    (p + "b3", (n_out,))]
+        shapes = net("a_", K, 2 * D) + net("q0_", K + D, 1) + net("q1_", K + D, 1) + [("log_temp", (1,)),
+                                                                                        ("log_alpha", (1,))]
+        n = sum(math.prod(s) for _, s in shapes)
+        g = torch.Generator(device="cpu").manual_seed(seed)
+        self.flat = torch.zeros(n, dtype=torch.float32, device=self.device, requires_grad=True)
+        off, fan = 0, 1
+        with torch.no_grad():
+            for name, shape in shapes:
+                k = math.prod(shape)
+                v = self.flat[off:off + k].view(shape)
+                if name == "log_temp":
+                    v.fill_(math.log(initial_temperature))
+                elif name == "log_alpha":
+                    v.fill_(math.log(initial_alpha))
+                else:
+                    fan = shape[0] if len(shape) == 2 else fan          # a bias follows its weight
+                    bound = 1.0 / math.sqrt(fan)
+                    v.copy_(((torch.rand(shape, generator=g) * 2 - 1) * bound).to(self.device))
+                off += k
+        self._shapes, self.n_params = shapes, n
+        size = {name: math.prod(s) for name, s in shapes}
+        self.n_actor = sum(v for k, v in size.items() if k.startswith("a_"))
+        self.n_critic = sum(v for k, v in size.items() if k.startswith("q0_"))
+        self.t0, self.n_target = self.n_actor, 2 * self.n_critic
+        self.lt, self.la = n - 2, n - 1
+        self.target = self.flat.detach()[self.t0:self.t0 + self.n_target].clone()
+
+    def params(self, flat=None):
+        flat = self.flat if flat is None else flat
+        out, off = {}, 0
+        for name, shape in self._shapes:
+            k = math.prod(shape)
+            out[name] = flat[off:off + k].view(shape)
+            off += k
+        return out
+
+    def target_params(self, target=None, dtype=None):
+        """The target critics as a params() dict (q0_*, q1_*)."""
+        t = self.target if target is None else target
+        full = torch.zeros(self.n_params, dtype=dtype or t.dtype, device=t.device)
+        full[self.t0:self.t0 + self.n_target] = t.to(full.dtype)
+        return self.params(full)
+
+    @staticmethod
+    def _mlp(p, pre, x):
+        h = torch.relu(x @ p[pre + "w1"] + p[pre + "b1"])
+        return torch.relu(h @ p[pre + "w2"] + p[pre + "b2"]) @ p[pre + "w3"] + p[pre + "b3"]
+
+    def actor(self, x, p):
+        """-> (mu, the raw logstd), each [..., D]."""
+        o = self._mlp(p, "a_", x)
+        return o[..., :self.D], o[..., self.D:]
+
+    @staticmethod
+    def sample(mu, ls_raw, eps):
+        """SquashedNormalPolicy.sample_with_log_prob with the given normal draws: -> (tanh(u), log pi [...]), u = mu +
+        exp(clamp(logstd, -20, 2)) eps; log pi = Normal(mu, std).log_prob(u) - 2 (log 2 - u - softplus(-2 u)), summed."""
+        ls = ls_raw.clamp(-20.0, 2.0)
+        std = ls.exp()
+        u = mu + std * eps
+        logp = -((u - mu) ** 2) / (2 * std * std) - ls - 0.5 * math.log(2 * math.pi)
+        jacob = 2 * (math.log(2) - u - torch.nn.functional.softplus(-2 * u))
+        return torch.tanh(u), (logp - jacob).sum(-1)
+
+    def critic(self, x, a, k, p):
+        return self._mlp(p, "q%d_" % k, torch.cat([x, a], -1)).squeeze(-1)
+
+    def predict(self, x, flat=None):
+        """d3rlpy predict: tanh(mu) [n, D]."""
+        return torch.tanh(self.actor(x, self.params(flat))[0])
+
+    def predict_value(self, x, a, flat=None):
+        """d3rlpy predict_value: the mean of the two critics [n]."""
+        p = self.params(flat)
+        return 0.5 * (self.critic(x, a, 0, p) + self.critic(x, a, 1, p))
+
+    def noise(self, seed, step, n, S, dtype=torch.float32):
+        """The six draws of step `step` (kernel streams 0..5) as tensors: temp and actor [n, D], the others [n, S, D]."""
+        out = {}
+        for st, name in enumerate(self.STREAMS):
+            one = name in ("temp", "actor")
+            d = cqlc_draws(seed, step, st, n, 1 if one else S, self.D)
+            t = torch.from_numpy(d[:, 0] if one else d)
+            out[name] = t.to(device=self.device, dtype=dtype)
+        return out
+
+    def conservative(self, p, obs, act, mu, ls, eps_p, unif, hp):
+        """clamp(exp(log_alpha), 0, 1e6) mean_i sum_k (w (lse - Q_k(s, a)) - threshold) with lse the max-subtracted
+        logsumexp over the S policy samples (minus their log-probs; mu and ls carry no gradient) and the S uniform ones
+        (minus D log 0.5).  -> (the term, the per-row sum over critics before alpha)."""
+        n, S = eps_p.shape[:2]
+        a_p, lp_p = self.sample(mu[:, None], ls[:, None], eps_p)
+        xr = obs[:, None].expand(n, S, obs.shape[-1])
+        lrand = math.log(0.5 ** self.D)
+        rows = 0
+        for k in (0, 1):
+            qp, qu, qd = self.critic(xr, a_p, k, p), self.critic(xr, unif, k, p), self.critic(obs, act, k, p)
+            tv = torch.cat([qp - lp_p, qu - lrand], 1)
+            mx = tv.max(1, keepdim=True).values.detach()
+            lse = mx.squeeze(1) + torch.log(torch.exp(tv - mx).sum(1))
+            rows = rows + hp["conservative_weight"] * (lse - qd) - hp["alpha_threshold"]
+        alpha = p["log_alpha"][0].exp().clamp(0.0, 1e6)
+        return alpha * rows.mean(), rows
+
+    def losses(self, batch, noise, hp, flat=None, target=None):
+        """The four losses of one step at one parameter vector (r4_cqlc_grad's definition): -> ({'temp', 'alpha', 'critic',
+        'actor'} losses, stats [5]).  Each loss is to be differentiated for its own group only."""
+        obs, act, rew, nobs, term = batch
+        flat = self.flat if flat is None else flat
+        p = self.params(flat)
+        dt = flat.dtype
+        obs, act, nobs = obs.to(dt), act.to(dt), nobs.to(dt)
+        nz = {k: v.to(dt) for k, v in noise.items()}
+        mu, ls = self.actor(obs, p)
+        with torch.no_grad():
+            _, lp_t = self.sample(mu, ls, nz["temp"])
+        temp_loss = -(p["log_temp"][0].exp() * (lp_t - self.D)).mean()
+        mu_d, ls_d = mu.detach(), ls.detach()
+        cons_a, _ = self.conservative(p, obs, act, mu_d, ls_d, nz["alpha_policy"], nz["alpha_uniform"], hp)
+        alpha_loss = -cons_a
+        with torch.no_grad():
+            tp = self.target_params(target, dt)
+            a2 = torch.tanh(self.actor(nobs, p)[0])
+            qt = torch.min(self.critic(nobs, a2, 0, tp), self.critic(nobs, a2, 1, tp))
+            r = (rew.to(dt) - hp["reward_mean"]) / hp["reward_den"]
+            y = r + hp["gamma"] * (1.0 - term.to(dt)) * qt
+        q0 = self.critic(obs, act, 0, p)
+        td = ((q0 - y) ** 2).mean() + ((self.critic(obs, act, 1, p) - y) ** 2).mean()
+        cons_c, _ = self.conservative(p, obs, act, mu_d, ls_d, nz["critic_policy"], nz["critic_uniform"], hp)
+        critic_loss = td + cons_c
+        a_pi, lp_pi = self.sample(mu, ls, nz["actor"])
+        qmin = torch.stack([self.critic(obs, a_pi, 0, p), self.critic(obs, a_pi, 1, p)]).min(0).values
+        actor_loss = (p["log_temp"][0].exp() * lp_pi - qmin).mean()
+        st = torch.stack([critic_loss, actor_loss, temp_loss, alpha_loss, q0.mean()]).detach()
+        return {"temp": temp_loss, "alpha": alpha_loss, "critic": critic_loss, "actor": actor_loss}, st
+
+    def group(self, name):
+        """The slice of the flat vector the loss `name` updates."""
+        return {"actor": slice(0, self.n_actor), "critic": slice(self.t0, self.t0 + self.n_target),
+                "temp": slice(self.lt, self.lt + 1), "alpha": slice(self.la, self.la + 1)}[name]
+
+    def grads(self, batch, noise, hp, flat=None, target=None):
+        """r4_cqlc_grad: every group's gradient of its own loss at one parameter vector -> (grad [n_params], stats)."""
+        flat = self.flat if flat is None else flat
+        if not flat.requires_grad:
+            flat = flat.detach().requires_grad_(True)
+        losses, st = self.losses(batch, noise, hp, flat, target)
+        g = torch.zeros_like(flat.detach())
+        for name, loss in losses.items():
+            sl = self.group(name)
+            g[sl] = torch.autograd.grad(loss, flat, retain_graph=True)[0][sl]
+        return g, st
+
+    @torch.no_grad()
+    def soft_update(self, tau):
+        """target = tau * critics + (1 - tau) * target."""
+        c = self.flat.detach()[self.t0:self.t0 + self.n_target]
+        self.target.copy_(tau * c + (1.0 - tau) * self.target)
+
+
+class BatchRLContiBCQNet(BatchRLContiNet):
+    """The networks of continuous-action BCQ (script/batchrl_trainer.py:61-73 'BCQ-conti', d3rlpy 0.91 BCQ with its default
+    VectorEncoderFactory), in csrc/r4_bcqconti.cuh's flat layout (each net 256 relu -> 256 relu -> out):
+        actor     [obs | a] -> f [D];  pi(s, a) = clamp(a + flex tanh(f), -1, 1)   (DeterministicResidualPolicy)
+        critic k  [obs | a] -> Q [1]   (k = 0, 1)
+        encoder   [obs | a] -> [mu | logstd] [2 L] (logstd clamped to [-20, 2]);  decoder  [obs | z] -> tanh [D]
+    Torch default init.  The target is a copy of [actor | critic 0 | critic 1].  The noise enters explicitly."""
+
+    STREAMS = ("vae", "target", "actor")
+
+    def __init__(self, obs_dim, action_dim, device="cuda", seed=0, latent_size=32):
+        self.K, self.D, self.L = int(obs_dim), int(action_dim), int(latent_size)
+        self.device = torch.device(device)
+        K, D, L, H = self.K, self.D, self.L, self.H
+
+        def net(p, n_in, n_out):
+            return [(p + "w1", (n_in, H)), (p + "b1", (H,)), (p + "w2", (H, H)), (p + "b2", (H,)), (p + "w3", (H, n_out)),
+                    (p + "b3", (n_out,))]
+        shapes = net("a_", K + D, D) + net("q0_", K + D, 1) + net("q1_", K + D, 1) + net("e_", K + D, 2 * L) + \
+            net("d_", K + L, D)
+        n = sum(math.prod(s) for _, s in shapes)
+        g = torch.Generator(device="cpu").manual_seed(seed)
+        self.flat = torch.zeros(n, dtype=torch.float32, device=self.device, requires_grad=True)
+        off, fan = 0, 1
+        with torch.no_grad():
+            for name, shape in shapes:
+                k = math.prod(shape)
+                fan = shape[0] if len(shape) == 2 else fan
+                bound = 1.0 / math.sqrt(fan)
+                self.flat[off:off + k].view(shape).copy_(((torch.rand(shape, generator=g) * 2 - 1) * bound).to(self.device))
+                off += k
+        self._shapes, self.n_params = shapes, n
+        size = {name: math.prod(s) for name, s in shapes}
+        part = lambda pre: sum(v for k, v in size.items() if k.startswith(pre))
+        self.n_actor, self.n_critic = part("a_"), part("q0_")
+        self.t0, self.n_target = 0, self.n_actor + 2 * self.n_critic
+        self.target = self.flat.detach()[:self.n_target].clone()
+
+    def group(self, name):
+        return {"actor": slice(0, self.n_actor), "critic": slice(self.n_actor, self.n_target),
+                "imitator": slice(self.n_target, self.n_params)}[name]
+
+    def perturb(self, p, pre, x, a, flex):
+        """pi(x, a) = clamp(a + flex tanh(f([x | a])), -1, 1)."""
+        return (a + flex * torch.tanh(self._mlp(p, pre, torch.cat([x, a], -1)))).clamp(-1.0, 1.0)
+
+    def decode(self, p, x, z):
+        return torch.tanh(self._mlp(p, "d_", torch.cat([x, z], -1)))
+
+    def candidates(self, p, x, z, flex, tp=None):
+        """The S perturbed, decoded actions of rows x [n, K] for latent draws z [n, S, L] (clamped to +-0.5), with the actor
+        of tp (default p) -> [n, S, D]."""
+        xr = x[:, None].expand(x.shape[0], z.shape[1], x.shape[1])
+        a = self.decode(p, xr, z.clamp(-0.5, 0.5))
+        return self.perturb(p if tp is None else tp, "a_", xr, a, flex)
+
+    def noise(self, seed, step, n, S, dtype=torch.float32):
+        out = {}
+        for st, name in enumerate(self.STREAMS):
+            d = cqlc_draws(seed, step, st, n, S if name == "target" else 1, self.L, uniform=False)
+            out[name] = torch.from_numpy(d if name == "target" else d[:, 0]).to(device=self.device, dtype=dtype)
+        return out
+
+    def predict_noise(self, seed, counter, n, S, dtype=torch.float32):
+        """The latent draws of one predict call (kernel stream 3) [n, S, L]."""
+        return torch.from_numpy(cqlc_draws(seed, counter, 3, n, S, self.L, uniform=False)).to(self.device, dtype)
+
+    def predict(self, x, z, hp, flat=None):
+        """d3rlpy BCQ predict: the candidate with the largest Q_0 (the first on ties) -> [n, D]."""
+        p = self.params(flat)
+        c = self.candidates(p, x, z.to(x.dtype), hp["action_flexibility"])
+        xr = x[:, None].expand(x.shape[0], c.shape[1], x.shape[1])
+        q = self.critic(xr, c, 0, p)
+        return c[torch.arange(x.shape[0], device=x.device), q.argmax(1)]
+
+    def losses(self, batch, noise, hp, flat=None, target=None):
+        """The three losses of one step at one parameter vector (r4_bcqc_grad's definition): -> ({'imitator', 'critic',
+        'actor'}, stats [5] = imitator loss, critic loss, actor loss, mean Q_0(s, a), reconstruction mse)."""
+        obs, act, rew, nobs, term = batch
+        flat = self.flat if flat is None else flat
+        p, dt = self.params(flat), flat.dtype
+        obs, act, nobs = obs.to(dt), act.to(dt), nobs.to(dt)
+        nz = {k: v.to(dt) for k, v in noise.items()}
+        L, flex = self.L, hp["action_flexibility"]
+        e = self._mlp(p, "e_", torch.cat([obs, act], -1))
+        mu, ls = e[:, :L], e[:, L:].clamp(-20.0, 2.0)
+        recon = self.decode(p, obs, mu + ls.exp() * nz["vae"])
+        mse = ((recon - act) ** 2).mean()
+        kl = (-ls + 0.5 * ((2 * ls).exp() + mu * mu) - 0.5).mean()
+        imitator = mse + hp["beta"] * kl
+        with torch.no_grad():
+            tp = self.target_params(target, dt)
+            c = self.candidates(p, nobs, nz["target"], flex, tp)
+            xr = nobs[:, None].expand(nobs.shape[0], c.shape[1], nobs.shape[1])
+            qa, qb = self.critic(xr, c, 0, tp), self.critic(xr, c, 1, tp)
+            v = hp["lam"] * torch.minimum(qa, qb) + (1 - hp["lam"]) * torch.maximum(qa, qb)
+            r = (rew.to(dt) - hp["reward_mean"]) / hp["reward_den"]
+            y = r + hp["gamma"] * (1.0 - term.to(dt)) * v.max(1).values
+        q0 = self.critic(obs, act, 0, p)
+        critic = ((q0 - y) ** 2).mean() + ((self.critic(obs, act, 1, p) - y) ** 2).mean()
+        with torch.no_grad():
+            a_s = self.decode(p, obs, nz["actor"].clamp(-0.5, 0.5))
+        actor = -self.critic(obs, self.perturb(p, "a_", obs, a_s, flex), 0, p).mean()
+        st = torch.stack([imitator, critic, actor, q0.mean(), mse]).detach()
+        return {"imitator": imitator, "critic": critic, "actor": actor}, st
+
+    @torch.no_grad()
+    def soft_update(self, tau):
+        """target = tau * [actor | critics] + (1 - tau) * target."""
+        self.target.copy_(tau * self.flat.detach()[:self.n_target] + (1.0 - tau) * self.target)
