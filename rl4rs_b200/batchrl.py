@@ -19,6 +19,10 @@ project's environment).
 'BCQ-conti' (ContinuousBCQ) and 'CQL-conti' (ContinuousCQL) train on the continuous dataset (data_generate_rl4rs_a_conti /
 _b_conti) for a config with support_conti_env: r4_bcqc_epoch / r4_cqlc_epoch on CUDA (csrc/r4_bcqconti.cuh,
 csrc/r4_cqlconti.cuh), policy.BatchRLContiBCQNet / BatchRLContiNet on the CPU, r4_bcqc_act / r4_cqlc_act to act.
+
+Both kinds share one front: DeviceDataset holds either kind of action, and BatchRLBase owns the set-up, the reward
+scaler, fit and its epoch loops, and the checkpoints.  The discrete models (BatchRLModel) and the continuous ones
+(ContinuousCQL, ContinuousBCQ) add their twin, hyper-parameters, entry-point calls, act and checkpoint keys.
 """
 import ctypes as C
 import math
@@ -119,24 +123,37 @@ def transitions_host(terminals):
 
 
 class DeviceDataset(object):
-    """The dataset where the learner runs: obs f32 [N, K], action i32 [N], reward f32 [N], terminal u8 [N] and the
-    transition entries i64 [T].  On CUDA it is uploaded once; a dataset that does not fit raises MemoryError."""
+    """The dataset where the learner runs: obs f32 [N, K], action i32 [N] (discrete: item ids) or f32 [N, D] (continuous:
+    the logged items' embeddings, not clipped), reward f32 [N], terminal u8 [N] and the transition entries i64 [T].
+    continuous: the kind the model needs; None takes the dataset's own (its discrete_action flag, else a single action
+    column means discrete).  On CUDA it is uploaded once; a dataset that does not fit raises MemoryError."""
 
-    def __init__(self, dataset, device):
+    def __init__(self, dataset, device, continuous=None):
         obs = np.asarray(dataset["observations"], dtype=np.float32)
         N = obs.shape[0]
-        act = np.asarray(dataset["actions"]).reshape(N)
-        if np.any(act != np.round(act)) or act.min(initial=0) < 0:
-            raise ValueError("batch RL here is discrete: the dataset's actions must be item ids")
+        act = np.asarray(dataset["actions"])
+        discrete = np.asarray(dataset.get("discrete_action", act.ndim < 2 or act.shape[1] == 1)).item()
+        self.continuous = not discrete if continuous is None else bool(continuous)
+        if self.continuous:
+            act = np.asarray(act, dtype=np.float32)
+            if discrete or act.ndim != 2 or act.shape[0] != N:
+                raise ValueError("continuous batch RL needs the continuous dataset (actions f32 [N, D], discrete_action "
+                                 "False): data_generate_rl4rs_a_conti / _b_conti")
+        else:
+            act = act.reshape(N)
+            if np.any(act != np.round(act)) or act.min(initial=0) < 0:
+                raise ValueError("batch RL here is discrete: the dataset's actions must be item ids")
+            act = act.astype(np.int32)
         self.device, self.N, self.K = torch.device(device), N, obs.shape[1]
-        need = N * (self.K * 4 + 4 + 4 + 1 + 8)
+        self.D = act.shape[1] if self.continuous else None
+        need = obs.nbytes + act.nbytes + N * (4 + 1 + 8)
         if self.device.type == "cuda":
             free = torch.cuda.mem_get_info(self.device)[0]
             if need > free:
                 raise MemoryError("the dataset needs %d bytes on %s, %d are free" % (need, self.device, free))
         try:
             self.obs = torch.from_numpy(obs).to(self.device)
-            self.action = torch.from_numpy(act.astype(np.int32)).to(self.device)
+            self.action = torch.from_numpy(act).to(self.device)
             self.reward = torch.from_numpy(np.asarray(dataset["rewards"], dtype=np.float32).reshape(N)).to(self.device)
             self.terminal = torch.from_numpy((np.asarray(dataset["terminals"]).reshape(N) != 0).astype(np.uint8)).to(self.device)
             if self.device.type == "cuda":
@@ -157,11 +174,24 @@ class DeviceDataset(object):
         e = self.transitions[pos]
         return self.obs[e], self.action[e], self.reward[e + 1], self.obs[e + 1], self.terminal[e + 1]
 
+    def c_data(self):
+        """The r4_cqlc_data structure of a continuous dataset (r4_cqlc_* and r4_bcqc_*)."""
+        return _capi.CQLContiData(self.obs.data_ptr(), self.action.data_ptr(), self.reward.data_ptr(),
+                                  self.terminal.data_ptr(), self.transitions.data_ptr())
 
-class BatchRLModel(object):
-    """d3rlpy AlgoBase's surface the scripts use, over policy.BatchRLNet (CPU) or the r4_batchrl_* kernels (CUDA)."""
+
+class BatchRLBase(object):
+    """d3rlpy AlgoBase's surface the scripts use (fit, save_model, load_model, predict, predict_value), shared by the
+    discrete and continuous learners.  A family supplies its twin net (_new_net), its kernels' shape checks
+    (_scratch_size), its hyper-parameters (_hyper, _hyper_c), one epoch and one gradient through its entry points
+    (_epoch_call, grad_kernels), one twin step (train_step_twin), act, STAT_NAMES and its checkpoint keys (CKPT_ACTION,
+    _extra_state / _load_extra)."""
 
     algo = None
+    continuous = False
+    STAT_NAMES = ()
+    PREFIX = None
+    CKPT_ACTION = None              # (the checkpoint key of the action shape, the attribute holding it, its unit)
 
     def __init__(self, config, device=None, seed=0, use_kernels=None, **overrides):
         self.config = dict(config)
@@ -171,10 +201,6 @@ class BatchRLModel(object):
             device = "cuda" if torch.cuda.is_available() and config.get("gpu", True) else "cpu"
         self.device = torch.device(device)
         self.use_kernels = (self.device.type == "cuda") if use_kernels is None else bool(use_kernels)
-        self.A = int(config.get("action_size", 284))
-        if int(config.get("page_items", 9)) != 9:
-            raise ValueError("the custom encoder reads 9 prev actions (page_items = 9)")
-        self.location_mask, self.special_items = _masks(config, self.A)
         self.seed = seed
         self.net = None
         self.reward_mean, self.reward_std = 0.0, 1.0
@@ -184,23 +210,17 @@ class BatchRLModel(object):
 
     # ---- building ------------------------------------------------------------------------------------
     def create_impl(self, obs_dim):
-        self.net = BatchRLNet(self.algo, obs_dim, self.location_mask, self.special_items, self.A, self.device, self.seed)
+        self.net = self._new_net(obs_dim)
         z = lambda: torch.zeros(self.net.n_params, dtype=torch.float32, device=self.device)
         self.m, self.v = z(), z()
         self.step = 0
         self._gen = torch.Generator(device=self.device).manual_seed(self.seed)
         if self.use_kernels:
             self.lib = _capi.load_library()
-            k = ALGOS[self.algo]
-            assert self.lib.r4_batchrl_num_params(k, obs_dim, self.A) == self.net.n_params
-            assert self.lib.r4_batchrl_target_size(k, obs_dim, self.A) == self.net.n_target
+            n = self._scratch_size(obs_dim)
             self.grad = z()
-            self.stats = torch.zeros(3, dtype=torch.float32, device=self.device)
-            n = self.lib.r4_batchrl_scratch_size(k, obs_dim, self.A, self.batch_size)
-            if n < 0:
-                raise ValueError("obs_dim %d / action_size %d is outside the kernels' range" % (obs_dim, self.A))
+            self.stats = torch.zeros(len(self.STAT_NAMES), dtype=torch.float32, device=self.device)
             self.scratch = torch.zeros(n, dtype=torch.float32, device=self.device)
-            self._tables = BatchRLDataPtrs(self.net)
 
     def build_with_dataset(self, dataset):
         obs = dataset["observations"]
@@ -217,32 +237,32 @@ class BatchRLModel(object):
         self.reward_mean, self.reward_std = float(r.mean()), float(r.std())
         self.reward_scaler = "standard"
 
-    def _hyper(self):
-        hp = self.hp
-        return {"gamma": float(hp.get("gamma", 0.0)), "beta": float(hp.get("beta", 0.0)), "alpha": float(hp.get("alpha", 0.0)),
-                "log_flex": float(np.float32(math.log(hp.get("action_flexibility", 0.3)))),
-                "reward_mean": self.reward_mean if self.reward_scaler else 0.0,
+    def _reward_norm(self):
+        """The reward normalisation the losses apply, r -> (r - reward_mean) / reward_den (identity without a scaler)."""
+        return {"reward_mean": self.reward_mean if self.reward_scaler else 0.0,
                 "reward_den": (self.reward_std + 1e-3) if self.reward_scaler else 1.0}
 
     # ---- training ------------------------------------------------------------------------------------
     def _device_data(self, dataset):
         if self._data_src is not dataset:
             self._data = None                       # release the previous upload first
-            self._data = DeviceDataset(dataset, self.device)
+            self._data = DeviceDataset(dataset, self.device, self.continuous)
             self._data_src = dataset
         return self._data
 
     def fit(self, dataset, n_epochs=1, eval_episodes=None, show_progress=False, **kwargs):
         """d3rlpy fit with its RoundIterator: per epoch one permutation of the transitions (drawn on the device) and
         floor(n / batch_size) minibatches in order.  eval_episodes is accepted and not scored (no scorers are passed).
-        CQL's reward scaler is fitted here only when it has not been fitted yet (on the first dataset, or by
+        A standard reward scaler is fitted here only when it has not been fitted yet (on the first dataset, or by
         build_with_dataset): a later fit on another dataset keeps those statistics; build_with_dataset refits them.
-        Returns [(epoch, {'loss', 'td' or 'nll', 'q' or 'penalty'})]."""
-        if self.net is None or self.net.K != dataset["observations"].shape[1]:
+        Returns [(epoch, {STAT_NAMES: the epoch's means})]."""
+        data = self._device_data(dataset)
+        if self.continuous and data.D != self.D:
+            raise ValueError("the dataset's actions have %d dims, the model %d" % (data.D, self.D))
+        if self.net is None or self.net.K != data.K:
             self.build_with_dataset(dataset)
         elif self.hp.get("reward_scaler") == "standard" and self.reward_scaler is None:
             self.fit_reward_scaler(dataset)
-        data = self._device_data(dataset)
         mb = self.batch_size
         if data.n < mb:
             raise ValueError("the dataset has %d transitions, fewer than one minibatch of %d" % (data.n, mb))
@@ -250,21 +270,115 @@ class BatchRLModel(object):
         for epoch in range(1, int(n_epochs) + 1):
             perm = torch.randperm(data.n, generator=self._gen, device=self.device)
             st = self._epoch_kernels(data, perm) if self.use_kernels else self._epoch_twin(data, perm)
-            names = ("loss", "nll", "penalty") if self.algo == "BC" else ("loss", "td", "q")
-            out.append((epoch, dict(zip(names, st))))
+            out.append((epoch, dict(zip(self.STAT_NAMES, st))))
             if show_progress:
                 print("epoch %d %s" % (epoch, out[-1][1]))
         return out
 
     def _epoch_twin(self, data, perm):
-        hp, mb = self._hyper(), self.batch_size
-        acc = torch.zeros(3, dtype=torch.float64)
-        steps = data.n // mb
+        mb, steps = self.batch_size, data.n // self.batch_size
+        acc = torch.zeros(len(self.STAT_NAMES), dtype=torch.float64)
         for k in range(steps):
-            self.train_step_twin(data.batch(perm[k * mb:(k + 1) * mb]), hp)
-            acc += self._last_stats.double().cpu()
+            acc += self.train_step_twin(data.batch(perm[k * mb:(k + 1) * mb])).double().cpu()
         return [float(v) for v in acc / max(steps, 1)]
 
+    def _epoch_kernels(self, data, perm):
+        steps, nst = data.n // self.batch_size, len(self.STAT_NAMES)
+        stats = torch.zeros(steps * nst, dtype=torch.float32, device=self.device)
+        rc = self._epoch_call(data, perm, stats)
+        if rc < 0:
+            self._check(rc, self.PREFIX + "_epoch")
+        self.step += rc
+        return [float(v) for v in stats.view(steps, nst).double().mean(0)]
+
+    def _stream(self):
+        return _capi.stream(self.device)
+
+    def _check(self, rc, what):
+        _capi.check(self.lib, None, rc, what)
+
+    # ---- acting --------------------------------------------------------------------------------------
+    def _obs(self, obs):
+        """Observations (numpy or torch, f32 or f64 [n, K]) as a contiguous device tensor, f32 or f64."""
+        x = torch.as_tensor(obs, device=self.device)
+        if x.dtype not in (torch.float32, torch.float64):
+            x = x.to(torch.float32)
+        return x.reshape(-1, self.net.K).contiguous()
+
+    # ---- checkpoints ---------------------------------------------------------------------------------
+    def save_model(self, fname):
+        """torch.save of every network (the flat vector), the target, the Adam moments, the step counter, the reward
+        scaler and the family's own keys (_extra_state), so a loaded model predicts and continues fit as the saved one
+        would."""
+        key, attr, _ = self.CKPT_ACTION
+        torch.save(dict({"algo": self.algo, "obs_dim": self.net.K, key: getattr(self, attr),
+                         "params": self.net.flat.detach().cpu(), "target": self.net.target.cpu(), "m": self.m.cpu(),
+                         "v": self.v.cpu(), "step": self.step, "reward_scaler": self.reward_scaler,
+                         "reward_mean": self.reward_mean, "reward_std": self.reward_std}, **self._extra_state()), fname)
+
+    def load_model(self, fname):
+        ck = torch.load(fname, map_location="cpu")
+        key, attr, unit = self.CKPT_ACTION
+        if ck["algo"] != self.algo or ck.get(key) != getattr(self, attr):
+            raise ValueError("%s holds a %s model for %d %s" % (fname, ck["algo"], ck.get(key, -1), unit))
+        if self.net is None or self.net.K != ck["obs_dim"]:
+            self.create_impl(ck["obs_dim"])
+        with torch.no_grad():
+            for dst, k in ((self.net.flat, "params"), (self.net.target, "target"), (self.m, "m"), (self.v, "v")):
+                dst.copy_(ck[k].to(self.device))
+        self.step = int(ck["step"])
+        self.reward_scaler, self.reward_mean, self.reward_std = ck["reward_scaler"], ck["reward_mean"], ck["reward_std"]
+        self._load_extra(ck)
+
+    def _extra_state(self):
+        return {}
+
+    def _load_extra(self, ck):
+        pass
+
+
+class BatchRLModel(BatchRLBase):
+    """The discrete learners over policy.BatchRLNet (CPU) or the r4_batchrl_* kernels (CUDA)."""
+
+    STAT_NAMES = ("loss", "td", "q")
+    PREFIX = "r4_batchrl"
+    CKPT_ACTION = ("action_size", "A", "actions")
+
+    def __init__(self, config, **kw):
+        super(BatchRLModel, self).__init__(config, **kw)
+        self.A = int(config.get("action_size", 284))
+        if int(config.get("page_items", 9)) != 9:
+            raise ValueError("the custom encoder reads 9 prev actions (page_items = 9)")
+        self.location_mask, self.special_items = _masks(config, self.A)
+
+    # ---- building ------------------------------------------------------------------------------------
+    def _new_net(self, obs_dim):
+        return BatchRLNet(self.algo, obs_dim, self.location_mask, self.special_items, self.A, self.device, self.seed)
+
+    def _scratch_size(self, obs_dim):
+        k = ALGOS[self.algo]
+        assert self.lib.r4_batchrl_num_params(k, obs_dim, self.A) == self.net.n_params
+        assert self.lib.r4_batchrl_target_size(k, obs_dim, self.A) == self.net.n_target
+        n = self.lib.r4_batchrl_scratch_size(k, obs_dim, self.A, self.batch_size)
+        if n < 0:
+            raise ValueError("obs_dim %d / action_size %d is outside the kernels' range" % (obs_dim, self.A))
+        return n
+
+    @property
+    def _tables(self):
+        return BatchRLDataPtrs(self.net)
+
+    def _hyper(self):
+        hp = self.hp
+        return dict({"gamma": float(hp.get("gamma", 0.0)), "beta": float(hp.get("beta", 0.0)),
+                     "alpha": float(hp.get("alpha", 0.0)),
+                     "log_flex": float(np.float32(math.log(hp.get("action_flexibility", 0.3))))}, **self._reward_norm())
+
+    def _hyper_c(self):
+        h = self._hyper()
+        return _capi.BatchRLHyper(h["gamma"], h["beta"], h["alpha"], h["log_flex"], h["reward_mean"], h["reward_den"])
+
+    # ---- training ------------------------------------------------------------------------------------
     def train_step_twin(self, batch, hp=None):
         """One SGD step of the twin: autograd gradient, the kernels' Adam, the hard target copy when due."""
         hp = hp or self._hyper()
@@ -285,29 +399,13 @@ class BatchRLModel(object):
         ti = int(self.hp.get("target_update_interval", 0))
         return self.net.n_target > 0 and ti > 0 and (step - 1) % ti == 0
 
-    def _epoch_kernels(self, data, perm):
-        mb = self.batch_size
-        steps = data.n // mb
-        stats = torch.zeros(steps * 3, dtype=torch.float32, device=self.device)
-        rc = self.lib.r4_batchrl_epoch(ALGOS[self.algo], self.net.K, self.A, ptr(self.net.flat), ptr(self.net.target),
-                                       ptr(self.m), ptr(self.v), C.byref(self._tables.data(data)), C.byref(self._hyper_c()),
-                                       ptr(perm), perm.numel(), mb, self.step, self.hp["learning_rate"], self.hp["eps"],
-                                       int(self.hp.get("target_update_interval", 0)), ptr(self.scratch), ptr(stats),
-                                       self._stream())
-        if rc < 0:
-            self._check(rc, "r4_batchrl_epoch")
-        self.step += rc
-        return [float(v) for v in stats.view(steps, 3).double().mean(0)]
-
-    def _hyper_c(self):
-        h = self._hyper()
-        return _capi.BatchRLHyper(h["gamma"], h["beta"], h["alpha"], h["log_flex"], h["reward_mean"], h["reward_den"])
-
-    def _stream(self):
-        return _capi.stream(self.device)
-
-    def _check(self, rc, what):
-        _capi.check(self.lib, None, rc, what)
+    def _epoch_call(self, data, perm, stats):
+        return self.lib.r4_batchrl_epoch(ALGOS[self.algo], self.net.K, self.A, ptr(self.net.flat), ptr(self.net.target),
+                                         ptr(self.m), ptr(self.v), C.byref(self._tables.data(data)),
+                                         C.byref(self._hyper_c()), ptr(perm), perm.numel(), self.batch_size, self.step,
+                                         self.hp["learning_rate"], self.hp["eps"],
+                                         int(self.hp.get("target_update_interval", 0)), ptr(self.scratch), ptr(stats),
+                                         self._stream())
 
     def grad_kernels(self, data, pos):
         """r4_batchrl_grad over the transitions at positions pos (i64, device) -> self.grad, self.stats."""
@@ -320,10 +418,7 @@ class BatchRLModel(object):
     def act(self, obs, mode=0, want_probs=False, want_values=False):
         """The act rule on observations (numpy or torch, f32 or f64 [n, K]) -> (action i32 [n], probs or None, values or
         None) as device tensors.  mode 0: predict_with_mask's rule; mode 1: d3rlpy's predict."""
-        x = torch.as_tensor(obs, device=self.device)
-        if x.dtype not in (torch.float32, torch.float64):
-            x = x.to(torch.float32)
-        x = x.reshape(-1, self.net.K).contiguous()
+        x = self._obs(obs)
         log_flex = self._hyper()["log_flex"]
         if not self.use_kernels:
             a, probs, raw = self.net.act(x, mode, log_flex)
@@ -348,31 +443,10 @@ class BatchRLModel(object):
         a = torch.as_tensor(np.asarray(action), device=self.device).long().reshape(-1)
         return vals[torch.arange(vals.shape[0], device=self.device), a].cpu().numpy()
 
-    # ---- checkpoints ---------------------------------------------------------------------------------
-    def save_model(self, fname):
-        """torch.save of the flat parameters, the target, the Adam moments, the step counter and the reward scaler."""
-        torch.save({"algo": self.algo, "obs_dim": self.net.K, "action_size": self.A, "params": self.net.flat.detach().cpu(),
-                    "target": self.net.target.cpu(), "m": self.m.cpu(), "v": self.v.cpu(), "step": self.step,
-                    "reward_scaler": self.reward_scaler, "reward_mean": self.reward_mean, "reward_std": self.reward_std},
-                   fname)
-
-    def load_model(self, fname):
-        ck = torch.load(fname, map_location="cpu")
-        if ck["algo"] != self.algo or ck["action_size"] != self.A:
-            raise ValueError("%s holds a %s model for %d actions" % (fname, ck["algo"], ck["action_size"]))
-        if self.net is None or self.net.K != ck["obs_dim"]:
-            self.create_impl(ck["obs_dim"])
-        with torch.no_grad():
-            self.net.flat.copy_(ck["params"].to(self.device))
-            self.net.target.copy_(ck["target"].to(self.device))
-            self.m.copy_(ck["m"].to(self.device))
-            self.v.copy_(ck["v"].to(self.device))
-        self.step = int(ck["step"])
-        self.reward_scaler, self.reward_mean, self.reward_std = ck["reward_scaler"], ck["reward_mean"], ck["reward_std"]
-
 
 class DiscreteBC(BatchRLModel):
     algo = "BC"
+    STAT_NAMES = ("loss", "nll", "penalty")
 
 
 class DiscreteBCQ(BatchRLModel):
@@ -383,86 +457,32 @@ class DiscreteCQL(BatchRLModel):
     algo = "CQL"
 
 
-class ContiDeviceDataset(object):
-    """The continuous dataset where the learner runs: obs f32 [N, K], action f32 [N, D] (the logged items' embeddings,
-    not clipped), reward f32 [N], terminal u8 [N] and the transition entries i64 [T] (r4_batchrl_transitions).  On CUDA
-    it is uploaded once; a dataset that does not fit raises MemoryError."""
-
-    def __init__(self, dataset, device):
-        obs = np.asarray(dataset["observations"], dtype=np.float32)
-        N = obs.shape[0]
-        act = np.asarray(dataset["actions"], dtype=np.float32)
-        discrete = np.asarray(dataset.get("discrete_action", act.ndim < 2 or act.shape[1] == 1)).item()
-        if discrete or act.ndim != 2 or act.shape[0] != N:
-            raise ValueError("continuous batch RL needs the continuous dataset (actions f32 [N, D], discrete_action "
-                             "False): data_generate_rl4rs_a_conti / _b_conti")
-        self.device, self.N, self.K, self.D = torch.device(device), N, obs.shape[1], act.shape[1]
-        need = N * (self.K * 4 + self.D * 4 + 4 + 1 + 8)
-        if self.device.type == "cuda":
-            free = torch.cuda.mem_get_info(self.device)[0]
-            if need > free:
-                raise MemoryError("the dataset needs %d bytes on %s, %d are free" % (need, self.device, free))
-        try:
-            self.obs = torch.from_numpy(obs).to(self.device)
-            self.action = torch.from_numpy(act).to(self.device)
-            self.reward = torch.from_numpy(np.asarray(dataset["rewards"], dtype=np.float32).reshape(N)).to(self.device)
-            self.terminal = torch.from_numpy((np.asarray(dataset["terminals"]).reshape(N) != 0).astype(np.uint8)).to(self.device)
-            if self.device.type == "cuda":
-                lib = _capi.load_library()
-                index = torch.empty(N, dtype=torch.int64, device=self.device)
-                count = torch.zeros(1, dtype=torch.int64, device=self.device)
-                rc = lib.r4_batchrl_transitions(ptr(self.terminal), N, ptr(index), ptr(count), _capi.stream(self.device))
-                _capi.check(lib, None, rc, "r4_batchrl_transitions")
-                self.transitions = index[:int(count)]
-            else:
-                self.transitions = transitions_host(self.terminal)
-        except torch.OutOfMemoryError as exc:
-            raise MemoryError("the dataset needs %d bytes on %s: %s" % (need, self.device, exc)) from exc
-        self.n = int(self.transitions.numel())
-
-    batch = DeviceDataset.batch
-
-    def c_data(self):
-        return _capi.CQLContiData(self.obs.data_ptr(), self.action.data_ptr(), self.reward.data_ptr(),
-                                  self.terminal.data_ptr(), self.transitions.data_ptr())
-
-
-class ContinuousCQL(object):
-    """d3rlpy 0.91 CQL (continuous actions) as batchrl_trainer.py:61-73 configures 'CQL-conti', with d3rlpy AlgoBase's
-    surface the scripts call, over policy.BatchRLContiNet (CPU) or the r4_cqlc_* kernels (CUDA).  One SGD step updates the
-    temperature, alpha, the critics and the actor in that order, each with its own Adam, then the critics' soft target.
-    The noise of step t is keyed by (seed, t) (policy.cqlc_draws), so the CPU and CUDA paths draw the same numbers."""
+class ContinuousCQL(BatchRLBase):
+    """d3rlpy 0.91 CQL (continuous actions) as batchrl_trainer.py:61-73 configures 'CQL-conti', over
+    policy.BatchRLContiNet (CPU) or the r4_cqlc_* kernels (CUDA).  One SGD step updates the temperature, alpha, the
+    critics and the actor in that order, each with its own Adam, then the critics' soft target.  The noise of step t is
+    keyed by (seed, t) (policy.cqlc_draws), so the CPU and CUDA paths draw the same numbers.  Its checkpoint also holds
+    the act counter and the epoch-permutation generator's state."""
 
     algo = "CQL-conti"
+    continuous = True
     PREFIX = "r4_cqlc"
     STAT_NAMES = ("critic_loss", "actor_loss", "temp_loss", "alpha_loss", "q")
+    CKPT_ACTION = ("action_dim", "D", "action dims")
     # (loss, learning-rate key, its stats slots), in update order; the soft target update follows SOFT_AFTER's update
     PHASES = (("temp", "temp_learning_rate", (2,)), ("alpha", "alpha_learning_rate", (3,)),
               ("critic", "critic_learning_rate", (0, 4)), ("actor", "actor_learning_rate", (1,)))
     SOFT_AFTER = "critic"
 
-    def __init__(self, config, device=None, seed=0, use_kernels=None, **overrides):
-        self.config = dict(config)
-        self.hp = dict(DEFAULTS[self.algo], **overrides)
+    def __init__(self, config, **kw):
+        super(ContinuousCQL, self).__init__(config, **kw)
         if self.hp.get("soft_q_backup"):
             raise NotImplementedError("CQL-conti: soft_q_backup is not built (the script leaves it False)")
-        self.batch_size = int(self.hp["batch_size"])
-        if device is None:
-            device = "cuda" if torch.cuda.is_available() and config.get("gpu", True) else "cpu"
-        self.device = torch.device(device)
-        self.use_kernels = (self.device.type == "cuda") if use_kernels is None else bool(use_kernels)
         onehot = config.get("support_onehot_action", False)
         self.D = int(config.get("action_size", 284)) if onehot else int(config.get("action_emb_size", 32))
-        self.seed = seed
-        self.net = None
-        self.reward_mean, self.reward_std = 0.0, 1.0
-        self.reward_scaler = None
-        self._data, self._data_src = None, None
-        self.step = 0
         self.act_counter = 0
 
-    fit_reward_scaler = BatchRLModel.fit_reward_scaler
-
+    # ---- building ------------------------------------------------------------------------------------
     def _new_net(self, obs_dim):
         hp = self.hp
         return BatchRLContiNet(obs_dim, self.D, self.device, self.seed, hp["initial_temperature"], hp["initial_alpha"])
@@ -471,43 +491,28 @@ class ContinuousCQL(object):
         """The leading shape arguments of the r4_*_num_params / _target_size / _scratch_size calls."""
         return (K, self.D)
 
-    def create_impl(self, obs_dim):
-        hp = self.hp
-        self.net = self._new_net(obs_dim)
-        z = lambda: torch.zeros(self.net.n_params, dtype=torch.float32, device=self.device)
-        self.m, self.v = z(), z()
-        self.step = 0
-        self._gen = torch.Generator(device=self.device).manual_seed(self.seed)
-        if self.use_kernels:
-            self.lib = _capi.load_library()
-            K, D, dims = obs_dim, self.D, self._dims(obs_dim)
-            if getattr(self.lib, self.PREFIX + "_num_params")(*dims) != self.net.n_params:
-                raise ValueError("obs_dim %d / action_dim %d is outside the kernels' range" % (K, D))
-            assert getattr(self.lib, self.PREFIX + "_target_size")(*dims) == self.net.n_target
-            self.grad = z()
-            self.stats = torch.zeros(5, dtype=torch.float32, device=self.device)
-            n = getattr(self.lib, self.PREFIX + "_scratch_size")(*dims, int(hp["n_action_samples"]), self.batch_size)
-            if n < 0:
-                raise ValueError("batch_size %d / n_action_samples %d is outside the kernels' range"
-                                 % (self.batch_size, hp["n_action_samples"]))
-            self.scratch = torch.zeros(n, dtype=torch.float32, device=self.device)
+    def _scratch_size(self, obs_dim):
+        dims = self._dims(obs_dim)
+        if getattr(self.lib, self.PREFIX + "_num_params")(*dims) != self.net.n_params:
+            raise ValueError("obs_dim %d / action_dim %d is outside the kernels' range" % (obs_dim, self.D))
+        assert getattr(self.lib, self.PREFIX + "_target_size")(*dims) == self.net.n_target
+        n = getattr(self.lib, self.PREFIX + "_scratch_size")(*dims, int(self.hp["n_action_samples"]), self.batch_size)
+        if n < 0:
+            raise ValueError("batch_size %d / n_action_samples %d is outside the kernels' range"
+                             % (self.batch_size, self.hp["n_action_samples"]))
+        return n
 
     def build_with_dataset(self, dataset):
-        obs, act = dataset["observations"], np.asarray(dataset["actions"])
+        act = np.asarray(dataset["actions"])
         if act.ndim != 2 or act.shape[1] != self.D:
             raise ValueError("the dataset's actions have shape %s, the model takes [N, %d] (action_emb_size, or "
                              "action_size with support_onehot_action)" % (act.shape, self.D))
-        if self.net is None or self.net.K != obs.shape[1]:
-            self.create_impl(obs.shape[1])
-        if self.hp.get("reward_scaler") == "standard":
-            self.fit_reward_scaler(dataset)
+        super(ContinuousCQL, self).build_with_dataset(dataset)
 
     def _hyper(self):
         hp = self.hp
-        return {"gamma": float(hp["gamma"]), "tau": float(hp["tau"]), "alpha_threshold": float(hp["alpha_threshold"]),
-                "conservative_weight": float(hp["conservative_weight"]),
-                "reward_mean": self.reward_mean if self.reward_scaler else 0.0,
-                "reward_den": (self.reward_std + 1e-3) if self.reward_scaler else 1.0}
+        return dict({"gamma": float(hp["gamma"]), "tau": float(hp["tau"]), "alpha_threshold": float(hp["alpha_threshold"]),
+                     "conservative_weight": float(hp["conservative_weight"])}, **self._reward_norm())
 
     def _hyper_c(self):
         h, hp = self._hyper(), self.hp
@@ -517,44 +522,6 @@ class ContinuousCQL(object):
                                    self.seed)
 
     # ---- training ------------------------------------------------------------------------------------
-    def _device_data(self, dataset):
-        if self._data_src is not dataset:
-            self._data = None
-            self._data = ContiDeviceDataset(dataset, self.device)
-            self._data_src = dataset
-        return self._data
-
-    def fit(self, dataset, n_epochs=1, eval_episodes=None, show_progress=False, **kwargs):
-        """d3rlpy fit with its RoundIterator (one device permutation per epoch, floor(n / batch_size) minibatches).
-        eval_episodes is accepted and not scored.  The reward scaler as in the discrete models.  Returns
-        [(epoch, {STAT_NAMES: the epoch's means})]."""
-        data = self._device_data(dataset)
-        if data.D != self.D:
-            raise ValueError("the dataset's actions have %d dims, the model %d" % (data.D, self.D))
-        if self.net is None or self.net.K != data.K:
-            self.build_with_dataset(dataset)
-        elif self.hp.get("reward_scaler") == "standard" and self.reward_scaler is None:
-            self.fit_reward_scaler(dataset)
-        mb = self.batch_size
-        if data.n < mb:
-            raise ValueError("the dataset has %d transitions, fewer than one minibatch of %d" % (data.n, mb))
-        names = self.STAT_NAMES
-        out = []
-        for epoch in range(1, int(n_epochs) + 1):
-            perm = torch.randperm(data.n, generator=self._gen, device=self.device)
-            st = self._epoch_kernels(data, perm) if self.use_kernels else self._epoch_twin(data, perm)
-            out.append((epoch, dict(zip(names, st))))
-            if show_progress:
-                print("epoch %d %s" % (epoch, out[-1][1]))
-        return out
-
-    def _epoch_twin(self, data, perm):
-        mb, steps = self.batch_size, data.n // self.batch_size
-        acc = torch.zeros(5, dtype=torch.float64)
-        for k in range(steps):
-            acc += self.train_step_twin(data.batch(perm[k * mb:(k + 1) * mb])).double().cpu()
-        return [float(v) for v in acc / max(steps, 1)]
-
     def train_step_twin(self, batch):
         """One SGD step of the twin with the kernels' noise: the PHASES' updates in order (each loss at the parameters the
         earlier updates left), the soft target update after SOFT_AFTER's.  -> stats [5]."""
@@ -574,32 +541,24 @@ class ContinuousCQL(object):
         self._last_stats = st
         return st
 
-    def _epoch_kernels(self, data, perm):
-        mb = self.batch_size
-        steps = data.n // mb
-        stats = torch.zeros(steps * 5, dtype=torch.float32, device=self.device)
-        rc = getattr(self.lib, self.PREFIX + "_epoch")(self.net.K, self.D, ptr(self.net.flat), ptr(self.net.target), ptr(self.m),
-                                    ptr(self.v), C.byref(data.c_data()), C.byref(self._hyper_c()), ptr(perm),
-                                    perm.numel(), mb, self.step, ptr(self.scratch), ptr(stats), _capi.stream(self.device))
-        if rc < 0:
-            _capi.check(self.lib, None, rc, self.PREFIX + "_epoch")
-        self.step += rc
-        return [float(v) for v in stats.view(steps, 5).double().mean(0)]
+    def _epoch_call(self, data, perm, stats):
+        return getattr(self.lib, self.PREFIX + "_epoch")(self.net.K, self.D, ptr(self.net.flat), ptr(self.net.target),
+                                                          ptr(self.m), ptr(self.v), C.byref(data.c_data()),
+                                                          C.byref(self._hyper_c()), ptr(perm), perm.numel(),
+                                                          self.batch_size, self.step, ptr(self.scratch), ptr(stats),
+                                                          self._stream())
 
     def grad_kernels(self, data, pos, step=None):
         """r4_cqlc_grad / r4_bcqc_grad over the transitions at positions pos (i64, device) with the noise of `step`
         (default: the next step) -> self.grad, self.stats."""
         rc = getattr(self.lib, self.PREFIX + "_grad")(self.net.K, self.D, ptr(self.net.flat), ptr(self.net.target), C.byref(data.c_data()),
                                    C.byref(self._hyper_c()), ptr(pos), pos.numel(), self.step + 1 if step is None else step,
-                                   ptr(self.scratch), ptr(self.grad), ptr(self.stats), _capi.stream(self.device))
-        _capi.check(self.lib, None, rc, self.PREFIX + "_grad")
+                                   ptr(self.scratch), ptr(self.grad), ptr(self.stats), self._stream())
+        self._check(rc, self.PREFIX + "_grad")
 
     # ---- acting --------------------------------------------------------------------------------------
     def _act_inputs(self, obs, action):
-        x = torch.as_tensor(obs, device=self.device)
-        if x.dtype not in (torch.float32, torch.float64):
-            x = x.to(torch.float32)
-        x = x.reshape(-1, self.net.K).contiguous()
+        x = self._obs(obs)
         a_in = None if action is None else torch.as_tensor(np.asarray(action) if not torch.is_tensor(action) else action,
                                                              device=self.device, dtype=torch.float32).reshape(-1, self.D)
         return x, None if a_in is None else a_in.contiguous()
@@ -619,8 +578,8 @@ class ContinuousCQL(object):
         scratch = torch.empty(self.lib.r4_cqlc_act_scratch_size(self.net.K, self.D, n), dtype=torch.float32,
                               device=self.device)
         rc = self.lib.r4_cqlc_act(self.net.K, self.D, ptr(self.net.flat), ptr(x), int(x.dtype == torch.float64), n,
-                                  ptr(a_in), ptr(a), ptr(q), ptr(scratch), _capi.stream(self.device))
-        _capi.check(self.lib, None, rc, "r4_cqlc_act")
+                                  ptr(a_in), ptr(a), ptr(q), ptr(scratch), self._stream())
+        self._check(rc, "r4_cqlc_act")
         return a, q
 
     def predict(self, x):
@@ -632,28 +591,12 @@ class ContinuousCQL(object):
         return self.act(x, action, want_q=True)[1].cpu().numpy()
 
     # ---- checkpoints ---------------------------------------------------------------------------------
-    def save_model(self, fname):
-        """torch.save of every network (the flat vector: CQL's actor, critics, log_temp and log_alpha; BCQ's actor, critics
-        and VAE), the targets, the Adam moments, the step and act counters, the epoch-permutation generator's state and
-        the reward scaler, so a loaded model predicts and continues fit as the saved one would."""
-        torch.save({"algo": self.algo, "obs_dim": self.net.K, "action_dim": self.D, "params": self.net.flat.detach().cpu(),
-                    "target": self.net.target.cpu(), "m": self.m.cpu(), "v": self.v.cpu(), "step": self.step,
-                    "act_counter": self.act_counter, "gen": self._gen.get_state(),
-                    "reward_scaler": self.reward_scaler, "reward_mean": self.reward_mean, "reward_std": self.reward_std},
-                   fname)
+    def _extra_state(self):
+        return {"act_counter": self.act_counter, "gen": self._gen.get_state()}
 
-    def load_model(self, fname):
-        ck = torch.load(fname, map_location="cpu")
-        if ck["algo"] != self.algo or ck["action_dim"] != self.D:
-            raise ValueError("%s holds a %s model for %d action dims" % (fname, ck["algo"], ck.get("action_dim", -1)))
-        if self.net is None or self.net.K != ck["obs_dim"]:
-            self.create_impl(ck["obs_dim"])
-        with torch.no_grad():
-            for dst, key in ((self.net.flat, "params"), (self.net.target, "target"), (self.m, "m"), (self.v, "v")):
-                dst.copy_(ck[key].to(self.device))
-        self.step, self.act_counter = int(ck["step"]), int(ck["act_counter"])
+    def _load_extra(self, ck):
+        self.act_counter = int(ck["act_counter"])
         self._gen.set_state(ck["gen"])
-        self.reward_scaler, self.reward_mean, self.reward_std = ck["reward_scaler"], ck["reward_mean"], ck["reward_std"]
 
 
 class ContinuousBCQ(ContinuousCQL):
@@ -719,8 +662,8 @@ class ContinuousBCQ(ContinuousCQL):
         scratch = torch.empty(size, dtype=torch.float32, device=self.device)
         rc = self.lib.r4_bcqc_act(self.net.K, self.D, ptr(self.net.flat), ptr(x), int(x.dtype == torch.float64), n,
                                   C.byref(self._hyper_c()), self.act_counter, ptr(a_in), ptr(a), ptr(q), ptr(scratch),
-                                  _capi.stream(self.device))
-        _capi.check(self.lib, None, rc, "r4_bcqc_act")
+                                  self._stream())
+        self._check(rc, "r4_bcqc_act")
         return a, q
 
 
@@ -769,7 +712,7 @@ class policy_model(object):
         support_conti_env it is predict (policy_model.py:18-19); a continuous model then returns device actions
         f32 [n, D] for a device tensor."""
         if self.config.get("support_conti_env", False):
-            if hasattr(obs, "is_cuda") and isinstance(self.policy, ContinuousCQL):     # ContinuousBCQ too
+            if hasattr(obs, "is_cuda") and self.policy.continuous:
                 return self.policy.act(obs)[0]
             return self.predict(obs)
         a = self.policy.act(obs, 0)[0]

@@ -674,7 +674,34 @@ int r4_rainbow_train_step(r4_comm* comm, float* params, float* target, float* m,
   return r4_replay_update_priorities(r_prio, max_prio, P.idx, P.td, n, alpha, prio_eps, stream);
 }
 
+}  // extern "C"
+
 // ---- batch RL: discrete BC / BCQ / CQL (r4_batchrl.cuh) -----------------------------------------------------------
+namespace {
+// The epoch of every batch-RL family: n_perm / mb SGD steps, step k (1-based step0 + k + 1) on the rows perm[k mb, (k + 1)
+// mb) with its statistics at stats + nstat k.  -> the number of steps.
+template <typename Step>
+int batchrl_epoch(const char* fn, const int64_t* perm, int64_t n_perm, int mb, int step0, float* stats, int nstat,
+                  Step&& sgd_step) {
+  const int64_t steps = n_perm / mb;
+  if (steps > (int64_t)0x7fffffff - step0) return fail(R4_ERR_ARG, std::string(fn) + ": too many steps");
+  for (int64_t k = 0; k < steps; ++k) {
+    const int rc = sgd_step(perm + k * mb, step0 + (int)k + 1, stats ? stats + nstat * k : nullptr);
+    if (rc) return rc;
+  }
+  return (int)steps;
+}
+
+// the dataset planes of both continuous families (r4_cqlc_data) as their kernels take them; false when one is missing
+bool conti_data(const r4_cqlc_data* d, r4cqlc::Data* out) {
+  if (!d || !d->obs || !d->action || !d->reward || !d->terminal || !d->transitions) return false;
+  *out = r4cqlc::Data{d->obs, d->action, d->reward, d->terminal, d->transitions};
+  return true;
+}
+}  // namespace
+
+extern "C" {
+
 int64_t r4_batchrl_launch_count(void) { return g_launches[FAM_BATCHRL].load(std::memory_order_relaxed); }
 
 int r4_batchrl_num_params(int algo, int obs_dim, int action_size) {
@@ -756,20 +783,14 @@ int r4_batchrl_epoch(int algo, int obs_dim, int action_size, float* params, floa
   if (!r4bq::dims_ok(algo, obs_dim, action_size) || !params || (algo != r4bq::BC && !target) || !m || !v || !bq_data_ok(data) ||
       !hp || !perm || n_perm < 1 || mb < 1 || step0 < 0 || !scratch)
     return fail(R4_ERR_ARG, "r4_batchrl_epoch: bad argument");
-  const int64_t steps = n_perm / mb;
-  if (steps > (int64_t)0x7fffffff - step0) return fail(R4_ERR_ARG, "r4_batchrl_epoch: too many steps");
   const r4bq::Layout L = r4bq::make_layout(algo, obs_dim, action_size);
   float* grad = r4bq::make_planes(scratch, L, mb).grad;
   cudaStream_t st = S(stream);
-  for (int64_t k = 0; k < steps; ++k) {
-    const int step = step0 + (int)k + 1;
+  return batchrl_epoch("r4_batchrl_epoch", perm, n_perm, mb, step0, stats, 3, [&](const int64_t* idx, int step, float* sk) {
     const int copy = L.ntgt > 0 && target_interval > 0 && (step - 1) % target_interval == 0;
-    int rc = bq_grad(algo, obs_dim, action_size, params, target, data, hp, perm + k * mb, mb, scratch, grad,
-                     stats ? stats + 3 * k : nullptr, st, true);
-    if (rc) return rc;
-    if ((rc = bq_apply(algo, obs_dim, action_size, params, target, grad, m, v, step, lr, adam_eps, copy, st, true))) return rc;
-  }
-  return (int)steps;
+    const int rc = bq_grad(algo, obs_dim, action_size, params, target, data, hp, idx, mb, scratch, grad, sk, st, true);
+    return rc ? rc : bq_apply(algo, obs_dim, action_size, params, target, grad, m, v, step, lr, adam_eps, copy, st, true);
+  });
 }
 
 int r4_batchrl_act(int algo, int obs_dim, int action_size, const float* params, const void* obs, int obs_f64, int n,
@@ -901,9 +922,10 @@ r4cqlc::Hyper cq_hyper(const r4_cqlc_hyper* h, int D) {
                        h->reward_den, (float)((double)D * std::log(0.5)), h->lr_actor, h->lr_critic, h->lr_temp,
                        h->lr_alpha, h->n_action_samples, h->seed};
 }
-bool cq_args_ok(int K, int D, const r4_cqlc_data* d, const r4_cqlc_hyper* h, int n) {
-  return r4cqlc::dims_ok(K, D) && d && d->obs && d->action && d->reward && d->terminal && d->transitions && h &&
-         h->n_action_samples >= 1 && h->n_action_samples <= r4cqlc::MAXS && n >= 1 && n <= r4cqlc::MAXN;
+// the arguments r4_cqlc_grad and r4_cqlc_epoch share, and the dataset planes into *out
+bool cq_args_ok(int K, int D, const r4_cqlc_data* d, const r4_cqlc_hyper* h, int n, r4cqlc::Data* out) {
+  return r4cqlc::dims_ok(K, D) && conti_data(d, out) && h && h->n_action_samples >= 1 && h->n_action_samples <= r4cqlc::MAXS &&
+         n >= 1 && n <= r4cqlc::MAXN;
 }
 }  // namespace
 
@@ -932,12 +954,12 @@ int64_t r4_cqlc_act_scratch_size(int obs_dim, int action_dim, int n) {
 int r4_cqlc_grad(int obs_dim, int action_dim, const float* params, const float* target, const r4_cqlc_data* data,
                  const r4_cqlc_hyper* hp, const int64_t* idx, int n, int step, float* scratch, float* grad, float* stats,
                  void* stream) {
-  if (!cq_args_ok(obs_dim, action_dim, data, hp, n) || !params || !target || !idx || step < 1 || !scratch || !grad)
+  r4cqlc::Data D;
+  if (!cq_args_ok(obs_dim, action_dim, data, hp, n, &D) || !params || !target || !idx || step < 1 || !scratch || !grad)
     return fail(R4_ERR_ARG, "r4_cqlc_grad: bad argument (obs_dim 1..4096, action_dim 1..512, n 1..4096, samples 1..64)");
   const r4cqlc::Layout L = r4cqlc::make_layout(obs_dim, action_dim);
   r4cqlc::Planes P = r4cqlc::make_planes(scratch, L, hp->n_action_samples, n);
   P.grad = grad;
-  const r4cqlc::Data D{data->obs, data->action, data->reward, data->terminal, data->transitions};
   return cq_step(L, cq_hyper(hp, action_dim), const_cast<float*>(params), const_cast<float*>(target), nullptr, nullptr, D,
                  idx, n, step, 0, P, stats, S(stream), false);
 }
@@ -945,21 +967,17 @@ int r4_cqlc_grad(int obs_dim, int action_dim, const float* params, const float* 
 int r4_cqlc_epoch(int obs_dim, int action_dim, float* params, float* target, float* m, float* v, const r4_cqlc_data* data,
                   const r4_cqlc_hyper* hp, const int64_t* perm, int64_t n_perm, int mb, int step0, float* scratch,
                   float* stats, void* stream) {
-  if (!cq_args_ok(obs_dim, action_dim, data, hp, mb) || !params || !target || !m || !v || !perm || n_perm < 1 ||
+  r4cqlc::Data D;
+  if (!cq_args_ok(obs_dim, action_dim, data, hp, mb, &D) || !params || !target || !m || !v || !perm || n_perm < 1 ||
       step0 < 0 || !scratch)
     return fail(R4_ERR_ARG, "r4_cqlc_epoch: bad argument");
-  const int64_t steps = n_perm / mb;
-  if (steps > (int64_t)0x7fffffff - step0) return fail(R4_ERR_ARG, "r4_cqlc_epoch: too many steps");
   const r4cqlc::Layout L = r4cqlc::make_layout(obs_dim, action_dim);
   const r4cqlc::Planes P = r4cqlc::make_planes(scratch, L, hp->n_action_samples, mb);
-  const r4cqlc::Data D{data->obs, data->action, data->reward, data->terminal, data->transitions};
   const r4cqlc::Hyper h = cq_hyper(hp, action_dim);
-  for (int64_t k = 0; k < steps; ++k) {
-    const int rc = cq_step(L, h, params, target, m, v, D, perm + k * mb, mb, step0 + (int)k + 1, 1, P,
-                           stats ? stats + r4cqlc::NSTAT * k : nullptr, S(stream), true);
-    if (rc) return rc;
-  }
-  return (int)steps;
+  return batchrl_epoch("r4_cqlc_epoch", perm, n_perm, mb, step0, stats, r4cqlc::NSTAT,
+                       [&](const int64_t* idx, int step, float* sk) {
+                         return cq_step(L, h, params, target, m, v, D, idx, mb, step, 1, P, sk, S(stream), true);
+                       });
 }
 
 int r4_cqlc_act(int obs_dim, int action_dim, const float* params, const void* obs, int obs_f64, int n,
@@ -2004,9 +2022,10 @@ r4bcqc::Hyper bc_hyper(const r4_bcqc_hyper* h) {
   return r4bcqc::Hyper{h->gamma, h->tau, h->lam, h->beta, h->action_flexibility, h->adam_eps, h->reward_mean, h->reward_den,
                        h->lr_actor, h->lr_critic, h->lr_imitator, h->n_action_samples, h->seed};
 }
-bool bc_args_ok(int K, int D, const r4_cqlc_data* d, const r4_bcqc_hyper* h, int n) {
-  return h && r4bcqc::dims_ok(K, D, h->latent_size) && d && d->obs && d->action && d->reward && d->terminal &&
-         d->transitions && h->n_action_samples >= 1 && h->n_action_samples <= r4bcqc::MAXS && n >= 1 && n <= r4bcqc::MAXN;
+// the arguments r4_bcqc_grad and r4_bcqc_epoch share, and the dataset planes into *out
+bool bc_args_ok(int K, int D, const r4_cqlc_data* d, const r4_bcqc_hyper* h, int n, r4cqlc::Data* out) {
+  return h && r4bcqc::dims_ok(K, D, h->latent_size) && conti_data(d, out) && h->n_action_samples >= 1 &&
+         h->n_action_samples <= r4bcqc::MAXS && n >= 1 && n <= r4bcqc::MAXN;
 }
 }  // namespace
 
@@ -2037,13 +2056,13 @@ int64_t r4_bcqc_act_scratch_size(int obs_dim, int action_dim, int latent_size, i
 int r4_bcqc_grad(int obs_dim, int action_dim, const float* params, const float* target, const r4_cqlc_data* data,
                  const r4_bcqc_hyper* hp, const int64_t* idx, int n, int step, float* scratch, float* grad, float* stats,
                  void* stream) {
-  if (!bc_args_ok(obs_dim, action_dim, data, hp, n) || !params || !target || !idx || step < 1 || !scratch || !grad)
+  r4cqlc::Data D;
+  if (!bc_args_ok(obs_dim, action_dim, data, hp, n, &D) || !params || !target || !idx || step < 1 || !scratch || !grad)
     return fail(R4_ERR_ARG, "r4_bcqc_grad: bad argument (obs_dim 1..4096, action_dim 1..512, latent 1..512, n 1..4096, "
                             "samples 1..256)");
   const r4bcqc::Layout L = r4bcqc::make_layout(obs_dim, action_dim, hp->latent_size);
   r4bcqc::Planes P = r4bcqc::make_planes(scratch, L, hp->n_action_samples, n);
   P.grad = grad;
-  const r4cqlc::Data D{data->obs, data->action, data->reward, data->terminal, data->transitions};
   return bc_step(L, bc_hyper(hp), const_cast<float*>(params), const_cast<float*>(target), nullptr, nullptr, D, idx, n, step,
                  0, P, stats, S(stream), false);
 }
@@ -2051,21 +2070,17 @@ int r4_bcqc_grad(int obs_dim, int action_dim, const float* params, const float* 
 int r4_bcqc_epoch(int obs_dim, int action_dim, float* params, float* target, float* m, float* v, const r4_cqlc_data* data,
                   const r4_bcqc_hyper* hp, const int64_t* perm, int64_t n_perm, int mb, int step0, float* scratch,
                   float* stats, void* stream) {
-  if (!bc_args_ok(obs_dim, action_dim, data, hp, mb) || !params || !target || !m || !v || !perm || n_perm < 1 ||
+  r4cqlc::Data D;
+  if (!bc_args_ok(obs_dim, action_dim, data, hp, mb, &D) || !params || !target || !m || !v || !perm || n_perm < 1 ||
       step0 < 0 || !scratch)
     return fail(R4_ERR_ARG, "r4_bcqc_epoch: bad argument");
-  const int64_t steps = n_perm / mb;
-  if (steps > (int64_t)0x7fffffff - step0) return fail(R4_ERR_ARG, "r4_bcqc_epoch: too many steps");
   const r4bcqc::Layout L = r4bcqc::make_layout(obs_dim, action_dim, hp->latent_size);
   const r4bcqc::Planes P = r4bcqc::make_planes(scratch, L, hp->n_action_samples, mb);
-  const r4cqlc::Data D{data->obs, data->action, data->reward, data->terminal, data->transitions};
   const r4bcqc::Hyper h = bc_hyper(hp);
-  for (int64_t k = 0; k < steps; ++k) {
-    const int rc = bc_step(L, h, params, target, m, v, D, perm + k * mb, mb, step0 + (int)k + 1, 1, P,
-                           stats ? stats + r4bcqc::NSTAT * k : nullptr, S(stream), true);
-    if (rc) return rc;
-  }
-  return (int)steps;
+  return batchrl_epoch("r4_bcqc_epoch", perm, n_perm, mb, step0, stats, r4bcqc::NSTAT,
+                       [&](const int64_t* idx, int step, float* sk) {
+                         return bc_step(L, h, params, target, m, v, D, idx, mb, step, 1, P, sk, S(stream), true);
+                       });
 }
 
 int r4_bcqc_act(int obs_dim, int action_dim, const float* params, const void* obs, int obs_f64, int n,

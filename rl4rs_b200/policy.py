@@ -466,7 +466,47 @@ class RawStatePolicy(object):
     act, terms = MaskedPolicy.act, MaskedPolicy.terms
 
 
-class BatchRLNet(object):
+class BatchRLFlat(object):
+    """The flat parameter vector of the batch-RL twins, in their kernels' layout, and its named views."""
+
+    def _init_flat(self, shapes, seed, fixed=None):
+        """self.flat for `shapes` [(name, shape)] in layout order, drawn from a CPU generator seeded with `seed`: a name in
+        `fixed` is filled with its value and draws nothing, a name ending in 'emb' is drawn N(0, 1) (torch's Embedding),
+        the rest torch's default U(+-1/sqrt(fan_in)) (Linear), a bias with the fan of the weight before it."""
+        fixed = fixed or {}
+        n = sum(math.prod(s) for _, s in shapes)
+        g = torch.Generator(device="cpu").manual_seed(seed)
+        self.flat = torch.zeros(n, dtype=torch.float32, device=self.device, requires_grad=True)
+        off, fan = 0, 1
+        with torch.no_grad():
+            for name, shape in shapes:
+                k = math.prod(shape)
+                v = self.flat[off:off + k].view(shape)
+                if name in fixed:
+                    v.fill_(fixed[name])
+                elif name.endswith("emb"):
+                    v.copy_(torch.randn(shape, generator=g).to(self.device))
+                else:
+                    fan = shape[0] if len(shape) == 2 else fan          # a bias follows its weight
+                    bound = 1.0 / math.sqrt(fan)
+                    v.copy_(((torch.rand(shape, generator=g) * 2 - 1) * bound).to(self.device))
+                off += k
+        self._shapes, self.n_params = shapes, n
+
+    def params(self, flat=None):
+        """name -> its view of flat (default self.flat); a shorter vector (BCQ's target) gives the names it holds."""
+        flat = self.flat if flat is None else flat
+        out, off = {}, 0
+        for name, shape in self._shapes:
+            k = math.prod(shape)
+            if off + k > flat.numel():
+                break
+            out[name] = flat[off:off + k].view(shape)
+            off += k
+        return out
+
+
+class BatchRLNet(BatchRLFlat):
     """The networks of the discrete batch-RL learners (script/batchrl_trainer.py:34-90, d3rlpy 0.91 as the script configures
     it), in csrc/r4_batchrl.cuh's flat layout.  The masked net M (BC's imitator; BCQ's Q function and, separately, its
     imitator) is rl4rs/nets/cql/encoder.py CustomVectorEncoder with_q plus d3rlpy's Linear(A, A) head:
@@ -491,41 +531,14 @@ class BatchRLNet(object):
             return [(p + "w1", (K, H)), (p + "b1", (H,)), (p + "emb", (A, E)), (p + "w2", (H + W * E, A)), (p + "b2", (A,)),
                     (p + "w3", (A, A)), (p + "b3", (A,))]
         cnet = [("w1", (K, H)), ("b1", (H,)), ("w2", (H, H)), ("b2", (H,)), ("w3", (H, A)), ("b3", (A,))]
-        shapes = {"BC": mnet("i_"), "BCQ": mnet("q_") + mnet("i_"), "CQL": cnet}[algo]
-        n = sum(math.prod(s) for _, s in shapes)
-        self.n_target = {"BC": 0, "BCQ": n // 2, "CQL": n}[algo]
-        g = torch.Generator(device="cpu").manual_seed(seed)
-        self.flat = torch.zeros(n, dtype=torch.float32, device=self.device, requires_grad=True)
-        off, fan = 0, 1
-        with torch.no_grad():
-            for name, shape in shapes:
-                k = math.prod(shape)
-                v = self.flat[off:off + k].view(shape)
-                if name.endswith("emb"):
-                    v.copy_(torch.randn(shape, generator=g).to(self.device))
-                else:
-                    fan = shape[0] if len(shape) == 2 else fan          # a bias follows its weight
-                    bound = 1.0 / math.sqrt(fan)
-                    v.copy_(((torch.rand(shape, generator=g) * 2 - 1) * bound).to(self.device))
-                off += k
-        self._shapes, self.n_params = shapes, n
+        self._init_flat({"BC": mnet("i_"), "BCQ": mnet("q_") + mnet("i_"), "CQL": cnet}[algo], seed)
+        self.n_target = {"BC": 0, "BCQ": self.n_params // 2, "CQL": self.n_params}[algo]
         self.target = self.flat.detach()[:self.n_target].clone()
         lm = torch.as_tensor(np.asarray(location_mask)[:3] >= 0.01, dtype=torch.uint8)
         self.location_mask = lm.to(self.device)
         sp = torch.zeros(A, dtype=torch.uint8)
         sp[torch.as_tensor(np.asarray(list(special_items), dtype=np.int64))] = 1
         self.special = sp.to(self.device)
-
-    def params(self, flat=None):
-        flat = self.flat if flat is None else flat
-        out, off = {}, 0
-        for name, shape in self._shapes:
-            k = math.prod(shape)
-            if off + k > flat.numel():
-                break
-            out[name] = flat[off:off + k].view(shape)
-            off += k
-        return out
 
     def keep(self, x):
         """bool [n, A]: the custom encoder's mask (encoder.py:43-65), the same as the eval rule's (policy_model.py:24-33)."""
@@ -642,7 +655,7 @@ def cqlc_draws(seed, counter, stream, rows, samples, dims, uniform=None):
     return np.sqrt(-2.0 * np.log(u1)) * np.cos(2.0 * np.pi * u2)
 
 
-class BatchRLContiNet(object):
+class BatchRLContiNet(BatchRLFlat):
     """The networks of continuous-action CQL (script/batchrl_trainer.py:61-73 'CQL-conti', d3rlpy 0.91 CQL with its default
     VectorEncoderFactory), in csrc/r4_cqlconti.cuh's flat layout:
         actor     obs [K] -> 256 relu -> 256 relu -> [mu | logstd] [2D]   (SquashedNormalPolicy; logstd clamped to [-20, 2])
@@ -665,39 +678,14 @@ class BatchRLContiNet(object):
                     (p + "b3", (n_out,))]
         shapes = net("a_", K, 2 * D) + net("q0_", K + D, 1) + net("q1_", K + D, 1) + [("log_temp", (1,)),
                                                                                         ("log_alpha", (1,))]
-        n = sum(math.prod(s) for _, s in shapes)
-        g = torch.Generator(device="cpu").manual_seed(seed)
-        self.flat = torch.zeros(n, dtype=torch.float32, device=self.device, requires_grad=True)
-        off, fan = 0, 1
-        with torch.no_grad():
-            for name, shape in shapes:
-                k = math.prod(shape)
-                v = self.flat[off:off + k].view(shape)
-                if name == "log_temp":
-                    v.fill_(math.log(initial_temperature))
-                elif name == "log_alpha":
-                    v.fill_(math.log(initial_alpha))
-                else:
-                    fan = shape[0] if len(shape) == 2 else fan          # a bias follows its weight
-                    bound = 1.0 / math.sqrt(fan)
-                    v.copy_(((torch.rand(shape, generator=g) * 2 - 1) * bound).to(self.device))
-                off += k
-        self._shapes, self.n_params = shapes, n
+        self._init_flat(shapes, seed, {"log_temp": math.log(initial_temperature), "log_alpha": math.log(initial_alpha)})
+        n = self.n_params
         size = {name: math.prod(s) for name, s in shapes}
         self.n_actor = sum(v for k, v in size.items() if k.startswith("a_"))
         self.n_critic = sum(v for k, v in size.items() if k.startswith("q0_"))
         self.t0, self.n_target = self.n_actor, 2 * self.n_critic
         self.lt, self.la = n - 2, n - 1
         self.target = self.flat.detach()[self.t0:self.t0 + self.n_target].clone()
-
-    def params(self, flat=None):
-        flat = self.flat if flat is None else flat
-        out, off = {}, 0
-        for name, shape in self._shapes:
-            k = math.prod(shape)
-            out[name] = flat[off:off + k].view(shape)
-            off += k
-        return out
 
     def target_params(self, target=None, dtype=None):
         """The target critics as a params() dict (q0_*, q1_*)."""
@@ -843,18 +831,7 @@ class BatchRLContiBCQNet(BatchRLContiNet):
                     (p + "b3", (n_out,))]
         shapes = net("a_", K + D, D) + net("q0_", K + D, 1) + net("q1_", K + D, 1) + net("e_", K + D, 2 * L) + \
             net("d_", K + L, D)
-        n = sum(math.prod(s) for _, s in shapes)
-        g = torch.Generator(device="cpu").manual_seed(seed)
-        self.flat = torch.zeros(n, dtype=torch.float32, device=self.device, requires_grad=True)
-        off, fan = 0, 1
-        with torch.no_grad():
-            for name, shape in shapes:
-                k = math.prod(shape)
-                fan = shape[0] if len(shape) == 2 else fan
-                bound = 1.0 / math.sqrt(fan)
-                self.flat[off:off + k].view(shape).copy_(((torch.rand(shape, generator=g) * 2 - 1) * bound).to(self.device))
-                off += k
-        self._shapes, self.n_params = shapes, n
+        self._init_flat(shapes, seed)
         size = {name: math.prod(s) for name, s in shapes}
         part = lambda pre: sum(v for k, v in size.items() if k.startswith(pre))
         self.n_actor, self.n_critic = part("a_"), part("q0_")
