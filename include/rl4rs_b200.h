@@ -777,9 +777,75 @@ int r4_exactk_adam(int net, float* params, float* grad, float* m, float* v, int 
                    float eps, void* stream);
 /* kernels launched so far by the r4_exactk_* entry points in this process */
 int64_t r4_exactk_launch_count(void);
+/* ---- The MDP checker's seq2seq transformer (keras-transformer 0.40's get_model, rl4rs_b200/mdpchecker) ----
+ * Every call is asynchronous on `stream`; pointers other than cfg are DEVICE memory; results are deterministic.
+ * Config: src_tokens / tgt_tokens in 4..65536 (equal when use_same_embed), embed_dim E a multiple of 32 up to 512,
+ * head_num dividing E, hidden_dim F a multiple of 32 up to 1024, encoder_num / decoder_num in 1..6.
+ * Flat parameters, in this order (kernels [in, out]):
+ *   the encoder token table [src_tokens, E], then the decoder's [tgt_tokens, E] unless use_same_embed
+ *   per encoder block: self-attention Wq[E,E] bq[E] Wk bk Wv bv Wo bo, its LayerNorm gamma[E] beta[E],
+ *                      FeedForward W1[E,F] b1[F] W2[F,E] b2[E], its LayerNorm gamma beta
+ *   per decoder block: self-attention (as above), LayerNorm, query attention (as above), LayerNorm, FeedForward, LayerNorm
+ *   the output bias [tgt_tokens]
+ * Tokens are int32; 0 is PAD (masked as a key, and out of the loss as a decoder input); tokens outside the table are
+ * clamped into it.  Sequence lengths are 1..64.  Dropout (rate in [0, 1)) follows each sub-layer before its residual add;
+ * its keep draws are Exact-K's (r4_exactk.cuh: draw24) on the key (seed, call * 32 + sub-layer, 0, row * E + column), the
+ * sub-layers numbered encoder blocks first (2 each), then decoder blocks (3 each). */
+typedef struct {
+  int32_t src_tokens, tgt_tokens, embed_dim, head_num, hidden_dim, encoder_num, decoder_num, use_same_embed;
+} r4_s2s_config;
+enum { R4_S2S_TRAIN = 0, R4_S2S_PREDICT = 1, R4_S2S_SEARCH = 2, R4_S2S_STEP = 3 };
+/* parameter count; -1 for a config out of range */
+int64_t r4_s2s_num_params(const r4_s2s_config* cfg);
+/* BYTES of scratch for one call of `mode` over n source rows of length src_len: TRAIN (r4_s2s_grad, and r4_s2s_epoch at
+ * n = its batch), PREDICT (r4_s2s_predict, r4_s2s_score: tgt_len decoder positions of `beam` paths per row),
+ * SEARCH (r4_s2s_beam_search: tgt_len = target_len, k = candidates), STEP (r4_s2s_decode_step: k = its k); -1 out of
+ * range.  Grid limits: n * beam * head_num <= 65535. */
+int64_t r4_s2s_scratch_size(const r4_s2s_config* cfg, int mode, int n, int src_len, int tgt_len, int beam, int k);
+/* The loss sum(mask ce) / sum(mask) of keras 2.2.5's sparse categorical cross-entropy (probabilities clipped to
+ * [1e-7, 1 - 1e-7]) on enc i32[n, src_len], dec / target i32[n, tgt_len], and its gradient into grad f32[num_params]
+ * (overwritten); loss f32[1] may be NULL. */
+int r4_s2s_grad(const r4_s2s_config* cfg, const float* params, const int32_t* enc, const int32_t* dec, const int32_t* target,
+                int n, int src_len, int tgt_len, uint64_t seed, uint64_t call, float dropout, float* grad, float* loss,
+                void* scratch, void* stream);
+/* After r4_s2s_grad over (n, src_len, tgt_len), its scratch holds each FeedForward's relu(x W1 + b1), f32[n * len,
+ * hidden_dim], encoder blocks first, then decoder blocks: their BYTE offsets into offsets[encoder_num + decoder_num].
+ * Returns the count, or -1 out of range. */
+int r4_s2s_relu_offsets(const r4_s2s_config* cfg, int n, int src_len, int tgt_len, int64_t* offsets);
+/* keras 2.2.5 Adam step `step` (1-based) over every parameter: m, v, params updated in place.  1 launch. */
+int r4_s2s_apply(const r4_s2s_config* cfg, float* params, const float* grad, float* m, float* v, int step, float lr,
+                 float beta1, float beta2, float eps, void* stream);
+/* One epoch: for each minibatch k of `batch` rows of perm i64[n_perm] (the last one partial), gather its rows of the
+ * N-row arrays enc / dec / target, r4_s2s_grad with call = call0 + k, and Adam step step0 + k + 1; losses f32[steps]. */
+int r4_s2s_epoch(const r4_s2s_config* cfg, float* params, float* grad, float* m, float* v, const int32_t* enc,
+                 const int32_t* dec, const int32_t* target, int64_t N, int src_len, int tgt_len, const int64_t* perm,
+                 int64_t n_perm, int batch, int step0, uint64_t seed, uint64_t call0, float dropout, float lr, float beta1,
+                 float beta2, float eps, float* losses, void* scratch, void* stream);
+/* Softmax probabilities f32[n, tgt_len, tgt_tokens] of the decoder on enc i32[n, src_len] and dec i32[n, tgt_len]. */
+int r4_s2s_predict(const r4_s2s_config* cfg, const float* params, const int32_t* enc, const int32_t* dec, int n, int src_len,
+                   int tgt_len, float* probs, void* scratch, void* stream);
+/* The k most probable next tokens after dec i32[n, tgt_len] (times the candidate mask of cand i32[n, n_cand] when cand is
+ * not NULL), by probability descending, ties to the lower token: val f64[n, k], idx i32[n, k].  1 <= k < tgt_tokens. */
+int r4_s2s_decode_step(const r4_s2s_config* cfg, const float* params, const int32_t* enc, int n, int src_len,
+                       const int32_t* dec, int tgt_len, const int32_t* cand, int n_cand, int k, double* val, int32_t* idx,
+                       void* scratch, void* stream);
+/* rl4rs/mdpchecker/decoder.py's beam_search: paths i32[n, beam, target_len + 1] (START = 1 first) and their products of
+ * probabilities f64[n, beam].  Step 1 takes the top beam; with n_cand > 0 the later steps keep only the n_cand best tokens
+ * of step 1 (the reference's candidates); each later step takes the top beam of the beam^2 products, ties to the lower
+ * (beam, token) flat index.  beam in 1..256, < tgt_tokens; n_cand < tgt_tokens, at most 8192; target_len 1..63. */
+int r4_s2s_beam_search(const r4_s2s_config* cfg, const float* params, const int32_t* enc, int n, int src_len, int beam,
+                       int target_len, int n_cand, int32_t* path, double* score, void* scratch, void* stream);
+/* Experiment I's scores: prob f32[n, beam, target_len], entry i the probability the decoder gives path[., ., i + 1] after
+ * the prefix path[., ., :i + 1] (one causal pass over each path). */
+int r4_s2s_score(const r4_s2s_config* cfg, const float* params, const int32_t* enc, int n, int src_len, const int32_t* path,
+                 int beam, int target_len, float* prob, void* scratch, void* stream);
+/* kernels launched so far by the r4_s2s_* entry points in this process */
+int64_t r4_s2s_launch_count(void);
+
 /* kernels launched so far by every learner entry point in this process (r4_policy_*, r4_gae, r4_adam_step, r4_ppo_epoch*,
- * r4_grad_exchange*, r4_gauss_*, r4_vtrace, r4_impala_step, r4_ddpg_*, r4_replay_*, r4_rainbow_*, r4_batchrl_*, r4_simtrain_*, r4_exactk_*): the
- * sum of the batch RL, simulator-trainer and Exact-K counts above and the online learners'. */
+ * r4_grad_exchange*, r4_gauss_*, r4_vtrace, r4_impala_step, r4_ddpg_*, r4_replay_*, r4_rainbow_*, r4_batchrl_*,
+ * r4_simtrain_*, r4_exactk_*, r4_s2s_*): the sum of the batch RL, simulator-trainer, Exact-K and seq2seq counts above and
+ * the online learners'. */
 int64_t r4_learner_launch_count(void);
 
 #ifdef __cplusplus

@@ -219,7 +219,29 @@ EXPORTS = {
     "r4_exactk_critic": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 6),
     "r4_exactk_adam": (C.c_int, [C.c_int] + [C.c_void_p] * 4 + [C.c_int] + [C.c_float] * 4 + [C.c_void_p]),
     "r4_exactk_launch_count": (C.c_int64, []),
+    "r4_s2s_num_params": (C.c_int64, [C.c_void_p]),
+    "r4_s2s_scratch_size": (C.c_int64, [C.c_void_p] + [C.c_int] * 6),
+    "r4_s2s_grad": (C.c_int, [C.c_void_p] * 5 + [C.c_int] * 3 + [C.c_uint64, C.c_uint64, C.c_float] + [C.c_void_p] * 4),
+    "r4_s2s_relu_offsets": (C.c_int, [C.c_void_p] + [C.c_int] * 3 + [C.c_void_p]),
+    "r4_s2s_apply": (C.c_int, [C.c_void_p] * 5 + [C.c_int] + [C.c_float] * 4 + [C.c_void_p]),
+    "r4_s2s_epoch": (C.c_int, [C.c_void_p] * 8 + [C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int,
+                                                  C.c_uint64, C.c_uint64] + [C.c_float] * 5 + [C.c_void_p] * 3),
+    "r4_s2s_predict": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 3 + [C.c_void_p] * 3),
+    "r4_s2s_decode_step": (C.c_int, [C.c_void_p] * 3 + [C.c_int] * 2 + [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int] +
+                           [C.c_void_p] * 4),
+    "r4_s2s_beam_search": (C.c_int, [C.c_void_p] * 3 + [C.c_int] * 5 + [C.c_void_p] * 4),
+    "r4_s2s_score": (C.c_int, [C.c_void_p] * 3 + [C.c_int] * 2 + [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 3),
+    "r4_s2s_launch_count": (C.c_int64, []),
 }
+
+
+class S2SConfig(C.Structure):
+    """r4_s2s_config of include/rl4rs_b200.h."""
+    _fields_ = [(k, C.c_int32) for k in ("src_tokens", "tgt_tokens", "embed_dim", "head_num", "hidden_dim", "encoder_num",
+                                         "decoder_num", "use_same_embed")]
+
+
+S2S_TRAIN, S2S_PREDICT, S2S_SEARCH, S2S_STEP = 0, 1, 2, 3
 
 _lib = None
 

@@ -2131,3 +2131,592 @@ int r4_bcqc_act(int obs_dim, int action_dim, const float* params, const void* ob
 }
 
 }  // extern "C"
+
+// ---- the MDP checker's seq2seq transformer (r4_seq2seq.cuh) ---------------------------------------------------------------
+namespace {
+using namespace r4s2s;
+
+template <typename... P, typename... A>
+int s2_launch(const char* name, void (*kernel)(P...), dim3 grid, int threads, size_t smem, cudaStream_t st, A&&... args) {
+  return launch(FAM_SEQ2SEQ, name, kernel, grid, threads, smem, st, false, std::forward<A>(args)...);
+}
+unsigned s2_blocks(int64_t n, int per) { return (unsigned)((n + per - 1) / per); }
+Op s2_rm(const float* p, int64_t ld) { return Op{p, 0, 0, ld, 1}; }
+Op s2_tr(const float* p, int64_t ld) { return Op{p, 0, 0, 1, ld}; }
+
+// C[M, N] (ldc) (+)= epilogue(A B + bias)
+int s2_mm(cudaStream_t st, Op A, Op B, float* C, int64_t ldc, int64_t M, int N, int K, const float* bias, int accum = 0,
+          int epi = EP_LIN, const float* aux = nullptr) {
+  const Gemm g{A, B, C, 0, 0, ldc, 1, bias, aux, nullptr, nullptr, (int)M, N, K, 1, 0, 1.f, epi, accum};
+  return s2_launch("k_dense_gemm", gemm_kernel(g), dim3(s2_blocks(N, GT), s2_blocks(M, GT), 1), NT, 0, st, g);
+}
+// per (group, head) products: batch z = g H + h; C element (m, n) of batch (g, h) at C + g cso + h csi + m cs0 + n
+int s2_bmm(cudaStream_t st, Op A, Op B, float* C, int64_t cso, int64_t csi, int64_t cs0, int M, int N, int K, int64_t G, int H,
+           float alpha) {
+  const Gemm g{A, B, C, cso, csi, cs0, 1, nullptr, nullptr, nullptr, nullptr, M, N, K, H, 0, alpha, EP_LIN, 0};
+  return s2_launch("k_dense_gemm", gemm_kernel(g), dim3(s2_blocks(N, GT), s2_blocks(M, GT), (unsigned)(G * H)), NT, 0, st, g);
+}
+int s2_wgrad(cudaStream_t st, Jobs& J, int njob, int64_t rows, float* grad) {
+  tile_jobs(J, njob);
+  const Stats none{nullptr, 0, nullptr, nullptr, 0.f, 0};
+  return s2_launch("k_dense_wgrad", k_dense_wgrad, dim3(J.ntiles + 1), NT, 0, st, J, (int)rows, 0, grad, none);
+}
+Job s2_job(const float* X, int ldx, const float* Z, int M, int N, int64_t off) { return Job{X, Z, ldx, M, N, (int)off, 0}; }
+
+bool s2_cfg_ok(const r4_s2s_config* c) {
+  if (!c) return false;
+  const bool v = c->src_tokens >= MINV && c->src_tokens <= MAXV && c->tgt_tokens >= MINV && c->tgt_tokens <= MAXV;
+  return v && (!c->use_same_embed || c->src_tokens == c->tgt_tokens) && c->embed_dim >= 32 && c->embed_dim <= MAXE &&
+         c->embed_dim % 32 == 0 && c->head_num >= 1 && c->embed_dim % c->head_num == 0 && c->hidden_dim >= 32 &&
+         c->hidden_dim <= MAXF && c->hidden_dim % 32 == 0 && c->encoder_num >= 1 && c->encoder_num <= MAXBLK &&
+         c->decoder_num >= 1 && c->decoder_num <= MAXBLK;
+}
+Cfg s2_cfg(const r4_s2s_config* c) {
+  return Cfg{c->src_tokens, c->tgt_tokens, c->embed_dim, c->head_num, c->hidden_dim, c->encoder_num, c->decoder_num,
+             c->use_same_embed ? 1 : 0};
+}
+
+// The activations of one sub-layer: attention Q, K, V, the concatenated heads O, the softmax A; FeedForward relu(x W1 + b1)
+// in q; the sub-layer output y, the LayerNorm output, its normalised input and 1 / std.
+struct SubP { int64_t q, k, v, o, a, y, out, xh, rs; };
+// Scratch planes (floats) of one call over n source rows of Ts and R decoder prefixes per row of Tt positions; logits of
+// `lrows` rows; the backward's planes when train; a search's paths and scores for `beam`, and its candidate list of k.
+struct Plan {
+  int64_t xe, xd;
+  SubP enc[MAXBLK][2], dec[MAXBLK][3];
+  int64_t logits, ce, inv;
+  int64_t g[2], dy, gx, dq, dk, dv, dO, dA, dF, denc, cnt, off, order;
+  int64_t et, dt, yt;                              // a minibatch's tokens (epoch)
+  int64_t path[2], score[2], val, idx, cval, cand;  // search; cval / cand: the candidate list
+  int64_t n;
+};
+Plan s2_plan(const Cfg& c, int64_t n, int64_t Ts, int64_t Tt, int64_t R, int64_t lrows, bool train, int64_t beam, int64_t k) {
+  Plan p = {};
+  int64_t o = 0;
+  auto take = [&](int64_t x) { int64_t r = o; o += (x + 63) / 64 * 64; return r; };
+  const int64_t E = c.E, F = c.F, Ne = n * Ts, Nd = n * R * Tt, H = c.H;
+  auto sub = [&](SubP& s, int64_t rows, int64_t kvrows, int64_t att, bool ffn) {
+    s.q = take(rows * (ffn ? F : E));
+    if (!ffn) { s.k = take(kvrows * E); s.v = take(kvrows * E); s.o = take(rows * E); s.a = take(att); }
+    s.y = take(rows * E); s.out = take(rows * E); s.xh = take(rows * E); s.rs = take(rows);
+  };
+  p.xe = take(Ne * E);
+  for (int l = 0; l < c.Le; ++l) { sub(p.enc[l][0], Ne, Ne, n * H * Ts * Ts, false); sub(p.enc[l][1], Ne, 0, 0, true); }
+  p.xd = take(Nd * E);
+  for (int l = 0; l < c.Ld; ++l) {
+    sub(p.dec[l][0], Nd, Nd, n * R * H * Tt * Tt, false);
+    sub(p.dec[l][1], Nd, Ne, n * H * R * Tt * Ts, false);
+    sub(p.dec[l][2], Nd, 0, 0, true);
+  }
+  p.logits = take(lrows * c.Vt);
+  if (train) {
+    const int64_t rows = std::max(Ne, Nd);
+    p.ce = take(Nd); p.inv = take(1);
+    p.g[0] = take(rows * E); p.g[1] = take(rows * E); p.dy = take(rows * E); p.gx = take(rows * E);
+    p.dq = take(rows * E); p.dk = take(rows * E); p.dv = take(rows * E); p.dO = take(rows * E);
+    p.dA = take(std::max(n * H * Ts * Ts, std::max(n * R * H * Tt * Tt, n * H * R * Tt * Ts)));
+    p.dF = take(rows * F); p.denc = take(Ne * E);
+    p.cnt = take(std::max(c.Vs, c.Vt)); p.off = take(std::max(c.Vs, c.Vt)); p.order = take(rows);
+    p.et = take(Ne); p.dt = take(Nd); p.yt = take(Nd);
+  }
+  if (beam > 0) {
+    const int64_t L = Tt + 1;
+    p.path[0] = take(n * beam * L); p.path[1] = take(n * beam * L);
+    p.score[0] = take(2 * n * beam); p.score[1] = take(2 * n * beam);
+    p.val = take(2 * n * beam * beam); p.idx = take(n * beam * beam);
+  }
+  if (k > 0) { p.cval = take(2 * n * k); p.cand = take(n * k); }
+  p.n = o;
+  return p;
+}
+
+struct S2Run {
+  const float* prm;
+  Cfg c;
+  Layout L;
+  Plan p;
+  float* s;
+  cudaStream_t st;
+  int n, Ts;
+  const int32_t* etok;
+  uint64_t seed, call;
+  float rate;
+  float* f(int64_t o) const { return s + o; }
+  template <class T> T* as(int64_t o) const { return reinterpret_cast<T*>(s + o); }
+};
+
+// One attention sub-layer: out = LN(xq + dropout(MHA(xq, xkv))).  Groups g of Mq queries attend over Tk keys each
+// (the query rows of group g are g Mq .., its key rows g Tk ..); key j of group g is masked when ktok[g kld + j] == 0,
+// and, when causal, when j > m % Tq.  kv: compute K and V (else they are already in P).
+int s2_att(const S2Run& r, const Att& W, const Norm& Nw, const SubP& P, const float* xq, int64_t Nq, const float* xkv,
+           int64_t Nk, int64_t G, int Mq, int Tk, int Tq, int causal, const int32_t* ktok, int64_t kld, bool kv, int layer) {
+  const int E = r.c.E, H = r.c.H, dh = E / H;
+  const float* w = r.prm;
+  cudaStream_t st = r.st;
+  float *Q = r.f(P.q), *K = r.f(P.k), *V = r.f(P.v), *O = r.f(P.o), *A = r.f(P.a), *Y = r.f(P.y);
+  int rc;
+  if ((rc = s2_mm(st, s2_rm(xq, E), s2_rm(w + W.wq, E), Q, E, Nq, E, E, w + W.bq))) return rc;
+  if (kv) {
+    if ((rc = s2_mm(st, s2_rm(xkv, E), s2_rm(w + W.wk, E), K, E, Nk, E, E, w + W.bk))) return rc;
+    if ((rc = s2_mm(st, s2_rm(xkv, E), s2_rm(w + W.wv, E), V, E, Nk, E, E, w + W.bv))) return rc;
+  }
+  const int64_t cso = (int64_t)H * Mq * Tk, csi = (int64_t)Mq * Tk;
+  if ((rc = s2_bmm(st, Op{Q, (int64_t)Mq * E, dh, E, 1}, Op{K, (int64_t)Tk * E, dh, 1, E}, A, cso, csi, Tk, Mq, Tk, dh, G, H,
+                   1.0f / sqrtf((float)dh))))
+    return rc;
+  const int64_t rows = G * H * Mq;
+  if ((rc = s2_launch("k_s2s_softmax", k_s2s_softmax, s2_blocks(rows * 32, 256), 256, 0, st, A, ktok, kld, rows, H, Mq, Tk,
+                      Tq, causal)))
+    return rc;
+  if ((rc = s2_bmm(st, Op{A, cso, csi, Tk, 1}, Op{V, (int64_t)Tk * E, dh, E, 1}, O, (int64_t)Mq * E, dh, E, Mq, dh, Tk, G, H,
+                   1.f)))
+    return rc;
+  if ((rc = s2_mm(st, s2_rm(O, E), s2_rm(w + W.wo, E), Y, E, Nq, E, E, w + W.bo))) return rc;
+  return s2_launch("k_s2s_ln", k_s2s_ln, s2_blocks(Nq * 32, 256), 256, 0, st, xq, (const float*)Y, Nq, E, w + Nw.g, w + Nw.b,
+                   r.seed, r.call, layer, r.rate, r.f(P.out), r.f(P.xh), r.f(P.rs));
+}
+
+int s2_ffn(const S2Run& r, const FF& W, const Norm& Nw, const SubP& P, const float* x, int64_t N, int layer) {
+  const int E = r.c.E, F = r.c.F;
+  const float* w = r.prm;
+  int rc;
+  if ((rc = s2_mm(r.st, s2_rm(x, E), s2_rm(w + W.w1, F), r.f(P.q), F, N, F, E, w + W.b1, 0, EP_RELU))) return rc;
+  if ((rc = s2_mm(r.st, s2_rm(r.f(P.q), F), s2_rm(w + W.w2, E), r.f(P.y), E, N, E, F, w + W.b2))) return rc;
+  return s2_launch("k_s2s_ln", k_s2s_ln, s2_blocks(N * 32, 256), 256, 0, r.st, x, (const float*)r.f(P.y), N, E, w + Nw.g,
+                   w + Nw.b, r.seed, r.call, layer, r.rate, r.f(P.out), r.f(P.xh), r.f(P.rs));
+}
+
+const float* s2_enc_out(const S2Run& r) { return r.f(r.p.enc[r.c.Le - 1][1].out); }
+const float* s2_dec_out(const S2Run& r) { return r.f(r.p.dec[r.c.Ld - 1][2].out); }
+
+int s2_encoder(const S2Run& r) {
+  const int64_t Ne = (int64_t)r.n * r.Ts;
+  int rc;
+  if ((rc = s2_launch("k_s2s_embed", k_s2s_embed, s2_blocks(Ne * r.c.E, 256), 256, 0, r.st, r.etok, (int64_t)r.Ts, r.n, r.Ts,
+                      r.prm + r.L.emb_enc, r.c.Vs, r.c.E, r.f(r.p.xe))))
+    return rc;
+  const float* x = r.f(r.p.xe);
+  for (int l = 0; l < r.c.Le; ++l) {
+    const EncBlk& B = r.L.enc[l];
+    if ((rc = s2_att(r, B.sa, B.n1, r.p.enc[l][0], x, Ne, x, Ne, r.n, r.Ts, r.Ts, r.Ts, 0, r.etok, r.Ts, true, 2 * l)))
+      return rc;
+    if ((rc = s2_ffn(r, B.ff, B.n2, r.p.enc[l][1], r.f(r.p.enc[l][0].out), Ne, 2 * l + 1))) return rc;
+    x = r.f(r.p.enc[l][1].out);
+  }
+  return R4_OK;
+}
+
+// the cross-attention K / V of every decoder block from the encoder output (once per source row)
+int s2_cross_kv(const S2Run& r) {
+  const int E = r.c.E;
+  const int64_t Ne = (int64_t)r.n * r.Ts;
+  int rc;
+  for (int l = 0; l < r.c.Ld; ++l) {
+    const Att& W = r.L.dec[l].qa;
+    if ((rc = s2_mm(r.st, s2_rm(s2_enc_out(r), E), s2_rm(r.prm + W.wk, E), r.f(r.p.dec[l][1].k), E, Ne, E, E, r.prm + W.bk)))
+      return rc;
+    if ((rc = s2_mm(r.st, s2_rm(s2_enc_out(r), E), s2_rm(r.prm + W.wv, E), r.f(r.p.dec[l][1].v), E, Ne, E, E, r.prm + W.bv)))
+      return rc;
+  }
+  return R4_OK;
+}
+
+// the decoder over R prefixes per source row, each of Tt tokens at dtok + (row R + i) dld; kv: compute the cross K / V
+int s2_decoder(const S2Run& r, const int32_t* dtok, int64_t dld, int R, int Tt, bool kv) {
+  const int64_t P = (int64_t)r.n * R, Nd = P * Tt, Ne = (int64_t)r.n * r.Ts;
+  int rc;
+  if ((rc = s2_launch("k_s2s_embed", k_s2s_embed, s2_blocks(Nd * r.c.E, 256), 256, 0, r.st, dtok, dld, (int)P, Tt,
+                      r.prm + r.L.emb_dec, r.c.Vt, r.c.E, r.f(r.p.xd))))
+    return rc;
+  const float* x = r.f(r.p.xd);
+  const int base = 2 * r.c.Le;
+  for (int l = 0; l < r.c.Ld; ++l) {
+    const DecBlk& B = r.L.dec[l];
+    if ((rc = s2_att(r, B.sa, B.n1, r.p.dec[l][0], x, Nd, x, Nd, P, Tt, Tt, Tt, 1, dtok, dld, true, base + 3 * l))) return rc;
+    if ((rc = s2_att(r, B.qa, B.n2, r.p.dec[l][1], r.f(r.p.dec[l][0].out), Nd, s2_enc_out(r), Ne, r.n, R * Tt, r.Ts, R * Tt, 0,
+                     r.etok, r.Ts, kv, base + 3 * l + 1)))
+      return rc;
+    if ((rc = s2_ffn(r, B.ff, B.n3, r.p.dec[l][2], r.f(r.p.dec[l][1].out), Nd, base + 3 * l + 2))) return rc;
+    x = r.f(r.p.dec[l][2].out);
+  }
+  return R4_OK;
+}
+
+// logits [rows, Vt] = h emb_dec^T + b for rows at row stride ld of the decoder output, from position `pos0`
+int s2_logits(const S2Run& r, int64_t rows, int64_t ld, int pos0, float* out) {
+  const int E = r.c.E;
+  return s2_mm(r.st, Op{s2_dec_out(r) + (int64_t)pos0 * E, 0, 0, ld, 1}, s2_tr(r.prm + r.L.emb_dec, E), out, r.c.Vt, rows,
+               r.c.Vt, E, r.prm + r.L.out_b);
+}
+
+// ---- backward ----
+// LN backward of a sub-layer from dOut: gz <- the residual's gradient, dy <- the sub-layer output's; gx for gamma
+int s2_ln_bwd(const S2Run& r, const Norm& Nw, const SubP& P, const float* dOut, int64_t N, int layer, float* gz) {
+  return s2_launch("k_s2s_ln_bwd", k_s2s_ln_bwd, s2_blocks(N * 32, 256), 256, 0, r.st, dOut, (const float*)r.f(P.xh),
+                   (const float*)r.f(P.rs), N, r.c.E, r.prm + Nw.g, r.seed, r.call, layer, r.rate, gz, r.f(r.p.dy),
+                   r.f(r.p.gx));
+}
+
+// FeedForward sub-layer backward: gz <- d(x) (x the sub-layer input) from dOut; weight gradients into grad
+int s2_ffn_bwd(const S2Run& r, const FF& W, const Norm& Nw, const SubP& P, const float* x, int64_t N, int layer,
+               const float* dOut, float* gz, float* grad) {
+  const int E = r.c.E, F = r.c.F;
+  const float* w = r.prm;
+  int rc;
+  if ((rc = s2_ln_bwd(r, Nw, P, dOut, N, layer, gz))) return rc;
+  float *dy = r.f(r.p.dy), *dF = r.f(r.p.dF);
+  if ((rc = s2_mm(r.st, s2_rm(dy, E), s2_tr(w + W.w2, E), dF, F, N, F, E, nullptr, 0, EP_DRELU, r.f(P.q)))) return rc;
+  if ((rc = s2_mm(r.st, s2_rm(dF, F), s2_tr(w + W.w1, F), gz, E, N, E, F, nullptr, 1))) return rc;
+  Jobs J;
+  J.j[0] = s2_job(nullptr, 0, r.f(r.p.gx), 1, E, Nw.g);
+  J.j[1] = s2_job(nullptr, 0, dOut, 1, E, Nw.b);
+  J.j[2] = s2_job(r.f(P.q), F, dy, F, E, W.w2);
+  J.j[3] = s2_job(nullptr, 0, dy, 1, E, W.b2);
+  J.j[4] = s2_job(x, E, dF, E, F, W.w1);
+  J.j[5] = s2_job(nullptr, 0, dF, 1, F, W.b1);
+  return s2_wgrad(r.st, J, 6, N, grad);
+}
+
+// attention sub-layer backward (the forward's arguments): gz <- d(xq); d(xkv) added into gkv (== gz for self-attention).
+// Self-attention's key / value weight gradients share the query side's wgrad launch; cross-attention's, over the encoder
+// rows, take a second one.
+int s2_att_bwd(const S2Run& r, const Att& W, const Norm& Nw, const SubP& P, const float* xq, int64_t Nq, const float* xkv,
+               int64_t Nk, int64_t G, int Mq, int Tk, bool self, int layer, const float* dOut, float* gz, float* gkv,
+               float* grad) {
+  const int E = r.c.E, H = r.c.H, dh = E / H;
+  const float* w = r.prm;
+  cudaStream_t st = r.st;
+  int rc;
+  if ((rc = s2_ln_bwd(r, Nw, P, dOut, Nq, layer, gz))) return rc;
+  float *dy = r.f(r.p.dy), *dO = r.f(r.p.dO), *dA = r.f(r.p.dA), *dq = r.f(r.p.dq), *dk = r.f(r.p.dk), *dv = r.f(r.p.dv);
+  const float *Q = r.f(P.q), *K = r.f(P.k), *V = r.f(P.v), *A = r.f(P.a);
+  const int64_t cso = (int64_t)H * Mq * Tk, csi = (int64_t)Mq * Tk;
+  const float alpha = 1.0f / sqrtf((float)dh);
+  if ((rc = s2_mm(st, s2_rm(dy, E), s2_tr(w + W.wo, E), dO, E, Nq, E, E, nullptr))) return rc;
+  // dA = dO_h V_h^T; dV_h = A^T dO_h
+  if ((rc = s2_bmm(st, Op{dO, (int64_t)Mq * E, dh, E, 1}, Op{V, (int64_t)Tk * E, dh, 1, E}, dA, cso, csi, Tk, Mq, Tk, dh, G, H,
+                   1.f)))
+    return rc;
+  if ((rc = s2_bmm(st, Op{A, cso, csi, 1, Tk}, Op{dO, (int64_t)Mq * E, dh, E, 1}, dv, (int64_t)Tk * E, dh, E, Tk, dh, Mq, G, H,
+                   1.f)))
+    return rc;
+  const int64_t rows = G * H * Mq;
+  if ((rc = s2_launch("k_s2s_softmax_bwd", k_s2s_softmax_bwd, s2_blocks(rows * 32, 256), 256, 0, st, A, dA, rows, Tk))) return rc;
+  // dQ_h = alpha dS K_h; dK_h = alpha dS^T Q_h
+  if ((rc = s2_bmm(st, Op{dA, cso, csi, Tk, 1}, Op{K, (int64_t)Tk * E, dh, E, 1}, dq, (int64_t)Mq * E, dh, E, Mq, dh, Tk, G, H,
+                   alpha)))
+    return rc;
+  if ((rc = s2_bmm(st, Op{dA, cso, csi, 1, Tk}, Op{Q, (int64_t)Mq * E, dh, E, 1}, dk, (int64_t)Tk * E, dh, E, Tk, dh, Mq, G, H,
+                   alpha)))
+    return rc;
+  if ((rc = s2_mm(st, s2_rm(dq, E), s2_tr(w + W.wq, E), gz, E, Nq, E, E, nullptr, 1))) return rc;
+  if ((rc = s2_mm(st, s2_rm(dk, E), s2_tr(w + W.wk, E), gkv, E, Nk, E, E, nullptr, 1))) return rc;
+  if ((rc = s2_mm(st, s2_rm(dv, E), s2_tr(w + W.wv, E), gkv, E, Nk, E, E, nullptr, 1))) return rc;
+  Jobs J;
+  J.j[0] = s2_job(nullptr, 0, r.f(r.p.gx), 1, E, Nw.g);
+  J.j[1] = s2_job(nullptr, 0, dOut, 1, E, Nw.b);
+  J.j[2] = s2_job(r.f(P.o), E, dy, E, E, W.wo);
+  J.j[3] = s2_job(nullptr, 0, dy, 1, E, W.bo);
+  J.j[4] = s2_job(xq, E, dq, E, E, W.wq);
+  J.j[5] = s2_job(nullptr, 0, dq, 1, E, W.bq);
+  int nj = 6;
+  if (self) {
+    J.j[6] = s2_job(xkv, E, dk, E, E, W.wk);
+    J.j[7] = s2_job(nullptr, 0, dk, 1, E, W.bk);
+    J.j[8] = s2_job(xkv, E, dv, E, E, W.wv);
+    J.j[9] = s2_job(nullptr, 0, dv, 1, E, W.bv);
+    nj = 10;
+  }
+  if ((rc = s2_wgrad(st, J, nj, Nq, grad))) return rc;
+  if (self) return R4_OK;
+  Jobs K2;
+  K2.j[0] = s2_job(xkv, E, dk, E, E, W.wk);
+  K2.j[1] = s2_job(nullptr, 0, dk, 1, E, W.bk);
+  K2.j[2] = s2_job(xkv, E, dv, E, E, W.wv);
+  K2.j[3] = s2_job(nullptr, 0, dv, 1, E, W.bv);
+  return s2_wgrad(st, K2, 4, Nk, grad);
+}
+
+// emb[tok] += dX over the positions of tok [rows, T] (contiguous)
+int s2_emb_bwd(const S2Run& r, const int32_t* tok, int rows, int T, int V, const float* dX, float* demb) {
+  int *cnt = r.as<int>(r.p.cnt), *off = r.as<int>(r.p.off), *order = r.as<int>(r.p.order);
+  int rc;
+  if ((rc = s2_launch("k_s2s_tok_csr", k_s2s_tok_csr, 1, 1024, 0, r.st, tok, (int64_t)T, rows, T, V, cnt, off))) return rc;
+  if ((rc = s2_launch("k_s2s_tok_place", k_s2s_tok_place, s2_blocks((int64_t)rows * T, 256), 256, 0, r.st, tok, (int64_t)T,
+                      rows, T, V, (const int*)off, order)))
+    return rc;
+  return s2_launch("k_s2s_emb_grad", k_s2s_emb_grad, s2_blocks((int64_t)V * r.c.E, 256), 256, 0, r.st, dX, r.c.E, V,
+                   (const int*)cnt, (const int*)off, (const int*)order, demb);
+}
+
+// forward, loss and backward of one minibatch (tokens contiguous); grad overwritten
+int s2_train(const S2Run& r, const int32_t* dtok, const int32_t* ytok, int Tt, float* grad, float* loss) {
+  const int E = r.c.E, V = r.c.Vt, n = r.n;
+  const int64_t Nd = (int64_t)n * Tt, Ne = (int64_t)n * r.Ts;
+  const Layout& L = r.L;
+  int rc;
+  if (cudaMemsetAsync(grad, 0, L.n * sizeof(float), r.st) != cudaSuccess ||
+      cudaMemsetAsync(r.f(r.p.denc), 0, Ne * E * sizeof(float), r.st) != cudaSuccess)
+    return fail(R4_ERR_CUDA, "r4_s2s_grad: memset");
+  if ((rc = s2_encoder(r))) return rc;
+  if ((rc = s2_decoder(r, dtok, Tt, 1, Tt, true))) return rc;
+  float* Z = r.f(r.p.logits);
+  if ((rc = s2_logits(r, Nd, E, 0, Z))) return rc;
+  if ((rc = s2_launch("k_s2s_count", k_s2s_count, 1, 1024, 0, r.st, dtok, (int)Nd, r.f(r.p.inv)))) return rc;
+  if ((rc = s2_launch("k_s2s_out", k_s2s_out, (unsigned)Nd, 256, 0, r.st, Z, V, ytok, dtok, (const float*)r.f(r.p.inv),
+                      r.f(r.p.ce))))
+    return rc;
+  if (loss && (rc = s2_launch("k_s2s_lsum", k_s2s_lsum, 1, 1024, 0, r.st, (const float*)r.f(r.p.ce), (int)Nd,
+                              (const float*)r.f(r.p.inv), loss)))
+    return rc;
+  // output: dH = dZ emb_dec; emb_dec += dZ^T H; b += colsum dZ
+  float* g[2] = {r.f(r.p.g[0]), r.f(r.p.g[1])};
+  if ((rc = s2_mm(r.st, s2_rm(Z, V), s2_rm(r.prm + L.emb_dec, E), g[0], E, Nd, E, V, nullptr))) return rc;
+  Jobs J;
+  J.j[0] = s2_job(Z, V, s2_dec_out(r), V, E, L.emb_dec);
+  J.j[1] = s2_job(nullptr, 0, Z, 1, V, L.out_b);
+  if ((rc = s2_wgrad(r.st, J, 2, Nd, grad))) return rc;
+  int a = 0;
+  const int base = 2 * r.c.Le;
+  float* denc = r.f(r.p.denc);
+  for (int l = r.c.Ld - 1; l >= 0; --l) {
+    const DecBlk& B = L.dec[l];
+    const Plan& p = r.p;
+    const float* xin = l == 0 ? r.f(p.xd) : r.f(p.dec[l - 1][2].out);
+    if ((rc = s2_ffn_bwd(r, B.ff, B.n3, p.dec[l][2], r.f(p.dec[l][1].out), Nd, base + 3 * l + 2, g[a], g[1 - a], grad)))
+      return rc;
+    a = 1 - a;
+    if ((rc = s2_att_bwd(r, B.qa, B.n2, p.dec[l][1], r.f(p.dec[l][0].out), Nd, s2_enc_out(r), Ne, n, Tt, r.Ts, false,
+                         base + 3 * l + 1, g[a], g[1 - a], denc, grad)))
+      return rc;
+    a = 1 - a;
+    if ((rc = s2_att_bwd(r, B.sa, B.n1, p.dec[l][0], xin, Nd, xin, Nd, n, Tt, Tt, true, base + 3 * l, g[a], g[1 - a],
+                         g[1 - a], grad)))
+      return rc;
+    a = 1 - a;
+  }
+  if ((rc = s2_emb_bwd(r, dtok, n, Tt, V, g[a], grad + L.emb_dec))) return rc;
+  const float* cur = denc;
+  for (int l = r.c.Le - 1; l >= 0; --l) {
+    const EncBlk& B = L.enc[l];
+    const Plan& p = r.p;
+    const float* xin = l == 0 ? r.f(p.xe) : r.f(p.enc[l - 1][1].out);
+    if ((rc = s2_ffn_bwd(r, B.ff, B.n2, p.enc[l][1], r.f(p.enc[l][0].out), Ne, 2 * l + 1, cur, g[a], grad))) return rc;
+    if ((rc = s2_att_bwd(r, B.sa, B.n1, p.enc[l][0], xin, Ne, xin, Ne, n, r.Ts, r.Ts, true, 2 * l, g[a], g[1 - a], g[1 - a],
+                         grad)))
+      return rc;
+    cur = g[1 - a];
+  }
+  return s2_emb_bwd(r, r.etok, n, r.Ts, r.c.Vs, cur, grad + L.emb_enc);
+}
+
+bool s2_len_ok(int T) { return T >= 1 && T <= MAXT; }
+
+int s2_init(S2Run* r, const r4_s2s_config* cfg, const float* params, const int32_t* enc, int n, int Ts, void* scratch,
+            void* stream) {
+  if (!s2_cfg_ok(cfg) || !params || !enc || !scratch || n < 1 || !s2_len_ok(Ts) || (int64_t)n * cfg->head_num > 65535)
+    return fail(R4_ERR_ARG, "bad argument");
+  r->prm = params; r->c = s2_cfg(cfg); r->L = make_layout(r->c); r->s = static_cast<float*>(scratch); r->st = S(stream);
+  r->n = n; r->Ts = Ts; r->etok = enc; r->seed = 0; r->call = 0; r->rate = 0.f;
+  return R4_OK;
+}
+
+int s2_adam(const Cfg& c, float* params, const float* grad, float* m, float* v, int step, float lr, float b1, float b2,
+            float eps, cudaStream_t st) {
+  const int64_t np = make_layout(c).n;
+  const float alpha = lr * sqrtf(1.f - powf(b2, (float)step)) / (1.f - powf(b1, (float)step));
+  return s2_launch("k_s2s_adam", k_s2s_adam, s2_blocks(np, 256), 256, 0, st, np, (int64_t)0, np, np, params,
+                   const_cast<float*>(grad), m, v, alpha, b1, b2, eps);
+}
+
+// the top-k step after the decoder ran over n R prefixes of Tt tokens: probabilities of the last position, then top-k
+int s2_topk(const S2Run& r, int64_t P, int Tt, const int32_t* cand, int C, int group, int k, double* val, int32_t* idx) {
+  float* Z = r.f(r.p.logits);
+  const int V = r.c.Vt;
+  int rc;
+  if ((rc = s2_logits(r, P, (int64_t)Tt * r.c.E, Tt - 1, Z))) return rc;
+  if ((rc = s2_launch("k_s2s_out", k_s2s_out, (unsigned)P, 256, 0, r.st, Z, V, (const int32_t*)nullptr,
+                      (const int32_t*)nullptr, (const float*)nullptr, (float*)nullptr)))
+    return rc;
+  const int P2 = pow2_at_least(k);
+  const size_t smem = (size_t)P2 * 12 + (cand ? (size_t)(V + 31) / 32 * 4 : 0);
+  return s2_launch("k_s2s_topk", k_s2s_topk, (unsigned)P, 256, smem, r.st, (const float*)Z, V, cand, C, group, k, val, idx);
+}
+
+}  // namespace
+
+extern "C" {
+
+int64_t r4_s2s_launch_count(void) { return g_launches[FAM_SEQ2SEQ].load(std::memory_order_relaxed); }
+
+int64_t r4_s2s_num_params(const r4_s2s_config* cfg) { return s2_cfg_ok(cfg) ? make_layout(s2_cfg(cfg)).n : -1; }
+
+int64_t r4_s2s_scratch_size(const r4_s2s_config* cfg, int mode, int n, int src_len, int tgt_len, int beam, int k) {
+  if (!s2_cfg_ok(cfg) || n < 1 || !s2_len_ok(src_len) || !s2_len_ok(tgt_len) || beam < 1 || beam > MAXBEAM) return -1;
+  if ((int64_t)n * beam * cfg->head_num > 65535) return -1;
+  const Cfg c = s2_cfg(cfg);
+  Plan p;
+  if (mode == R4_S2S_TRAIN) p = s2_plan(c, n, src_len, tgt_len, 1, (int64_t)n * tgt_len, true, 0, 0);
+  else if (mode == R4_S2S_PREDICT) p = s2_plan(c, n, src_len, tgt_len, beam, (int64_t)n * beam * tgt_len, false, 0, 0);
+  else if (mode == R4_S2S_SEARCH) {
+    if (tgt_len >= MAXT || k < 0 || k > MAXK) return -1;
+    p = s2_plan(c, n, src_len, tgt_len, beam, (int64_t)n * beam, false, beam, k);
+  } else if (mode == R4_S2S_STEP) {
+    if (k < 1 || k > MAXK) return -1;
+    p = s2_plan(c, n, src_len, tgt_len, 1, n, false, 0, 0);
+  } else {
+    return -1;
+  }
+  return p.n * (int64_t)sizeof(float);
+}
+
+int r4_s2s_relu_offsets(const r4_s2s_config* cfg, int n, int src_len, int tgt_len, int64_t* offsets) {
+  if (!s2_cfg_ok(cfg) || !offsets || n < 1 || !s2_len_ok(src_len) || !s2_len_ok(tgt_len)) return fail(R4_ERR_ARG, "bad argument");
+  const Cfg c = s2_cfg(cfg);
+  const Plan p = s2_plan(c, n, src_len, tgt_len, 1, (int64_t)n * tgt_len, true, 0, 0);
+  int k = 0;
+  for (int l = 0; l < c.Le; ++l) offsets[k++] = p.enc[l][1].q * (int64_t)sizeof(float);
+  for (int l = 0; l < c.Ld; ++l) offsets[k++] = p.dec[l][2].q * (int64_t)sizeof(float);
+  return k;
+}
+
+int r4_s2s_grad(const r4_s2s_config* cfg, const float* params, const int32_t* enc, const int32_t* dec, const int32_t* target,
+                int n, int src_len, int tgt_len, uint64_t seed, uint64_t call, float dropout, float* grad, float* loss,
+                void* scratch, void* stream) {
+  S2Run r;
+  if (int rc = s2_init(&r, cfg, params, enc, n, src_len, scratch, stream)) return rc;
+  if (!dec || !target || !grad || !s2_len_ok(tgt_len) || !(dropout >= 0.f && dropout < 1.f))
+    return fail(R4_ERR_ARG, "bad argument");
+  r.seed = seed; r.call = call; r.rate = dropout;
+  r.p = s2_plan(r.c, n, src_len, tgt_len, 1, (int64_t)n * tgt_len, true, 0, 0);
+  return s2_train(r, dec, target, tgt_len, grad, loss);
+}
+
+int r4_s2s_apply(const r4_s2s_config* cfg, float* params, const float* grad, float* m, float* v, int step, float lr,
+                 float beta1, float beta2, float eps, void* stream) {
+  if (!s2_cfg_ok(cfg) || !params || !grad || !m || !v || step < 1) return fail(R4_ERR_ARG, "bad argument");
+  return s2_adam(s2_cfg(cfg), params, grad, m, v, step, lr, beta1, beta2, eps, S(stream));
+}
+
+int r4_s2s_epoch(const r4_s2s_config* cfg, float* params, float* grad, float* m, float* v, const int32_t* enc,
+                 const int32_t* dec, const int32_t* target, int64_t N, int src_len, int tgt_len, const int64_t* perm,
+                 int64_t n_perm, int batch, int step0, uint64_t seed, uint64_t call0, float dropout, float lr, float beta1,
+                 float beta2, float eps, float* losses, void* scratch, void* stream) {
+  S2Run r;
+  if (int rc = s2_init(&r, cfg, params, enc, batch, src_len, scratch, stream)) return rc;
+  if (!grad || !m || !v || !dec || !target || !perm || !losses || N < 1 || n_perm < 1 || step0 < 0 || !s2_len_ok(tgt_len) ||
+      !(dropout >= 0.f && dropout < 1.f))
+    return fail(R4_ERR_ARG, "bad argument");
+  const int64_t steps = (n_perm + batch - 1) / batch;
+  const Plan full = s2_plan(r.c, batch, src_len, tgt_len, 1, (int64_t)batch * tgt_len, true, 0, 0);
+  int32_t *et = r.as<int32_t>(full.et), *dt = r.as<int32_t>(full.dt), *yt = r.as<int32_t>(full.yt);
+  r.seed = seed; r.rate = dropout;
+  for (int64_t k = 0; k < steps; ++k) {
+    const int nb = (int)std::min<int64_t>(batch, n_perm - k * batch);
+    const int W = src_len + 2 * tgt_len;
+    if (int rc = s2_launch("k_s2s_gather", k_s2s_gather, s2_blocks((int64_t)nb * W, 256), 256, 0, r.st, enc, src_len, dec,
+                           target, tgt_len, perm + k * batch, nb, et, dt, yt))
+      return rc;
+    // the minibatch's planes: the plan of nb rows, its token planes at the full batch's offsets (past every other plane)
+    r.n = nb; r.etok = et; r.call = call0 + (uint64_t)k;
+    r.p = s2_plan(r.c, nb, src_len, tgt_len, 1, (int64_t)nb * tgt_len, true, 0, 0);
+    if (int rc = s2_train(r, dt, yt, tgt_len, grad, losses + k)) return rc;
+    if (int rc = s2_adam(r.c, params, grad, m, v, step0 + (int)k + 1, lr, beta1, beta2, eps, r.st)) return rc;
+  }
+  return R4_OK;
+}
+
+int r4_s2s_predict(const r4_s2s_config* cfg, const float* params, const int32_t* enc, const int32_t* dec, int n, int src_len,
+                   int tgt_len, float* probs, void* scratch, void* stream) {
+  S2Run r;
+  if (int rc = s2_init(&r, cfg, params, enc, n, src_len, scratch, stream)) return rc;
+  if (!dec || !probs || !s2_len_ok(tgt_len)) return fail(R4_ERR_ARG, "bad argument");
+  r.p = s2_plan(r.c, n, src_len, tgt_len, 1, 0, false, 0, 0);
+  int rc;
+  if ((rc = s2_encoder(r)) || (rc = s2_decoder(r, dec, tgt_len, 1, tgt_len, true))) return rc;
+  const int64_t rows = (int64_t)n * tgt_len;
+  if ((rc = s2_logits(r, rows, r.c.E, 0, probs))) return rc;
+  return s2_launch("k_s2s_out", k_s2s_out, (unsigned)rows, 256, 0, r.st, probs, r.c.Vt, (const int32_t*)nullptr,
+                   (const int32_t*)nullptr, (const float*)nullptr, (float*)nullptr);
+}
+
+int r4_s2s_decode_step(const r4_s2s_config* cfg, const float* params, const int32_t* enc, int n, int src_len,
+                       const int32_t* dec, int tgt_len, const int32_t* cand, int n_cand, int k, double* val, int32_t* idx,
+                       void* scratch, void* stream) {
+  S2Run r;
+  if (int rc = s2_init(&r, cfg, params, enc, n, src_len, scratch, stream)) return rc;
+  if (!dec || !val || !idx || !s2_len_ok(tgt_len) || k < 1 || k > MAXK || k >= cfg->tgt_tokens ||
+      (cand && (n_cand < 1 || n_cand > MAXK)))
+    return fail(R4_ERR_ARG, "bad argument");
+  r.p = s2_plan(r.c, n, src_len, tgt_len, 1, n, false, 0, 0);
+  int rc;
+  if ((rc = s2_encoder(r)) || (rc = s2_decoder(r, dec, tgt_len, 1, tgt_len, true))) return rc;
+  return s2_topk(r, n, tgt_len, cand, n_cand, 1, k, val, idx);
+}
+
+int r4_s2s_beam_search(const r4_s2s_config* cfg, const float* params, const int32_t* enc, int n, int src_len, int beam,
+                       int target_len, int n_cand, int32_t* path, double* score, void* scratch, void* stream) {
+  S2Run r;
+  if (int rc = s2_init(&r, cfg, params, enc, n, src_len, scratch, stream)) return rc;
+  if (!path || !score || beam < 1 || beam > MAXBEAM || beam >= cfg->tgt_tokens || target_len < 1 || target_len >= MAXT ||
+      n_cand < 0 || n_cand > MAXK || n_cand >= cfg->tgt_tokens || (int64_t)n * beam * cfg->head_num > 65535)
+    return fail(R4_ERR_ARG, "bad argument");
+  r.p = s2_plan(r.c, n, src_len, target_len, beam, (int64_t)n * beam, false, beam, n_cand);
+  const int L = target_len + 1;
+  const int64_t P = (int64_t)n * beam;
+  int32_t* pa[2] = {r.as<int32_t>(r.p.path[0]), r.as<int32_t>(r.p.path[1])};
+  double* sa[2] = {r.as<double>(r.p.score[0]), r.as<double>(r.p.score[1])};
+  double* val = r.as<double>(r.p.val);
+  int32_t* idx = r.as<int32_t>(r.p.idx);
+  int32_t* cand = n_cand > 0 ? r.as<int32_t>(r.p.cand) : nullptr;
+  int rc;
+  if ((rc = s2_launch("k_s2s_start", k_s2s_start, s2_blocks(P * L, 256), 256, 0, r.st, P, L, pa[0]))) return rc;
+  if ((rc = s2_encoder(r)) || (rc = s2_cross_kv(r))) return rc;
+  // step 1: the n START prefixes (row b's beam 0), top beam; the candidates are the top n_cand of the same probabilities
+  if ((rc = s2_decoder(r, pa[0], (int64_t)beam * L, 1, 1, false))) return rc;
+  if ((rc = s2_topk(r, n, 1, nullptr, 0, 1, beam, val, idx))) return rc;
+  if ((rc = s2_launch("k_s2s_first", k_s2s_first, s2_blocks(P, 256), 256, 0, r.st, (const double*)val, (const int32_t*)idx, P,
+                      L, pa[0], sa[0])))
+    return rc;
+  if (cand) {
+    const size_t smem = (size_t)pow2_at_least(n_cand) * 12;
+    if ((rc = s2_launch("k_s2s_topk", k_s2s_topk, (unsigned)n, 256, smem, r.st, (const float*)r.f(r.p.logits), r.c.Vt,
+                        (const int32_t*)nullptr, 0, 1, n_cand, r.as<double>(r.p.cval), cand)))
+      return rc;
+  }
+  int cur = 0;
+  const size_t bsm = (size_t)pow2_at_least(beam) * 12;
+  for (int i = 1; i < target_len; ++i) {
+    if ((rc = s2_decoder(r, pa[cur], L, beam, i + 1, false))) return rc;
+    if ((rc = s2_topk(r, P, i + 1, cand, n_cand, beam, beam, val, idx))) return rc;
+    if ((rc = s2_launch("k_s2s_beam", k_s2s_beam, (unsigned)n, 256, bsm, r.st, (const double*)sa[cur], (const double*)val,
+                        (const int32_t*)idx, (const int32_t*)pa[cur], beam, L, i + 1, pa[1 - cur], sa[1 - cur])))
+      return rc;
+    cur = 1 - cur;
+  }
+  if (cudaMemcpyAsync(path, pa[cur], P * L * sizeof(int32_t), cudaMemcpyDeviceToDevice, r.st) != cudaSuccess ||
+      cudaMemcpyAsync(score, sa[cur], P * sizeof(double), cudaMemcpyDeviceToDevice, r.st) != cudaSuccess)
+    return fail(R4_ERR_CUDA, "r4_s2s_beam_search: copy");
+  return R4_OK;
+}
+
+int r4_s2s_score(const r4_s2s_config* cfg, const float* params, const int32_t* enc, int n, int src_len, const int32_t* path,
+                 int beam, int target_len, float* prob, void* scratch, void* stream) {
+  S2Run r;
+  if (int rc = s2_init(&r, cfg, params, enc, n, src_len, scratch, stream)) return rc;
+  if (!path || !prob || beam < 1 || beam > MAXBEAM || !s2_len_ok(target_len) || (int64_t)n * beam * cfg->head_num > 65535)
+    return fail(R4_ERR_ARG, "bad argument");
+  const int64_t P = (int64_t)n * beam, rows = P * target_len;
+  r.p = s2_plan(r.c, n, src_len, target_len, beam, rows, false, 0, 0);
+  int rc;
+  if ((rc = s2_encoder(r)) || (rc = s2_decoder(r, path, target_len + 1, beam, target_len, true))) return rc;
+  float* Z = r.f(r.p.logits);
+  if ((rc = s2_logits(r, rows, r.c.E, 0, Z))) return rc;
+  if ((rc = s2_launch("k_s2s_out", k_s2s_out, (unsigned)rows, 256, 0, r.st, Z, r.c.Vt, (const int32_t*)nullptr,
+                      (const int32_t*)nullptr, (const float*)nullptr, (float*)nullptr)))
+    return rc;
+  return s2_launch("k_s2s_pick", k_s2s_pick, s2_blocks(rows, 256), 256, 0, r.st, (const float*)Z, r.c.Vt, path,
+                   target_len + 1, (int)P, target_len, prob);
+}
+
+}  // extern "C"
