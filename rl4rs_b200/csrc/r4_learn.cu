@@ -2571,7 +2571,11 @@ int64_t r4_s2s_scratch_size(const r4_s2s_config* cfg, int mode, int n, int src_l
 }
 
 int r4_s2s_relu_offsets(const r4_s2s_config* cfg, int n, int src_len, int tgt_len, int64_t* offsets) {
-  if (!s2_cfg_ok(cfg) || !offsets || n < 1 || !s2_len_ok(src_len) || !s2_len_ok(tgt_len)) return fail(R4_ERR_ARG, "bad argument");
+  // the shapes r4_s2s_grad accepts, the grid's z extent n * heads included: offsets of a plan no training call can run
+  // would describe nothing
+  if (!s2_cfg_ok(cfg) || !offsets || n < 1 || !s2_len_ok(src_len) || !s2_len_ok(tgt_len) ||
+      (int64_t)n * cfg->head_num > 65535)
+    return fail(R4_ERR_ARG, "bad argument");
   const Cfg c = s2_cfg(cfg);
   const Plan p = s2_plan(c, n, src_len, tgt_len, 1, (int64_t)n * tgt_len, true, 0, 0);
   int k = 0;
