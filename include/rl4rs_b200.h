@@ -842,10 +842,41 @@ int r4_s2s_score(const r4_s2s_config* cfg, const float* params, const int32_t* e
 /* kernels launched so far by the r4_s2s_* entry points in this process */
 int64_t r4_s2s_launch_count(void);
 
+/* ---- Off-policy evaluation (script/offline_evaluation.py's `ope` stage, rl4rs_b200/offline_evaluation.py) ----
+ * Every call is asynchronous on `stream`; pointers are caller-owned DEVICE memory; results are deterministic.
+ * The logged-policy (behaviour) net is nets/dnn.py's graph at 50 dense features and C classes (149 <= C <= 65536), with
+ * flat parameters in this order (kernels [in, out]): emb_cat [H, 128], dense_w1 [50, 128], dense_b1 [128],
+ * dense_w2 [128, 128], dense_b2 [128], fc_w [256, 256], fc_b [256], obs_w [256, 256], obs_b [256], rew_w [256, C],
+ * rew_b [C].  1 <= H <= 2^24, 1 <= B <= 2^21. */
+/* parameter count; -1 out of range */
+int64_t r4_ope_num_params(int H, int C);
+/* FLOATS of scratch for one r4_ope_behavior call over B rows; -1 out of range */
+int64_t r4_ope_behavior_scratch_size(int B, int C);
+/* The behaviour probabilities of page `page` (0 <= page < P) of B records: the page's category ids -- head i32[B, 11]
+ * (user_protrait[:10], sequence_id), then items i32[B, P * K] at [page K, page K + K), post-padded with 0 to 21; ids
+ * outside [0, H) are clamped into the table -- and its dense row, feat f32[B, P * 5K] at [page 5K, page 5K + 5K),
+ * post-padded with 0 to 50 (1 <= K <= 10).  y = softmax of the net; out f32[B, C - 1] column c - 1 = y[c] divided by the
+ * sum of its slice: y[1:40], y[40:148] or y[148:C] (sums in f64).  7 launches. */
+int r4_ope_behavior(int B, int H, int C, int K, int P, int page, const float* params, const int32_t* head,
+                    const int32_t* items, const float* feat, float* out, float* scratch, void* stream);
+/* Step t (0 <= t < T) of an evaluation episode: column t of the [T, B] buffers.  1 launch.
+ *   pol f32  the policy's probability of the offline action off i32[B]: probs f32[B, A] (logits 0) or the softmax of the
+ *            logits f32[B, A] (logits 1; the sum in f64);
+ *   beh f32  the behaviour probability of the offline action: block f32[B, C - 1] (r4_ope_behavior's page) at layer
+ *            (>= 1) with behavior_model.action_probs' slice and clip (layer 1, 2, any other);
+ *   val f32  values f32[B, A] at own i32[B] (per_action 1), or values f32[B] (per_action 0; own may be NULL);
+ *   rew f64  reward f64[B];  offr f64  off_reward f64[B].
+ * 2 <= A <= 65536, A <= C.  A device-side action outside [0, A) writes NaN into the columns that index with it. */
+int r4_ope_step(int t, int T, int B, int A, int C, int layer, const float* probs, int logits, const int32_t* off,
+                const float* block, const int32_t* own, const float* values, int per_action, const double* reward,
+                const double* off_reward, float* pol, float* beh, float* val, double* rew, double* offr, void* stream);
+/* kernels launched so far by the r4_ope_* entry points in this process */
+int64_t r4_ope_launch_count(void);
+
 /* kernels launched so far by every learner entry point in this process (r4_policy_*, r4_gae, r4_adam_step, r4_ppo_epoch*,
  * r4_grad_exchange*, r4_gauss_*, r4_vtrace, r4_impala_step, r4_ddpg_*, r4_replay_*, r4_rainbow_*, r4_batchrl_*,
- * r4_simtrain_*, r4_exactk_*, r4_s2s_*): the sum of the batch RL, simulator-trainer, Exact-K and seq2seq counts above and
- * the online learners'. */
+ * r4_simtrain_*, r4_exactk_*, r4_s2s_*, r4_ope_*): the sum of the batch RL, simulator-trainer, Exact-K, seq2seq and OPE
+ * counts above and the online learners'. */
 int64_t r4_learner_launch_count(void);
 
 #ifdef __cplusplus

@@ -232,6 +232,12 @@ EXPORTS = {
     "r4_s2s_beam_search": (C.c_int, [C.c_void_p] * 3 + [C.c_int] * 5 + [C.c_void_p] * 4),
     "r4_s2s_score": (C.c_int, [C.c_void_p] * 3 + [C.c_int] * 2 + [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 3),
     "r4_s2s_launch_count": (C.c_int64, []),
+    "r4_ope_num_params": (C.c_int64, [C.c_int, C.c_int]),
+    "r4_ope_behavior_scratch_size": (C.c_int64, [C.c_int, C.c_int]),
+    "r4_ope_behavior": (C.c_int, [C.c_int] * 6 + [C.c_void_p] * 7),
+    "r4_ope_step": (C.c_int, [C.c_int] * 6 + [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int] +
+                    [C.c_void_p] * 8),
+    "r4_ope_launch_count": (C.c_int64, []),
 }
 
 

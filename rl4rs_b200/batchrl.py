@@ -97,6 +97,8 @@ def d3rlpy_eval(*args, **kwargs):
 
 
 def ope_eval(*args, **kwargs):
+    """Not here: the `ope` stage is rl4rs_b200.offline_evaluation.ope_eval (with its behavior_model), as the reference
+    keeps it in script/offline_evaluation.py."""
     raise NotImplementedError("ope: the off-policy evaluation stage is not built in this project")
 
 
@@ -696,7 +698,8 @@ def adam_(p, g, m, v, step, lr, eps, b1=0.9, b2=0.999):
 
 
 class policy_model(object):
-    """rl4rs/policy/policy_model.py over a batch-RL model."""
+    """rl4rs/policy/policy_model.py over a batch-RL model or a model-free trainer (trainer.get_rl_model's PPO / A2C /
+    PG / IMPALA and RAINBOW: the RLlib branch of policy_model.py:37-38, 47-50, 62-69, 83-87, through compute_actions)."""
 
     def __init__(self, model, config={}):
         self.policy = model
@@ -706,11 +709,23 @@ class policy_model(object):
         self.location_mask = config.get("location_mask", None)
         self.special_items = config.get("special_items", None)
 
+    @property
+    def _rllib(self):
+        return hasattr(self.policy, "compute_actions")
+
+    @staticmethod
+    def _rllib_obs(obs):
+        """policy_model.py's dict(enumerate(obs)) for a list of rows; batched arrays, tensors and field dicts go as they
+        are (compute_actions takes both forms)."""
+        return dict(enumerate(obs)) if isinstance(obs, list) else obs
+
     def predict_with_mask(self, obs):
         """policy_model.py:17-36: action_probs, -2^15 where the location layer, the prev actions or the special-item rule
         exclude an item, the first argmax.  A device tensor in gives a device tensor out, else a numpy array.  Under
         support_conti_env it is predict (policy_model.py:18-19); a continuous model then returns device actions
-        f32 [n, D] for a device tensor."""
+        f32 [n, D] for a device tensor.  A trainer: predict (policy_model.py:37-38)."""
+        if self._rllib:
+            return self.predict(obs)
         if self.config.get("support_conti_env", False):
             if hasattr(obs, "is_cuda") and self.policy.continuous:
                 return self.policy.act(obs)[0]
@@ -719,17 +734,48 @@ class policy_model(object):
         return a if hasattr(obs, "is_cuda") else a.long().cpu().numpy()
 
     def predict(self, obs):
+        if self._rllib:
+            a = self.policy.compute_actions(self._rllib_obs(obs), explore=False)
+            return np.array(list(a.values())) if isinstance(a, dict) else np.asarray(a)
         return self.policy.predict(obs)
 
     def predict_q(self, obs, action):
+        if self._rllib:
+            _, _, infos = self.policy.compute_actions(self._rllib_obs(obs), explore=False, full_fetch=True)
+            if "q_values" in infos:
+                return infos["q_values"][range(len(action)), action]
+            return infos["vf_preds"]
         q = self.policy.predict_value(obs, action)
         if self.policy.reward_scaler is not None:
             return q * (self.policy.reward_std + 1e-3) + self.policy.reward_mean
         return q
 
     def action_probs(self, obs):
-        """BC: the imitator's log-probs; BCQ / CQL: softmax(Q)."""
+        """BC: the imitator's log-probs; BCQ / CQL: softmax(Q); a trainer: softmax(action_dist_inputs)."""
+        if self._rllib:
+            from scipy.special import softmax
+            _, _, infos = self.policy.compute_actions(self._rllib_obs(obs), explore=False, full_fetch=True)
+            return softmax(infos["action_dist_inputs"], axis=1)
         return self.policy.act(obs, 0, want_probs=True)[1].cpu().numpy()
+
+    def _ope_fetch(self, obs):
+        """One act of the policy for offline_evaluation.ope_eval, as device tensors where the policy runs: (the env
+        action, probs [n, A] or logits, whether they are logits, the own action or None, values [n, A] or [n], the host
+        fix of the values or None).  The same numbers predict_with_mask, action_probs and predict_q give."""
+        if self._rllib:
+            a, infos = self.policy._fetch(obs)
+            env_a = a if hasattr(obs, "is_cuda") or isinstance(obs, dict) and hasattr(next(iter(obs.values())), "is_cuda") \
+                else a.long().cpu().numpy()
+            if "q_values" in infos:
+                return env_a, infos["action_dist_inputs"], True, a, infos["q_values"], None
+            return env_a, infos["action_dist_inputs"], True, None, infos["vf_preds"], None
+        a, probs, vals = self.policy.act(obs, 0, want_probs=True, want_values=True)
+        env_a = a if hasattr(obs, "is_cuda") else a.long().cpu().numpy()
+        fix = None
+        if self.policy.reward_scaler is not None:
+            std, mean = self.policy.reward_std, self.policy.reward_mean
+            fix = lambda q: q * (std + 1e-3) + mean
+        return env_a, probs, False, a, vals, fix
 
 
 def make_eval_env(config, batch_size=2048):

@@ -536,3 +536,4 @@ __global__ void __launch_bounds__(TRT) k_bq_transitions(const uint8_t* __restric
 
 #include "r4_cqlconti.cuh"   // continuous-action CQL, on the same dataset planes and launch family
 #include "r4_bcqconti.cuh"   // continuous-action BCQ, likewise
+#include "r4_ope.cuh"         // off-policy evaluation of the batch-RL and model-free policies: its own launch family

@@ -2724,3 +2724,96 @@ int r4_s2s_score(const r4_s2s_config* cfg, const float* params, const int32_t* e
 }
 
 }  // extern "C"
+
+// ---- off-policy evaluation (r4_ope.cuh) ------------------------------------------------------------------------------------
+namespace {
+using namespace r4ope;
+
+template <typename... P, typename... A>
+int ope_launch(const char* name, void (*kernel)(P...), dim3 grid, int threads, cudaStream_t st, A&&... args) {
+  return launch(FAM_OPE, name, kernel, grid, threads, 0, st, false, std::forward<A>(args)...);
+}
+
+constexpr int OPE_MAX_B = 1 << 21, OPE_MAX_C = 1 << 16, OPE_MAX_H = 1 << 24, OPE_MAX_A = 1 << 16;
+constexpr int OPE_U = 128, OPE_F = 256;        // the dense tower's width, the two 256-unit layers
+
+bool ope_c_ok(int C) { return C >= 149 && C <= OPE_MAX_C; }
+
+// Float offsets of the behaviour net's flat parameters, in the order include/rl4rs_b200.h documents.
+struct OpeLayout { int64_t emb, w1, b1, w2, b2, fc_w, fc_b, obs_w, obs_b, rew_w, rew_b, n; };
+OpeLayout ope_layout(int H, int C) {
+  OpeLayout L;
+  int64_t o = 0;
+  auto take = [&](int64_t k) { const int64_t r = o; o += k; return r; };
+  L.emb = take((int64_t)H * E);
+  L.w1 = take((int64_t)NDENSE * OPE_U); L.b1 = take(OPE_U);
+  L.w2 = take((int64_t)OPE_U * OPE_U); L.b2 = take(OPE_U);
+  L.fc_w = take((int64_t)CAT_LD * OPE_F); L.fc_b = take(OPE_F);
+  L.obs_w = take((int64_t)OPE_F * OPE_F); L.obs_b = take(OPE_F);
+  L.rew_w = take((int64_t)OPE_F * C); L.rew_b = take(C);
+  L.n = o;
+  return L;
+}
+
+// C[M, N] (ldc) = epi(A[M, K] (lda) W[K, N] + bias), row-major operands
+int ope_mm(cudaStream_t st, const float* A, int lda, const float* W, float* C, int ldc, int M, int N, int K,
+           const float* bias, int epi) {
+  const Gemm g{Op{A, 0, 0, lda, 1}, Op{W, 0, 0, N, 1}, C, 0, 0, ldc, 1, bias, nullptr, nullptr, nullptr, M, N, K, 1, 0,
+               1.f, epi, 0};
+  return ope_launch("k_dense_gemm", gemm_kernel(g), dim3((N + GT - 1) / GT, (M + GT - 1) / GT), r4dense::NT, st, g);
+}
+}  // namespace
+
+extern "C" {
+
+int64_t r4_ope_num_params(int H, int C) {
+  if (H < 1 || H > OPE_MAX_H || !ope_c_ok(C)) return -1;
+  return ope_layout(H, C).n;
+}
+
+int64_t r4_ope_behavior_scratch_size(int B, int C) {
+  if (B < 1 || B > OPE_MAX_B || !ope_c_ok(C)) return -1;
+  return (int64_t)B * (NDENSE + OPE_U + CAT_LD + 2 * OPE_F + C);
+}
+
+int r4_ope_behavior(int B, int H, int C, int K, int P, int page, const float* params, const int32_t* head,
+                    const int32_t* items, const float* feat, float* out, float* scratch, void* stream) {
+  if (B < 1 || B > OPE_MAX_B || H < 1 || H > OPE_MAX_H || !ope_c_ok(C) || K < 1 || K > NCAT - NHEAD || P < 1 ||
+      page < 0 || page >= P || !params || !head || !items || !feat || !out || !scratch)
+    return fail(R4_ERR_ARG, "r4_ope_behavior: bad argument");
+  const OpeLayout L = ope_layout(H, C);
+  const cudaStream_t st = S(stream);
+  float* dense = scratch;
+  float* h1 = dense + (size_t)B * NDENSE;
+  float* cat = h1 + (size_t)B * OPE_U;
+  float* a = cat + (size_t)B * CAT_LD;
+  float* o = a + (size_t)B * OPE_F;
+  float* z = o + (size_t)B * OPE_F;
+  const float* p = params;
+  int rc;
+  if ((rc = ope_launch("k_ope_inputs", k_ope_inputs, dim3(B), E, st, B, K, P, page, H, head, items, feat, p + L.emb, cat,
+                       dense)) ||
+      (rc = ope_mm(st, dense, NDENSE, p + L.w1, h1, OPE_U, B, OPE_U, NDENSE, p + L.b1, EP_ELU)) ||
+      (rc = ope_mm(st, h1, OPE_U, p + L.w2, cat + E, CAT_LD, B, OPE_U, OPE_U, p + L.b2, EP_ELU)) ||
+      (rc = ope_mm(st, cat, CAT_LD, p + L.fc_w, a, OPE_F, B, OPE_F, CAT_LD, p + L.fc_b, EP_ELU)) ||
+      (rc = ope_mm(st, a, OPE_F, p + L.obs_w, o, OPE_F, B, OPE_F, OPE_F, p + L.obs_b, EP_ELU)) ||
+      (rc = ope_mm(st, o, OPE_F, p + L.rew_w, z, C, B, C, OPE_F, p + L.rew_b, EP_LIN)))
+    return rc;
+  return ope_launch("k_ope_softmax", k_ope_softmax, dim3(B), r4ope::NT, st, B, C, (const float*)z, out);
+}
+
+int r4_ope_step(int t, int T, int B, int A, int C, int layer, const float* probs, int logits, const int32_t* off,
+                const float* block, const int32_t* own, const float* values, int per_action, const double* reward,
+                const double* off_reward, float* pol, float* beh, float* val, double* rew, double* offr, void* stream) {
+  if (T < 1 || t < 0 || t >= T || B < 1 || B > OPE_MAX_B || A < 2 || A > OPE_MAX_A || !ope_c_ok(C) || C < A ||
+      layer < 1 || (logits != 0 && logits != 1) || (per_action != 0 && per_action != 1) || !probs || !off || !block ||
+      (per_action && !own) || !values || !reward || !off_reward || !pol || !beh || !val || !rew || !offr)
+    return fail(R4_ERR_ARG, "r4_ope_step: bad argument");
+  constexpr int rows = r4ope::NT / 32;
+  return ope_launch("k_ope_step", k_ope_step, dim3((B + rows - 1) / rows), r4ope::NT, S(stream), t, B, A, C, layer, probs,
+                    logits, off, block, own, values, per_action, reward, off_reward, pol, beh, val, rew, offr);
+}
+
+int64_t r4_ope_launch_count(void) { return g_launches[FAM_OPE].load(std::memory_order_relaxed); }
+
+}  // extern "C"

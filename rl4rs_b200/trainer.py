@@ -497,19 +497,33 @@ class _TrainerBase(object):
         return self._global_mean(torch.tensor(tot / episodes, device=self.device))
 
     @torch.no_grad()
-    def compute_actions(self, obs, explore=False):
+    def compute_actions(self, obs, explore=False, full_fetch=False):
         """trainer.compute_actions (modelfree_train.py:454): one batch of observations in the env's format (arrays or
         tensors), or RLlib's {env_id: observation} dict -> the actions: i32 [n] of the mask policy, clipped f32 [n, D] of the
-        Gaussian policy (a dict keyed like the input for the RLlib form)."""
+        Gaussian policy (a dict keyed like the input for the RLlib form).  full_fetch: RLlib 1.5's (actions, [], infos),
+        infos the batched extra fetches as arrays (_fetch)."""
         import numpy as np
         if isinstance(obs, dict) and not {"obs", "action_mask"} & obs.keys():      # RLlib's {env_id: observation} form
             keys = list(obs.keys())
             rows = [obs[k] for k in keys]
             if isinstance(rows[0], dict):
-                a = self.compute_actions({f: np.stack([np.asarray(r[f]) for r in rows]) for f in rows[0]}, explore)
+                batch = {f: np.stack([np.asarray(r[f]) for r in rows]) for f in rows[0]}
             else:
-                a = self.compute_actions(np.stack([np.asarray(r) for r in rows]), explore)
-            return dict(zip(keys, a.tolist() if a.ndim == 1 else list(a)))
+                batch = np.stack([np.asarray(r) for r in rows])
+            out = self.compute_actions(batch, explore, full_fetch)
+            a = out[0] if full_fetch else out
+            a = dict(zip(keys, a.tolist() if a.ndim == 1 else list(a)))
+            return (a, [], out[2]) if full_fetch else a
+        if full_fetch:
+            a, infos = self._fetch(obs, explore)
+            return a.cpu().numpy(), [], {k: v.cpu().numpy() for k, v in infos.items()}
+        return self._fetch(obs, explore, infos=False)[0].cpu().numpy()
+
+    @torch.no_grad()
+    def _fetch(self, obs, explore=False, infos=True):
+        """One act on a batch (arrays or tensors) -> (actions, RLlib's extra fetches) as device tensors: PPO / A2C / PG /
+        IMPALA's action_dist_inputs (the masked logits, or the Gaussian's mean | log_std), vf_preds, action_logp and
+        action_prob.  infos=False: (actions, None), and the act kernel writes no distribution inputs."""
         if isinstance(obs, dict):
             obs = {k: torch.as_tensor(v, device=self.device) for k, v in obs.items()}
         o, *mask = self.policy.inputs(obs)
@@ -517,15 +531,19 @@ class _TrainerBase(object):
         mask = [m.to(torch.uint8).contiguous() for m in mask]
         n = o.shape[0]
         e = lambda *s: torch.empty(*s, dtype=torch.float32, device=self.device)
+        logp, value = e(n), e(n)
         if not self.use_kernels:
-            a = self.policy.act(o, *mask, explore=explore)[1 if self.conti else 0]
+            out = self.policy.act(o, *mask, explore=explore)
+            a, logp, value, dist = (out[1], out[2], out[3], out[4]) if self.conti else out
         elif self.conti:
-            a = e(n, self.D)
-            self.ops.act(self.policy.flat, o, explore, self._seed, e(n, self.D), a, e(n), e(n), None)
+            a, dist = e(n, self.D), e(n, 2 * self.D) if infos else None
+            self.ops.act(self.policy.flat, o, explore, self._seed, e(n, self.D), a, logp, value, dist)
         else:
-            a = torch.empty(n, dtype=torch.int32, device=self.device)
-            self.ops.act(self.policy.flat, o, *mask, explore, self._seed, a, e(n), e(n), None)
-        return a.cpu().numpy()
+            a, dist = torch.empty(n, dtype=torch.int32, device=self.device), e(n, self.A) if infos else None
+            self.ops.act(self.policy.flat, o, *mask, explore, self._seed, a, logp, value, dist)
+        if not infos:
+            return a, None
+        return a, {"action_dist_inputs": dist, "vf_preds": value, "action_logp": logp, "action_prob": logp.exp()}
 
     # ---- checkpoint / resume (trainer.save / restore, modelfree_train.py:421-435) -----------------
     def save(self, checkpoint_dir):
@@ -1104,11 +1122,18 @@ class _ReplayTrainer(_TrainerBase):
         return self
 
     @torch.no_grad()
-    def compute_actions(self, obs, explore=False):
+    def compute_actions(self, obs, explore=False, full_fetch=False):
         if isinstance(obs, dict) and "obs" not in obs:                 # RLlib's {env_id: observation} form
-            return super().compute_actions(obs, explore)
+            return super().compute_actions(obs, explore, full_fetch)
+        if full_fetch:
+            a, infos = self._fetch(obs, explore)
+            return a.cpu().numpy(), [], {k: v.cpu().numpy() for k, v in infos.items()}
         o = torch.as_tensor(self.policy.inputs(obs)[0], dtype=torch.float32, device=self.device).contiguous()
         return self._act(o, explore, self._actions(o.shape[0])).cpu().numpy()
+
+    def _fetch(self, obs, explore=False):
+        raise NotImplementedError("%s: compute_actions(full_fetch=True) is built for PPO / A2C / PG / IMPALA and RAINBOW"
+                                  % self.algo)
 
     def train(self):
         c, w = self.config, _world()
@@ -1378,17 +1403,30 @@ class RainbowTrainer(_ReplayTrainer):
         return torch.zeros(*lead, dtype=torch.int32, device=self.device)
 
     @torch.no_grad()
-    def _act(self, obs, explore, out):
-        """out i32 [n] = the action of obs [n, 256]: SoftQ sampling when exploring, else argmax Q."""
+    def _act(self, obs, explore, out, q=None):
+        """out i32 [n] = the action of obs [n, 256]: SoftQ sampling when exploring, else argmax Q; q f32 [n, A] (may be
+        None) receives the expected Q."""
         n = obs.shape[0]
         if self.use_kernels:
-            self.ops.act(self.policy, obs, explore, self._seed, self.counter, out)
+            self.ops.act(self.policy, obs, explore, self._seed, self.counter, out, q)
         else:
-            out.copy_(self.policy.act(obs, explore, self._seed, self.counter)[0])
+            a, qq = self.policy.act(obs, explore, self._seed, self.counter)
+            out.copy_(a)
+            if q is not None:
+                q.copy_(qq)
         self.counter += n
         if explore:
             self.policy_ts += n * _world()
         return out
+
+    @torch.no_grad()
+    def _fetch(self, obs, explore=False):
+        """One act -> (actions, RLlib DQN's extra fetches): q_values, the expected Q [n, A], which is also its
+        action_dist_inputs."""
+        o = torch.as_tensor(self.policy.inputs(obs)[0], dtype=torch.float32, device=self.device).contiguous()
+        q = torch.empty(o.shape[0], self.A, dtype=torch.float32, device=self.device)
+        a = self._act(o, explore, self._actions(o.shape[0]), q)
+        return a, {"q_values": q, "action_dist_inputs": q}
 
     def _hp(self):
         c = self.config
