@@ -26,6 +26,7 @@
 #include <stdint.h>
 
 #include "r4_ddpg.cuh"
+#include "r4_dense.cuh"
 
 namespace r4bq {
 
@@ -372,21 +373,17 @@ __global__ void __launch_bounds__(NT) k_bq_rows(Layout L, Hyper hp, const float*
 inline r4dense::Jobs make_jobs(const Layout& L, const Planes& P) {
   r4dense::Jobs J;
   int k = 0;
-  auto layer = [&](const float* X, int ldx, const float* dZ, int M, int N, int w, int b) {
-    J.j[k++] = {X, dZ, ldx, M, N, w, 0};
-    J.j[k++] = {nullptr, dZ, 1, 1, N, b, 0};
-  };
   auto mnet = [&](const MNet& m, const MPlanes& M) {
-    layer(P.x, L.K, M.d1, L.K, H, m.w1, m.b1);
-    layer(M.he, HE, M.d2, HE, L.A, m.w2, m.b2);
-    layer(M.f, L.A, M.d3, L.A, L.A, m.w3, m.b3);
+    r4dense::layer_jobs(J, k, P.x, L.K, M.d1, L.K, H, m.w1, m.b1);
+    r4dense::layer_jobs(J, k, M.he, HE, M.d2, HE, L.A, m.w2, m.b2);
+    r4dense::layer_jobs(J, k, M.f, L.A, M.d3, L.A, L.A, m.w3, m.b3);
   };
   if (L.algo == BC) mnet(L.imi, P.mp[0]);
   if (L.algo == BCQ) { mnet(L.q, P.mp[0]); mnet(L.imi, P.mp[1]); }
   if (L.algo == CQL) {
-    layer(P.x, L.K, P.c1, L.K, H, L.c.w1, L.c.b1);
-    layer(P.h1, H, P.c2, H, H, L.c.w2, L.c.b2);
-    layer(P.h2, H, P.c3, H, L.A, L.c.w3, L.c.b3);
+    r4dense::layer_jobs(J, k, P.x, L.K, P.c1, L.K, H, L.c.w1, L.c.b1);
+    r4dense::layer_jobs(J, k, P.h1, H, P.c2, H, H, L.c.w2, L.c.b2);
+    r4dense::layer_jobs(J, k, P.h2, H, P.c3, H, L.A, L.c.w3, L.c.b3);
   }
   r4dense::tile_jobs(J, k);
   return J;
@@ -533,7 +530,3 @@ __global__ void __launch_bounds__(TRT) k_bq_transitions(const uint8_t* __restric
 }
 
 }  // namespace r4bq
-
-#include "r4_cqlconti.cuh"   // continuous-action CQL, on the same dataset planes and launch family
-#include "r4_bcqconti.cuh"   // continuous-action BCQ, likewise
-#include "r4_ope.cuh"         // off-policy evaluation of the batch-RL and model-free policies: its own launch family

@@ -25,6 +25,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "r4_batchrl.cuh"
 #include "r4_dense.cuh"
 #include "r4_ppo.cuh"
 

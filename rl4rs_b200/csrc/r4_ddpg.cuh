@@ -455,9 +455,9 @@ inline r4dense::Jobs make_jobs(const Layout& L, const Planes& P) {
   int k = 0;
   auto net = [&](const Net& q, const float* X, int ldx, const float* h1, const float* h2, const float* d1, const float* d2,
                  const float* d3) {
-    J.j[k++] = {X, d1, ldx, q.K, H1, q.w1, 0};     J.j[k++] = {nullptr, d1, 1, 1, H1, q.b1, 0};
-    J.j[k++] = {h1, d2, H1, H1, H2, q.w2, 0};      J.j[k++] = {nullptr, d2, 1, 1, H2, q.b2, 0};
-    J.j[k++] = {h2, d3, H2, H2, q.N3, q.w3, 0};    J.j[k++] = {nullptr, d3, 1, 1, q.N3, q.b3, 0};
+    r4dense::layer_jobs(J, k, X, ldx, d1, q.K, H1, q.w1, q.b1);
+    r4dense::layer_jobs(J, k, h1, H1, d2, H1, H2, q.w2, q.b2);
+    r4dense::layer_jobs(J, k, h2, H2, d3, H2, q.N3, q.w3, q.b3);
   };
   net(L.actor, P.x, XIN, P.ah1, P.ah2, P.ad1, P.ad2, P.ad3);
   net(L.q1, P.x, XIN, P.ch1[0], P.ch2[0], P.cd1[0], P.cd2[0], P.cd3[0]);

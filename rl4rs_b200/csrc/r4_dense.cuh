@@ -147,6 +147,16 @@ inline void tile_jobs(Jobs& J, int njob) {
   }
   J.ntiles = t;
 }
+// The job of the gradient [M][N] at grad + off from X (row stride ldx; NULL: a bias, M = 1) and dZ [n][N].
+inline Job grad_job(const float* X, int ldx, const float* dZ, int M, int N, int64_t off) {
+  return Job{X, dZ, ldx, M, N, (int)off, 0};
+}
+// Appends the two jobs of one dense layer over its output gradient dZ [n][N] at k: its weight [M][N] at off w from X at
+// row stride ldx, then its bias [N] at off b.
+inline void layer_jobs(Jobs& J, int& k, const float* X, int ldx, const float* dZ, int M, int N, int64_t w, int64_t b) {
+  J.j[k++] = grad_job(X, ldx, dZ, M, N, w);
+  J.j[k++] = grad_job(nullptr, 1, dZ, 1, N, b);
+}
 // The statistics: column c < cols of the rows in[n][cols], summed in row order from 0, or from run[c] when run is given and
 // first == 0.  run (may be NULL) keeps the sum; out (may be NULL) receives sum * scale, or with add fmaf(sum, scale, out).
 struct Stats {

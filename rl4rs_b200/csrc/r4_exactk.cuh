@@ -664,6 +664,3 @@ __global__ void k_ek_gloss(const float* __restrict__ ce, const float* __restrict
 }
 
 }  // namespace r4ek
-
-// The MDP checker's seq2seq transformer draws its dropout with r4ek::kept.
-#include "r4_seq2seq.cuh"

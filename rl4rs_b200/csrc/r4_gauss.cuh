@@ -301,16 +301,12 @@ __global__ void __launch_bounds__(NT) k_gauss_rows(Layout L, r4ppo::LossHyper hp
 inline r4dense::Jobs make_jobs(const Layout& L, const Planes& P) {
   r4dense::Jobs J;
   int k = 0;
-  auto layer = [&](const float* X, const float* dZ, int M, int N, int w, int b) {
-    J.j[k++] = {X, dZ, M, M, N, w, 0};
-    J.j[k++] = {nullptr, dZ, 1, 1, N, b, 0};
-  };
-  layer(P.x, P.d1, OBS, H, L.p_w1, L.p_b1);
-  layer(P.h1, P.d2, H, H, L.p_w2, L.p_b2);
-  layer(P.h2, P.dout, H, 2 * L.D, L.p_wo, L.p_bo);
-  layer(P.x, P.e1, OBS, H, L.v_w1, L.v_b1);
-  layer(P.g1, P.e2, H, H, L.v_w2, L.v_b2);
-  layer(P.g2, P.dv, H, 1, L.v_wo, L.v_bo);
+  r4dense::layer_jobs(J, k, P.x, OBS, P.d1, OBS, H, L.p_w1, L.p_b1);
+  r4dense::layer_jobs(J, k, P.h1, H, P.d2, H, H, L.p_w2, L.p_b2);
+  r4dense::layer_jobs(J, k, P.h2, H, P.dout, H, 2 * L.D, L.p_wo, L.p_bo);
+  r4dense::layer_jobs(J, k, P.x, OBS, P.e1, OBS, H, L.v_w1, L.v_b1);
+  r4dense::layer_jobs(J, k, P.g1, H, P.e2, H, H, L.v_w2, L.v_b2);
+  r4dense::layer_jobs(J, k, P.g2, H, P.dv, H, 1, L.v_wo, L.v_bo);
   r4dense::tile_jobs(J, k);
   return J;
 }

@@ -9,9 +9,13 @@
 #include "r4_ddpg.cuh"
 #include "r4_rainbow.cuh"
 #include "r4_batchrl.cuh"
+#include "r4_cqlconti.cuh"
+#include "r4_bcqconti.cuh"
 #include "r4_simtrain.cuh"
 #include "r4_dense.cuh"
 #include "r4_exactk.cuh"
+#include "r4_seq2seq.cuh"
+#include "r4_ope.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -29,6 +33,41 @@ using namespace r4dense;
 // H100.  This never-launched kernel keeps a 1024-byte-aligned array in use, so the learner module keeps the alignment.
 extern __shared__ __align__(1024) uint8_t r4_learn_smem_align[];
 __global__ void r4_learn_smem_align_anchor() { r4_learn_smem_align[threadIdx.x] = 0; }
+
+// ---- the shared dense kernels (r4_dense.cuh): every family launches k_dense_gemm and k_dense_wgrad through these -----------
+namespace {
+unsigned blocks(int64_t n, int per) { return (unsigned)((n + per - 1) / per); }
+
+// a [rows, cols] row-major matrix at leading dimension ld as a GEMM operand, or its transpose
+Op rm(const float* p, int64_t ld) { return Op{p, 0, 0, ld, 1}; }
+Op tr(const float* p, int64_t ld) { return Op{p, 0, 0, 1, ld}; }
+
+// k_dense_gemm over the 64 x 64 tiles of C in z batches
+int dense_gemm(Family fam, cudaStream_t st, const Gemm& g, unsigned z) {
+  return launch(fam, "k_dense_gemm", gemm_kernel(g), dim3(blocks(g.N, GT), blocks(g.M, GT), z), NT, 0, st, false, g);
+}
+
+// C[M, N] (ldc) (+ C when accum) = epi(A B + bias), aux the forward activation of a derivative epilogue; pre and mul as
+// k_dense_gemm's epilogue
+int dense_mm(Family fam, cudaStream_t st, Op A, Op B, float* C, int64_t ldc, int M, int N, int K, const float* bias = nullptr,
+             int accum = 0, int epi = EP_LIN, const float* aux = nullptr, const float* mul = nullptr, float* pre = nullptr) {
+  return dense_gemm(fam, st, Gemm{A, B, C, 0, 0, ldc, 1, bias, aux, mul, pre, M, N, K, 1, 0, 1.f, epi, accum}, 1);
+}
+
+// Per (group, head) products C = alpha A B, batch z = g H + h, element (m, n) of C at C + g cso + h csi + m cs0 + n.
+// ktot > 0: split-K instead, G partials (H = 1) of K rows each out of ktot, partial g at C + g cso.
+int dense_bmm(Family fam, cudaStream_t st, Op A, Op B, float* C, int64_t cso, int64_t csi, int64_t cs0, int M, int N, int K,
+              int64_t G, int H, float alpha, int64_t ktot = 0) {
+  const Gemm g{A, B, C, cso, csi, cs0, 1, nullptr, nullptr, nullptr, nullptr, M, N, K, H, ktot, alpha, EP_LIN, 0};
+  return dense_gemm(fam, st, g, (unsigned)(G * H));
+}
+
+// k_dense_wgrad over the tiled jobs J on n rows (first: store the gradients, else add them), with its ntiles + 1 CTAs:
+// the last sums the statistics s, and returns at once without them.
+int dense_wgrad(Family fam, cudaStream_t st, const Jobs& J, int64_t n, int first, float* grad, const Stats& s = Stats{}) {
+  return launch(fam, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, st, false, J, (int)n, first, grad, s);
+}
+}  // namespace
 
 struct r4_comm {
   int rank = 0, world = 1, n = 0, nblk = 0, device = 0;
@@ -304,8 +343,8 @@ static int gauss_grad_impl(int mode, const float* params, const float* obs, cons
                     r4gauss::ROWS_SMEM, S(stream), false, L, hp, params, obs, action, old_logp, old_dist, old_value, adv, target,
                     idx, c0, cn, P);
     if (!rc)
-      rc = launch(FAM_ONLINE, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, S(stream), false, J, cn, c0 == 0, grad_out,
-                  Stats{P.stats, 5, stat_sum, last ? stats_accum : nullptr, stat_scale, 1});
+      rc = dense_wgrad(FAM_ONLINE, S(stream), J, cn, c0 == 0, grad_out,
+                       Stats{P.stats, 5, stat_sum, last ? stats_accum : nullptr, stat_scale, 1});
     if (rc) return rc;
   }
   return R4_OK;
@@ -537,8 +576,7 @@ int r4_ddpg_grad(const float* params, const float* target, int action_dim, int t
   if (int rc = launch(FAM_ONLINE, "k_ddpg_rows", r4ddpg::k_ddpg_rows, (n + r4ddpg::TS - 1) / r4ddpg::TS, r4ddpg::NT,
                       r4ddpg::ROWS_SMEM, S(stream), false, L, hp, params, target, R, idx, weights, smooth_noise, n, P))
     return rc;
-  return launch(FAM_ONLINE, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, S(stream), false, J, n, 1, grad,
-                Stats{P.stats, 3, nullptr, stats, inv_n, 0});
+  return dense_wgrad(FAM_ONLINE, S(stream), J, n, 1, grad, Stats{P.stats, 3, nullptr, stats, inv_n, 0});
 }
 
 int r4_ddpg_apply(float* params, float* target, const float* grad, float* m, float* v, int action_dim, int twin, int actor_step,
@@ -633,8 +671,7 @@ int r4_rainbow_grad(const float* params, const float* target, int num_actions, i
   if (int rc = launch(FAM_ONLINE, "k_rainbow_rows", r4rb::k_rainbow_rows, (n + r4rb::TS - 1) / r4rb::TS, r4rb::NT,
                       r4rb::rows_smem(L.A, L.AZ), S(stream), false, L, hp, params, target, R, idx, weights, n, P))
     return rc;
-  return launch(FAM_ONLINE, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, S(stream), false, J, n, 1, grad,
-                Stats{P.stats, 3, nullptr, stats, inv_n, 0});
+  return dense_wgrad(FAM_ONLINE, S(stream), J, n, 1, grad, Stats{P.stats, 3, nullptr, stats, inv_n, 0});
 }
 
 int r4_rainbow_apply(float* params, float* target, const float* grad, float* m, float* v, int num_actions, int num_atoms,
@@ -741,9 +778,7 @@ static int bq_grad(int algo, int K, int A, const float* params, const float* tar
                   L, hp, params, target, bq_data(data), idx, n, P);
   if (rc) return rc;
   const Jobs J = r4bq::make_jobs(L, P);
-  if ((rc = launch(FAM_BATCHRL, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, st, false, J, n, 1, grad,
-                   Stats{P.stats, 3, nullptr, stats, 1.0f / (float)n, 0})))
-    return rc;
+  if ((rc = dense_wgrad(FAM_BATCHRL, st, J, n, 1, grad, Stats{P.stats, 3, nullptr, stats, 1.0f / (float)n, 0}))) return rc;
   const int nets = r4bq::n_mnets(algo);
   if (!nets) return R4_OK;
   const int per = (A * r4bq::E + r4bq::EGT - 1) / r4bq::EGT;
@@ -813,43 +848,33 @@ int r4_batchrl_act(int algo, int obs_dim, int action_size, const float* params, 
 namespace {
 using r4cqlc::H;
 
-// C = epi(A B + bias): A row-major [M][K] at row stride lda, B = W [K][N] row-major, or its transpose (bt: W [N][K]).
-int cq_gemm(cudaStream_t st, const float* A, int lda, const float* W, int ldw, bool bt, float* C, int M, int N, int K,
-            const float* bias, int epi, const float* aux, int accum) {
-  const Op b = bt ? Op{W, 0, 0, 1, ldw} : Op{W, 0, 0, ldw, 1};
-  const Gemm g{Op{A, 0, 0, lda, 1}, b, C, 0, 0, N, 1, bias, aux, nullptr, nullptr, M, N, K, 1, 0, 1.f, epi, accum};
-  return launch(FAM_BATCHRL, "k_dense_gemm", gemm_kernel(g), dim3((N + GT - 1) / GT, (M + GT - 1) / GT), NT, 0, st, false, g);
-}
 // the relu MLP of net m on rows x [M][m.in] -> h1, h2 [M][H], out [M][m.out]
 int cq_forward(cudaStream_t st, const float* prm, const r4cqlc::Net& m, const float* x, int M, float* h1, float* h2,
                float* out) {
   int rc;
-  if ((rc = cq_gemm(st, x, m.in, prm + m.w1, H, false, h1, M, H, m.in, prm + m.b1, EP_RELU, nullptr, 0))) return rc;
-  if ((rc = cq_gemm(st, h1, H, prm + m.w2, H, false, h2, M, H, H, prm + m.b2, EP_RELU, nullptr, 0))) return rc;
-  return cq_gemm(st, h2, H, prm + m.w3, m.out, false, out, M, m.out, H, prm + m.b3, EP_LIN, nullptr, 0);
+  if ((rc = dense_mm(FAM_BATCHRL, st, rm(x, m.in), rm(prm + m.w1, H), h1, H, M, H, m.in, prm + m.b1, 0, EP_RELU))) return rc;
+  if ((rc = dense_mm(FAM_BATCHRL, st, rm(h1, H), rm(prm + m.w2, H), h2, H, M, H, H, prm + m.b2, 0, EP_RELU))) return rc;
+  return dense_mm(FAM_BATCHRL, st, rm(h2, H), rm(prm + m.w3, m.out), out, m.out, M, m.out, H, prm + m.b3);
 }
 // dout [M][m.out] -> dz2 = dout W3^T [h2 > 0], dz1 = dz2 W2^T [h1 > 0]
 int cq_backward(cudaStream_t st, const float* prm, const r4cqlc::Net& m, const float* dout, int M, const float* h1,
                 const float* h2, float* dz2, float* dz1) {
   int rc;
-  if ((rc = cq_gemm(st, dout, m.out, prm + m.w3, m.out, true, dz2, M, H, m.out, nullptr, EP_DRELU, h2, 0))) return rc;
-  return cq_gemm(st, dz2, H, prm + m.w2, H, true, dz1, M, H, H, nullptr, EP_DRELU, h1, 0);
+  if ((rc = dense_mm(FAM_BATCHRL, st, rm(dout, m.out), tr(prm + m.w3, m.out), dz2, H, M, H, m.out, nullptr, 0, EP_DRELU, h2)))
+    return rc;
+  return dense_mm(FAM_BATCHRL, st, rm(dz2, H), tr(prm + m.w2, H), dz1, H, M, H, H, nullptr, 0, EP_DRELU, h1);
 }
 // the six weight-gradient jobs of net m over rows x, h1, h2 and their output gradients dz1, dz2, dout
 void cq_jobs(Jobs& J, int& k, const r4cqlc::Net& m, const float* x, const float* h1, const float* h2, const float* dz1,
              const float* dz2, const float* dout) {
-  J.j[k++] = {x, dz1, m.in, m.in, H, m.w1, 0};
-  J.j[k++] = {nullptr, dz1, 1, 1, H, m.b1, 0};
-  J.j[k++] = {h1, dz2, H, H, H, m.w2, 0};
-  J.j[k++] = {nullptr, dz2, 1, 1, H, m.b2, 0};
-  J.j[k++] = {h2, dout, H, H, m.out, m.w3, 0};
-  J.j[k++] = {nullptr, dout, 1, 1, m.out, m.b3, 0};
+  layer_jobs(J, k, x, m.in, dz1, m.in, H, m.w1, m.b1);
+  layer_jobs(J, k, h1, H, dz2, H, H, m.w2, m.b2);
+  layer_jobs(J, k, h2, H, dout, H, m.out, m.w3, m.b3);
 }
 template <typename... P, typename... A>
 int cq_launch(const char* name, void (*kernel)(P...), unsigned grid, cudaStream_t st, bool pdl, A&&... args) {
   return launch(FAM_BATCHRL, name, kernel, grid, r4cqlc::NT, 0, st, pdl, std::forward<A>(args)...);
 }
-unsigned cq_blocks(int64_t n, int per) { return (unsigned)((n + per - 1) / per); }
 
 // One SGD step at 1-based step `step` (the noise counter): temperature, alpha, critic, actor.  apply: each phase's Adam
 // (the critic's with the soft target update) runs before the next phase; else the phases' gradients at the given
@@ -865,18 +890,18 @@ int cq_step(const r4cqlc::Layout& L, const r4cqlc::Hyper& hp, float* prm, float*
   if ((rc = cq_forward(st, prm, L.actor, P.xs, n, P.ah1, P.ah2, P.ao))) return rc;
   if ((rc = cq_launch("k_cqlc_temp", k_cqlc_temp, 1, st, pdl, L, hp, n, P, prm, m, v, ap, apply, stats))) return rc;
   // alpha
-  if ((rc = cq_launch("k_cqlc_pack", k_cqlc_pack, cq_blocks(R, NT / 32), st, pdl, L, S, n, (int)PK_ALPHA, P))) return rc;
+  if ((rc = cq_launch("k_cqlc_pack", k_cqlc_pack, blocks(R, NT / 32), st, pdl, L, S, n, (int)PK_ALPHA, P))) return rc;
   for (int k = 0; k < 2; ++k)
     if ((rc = cq_forward(st, prm, L.c[k], P.x, R, P.c[k].h1, P.c[k].h2, P.c[k].q))) return rc;
   if ((rc = cq_launch("k_cqlc_loss", k_cqlc_loss, 1, st, pdl, L, hp, n, (int)PH_ALPHA, P, prm, m, v, ap, apply, stats))) return rc;
   // critic: the target on s', then the critic rows
   if ((rc = cq_forward(st, prm, L.actor, P.xn, n, P.nh1, P.nh2, P.no))) return rc;
-  if ((rc = cq_launch("k_cqlc_pack", k_cqlc_pack, cq_blocks(n, NT / 32), st, pdl, L, S, n, (int)PK_TARGET, P))) return rc;
+  if ((rc = cq_launch("k_cqlc_pack", k_cqlc_pack, blocks(n, NT / 32), st, pdl, L, S, n, (int)PK_TARGET, P))) return rc;
   for (int k = 0; k < 2; ++k)
     if ((rc = cq_forward(st, tgt, r4cqlc::make_net(L.c[k].w1 - L.t0, L.c[k].in, L.c[k].out), P.x, n, P.c[k].h1, P.c[k].h2,
                          P.qt + (size_t)k * n)))
       return rc;
-  if ((rc = cq_launch("k_cqlc_pack", k_cqlc_pack, cq_blocks(R, NT / 32), st, pdl, L, S, n, (int)PK_CRITIC, P))) return rc;
+  if ((rc = cq_launch("k_cqlc_pack", k_cqlc_pack, blocks(R, NT / 32), st, pdl, L, S, n, (int)PK_CRITIC, P))) return rc;
   for (int k = 0; k < 2; ++k)
     if ((rc = cq_forward(st, prm, L.c[k], P.x, R, P.c[k].h1, P.c[k].h2, P.c[k].q))) return rc;
   if ((rc = cq_launch("k_cqlc_loss", k_cqlc_loss, 1, st, pdl, L, hp, n, (int)PH_CRITIC, P, prm, m, v, ap, apply, stats))) return rc;
@@ -888,30 +913,30 @@ int cq_step(const r4cqlc::Layout& L, const r4cqlc::Hyper& hp, float* prm, float*
     cq_jobs(J, nj, L.c[k], P.x, c.h1, c.h2, c.dz1, c.dz2, c.dq);
   }
   tile_jobs(J, nj);
-  const Stats none{nullptr, 0, nullptr, nullptr, 0.f, 0};
-  if ((rc = launch(FAM_BATCHRL, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, st, false, J, R, 1, P.grad, none))) return rc;
-  if (apply && (rc = cq_launch("k_cqlc_adam", k_cqlc_adam, cq_blocks(L.ntgt, NT), st, pdl, L.t0, L.ntgt, prm,
+  if ((rc = dense_wgrad(FAM_BATCHRL, st, J, R, 1, P.grad))) return rc;
+  if (apply && (rc = cq_launch("k_cqlc_adam", k_cqlc_adam, blocks(L.ntgt, NT), st, pdl, L.t0, L.ntgt, prm,
                                (const float*)P.grad, m, v, step, hp.lr_critic, hp.eps, tgt, hp.tau)))
     return rc;
   // actor: d(-min_k Q_k)/da through the critics, then the squashed head and the actor's layers
-  if ((rc = cq_launch("k_cqlc_pack", k_cqlc_pack, cq_blocks(n, NT / 32), st, pdl, L, S, n, (int)PK_ACTOR, P))) return rc;
+  if ((rc = cq_launch("k_cqlc_pack", k_cqlc_pack, blocks(n, NT / 32), st, pdl, L, S, n, (int)PK_ACTOR, P))) return rc;
   for (int k = 0; k < 2; ++k)
     if ((rc = cq_forward(st, prm, L.c[k], P.x, n, P.c[k].h1, P.c[k].h2, P.c[k].q))) return rc;
   if ((rc = cq_launch("k_cqlc_loss", k_cqlc_loss, 1, st, pdl, L, hp, n, (int)PH_ACTOR, P, prm, m, v, ap, apply, stats))) return rc;
   for (int k = 0; k < 2; ++k) {
     const CPlanes& c = P.c[k];
     if ((rc = cq_backward(st, prm, L.c[k], c.dq, n, c.h1, c.h2, c.dz2, c.dz1))) return rc;
-    if ((rc = cq_gemm(st, c.dz1, H, prm + L.c[k].w1 + (size_t)L.K * H, H, true, P.da, n, L.D, H, nullptr, EP_LIN, nullptr, k)))
+    if ((rc = dense_mm(FAM_BATCHRL, st, rm(c.dz1, H), tr(prm + L.c[k].w1 + (size_t)L.K * H, H), P.da, L.D, n, L.D, H, nullptr,
+                       k)))
       return rc;
   }
-  if ((rc = cq_launch("k_cqlc_head", k_cqlc_head, cq_blocks((int64_t)n * L.D, NT), st, pdl, L, hp, n, P, (const float*)prm)))
+  if ((rc = cq_launch("k_cqlc_head", k_cqlc_head, blocks((int64_t)n * L.D, NT), st, pdl, L, hp, n, P, (const float*)prm)))
     return rc;
   if ((rc = cq_backward(st, prm, L.actor, P.dout, n, P.ah1, P.ah2, P.adz2, P.adz1))) return rc;
   nj = 0;
   cq_jobs(J, nj, L.actor, P.xs, P.ah1, P.ah2, P.adz1, P.adz2, P.dout);
   tile_jobs(J, nj);
-  if ((rc = launch(FAM_BATCHRL, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, st, false, J, n, 1, P.grad, none))) return rc;
-  if (apply && (rc = cq_launch("k_cqlc_adam", k_cqlc_adam, cq_blocks(L.actor.end, NT), st, pdl, 0, L.actor.end, prm,
+  if ((rc = dense_wgrad(FAM_BATCHRL, st, J, n, 1, P.grad))) return rc;
+  if (apply && (rc = cq_launch("k_cqlc_adam", k_cqlc_adam, blocks(L.actor.end, NT), st, pdl, 0, L.actor.end, prm,
                                (const float*)P.grad, m, v, step, hp.lr_actor, hp.eps, (float*)nullptr, 0.f)))
     return rc;
   return R4_OK;
@@ -993,11 +1018,11 @@ int r4_cqlc_act(int obs_dim, int action_dim, const float* params, const void* ob
   float* ch = xa + (size_t)n * (K + D);          // per critic: h1, h2 [n][H], q [n]
   const int64_t total = (int64_t)n * K;
   int rc;
-  if ((rc = cq_launch("k_cqlc_obs", k_cqlc_obs, cq_blocks(total, NT), st, false, obs_f64 ? nullptr : (const float*)obs,
+  if ((rc = cq_launch("k_cqlc_obs", k_cqlc_obs, blocks(total, NT), st, false, obs_f64 ? nullptr : (const float*)obs,
                       obs_f64 ? (const double*)obs : nullptr, total, x)))
     return rc;
   if ((rc = cq_forward(st, params, L.actor, x, n, h1, h2, o))) return rc;
-  if ((rc = cq_launch("k_cqlc_predict", k_cqlc_predict, cq_blocks((int64_t)n * (K + D), NT), st, false, K, D, n,
+  if ((rc = cq_launch("k_cqlc_predict", k_cqlc_predict, blocks((int64_t)n * (K + D), NT), st, false, K, D, n,
                       (const float*)x, (const float*)o, action_in, action, q ? xa : nullptr)))
     return rc;
   if (!q) return R4_OK;
@@ -1007,7 +1032,7 @@ int r4_cqlc_act(int obs_dim, int action_dim, const float* params, const void* ob
     qk[k] = c + (size_t)n * 2 * H;
     if ((rc = cq_forward(st, params, L.c[k], xa, n, c, c + (size_t)n * H, qk[k]))) return rc;
   }
-  return cq_launch("k_cqlc_qmean", k_cqlc_qmean, cq_blocks(n, NT), st, false, n, (const float*)qk[0], (const float*)qk[1], q);
+  return cq_launch("k_cqlc_qmean", k_cqlc_qmean, blocks(n, NT), st, false, n, (const float*)qk[0], (const float*)qk[1], q);
 }
 
 }  // extern "C"
@@ -1028,47 +1053,36 @@ static bool st_data_ok(const r4_simtrain_data* d) {
   return d && d->user_cat && d->user_dense && d->sequence_id && d->items && d->feedback && d->item_feature && d->seq;
 }
 
-static int st_gemm(bool tb, const float* A, int lda, const float* B, int ldb, const float* bias, float* C, int ldc, int M, int N,
-                   int K, int epi, cudaStream_t st, const float* aux = nullptr, const float* mul = nullptr, float* pre = nullptr,
-                   int accum = 0) {
-  const Op b = tb ? Op{B, 0, 0, 1, ldb} : Op{B, 0, 0, ldb, 1};
-  const Gemm g{Op{A, 0, 0, lda, 1}, b, C, 0, 0, ldc, 1, bias, aux, mul, pre, M, N, K, 1, 0, 1.f, epi, accum};
-  return st_launch("k_dense_gemm", gemm_kernel(g), dim3((N + GT - 1) / GT, (M + GT - 1) / GT), NT, st, g);
-}
-
 // The pieces every net shares.  Lay / Pl are a net's layout and planes (Layout / Planes for DIEN, NLayout / NPlanes for the
 // others), which name the dense tower's weights and planes alike.
 // The dense tower with dropout: T1d = ELU(dense dw1 + db1) keep0 (T1 before the keep), out (ld ldo) = ELU(T1d dw2 + db2) keep1.
 template <class Lay, class Pl>
 static int st_tower(const Lay& L, const float* prm, const Pl& P, int n, float* out, int ldo, cudaStream_t st) {
   using namespace r4st;
-  const int rc = st_gemm(false, P.dense, ND, prm + L.dw1, U, prm + L.db1, P.T1d, U, n, U, ND, EP_ELU, st, nullptr, P.keep, P.T1);
-  return rc ? rc : st_gemm(false, P.T1d, U, prm + L.dw2, U, prm + L.db2, out, ldo, n, U, U, EP_ELU, st, nullptr, P.keep + (size_t)n * U, P.T2);
+  const int rc = dense_mm(FAM_SIMTRAIN, st, rm(P.dense, ND), rm(prm + L.dw1, U), P.T1d, U, n, U, ND, prm + L.db1, 0, EP_ELU,
+                          nullptr, P.keep, P.T1);
+  return rc ? rc : dense_mm(FAM_SIMTRAIN, st, rm(P.T1d, U), rm(prm + L.dw2, U), out, ldo, n, U, U, prm + L.db2, 0, EP_ELU,
+                            nullptr, P.keep + (size_t)n * U, P.T2);
 }
 // Its backward from the layer above: dT2 = (dtop W^T) elu'(T2) keep1, with W the rows of that layer's weight (ld wide) the
 // tower feeds, then dT1 = (dT2 dw2^T) elu'(T1) keep0.
 template <class Lay, class Pl>
 static int st_tower_bwd(const Lay& L, const float* prm, const Pl& P, int n, const float* dtop, const float* W, int ld, cudaStream_t st) {
   using namespace r4st;
-  const int rc = st_gemm(true, dtop, ld, W, ld, nullptr, P.dT2, U, n, U, ld, EP_DELU, st, P.T2, P.keep + (size_t)n * U);
-  return rc ? rc : st_gemm(true, P.dT2, U, prm + L.dw2, U, nullptr, P.dT1, U, n, U, U, EP_DELU, st, P.T1, P.keep);
+  const int rc = dense_mm(FAM_SIMTRAIN, st, rm(dtop, ld), tr(W, ld), P.dT2, U, n, U, ld, nullptr, 0, EP_DELU, P.T2,
+                          P.keep + (size_t)n * U);
+  return rc ? rc : dense_mm(FAM_SIMTRAIN, st, rm(P.dT2, U), tr(prm + L.dw2, U), P.dT1, U, n, U, U, nullptr, 0, EP_DELU, P.T1,
+                            P.keep);
 }
 
-static Job st_job(const float* X, int ldx, const float* Z, int M, int N, int64_t off) {
-  return Job{X, Z, ldx, M, N, (int)off, 0};
-}
 // the tower's four weight-gradient jobs, the first of a net's n-row jobs; returns the job count
 template <class Lay, class Pl>
 static int st_tower_jobs(Jobs& J, const Lay& L, const Pl& P) {
   using namespace r4st;
   int k = 0;
-  J.j[k++] = st_job(P.dense, ND, P.dT1, ND, U, L.dw1);  J.j[k++] = st_job(nullptr, 1, P.dT1, 1, U, L.db1);
-  J.j[k++] = st_job(P.T1d, U, P.dT2, U, U, L.dw2);      J.j[k++] = st_job(nullptr, 1, P.dT2, 1, U, L.db2);
+  layer_jobs(J, k, P.dense, ND, P.dT1, ND, U, L.dw1, L.db1);
+  layer_jobs(J, k, P.T1d, U, P.dT2, U, U, L.dw2, L.db2);
   return k;
-}
-static int st_wgrad(Jobs J, int njob, int rows, float* grad, cudaStream_t st) {
-  tile_jobs(J, njob);
-  return st_launch("k_dense_wgrad", k_dense_wgrad, J.ntiles, NT, st, J, rows, 1, grad, Stats{});
 }
 
 // The head's loss: logits Z [n][C] -> dZ (may be NULL), the per-sample rows srow, stats, acc and probs.
@@ -1120,22 +1134,25 @@ static int st_forward(int head, const r4st::Layout& L, const float* prm, const r
   for (int i = 0; i < 2; ++i) {
     const Seq& w = L.s[i];
     const SeqPlanes& s = P.sp[i];
-    if ((rc = st_gemm(false, s.X, E, prm + w.gwg, 2 * E, prm + w.gbg, s.XG1, 2 * E, R, 2 * E, E, EP_LIN, st))) return rc;
-    if ((rc = st_gemm(false, s.X, E, prm + w.gwc, E, prm + w.gbc, s.XC1, E, R, E, E, EP_LIN, st))) return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(s.X, E), rm(prm + w.gwg, 2 * E), s.XG1, 2 * E, R, 2 * E, E, prm + w.gbg))) return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(s.X, E), rm(prm + w.gwc, E), s.XC1, E, R, E, E, prm + w.gbc))) return rc;
     const RecArgs<E> g1{prm + w.gwg + E * 2 * E, prm + w.gwc + E * E, s.XG1, s.XC1, nullptr, s.Hp1, s.G1, s.C1, s.RH1, s.H1, nullptr, 0, n};
     if ((rc = st_launch("k_st_gru_fwd<128>", k_st_gru_fwd<E>, (n + SB - 1) / SB, NTH, st, g1))) return rc;
     if ((rc = st_launch("k_st_attin", k_st_attin, (unsigned)(((size_t)R * E + 255) / 256), 256, st, P.q, s.H1, s.Ain, n))) return rc;
-    if ((rc = st_gemm(false, s.Ain, 4 * E, prm + w.aw1, A1, prm + w.ab1, s.At1, A1, R, A1, 4 * E, EP_SIG, st))) return rc;
-    if ((rc = st_gemm(false, s.At1, A1, prm + w.aw2, A2, prm + w.ab2, s.At2, A2, R, A2, A1, EP_SIG, st))) return rc;
-    if ((rc = st_gemm(false, s.At2, A2, prm + w.ak, 1, prm + w.ab, s.S, 1, R, 1, A2, EP_LIN, st))) return rc;
-    if ((rc = st_gemm(false, s.H1, E, prm + w.uwg, 4 * E, prm + w.ubg, s.XG2, 4 * E, R, 4 * E, E, EP_LIN, st))) return rc;
-    if ((rc = st_gemm(false, s.H1, E, prm + w.uwc, 2 * E, prm + w.ubc, s.XC2, 2 * E, R, 2 * E, E, EP_LIN, st))) return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(s.Ain, 4 * E), rm(prm + w.aw1, A1), s.At1, A1, R, A1, 4 * E, prm + w.ab1, 0, EP_SIG)))
+      return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(s.At1, A1), rm(prm + w.aw2, A2), s.At2, A2, R, A2, A1, prm + w.ab2, 0, EP_SIG)))
+      return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(s.At2, A2), rm(prm + w.ak, 1), s.S, 1, R, 1, A2, prm + w.ab))) return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(s.H1, E), rm(prm + w.uwg, 4 * E), s.XG2, 4 * E, R, 4 * E, E, prm + w.ubg))) return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(s.H1, E), rm(prm + w.uwc, 2 * E), s.XC2, 2 * E, R, 2 * E, E, prm + w.ubc))) return rc;
     const RecArgs<HA> g2{prm + w.uwg + E * 4 * E, prm + w.uwc + E * 2 * E, s.XG2, s.XC2, s.S, s.Hp2, s.G2, s.C2, s.RH2, nullptr,
                          P.allf + i * HA, FEAT, n};
     if ((rc = st_launch("k_st_gru_fwd<256>", k_st_gru_fwd<HA>, (n + SB - 1) / SB, NTH, st, g2))) return rc;
   }
-  if ((rc = st_gemm(false, P.allf, FEAT, prm + L.ow, OBS, prm + L.ob, P.O, OBS, n, OBS, FEAT, EP_ELU, st))) return rc;
-  if ((rc = st_gemm(false, P.O, OBS, prm + L.rw, C, prm + L.rb, P.Z, C, n, C, OBS, EP_LIN, st))) return rc;
+  if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.allf, FEAT), rm(prm + L.ow, OBS), P.O, OBS, n, OBS, FEAT, prm + L.ob, 0, EP_ELU)))
+    return rc;
+  if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.O, OBS), rm(prm + L.rw, C), P.Z, C, n, C, OBS, prm + L.rb))) return rc;
   return st_loss(head, D, idx, n, P.Z, with_grad ? P.dZ : nullptr, P.stats, stats, acc, probs, st);
 }
 
@@ -1145,8 +1162,9 @@ static int st_backward(int head, const r4st::Layout& L, const float* prm, const 
   const int R = n * T, C = head_classes(head);
   int rc;
   // head: dO = dZ rew_w^T elu'(O); dAllf = dO obs_w^T; the dense tower's columns again with its activation and dropout
-  if ((rc = st_gemm(true, P.dZ, C, prm + L.rw, C, nullptr, P.dO, OBS, n, OBS, C, EP_DELU, st, P.O))) return rc;
-  if ((rc = st_gemm(true, P.dO, OBS, prm + L.ow, OBS, nullptr, P.dAllf, FEAT, n, FEAT, OBS, EP_LIN, st))) return rc;
+  if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.dZ, C), tr(prm + L.rw, C), P.dO, OBS, n, OBS, C, nullptr, 0, EP_DELU, P.O)))
+    return rc;
+  if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.dO, OBS), tr(prm + L.ow, OBS), P.dAllf, FEAT, n, FEAT, OBS))) return rc;
   if ((rc = st_tower_bwd(L, prm, P, n, P.dO, prm + L.ow + (int64_t)F_DENSE * OBS, OBS, st))) return rc;
   if ((rc = st_launch("k_st_cat_bwd", k_st_cat_bwd, n, E, st, P.allf, P.P, P.dAllf, P.dEcat))) return rc;
   for (int i = 0; i < 2; ++i) {
@@ -1155,43 +1173,45 @@ static int st_backward(int head, const r4st::Layout& L, const float* prm, const 
     const RecBack<HA> b2{prm + w.uwg + E * 4 * E, prm + w.uwc + E * 2 * E, s.Hp2, s.G2, s.C2, s.S, nullptr, P.dAllf + i * HA, FEAT,
                          s.XG2, s.XC2, s.dS, n};
     if ((rc = st_launch("k_st_gru_bwd<256>", k_st_gru_bwd<HA>, (n + SB - 1) / SB, NTH, st, b2))) return rc;
-    if ((rc = st_gemm(true, s.XG2, 4 * E, prm + w.uwg, 4 * E, nullptr, s.dH1, E, R, E, 4 * E, EP_LIN, st))) return rc;
-    if ((rc = st_gemm(true, s.XC2, 2 * E, prm + w.uwc, 2 * E, nullptr, s.dH1, E, R, E, 2 * E, EP_LIN, st, nullptr, nullptr,
-                      nullptr, 1)))
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(s.XG2, 4 * E), tr(prm + w.uwg, 4 * E), s.dH1, E, R, E, 4 * E))) return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(s.XC2, 2 * E), tr(prm + w.uwc, 2 * E), s.dH1, E, R, E, 2 * E, nullptr, 1))) return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(s.dS, 1), tr(prm + w.ak, 1), s.dA2, A2, R, A2, 1, nullptr, 0, EP_DSIG, s.At2)))
       return rc;
-    if ((rc = st_gemm(true, s.dS, 1, prm + w.ak, 1, nullptr, s.dA2, A2, R, A2, 1, EP_DSIG, st, s.At2))) return rc;
-    if ((rc = st_gemm(true, s.dA2, A2, prm + w.aw2, A2, nullptr, s.dA1, A1, R, A1, A2, EP_DSIG, st, s.At1))) return rc;
-    if ((rc = st_gemm(true, s.dA1, A1, prm + w.aw1, A1, nullptr, s.dAin, 4 * E, R, 4 * E, A1, EP_LIN, st))) return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(s.dA2, A2), tr(prm + w.aw2, A2), s.dA1, A1, R, A1, A2, nullptr, 0, EP_DSIG, s.At1)))
+      return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(s.dA1, A1), tr(prm + w.aw1, A1), s.dAin, 4 * E, R, 4 * E, A1))) return rc;
     if ((rc = st_launch("k_st_attin_bwd", k_st_attin_bwd, n, E, st, P.q, s.H1, s.dAin, s.dH1, s.dq))) return rc;
     const RecBack<E> b1{prm + w.gwg + E * 2 * E, prm + w.gwc + E * E, s.Hp1, s.G1, s.C1, nullptr, s.dH1, nullptr, 0, s.XG1, s.XC1,
                         nullptr, n};
     if ((rc = st_launch("k_st_gru_bwd<128>", k_st_gru_bwd<E>, (n + SB - 1) / SB, NTH, st, b1))) return rc;
-    if ((rc = st_gemm(true, s.XG1, 2 * E, prm + w.gwg, 2 * E, nullptr, s.dX, E, R, E, 2 * E, EP_LIN, st))) return rc;
-    if ((rc = st_gemm(true, s.XC1, E, prm + w.gwc, E, nullptr, s.dX, E, R, E, E, EP_LIN, st, nullptr, nullptr, nullptr, 1)))
-      return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(s.XG1, 2 * E), tr(prm + w.gwg, 2 * E), s.dX, E, R, E, 2 * E))) return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(s.XC1, E), tr(prm + w.gwc, E), s.dX, E, R, E, E, nullptr, 1))) return rc;
   }
   // dense weight gradients: one launch over the n-row jobs, one per sequence over its 64 n-row jobs
   Jobs J;
   int k = st_tower_jobs(J, L, P);
-  J.j[k++] = st_job(P.allf, FEAT, P.dO, FEAT, OBS, L.ow); J.j[k++] = st_job(nullptr, 1, P.dO, 1, OBS, L.ob);
-  J.j[k++] = st_job(P.O, OBS, P.dZ, OBS, C, L.rw);      J.j[k++] = st_job(nullptr, 1, P.dZ, 1, C, L.rb);
-  if ((rc = st_wgrad(J, k, n, grad, st))) return rc;
+  layer_jobs(J, k, P.allf, FEAT, P.dO, FEAT, OBS, L.ow, L.ob);
+  layer_jobs(J, k, P.O, OBS, P.dZ, OBS, C, L.rw, L.rb);
+  tile_jobs(J, k);
+  if ((rc = dense_wgrad(FAM_SIMTRAIN, st, J, n, 1, grad))) return rc;
   for (int i = 0; i < 2; ++i) {
     const Seq& w = L.s[i];
     const SeqPlanes& s = P.sp[i];
     k = 0;
-    J.j[k++] = st_job(s.X, E, s.XG1, E, 2 * E, w.gwg);   J.j[k++] = st_job(s.Hp1, E, s.XG1, E, 2 * E, w.gwg + E * 2 * E);
-    J.j[k++] = st_job(nullptr, 1, s.XG1, 1, 2 * E, w.gbg);
-    J.j[k++] = st_job(s.X, E, s.XC1, E, E, w.gwc);       J.j[k++] = st_job(s.RH1, E, s.XC1, E, E, w.gwc + E * E);
-    J.j[k++] = st_job(nullptr, 1, s.XC1, 1, E, w.gbc);
-    J.j[k++] = st_job(s.Ain, 4 * E, s.dA1, 4 * E, A1, w.aw1); J.j[k++] = st_job(nullptr, 1, s.dA1, 1, A1, w.ab1);
-    J.j[k++] = st_job(s.At1, A1, s.dA2, A1, A2, w.aw2);  J.j[k++] = st_job(nullptr, 1, s.dA2, 1, A2, w.ab2);
-    J.j[k++] = st_job(s.At2, A2, s.dS, A2, 1, w.ak);     J.j[k++] = st_job(nullptr, 1, s.dS, 1, 1, w.ab);
-    J.j[k++] = st_job(s.H1, E, s.XG2, E, 4 * E, w.uwg);  J.j[k++] = st_job(s.Hp2, HA, s.XG2, HA, 4 * E, w.uwg + E * 4 * E);
-    J.j[k++] = st_job(nullptr, 1, s.XG2, 1, 4 * E, w.ubg);
-    J.j[k++] = st_job(s.H1, E, s.XC2, E, 2 * E, w.uwc);  J.j[k++] = st_job(s.RH2, HA, s.XC2, HA, 2 * E, w.uwc + E * 2 * E);
-    J.j[k++] = st_job(nullptr, 1, s.XC2, 1, 2 * E, w.ubc);
-    if ((rc = st_wgrad(J, k, R, grad, st))) return rc;
+    // a GRU kernel's input rows and its recurrent rows are two jobs, the second with the bias
+    J.j[k++] = grad_job(s.X, E, s.XG1, E, 2 * E, w.gwg);
+    layer_jobs(J, k, s.Hp1, E, s.XG1, E, 2 * E, w.gwg + E * 2 * E, w.gbg);
+    J.j[k++] = grad_job(s.X, E, s.XC1, E, E, w.gwc);
+    layer_jobs(J, k, s.RH1, E, s.XC1, E, E, w.gwc + E * E, w.gbc);
+    layer_jobs(J, k, s.Ain, 4 * E, s.dA1, 4 * E, A1, w.aw1, w.ab1);
+    layer_jobs(J, k, s.At1, A1, s.dA2, A1, A2, w.aw2, w.ab2);
+    layer_jobs(J, k, s.At2, A2, s.dS, A2, 1, w.ak, w.ab);
+    J.j[k++] = grad_job(s.H1, E, s.XG2, E, 4 * E, w.uwg);
+    layer_jobs(J, k, s.Hp2, HA, s.XG2, HA, 4 * E, w.uwg + E * 4 * E, w.ubg);
+    J.j[k++] = grad_job(s.H1, E, s.XC2, E, 2 * E, w.uwc);
+    layer_jobs(J, k, s.RH2, HA, s.XC2, HA, 2 * E, w.uwc + E * 2 * E, w.ubc);
+    tile_jobs(J, k);
+    if ((rc = dense_wgrad(FAM_SIMTRAIN, st, J, R, 1, grad))) return rc;
   }
   // embedding gradients: the 21 cat slots, both sequences and the query's 10 emb_seq slots (dqs)
   if ((rc = st_launch("k_st_dq", k_st_dq, (n * E + 255) / 256, 256, st, P.sp[0].dq, P.sp[1].dq, P.dqs, n))) return rc;
@@ -1223,22 +1243,26 @@ static int sn_forward(int head, const r4st::NLayout& L, const float* prm, const 
     for (int i = 0; i < 3; ++i) {
       const GruPlanes& g = P.g[i];
       const int nt = i ? T : NC, R = n * nt;
-      if ((rc = st_gemm(false, g.X, E, prm + L.g[i].k, NG3, prm + L.g[i].b, g.XG, NG3, R, NG3, E, EP_LIN, st))) return rc;
+      if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(g.X, E), rm(prm + L.g[i].k, NG3), g.XG, NG3, R, NG3, E, prm + L.g[i].b))) return rc;
       const KGru a{prm + L.g[i].rk, g.XG, g.Hp, g.A, g.HH, g.RH, P.A + col[i], L.FA, n, nt};
       if ((rc = st_launch("k_st_kgru_fwd", k_st_kgru_fwd, (n + SB - 1) / SB, NTH, st, a))) return rc;
     }
   }
   if (L.net == NET_DNN) {
-    if ((rc = st_gemm(false, P.A, L.FA, prm + L.fcw, OBS, prm + L.fcb, P.F, OBS, n, OBS, L.FA, EP_ELU, st))) return rc;
-    if ((rc = st_gemm(false, P.F, OBS, prm + L.ow, OBS, prm + L.ob, P.O, OBS, n, OBS, OBS, EP_ELU, st))) return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.A, L.FA), rm(prm + L.fcw, OBS), P.F, OBS, n, OBS, L.FA, prm + L.fcb, 0, EP_ELU)))
+      return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.F, OBS), rm(prm + L.ow, OBS), P.O, OBS, n, OBS, OBS, prm + L.ob, 0, EP_ELU)))
+      return rc;
   } else if (L.net == NET_WIDEDEEP) {             // O[:, :256], its activations kept apart in F for the backward
-    if ((rc = st_gemm(false, P.A, L.FA, prm + L.fcw, OBS, prm + L.fcb, P.O, L.FO, n, OBS, L.FA, EP_ELU, st, nullptr, nullptr, P.F)))
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.A, L.FA), rm(prm + L.fcw, OBS), P.O, L.FO, n, OBS, L.FA, prm + L.fcb, 0, EP_ELU,
+                       nullptr, nullptr, P.F)))
       return rc;
   } else if (L.net == NET_LSTM) {
-    if ((rc = st_gemm(false, P.A, L.FA, prm + L.ow, OBS, prm + L.ob, P.O, OBS, n, OBS, L.FA, EP_ELU, st))) return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.A, L.FA), rm(prm + L.ow, OBS), P.O, OBS, n, OBS, L.FA, prm + L.ob, 0, EP_ELU)))
+      return rc;
   }
   const float* hin = L.FO ? P.O : P.A;
-  if ((rc = st_gemm(false, hin, L.FH, prm + L.rw, L.C, prm + L.rb, P.Z, L.C, n, L.C, L.FH, EP_LIN, st))) return rc;
+  if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(hin, L.FH), rm(prm + L.rw, L.C), P.Z, L.C, n, L.C, L.FH, prm + L.rb))) return rc;
   return st_loss(head, D, idx, n, P.Z, with_grad ? P.dZ : nullptr, P.srow, stats, acc, probs, st);
 }
 
@@ -1253,21 +1277,27 @@ static int sn_backward(int head, const r4st::NLayout& L, const float* prm, const
   int tower_r0 = 0, tower_ld = 0;
   const float* dtop = nullptr;
   if (L.net == NET_DNN) {
-    if ((rc = st_gemm(true, P.dZ, C, Wt(L.rw, 0, C), C, nullptr, P.dO, OBS, n, OBS, C, EP_DELU, st, P.O))) return rc;
-    if ((rc = st_gemm(true, P.dO, OBS, Wt(L.ow, 0, OBS), OBS, nullptr, P.dF, OBS, n, OBS, OBS, EP_DELU, st, P.F))) return rc;
-    if ((rc = st_gemm(true, P.dF, OBS, Wt(L.fcw, 0, OBS), OBS, nullptr, P.dA, L.FA, n, E, OBS, EP_LIN, st))) return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.dZ, C), tr(Wt(L.rw, 0, C), C), P.dO, OBS, n, OBS, C, nullptr, 0, EP_DELU, P.O)))
+      return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.dO, OBS), tr(Wt(L.ow, 0, OBS), OBS), P.dF, OBS, n, OBS, OBS, nullptr, 0, EP_DELU,
+                       P.F)))
+      return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.dF, OBS), tr(Wt(L.fcw, 0, OBS), OBS), P.dA, L.FA, n, E, OBS))) return rc;
     dtop = P.dF; tower_r0 = E; tower_ld = OBS;
   } else if (L.net == NET_WIDEDEEP) {
-    if ((rc = st_gemm(true, P.dZ, C, Wt(L.rw, 0, C), C, nullptr, P.dF, OBS, n, OBS, C, EP_DELU, st, P.F))) return rc;
-    if ((rc = st_gemm(true, P.dZ, C, Wt(L.rw, OBS + U, C), C, nullptr, P.dO + OBS + U, L.FO, n, NC * E, C, EP_LIN, st))) return rc;
-    if ((rc = st_gemm(true, P.dF, OBS, Wt(L.fcw, 0, OBS), OBS, nullptr, P.dA, L.FA, n, L.FA, OBS, EP_LIN, st))) return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.dZ, C), tr(Wt(L.rw, 0, C), C), P.dF, OBS, n, OBS, C, nullptr, 0, EP_DELU, P.F)))
+      return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.dZ, C), tr(Wt(L.rw, OBS + U, C), C), P.dO + OBS + U, L.FO, n, NC * E, C)))
+      return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.dF, OBS), tr(Wt(L.fcw, 0, OBS), OBS), P.dA, L.FA, n, L.FA, OBS))) return rc;
     dtop = P.dZ; tower_r0 = OBS; tower_ld = C;
   } else if (L.net == NET_LSTM) {
-    if ((rc = st_gemm(true, P.dZ, C, Wt(L.rw, 0, C), C, nullptr, P.dO, OBS, n, OBS, C, EP_DELU, st, P.O))) return rc;
-    if ((rc = st_gemm(true, P.dO, OBS, Wt(L.ow, 0, OBS), OBS, nullptr, P.dA, L.FA, n, L.FA, OBS, EP_LIN, st))) return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.dZ, C), tr(Wt(L.rw, 0, C), C), P.dO, OBS, n, OBS, C, nullptr, 0, EP_DELU, P.O)))
+      return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.dO, OBS), tr(Wt(L.ow, 0, OBS), OBS), P.dA, L.FA, n, L.FA, OBS))) return rc;
     dtop = P.dO; tower_r0 = L.A_tower; tower_ld = OBS;
   } else {
-    if ((rc = st_gemm(true, P.dZ, C, Wt(L.rw, 0, C), C, nullptr, P.dA, L.FA, n, L.FA, C, EP_LIN, st))) return rc;
+    if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(P.dZ, C), tr(Wt(L.rw, 0, C), C), P.dA, L.FA, n, L.FA, C))) return rc;
     dtop = P.dZ; tower_r0 = L.A_tower; tower_ld = C;
   }
   const int64_t tw = L.net == NET_DNN ? L.fcw : L.net == NET_LSTM ? L.ow : L.rw;
@@ -1289,44 +1319,45 @@ static int sn_backward(int head, const r4st::NLayout& L, const float* prm, const
       const KGruBack b{prm + L.g[i].rk, g.Hp, g.A, g.HH, P.dA + col[i], L.FA, g.dZR, g.dHH, n, nt};
       if ((rc = st_launch("k_st_kgru_bwd", k_st_kgru_bwd, (n + SB - 1) / SB, NTH, st, b))) return rc;
       float* dX = i ? P.dX[i - 1] : P.dEcat;      // the category GRU's input gradient adds to the Flatten one
-      if ((rc = st_gemm(true, g.dZR, 2 * U, prm + L.g[i].k, NG3, nullptr, dX, E, R, E, 2 * U, EP_LIN, st, nullptr, nullptr, nullptr,
-                        i ? 0 : 1)))
+      if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(g.dZR, 2 * U), tr(prm + L.g[i].k, NG3), dX, E, R, E, 2 * U, nullptr, i ? 0 : 1)))
         return rc;
-      if ((rc = st_gemm(true, g.dHH, U, prm + L.g[i].k + 2 * U, NG3, nullptr, dX, E, R, E, U, EP_LIN, st, nullptr, nullptr, nullptr, 1)))
-        return rc;
+      if ((rc = dense_mm(FAM_SIMTRAIN, st, rm(g.dHH, U), tr(prm + L.g[i].k + 2 * U, NG3), dX, E, R, E, U, nullptr, 1))) return rc;
     }
   }
   // dense weight gradients over the n-row jobs
   Jobs J;
   int k = st_tower_jobs(J, L, P);
   if (L.net == NET_DNN) {
-    J.j[k++] = st_job(P.A, L.FA, P.dF, L.FA, OBS, L.fcw); J.j[k++] = st_job(nullptr, 1, P.dF, 1, OBS, L.fcb);
-    J.j[k++] = st_job(P.F, OBS, P.dO, OBS, OBS, L.ow);    J.j[k++] = st_job(nullptr, 1, P.dO, 1, OBS, L.ob);
+    layer_jobs(J, k, P.A, L.FA, P.dF, L.FA, OBS, L.fcw, L.fcb);
+    layer_jobs(J, k, P.F, OBS, P.dO, OBS, OBS, L.ow, L.ob);
   } else if (L.net == NET_WIDEDEEP) {
-    J.j[k++] = st_job(P.A, L.FA, P.dF, L.FA, OBS, L.fcw); J.j[k++] = st_job(nullptr, 1, P.dF, 1, OBS, L.fcb);
+    layer_jobs(J, k, P.A, L.FA, P.dF, L.FA, OBS, L.fcw, L.fcb);
   } else if (L.net == NET_LSTM) {
-    J.j[k++] = st_job(P.A, L.FA, P.dO, L.FA, OBS, L.ow);  J.j[k++] = st_job(nullptr, 1, P.dO, 1, OBS, L.ob);
+    layer_jobs(J, k, P.A, L.FA, P.dO, L.FA, OBS, L.ow, L.ob);
   }
   const float* hin = L.FO ? P.O : P.A;
-  J.j[k++] = st_job(hin, L.FH, P.dZ, L.FH, C, L.rw);    J.j[k++] = st_job(nullptr, 1, P.dZ, 1, C, L.rb);
-  if ((rc = st_wgrad(J, k, n, grad, st))) return rc;
+  layer_jobs(J, k, hin, L.FH, P.dZ, L.FH, C, L.rw, L.rb);
+  tile_jobs(J, k);
+  if ((rc = dense_wgrad(FAM_SIMTRAIN, st, J, n, 1, grad))) return rc;
   if (L.net == NET_LSTM) {
     // each GRU's [z | r] and h column blocks into gtmp, the category GRU's (21 n rows) then both sequence GRUs' (64 n rows)
     auto gru_jobs = [&](int i, int& kk) {
       const GruPlanes& g = P.g[i];
       const int64_t zr = (int64_t)i * GROWS * NG3, hc = zr + (int64_t)GROWS * 2 * U;
-      J.j[kk++] = st_job(g.X, E, g.dZR, E, 2 * U, zr);  J.j[kk++] = st_job(g.Hp, U, g.dZR, U, 2 * U, zr + (int64_t)E * 2 * U);
-      J.j[kk++] = st_job(nullptr, 1, g.dZR, 1, 2 * U, zr + (int64_t)(E + U) * 2 * U);
-      J.j[kk++] = st_job(g.X, E, g.dHH, E, U, hc);      J.j[kk++] = st_job(g.RH, U, g.dHH, U, U, hc + (int64_t)E * U);
-      J.j[kk++] = st_job(nullptr, 1, g.dHH, 1, U, hc + (int64_t)(E + U) * U);
+      J.j[kk++] = grad_job(g.X, E, g.dZR, E, 2 * U, zr);
+      layer_jobs(J, kk, g.Hp, U, g.dZR, U, 2 * U, zr + (int64_t)E * 2 * U, zr + (int64_t)(E + U) * 2 * U);
+      J.j[kk++] = grad_job(g.X, E, g.dHH, E, U, hc);
+      layer_jobs(J, kk, g.RH, U, g.dHH, U, U, hc + (int64_t)E * U, hc + (int64_t)(E + U) * U);
     };
     k = 0;
     gru_jobs(0, k);
-    if ((rc = st_wgrad(J, k, n * NC, P.gtmp, st))) return rc;
+    tile_jobs(J, k);
+    if ((rc = dense_wgrad(FAM_SIMTRAIN, st, J, n * NC, 1, P.gtmp))) return rc;
     k = 0;
     gru_jobs(1, k);
     gru_jobs(2, k);
-    if ((rc = st_wgrad(J, k, n * T, P.gtmp, st))) return rc;
+    tile_jobs(J, k);
+    if ((rc = dense_wgrad(FAM_SIMTRAIN, st, J, n * T, 1, P.gtmp))) return rc;
     if ((rc = st_launch("k_st_kgru_merge", k_st_kgru_merge, (3 * GROWS * NG3 + 255) / 256, 256, st, (const float*)P.gtmp, grad,
                         L.g[0].k, L.g[1].k, L.g[2].k)))
       return rc;
@@ -1499,28 +1530,8 @@ int ek_launch(const char* name, void (*kernel)(P...), dim3 grid, int threads, si
   return launch(FAM_EXACTK, name, kernel, grid, threads, smem, st, false, std::forward<A>(args)...);
 }
 
-unsigned blocks(int64_t n, int per) { return (unsigned)((n + per - 1) / per); }
-
 constexpr int EK_SPLITS = 128;                 // split-K partials of a weight gradient at most
 constexpr int64_t EK_KC = 1024;                // rows per split-K partial at least
-
-// a [rows, cols] row-major matrix at leading dimension ld as a GEMM operand, or its transpose
-Op rm(const float* p, int64_t ld) { return Op{p, 0, 0, ld, 1}; }
-Op tr(const float* p, int64_t ld) { return Op{p, 0, 0, 1, ld}; }
-
-// C[M, N] (ldc) = alpha A B (+ C if beta) (+ bias) (relu), one batch
-int ek_mm(cudaStream_t st, Op A, Op B, float* C, int64_t ldc, int M, int N, int K, const float* bias = nullptr,
-          int relu = 0, int beta = 0, float alpha = 1.f) {
-  const Gemm g{A, B, C, 0, 0, ldc, 1, bias, nullptr, nullptr, nullptr, M, N, K, 1, 0, alpha, relu ? EP_RELU : EP_LIN, beta};
-  return ek_launch("k_dense_gemm", gemm_kernel(g), dim3(blocks(N, GT), blocks(M, GT), 1), NT, 0, st, g);
-}
-
-// the per-(row, head) attention products: batch z = 4 b + h
-int ek_bmm(cudaStream_t st, Op A, Op B, float* C, int64_t cso, int64_t csi, int64_t cs0, int64_t cs1, int M, int N, int K,
-           int n, float alpha, int beta = 0) {
-  const Gemm g{A, B, C, cso, csi, cs0, cs1, nullptr, nullptr, nullptr, nullptr, M, N, K, r4ek::NH, 0, alpha, EP_LIN, beta};
-  return ek_launch("k_dense_gemm", gemm_kernel(g), dim3(blocks(N, GT), blocks(M, GT), n * r4ek::NH), NT, 0, st, g);
-}
 
 // out[N] (+)= sum over R rows (stride rs) of in[r, (i / w) ls + i % w]: chunks of rows into partials, then their sum
 // (two launches at every size, so a pass launches the same number of kernels for every n)
@@ -1540,9 +1551,7 @@ int ek_wgrad(cudaStream_t st, const float* X, int64_t ldx, const float* dY, int6
              float* part) {
   const int64_t S = std::min<int64_t>(EK_SPLITS, (R + EK_KC - 1) / EK_KC);
   const int64_t kc = (R + S - 1) / S;
-  const Gemm g{tr(X, ldx), rm(dY, ldy), part, (int64_t)K * N, 0, N, 1, nullptr, nullptr, nullptr, nullptr, K, N, (int)kc, 1, R,
-               1.f, EP_LIN, 0};
-  if (int rc = ek_launch("k_dense_gemm", gemm_kernel(g), dim3(blocks(N, GT), blocks(K, GT), (unsigned)S), NT, 0, st, g))
+  if (int rc = dense_bmm(FAM_EXACTK, st, tr(X, ldx), rm(dY, ldy), part, (int64_t)K * N, 0, N, K, N, (int)kc, S, 1, 1.f, R))
     return rc;
   return ek_launch("k_ek_colsum", r4ek::k_ek_colsum, dim3(blocks((int64_t)K * N, 128), 1), 128, 0, st, (const float*)part, S,
                    (int64_t)K * N, K * N, (int64_t)0, K * N, S, dW, (int64_t)0, 1.f, 1);
@@ -1613,7 +1622,8 @@ int ek_encoder(const EkRun& r, const float* user) {
   const Layout& L = r.L;
   cudaStream_t st = r.st;
   int rc;
-  if ((rc = ek_mm(st, rm(user, UIN), rm(prm + L.u_w, HU), r.f(r.p.uenc), HU, n, HU, UIN, prm + L.u_b, 1))) return rc;
+  if ((rc = dense_mm(FAM_EXACTK, st, rm(user, UIN), rm(prm + L.u_w, HU), r.f(r.p.uenc), HU, n, HU, UIN, prm + L.u_b, 0, EP_RELU)))
+    return rc;
   if ((rc = ek_launch("k_ek_input", k_ek_input, blocks(nT * D, 256), 256, 0, st, (const float*)r.f(r.p.uenc), prm + L.emb, n,
                       T, r.seed, r.call, r.rate, r.f(r.p.X0))))
     return rc;
@@ -1624,30 +1634,36 @@ int ek_encoder(const EkRun& r, const float* user) {
     float* QKV = r.f(r.p.QKV[l]);
     float* S = r.f(r.p.dP);
     if ((rc = ek_launch("k_ek_rowmask", k_ek_rowmask, blocks(nT * 32, 256), 256, 0, st, X, nT, r.f(r.p.m[l])))) return rc;
-    if ((rc = ek_mm(st, rm(X, D), rm(prm + B.qkv_w, 3 * D), QKV, 3 * D, (int)nT, 3 * D, D, prm + B.qkv_b, 1))) return rc;
-    if ((rc = ek_bmm(st, Op{QKV, T * 3 * D, DH, 3 * D, 1}, Op{QKV + D, T * 3 * D, DH, 1, 3 * D}, S, (int64_t)NH * T * T,
-                     (int64_t)T * T, T, 1, T, T, DH, n, inv)))
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(X, D), rm(prm + B.qkv_w, 3 * D), QKV, 3 * D, (int)nT, 3 * D, D, prm + B.qkv_b, 0,
+                       EP_RELU)))
+      return rc;
+    if ((rc = dense_bmm(FAM_EXACTK, st, Op{QKV, T * 3 * D, DH, 3 * D, 1}, Op{QKV + D, T * 3 * D, DH, 1, 3 * D}, S,
+                        (int64_t)NH * T * T, (int64_t)T * T, T, T, T, DH, n, NH, inv)))
       return rc;
     if ((rc = ek_launch("k_ek_softmax", k_ek_softmax, blocks((int64_t)n * NH * T * 32, 256), 256, 0, st, (const float*)S,
                         (const float*)r.f(r.p.m[l]), n, T, r.seed, r.call, l == 0 ? ST_ATT0 : ST_ATT1, r.rate, r.f(r.p.A[l]),
                         r.f(r.p.P[l]))))
       return rc;
-    if ((rc = ek_bmm(st, Op{r.f(r.p.P[l]), (int64_t)NH * T * T, (int64_t)T * T, T, 1}, Op{QKV + 2 * D, T * 3 * D, DH, 3 * D, 1},
-                     r.f(r.p.O[l]), (int64_t)T * D, DH, D, 1, T, DH, T, n, 1.f)))
+    if ((rc = dense_bmm(FAM_EXACTK, st, Op{r.f(r.p.P[l]), (int64_t)NH * T * T, (int64_t)T * T, T, 1},
+                        Op{QKV + 2 * D, T * 3 * D, DH, 3 * D, 1}, r.f(r.p.O[l]), (int64_t)T * D, DH, D, T, DH, T, n, NH, 1.f)))
       return rc;
     if ((rc = ek_launch("k_ek_ln", k_ek_ln, blocks(nT * 32, 256), 256, 0, st, (const float*)r.f(r.p.O[l]), X, nT,
                         prm + B.ln1_b, prm + B.ln1_g, r.f(r.p.Y1[l]), r.f(r.p.xh1[l]), r.f(r.p.rs1[l]))))
       return rc;
-    if ((rc = ek_mm(st, rm(r.f(r.p.Y1[l]), D), rm(prm + B.f1_w, FF), r.f(r.p.F1[l]), FF, (int)nT, FF, D, prm + B.f1_b, 1)))
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(r.f(r.p.Y1[l]), D), rm(prm + B.f1_w, FF), r.f(r.p.F1[l]), FF, (int)nT, FF, D,
+                       prm + B.f1_b, 0, EP_RELU)))
       return rc;
-    if ((rc = ek_mm(st, rm(r.f(r.p.F1[l]), FF), rm(prm + B.f2_w, D), r.f(r.p.dY), D, (int)nT, D, FF, prm + B.f2_b))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(r.f(r.p.F1[l]), FF), rm(prm + B.f2_w, D), r.f(r.p.dY), D, (int)nT, D, FF,
+                       prm + B.f2_b)))
+      return rc;
     if ((rc = ek_launch("k_ek_ln", k_ek_ln, blocks(nT * 32, 256), 256, 0, st, (const float*)r.f(r.p.dY),
                         (const float*)r.f(r.p.Y1[l]), nT, prm + B.ln2_b, prm + B.ln2_g, r.f(r.p.Y2[l]), r.f(r.p.xh2[l]),
                         r.f(r.p.rs2[l]))))
       return rc;
   }
   for (int a = 0; a < 2; ++a)
-    if ((rc = ek_mm(st, rm(r.f(r.p.Y2[1]), D), rm(prm + L.att[a].w_ref, D), r.f(r.p.eref[a]), D, (int)nT, D, D))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(r.f(r.p.Y2[1]), D), rm(prm + L.att[a].w_ref, D), r.f(r.p.eref[a]), D, (int)nT, D, D)))
+      return rc;
   return R4_OK;
 }
 
@@ -1672,23 +1688,25 @@ int ek_decoder(const EkRun& r, const r4ek::Dec& d, int mode, float temperature) 
   const size_t smT = (size_t)T * sizeof(float);
   int rc;
   // XH[0] = [first input | initial h] in every row: a K = 0 product with that row as its bias
-  if ((rc = ek_mm(st, Op{nullptr, 0, 0, 0, 0}, Op{prm + L.x0, 0, 0, 0, 1}, d.XH, 2 * D, n, 2 * D, 0, prm + L.x0))) return rc;
+  if ((rc = dense_mm(FAM_EXACTK, st, Op{nullptr, 0, 0, 0, 0}, Op{prm + L.x0, 0, 0, 0, 1}, d.XH, 2 * D, n, 2 * D, 0, prm + L.x0)))
+    return rc;
   for (int t = 0; t < RES; ++t) {
     float* H = d.H + plane(n, t, D);
     float* IN = d.IN + plane(n, t, D);
-    if ((rc = ek_mm(st, rm(d.XH + plane(n, t, 2 * D), 2 * D), rm(prm + L.lstm_w, 4 * D), d.G + plane(n, t, 4 * D), 4 * D, n,
-                    4 * D, 2 * D, prm + L.lstm_b)))
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(d.XH + plane(n, t, 2 * D), 2 * D), rm(prm + L.lstm_w, 4 * D), d.G + plane(n, t, 4 * D),
+                       4 * D, n, 4 * D, 2 * D, prm + L.lstm_b)))
       return rc;
     if ((rc = ek_launch("k_ek_cell", k_ek_cell, blocks((int64_t)n * D, 256), 256, 0, st, d, t, prm + L.c0))) return rc;
-    if ((rc = ek_mm(st, rm(H, D), rm(prm + L.w_bef, D), d.HB + plane(n, t, D), D, n, D, D))) return rc;
-    if ((rc = ek_mm(st, rm(H, D), rm(prm + L.w_b, D), d.QB + plane(n, t, D), D, n, D, D))) return rc;
-    if ((rc = ek_mm(st, rm(H, D), rm(prm + L.att[0].w_q, D), d.A1 + plane(n, t, D), D, n, D, D))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(H, D), rm(prm + L.w_bef, D), d.HB + plane(n, t, D), D, n, D, D))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(H, D), rm(prm + L.w_b, D), d.QB + plane(n, t, D), D, n, D, D))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(H, D), rm(prm + L.att[0].w_q, D), d.A1 + plane(n, t, D), D, n, D, D))) return rc;
     if ((rc = ek_launch("k_ek_intra", k_ek_intra, n, D, 0, st, d, t, prm, L))) return rc;
-    if ((rc = ek_mm(st, rm(IN, D), rm(prm + L.att[0].w_dec, D), d.A1 + plane(n, t, D), D, n, D, D, nullptr, 0, 1))) return rc;
-    if ((rc = ek_mm(st, rm(IN, D), rm(prm + L.att[1].w_dec, D), d.A2 + plane(n, t, D), D, n, D, D))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(IN, D), rm(prm + L.att[0].w_dec, D), d.A1 + plane(n, t, D), D, n, D, D, nullptr, 1)))
+      return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(IN, D), rm(prm + L.att[1].w_dec, D), d.A2 + plane(n, t, D), D, n, D, D))) return rc;
     if ((rc = ek_launch("k_ek_glimpse", k_ek_glimpse, n, RNT, smT, st, d, t, prm, L))) return rc;
-    if ((rc = ek_mm(st, rm(d.GL + plane(n, t, D), D), rm(prm + L.att[1].w_q, D), d.A2 + plane(n, t, D), D, n, D, D, nullptr, 0,
-                    1)))
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(d.GL + plane(n, t, D), D), rm(prm + L.att[1].w_q, D), d.A2 + plane(n, t, D), D, n, D,
+                       D, nullptr, 1)))
       return rc;
     if ((rc = ek_launch("k_ek_point", k_ek_point, n, RNT, smT, st, d, t, mode, temperature, r.seed, r.call, prm, L))) return rc;
   }
@@ -1723,19 +1741,22 @@ int ek_backward(const EkRun& r, const r4ek::Dec& d, const float* user, const flo
     float* dHt = g.dH;
     if ((rc = ek_launch("k_ek_loss_bwd", k_ek_loss_bwd, n, RNT, 0, st, d, g, t, reward, ceb))) return rc;
     if ((rc = ek_launch("k_ek_point_bwd", k_ek_point_bwd, n, RNT, smT, st, d, g, t, prm, L))) return rc;
-    if ((rc = ek_mm(st, rm(g.dA2, D), tr(prm + L.att[1].w_q, D), g.dGL, D, n, D, D))) return rc;
-    if ((rc = ek_mm(st, rm(g.dA2, D), tr(prm + L.att[1].w_dec, D), g.dIN, D, n, D, D))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(g.dA2, D), tr(prm + L.att[1].w_q, D), g.dGL, D, n, D, D))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(g.dA2, D), tr(prm + L.att[1].w_dec, D), g.dIN, D, n, D, D))) return rc;
     if ((rc = ek_launch("k_ek_glimpse_bwd", k_ek_glimpse_bwd, n, RNT, smT, st, d, g, t, prm, L))) return rc;
-    if ((rc = ek_mm(st, rm(g.dA1, D), tr(prm + L.att[0].w_dec, D), g.dIN, D, n, D, D, nullptr, 0, 1))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(g.dA1, D), tr(prm + L.att[0].w_dec, D), g.dIN, D, n, D, D, nullptr, 1))) return rc;
     if ((rc = ek_launch("k_ek_intra_bwd", k_ek_intra_bwd, n, D, 0, st, d, g, t, r.f(r.p.dHs), prm, L))) return rc;
     // dh_t: the later steps' direct terms (in dHs[t]) + the glimpse query + the intra-attention query and keys
-    if ((rc = ek_mm(st, rm(g.dA1, D), tr(prm + L.att[0].w_q, D), dHt, D, n, D, D, nullptr, 0, 1))) return rc;
-    if ((rc = ek_mm(st, rm(g.dQB, D), tr(prm + L.w_b, D), dHt, D, n, D, D, nullptr, 0, 1))) return rc;
-    if ((rc = ek_mm(st, rm(r.f(r.p.dHB) + plane(n, t, D), D), tr(prm + L.w_bef, D), dHt, D, n, D, D, nullptr, 0, 1))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(g.dA1, D), tr(prm + L.att[0].w_q, D), dHt, D, n, D, D, nullptr, 1))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(g.dQB, D), tr(prm + L.w_b, D), dHt, D, n, D, D, nullptr, 1))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(r.f(r.p.dHB) + plane(n, t, D), D), tr(prm + L.w_bef, D), dHt, D, n, D, D, nullptr, 1)))
+      return rc;
     if ((rc = ek_launch("k_ek_cell_bwd", k_ek_cell_bwd, blocks((int64_t)n * D, 256), 256, 0, st, d, g, t, prm + L.c0,
                         t + 1 < RES ? (const float*)(r.f(r.p.dXH) + plane(n, t + 1, 2 * D)) : (const float*)nullptr)))
       return rc;
-    if ((rc = ek_mm(st, rm(g.dG + plane(n, t, 4 * D), 4 * D), tr(prm + L.lstm_w, 4 * D), g.dXH, 2 * D, n, 2 * D, 4 * D))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(g.dG + plane(n, t, 4 * D), 4 * D), tr(prm + L.lstm_w, 4 * D), g.dXH, 2 * D, n, 2 * D,
+                       4 * D)))
+      return rc;
     if (t > 0 && (rc = ek_launch("k_ek_input_bwd", k_ek_input_bwd, blocks((int64_t)n * D, 256), 256, 0, st, d, g, t))) return rc;
   }
   if (loss && (rc = ek_launch("k_ek_gloss", k_ek_gloss, 1, 1, 0, st, (const float*)ceb, reward, n, 1.0f / n, loss))) return rc;
@@ -1761,7 +1782,8 @@ int ek_backward(const EkRun& r, const r4ek::Dec& d, const float* user, const flo
   float* dY = r.f(r.p.denc);
   for (int a = 0; a < 2; ++a) {
     if ((rc = ek_wgrad(st, enc, D, r.f(r.p.deref[a]), D, nT, D, D, dgr + L.att[a].w_ref, part))) return rc;
-    if ((rc = ek_mm(st, rm(r.f(r.p.deref[a]), D), tr(prm + L.att[a].w_ref, D), dY, D, (int)nT, D, D, nullptr, 0, 1))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(r.f(r.p.deref[a]), D), tr(prm + L.att[a].w_ref, D), dY, D, (int)nT, D, D, nullptr, 1)))
+      return rc;
   }
   const float inv = 1.0f / sqrtf((float)DH);
   for (int l = NBLK - 1; l >= 0; --l) {
@@ -1780,12 +1802,13 @@ int ek_backward(const EkRun& r, const r4ek::Dec& d, const float* user, const flo
       return rc;
     if ((rc = ek_colsum(st, gx, nT, D, D, 0, D, dgr + B.ln2_g, 1, part))) return rc;
     if ((rc = ek_lin_grad(st, r.f(r.p.F1[l]), FF, dY, D, nT, FF, D, dgr + B.f2_w, dgr + B.f2_b, part))) return rc;
-    if ((rc = ek_mm(st, rm(dY, D), tr(prm + B.f2_w, D), dF1, FF, (int)nT, FF, D))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(dY, D), tr(prm + B.f2_w, D), dF1, FF, (int)nT, FF, D))) return rc;
     if ((rc = ek_launch("k_ek_relu_bwd", k_ek_relu_bwd, blocks(nT * FF, 256), 256, 0, st, (const float*)r.f(r.p.F1[l]),
                         (int64_t)FF, dF1, (int64_t)FF, nT, FF)))
       return rc;
     if ((rc = ek_lin_grad(st, r.f(r.p.Y1[l]), D, dF1, FF, nT, D, FF, dgr + B.f1_w, dgr + B.f1_b, part))) return rc;
-    if ((rc = ek_mm(st, rm(dF1, FF), tr(prm + B.f1_w, FF), dY, D, (int)nT, D, FF, nullptr, 0, 1))) return rc;   // dY1
+    // dY1
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(dF1, FF), tr(prm + B.f1_w, FF), dY, D, (int)nT, D, FF, nullptr, 1))) return rc;
     // Y1 = LN(O + X)
     if ((rc = ek_colsum(st, dY, nT, D, D, 0, D, dgr + B.ln1_b, 1, part))) return rc;
     if ((rc = ek_launch("k_ek_ln_bwd", k_ek_ln_bwd, blocks(nT * 32, 256), 256, 0, st, (const float*)r.f(r.p.xh1[l]),
@@ -1793,29 +1816,32 @@ int ek_backward(const EkRun& r, const r4ek::Dec& d, const float* user, const flo
       return rc;
     if ((rc = ek_colsum(st, gx, nT, D, D, 0, D, dgr + B.ln1_g, 1, part))) return rc;
     // O_h = P V_h: dP = dO_h V_h^T, dV_h = P^T dO_h
-    if ((rc = ek_bmm(st, Op{dY, (int64_t)T * D, DH, D, 1}, Op{QKV + 2 * D, (int64_t)T * 3 * D, DH, 1, 3 * D}, dP,
-                     (int64_t)NH * T * T, (int64_t)T * T, T, 1, T, T, DH, n, 1.f)))
+    if ((rc = dense_bmm(FAM_EXACTK, st, Op{dY, (int64_t)T * D, DH, D, 1}, Op{QKV + 2 * D, (int64_t)T * 3 * D, DH, 1, 3 * D}, dP,
+                        (int64_t)NH * T * T, (int64_t)T * T, T, T, T, DH, n, NH, 1.f)))
       return rc;
-    if ((rc = ek_bmm(st, Op{r.f(r.p.P[l]), (int64_t)NH * T * T, (int64_t)T * T, 1, T}, Op{dY, (int64_t)T * D, DH, D, 1},
-                     dQKV + 2 * D, (int64_t)T * 3 * D, DH, 3 * D, 1, T, DH, T, n, 1.f)))
+    if ((rc = dense_bmm(FAM_EXACTK, st, Op{r.f(r.p.P[l]), (int64_t)NH * T * T, (int64_t)T * T, 1, T},
+                        Op{dY, (int64_t)T * D, DH, D, 1}, dQKV + 2 * D, (int64_t)T * 3 * D, DH, 3 * D, T, DH, T, n, NH, 1.f)))
       return rc;
     if ((rc = ek_launch("k_ek_softmax_bwd", k_ek_softmax_bwd, blocks((int64_t)n * NH * T * 32, 256), 256, 0, st,
                         (const float*)r.f(r.p.A[l]), (const float*)r.f(r.p.m[l]), n, T, r.seed, r.call,
                         l == 0 ? ST_ATT0 : ST_ATT1, r.rate, dP)))
       return rc;
     // S = Q K^T / sqrt(32): dQ_h = dS K_h / sqrt(32), dK_h = dS^T Q_h / sqrt(32)
-    if ((rc = ek_bmm(st, Op{dP, (int64_t)NH * T * T, (int64_t)T * T, T, 1}, Op{QKV + D, (int64_t)T * 3 * D, DH, 3 * D, 1},
-                     dQKV, (int64_t)T * 3 * D, DH, 3 * D, 1, T, DH, T, n, inv)))
+    if ((rc = dense_bmm(FAM_EXACTK, st, Op{dP, (int64_t)NH * T * T, (int64_t)T * T, T, 1},
+                        Op{QKV + D, (int64_t)T * 3 * D, DH, 3 * D, 1}, dQKV, (int64_t)T * 3 * D, DH, 3 * D, T, DH, T, n, NH,
+                        inv)))
       return rc;
-    if ((rc = ek_bmm(st, Op{dP, (int64_t)NH * T * T, (int64_t)T * T, 1, T}, Op{QKV, (int64_t)T * 3 * D, DH, 3 * D, 1},
-                     dQKV + D, (int64_t)T * 3 * D, DH, 3 * D, 1, T, DH, T, n, inv)))
+    if ((rc = dense_bmm(FAM_EXACTK, st, Op{dP, (int64_t)NH * T * T, (int64_t)T * T, 1, T},
+                        Op{QKV, (int64_t)T * 3 * D, DH, 3 * D, 1}, dQKV + D, (int64_t)T * 3 * D, DH, 3 * D, T, DH, T, n, NH,
+                        inv)))
       return rc;
     if ((rc = ek_launch("k_ek_relu_bwd", k_ek_relu_bwd, blocks(nT * 3 * D, 256), 256, 0, st, QKV, (int64_t)3 * D, dQKV,
                         (int64_t)3 * D, nT, 3 * D)))
       return rc;
     if ((rc = ek_lin_grad(st, X, D, dQKV, 3 * D, nT, D, 3 * D, dgr + B.qkv_w, dgr + B.qkv_b, part))) return rc;
     // dX = d(sum) (the residual) + dQKV W_qkv^T: the block input's gradient, kept in dY
-    if ((rc = ek_mm(st, rm(dQKV, 3 * D), tr(prm + B.qkv_w, 3 * D), dY, D, (int)nT, D, 3 * D, nullptr, 0, 1))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(dQKV, 3 * D), tr(prm + B.qkv_w, 3 * D), dY, D, (int)nT, D, 3 * D, nullptr, 1)))
+      return rc;
   }
   // X0 = dropout([relu(user W_u + b_u) | emb * 8])
   float* dU = r.f(r.p.dU);
@@ -1898,8 +1924,8 @@ int r4_exactk_critic(const float* params, const float* user, int n, const float*
   int rc;
   const float* X = user;
   for (int i = 0; i < 4; ++i) {
-    if ((rc = ek_mm(st, rm(X, in[i]), rm(params + L.w[i], out[i]), s + p.Z[i], out[i], n, out[i], in[i], params + L.b[i],
-                    i < 3)))
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(X, in[i]), rm(params + L.w[i], out[i]), s + p.Z[i], out[i], n, out[i], in[i],
+                       params + L.b[i], 0, i < 3 ? EP_RELU : EP_LIN)))
       return rc;
     X = s + p.Z[i];
   }
@@ -1912,7 +1938,8 @@ int r4_exactk_critic(const float* params, const float* user, int n, const float*
     if ((rc = ek_lin_grad(st, Xi, in[i], s + p.dZ[i], out[i], n, in[i], out[i], grad + L.w[i], grad + L.b[i], s + p.part)))
       return rc;
     if (i == 0) break;
-    if ((rc = ek_mm(st, rm(s + p.dZ[i], out[i]), tr(params + L.w[i], out[i]), s + p.dZ[i - 1], CH, n, CH, out[i]))) return rc;
+    if ((rc = dense_mm(FAM_EXACTK, st, rm(s + p.dZ[i], out[i]), tr(params + L.w[i], out[i]), s + p.dZ[i - 1], CH, n, CH, out[i])))
+      return rc;
     if ((rc = ek_launch("k_ek_relu_bwd", k_ek_relu_bwd, blocks((int64_t)n * CH, 256), 256, 0, st, (const float*)(s + p.Z[i - 1]),
                         (int64_t)CH, s + p.dZ[i - 1], (int64_t)CH, (int64_t)n, CH)))
       return rc;
@@ -1934,7 +1961,7 @@ namespace {
 
 int bc_pack(cudaStream_t st, bool pdl, const float* obs, int K, int rep, const float* A, int lda, const float* B, int W,
             int mode, float flex, int R, float* x, float* out) {
-  return cq_launch("k_bcqc_pack", r4bcqc::k_bcqc_pack, cq_blocks(R, NT / 32), st, pdl, obs, K, rep, A, lda, B, W, mode, flex, R,
+  return cq_launch("k_bcqc_pack", r4bcqc::k_bcqc_pack, blocks(R, NT / 32), st, pdl, obs, K, rep, A, lda, B, W, mode, flex, R,
                    x, out);
 }
 
@@ -1946,7 +1973,6 @@ int bc_step(const r4bcqc::Layout& L, const r4bcqc::Hyper& hp, float* prm, float*
             cudaStream_t st, bool pdl) {
   using namespace r4bcqc;
   const int K = L.K, D = L.D, La = L.L, S = hp.S, R = n * S;
-  const Stats none{nullptr, 0, nullptr, nullptr, 0.f, 0};
   int rc;
   if ((rc = cq_launch("k_bcqc_gather", k_bcqc_gather, 2 * sm_count(), st, pdl, K, D, Dt, idx, n, P))) return rc;
   if ((rc = cq_launch("k_bcqc_noise", k_bcqc_noise, 2 * sm_count(), st, pdl, L, hp, n, (uint64_t)step, P))) return rc;
@@ -1957,17 +1983,16 @@ int bc_step(const r4bcqc::Layout& L, const r4bcqc::Hyper& hp, float* prm, float*
   if ((rc = cq_forward(st, prm, L.dec, P.dx, n, P.dh1, P.dh2, P.o))) return rc;
   if ((rc = cq_launch("k_bcqc_vae", k_bcqc_vae, 1, st, pdl, L, hp, n, P, (const float*)P.o, stats))) return rc;
   if ((rc = cq_backward(st, prm, L.dec, P.dout, n, P.dh1, P.dh2, P.ddz2, P.ddz1))) return rc;
-  if ((rc = cq_gemm(st, P.ddz1, H, prm + L.dec.w1 + (size_t)K * H, H, true, P.dlat, n, La, H, nullptr, EP_LIN, nullptr, 0)))
-    return rc;
-  if ((rc = cq_launch("k_bcqc_vae_head", k_bcqc_vae_head, cq_blocks((int64_t)n * La, NT), st, pdl, L, hp, n, P))) return rc;
+  if ((rc = dense_mm(FAM_BATCHRL, st, rm(P.ddz1, H), tr(prm + L.dec.w1 + (size_t)K * H, H), P.dlat, La, n, La, H))) return rc;
+  if ((rc = cq_launch("k_bcqc_vae_head", k_bcqc_vae_head, blocks((int64_t)n * La, NT), st, pdl, L, hp, n, P))) return rc;
   if ((rc = cq_backward(st, prm, L.enc, P.deo, n, P.eh1, P.eh2, P.edz2, P.edz1))) return rc;
   Jobs J;
   int nj = 0;
   cq_jobs(J, nj, L.dec, P.dx, P.dh1, P.dh2, P.ddz1, P.ddz2, P.dout);
   cq_jobs(J, nj, L.enc, P.ex, P.eh1, P.eh2, P.edz1, P.edz2, P.deo);
   tile_jobs(J, nj);
-  if ((rc = launch(FAM_BATCHRL, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, st, false, J, n, 1, P.grad, none))) return rc;
-  if (apply && (rc = cq_launch("k_cqlc_adam", r4cqlc::k_cqlc_adam, cq_blocks(L.dec.end - L.enc.w1, NT), st, pdl, L.enc.w1,
+  if ((rc = dense_wgrad(FAM_BATCHRL, st, J, n, 1, P.grad))) return rc;
+  if (apply && (rc = cq_launch("k_cqlc_adam", r4cqlc::k_cqlc_adam, blocks(L.dec.end - L.enc.w1, NT), st, pdl, L.enc.w1,
                                L.dec.end - L.enc.w1, prm, (const float*)P.grad, m, v, step, hp.lr_imitator, hp.eps,
                                (float*)nullptr, 0.f)))
     return rc;
@@ -1989,9 +2014,9 @@ int bc_step(const r4bcqc::Layout& L, const r4bcqc::Hyper& hp, float* prm, float*
     cq_jobs(J, nj, L.c[k], P.cx, P.ch1[k], P.ch2[k], P.dz1[k], P.dz2[k], P.dq[k]);
   }
   tile_jobs(J, nj);
-  if ((rc = launch(FAM_BATCHRL, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, st, false, J, n, 1, P.grad, none))) return rc;
+  if ((rc = dense_wgrad(FAM_BATCHRL, st, J, n, 1, P.grad))) return rc;
   const int c0 = L.c[0].w1, nc = L.c[1].end - c0;
-  if (apply && (rc = cq_launch("k_cqlc_adam", r4cqlc::k_cqlc_adam, cq_blocks(nc, NT), st, pdl, c0, nc, prm,
+  if (apply && (rc = cq_launch("k_cqlc_adam", r4cqlc::k_cqlc_adam, blocks(nc, NT), st, pdl, c0, nc, prm,
                                (const float*)P.grad, m, v, step, hp.lr_critic, hp.eps, tgt + c0, hp.tau)))
     return rc;
   // actor: -Q_0(s, pi(s, dec(s, clamp(z))))
@@ -2003,16 +2028,15 @@ int bc_step(const r4bcqc::Layout& L, const r4bcqc::Hyper& hp, float* prm, float*
   if ((rc = cq_forward(st, prm, L.c[0], P.cx, n, P.ch1[0], P.ch2[0], P.cq[0]))) return rc;
   if ((rc = cq_launch("k_bcqc_actor_loss", k_bcqc_actor_loss, 1, st, pdl, n, P, stats))) return rc;
   if ((rc = cq_backward(st, prm, L.c[0], P.dq[0], n, P.ch1[0], P.ch2[0], P.dz2[0], P.dz1[0]))) return rc;
-  if ((rc = cq_gemm(st, P.dz1[0], H, prm + L.c[0].w1 + (size_t)K * H, H, true, P.da, n, D, H, nullptr, EP_LIN, nullptr, 0)))
-    return rc;
-  if ((rc = cq_launch("k_bcqc_actor_head", k_bcqc_actor_head, cq_blocks((int64_t)n * D, NT), st, pdl, D, hp.flex, n, P)))
+  if ((rc = dense_mm(FAM_BATCHRL, st, rm(P.dz1[0], H), tr(prm + L.c[0].w1 + (size_t)K * H, H), P.da, D, n, D, H))) return rc;
+  if ((rc = cq_launch("k_bcqc_actor_head", k_bcqc_actor_head, blocks((int64_t)n * D, NT), st, pdl, D, hp.flex, n, P)))
     return rc;
   if ((rc = cq_backward(st, prm, L.actor, P.dout, n, P.ah1, P.ah2, P.adz2, P.adz1))) return rc;
   nj = 0;
   cq_jobs(J, nj, L.actor, P.ax, P.ah1, P.ah2, P.adz1, P.adz2, P.dout);
   tile_jobs(J, nj);
-  if ((rc = launch(FAM_BATCHRL, "k_dense_wgrad", k_dense_wgrad, J.ntiles + 1, NT, 0, st, false, J, n, 1, P.grad, none))) return rc;
-  if (apply && (rc = cq_launch("k_cqlc_adam", r4cqlc::k_cqlc_adam, cq_blocks(L.actor.end, NT), st, pdl, 0, L.actor.end, prm,
+  if ((rc = dense_wgrad(FAM_BATCHRL, st, J, n, 1, P.grad))) return rc;
+  if (apply && (rc = cq_launch("k_cqlc_adam", r4cqlc::k_cqlc_adam, blocks(L.actor.end, NT), st, pdl, 0, L.actor.end, prm,
                                (const float*)P.grad, m, v, step, hp.lr_actor, hp.eps, tgt, hp.tau)))
     return rc;
   return R4_OK;
@@ -2100,11 +2124,11 @@ int r4_bcqc_act(int obs_dim, int action_dim, const float* params, const void* ob
   float *xa = z + (size_t)R * La, *ch = xa + (size_t)n * (K + D);
   const int64_t total = (int64_t)n * K;
   int rc;
-  if ((rc = cq_launch("k_cqlc_obs", r4cqlc::k_cqlc_obs, cq_blocks(total, NT), st, false,
+  if ((rc = cq_launch("k_cqlc_obs", r4cqlc::k_cqlc_obs, blocks(total, NT), st, false,
                       obs_f64 ? nullptr : (const float*)obs, obs_f64 ? (const double*)obs : nullptr, total, x)))
     return rc;
   if (action) {
-    if ((rc = cq_launch("k_bcqc_predict_noise", k_bcqc_predict_noise, cq_blocks((int64_t)R * La, NT), st, false, La, NS, n,
+    if ((rc = cq_launch("k_bcqc_predict_noise", k_bcqc_predict_noise, blocks((int64_t)R * La, NT), st, false, La, NS, n,
                         hp->seed, counter, z)))
       return rc;
     if ((rc = bc_pack(st, false, x, K, NS, z, La, nullptr, La, PK_LATENT, 0.f, R, xin, nullptr))) return rc;
@@ -2113,7 +2137,7 @@ int r4_bcqc_act(int obs_dim, int action_dim, const float* params, const void* ob
     if ((rc = cq_forward(st, params, L.actor, xin, R, h1, h2, o))) return rc;
     if ((rc = bc_pack(st, false, x, K, NS, o, D, base, D, PK_PERTURB, hp->action_flexibility, R, xin, base))) return rc;
     if ((rc = cq_forward(st, params, L.c[0], xin, R, h1, h2, cq))) return rc;
-    if ((rc = cq_launch("k_bcqc_argmax", k_bcqc_argmax, cq_blocks(n, NT / 32), st, false, D, NS, n, (const float*)cq,
+    if ((rc = cq_launch("k_bcqc_argmax", k_bcqc_argmax, blocks(n, NT / 32), st, false, D, NS, n, (const float*)cq,
                         (const float*)base, action)))
       return rc;
   }
@@ -2126,7 +2150,7 @@ int r4_bcqc_act(int obs_dim, int action_dim, const float* params, const void* ob
     qk[k] = c + (size_t)n * 2 * H;
     if ((rc = cq_forward(st, params, L.c[k], xa, n, c, c + (size_t)n * H, qk[k]))) return rc;
   }
-  return cq_launch("k_cqlc_qmean", r4cqlc::k_cqlc_qmean, cq_blocks(n, NT), st, false, n, (const float*)qk[0],
+  return cq_launch("k_cqlc_qmean", r4cqlc::k_cqlc_qmean, blocks(n, NT), st, false, n, (const float*)qk[0],
                    (const float*)qk[1], q);
 }
 
@@ -2140,28 +2164,6 @@ template <typename... P, typename... A>
 int s2_launch(const char* name, void (*kernel)(P...), dim3 grid, int threads, size_t smem, cudaStream_t st, A&&... args) {
   return launch(FAM_SEQ2SEQ, name, kernel, grid, threads, smem, st, false, std::forward<A>(args)...);
 }
-unsigned s2_blocks(int64_t n, int per) { return (unsigned)((n + per - 1) / per); }
-Op s2_rm(const float* p, int64_t ld) { return Op{p, 0, 0, ld, 1}; }
-Op s2_tr(const float* p, int64_t ld) { return Op{p, 0, 0, 1, ld}; }
-
-// C[M, N] (ldc) (+)= epilogue(A B + bias)
-int s2_mm(cudaStream_t st, Op A, Op B, float* C, int64_t ldc, int64_t M, int N, int K, const float* bias, int accum = 0,
-          int epi = EP_LIN, const float* aux = nullptr) {
-  const Gemm g{A, B, C, 0, 0, ldc, 1, bias, aux, nullptr, nullptr, (int)M, N, K, 1, 0, 1.f, epi, accum};
-  return s2_launch("k_dense_gemm", gemm_kernel(g), dim3(s2_blocks(N, GT), s2_blocks(M, GT), 1), NT, 0, st, g);
-}
-// per (group, head) products: batch z = g H + h; C element (m, n) of batch (g, h) at C + g cso + h csi + m cs0 + n
-int s2_bmm(cudaStream_t st, Op A, Op B, float* C, int64_t cso, int64_t csi, int64_t cs0, int M, int N, int K, int64_t G, int H,
-           float alpha) {
-  const Gemm g{A, B, C, cso, csi, cs0, 1, nullptr, nullptr, nullptr, nullptr, M, N, K, H, 0, alpha, EP_LIN, 0};
-  return s2_launch("k_dense_gemm", gemm_kernel(g), dim3(s2_blocks(N, GT), s2_blocks(M, GT), (unsigned)(G * H)), NT, 0, st, g);
-}
-int s2_wgrad(cudaStream_t st, Jobs& J, int njob, int64_t rows, float* grad) {
-  tile_jobs(J, njob);
-  const Stats none{nullptr, 0, nullptr, nullptr, 0.f, 0};
-  return s2_launch("k_dense_wgrad", k_dense_wgrad, dim3(J.ntiles + 1), NT, 0, st, J, (int)rows, 0, grad, none);
-}
-Job s2_job(const float* X, int ldx, const float* Z, int M, int N, int64_t off) { return Job{X, Z, ldx, M, N, (int)off, 0}; }
 
 bool s2_cfg_ok(const r4_s2s_config* c) {
   if (!c) return false;
@@ -2255,24 +2257,24 @@ int s2_att(const S2Run& r, const Att& W, const Norm& Nw, const SubP& P, const fl
   cudaStream_t st = r.st;
   float *Q = r.f(P.q), *K = r.f(P.k), *V = r.f(P.v), *O = r.f(P.o), *A = r.f(P.a), *Y = r.f(P.y);
   int rc;
-  if ((rc = s2_mm(st, s2_rm(xq, E), s2_rm(w + W.wq, E), Q, E, Nq, E, E, w + W.bq))) return rc;
+  if ((rc = dense_mm(FAM_SEQ2SEQ, st, rm(xq, E), rm(w + W.wq, E), Q, E, Nq, E, E, w + W.bq))) return rc;
   if (kv) {
-    if ((rc = s2_mm(st, s2_rm(xkv, E), s2_rm(w + W.wk, E), K, E, Nk, E, E, w + W.bk))) return rc;
-    if ((rc = s2_mm(st, s2_rm(xkv, E), s2_rm(w + W.wv, E), V, E, Nk, E, E, w + W.bv))) return rc;
+    if ((rc = dense_mm(FAM_SEQ2SEQ, st, rm(xkv, E), rm(w + W.wk, E), K, E, Nk, E, E, w + W.bk))) return rc;
+    if ((rc = dense_mm(FAM_SEQ2SEQ, st, rm(xkv, E), rm(w + W.wv, E), V, E, Nk, E, E, w + W.bv))) return rc;
   }
   const int64_t cso = (int64_t)H * Mq * Tk, csi = (int64_t)Mq * Tk;
-  if ((rc = s2_bmm(st, Op{Q, (int64_t)Mq * E, dh, E, 1}, Op{K, (int64_t)Tk * E, dh, 1, E}, A, cso, csi, Tk, Mq, Tk, dh, G, H,
-                   1.0f / sqrtf((float)dh))))
+  if ((rc = dense_bmm(FAM_SEQ2SEQ, st, Op{Q, (int64_t)Mq * E, dh, E, 1}, Op{K, (int64_t)Tk * E, dh, 1, E}, A, cso, csi, Tk, Mq,
+                      Tk, dh, G, H, 1.0f / sqrtf((float)dh))))
     return rc;
   const int64_t rows = G * H * Mq;
-  if ((rc = s2_launch("k_s2s_softmax", k_s2s_softmax, s2_blocks(rows * 32, 256), 256, 0, st, A, ktok, kld, rows, H, Mq, Tk,
+  if ((rc = s2_launch("k_s2s_softmax", k_s2s_softmax, blocks(rows * 32, 256), 256, 0, st, A, ktok, kld, rows, H, Mq, Tk,
                       Tq, causal)))
     return rc;
-  if ((rc = s2_bmm(st, Op{A, cso, csi, Tk, 1}, Op{V, (int64_t)Tk * E, dh, E, 1}, O, (int64_t)Mq * E, dh, E, Mq, dh, Tk, G, H,
-                   1.f)))
+  if ((rc = dense_bmm(FAM_SEQ2SEQ, st, Op{A, cso, csi, Tk, 1}, Op{V, (int64_t)Tk * E, dh, E, 1}, O, (int64_t)Mq * E, dh, E, Mq,
+                      dh, Tk, G, H, 1.f)))
     return rc;
-  if ((rc = s2_mm(st, s2_rm(O, E), s2_rm(w + W.wo, E), Y, E, Nq, E, E, w + W.bo))) return rc;
-  return s2_launch("k_s2s_ln", k_s2s_ln, s2_blocks(Nq * 32, 256), 256, 0, st, xq, (const float*)Y, Nq, E, w + Nw.g, w + Nw.b,
+  if ((rc = dense_mm(FAM_SEQ2SEQ, st, rm(O, E), rm(w + W.wo, E), Y, E, Nq, E, E, w + W.bo))) return rc;
+  return s2_launch("k_s2s_ln", k_s2s_ln, blocks(Nq * 32, 256), 256, 0, st, xq, (const float*)Y, Nq, E, w + Nw.g, w + Nw.b,
                    r.seed, r.call, layer, r.rate, r.f(P.out), r.f(P.xh), r.f(P.rs));
 }
 
@@ -2280,9 +2282,9 @@ int s2_ffn(const S2Run& r, const FF& W, const Norm& Nw, const SubP& P, const flo
   const int E = r.c.E, F = r.c.F;
   const float* w = r.prm;
   int rc;
-  if ((rc = s2_mm(r.st, s2_rm(x, E), s2_rm(w + W.w1, F), r.f(P.q), F, N, F, E, w + W.b1, 0, EP_RELU))) return rc;
-  if ((rc = s2_mm(r.st, s2_rm(r.f(P.q), F), s2_rm(w + W.w2, E), r.f(P.y), E, N, E, F, w + W.b2))) return rc;
-  return s2_launch("k_s2s_ln", k_s2s_ln, s2_blocks(N * 32, 256), 256, 0, r.st, x, (const float*)r.f(P.y), N, E, w + Nw.g,
+  if ((rc = dense_mm(FAM_SEQ2SEQ, r.st, rm(x, E), rm(w + W.w1, F), r.f(P.q), F, N, F, E, w + W.b1, 0, EP_RELU))) return rc;
+  if ((rc = dense_mm(FAM_SEQ2SEQ, r.st, rm(r.f(P.q), F), rm(w + W.w2, E), r.f(P.y), E, N, E, F, w + W.b2))) return rc;
+  return s2_launch("k_s2s_ln", k_s2s_ln, blocks(N * 32, 256), 256, 0, r.st, x, (const float*)r.f(P.y), N, E, w + Nw.g,
                    w + Nw.b, r.seed, r.call, layer, r.rate, r.f(P.out), r.f(P.xh), r.f(P.rs));
 }
 
@@ -2292,7 +2294,7 @@ const float* s2_dec_out(const S2Run& r) { return r.f(r.p.dec[r.c.Ld - 1][2].out)
 int s2_encoder(const S2Run& r) {
   const int64_t Ne = (int64_t)r.n * r.Ts;
   int rc;
-  if ((rc = s2_launch("k_s2s_embed", k_s2s_embed, s2_blocks(Ne * r.c.E, 256), 256, 0, r.st, r.etok, (int64_t)r.Ts, r.n, r.Ts,
+  if ((rc = s2_launch("k_s2s_embed", k_s2s_embed, blocks(Ne * r.c.E, 256), 256, 0, r.st, r.etok, (int64_t)r.Ts, r.n, r.Ts,
                       r.prm + r.L.emb_enc, r.c.Vs, r.c.E, r.f(r.p.xe))))
     return rc;
   const float* x = r.f(r.p.xe);
@@ -2313,9 +2315,11 @@ int s2_cross_kv(const S2Run& r) {
   int rc;
   for (int l = 0; l < r.c.Ld; ++l) {
     const Att& W = r.L.dec[l].qa;
-    if ((rc = s2_mm(r.st, s2_rm(s2_enc_out(r), E), s2_rm(r.prm + W.wk, E), r.f(r.p.dec[l][1].k), E, Ne, E, E, r.prm + W.bk)))
+    if ((rc = dense_mm(FAM_SEQ2SEQ, r.st, rm(s2_enc_out(r), E), rm(r.prm + W.wk, E), r.f(r.p.dec[l][1].k), E, Ne, E, E,
+                       r.prm + W.bk)))
       return rc;
-    if ((rc = s2_mm(r.st, s2_rm(s2_enc_out(r), E), s2_rm(r.prm + W.wv, E), r.f(r.p.dec[l][1].v), E, Ne, E, E, r.prm + W.bv)))
+    if ((rc = dense_mm(FAM_SEQ2SEQ, r.st, rm(s2_enc_out(r), E), rm(r.prm + W.wv, E), r.f(r.p.dec[l][1].v), E, Ne, E, E,
+                       r.prm + W.bv)))
       return rc;
   }
   return R4_OK;
@@ -2325,7 +2329,7 @@ int s2_cross_kv(const S2Run& r) {
 int s2_decoder(const S2Run& r, const int32_t* dtok, int64_t dld, int R, int Tt, bool kv) {
   const int64_t P = (int64_t)r.n * R, Nd = P * Tt, Ne = (int64_t)r.n * r.Ts;
   int rc;
-  if ((rc = s2_launch("k_s2s_embed", k_s2s_embed, s2_blocks(Nd * r.c.E, 256), 256, 0, r.st, dtok, dld, (int)P, Tt,
+  if ((rc = s2_launch("k_s2s_embed", k_s2s_embed, blocks(Nd * r.c.E, 256), 256, 0, r.st, dtok, dld, (int)P, Tt,
                       r.prm + r.L.emb_dec, r.c.Vt, r.c.E, r.f(r.p.xd))))
     return rc;
   const float* x = r.f(r.p.xd);
@@ -2345,14 +2349,14 @@ int s2_decoder(const S2Run& r, const int32_t* dtok, int64_t dld, int R, int Tt, 
 // logits [rows, Vt] = h emb_dec^T + b for rows at row stride ld of the decoder output, from position `pos0`
 int s2_logits(const S2Run& r, int64_t rows, int64_t ld, int pos0, float* out) {
   const int E = r.c.E;
-  return s2_mm(r.st, Op{s2_dec_out(r) + (int64_t)pos0 * E, 0, 0, ld, 1}, s2_tr(r.prm + r.L.emb_dec, E), out, r.c.Vt, rows,
-               r.c.Vt, E, r.prm + r.L.out_b);
+  return dense_mm(FAM_SEQ2SEQ, r.st, Op{s2_dec_out(r) + (int64_t)pos0 * E, 0, 0, ld, 1}, tr(r.prm + r.L.emb_dec, E), out, r.c.Vt,
+                  rows, r.c.Vt, E, r.prm + r.L.out_b);
 }
 
 // ---- backward ----
 // LN backward of a sub-layer from dOut: gz <- the residual's gradient, dy <- the sub-layer output's; gx for gamma
 int s2_ln_bwd(const S2Run& r, const Norm& Nw, const SubP& P, const float* dOut, int64_t N, int layer, float* gz) {
-  return s2_launch("k_s2s_ln_bwd", k_s2s_ln_bwd, s2_blocks(N * 32, 256), 256, 0, r.st, dOut, (const float*)r.f(P.xh),
+  return s2_launch("k_s2s_ln_bwd", k_s2s_ln_bwd, blocks(N * 32, 256), 256, 0, r.st, dOut, (const float*)r.f(P.xh),
                    (const float*)r.f(P.rs), N, r.c.E, r.prm + Nw.g, r.seed, r.call, layer, r.rate, gz, r.f(r.p.dy),
                    r.f(r.p.gx));
 }
@@ -2365,16 +2369,16 @@ int s2_ffn_bwd(const S2Run& r, const FF& W, const Norm& Nw, const SubP& P, const
   int rc;
   if ((rc = s2_ln_bwd(r, Nw, P, dOut, N, layer, gz))) return rc;
   float *dy = r.f(r.p.dy), *dF = r.f(r.p.dF);
-  if ((rc = s2_mm(r.st, s2_rm(dy, E), s2_tr(w + W.w2, E), dF, F, N, F, E, nullptr, 0, EP_DRELU, r.f(P.q)))) return rc;
-  if ((rc = s2_mm(r.st, s2_rm(dF, F), s2_tr(w + W.w1, F), gz, E, N, E, F, nullptr, 1))) return rc;
+  if ((rc = dense_mm(FAM_SEQ2SEQ, r.st, rm(dy, E), tr(w + W.w2, E), dF, F, N, F, E, nullptr, 0, EP_DRELU, r.f(P.q)))) return rc;
+  if ((rc = dense_mm(FAM_SEQ2SEQ, r.st, rm(dF, F), tr(w + W.w1, F), gz, E, N, E, F, nullptr, 1))) return rc;
   Jobs J;
-  J.j[0] = s2_job(nullptr, 0, r.f(r.p.gx), 1, E, Nw.g);
-  J.j[1] = s2_job(nullptr, 0, dOut, 1, E, Nw.b);
-  J.j[2] = s2_job(r.f(P.q), F, dy, F, E, W.w2);
-  J.j[3] = s2_job(nullptr, 0, dy, 1, E, W.b2);
-  J.j[4] = s2_job(x, E, dF, E, F, W.w1);
-  J.j[5] = s2_job(nullptr, 0, dF, 1, F, W.b1);
-  return s2_wgrad(r.st, J, 6, N, grad);
+  J.j[0] = grad_job(nullptr, 1, r.f(r.p.gx), 1, E, Nw.g);
+  J.j[1] = grad_job(nullptr, 1, dOut, 1, E, Nw.b);
+  int k = 2;
+  layer_jobs(J, k, r.f(P.q), F, dy, F, E, W.w2, W.b2);
+  layer_jobs(J, k, x, E, dF, E, F, W.w1, W.b1);
+  tile_jobs(J, k);
+  return dense_wgrad(FAM_SEQ2SEQ, r.st, J, N, 0, grad);
 }
 
 // attention sub-layer backward (the forward's arguments): gz <- d(xq); d(xkv) added into gkv (== gz for self-attention).
@@ -2392,49 +2396,45 @@ int s2_att_bwd(const S2Run& r, const Att& W, const Norm& Nw, const SubP& P, cons
   const float *Q = r.f(P.q), *K = r.f(P.k), *V = r.f(P.v), *A = r.f(P.a);
   const int64_t cso = (int64_t)H * Mq * Tk, csi = (int64_t)Mq * Tk;
   const float alpha = 1.0f / sqrtf((float)dh);
-  if ((rc = s2_mm(st, s2_rm(dy, E), s2_tr(w + W.wo, E), dO, E, Nq, E, E, nullptr))) return rc;
+  if ((rc = dense_mm(FAM_SEQ2SEQ, st, rm(dy, E), tr(w + W.wo, E), dO, E, Nq, E, E))) return rc;
   // dA = dO_h V_h^T; dV_h = A^T dO_h
-  if ((rc = s2_bmm(st, Op{dO, (int64_t)Mq * E, dh, E, 1}, Op{V, (int64_t)Tk * E, dh, 1, E}, dA, cso, csi, Tk, Mq, Tk, dh, G, H,
-                   1.f)))
+  if ((rc = dense_bmm(FAM_SEQ2SEQ, st, Op{dO, (int64_t)Mq * E, dh, E, 1}, Op{V, (int64_t)Tk * E, dh, 1, E}, dA, cso, csi, Tk, Mq,
+                      Tk, dh, G, H, 1.f)))
     return rc;
-  if ((rc = s2_bmm(st, Op{A, cso, csi, 1, Tk}, Op{dO, (int64_t)Mq * E, dh, E, 1}, dv, (int64_t)Tk * E, dh, E, Tk, dh, Mq, G, H,
-                   1.f)))
+  if ((rc = dense_bmm(FAM_SEQ2SEQ, st, Op{A, cso, csi, 1, Tk}, Op{dO, (int64_t)Mq * E, dh, E, 1}, dv, (int64_t)Tk * E, dh, E, Tk,
+                      dh, Mq, G, H, 1.f)))
     return rc;
   const int64_t rows = G * H * Mq;
-  if ((rc = s2_launch("k_s2s_softmax_bwd", k_s2s_softmax_bwd, s2_blocks(rows * 32, 256), 256, 0, st, A, dA, rows, Tk))) return rc;
+  if ((rc = s2_launch("k_s2s_softmax_bwd", k_s2s_softmax_bwd, blocks(rows * 32, 256), 256, 0, st, A, dA, rows, Tk))) return rc;
   // dQ_h = alpha dS K_h; dK_h = alpha dS^T Q_h
-  if ((rc = s2_bmm(st, Op{dA, cso, csi, Tk, 1}, Op{K, (int64_t)Tk * E, dh, E, 1}, dq, (int64_t)Mq * E, dh, E, Mq, dh, Tk, G, H,
-                   alpha)))
+  if ((rc = dense_bmm(FAM_SEQ2SEQ, st, Op{dA, cso, csi, Tk, 1}, Op{K, (int64_t)Tk * E, dh, E, 1}, dq, (int64_t)Mq * E, dh, E, Mq,
+                      dh, Tk, G, H, alpha)))
     return rc;
-  if ((rc = s2_bmm(st, Op{dA, cso, csi, 1, Tk}, Op{Q, (int64_t)Mq * E, dh, E, 1}, dk, (int64_t)Tk * E, dh, E, Tk, dh, Mq, G, H,
-                   alpha)))
+  if ((rc = dense_bmm(FAM_SEQ2SEQ, st, Op{dA, cso, csi, 1, Tk}, Op{Q, (int64_t)Mq * E, dh, E, 1}, dk, (int64_t)Tk * E, dh, E, Tk,
+                      dh, Mq, G, H, alpha)))
     return rc;
-  if ((rc = s2_mm(st, s2_rm(dq, E), s2_tr(w + W.wq, E), gz, E, Nq, E, E, nullptr, 1))) return rc;
-  if ((rc = s2_mm(st, s2_rm(dk, E), s2_tr(w + W.wk, E), gkv, E, Nk, E, E, nullptr, 1))) return rc;
-  if ((rc = s2_mm(st, s2_rm(dv, E), s2_tr(w + W.wv, E), gkv, E, Nk, E, E, nullptr, 1))) return rc;
+  if ((rc = dense_mm(FAM_SEQ2SEQ, st, rm(dq, E), tr(w + W.wq, E), gz, E, Nq, E, E, nullptr, 1))) return rc;
+  if ((rc = dense_mm(FAM_SEQ2SEQ, st, rm(dk, E), tr(w + W.wk, E), gkv, E, Nk, E, E, nullptr, 1))) return rc;
+  if ((rc = dense_mm(FAM_SEQ2SEQ, st, rm(dv, E), tr(w + W.wv, E), gkv, E, Nk, E, E, nullptr, 1))) return rc;
   Jobs J;
-  J.j[0] = s2_job(nullptr, 0, r.f(r.p.gx), 1, E, Nw.g);
-  J.j[1] = s2_job(nullptr, 0, dOut, 1, E, Nw.b);
-  J.j[2] = s2_job(r.f(P.o), E, dy, E, E, W.wo);
-  J.j[3] = s2_job(nullptr, 0, dy, 1, E, W.bo);
-  J.j[4] = s2_job(xq, E, dq, E, E, W.wq);
-  J.j[5] = s2_job(nullptr, 0, dq, 1, E, W.bq);
-  int nj = 6;
+  J.j[0] = grad_job(nullptr, 1, r.f(r.p.gx), 1, E, Nw.g);
+  J.j[1] = grad_job(nullptr, 1, dOut, 1, E, Nw.b);
+  int nj = 2;
+  layer_jobs(J, nj, r.f(P.o), E, dy, E, E, W.wo, W.bo);
+  layer_jobs(J, nj, xq, E, dq, E, E, W.wq, W.bq);
   if (self) {
-    J.j[6] = s2_job(xkv, E, dk, E, E, W.wk);
-    J.j[7] = s2_job(nullptr, 0, dk, 1, E, W.bk);
-    J.j[8] = s2_job(xkv, E, dv, E, E, W.wv);
-    J.j[9] = s2_job(nullptr, 0, dv, 1, E, W.bv);
-    nj = 10;
+    layer_jobs(J, nj, xkv, E, dk, E, E, W.wk, W.bk);
+    layer_jobs(J, nj, xkv, E, dv, E, E, W.wv, W.bv);
   }
-  if ((rc = s2_wgrad(st, J, nj, Nq, grad))) return rc;
+  tile_jobs(J, nj);
+  if ((rc = dense_wgrad(FAM_SEQ2SEQ, st, J, Nq, 0, grad))) return rc;
   if (self) return R4_OK;
   Jobs K2;
-  K2.j[0] = s2_job(xkv, E, dk, E, E, W.wk);
-  K2.j[1] = s2_job(nullptr, 0, dk, 1, E, W.bk);
-  K2.j[2] = s2_job(xkv, E, dv, E, E, W.wv);
-  K2.j[3] = s2_job(nullptr, 0, dv, 1, E, W.bv);
-  return s2_wgrad(st, K2, 4, Nk, grad);
+  nj = 0;
+  layer_jobs(K2, nj, xkv, E, dk, E, E, W.wk, W.bk);
+  layer_jobs(K2, nj, xkv, E, dv, E, E, W.wv, W.bv);
+  tile_jobs(K2, nj);
+  return dense_wgrad(FAM_SEQ2SEQ, st, K2, Nk, 0, grad);
 }
 
 // emb[tok] += dX over the positions of tok [rows, T] (contiguous)
@@ -2442,10 +2442,10 @@ int s2_emb_bwd(const S2Run& r, const int32_t* tok, int rows, int T, int V, const
   int *cnt = r.as<int>(r.p.cnt), *off = r.as<int>(r.p.off), *order = r.as<int>(r.p.order);
   int rc;
   if ((rc = s2_launch("k_s2s_tok_csr", k_s2s_tok_csr, 1, 1024, 0, r.st, tok, (int64_t)T, rows, T, V, cnt, off))) return rc;
-  if ((rc = s2_launch("k_s2s_tok_place", k_s2s_tok_place, s2_blocks((int64_t)rows * T, 256), 256, 0, r.st, tok, (int64_t)T,
+  if ((rc = s2_launch("k_s2s_tok_place", k_s2s_tok_place, blocks((int64_t)rows * T, 256), 256, 0, r.st, tok, (int64_t)T,
                       rows, T, V, (const int*)off, order)))
     return rc;
-  return s2_launch("k_s2s_emb_grad", k_s2s_emb_grad, s2_blocks((int64_t)V * r.c.E, 256), 256, 0, r.st, dX, r.c.E, V,
+  return s2_launch("k_s2s_emb_grad", k_s2s_emb_grad, blocks((int64_t)V * r.c.E, 256), 256, 0, r.st, dX, r.c.E, V,
                    (const int*)cnt, (const int*)off, (const int*)order, demb);
 }
 
@@ -2471,11 +2471,12 @@ int s2_train(const S2Run& r, const int32_t* dtok, const int32_t* ytok, int Tt, f
     return rc;
   // output: dH = dZ emb_dec; emb_dec += dZ^T H; b += colsum dZ
   float* g[2] = {r.f(r.p.g[0]), r.f(r.p.g[1])};
-  if ((rc = s2_mm(r.st, s2_rm(Z, V), s2_rm(r.prm + L.emb_dec, E), g[0], E, Nd, E, V, nullptr))) return rc;
+  if ((rc = dense_mm(FAM_SEQ2SEQ, r.st, rm(Z, V), rm(r.prm + L.emb_dec, E), g[0], E, Nd, E, V))) return rc;
   Jobs J;
-  J.j[0] = s2_job(Z, V, s2_dec_out(r), V, E, L.emb_dec);
-  J.j[1] = s2_job(nullptr, 0, Z, 1, V, L.out_b);
-  if ((rc = s2_wgrad(r.st, J, 2, Nd, grad))) return rc;
+  J.j[0] = grad_job(Z, V, s2_dec_out(r), V, E, L.emb_dec);
+  J.j[1] = grad_job(nullptr, 1, Z, 1, V, L.out_b);
+  tile_jobs(J, 2);
+  if ((rc = dense_wgrad(FAM_SEQ2SEQ, r.st, J, Nd, 0, grad))) return rc;
   int a = 0;
   const int base = 2 * r.c.Le;
   float* denc = r.f(r.p.denc);
@@ -2525,7 +2526,7 @@ int s2_adam(const Cfg& c, float* params, const float* grad, float* m, float* v, 
             float eps, cudaStream_t st) {
   const int64_t np = make_layout(c).n;
   const float alpha = lr * sqrtf(1.f - powf(b2, (float)step)) / (1.f - powf(b1, (float)step));
-  return s2_launch("k_s2s_adam", k_s2s_adam, s2_blocks(np, 256), 256, 0, st, np, (int64_t)0, np, np, params,
+  return s2_launch("k_s2s_adam", k_s2s_adam, blocks(np, 256), 256, 0, st, np, (int64_t)0, np, np, params,
                    const_cast<float*>(grad), m, v, alpha, b1, b2, eps);
 }
 
@@ -2618,7 +2619,7 @@ int r4_s2s_epoch(const r4_s2s_config* cfg, float* params, float* grad, float* m,
   for (int64_t k = 0; k < steps; ++k) {
     const int nb = (int)std::min<int64_t>(batch, n_perm - k * batch);
     const int W = src_len + 2 * tgt_len;
-    if (int rc = s2_launch("k_s2s_gather", k_s2s_gather, s2_blocks((int64_t)nb * W, 256), 256, 0, r.st, enc, src_len, dec,
+    if (int rc = s2_launch("k_s2s_gather", k_s2s_gather, blocks((int64_t)nb * W, 256), 256, 0, r.st, enc, src_len, dec,
                            target, tgt_len, perm + k * batch, nb, et, dt, yt))
       return rc;
     // the minibatch's planes: the plan of nb rows, its token planes at the full batch's offsets (past every other plane)
@@ -2674,12 +2675,12 @@ int r4_s2s_beam_search(const r4_s2s_config* cfg, const float* params, const int3
   int32_t* idx = r.as<int32_t>(r.p.idx);
   int32_t* cand = n_cand > 0 ? r.as<int32_t>(r.p.cand) : nullptr;
   int rc;
-  if ((rc = s2_launch("k_s2s_start", k_s2s_start, s2_blocks(P * L, 256), 256, 0, r.st, P, L, pa[0]))) return rc;
+  if ((rc = s2_launch("k_s2s_start", k_s2s_start, blocks(P * L, 256), 256, 0, r.st, P, L, pa[0]))) return rc;
   if ((rc = s2_encoder(r)) || (rc = s2_cross_kv(r))) return rc;
   // step 1: the n START prefixes (row b's beam 0), top beam; the candidates are the top n_cand of the same probabilities
   if ((rc = s2_decoder(r, pa[0], (int64_t)beam * L, 1, 1, false))) return rc;
   if ((rc = s2_topk(r, n, 1, nullptr, 0, 1, beam, val, idx))) return rc;
-  if ((rc = s2_launch("k_s2s_first", k_s2s_first, s2_blocks(P, 256), 256, 0, r.st, (const double*)val, (const int32_t*)idx, P,
+  if ((rc = s2_launch("k_s2s_first", k_s2s_first, blocks(P, 256), 256, 0, r.st, (const double*)val, (const int32_t*)idx, P,
                       L, pa[0], sa[0])))
     return rc;
   if (cand) {
@@ -2719,7 +2720,7 @@ int r4_s2s_score(const r4_s2s_config* cfg, const float* params, const int32_t* e
   if ((rc = s2_launch("k_s2s_out", k_s2s_out, (unsigned)rows, 256, 0, r.st, Z, r.c.Vt, (const int32_t*)nullptr,
                       (const int32_t*)nullptr, (const float*)nullptr, (float*)nullptr)))
     return rc;
-  return s2_launch("k_s2s_pick", k_s2s_pick, s2_blocks(rows, 256), 256, 0, r.st, (const float*)Z, r.c.Vt, path,
+  return s2_launch("k_s2s_pick", k_s2s_pick, blocks(rows, 256), 256, 0, r.st, (const float*)Z, r.c.Vt, path,
                    target_len + 1, (int)P, target_len, prob);
 }
 
@@ -2754,14 +2755,6 @@ OpeLayout ope_layout(int H, int C) {
   L.n = o;
   return L;
 }
-
-// C[M, N] (ldc) = epi(A[M, K] (lda) W[K, N] + bias), row-major operands
-int ope_mm(cudaStream_t st, const float* A, int lda, const float* W, float* C, int ldc, int M, int N, int K,
-           const float* bias, int epi) {
-  const Gemm g{Op{A, 0, 0, lda, 1}, Op{W, 0, 0, N, 1}, C, 0, 0, ldc, 1, bias, nullptr, nullptr, nullptr, M, N, K, 1, 0,
-               1.f, epi, 0};
-  return ope_launch("k_dense_gemm", gemm_kernel(g), dim3((N + GT - 1) / GT, (M + GT - 1) / GT), r4dense::NT, st, g);
-}
 }  // namespace
 
 extern "C" {
@@ -2793,11 +2786,11 @@ int r4_ope_behavior(int B, int H, int C, int K, int P, int page, const float* pa
   int rc;
   if ((rc = ope_launch("k_ope_inputs", k_ope_inputs, dim3(B), E, st, B, K, P, page, H, head, items, feat, p + L.emb, cat,
                        dense)) ||
-      (rc = ope_mm(st, dense, NDENSE, p + L.w1, h1, OPE_U, B, OPE_U, NDENSE, p + L.b1, EP_ELU)) ||
-      (rc = ope_mm(st, h1, OPE_U, p + L.w2, cat + E, CAT_LD, B, OPE_U, OPE_U, p + L.b2, EP_ELU)) ||
-      (rc = ope_mm(st, cat, CAT_LD, p + L.fc_w, a, OPE_F, B, OPE_F, CAT_LD, p + L.fc_b, EP_ELU)) ||
-      (rc = ope_mm(st, a, OPE_F, p + L.obs_w, o, OPE_F, B, OPE_F, OPE_F, p + L.obs_b, EP_ELU)) ||
-      (rc = ope_mm(st, o, OPE_F, p + L.rew_w, z, C, B, C, OPE_F, p + L.rew_b, EP_LIN)))
+      (rc = dense_mm(FAM_OPE, st, rm(dense, NDENSE), rm(p + L.w1, OPE_U), h1, OPE_U, B, OPE_U, NDENSE, p + L.b1, 0, EP_ELU)) ||
+      (rc = dense_mm(FAM_OPE, st, rm(h1, OPE_U), rm(p + L.w2, OPE_U), cat + E, CAT_LD, B, OPE_U, OPE_U, p + L.b2, 0, EP_ELU)) ||
+      (rc = dense_mm(FAM_OPE, st, rm(cat, CAT_LD), rm(p + L.fc_w, OPE_F), a, OPE_F, B, OPE_F, CAT_LD, p + L.fc_b, 0, EP_ELU)) ||
+      (rc = dense_mm(FAM_OPE, st, rm(a, OPE_F), rm(p + L.obs_w, OPE_F), o, OPE_F, B, OPE_F, OPE_F, p + L.obs_b, 0, EP_ELU)) ||
+      (rc = dense_mm(FAM_OPE, st, rm(o, OPE_F), rm(p + L.rew_w, C), z, C, B, C, OPE_F, p + L.rew_b)))
     return rc;
   return ope_launch("k_ope_softmax", k_ope_softmax, dim3(B), r4ope::NT, st, B, C, (const float*)z, out);
 }

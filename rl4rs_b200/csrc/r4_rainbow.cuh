@@ -23,6 +23,7 @@
 #include <stdint.h>
 
 #include "r4_ddpg.cuh"
+#include "r4_dense.cuh"
 
 namespace r4rb {
 
@@ -354,16 +355,12 @@ __global__ void __launch_bounds__(NT) k_rainbow_rows(Layout L, Hyper hp, const f
 inline r4dense::Jobs make_jobs(const Layout& L, const Planes& P) {
   r4dense::Jobs J;
   int k = 0;
-  auto layer = [&](const float* X, const float* dZ, int M, int N, int w, int b) {
-    J.j[k++] = {X, dZ, M, M, N, w, 0};
-    J.j[k++] = {nullptr, dZ, 1, 1, N, b, 0};
-  };
-  layer(P.x, P.d1, OBS, HT, L.w1, L.b1);
-  layer(P.h1, P.d2, HT, HT, L.w2, L.b2);
-  layer(P.h2, P.da1, HT, HQ, L.aw1, L.ab1);
-  layer(P.ha, P.da2, HQ, L.AZ, L.aw2, L.ab2);
-  layer(P.h2, P.ds1, HT, HQ, L.sw1, L.sb1);
-  layer(P.hs, P.ds2, HQ, L.Z, L.sw2, L.sb2);
+  r4dense::layer_jobs(J, k, P.x, OBS, P.d1, OBS, HT, L.w1, L.b1);
+  r4dense::layer_jobs(J, k, P.h1, HT, P.d2, HT, HT, L.w2, L.b2);
+  r4dense::layer_jobs(J, k, P.h2, HT, P.da1, HT, HQ, L.aw1, L.ab1);
+  r4dense::layer_jobs(J, k, P.ha, HQ, P.da2, HQ, L.AZ, L.aw2, L.ab2);
+  r4dense::layer_jobs(J, k, P.h2, HT, P.ds1, HT, HQ, L.sw1, L.sb1);
+  r4dense::layer_jobs(J, k, P.hs, HQ, P.ds2, HQ, L.Z, L.sw2, L.sb2);
   r4dense::tile_jobs(J, k);
   return J;
 }

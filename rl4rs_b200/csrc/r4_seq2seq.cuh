@@ -1,7 +1,7 @@
 // r4_seq2seq.cuh -- the MDP checker's encoder-decoder transformer (keras-transformer 0.40's get_model): the row kernels of
 // its forward and backward, the clipped masked cross-entropy, the embedding-gradient scatter and the beam-search selection.
 // fp32 CUDA cores (parity with a float64 autograd reference is the bar), deterministic: every output element has one
-// writer that sums in a fixed order.  Included from r4_exactk.cuh: the dropout draws are Exact-K's (r4ek::kept).
+// writer that sums in a fixed order.  The dropout draws are Exact-K's (r4ek::kept).
 //
 // Model, E = embed_dim, H heads of E / H, F = hidden_dim (include/rl4rs_b200.h lists the flat parameters):
 //   X0 = emb[token] + trig(position)                                  k_s2s_embed
@@ -19,6 +19,7 @@
 #include <stdint.h>
 
 #include "r4_dense.cuh"
+#include "r4_exactk.cuh"
 
 namespace r4s2s {
 

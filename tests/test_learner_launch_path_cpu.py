@@ -1,6 +1,7 @@
 """CPU: the learner entry points launch their kernels through one launcher (csrc/r4_host.h: r4h::launch), which sets the
-shared-memory opt-in and PDL and counts every launch; the env's translation unit holds no learner code, and the trainers
-read the launch count from the library instead of re-deriving it."""
+shared-memory opt-in and PDL and counts every launch; the shared dense kernels have one host front in r4_learn.cu; every
+header includes what it uses at its head; the env's translation unit holds no learner code, and the trainers read the
+launch count from the library instead of re-deriving it."""
 import os
 import re
 
@@ -51,13 +52,32 @@ def test_env_translation_unit_names_no_learner():
         assert ns not in capi, ns
 
 
-def test_each_kernel_header_including_the_shared_dense_one_is_included_by_one_translation_unit():
+def test_learn_unit_includes_the_thirteen_learner_headers_and_the_env_unit_none():
     sources = [f for f in os.listdir(CSRC) if f.endswith(".cu")]
     assert sorted(sources) == ["r4_capi.cu", "r4_learn.cu"]
     includes = {f: set(re.findall(r'#include "(r4_\w+\.cuh)"', _src(os.path.join(CSRC, f)))) for f in sources}
     assert includes["r4_learn.cu"] == {"r4_ppo.cuh", "r4_comm.cuh", "r4_gauss.cuh", "r4_ddpg.cuh", "r4_rainbow.cuh",
-                                       "r4_batchrl.cuh", "r4_simtrain.cuh", "r4_dense.cuh", "r4_exactk.cuh"}
+                                       "r4_batchrl.cuh", "r4_cqlconti.cuh", "r4_bcqconti.cuh", "r4_simtrain.cuh",
+                                       "r4_dense.cuh", "r4_exactk.cuh", "r4_seq2seq.cuh", "r4_ope.cuh"}
     assert not includes["r4_capi.cu"] & includes["r4_learn.cu"]
+
+
+def test_headers_include_only_at_their_head():
+    for f in sorted(f for f in os.listdir(CSRC) if f.endswith(".cuh")):
+        lines = [l.strip() for l in _src(os.path.join(CSRC, f)).splitlines()]
+        first = next(i for i, l in enumerate(lines) if l and not l.startswith("#"))
+        assert not [l for l in lines[first:] if l.startswith("#include")], f
+
+
+def test_the_dense_kernels_have_one_host_front():
+    src = _src(os.path.join(CSRC, "r4_learn.cu"))
+    for token in ("gemm_kernel(", '"k_dense_gemm"', '"k_dense_wgrad"'):
+        assert src.count(token) == 1, token
+    code = _code(os.path.join(CSRC, "r4_learn.cu"))
+    for name in ("cq_gemm", "st_gemm", "ek_mm", "ek_bmm", "s2_mm", "s2_bmm", "ope_mm", "st_wgrad", "s2_wgrad", "cq_blocks",
+                 "s2_blocks", "s2_rm", "s2_tr"):
+        assert not re.search(r"\b%s\b" % name, code), name
+    assert not re.search(r"\bStats\s+none\b", code)
 
 
 def test_trainers_do_not_count_launches_by_hand():
