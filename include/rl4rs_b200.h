@@ -739,7 +739,10 @@ int64_t r4_simtrain_launch_count(void);
  *   glimpse_0, then attention (the pointer), each: W_q[128,128] W_dec[128,128] v[128] bias[128] W_ref[128,128]
  * Critic (R4_EXACTK_CRITIC): w1[256,128] b1 w2[128,128] b2 w3[128,128] b3 w4[128,1] b4[1]; relu on the three hidden layers.
  *
- * user: f32[n, 256]; n in 1..4096; seq_length T in 9..500 (the candidates are the item ids 0..T-1).  masks: u8[4, T], rows
+ * user: f32[n, 256]; n in 1..4096; seq_length T in 9..500 (the candidates are the item ids 0..T-1); and n T^2 at most
+ * 4096 * 284^2 = 330366976 (every batch at 284 candidates, up to 1321 rows at 500), which bounds the generator's scratch
+ * to 47.4 GB, reached at (4096, 284).  An all-masked step (every candidate masked) picks candidate 0 under GREEDY and the
+ * uniform inverse CDF under SAMPLE; under TRAIN its d(logits) is 0 and its CE log T.  masks: u8[4, T], rows
  * the location masks of positions 0-2, 3-5 and 6-8 and the special items; the point mask of position t is its location
  * mask, minus the items already chosen, minus every special item once one is chosen (position 0: its location mask).
  * Masked logits are -2^32 + 1.  dropout (the rate, in [0, 1)) is live on the encoder input and both blocks' attention

@@ -36,6 +36,10 @@ constexpr int RES = 9;             // res_length: slate positions
 constexpr int NBLK = 2;            // encoder blocks
 constexpr int TMIN = 9, TMAX = 500;
 constexpr int MAXN = 4096;
+// n T^2 at most: five [n, 4, T, T] planes (both blocks' softmax and dropped probabilities, the attention gradient) dominate
+// the generator's scratch; the bound keeps every batch at the script's 284 candidates, and the largest scratch it admits is
+// the one at (4096, 284), 47.4 GB
+constexpr int64_t MAXNTT = (int64_t)MAXN * 284 * 284;
 constexpr float NEG = -4294967295.0f;        // -2^32 + 1 (rounds to -2^32 in fp32, as in the reference graph)
 
 // ---- parameter layouts (floats), in the order include/rl4rs_b200.h documents ----
@@ -462,7 +466,9 @@ __global__ void __launch_bounds__(RNT) k_ek_loss_bwd(Dec d, DecBack g, int t, co
     for (int j = 0; j < T; ++j) mx = fmaxf(mx, lg[j]);
     for (int j = 0; j < T; ++j) den += expf(lg[j] - mx);
     red[0] = mx; red[1] = den;
-    const float l = logf(den) + mx - lg[d.path[(int64_t)b * RES + t]];
+    // max - target first: on a step with every candidate masked (all logits -2^32) that is 0 and CE is log T, where
+    // log T + max would round away in fp32
+    const float l = logf(den) + (mx - lg[d.path[(int64_t)b * RES + t]]);
     ce[b] = (t == RES - 1 ? 0.f : ce[b]) + l;
   }
   __syncthreads();

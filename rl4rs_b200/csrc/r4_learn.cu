@@ -1599,7 +1599,9 @@ EkPlanes ek_planes(int64_t n, int64_t T) {
   return p;
 }
 
-bool ek_shape_ok(int n, int T) { return n >= 1 && n <= r4ek::MAXN && T >= r4ek::TMIN && T <= r4ek::TMAX; }
+bool ek_shape_ok(int n, int T) {
+  return n >= 1 && n <= r4ek::MAXN && T >= r4ek::TMIN && T <= r4ek::TMAX && (int64_t)n * T * T <= r4ek::MAXNTT;
+}
 
 struct EkRun {
   const float* prm;

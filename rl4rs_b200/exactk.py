@@ -27,6 +27,7 @@ GENERATOR, CRITIC = 0, 1
 NEG = -2.0 ** 32 + 1
 ADAM = dict(beta1=0.9, beta2=0.98, eps=1e-8)
 ST_INPUT, ST_ATT0, ST_ATT1, ST_SAMPLE = 0, 1, 2, 3
+MAXN, MAX_NTT = 4096, 4096 * 284 * 284    # rows, and rows x candidates^2 (r4_exactk.cuh: MAXN, MAXNTT)
 
 CONFIG = {"epoch": 10000, "maxlen": 64, "batch_size": 256, "action_size": 284, "class_num": 2, "dense_feature_num": 432,
           "category_feature_num": 21, "category_hash_size": 100000, "seq_num": 2, "emb_size": 128, "page_items": 9,
@@ -274,6 +275,14 @@ class _Adam(object):
         self.flat -= alpha * self.m / (self.v.sqrt() + eps)
 
 
+def check_shape(n, T):
+    """Raise ValueError unless the generator runs n rows over T candidates: n in 1..4096 and n T^2 <= 4096 * 284^2 (the
+    generator's scratch holds five [n, 4, T, T] planes: 47.4 GB at that bound)."""
+    if not 1 <= n <= MAXN or n * T * T > MAX_NTT:
+        raise ValueError("Exact-K runs 1..%d rows with rows x seq_length^2 <= %d (4096 rows at 284 candidates, %d at %d); "
+                         "got %d rows at seq_length %d" % (MAXN, MAX_NTT, min(MAXN, MAX_NTT // (T * T)), T, n, T))
+
+
 def _not_built(**opts):
     for name, (value, ok) in opts.items():
         if not ok:
@@ -326,6 +335,7 @@ class Generator(object):
             raise NotImplementedError("Exact-K decode mode %s is not built (the script samples and decodes greedily)" % mode)
         if mode not in (SAMPLE, GREEDY):
             raise ValueError("draw mode must be SAMPLE or GREEDY, got %r" % (mode,))
+        check_shape(user.shape[0], self.T)
         call = self._next_call()
         user = user.to(self.device, torch.float32).contiguous()
         n = user.shape[0]
@@ -344,6 +354,7 @@ class Generator(object):
 
     def grad(self, user, target, reward):
         """The gradient of the policy loss on the teacher path target [n, 9] -> (grad [num_params], loss [1])."""
+        check_shape(user.shape[0], self.T)
         call = self._next_call()
         user = user.to(self.device, torch.float32).contiguous()
         reward = reward.to(self.device, torch.float32).contiguous()
@@ -459,6 +470,7 @@ def make_env(config):
 def build_nets(config, device, seed=0):
     from rl4rs_b200.env.slate import SlateState
     A = config["action_size"]
+    check_shape(config.get("batch_size", CONFIG["batch_size"]), A)
     if "catalog" in config:
         location_mask = SlateState._location_mask(A)
         special_items = [int(x) for x in config["catalog"].special_items]

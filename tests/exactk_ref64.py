@@ -4,8 +4,15 @@ tf.where with the -2^32 + 1 padding, LayerNorm through the moments, the pointer-
 glimpse / intra_attention, and the policy loss through sparse softmax cross-entropy.  The tests hold the device kernels and
 the torch twin to it.
 
-Rows are independent except through the weight gradients, so the reference runs on any slice of rows [row0, row0 + m) of
-a batch of n_total (the draws are keyed by global row, the loss is divided by n_total) and its gradients add up."""
+Rows are independent except through the weight gradients, so the reference runs on any set of rows of a batch of n_total
+(the draws are keyed by global row, the loss is divided by n_total) and its gradients add up.  `row0` is the first global
+row of a contiguous slice, or an int64 tensor of the global rows themselves (a planted, non-contiguous set).
+
+Also here: the mask regimes the shape tests run (masks_for), the all-masked step's rule, the chunking that keeps one
+reference chunk at a few GB at any T, the reading of the kernels' relu decisions from the scratch, the TF1 Adam update
+and the C-ABI rejections."""
+import ctypes as C
+
 import numpy as np
 import torch
 
@@ -14,10 +21,16 @@ from rl4rs_b200 import exactk as ek
 NEG = -2.0 ** 32 + 1
 
 
+def _rows(row0, N, dev):
+    if torch.is_tensor(row0):
+        return row0.to(dev, torch.int64)
+    return torch.arange(row0, row0 + N, dtype=torch.int64, device=dev)
+
+
 def _keep(seed, call, stream, row0, m, per_row, shape, rate, dev):
     if rate <= 0:
         return torch.ones(shape, dtype=torch.float64, device=dev)
-    e = torch.arange(row0 * per_row, (row0 + m) * per_row, dtype=torch.int64, device=dev)
+    e = (_rows(row0, m, dev).unsqueeze(1) * per_row + torch.arange(per_row, dtype=torch.int64, device=dev)).reshape(-1)
     u = ek.draw24(seed, call, stream, e).to(torch.float32) * (1.0 / 16777216.0)
     return ((u >= rate).to(torch.float64) / float(1.0 - np.float32(rate))).view(shape)
 
@@ -71,9 +84,22 @@ def encoder(w, user, seed, call, rate, T, row0=0, relu_keep=None):
     return enc
 
 
-def decoder(w, enc, masks, mode, seed, call, target=None, temperature=1.0, row0=0):
+def dead_pick(mode, seed, call, rows, t, T, temperature):
+    """The choice at an all-masked step (every logit -2^32 + 1): GREEDY takes candidate 0 (the first of the equal
+    maxima); SAMPLE is the uniform inverse CDF, the first j with j + 1 >= u T, with u T formed in float32 as the kernel
+    forms it (exact: the running sum of T ones is exact in float32), so no margin applies."""
+    if mode == ek.GREEDY:
+        return torch.zeros(rows.shape[0], dtype=torch.int64, device=rows.device)
+    bits = ek.draw24(seed, call, ek.ST_SAMPLE, rows * 9 + t)
+    u = (bits.float() + 0.5) * np.float32(1.0 / 16777216.0) * np.float32(T)
+    return (torch.ceil(u.double()).long() - 1).clamp(0, T - 1)
+
+
+def decoder(w, enc, masks, mode, seed, call, target=None, temperature=1.0, row0=0, dead_out=None):
     """ptn_rnn_decoder: -> (logits [N, 9, T], path [N, 9], margins [N] float64: the smallest decision margin of each row
-    (GREEDY: top-2 logit gap; SAMPLE: distance of the draw to a CDF edge, relative to the total))."""
+    (GREEDY: top-2 logit gap; SAMPLE: distance of the draw to a CDF edge, relative to the total)).  A step whose point
+    mask is empty is its own kind of decision: it takes dead_pick's rule and adds no margin; dead_out (a list), if given,
+    receives the [N, 9] bool of those steps."""
     N, T, _ = enc.shape
     refs = {a: torch.tensordot(enc, w[a + "_w_ref"], dims=([2], [0])) for a in ("g", "p")}
 
@@ -96,6 +122,8 @@ def decoder(w, enc, masks, mode, seed, call, target=None, temperature=1.0, row0=
     output_ref, logits_all, idxs = [], [], []
     margins = torch.full((N,), float("inf"), dtype=torch.float64, device=enc.device)
     rows = torch.arange(N, device=enc.device)
+    grows = _rows(row0, N, enc.device)
+    dead = torch.zeros(N, 9, dtype=torch.bool, device=enc.device)
     inp = w["x0"].expand(N, 128)
     path = torch.zeros(N, 9, dtype=torch.int64, device=enc.device)
     for i in range(9):
@@ -109,28 +137,35 @@ def decoder(w, enc, masks, mode, seed, call, target=None, temperature=1.0, row0=
         output_ref.append(h)
         glimpse = (attention("g", h, intra, True).unsqueeze(2) * enc).sum(1)
         logits = attention("p", glimpse, intra, False)
-        logits = torch.where(ek.point_masks(masks, path, i), logits, torch.full_like(logits, NEG))
+        pm = ek.point_masks(masks, path, i)
+        logits = torch.where(pm, logits, torch.full_like(logits, NEG))
         logits_all.append(logits)
         lg = logits.detach()
+        dead[:, i] = ~pm.any(1)
+        inf = torch.full_like(margins, float("inf"))
         if mode == ek.TRAIN:
             idx = target[:, i].long()
         elif mode == ek.GREEDY:
             top = lg.topk(2, 1)
             idx = top.indices[:, 0]
-            margins = torch.minimum(margins, top.values[:, 0] - top.values[:, 1])
+            margins = torch.minimum(margins, torch.where(dead[:, i], inf, top.values[:, 0] - top.values[:, 1]))
         else:
             x = lg / temperature
             e = torch.exp(x - x.max(1, keepdim=True).values)
             cdf = torch.cumsum(e, 1) / e.sum(1, keepdim=True)
-            bits = ek.draw24(seed, call, ek.ST_SAMPLE, (torch.arange(N, device=enc.device) + row0) * 9 + i)
+            bits = ek.draw24(seed, call, ek.ST_SAMPLE, grows * 9 + i)
             u = ((bits.double() + 0.5) / 16777216.0).unsqueeze(1)
             idx = (cdf < u).sum(1)
             last = T - 1 - torch.flip(e > 0, [1]).int().argmax(1)
             idx = torch.where(idx < T, idx.clamp(max=T - 1), last)
-            margins = torch.minimum(margins, (cdf - u).abs().min(1).values)
+            margins = torch.minimum(margins, torch.where(dead[:, i], inf, (cdf - u).abs().min(1).values))
+        if mode != ek.TRAIN:
+            idx = torch.where(dead[:, i], dead_pick(mode, seed, call, grows, i, T, temperature), idx)
         path[:, i] = idx
         idxs.append(idx)
         inp = enc[rows, idx]
+    if dead_out is not None:
+        dead_out.append(dead)
     return torch.stack(logits_all, 1), path, margins
 
 
@@ -179,3 +214,177 @@ def critic(flat, user, target=None):
     loss = torch.square(torch.abs(target.double() - pred)).sum()
     loss.backward()
     return pred.detach(), flat.grad.detach(), loss.detach()
+
+
+# ---- what the shape tests run ------------------------------------------------------------------------------------------
+MASK_REGIMES = ("ones", "slate", "sparse")
+
+
+def masks_for(T, regime, device="cpu"):
+    """u8 [4, T]: the location masks of positions 0-2, 3-5, 6-8 and the special items.
+      ones    every candidate at every position, no special item
+      slate   SlateState._location_mask(T) with the synthetic catalog's special items below T (below T = 41 positions
+              3-8 have no candidate, below 149 positions 6-8 have none: all-masked steps of the env's own masks)
+      sparse  positions 0-5 take every candidate; positions 6-8 take three special items (the last three candidates) and
+              one other (candidate 0).  A slate holds one special item at most, so positions 6-8 can fill two of their
+              three places: every row meets an all-masked step by position 8, earlier when it chose a special item first."""
+    m = np.zeros((4, T))
+    if regime == "ones":
+        m[:3] = 1
+    elif regime == "slate":
+        from rl4rs_b200 import synth
+        from rl4rs_b200.env.slate import SlateState
+        m[:3] = SlateState._location_mask(T)[:3]
+        m[3, [int(x) for x in synth.make_catalog().special_items if int(x) < T]] = 1
+    elif regime == "sparse":
+        m[:2] = 1
+        m[3, T - 3:] = 1
+        m[2, T - 3:] = 1
+        m[2, 0] = 1
+    else:
+        raise ValueError(regime)
+    return torch.tensor(m != 0, dtype=torch.uint8, device=device)
+
+
+# one [m, 4, T, T] float64 plane per chunk at most this many bytes (autograd holds about a dozen of them per block)
+PLANE_BYTES = 1 << 27
+
+
+def chunk_rows(T):
+    return int(max(1, min(128, PLANE_BYTES // (32 * T * T))))
+
+
+def chunks(rows, T):
+    """Split a sorted int64 row tensor into reference chunks of chunk_rows(T) rows."""
+    c = chunk_rows(T)
+    return [rows[i:i + c] for i in range(0, rows.numel(), c)]
+
+
+def ref_decode(flat, user, masks, mode, seed, call, rate, temperature=1.0, rows=None):
+    """The reference's SAMPLE / GREEDY decode of the global rows `rows` (default: all of user's), chunked:
+    -> (path [m, 9], margins [m], mask margins [m], dead [m, 9] bool)."""
+    T = masks.shape[1]
+    w = unflat64(flat)
+    rows = torch.arange(user.shape[0], device=user.device) if rows is None else rows.to(user.device)
+    out = [[], [], [], []]
+    for r in chunks(rows, T):
+        u = user[r].double()
+        dead = []
+        with torch.no_grad():
+            enc = encoder(w, u, seed, call, rate, T, r)
+            _, p, mg = decoder(w, enc, masks, mode, seed, call, temperature=temperature, row0=r, dead_out=dead)
+        for k, v in enumerate((p, mg, mask_margin(w, u, seed, call, rate, T, r), dead[0])):
+            out[k].append(v)
+    return tuple(torch.cat(v) for v in out)
+
+
+def unflat64(flat):
+    return ek.unflatten(flat.detach().double(), ek.generator_shapes())
+
+
+def device_relu_decisions(g, n):
+    """The relu decisions of the kernels' last forward over n rows of generator g, read from the activation planes at
+    the head of the scratch (the order include/rl4rs_b200.h documents for r4_exactk_grad), at g.T candidates:
+    {"u", "b0_qkv", "b0_f1", "b1_qkv", "b1_f1"} -> bool."""
+    T = g.T
+    f = g._scr(n).view(torch.float32)
+    nT, S4, o, out = n * T, n * 4 * T * T, 0, {}
+
+    def take(k, shape=None):
+        nonlocal o
+        plane = f[o:o + k]
+        o += (k + 63) // 64 * 64
+        return None if shape is None else plane.view(shape) > 0
+
+    out["u"] = take(n * 64, (n, 64))
+    take(nT * 128)
+    for l in range(2):
+        take(nT)
+        out["b%d_qkv" % l] = take(nT * 384, (n, T, 384))
+        for k in (S4, S4, nT * 128, nT * 128, nT * 128, nT):
+            take(k)
+        out["b%d_f1" % l] = take(nT * 256, (n, T, 256))
+        for k in (nT * 128, nT * 128, nT):
+            take(k)
+    return out
+
+
+def grad_rows(flat, user, masks, target, reward, seed, call, rate, rows, n_total, relu_keep=None):
+    """generator_grad summed over the chunks of the global rows `rows` (user, target, reward, relu_keep indexed by
+    global row) -> (grad, loss, [(rows, logits)])."""
+    T = masks.shape[1]
+    grad, loss, logits = 0, 0.0, []
+    for r in chunks(rows, T):
+        keep = None if relu_keep is None else {k: v[r] for k, v in relu_keep.items()}
+        gr, l, lg = generator_grad(flat, user[r], masks, target[r], reward[r], seed, call, rate, row0=r, n_total=n_total,
+                                   relu_keep=keep)
+        grad = grad + gr
+        loss += float(l)
+        logits.append((r, lg))
+    return grad, loss, logits
+
+
+def tensor_errors(got, want, shapes=None):
+    """{tensor name: (max err, max |ref|)} over the flat layout of the generator (or shapes)."""
+    shapes = shapes or ek.generator_shapes()
+    a, b = ek.unflatten(got.double(), shapes), ek.unflatten(want.double().to(got.device), shapes)
+    return {k: ((a[k] - b[k]).abs().max().item(), b[k].abs().max().item()) for k in a}
+
+
+def adam64(flat, grad, m, v, step, lr, beta1=0.9, beta2=0.98, eps=1e-8):
+    """TF1 AdamOptimizer (ResourceApplyAdam) in float64: -> (params, m, v) after step `step` (1-based)."""
+    flat, grad, m, v = (x.double() for x in (flat, grad, m, v))
+    alpha = lr * (1 - beta2 ** step) ** 0.5 / (1 - beta1 ** step)
+    m = m + (grad - m) * (1 - beta1)
+    v = v + (grad * grad - v) * (1 - beta2)
+    return flat - alpha * m / (v.sqrt() + eps), m, v
+
+
+def abi_rejections(lib, P):
+    """[(label, rc)] of the r4_exactk_* entry points called one step past each edge their arguments accept, and of
+    r4_exactk_scratch_size at each shape edge.  P: a non-NULL address passed for every buffer; each call is refused on
+    the host before anything is read or launched, so P is never dereferenced.  Every rc must be R4_ERR_ARG (-1), and
+    every scratch size -1."""
+    nan = float("nan")
+    cap_T500 = ek.MAX_NTT // (500 * 500) + 1            # the first n past n T^2 <= 4096 * 284^2 at T = 500
+    base = dict(params=P, user=P, n=7, T=32, masks=P, mode=ek.SAMPLE, temperature=1.0, dropout=0.1, path=P, logits=P,
+                target=P, reward=P, grad=P, loss=P, scratch=P)
+
+    def decode(a):
+        return lib.r4_exactk_decode(a["params"], a["user"], a["n"], a["T"], a["masks"], a["mode"], a["temperature"], 3, 1,
+                                    a["dropout"], a["path"], a["logits"], a["scratch"], None)
+
+    def grad(a):
+        return lib.r4_exactk_grad(a["params"], a["user"], a["n"], a["T"], a["masks"], a["target"], a["reward"], 3, 1,
+                                  a["dropout"], a["grad"], a["loss"], a["scratch"], None)
+
+    shape_edges = [dict(n=0), dict(n=4097), dict(T=8), dict(T=501), dict(n=cap_T500, T=500), dict(n=4096, T=285)]
+    out = []
+    for e in shape_edges + [dict(dropout=-1e-7), dict(dropout=1.0), dict(dropout=nan)]:
+        for name, fn in (("decode", decode), ("grad", grad)):
+            out.append(("%s %s" % (name, e), fn(dict(base, **e))))
+    for e in (dict(temperature=0.0), dict(temperature=-1.0), dict(temperature=nan), dict(mode=-1), dict(mode=3)):
+        out.append(("decode %s" % e, decode(dict(base, **e))))
+    for k in ("params", "user", "masks", "path", "scratch"):
+        out.append(("decode %s NULL" % k, decode(dict(base, **{k: None}))))
+    for k in ("params", "user", "masks", "target", "reward", "grad", "scratch"):
+        out.append(("grad %s NULL" % k, grad(dict(base, **{k: None}))))
+    for e in shape_edges:
+        a = dict(base, **e)
+        out.append(("scratch_size generator %s" % e, lib.r4_exactk_scratch_size(ek.GENERATOR, a["n"], a["T"])))
+    for n in (0, 4097):
+        out.append(("scratch_size critic n=%d" % n, lib.r4_exactk_scratch_size(ek.CRITIC, n, 0)))
+        out.append(("critic n=%d" % n, lib.r4_exactk_critic(P, P, n, P, P, P, P, P, None)))
+    out.append(("scratch_size net 2", lib.r4_exactk_scratch_size(2, 7, 32)))
+    crit = dict(params=P, user=P, target=P, pred=P, grad=P, loss=P, scratch=P)
+    for k in ("params", "user", "scratch"):
+        a = dict(crit, **{k: None})
+        out.append(("critic %s NULL" % k, lib.r4_exactk_critic(a["params"], a["user"], 7, a["target"], a["pred"], a["grad"],
+                                                                a["loss"], a["scratch"], None)))
+    out.append(("critic target without grad", lib.r4_exactk_critic(P, P, 7, P, P, None, P, P, None)))
+    adam = dict(net=ek.CRITIC, params=P, grad=P, m=P, v=P, step=1)
+    for e in (dict(net=2), dict(net=-1), dict(step=0), dict(params=None), dict(grad=None), dict(m=None), dict(v=None)):
+        a = dict(adam, **e)
+        out.append(("adam %s" % e, lib.r4_exactk_adam(a["net"], a["params"], a["grad"], a["m"], a["v"], a["step"], 1e-3, 0.9,
+                                                      0.98, 1e-8, None)))
+    return out

@@ -51,31 +51,6 @@ def _close(name, got, want, tol=1e-4):
     assert err <= tol * max(scale, 1e-30), "%s: max err %.3g vs max |ref| %.3g" % (name, err, scale)
 
 
-def _device_relu_decisions(g, n):
-    """The relu decisions of the kernels' last forward, read from the activation planes at the head of the scratch (the
-    order include/rl4rs_b200.h documents for r4_exactk_grad): {"u", "b0_qkv", "b0_f1", "b1_qkv", "b1_f1"} -> bool."""
-    f = g._scr(n).view(torch.float32)
-    nT, S4, o, out = n * T, n * 4 * T * T, 0, {}
-
-    def take(k, shape=None):
-        nonlocal o
-        plane = f[o:o + k]
-        o += (k + 63) // 64 * 64
-        return None if shape is None else plane.view(shape) > 0
-
-    out["u"] = take(n * 64, (n, 64))
-    take(nT * 128)
-    for l in range(2):
-        take(nT)
-        out["b%d_qkv" % l] = take(nT * 384, (n, T, 384))
-        for k in (S4, S4, nT * 128, nT * 128, nT * 128, nT):
-            take(k)
-        out["b%d_f1" % l] = take(nT * 256, (n, T, 256))
-        for k in (nT * 128, nT * 128, nT):
-            take(k)
-    return out
-
-
 def _ref_decode(g, user, mode, call):
     w = ek.unflatten(g.flat.double(), ek.generator_shapes())
     paths, margins, mm = [], [], []
@@ -114,7 +89,7 @@ def test_generator_entry_points_match_float64(n):
     print("n=%d: %d rows near a mask decision left out of the gradient" % (n, int((mm <= MASK_GAP).sum())))
     reward = torch.randn(n, device="cuda") * (mm > MASK_GAP)
     grad, loss = g.grad(user, path, reward)
-    keep = _device_relu_decisions(g, n)
+    keep = ref.device_relu_decisions(g, n)
     got_logits = torch.empty(n, 9, T, device="cuda")
     lib = _capi.load_library()
     tgt = path.to(torch.int32).contiguous()
