@@ -458,6 +458,62 @@ int r4_rainbow_train_step(r4_comm* comm, float* params, float* target, float* m,
                           const float* u, float beta, float alpha, float prio_eps, float gamma_n, int step, float lr,
                           float adam_eps, float grad_clip, int copy_target, float* scratch, float* stats, void* stream);
 
+/* ---- parametric-action DQN (PA-DQN) on the discrete env: a state-action Q network over x = [obs (256) | e(a) (D)], e(a)
+ * row a of the env's fixed item vectors emb f32[A, D] (action_emb), Dense 256 tanh -> Dense 256 tanh -> Dense 1, and the
+ * masked values Qm(s, a) = Q(s, a) where mask[s][a] != 0, float32.min where it is 0.  RLlib 1.5 DQN with double Q, no
+ * dueling, no distributional head, n_step 1 (INTEGRATION.md section 3).  A = num_actions in 2..512, D = emb_dim in 1..512,
+ * n rows with n x A < 2^31 - 128.  Flat parameter layout (r4_padqn_num_params(A, D) floats; 140 033 at D = 32):
+ * w1[256+D,256] b1[256] w2[256,256] b2[256] w3[256,1] b3[1]; the target has the same layout.
+ * Every net has a cache (r4_padqn_cache_size(A) bytes of device memory): a pre-tiled bf16 image of w2 and P = e w1[256:]
+ * [A, 256].  r4_padqn_refresh rebuilds it and must run after every change of the parameters it caches; r4_padqn_apply and
+ * r4_padqn_train_step keep both caches current.  The pair scorer evaluates every (row, item) pair on the tensor cores with
+ * a three-way bf16 split of both operands; the [n A, 256] hidden planes are never stored.  The caches and the scratch
+ * must be 16-byte aligned (R4_ERR_ARG otherwise).  Stateless: every pointer is caller-owned DEVICE memory. */
+int r4_padqn_num_params(int num_actions, int emb_dim);
+/* floats of the scratch r4_padqn_act, r4_padqn_grad and r4_padqn_train_step need for n rows; -1 for bad arguments.  It
+ * grows with n (256 + D + A), never with n x A x 256. */
+int64_t r4_padqn_scratch_size(int num_actions, int emb_dim, int n);
+/* bytes of one net's cache; -1 for bad arguments */
+int64_t r4_padqn_cache_size(int num_actions);
+/* cache = the w2 image and P of params; cache2 (may be NULL, not cache) receives the same bytes.  1 launch. */
+int r4_padqn_refresh(const float* params, const float* emb, int num_actions, int emb_dim, uint8_t* cache, uint8_t* cache2,
+                     void* stream);
+/* The network on obs f32[n,256] with mask u8[n,A] -> action i32[n] and, when q != NULL, Qm f32[n,A] (else Qm goes to the
+ * scratch).  explore 0: the first argmax of Qm.  explore 1: SoftQ (temperature 1) over Qm, r4_rainbow_act's rule and
+ * draws.  cache: params' cache.  3 launches. */
+int r4_padqn_act(const float* params, const uint8_t* cache, const float* obs, const uint8_t* mask, int n, int num_actions,
+                 int emb_dim, int explore, uint64_t seed, uint64_t counter, int32_t* action, float* q, float* scratch,
+                 void* stream);
+/* The 1-step replay store of r4_replay_store_nstep (n_step 1) that also keeps the next state's mask: next_mask u8[C, A]
+ * slot of row r = t B + b is mask u8[T*B, A] row r + B, or final_mask u8[B, A] row b at t = T - 1.  1 launch. */
+int r4_padqn_store(float* r_obs, int32_t* r_action, float* r_reward, float* r_new_obs, uint8_t* r_done, uint8_t* r_next_mask,
+                   float* r_prio, const float* max_prio, int capacity, int num_actions, int64_t pos, float alpha,
+                   const float* obs, const float* final_obs, const uint8_t* mask, const uint8_t* final_mask,
+                   const int32_t* action, const float* reward, const uint8_t* done, int T, int B, void* stream);
+/* Gradient of the double-Q Huber loss over the replay rows idx[0..n) (weights f32[n] may be NULL = 1): a* = the first
+ * argmax of the online Qm(s', .) under the stored next mask, y = r + gamma (1 - done) Qm_target(s', a*), td = Q(s, a) - y,
+ * loss = sum_i w_i huber(td_i) inv_n (delta 1).  grad f32[num_params] receives the gradient (deterministic), td f32[n] (may
+ * be NULL) the td errors, stats f32[3] (may be NULL) {loss, mean td, mean Q(s, a)}, each sum times inv_n.  7 launches. */
+int r4_padqn_grad(const float* params, const float* target, const uint8_t* cache, const uint8_t* target_cache, const float* emb,
+                  int num_actions, int emb_dim, const float* r_obs, const int32_t* r_action, const float* r_reward,
+                  const float* r_new_obs, const uint8_t* r_done, const uint8_t* r_next_mask, const int64_t* idx,
+                  const float* weights, int n, float gamma, float inv_n, float* scratch, float* grad, float* td, float* stats,
+                  void* stream);
+/* The optimiser step: r4_rainbow_apply's per-tensor clip (each of the 6 tensors on its own), Adam and, when copy_target,
+ * target = params; then r4_padqn_refresh of cache and, when copy_target, of target_cache.  2 launches. */
+int r4_padqn_apply(float* params, float* target, const float* grad, float* m, float* v, const float* emb, int num_actions,
+                   int emb_dim, uint8_t* cache, uint8_t* target_cache, int step, float lr, float adam_eps, float grad_clip,
+                   int copy_target, void* stream);
+/* One SGD step with no host round trip: r4_replay_sample (n indices from u), r4_padqn_grad (loss = mean over n),
+ * r4_padqn_apply and, with prio != NULL, r4_replay_update_priorities from td.  stats (may be NULL) as r4_padqn_grad.
+ * 11 launches with prio, 10 without, whether or not the target is copied. */
+int r4_padqn_train_step(float* params, float* target, float* m, float* v, const float* emb, uint8_t* cache,
+                        uint8_t* target_cache, int num_actions, int emb_dim, const float* r_obs, const int32_t* r_action,
+                        const float* r_reward, const float* r_new_obs, const uint8_t* r_done, const uint8_t* r_next_mask,
+                        float* r_prio, float* max_prio, int size, int n, const float* u, float beta, float alpha,
+                        float prio_eps, float gamma, int step, float lr, float adam_eps, float grad_clip, int copy_target,
+                        float* scratch, float* stats, void* stream);
+
 /* ---- batch RL on the logged dataset (batchrl_trainer.py:34-90; d3rlpy 0.91 DiscreteBC / DiscreteBCQ / DiscreteCQL as the
  * reference configures them, INTEGRATION.md section 3).  algo 0 BC, 1 BCQ, 2 CQL; obs_dim K in 11..4096 (the d3rl
  * observation: simulator obs | 9 prev actions | cur_steps), A = action_size in 2..512, with the shared planes within
@@ -877,7 +933,7 @@ int r4_ope_step(int t, int T, int B, int A, int C, int layer, const float* probs
 int64_t r4_ope_launch_count(void);
 
 /* kernels launched so far by every learner entry point in this process (r4_policy_*, r4_gae, r4_adam_step, r4_ppo_epoch*,
- * r4_grad_exchange*, r4_gauss_*, r4_vtrace, r4_impala_step, r4_ddpg_*, r4_replay_*, r4_rainbow_*, r4_batchrl_*,
+ * r4_grad_exchange*, r4_gauss_*, r4_vtrace, r4_impala_step, r4_ddpg_*, r4_replay_*, r4_rainbow_*, r4_padqn_*, r4_batchrl_*,
  * r4_simtrain_*, r4_exactk_*, r4_s2s_*, r4_ope_*): the sum of the batch RL, simulator-trainer, Exact-K, seq2seq and OPE
  * counts above and the online learners'. */
 int64_t r4_learner_launch_count(void);

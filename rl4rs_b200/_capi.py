@@ -144,6 +144,19 @@ EXPORTS = {
     "r4_rainbow_train_step": (C.c_int, [C.c_void_p] * 5 + [C.c_int, C.c_int, C.c_float, C.c_float] + [C.c_void_p] * 7 +
                               [C.c_int, C.c_int, C.c_void_p] + [C.c_float] * 4 + [C.c_int, C.c_float, C.c_float, C.c_float,
                                                                                   C.c_int] + [C.c_void_p] * 3),
+    "r4_padqn_num_params": (C.c_int, [C.c_int, C.c_int]),
+    "r4_padqn_scratch_size": (C.c_int64, [C.c_int, C.c_int, C.c_int]),
+    "r4_padqn_cache_size": (C.c_int64, [C.c_int]),
+    "r4_padqn_refresh": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "r4_padqn_act": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 4 + [C.c_uint64, C.c_uint64] + [C.c_void_p] * 4),
+    "r4_padqn_store": (C.c_int, [C.c_void_p] * 8 + [C.c_int, C.c_int, C.c_int64, C.c_float] + [C.c_void_p] * 7 +
+                       [C.c_int, C.c_int, C.c_void_p]),
+    "r4_padqn_grad": (C.c_int, [C.c_void_p] * 5 + [C.c_int, C.c_int] + [C.c_void_p] * 8 + [C.c_int, C.c_float, C.c_float] +
+                      [C.c_void_p] * 5),
+    "r4_padqn_apply": (C.c_int, [C.c_void_p] * 6 + [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int] + [C.c_float] * 3 +
+                       [C.c_int, C.c_void_p]),
+    "r4_padqn_train_step": (C.c_int, [C.c_void_p] * 7 + [C.c_int, C.c_int] + [C.c_void_p] * 8 + [C.c_int, C.c_int, C.c_void_p] +
+                            [C.c_float] * 4 + [C.c_int] + [C.c_float] * 3 + [C.c_int] + [C.c_void_p] * 3),
     "r4_batchrl_num_params": (C.c_int, [C.c_int] * 3),
     "r4_batchrl_target_size": (C.c_int, [C.c_int] * 3),
     "r4_batchrl_scratch_size": (C.c_int64, [C.c_int] * 4),

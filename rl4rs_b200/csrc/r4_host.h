@@ -44,8 +44,8 @@ inline int sm_count() {
 }
 
 // Learner families, each with its own launch counter (r4_batchrl_launch_count, r4_simtrain_launch_count,
-// r4_exactk_launch_count, r4_s2s_launch_count, r4_ope_launch_count); the online learners (PPO / A2C, Gaussian, DDPG / TD3, RAINBOW and the
-// peer-memory exchange) share one.
+// r4_exactk_launch_count, r4_s2s_launch_count, r4_ope_launch_count); the online learners (PPO / A2C, Gaussian,
+// DDPG / TD3, RAINBOW, PA-DQN and the peer-memory exchange) share one.
 enum Family { FAM_ONLINE, FAM_BATCHRL, FAM_SIMTRAIN, FAM_EXACTK, FAM_SEQ2SEQ, FAM_OPE, FAM_COUNT };
 
 inline std::atomic<int64_t> g_launches[FAM_COUNT];

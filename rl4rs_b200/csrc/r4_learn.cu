@@ -1,5 +1,5 @@
 // r4_learn.cu -- host side of the learner entry points of include/rl4rs_b200.h: PPO / A2C, the peer-memory gradient
-// exchange, the Gaussian policy, DDPG / TD3, RAINBOW, batch RL and the simulator trainer.  Stateless: every call enqueues
+// exchange, the Gaussian policy, DDPG / TD3, RAINBOW, PA-DQN, batch RL and the simulator trainer.  Stateless: every call enqueues
 // its kernels on the caller's stream through r4h::launch, which counts them (r4_learner_launch_count).  See DESIGN.md.
 #include "../../include/rl4rs_b200.h"
 #include "r4_host.h"
@@ -707,6 +707,144 @@ int r4_rainbow_train_step(r4_comm* comm, float* params, float* target, float* m,
     g = sum;
   }
   rc = r4_rainbow_apply(params, target, g, m, v, num_actions, num_atoms, step, lr, adam_eps, grad_clip, copy_target, stream);
+  if (rc || !r_prio) return rc;
+  return r4_replay_update_priorities(r_prio, max_prio, P.idx, P.td, n, alpha, prio_eps, stream);
+}
+
+// ---- PA-DQN (r4_padqn.cuh) ----------------------------------------------------------------------------------
+static bool padqn_dims_ok(int A, int D) { return A >= 2 && A <= r4pa::MAXA && D >= 1 && D <= r4pa::MAXD; }
+// n rows of A pairs each: the flat pair index of the scorer's tiles stays an int
+static bool padqn_rows_ok(int A, int n) { return n >= 1 && (int64_t)n * A <= (int64_t)0x7fffffff - r4pa::PM; }
+// the scratch and the caches are read by float4 loads and bulk copies
+static bool a16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+int r4_padqn_num_params(int num_actions, int emb_dim) {
+  return padqn_dims_ok(num_actions, emb_dim) ? r4pa::make_layout(num_actions, emb_dim).n : -1;
+}
+
+int64_t r4_padqn_scratch_size(int num_actions, int emb_dim, int n) {
+  if (!padqn_dims_ok(num_actions, emb_dim) || !padqn_rows_ok(num_actions, n)) return -1;
+  return (int64_t)r4pa::scratch_floats(r4pa::make_layout(num_actions, emb_dim), n);
+}
+
+int64_t r4_padqn_cache_size(int num_actions) {
+  return num_actions >= 2 && num_actions <= r4pa::MAXA ? (int64_t)r4pa::cache_bytes(num_actions) : -1;
+}
+
+int r4_padqn_refresh(const float* params, const float* emb, int num_actions, int emb_dim, uint8_t* cache, uint8_t* cache2,
+                     void* stream) {
+  if (!params || !emb || !cache || cache == cache2 || !a16(cache) || !a16(cache2) || !padqn_dims_ok(num_actions, emb_dim))
+    return fail(R4_ERR_ARG, "r4_padqn_refresh: bad argument");
+  return launch(FAM_ONLINE, "k_padqn_refresh", r4pa::k_padqn_refresh, r4pa::IMG_CTAS + num_actions, 256, 0, S(stream), false,
+                r4pa::make_layout(num_actions, emb_dim), params, emb, cache, cache2);
+}
+
+// Qm [n][A] of the rows S [n][256] against the cache's items: the pair scorer, one persistent CTA per SM at most
+static int padqn_pairs(const r4pa::Layout& L, const float* params, const uint8_t* cache, const float* s, const uint8_t* mask,
+                       int n, float* qm, cudaStream_t st) {
+  const int64_t tiles = ((int64_t)n * L.A + r4pa::PM - 1) / r4pa::PM;
+  return launch(FAM_ONLINE, "k_padqn_pairs", r4pa::k_padqn_pairs, (unsigned)std::min<int64_t>(tiles, sm_count()),
+                r4pa::PTHREADS, r4pa::PAIRS_SMEM, st, false, s, cache, params, L, mask, n, qm);
+}
+
+int r4_padqn_act(const float* params, const uint8_t* cache, const float* obs, const uint8_t* mask, int n, int num_actions,
+                 int emb_dim, int explore, uint64_t seed, uint64_t counter, int32_t* action, float* q, float* scratch,
+                 void* stream) {
+  if (!params || !cache || !obs || !mask || !action || !scratch || !a16(cache) || !a16(scratch) ||
+      !padqn_dims_ok(num_actions, emb_dim) || !padqn_rows_ok(num_actions, n))
+    return fail(R4_ERR_ARG, "r4_padqn_act: bad argument (actions 2..512, emb_dim 1..512, n >= 1, n x actions < 2^31)");
+  const r4pa::Layout L = r4pa::make_layout(num_actions, emb_dim);
+  const r4pa::Planes P = r4pa::make_planes(scratch, L, n);
+  float* qm = q ? q : P.q_on;
+  cudaStream_t st = S(stream);
+  int rc = dense_mm(FAM_ONLINE, st, rm(obs, r4pa::OBS), rm(params + L.w1, r4pa::H), P.s_on, r4pa::H, n, r4pa::H, r4pa::OBS,
+                    params + L.b1);
+  if (!rc) rc = padqn_pairs(L, params, cache, P.s_on, mask, n, qm, st);
+  if (rc) return rc;
+  return launch(FAM_ONLINE, "k_padqn_act", r4pa::k_padqn_act, blocks(n, r4pa::NT / 32), r4pa::NT, 0, st, false, qm, n,
+                num_actions, explore != 0, seed, counter, action);
+}
+
+int r4_padqn_store(float* r_obs, int32_t* r_action, float* r_reward, float* r_new_obs, uint8_t* r_done, uint8_t* r_next_mask,
+                   float* r_prio, const float* max_prio, int capacity, int num_actions, int64_t pos, float alpha,
+                   const float* obs, const float* final_obs, const uint8_t* mask, const uint8_t* final_mask,
+                   const int32_t* action, const float* reward, const uint8_t* done, int T, int B, void* stream) {
+  if (!r_obs || !r_action || !r_reward || !r_new_obs || !r_done || !r_next_mask || (r_prio && !max_prio) || capacity < 1 ||
+      pos < 0 || num_actions < 2 || num_actions > r4pa::MAXA || !obs || !final_obs || !mask || !final_mask || !action ||
+      !reward || !done || T < 1 || B < 1)
+    return fail(R4_ERR_ARG, "r4_padqn_store: bad argument");
+  const int64_t rows = std::min<int64_t>((int64_t)T * B, capacity);
+  const r4pa::Ring R{r_obs, r_action, r_reward, r_new_obs, r_done, r_next_mask};
+  return launch(FAM_ONLINE, "k_padqn_store", r4pa::k_padqn_store, (unsigned)rows, 64, 0, S(stream), false, R, r_prio, max_prio,
+                capacity, num_actions, pos, alpha, obs, final_obs, mask, final_mask, action, reward, done, T, B);
+}
+
+int r4_padqn_grad(const float* params, const float* target, const uint8_t* cache, const uint8_t* target_cache, const float* emb,
+                  int num_actions, int emb_dim, const float* r_obs, const int32_t* r_action, const float* r_reward,
+                  const float* r_new_obs, const uint8_t* r_done, const uint8_t* r_next_mask, const int64_t* idx,
+                  const float* weights, int n, float gamma, float inv_n, float* scratch, float* grad, float* td, float* stats,
+                  void* stream) {
+  if (!params || !target || !cache || !target_cache || !emb || !padqn_dims_ok(num_actions, emb_dim) || !r_obs || !r_action ||
+      !r_reward || !r_new_obs || !r_done || !r_next_mask || !idx || !padqn_rows_ok(num_actions, n) || !scratch || !grad ||
+      !a16(scratch) || !a16(cache) || !a16(target_cache))
+    return fail(R4_ERR_ARG, "r4_padqn_grad: bad argument");
+  const r4pa::Layout L = r4pa::make_layout(num_actions, emb_dim);
+  r4pa::Planes P = r4pa::make_planes(scratch, L, n);
+  if (td) P.td = td;
+  cudaStream_t st = S(stream);
+  using r4pa::H;
+  using r4pa::OBS;
+  int rc = launch(FAM_ONLINE, "k_padqn_gather", r4pa::k_padqn_gather, n, 128, 0, st, false, r_new_obs, r_next_mask, num_actions,
+                  idx, P.x2, P.m2);
+  if (!rc) rc = dense_mm(FAM_ONLINE, st, rm(P.x2, OBS), rm(params + L.w1, H), P.s_on, H, n, H, OBS, params + L.b1);
+  if (!rc) rc = dense_mm(FAM_ONLINE, st, rm(P.x2, OBS), rm(target + L.w1, H), P.s_tg, H, n, H, OBS, target + L.b1);
+  if (!rc) rc = padqn_pairs(L, params, cache, P.s_on, P.m2, n, P.q_on, st);
+  if (!rc) rc = padqn_pairs(L, target, target_cache, P.s_tg, P.m2, n, P.q_tg, st);
+  if (!rc) rc = launch(FAM_ONLINE, "k_padqn_rows", r4pa::k_padqn_rows, blocks(n, r4pa::TS), r4pa::NT, r4pa::rows_smem(L), st,
+                       false, L, params, emb, r4pa::Replay{r_obs, r_action, r_reward, r_done}, gamma, inv_n, idx, weights, n, P);
+  if (rc) return rc;
+  return dense_wgrad(FAM_ONLINE, st, r4pa::make_jobs(L, P), n, 1, grad, Stats{P.stats, 3, nullptr, stats, inv_n, 0});
+}
+
+int r4_padqn_apply(float* params, float* target, const float* grad, float* m, float* v, const float* emb, int num_actions,
+                   int emb_dim, uint8_t* cache, uint8_t* target_cache, int step, float lr, float adam_eps, float grad_clip,
+                   int copy_target, void* stream) {
+  if (!params || !target || !grad || !m || !v || !emb || !cache || !target_cache || cache == target_cache || !a16(cache) ||
+      !a16(target_cache) || !padqn_dims_ok(num_actions, emb_dim) || step < 1)
+    return fail(R4_ERR_ARG, "r4_padqn_apply: bad argument");
+  const r4pa::Layout L = r4pa::make_layout(num_actions, emb_dim);
+  // k_rainbow_apply over PA-DQN's 6 tensors; the split's other 6 entries are empty and own no CTA
+  r4rb::Split Sp;
+  const int st6[7] = {L.w1, L.b1, L.w2, L.b2, L.w3, L.b3, L.n};
+  Sp.cta0[0] = 0;
+  for (int k = 0; k <= r4rb::NTEN; ++k) Sp.start[k] = k < 7 ? st6[k] : L.n;
+  for (int k = 0; k < r4rb::NTEN; ++k) Sp.cta0[k + 1] = Sp.cta0[k] + (Sp.start[k + 1] - Sp.start[k] + r4rb::ACH - 1) / r4rb::ACH;
+  int rc = launch(FAM_ONLINE, "k_rainbow_apply", r4rb::k_rainbow_apply, Sp.cta0[r4rb::NTEN], r4rb::ANT, 0, S(stream), false, Sp,
+                  params, target, grad, m, v, step, lr, adam_eps, grad_clip, copy_target != 0);
+  if (rc) return rc;
+  return r4_padqn_refresh(params, emb, num_actions, emb_dim, cache, copy_target ? target_cache : nullptr, stream);
+}
+
+int r4_padqn_train_step(float* params, float* target, float* m, float* v, const float* emb, uint8_t* cache,
+                        uint8_t* target_cache, int num_actions, int emb_dim, const float* r_obs, const int32_t* r_action,
+                        const float* r_reward, const float* r_new_obs, const uint8_t* r_done, const uint8_t* r_next_mask,
+                        float* r_prio, float* max_prio, int size, int n, const float* u, float beta, float alpha,
+                        float prio_eps, float gamma, int step, float lr, float adam_eps, float grad_clip, int copy_target,
+                        float* scratch, float* stats, void* stream) {
+  if (!scratch || !padqn_dims_ok(num_actions, emb_dim) || !padqn_rows_ok(num_actions, n) || (r_prio && !max_prio) ||
+      size < 1 || !u || step < 1 || !params || !target || !m || !v || !emb || !cache || !target_cache || cache == target_cache ||
+      !r_obs || !r_action || !r_reward || !r_new_obs || !r_done || !r_next_mask || !a16(scratch) || !a16(cache) ||
+      !a16(target_cache))
+    return fail(R4_ERR_ARG, "r4_padqn_train_step: bad argument");
+  const r4pa::Planes P = r4pa::make_planes(scratch, r4pa::make_layout(num_actions, emb_dim), n);
+  int rc = r4_replay_sample(r_prio, size, n, beta, u, P.idx, P.weights, stream);
+  if (rc) return rc;
+  rc = r4_padqn_grad(params, target, cache, target_cache, emb, num_actions, emb_dim, r_obs, r_action, r_reward, r_new_obs,
+                     r_done, r_next_mask, P.idx, r_prio ? P.weights : nullptr, n, gamma, 1.0f / (float)n, scratch, P.grad,
+                     nullptr, stats, stream);
+  if (rc) return rc;
+  rc = r4_padqn_apply(params, target, P.grad, m, v, emb, num_actions, emb_dim, cache, target_cache, step, lr, adam_eps,
+                      grad_clip, copy_target, stream);
   if (rc || !r_prio) return rc;
   return r4_replay_update_priorities(r_prio, max_prio, P.idx, P.td, n, alpha, prio_eps, stream);
 }

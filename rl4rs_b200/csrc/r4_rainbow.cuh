@@ -24,6 +24,7 @@
 
 #include "r4_ddpg.cuh"
 #include "r4_dense.cuh"
+#include "r4_padqn.cuh"   // the parametric-action sibling: PA-DQN's optimiser step is k_rainbow_apply below
 
 namespace r4rb {
 

@@ -393,6 +393,94 @@ class DistributionalQNetwork(object):
         return torch.as_tensor(a, dtype=torch.int32, device=q.device), q
 
 
+class ParametricQNetwork(object):
+    """The parametric-action Q network of PA-DQN: for a row s and an item a the input is x = [obs(s) (256) | e(a) (D)], e(a)
+    row a of the env's fixed item vectors emb [A, D] (engine.action_emb), through RLlib's default fcnet
+    (fcnet_hiddens [256, 256], tanh): Dense 256 tanh -> Dense 256 tanh -> Dense 1; normc(1.0) hidden kernels, normc(0.01)
+    output kernel, zero biases.  The masked values are Qm(s, a) = Q(s, a) where the mask is set and float32.min where it is
+    not (MyMaskActionsModel's Q + max(log mask, float32.min), as a select).  One flat buffer (csrc/r4_padqn.cuh's layout)
+    and a target copy of it.  This torch twin is the CPU path of PADQNTrainer and the autograd cross-check of the kernels
+    (tests/test_gpu_trainer_padqn.py)."""
+
+    H = 256
+
+    def __init__(self, emb, device="cuda", seed=0):
+        self.device = torch.device(device)
+        self.emb = torch.as_tensor(emb, dtype=torch.float32).to(self.device).contiguous()
+        self.A, self.D = self.emb.shape
+        H, K = self.H, OBS + self.D
+        shapes = [("w1", (K, H)), ("b1", (H,)), ("w2", (H, H)), ("b2", (H,)), ("w3", (H, 1)), ("b3", (1,))]
+        n = sum(math.prod(s) for _, s in shapes)
+        g = torch.Generator(device="cpu").manual_seed(seed)
+        self.flat = torch.zeros(n, dtype=torch.float32, device=self.device, requires_grad=True)
+        self.slices, off = [], 0
+        with torch.no_grad():
+            for name, shape in shapes:
+                k = math.prod(shape)
+                if len(shape) == 2:                    # normc_initializer(1.0), 0.01 for the output layer
+                    w = torch.randn(shape, generator=g)
+                    std = 0.01 if name == "w3" else 1.0
+                    self.flat[off:off + k].view(shape).copy_((w * std / w.pow(2).sum(0, keepdim=True).sqrt()).to(self.device))
+                self.slices.append((off, off + k))
+                off += k
+        self._shapes, self.n_params = shapes, n
+        self.target = self.flat.detach().clone()
+
+    params = DeterministicActorCritic.params
+    clip_per_tensor = DistributionalQNetwork.clip_per_tensor
+
+    def inputs(self, obs):
+        """env observation {'obs', 'action_mask'} -> (obs, mask)."""
+        return obs["obs"], obs["action_mask"]
+
+    def q_pairs(self, obs, action, flat=None):
+        """Q(s, a) [n] of the n pairs (obs [n, 256], action [n])."""
+        p = self.params(flat)
+        x = torch.cat([obs, self.emb[action.long()]], dim=1)
+        h = torch.tanh(torch.tanh(x @ p["w1"] + p["b1"]) @ p["w2"] + p["b2"])
+        return (h @ p["w3"] + p["b3"]).squeeze(-1)
+
+    def forward(self, obs, mask, flat=None):
+        """obs f32 [n, 256], mask {0, 1} [n, A] -> Qm [n, A], through the split first layer (S[s] + P[a]) in row chunks."""
+        p = self.params(flat)
+        S = obs @ p["w1"][:OBS] + p["b1"]
+        P = self.emb @ p["w1"][OBS:]
+        out = []
+        for i in range(0, obs.shape[0], 64):
+            h = torch.tanh(torch.tanh(S[i:i + 64, None, :] + P[None]) @ p["w2"] + p["b2"])
+            out.append((h @ p["w3"] + p["b3"]).squeeze(-1))
+        q = torch.cat(out) if out else S.new_zeros(0, self.A)
+        return torch.where(mask.to(torch.bool), q, torch.full_like(q, FLOAT_MIN))
+
+    def loss(self, obs, action, reward, new_obs, done, next_mask, weights=None, gamma=1.0, inv_n=None):
+        """The double-Q Huber loss sum_i w_i huber(td_i) * inv_n (default 1/n), td = Q(s, a) - (r + gamma (1 - done)
+        Qm_target(s', argmax Qm_online(s', .))) -> (loss, td [n], Q(s, a) [n])."""
+        n = obs.shape[0]
+        inv_n = 1.0 / n if inv_n is None else inv_n
+        rows = torch.arange(n, device=obs.device)
+        with torch.no_grad():
+            a_star = self.forward(new_obs, next_mask).argmax(1)
+            qt = self.forward(new_obs, next_mask, self.target)[rows, a_star]
+            y = reward.to(torch.float32) + gamma * (1.0 - done.to(torch.float32)) * qt
+        q = self.q_pairs(obs, action)
+        td = q - y
+        w = torch.ones(n, device=obs.device) if weights is None else weights
+        hub = torch.where(td.abs() <= 1.0, 0.5 * td * td, td.abs() - 0.5)
+        return (w * hub).sum() * inv_n, td.detach(), q.detach()
+
+    @torch.no_grad()
+    def act(self, obs, mask, explore, seed=0, counter=0):
+        """-> (action i32 [n], Qm [n, A]): the first argmax of Qm, or SoftQ over csrc/r4_padqn.cuh's uniform per row."""
+        import numpy as np
+        q = self.forward(obs, mask)
+        if not explore:
+            return q.argmax(1).to(torch.int32), q
+        u = (counter_draws(seed, counter, q.shape[0], 1)[0][:, 0] + 1.0) / 2.0       # the top 24 bits / 2^24
+        cdf = np.cumsum(torch.softmax(q.double(), 1).cpu().numpy(), 1)
+        a = np.minimum((cdf <= (u * cdf[:, -1])[:, None]).sum(1), self.A - 1)
+        return torch.as_tensor(a, dtype=torch.int32, device=q.device), q
+
+
 class RawStatePolicy(object):
     """RLlib 'mask_model_rawstate' (rl4rs/nets/rllib/rllib_mask_model.py:67-115 over rllib_rawstate_model.py:25-86): the
     policy reads the RAW state -- category ids [21], dense features [432], sequence ids [2,64] (`rawstate_as_obs`,

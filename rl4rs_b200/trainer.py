@@ -28,8 +28,8 @@ import torch.distributed as dist
 
 from . import _capi
 from ._capi import ptr
-from .policy import (DeterministicActorCritic, DistributionalQNetwork, GaussianPolicy, MaskedPolicy, RawStatePolicy,
-                     counter_draws)
+from .policy import (DeterministicActorCritic, DistributionalQNetwork, GaussianPolicy, MaskedPolicy, ParametricQNetwork,
+                     RawStatePolicy, counter_draws)
 
 
 def _hp(hp):
@@ -1141,7 +1141,7 @@ class _ReplayTrainer(_TrainerBase):
         rew, stats = [], torch.zeros(3, dtype=torch.float64, device=self.device)
         while sampled < c["timesteps_per_iteration"]:
             self.rollout(explore=True)
-            self.replay.store(self.buf_obs, self.final_obs, self.buf_action, self.buf_reward, self.buf_done)
+            self._store()
             sampled += self.T * self.B * w
             rew.append(self.buf_reward.sum(0).mean())
             if self.replay.added * w >= c["learning_starts"]:
@@ -1156,6 +1156,10 @@ class _ReplayTrainer(_TrainerBase):
                "num_steps_trained": self.critic_steps * self.n_local * w, "replay_size": self.replay.size}
         out.update({s: g[s] / k if steps else float("nan") for s in self.STATS})
         return out
+
+    def _store(self):
+        """The last rollout into the replay."""
+        self.replay.store(self.buf_obs, self.final_obs, self.buf_action, self.buf_reward, self.buf_done)
 
     def _state(self, kernel_adam):
         return {"target": self.policy.target.cpu(), "counter": self.counter, "policy_ts": self.policy_ts,
@@ -1491,6 +1495,262 @@ class RainbowTrainer(_ReplayTrainer):
         self.last_target_update, self.critic_steps = st["last_target_update"], st["sgd_steps"]
 
 
+# ---- PA-DQN ----------------------------------------------------------------------------------------------------------
+# The DQN block of modelfree_train.py:106-133 over RLlib 1.5's DQN defaults (INTEGRATION.md section 3): double Q, no
+# dueling, no distributional head (hiddens []), n-step 1.  train_batch_size None = min(B * max_steps, 1024).
+PADQN_DEFAULTS = {"gamma": 1.0, "lr": 5e-4, "adam_epsilon": 1e-8, "grad_clip": 40.0, "prioritized_replay": True,
+                  "prioritized_replay_alpha": 0.6, "prioritized_replay_beta": 0.4, "prioritized_replay_eps": 1e-6,
+                  "buffer_size": 100000, "learning_starts": 1000, "target_network_update_freq": 200,
+                  "timesteps_per_iteration": 1000, "train_batch_size": None}
+
+
+class PAReplayBuffer(ReplayBuffer):
+    """The 1-step replay of PA-DQN: ReplayBuffer's rows with i32 actions, and the next state's action mask u8 [C, A] (the
+    mask of row t + 1, or the final observation's at the last step).  `ops` is PADQNKernelOps, or None for torch."""
+
+    def __init__(self, capacity, A, device, prioritized, alpha=0.6, ops=None):
+        super().__init__(capacity, None, device, prioritized, alpha, ops, n_step=1)
+        self.A = A
+        self.next_mask = torch.empty(self.C, A, dtype=torch.uint8, device=device)
+
+    def store(self, obs, final_obs, action, reward, done, mask=None, final_mask=None):
+        """A [T, B] rollout with its masks [T, B, A] and the final masks [B, A]."""
+        T, B = reward.shape
+        n = T * B
+        if self.ops is not None:
+            self.ops.replay_store(self, obs, final_obs, mask, final_mask, action, reward, done)
+            self.added += n
+            return
+        rows = torch.arange(max(0, n - self.C), n, device=self.device)
+        slots = (self.added + rows) % self.C
+        nxt = torch.cat([mask[1:].reshape(-1, self.A), final_mask.reshape(B, self.A)])
+        self.next_mask[slots] = nxt[rows].to(torch.uint8)
+        super().store(obs, final_obs, action, reward, done)
+
+    def gather(self, idx):
+        return super().gather(idx) + (self.next_mask[idx],)
+
+
+class PADQNKernelOps(_ReplayOps):
+    """ctypes front of the PA-DQN kernels (include/rl4rs_b200.h: r4_padqn_*, and the sampling and priority kernels of the
+    DDPG replay): the Adam moments m, v, the learner scratch for n samples per step, the loss statistics, the item vectors
+    and the two nets' caches (the w2 image and the item half of the first layer, rebuilt by refresh)."""
+
+    def __init__(self, emb, device, n_params, n):
+        self.A, self.D = emb.shape
+        lib = _capi.load_library()
+        assert lib.r4_padqn_num_params(self.A, self.D) == n_params
+        super().__init__(device, n_params, n, lib.r4_padqn_scratch_size(self.A, self.D, n))
+        self.n = n                          # the most samples one SGD step may take: the scratch is sized for them
+        self.emb = emb.to(device=device, dtype=torch.float32).contiguous()
+        cb = lib.r4_padqn_cache_size(self.A)
+        self.cache = torch.zeros(cb, dtype=torch.uint8, device=device)
+        self.target_cache = torch.zeros(cb, dtype=torch.uint8, device=device)
+        self.act_scratch = torch.zeros(0, dtype=torch.float32, device=device)
+
+    def _fits(self, n):
+        if not 1 <= n <= self.n:
+            raise ValueError("PADQNKernelOps: %d samples per step, the scratch holds 1..%d" % (n, self.n))
+
+    def refresh(self, pol):
+        """Both caches from the current parameters (after construction, restore, or an update outside apply)."""
+        for p, c in ((pol.flat, self.cache), (pol.target, self.target_cache)):
+            rc = self.lib.r4_padqn_refresh(ptr(p), ptr(self.emb), self.A, self.D, ptr(c), None, self._stream())
+            self._check(rc, "r4_padqn_refresh")
+
+    def act(self, pol, obs, mask, explore, seed, counter, action, q=None):
+        n = obs.shape[0]
+        need = self.lib.r4_padqn_scratch_size(self.A, self.D, n)
+        if self.act_scratch.numel() < need:
+            self.act_scratch = torch.zeros(need, dtype=torch.float32, device=self.device)
+        rc = self.lib.r4_padqn_act(ptr(pol.flat), ptr(self.cache), ptr(obs), ptr(mask), n, self.A, self.D, int(bool(explore)),
+                                   seed, counter, ptr(action), ptr(q), ptr(self.act_scratch), self._stream())
+        self._check(rc, "r4_padqn_act")
+
+    def _replay(self, rb):
+        return super()._replay(rb) + (ptr(rb.next_mask),)
+
+    def replay_store(self, rb, obs, final_obs, mask, final_mask, action, reward, done):
+        T, B = reward.shape
+        rc = self.lib.r4_padqn_store(*self._replay(rb), ptr(rb.prio), ptr(rb.max_prio), rb.C, self.A, rb.added, rb.alpha,
+                                     ptr(obs), ptr(final_obs), ptr(mask), ptr(final_mask), ptr(action), ptr(reward), ptr(done),
+                                     T, B, self._stream())
+        self._check(rc, "r4_padqn_store")
+
+    def grad_(self, pol, rb, idx, weights, gamma, inv_n):
+        """self.grad, self.td, self.stats = r4_padqn_grad over replay rows idx."""
+        self._fits(idx.shape[0])
+        o, a, r, no, d, nm = self._replay(rb)
+        rc = self.lib.r4_padqn_grad(ptr(pol.flat), ptr(pol.target), ptr(self.cache), ptr(self.target_cache), ptr(self.emb),
+                                    self.A, self.D, o, a, r, no, d, nm, ptr(idx), ptr(weights), idx.shape[0], gamma, inv_n,
+                                    ptr(self.scratch), ptr(self.grad), ptr(self.td), ptr(self.stats), self._stream())
+        self._check(rc, "r4_padqn_grad")
+
+    def apply(self, pol, step, hp, copy_target):
+        rc = self.lib.r4_padqn_apply(ptr(pol.flat), ptr(pol.target), ptr(self.grad), ptr(self.m), ptr(self.v), ptr(self.emb),
+                                     self.A, self.D, ptr(self.cache), ptr(self.target_cache), step, hp["lr"], hp["adam_eps"],
+                                     hp["grad_clip"], int(copy_target), self._stream())
+        self._check(rc, "r4_padqn_apply")
+
+    def train_step(self, pol, rb, u, step, copy_target, hp):
+        """One whole SGD step in one library call (sample, gradient, clip + Adam + target copy, cache refresh,
+        priorities)."""
+        self._fits(u.shape[0])
+        rc = self.lib.r4_padqn_train_step(ptr(pol.flat), ptr(pol.target), ptr(self.m), ptr(self.v), ptr(self.emb),
+                                          ptr(self.cache), ptr(self.target_cache), self.A, self.D, *self._replay(rb),
+                                          ptr(rb.prio), ptr(rb.max_prio), rb.size, u.shape[0], ptr(u), hp["beta"], rb.alpha,
+                                          hp["eps"], hp["gamma"], step, hp["lr"], hp["adam_eps"], hp["grad_clip"],
+                                          int(copy_target), ptr(self.scratch), ptr(self.stats), self._stream())
+        self._check(rc, "r4_padqn_train_step")
+
+
+class PADQNTrainer(_ReplayTrainer):
+    """Parametric-action DQN (RLlib 1.5 DQNTrainer with modelfree_train.py's DQN block: double Q, no dueling, no
+    distributional head, n-step 1, prioritized replay) with the state-action network ParametricQNetwork over the env's
+    item vectors, masked as the script's mask_model masks, acting in Discrete(A) with SoftQ(T = 1) exploration and argmax
+    evaluation, on _ReplayTrainer's schedule.  The target net is hard-copied after the SGD step at which
+    target_network_update_freq timesteps were sampled since the last copy (the first step copies).  On CUDA: the pair
+    scorer and act kernels, the replay kernels and r4_padqn_train_step; on CPU the torch twin.  One GPU: data-parallel
+    PA-DQN is not built."""
+    algo = "PADQN"
+    DEFAULTS = PADQN_DEFAULTS
+    STATS = ("loss", "mean_td_error", "mean_q")
+
+    def __init__(self, config, env, device=None, seed=0):
+        import numpy as np
+        super().__init__(config, env, device, seed)
+        c = self.config
+        self.A = env.config["action_size"]
+        emb = torch.as_tensor(np.asarray(env.sim.engine.action_emb, dtype=np.float32))
+        self.policy = ParametricQNetwork(emb, self.device, seed=seed)
+        assert self.policy.A == self.A, "action_emb has %d rows for action_size %d" % (self.policy.A, self.A)
+        self.ops = PADQNKernelOps(self.policy.emb, self.device, self.policy.n_params, self.n_local) if self.use_kernels else None
+        if self.ops is not None:
+            self.ops.refresh(self.policy)
+        self.replay = PAReplayBuffer(c["buffer_size"], self.A, self.device, c["prioritized_replay"],
+                                     c["prioritized_replay_alpha"], self.ops)
+        z = lambda *s: torch.zeros(*s, dtype=torch.uint8, device=self.device)
+        self.buf_mask, self.final_mask = z(self.T, self.B, self.A), z(self.B, self.A)
+        self.opt = torch.optim.Adam([self.policy.flat], lr=c["lr"], eps=c["adam_epsilon"])
+        self.last_target_update = 0         # policy_ts at the last hard target copy
+        self.critic_steps = 0               # SGD steps taken (the Adam step count)
+
+    def _actions(self, *lead):
+        return torch.zeros(*lead, dtype=torch.int32, device=self.device)
+
+    @torch.no_grad()
+    def rollout(self, explore=True):
+        env = self.env
+        obs = env.reset()
+        for t in range(self.T):
+            o, m = self.policy.inputs(obs)
+            self.buf_obs[t].copy_(o)
+            self.buf_mask[t].copy_(m)
+            a = self._act(self.buf_obs[t], self.buf_mask[t], explore, self.buf_action[t])
+            obs, reward, done, info = env.step(a)
+            self.buf_reward[t].copy_(reward)
+            self.buf_done[t].copy_(torch.as_tensor(done))
+        o, m = self.policy.inputs(obs)
+        self.final_obs.copy_(o)
+        self.final_mask.copy_(m)
+        self.reward = self.buf_reward
+        return self
+
+    def _store(self):
+        self.replay.store(self.buf_obs, self.final_obs, self.buf_action, self.buf_reward, self.buf_done, self.buf_mask,
+                          self.final_mask)
+
+    @torch.no_grad()
+    def _act(self, obs, mask, explore, out, q=None):
+        """out i32 [n] = the action of obs [n, 256] under mask u8 [n, A]: SoftQ sampling when exploring, else the first
+        argmax of Qm; q f32 [n, A] (may be None) receives Qm."""
+        n = obs.shape[0]
+        if self.use_kernels:
+            self.ops.act(self.policy, obs, mask, explore, self._seed, self.counter, out, q)
+        else:
+            a, qq = self.policy.act(obs, mask, explore, self._seed, self.counter)
+            out.copy_(a)
+            if q is not None:
+                q.copy_(qq)
+        self.counter += n
+        if explore:
+            self.policy_ts += n * _world()
+        return out
+
+    @torch.no_grad()
+    def compute_actions(self, obs, explore=False, full_fetch=False):
+        if full_fetch or (isinstance(obs, dict) and "obs" not in obs):
+            return super().compute_actions(obs, explore, full_fetch)
+        return self._fetch(obs, explore)[0].cpu().numpy()
+
+    @torch.no_grad()
+    def _fetch(self, obs, explore=False):
+        """One act -> (actions, RLlib DQN's extra fetches): q_values, the masked Qm [n, A], which is also its
+        action_dist_inputs."""
+        if isinstance(obs, dict):
+            obs = {k: torch.as_tensor(v, device=self.device) for k, v in obs.items()}
+        o, m = self.policy.inputs(obs)
+        o = torch.as_tensor(o, dtype=torch.float32, device=self.device).contiguous()
+        m = torch.as_tensor(m, device=self.device).to(torch.uint8).contiguous()
+        q = torch.empty(o.shape[0], self.A, dtype=torch.float32, device=self.device)
+        a = self._act(o, m, explore, self._actions(o.shape[0]), q)
+        return a, {"q_values": q, "action_dist_inputs": q}
+
+    def _hp(self):
+        c = self.config
+        return {"gamma": c["gamma"], "lr": c["lr"], "adam_eps": c["adam_epsilon"], "grad_clip": float(c["grad_clip"] or 0.0),
+                "beta": c["prioritized_replay_beta"], "eps": c["prioritized_replay_eps"]}
+
+    def draws(self):
+        """The caller-side draws of one SGD step: the sampling uniforms [n]."""
+        return (torch.rand(self.n_local, generator=self.gen, device=self.device),)
+
+    def sgd_step(self, u):
+        """One SGD step on the replay with the uniforms u -> the statistics tensor [3] (loss, mean td, mean Q(s, a)); then
+        the hard target copy when due."""
+        c, hp, rb = self.config, self._hp(), self.replay
+        self.critic_steps += 1
+        copy = self.policy_ts - self.last_target_update >= c["target_network_update_freq"]
+        if copy:
+            self.last_target_update = self.policy_ts
+        if self.use_kernels:
+            self.ops.train_step(self.policy, rb, u, self.critic_steps, copy, hp)
+            return self.ops.stats
+        idx, wt = rb.sample(u, hp["beta"])
+        weights = wt if rb.prio is not None else None
+        td, stats = self.twin_step(*rb.gather(idx), weights, copy)
+        if rb.prio is not None:
+            rb.update_priorities(idx, td, hp["eps"])
+        return stats
+
+    def twin_step(self, obs, action, reward, new_obs, done, next_mask, weights, copy_target):
+        """The torch twin's step over an explicit batch: the loss (mean over the batch), the per-tensor clip,
+        torch.optim.Adam, then the hard target copy when asked -> (td, statistics [3])."""
+        c, pol = self.config, self.policy
+        if pol.flat.grad is not None:
+            pol.flat.grad.zero_()
+        inv_n = 1.0 / obs.shape[0]
+        loss, td, q = pol.loss(obs, action, reward, new_obs, done, next_mask, weights, c["gamma"], inv_n)
+        loss.backward()
+        pol.clip_per_tensor(pol.flat.grad, c["grad_clip"])
+        self.opt.step()
+        if copy_target:
+            with torch.no_grad():
+                pol.target.copy_(pol.flat.detach())
+        return td, torch.stack([loss.detach(), td.sum() * inv_n, q.sum() * inv_n])
+
+    def _state(self, kernel_adam):
+        return dict(super()._state(kernel_adam), opt=self.opt.state_dict(), last_target_update=self.last_target_update,
+                    sgd_steps=self.critic_steps)
+
+    def _load_state(self, st):
+        super()._load_state(st)
+        self.opt.load_state_dict(st["opt"])
+        self.last_target_update, self.critic_steps = st["last_target_update"], st["sgd_steps"]
+        if self.ops is not None:
+            self.ops.refresh(self.policy)
+
+
 def get_rl_model(algo, rllib_config, env=None, **kw):
     """script/modelfree_trainer.py:11-36.  Only the algorithms of the BASELINE configs are built.  On an env built with
     support_conti_env, PPO / A2C / PG / IMPALA (and their *_conti names, modelfree_train.py:46-48) train the Gaussian
@@ -1514,7 +1774,17 @@ def get_rl_model(algo, rllib_config, env=None, **kw):
             raise ValueError("RAINBOW takes the plain observation: build the env with support_rllib_mask=False "
                              "(the reference turns the mask off for RAINBOW, modelfree_train.py:50-51)")
         return RainbowTrainer(rllib_config, env, **kw)
-    gauss = {"PPO": GaussPPOTrainer, "A2C": GaussA2CTrainer, "PG": GaussPGTrainer, "IMPALA": GaussIMPALATrainer}
+    if algo in ("PADQN", "PADQN_rawstate"):              # exact names, as RAINBOW's
+        if algo.endswith("_rawstate") or (env is not None and env.config.get("rawstate_as_obs", False)):
+            raise NotImplementedError("%s on a rawstate_as_obs env (model_rawstate) is not built" % algo)
+        if conti:
+            raise ValueError("PADQN acts in Discrete(action_size): build the env without support_conti_env")
+        if env is None or not env.config.get("support_rllib_mask", False):
+            raise ValueError("PADQN masks its Q values as mask_model does: build the env with support_rllib_mask=True")
+        if _world() > 1:
+            raise NotImplementedError("data-parallel PADQN is not built: train it on one GPU")
+        return PADQNTrainer(rllib_config, env, **kw)
+    gauss ={"PPO": GaussPPOTrainer, "A2C": GaussA2CTrainer, "PG": GaussPGTrainer, "IMPALA": GaussIMPALATrainer}
     if algo.endswith("_conti") or (conti and algo in gauss):
         base = algo[:-len("_conti")] if algo.endswith("_conti") else algo
         if base not in gauss:
