@@ -462,7 +462,8 @@ int r4_rainbow_train_step(r4_comm* comm, float* params, float* target, float* m,
  * row a of the env's fixed item vectors emb f32[A, D] (action_emb), Dense 256 tanh -> Dense 256 tanh -> Dense 1, and the
  * masked values Qm(s, a) = Q(s, a) where mask[s][a] != 0, float32.min where it is 0.  RLlib 1.5 DQN with double Q, no
  * dueling, no distributional head, n_step 1 (INTEGRATION.md section 3).  A = num_actions in 2..512, D = emb_dim in 1..512,
- * n rows with n x A < 2^31 - 128.  Flat parameter layout (r4_padqn_num_params(A, D) floats; 140 033 at D = 32):
+ * n rows in 1..4 194 240 (65535 tiles of 64 rows: the row GEMM's grid limit; r4_padqn_scratch_size is -1 past it).
+ * Flat parameter layout (r4_padqn_num_params(A, D) floats; 140 033 at D = 32):
  * w1[256+D,256] b1[256] w2[256,256] b2[256] w3[256,1] b3[1]; the target has the same layout.
  * Every net has a cache (r4_padqn_cache_size(A) bytes of device memory): a pre-tiled bf16 image of w2 and P = e w1[256:]
  * [A, 256].  r4_padqn_refresh rebuilds it and must run after every change of the parameters it caches; r4_padqn_apply and

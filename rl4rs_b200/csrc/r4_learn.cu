@@ -713,8 +713,11 @@ int r4_rainbow_train_step(r4_comm* comm, float* params, float* target, float* m,
 
 // ---- PA-DQN (r4_padqn.cuh) ----------------------------------------------------------------------------------
 static bool padqn_dims_ok(int A, int D) { return A >= 2 && A <= r4pa::MAXA && D >= 1 && D <= r4pa::MAXD; }
-// n rows of A pairs each: the flat pair index of the scorer's tiles stays an int
-static bool padqn_rows_ok(int A, int n) { return n >= 1 && (int64_t)n * A <= (int64_t)0x7fffffff - r4pa::PM; }
+// n rows: k_dense_gemm puts the 64-row tiles of S = obs w1[:256] + b1 on gridDim.y (at most 65535), and the flat pair
+// index of the scorer's tiles stays an int (implied by the first bound at every A <= 512; kept as a guard)
+static bool padqn_rows_ok(int A, int n) {
+  return n >= 1 && n <= r4pa::MAXN && (int64_t)n * A <= (int64_t)0x7fffffff - r4pa::PM;
+}
 // the scratch and the caches are read by float4 loads and bulk copies
 static bool a16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 
@@ -752,7 +755,7 @@ int r4_padqn_act(const float* params, const uint8_t* cache, const float* obs, co
                  void* stream) {
   if (!params || !cache || !obs || !mask || !action || !scratch || !a16(cache) || !a16(scratch) ||
       !padqn_dims_ok(num_actions, emb_dim) || !padqn_rows_ok(num_actions, n))
-    return fail(R4_ERR_ARG, "r4_padqn_act: bad argument (actions 2..512, emb_dim 1..512, n >= 1, n x actions < 2^31)");
+    return fail(R4_ERR_ARG, "r4_padqn_act: bad argument (actions 2..512, emb_dim 1..512, n 1..4194240)");
   const r4pa::Layout L = r4pa::make_layout(num_actions, emb_dim);
   const r4pa::Planes P = r4pa::make_planes(scratch, L, n);
   float* qm = q ? q : P.q_on;

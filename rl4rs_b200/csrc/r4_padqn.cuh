@@ -31,6 +31,7 @@ namespace r4pa {
 using r4ddpg::NT;
 using r4ddpg::TS;
 constexpr int OBS = 256, H = 256, MAXA = 512, MAXD = 512;
+constexpr int MAXN = 65535 * 64;    // rows: k_dense_gemm's 64-row tiles of S on gridDim.y
 
 struct Layout {
   int A, D, K;                      // K = 256 + D: the first layer's input width

@@ -1502,6 +1502,7 @@ PADQN_DEFAULTS = {"gamma": 1.0, "lr": 5e-4, "adam_epsilon": 1e-8, "grad_clip": 4
                   "prioritized_replay_alpha": 0.6, "prioritized_replay_beta": 0.4, "prioritized_replay_eps": 1e-6,
                   "buffer_size": 100000, "learning_starts": 1000, "target_network_update_freq": 200,
                   "timesteps_per_iteration": 1000, "train_batch_size": None}
+PADQN_MAX_ROWS = 65535 * 64         # rows per act / gradient call: the row GEMM's 64-row tiles fill at most 65535 CTAs
 
 
 class PAReplayBuffer(ReplayBuffer):
@@ -1540,13 +1541,19 @@ class PADQNKernelOps(_ReplayOps):
         self.A, self.D = emb.shape
         lib = _capi.load_library()
         assert lib.r4_padqn_num_params(self.A, self.D) == n_params
-        super().__init__(device, n_params, n, lib.r4_padqn_scratch_size(self.A, self.D, n))
+        super().__init__(device, n_params, n, self._scratch_size(lib, n))
         self.n = n                          # the most samples one SGD step may take: the scratch is sized for them
         self.emb = emb.to(device=device, dtype=torch.float32).contiguous()
         cb = lib.r4_padqn_cache_size(self.A)
         self.cache = torch.zeros(cb, dtype=torch.uint8, device=device)
         self.target_cache = torch.zeros(cb, dtype=torch.uint8, device=device)
         self.act_scratch = torch.zeros(0, dtype=torch.float32, device=device)
+
+    def _scratch_size(self, lib, n):
+        size = lib.r4_padqn_scratch_size(self.A, self.D, n)
+        if size < 0:
+            raise ValueError("PADQNKernelOps: %d rows; the kernels take 1..%d rows per call" % (n, PADQN_MAX_ROWS))
+        return size
 
     def _fits(self, n):
         if not 1 <= n <= self.n:
@@ -1560,7 +1567,7 @@ class PADQNKernelOps(_ReplayOps):
 
     def act(self, pol, obs, mask, explore, seed, counter, action, q=None):
         n = obs.shape[0]
-        need = self.lib.r4_padqn_scratch_size(self.A, self.D, n)
+        need = self._scratch_size(self.lib, n)
         if self.act_scratch.numel() < need:
             self.act_scratch = torch.zeros(need, dtype=torch.float32, device=self.device)
         rc = self.lib.r4_padqn_act(ptr(pol.flat), ptr(self.cache), ptr(obs), ptr(mask), n, self.A, self.D, int(bool(explore)),
