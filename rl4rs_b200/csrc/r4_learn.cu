@@ -148,10 +148,10 @@ int r4_adam_step(float* params, const float* grad, float* m, float* v, int n, in
                  float beta2, float eps, float grad_scale, float clip, float* norm_scratch, void* stream) {
   if (!params || !grad || !m || !v || n < 1 || step < 1 || (clip > 0.f && !norm_scratch))
     return fail(R4_ERR_ARG, "r4_adam_step: bad argument");
-  if (clip > 0.f) {
-    cudaMemsetAsync(norm_scratch, 0, 4, S(stream));
-    if (int rc = launch(FAM_ONLINE, "k_sumsq", r4ppo::k_sumsq, 32, 256, 0, S(stream), false, n, grad, norm_scratch)) return rc;
-  }
+  // the norm in one CTA and a fixed order, so that two clipped steps from the same state are bit-identical
+  if (clip > 0.f)
+    if (int rc = launch(FAM_ONLINE, "k_sumsq_one", r4ppo::k_sumsq_one, 1, r4ppo::SQT, 0, S(stream), false, n, grad, norm_scratch))
+      return rc;
   return launch(FAM_ONLINE, "k_adam", r4ppo::k_adam, (n + 255) / 256, 256, 0, S(stream), false, n, params, grad, m, v, step, lr,
                 beta1, beta2, eps, grad_scale, clip > 0.f ? norm_scratch : nullptr, clip);
 }

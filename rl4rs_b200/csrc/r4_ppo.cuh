@@ -495,20 +495,6 @@ __global__ void k_gae(int T, int B, const float* __restrict__ reward, const floa
   }
 }
 
-__global__ void k_sumsq(int n, const float* __restrict__ x, float* __restrict__ out) {
-  __shared__ float red[32];
-  float s = 0.f;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) s += x[i] * x[i];
-  s = warp_sum(s);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    s = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
-    s = warp_sum(s);
-    if (threadIdx.x == 0) atomicAdd(out, s);
-  }
-}
-
 // ------------------------------------------------------------------------------------------------
 // IMPALA (RLlib 1.5 vtrace_torch_policy.py): the learner forward at the stored actions, V-trace, and the clip's norm.
 // ------------------------------------------------------------------------------------------------
@@ -577,7 +563,8 @@ __global__ void k_vtrace(int T, int B, const float* __restrict__ blogp, const fl
 }
 
 // out[0] = sum x_i^2 in ONE CTA and a fixed order (thread k adds i = k, k + SQT, ..., then a fixed tree over the warps):
-// k_sumsq adds its 32 CTAs' sums with atomics, whose order varies between runs, so IMPALA's clipped step uses this one.
+// the global norm of every clipped step (r4_adam_step, IMPALA), so that two steps from the same state are bit-identical.
+// Partial sums of several CTAs added with atomics would land in an order that varies between runs.
 __global__ void __launch_bounds__(SQT) k_sumsq_one(int n, const float* __restrict__ x, float* __restrict__ out) {
   __shared__ float red[SQT / 32];
   float s = 0.f;

@@ -3,6 +3,8 @@ pair, the double-Q target with done and masked next states, the Huber loss and e
 with torch.optim.Adam and the hard target copy, and the SoftQ / argmax rule on given uniforms."""
 import numpy as np
 
+import optim_ref64
+
 OBS, H = 256, 256
 FLOAT_MIN = float(np.finfo(np.float32).min)
 NAMES = ("w1", "b1", "w2", "b2", "w3", "b3")
@@ -76,11 +78,7 @@ def flat_grad(g, D):
 def apply(flat, target_flat, grad, m, v, step, D, lr=5e-4, eps=1e-8, clip=40.0, copy_target=False):
     """Per-tensor clip (minimize_and_clip), torch.optim.Adam (betas 0.9 / 0.999) at the 1-based step, then the hard copy ->
     (flat, target, m, v)."""
-    g = np.array(grad, dtype=np.float64)
-    for lo, hi in slices(D):
-        nrm = np.sqrt((g[lo:hi] ** 2).sum())
-        if clip > 0 and nrm > clip:
-            g[lo:hi] *= clip / nrm
+    g, _ = optim_ref64.clip_per_tensor(grad, slices(D), clip)
     m = 0.9 * m + 0.1 * g
     v = 0.999 * v + 0.001 * g * g
     denom = np.sqrt(v) / np.sqrt(1 - 0.999 ** step) + eps

@@ -59,12 +59,12 @@ def test_ppo_and_a2c_launches():
     data = _ppo_data(ops, pol, n, dev)
     perm = torch.randperm(n, generator=torch.Generator().manual_seed(2)).to(dev)
     flat = pol.flat.detach().clone()
-    for clip in (None, 0.5):      # fused: k_policy_grad + k_reduce_adam; clipped: + k_grad_reduce, k_sumsq, k_adam
+    for clip in (None, 0.5):      # fused: k_policy_grad + k_reduce_adam; clipped: + k_grad_reduce, k_sumsq_one, k_adam
         rc = []
         assert _launched(lambda: rc.append(ops.ppo_epoch(flat, data, perm, n, mb, HP, 1e-3, clip))) == \
             n // mb * (4 if clip else 2)
         assert rc == [n // mb]
-    for clip in (None, 10.0):     # A2C: k_policy_grad + k_grad_reduce, then k_adam (after k_sumsq when clipping)
+    for clip in (None, 10.0):     # A2C: k_policy_grad + k_grad_reduce, then k_adam (after k_sumsq_one when clipping)
         def a2c():
             ops.policy_grad(1, flat, data, None, 0, n, HP, 1.0, 1.0 / n)
             ops.adam(flat, 1e-3, 1.0, clip)
