@@ -240,7 +240,13 @@ int r4_ppo_epoch(float* params, const float* obs, const uint8_t* mask, const int
  * the gradient kernel and ONE kernel that reduces the local partials, pushes them into every rank's inbox, waits
  * for the peers' flags, sums in rank order and applies Adam (replicas stay bit-identical).  Every rank must call
  * it with the same n, mb and hyper-parameters.  mb = minibatch size PER RANK; the loss is the mean over
- * mb x world samples (RLlib: sgd_minibatch_size is the total over devices). */
+ * mb x world samples (RLlib: sgd_minibatch_size is the total over devices).
+ * r4_comm_create: world 1..16, rank 0..world-1, n_params >= 1 and out != NULL, else R4_ERR_ARG before any CUDA call with
+ * *out untouched; a world-1 communicator is ready at once.  Every entry point that takes a communicator checks it first,
+ * before it launches or writes anything: R4_ERR_STATE while the peers are not mapped (r4_comm_open not yet done),
+ * R4_ERR_ARG when its parameter count differs from the communicator's n_params.  A refused call leaves the
+ * communicator's step count where it was, so the ranks stay in step.  r4_ppo_epoch_dist also refuses an action_size
+ * outside 2..512 up front (R4_ERR_ARG), since the parameter count it checks against is derived from it. */
 typedef struct r4_comm r4_comm;
 int r4_comm_create(int rank, int world, int n_params, r4_comm** out);
 int r4_comm_handle(r4_comm* comm, void* handle_out_64);

@@ -74,7 +74,7 @@ __global__ void __launch_bounds__(BLK) k_exchange_adam(int n, int G, const float
   if (blockIdx.x == 0 && threadIdx.x < 5 && stats_accum) {
     float a = 0.f;
     for (int c = 0; c < G; ++c) a += stat_partial[c * 5 + threadIdx.x];
-    stats_accum[threadIdx.x] += a * stat_scale;
+    stats_accum[threadIdx.x] = fmaf(a, stat_scale, stats_accum[threadIdx.x]);   // one rounding, as k_dense_wgrad's Stats
   }
 }
 

@@ -256,11 +256,23 @@ int r4_policy_grad_partial(int mode, const float* params, const float* obs, cons
                           stream, false);
 }
 
+// The communicator check every entry point that takes one makes first, before it launches or writes anything: a
+// communicator whose peers are not mapped yet (r4_comm_open; world 1 is ready at creation) is R4_ERR_STATE, one created
+// for another parameter count R4_ERR_ARG.  NULL passes: the single-GPU form of the entry points that allow it.
+static int comm_check(const r4_comm* c, int np, const char* who) {
+  if (!c) return R4_OK;
+  if (!c->ready) return fail(R4_ERR_STATE, std::string(who) + ": open the peers' handles first (r4_comm_open)");
+  if (np != c->n) return fail(R4_ERR_ARG, std::string(who) + ": parameter count differs from the communicator's");
+  return R4_OK;
+}
+
+// The exchange kernel.  Its callers have checked the communicator up front (comm_check); the same check here is the
+// backstop in front of k_exchange_adam, which stores through and spins on the peers' pointers (null until r4_comm_open).
+// Either way a refused call never reaches the ++seq.
 static int exchange_launch(r4_comm* c, const float* scratch, int G, int np, float* flat, float* stats_accum, float stat_scale,
                            int do_adam, float* params, float* m, float* v, int step, float lr, float b1, float b2, float eps,
                            void* stream) {
-  if (!c->ready) return fail(R4_ERR_STATE, "r4_comm: open the peers' handles first (r4_comm_open)");
-  if (np != c->n) return fail(R4_ERR_ARG, "r4_comm: parameter count differs from the communicator's");
+  if (int rc = comm_check(c, np, "r4_comm")) return rc;
   ++c->seq;
   return launch(FAM_ONLINE, "k_exchange_adam", r4comm::k_exchange_adam, c->nblk, r4comm::BLK, 0, S(stream), false, np, G, scratch,
                 flat, scratch + (size_t)G * np, stats_accum, stat_scale, c->peers, c->rank, c->world, c->seq, do_adam, params, m,
@@ -278,10 +290,12 @@ int r4_ppo_epoch_dist(r4_comm* c, float* params, const float* obs, const uint8_t
                       float vf_clip, float vf_coeff, float kl_coeff, float ent_coeff, float* scratch, float* flat_grad,
                       float* stats_accum, float* m, float* v, int step0, float lr, float beta1, float beta2, float eps,
                       void* stream) {
-  if (!c || !params || !perm || !m || !v || !scratch || n < 1 || mb < 1 || mb > n || step0 < 0)
+  if (!c || !params || !perm || !m || !v || !scratch || n < 1 || mb < 1 || mb > n || step0 < 0 || action_size < 2 ||
+      action_size > 512)
     return fail(R4_ERR_ARG, "r4_ppo_epoch_dist: bad argument");
-  const int G = std::max(1, std::min((mb + r4ppo::TS - 1) / r4ppo::TS, sm_count()));
   const int np = r4ppo::make_layout(action_size).n;
+  if (int rc = comm_check(c, np, "r4_ppo_epoch_dist")) return rc;
+  const int G = std::max(1, std::min((mb + r4ppo::TS - 1) / r4ppo::TS, sm_count()));
   const float inv = 1.0f / ((float)mb * (float)c->world);
   int steps = 0;
   for (int s = 0; s + mb <= n; s += mb, ++steps) {
@@ -300,6 +314,7 @@ int r4_ppo_epoch_dist(r4_comm* c, float* params, const float* obs, const uint8_t
 int r4_grad_exchange_n(r4_comm* c, const float* partial, int G, int n_params, float* flat_grad, float* stats_accum,
                        float stat_scale, void* stream) {
   if (!c || !partial || !flat_grad || G < 1 || n_params < 1) return fail(R4_ERR_ARG, "r4_grad_exchange_n: bad argument");
+  if (int rc = comm_check(c, n_params, "r4_grad_exchange_n")) return rc;
   return exchange_launch(c, partial, G, n_params, flat_grad, stats_accum, stat_scale, 0, nullptr, nullptr, nullptr, 0, 0.f, 0.f, 0.f,
                          0.f, stream);
 }
@@ -391,6 +406,7 @@ int r4_gauss_ppo_epoch_dist(r4_comm* c, float* params, const float* obs, const f
   if (!c || !params || !perm || !m || !v || !scratch || n < 1 || mb < 1 || mb > n || step0 < 0 || !gauss_dim_ok(action_dim))
     return fail(R4_ERR_ARG, "r4_gauss_ppo_epoch_dist: bad argument");
   const int np = r4gauss::make_layout(action_dim).n;
+  if (int rc = comm_check(c, np, "r4_gauss_ppo_epoch_dist")) return rc;
   const float inv = 1.0f / ((float)mb * (float)c->world);
   float* gsum = gauss_gsum(scratch, action_dim);
   int steps = 0;
@@ -458,8 +474,6 @@ static int impala_tail(r4_comm* comm, const float* partial, int G, int np, float
                 b1, b2, eps, 1.f, grad_clip > 0.f ? norm_scratch : nullptr, grad_clip);
 }
 
-static bool impala_comm_ok(r4_comm* comm, int np) { return !comm || (comm->ready && comm->n == np); }
-
 int r4_impala_step(r4_comm* comm, float* params, const float* obs, const uint8_t* mask, const int64_t* action,
                    const float* behaviour_logp, const float* logits, const float* reward, int T, int B, int action_size,
                    float gamma, float rho_bar, float rho_pg_bar, int drop_last, float vf_coeff, float ent_coeff, float* logp,
@@ -468,11 +482,11 @@ int r4_impala_step(r4_comm* comm, float* params, const float* obs, const uint8_t
                    void* stream) {
   if (!params || !obs || !mask || !action || !behaviour_logp || !logits || !reward || !logp || !value || !vs || !pg_adv ||
       !scratch || !flat_grad || !m || !v || step < 1 || (grad_clip > 0.f && !norm_scratch) || action_size < 2 ||
-      action_size > 512 || !vtrace_args_ok(T, B, gamma, rho_bar, rho_pg_bar, drop_last) ||
-      !impala_comm_ok(comm, r4ppo::make_layout(action_size).n))
+      action_size > 512 || !vtrace_args_ok(T, B, gamma, rho_bar, rho_pg_bar, drop_last))
     return fail(R4_ERR_ARG, "r4_impala_step: bad argument");
-  const int n = T * B, nk = (drop_last ? T - 1 : T) * B;          // the kept rows are the first T - 1 (or T) time steps
   const int np = r4ppo::make_layout(action_size).n;
+  if (int rc = comm_check(comm, np, "r4_impala_step")) return rc;
+  const int n = T * B, nk = (drop_last ? T - 1 : T) * B;          // the kept rows are the first T - 1 (or T) time steps
   const int G = std::max(1, std::min((nk + r4ppo::TS - 1) / r4ppo::TS, sm_count()));
   cudaStream_t st = S(stream);
   int rc = r4_policy_eval(params, obs, mask, action, n, action_size, logp, value, stream);
@@ -492,11 +506,11 @@ int r4_gauss_impala_step(r4_comm* comm, float* params, const float* obs, const f
                          float beta1, float beta2, float eps, float grad_clip, float* norm_scratch, void* stream) {
   if (!params || !obs || !action || !behaviour_logp || !reward || !logp || !value || !vs || !pg_adv || !scratch || !flat_grad ||
       !m || !v || step < 1 || (grad_clip > 0.f && !norm_scratch) || !gauss_dim_ok(action_dim) ||
-      !vtrace_args_ok(T, B, gamma, rho_bar, rho_pg_bar, drop_last) ||
-      !impala_comm_ok(comm, r4gauss::make_layout(action_dim).n))
+      !vtrace_args_ok(T, B, gamma, rho_bar, rho_pg_bar, drop_last))
     return fail(R4_ERR_ARG, "r4_gauss_impala_step: bad argument");
-  const int n = T * B, nk = (drop_last ? T - 1 : T) * B;
   const int np = r4gauss::make_layout(action_dim).n;
+  if (int rc = comm_check(comm, np, "r4_gauss_impala_step")) return rc;
+  const int n = T * B, nk = (drop_last ? T - 1 : T) * B;
   float* gsum = gauss_gsum(scratch, action_dim);
   cudaStream_t st = S(stream);
   int rc = r4_gauss_eval(params, obs, action, n, action_dim, logp, value, stream);
@@ -597,6 +611,7 @@ int r4_ddpg_train_step(r4_comm* comm, float* params, float* target, float* m, fl
   if (!scratch || !ddpg_dim_ok(action_dim) || n < 1 || (r_prio && !max_prio))
     return fail(R4_ERR_ARG, "r4_ddpg_train_step: bad argument");
   const int np = r4ddpg::make_layout(action_dim, twin != 0).n;
+  if (int rc = comm_check(comm, np, "r4_ddpg_train_step")) return rc;
   const r4ddpg::Planes P = r4ddpg::make_planes(scratch, action_dim, twin != 0, n);
   const int world = comm ? comm->world : 1;
   int rc = r4_replay_sample(r_prio, size, n, beta, u, P.idx, P.weights, stream);
@@ -691,6 +706,7 @@ int r4_rainbow_train_step(r4_comm* comm, float* params, float* target, float* m,
   if (!scratch || !rainbow_dims_ok(num_actions, num_atoms) || n < 1 || (r_prio && !max_prio))
     return fail(R4_ERR_ARG, "r4_rainbow_train_step: bad argument");
   const r4rb::Layout L = r4rb::make_layout(num_actions, num_atoms);
+  if (int rc = comm_check(comm, L.n, "r4_rainbow_train_step")) return rc;
   const r4rb::Planes P = r4rb::make_planes(scratch, L, n);
   const int world = comm ? comm->world : 1;
   int rc = r4_replay_sample(r_prio, size, n, beta, u, P.idx, P.weights, stream);

@@ -40,6 +40,20 @@ def test_create_rejects_bad_config_without_gpu_work():
     assert b"maxlen=64" in lib.r4_last_error(None)
 
 
+def test_comm_create_rejects_bad_arguments_without_gpu_work():
+    """r4_comm_create checks world (1..16), rank (0..world-1), n_params (>= 1) and out before any CUDA call: R4_ERR_ARG
+    with *out untouched, with or without a device; r4_comm_destroy(NULL) is a no-op."""
+    import ctypes as C
+    lib = _capi.load_library()
+    for rank, world, n in ((0, 0, 10), (0, 17, 10), (-1, 2, 10), (2, 2, 10), (0, 1, 0), (0, 1, -5)):
+        h = C.c_void_p(0x5eed)
+        assert lib.r4_comm_create(rank, world, n, C.byref(h)) == R4_ERR_ARG, (rank, world, n)
+        assert h.value == 0x5eed, (rank, world, n)
+        assert b"r4_comm_create" in lib.r4_last_error(None)
+    assert lib.r4_comm_create(0, 1, 10, None) == R4_ERR_ARG
+    lib.r4_comm_destroy(None)
+
+
 R4_ERR_ARG = -1                     # include/rl4rs_b200.h
 
 
